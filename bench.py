@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Benchmark of the LightGlue matcher forward path on B200 (contract: see the task brief).
+"""Benchmark of the LightGlue matcher forward path on the H100.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 Workload at N GPUs: BASELINE.json configs[1] on every GPU -- SuperPoint-shaped synthetic pairs,
@@ -11,9 +11,11 @@ all_gather of the match indices and scores, SURVEY.md §8e).  One "step" = one f
 
 Prints ONE JSON line (rank 0).  `value` = pairs/s with inputs resident in HBM; `e2e` = pairs/s
 through the public `LightGlue.forward` API with pinned HOST inputs (H2D and the D2H of the results
-inside the timed region).  `roofline` = the attention kernel (dominant) against the measured bf16
-peak; `cpu_baseline` = the CPU oracle (a port of the reference algorithm) on this host's cores.
+inside the timed region).  `roofline` = the attention kernel (dominant) against the bf16 peak (MEASURED_PEAKS.json
+when present, else the H100 SXM data sheet); `cpu_baseline` = the CPU oracle (a port of the reference algorithm) on this host's cores.
 `--impl reference` times that CPU implementation alone, on a bounded sample of the same workload.
+`--dump-outputs DIR` writes the outputs of the last timed step as DIR/<name>.npy (float32 / float64); the inputs are
+seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -56,20 +58,7 @@ def measured_peaks():
         with open(path) as f:
             d = json.load(f)
         return d, "measured (MEASURED_PEAKS.json)"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback (B200_PROFILING.md)"
-
-
-def profiled_traffic(kernel: str, batch: int, precision: str):
-    """DRAM bytes per launch of `kernel` from the committed ncu --set full capture (profiles/traffic.json), or None
-    when this run's workload is not the one that was profiled."""
-    path = os.path.join(ROOT, "profiles", "traffic.json")
-    if not os.path.exists(path):
-        return None
-    with open(path) as f:
-        d = json.load(f)
-    if d.get("workload") != f"superpoint_n{N_KPTS}_l9_prune_off_b{batch}":
-        return None
-    return ((d.get(precision) or {}).get(kernel) or {}).get("bytes_per_launch")
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "H100 SXM data sheet (dense, 700 W); not a measured rate"
 
 
 class ClockSampler:
@@ -238,7 +227,7 @@ def run_reference(args, rank: int):
 
 
 def reference_on_gpu(dev, resident, sd, batch, budget_s=60.0):
-    """SURVEY 8d / BASELINE.md 4.5: the UNMODIFIED reference file on the SAME B200 -- the real bar.  benchmark.py:18-43
+    """SURVEY 8d / BASELINE.md 4.5: the UNMODIFIED reference file on the SAME GPU -- the real bar.  benchmark.py:18-43
     protocol (warm-up, then CUDA events around each forward, mean), pruning / early exit off, at the bench batch and
     at B=1.  Variants: eager fp32 with fp16 flash SDPA (`flash=True`, lightglue.py:116-121), autocast (`mp=True`,
     480, 508-510), each SDPA backend torch offers.  `.compile()` pads to static lengths <= 1536 (439-454) and so does
@@ -306,6 +295,28 @@ def reference_on_gpu(dev, resident, sd, batch, budget_s=60.0):
     return res
 
 
+def dump_outputs(out: dict, path: str) -> None:
+    """The result of one forward as DIR/<name>.npy: indices as float64 (exact), scores as float32; the per-pair match
+    lists are concatenated (`matches`, `scores`) with their lengths in `matches_counts`."""
+    import numpy as np
+
+    os.makedirs(path, exist_ok=True)
+    arrays = {}
+    for name, v in out.items():
+        if torch.is_tensor(v):
+            arrays[name] = v
+        elif isinstance(v, (list, tuple)) and v and torch.is_tensor(v[0]):
+            arrays[name] = torch.cat(list(v))
+            if name == "matches":
+                arrays["matches_counts"] = torch.tensor([len(t) for t in v])
+        elif isinstance(v, (int, list, tuple)):
+            arrays[name] = torch.tensor(v)
+    for name, t in arrays.items():
+        t = t.detach().cpu()
+        t = t.to(torch.float32) if t.is_floating_point() else t.to(torch.float64)
+        np.save(os.path.join(path, f"{name}.npy"), t.numpy())
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -319,7 +330,9 @@ def main():
     ap.add_argument("--no-reference-gpu", action="store_true")
     ap.add_argument("--no-other-mode", action="store_true")
     ap.add_argument("--no-extractor", action="store_true")
-    ap.add_argument("--profile", action="store_true", help="2 forwards and exit (for ncu; prints nothing timed)")
+    ap.add_argument("--profile", action="store_true", help="2 forwards and exit (for a profiler; prints nothing timed)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32 / float64)")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -383,7 +396,7 @@ def main():
                 # SURVEY 8e: the fixed-size results of every rank -- match indices of both images as int32 on the wire,
                 # both score tensors -- are collected on the device and gathered ONCE for the run, after the last forward
                 # (still inside the timed region).  A collective per step, concurrent with the next forward, cost 16 % at
-                # two ranks: its channels hold SMs while they wait for the slower rank, and the persistent CTA-pair
+                # two ranks: its channels hold SMs while they wait for the slower rank, and the persistent
                 # kernels then run short of SMs.
                 tt = cur.tensors
                 acc_i.append(torch.cat([tt["matches0"], tt["matches1"]], 1).to(torch.int32))
@@ -418,7 +431,7 @@ def main():
     in_flight = int(pick.item())
     launches_per_step = matcher.last_launch_count()
 
-    # ---- timed region 1: inputs resident in HBM (inputs 134 MB + multi-GB workspace: larger than the 126 MB L2)
+    # ---- timed region 1: inputs resident in HBM (inputs 134 MB + multi-GB workspace: larger than the 50 MB L2)
     sampler = ClockSampler(local_rank)
     if rank == 0:
         sampler.start()
@@ -438,6 +451,8 @@ def main():
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     ms = float(t.item())
     value = world * B * args.steps / (ms / 1000.0)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(out, args.dump_outputs)
 
     # ---- timed region 2: end to end through the public API with pinned host inputs
     from lightglue_b200.pipeline import match_stream
@@ -452,7 +467,7 @@ def main():
 
     run_e2e(4)  # warm-up: also allocates the three pinned result slots of match_stream
     barrier()
-    e2s = max(3, args.steps)
+    e2s = args.steps
     e0.record()
     res = run_e2e(e2s)
     e1.record()
@@ -477,10 +492,10 @@ def main():
         att_ms, att_n = kt["attention"]
         if att_n > 0 and args.precision != "fp32":
             ach = attention_flops_per_launch(B) / ((att_ms / att_n) / 1000.0) / 1e12
-            peak = peaks.get("bf16_tflops_sustained", peaks["bf16_tflops"])
+            peak = peaks["bf16_tflops"]
             roofline = {"kernel": "attention", "bound": "tensor", "achieved": ach, "peak": peak, "unit": "TFLOP/s",
-                        "frac": ach / peak, "traffic": profiled_traffic("attention", B, args.precision),
-                        "peak_source": how + ", sustained (kernel timed inside a long step)",
+                        "frac": ach / peak,
+                        "peak_source": how,
                         "flops_per_launch": attention_flops_per_launch(B), "avg_launch_ms": att_ms / att_n}
 
     # ---- assignment kernel, materialising variant (MatchAssignment.forward's declared output, lightglue.py:296):
@@ -507,7 +522,6 @@ def main():
                                          "[B, M+1, N+1] fp32 matrix write + term + dustbin + tail (filter, outputs)",
                                "bound": "hbm", "achieved": ach, "peak": peaks["hbm_gbs"], "unit": "GB/s",
                                "frac": ach / peaks["hbm_gbs"],
-                               "traffic": profiled_traffic("assign_matrix", B, args.precision),
                                "algorithmic_bytes_per_launch": abytes, "avg_stage_ms": st_ms / st_n,
                                "matrix_writing_sweep_alone_ms": am_ms / am_n,
                                "matrix_writing_sweep_alone_frac": abytes / ((am_ms / am_n) / 1000.0) / 1e9 / peaks["hbm_gbs"],
@@ -586,7 +600,7 @@ def main():
                 ms_img = a0.elapsed_time(a1) / reps
                 res[prec] = {"ms_per_image": ms_img, "images_per_s": 1000.0 / ms_img,
                              "algorithmic_tflops": flops_img / (ms_img * 1e-3) / 1e12,
-                             "frac_of_bf16_peak": flops_img / (ms_img * 1e-3) / 1e12 / peaks.get("bf16_tflops_sustained", 1400.0)}
+                             "frac_of_bf16_peak": flops_img / (ms_img * 1e-3) / 1e12 / peaks["bf16_tflops"]}
                 if prec == "bf16x3":
                     lg1 = LightGlue(features=None, depth_confidence=-1, width_confidence=-1, precision=args.precision)
                     lg1.load_state_dict(sd, strict=False)
@@ -615,7 +629,7 @@ def main():
         done, dt = cpu.run(16, budget_s=12.0)
         cpu_baseline = cpu.describe(done, dt)
 
-    # ---- the real bar (SURVEY 8d): the unmodified reference file on this same B200, same resident batch
+    # ---- the real bar (SURVEY 8d): the unmodified reference file on this same GPU, same resident batch
     reference_gpu = None
     if rank == 0 and not args.no_reference_gpu:
         try:
@@ -637,13 +651,13 @@ def main():
         line = {
             "metric": METRIC, "value": value, "unit": "pairs/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-            "dtype": {"bf16": "bf16", "bf16x3": "bf16x3 (split-bf16 hi+lo operands, 3 tcgen05 MMAs per product: index-exact mode)",
+            "dtype": {"bf16": "bf16", "bf16x3": "bf16x3 (split-bf16 hi+lo operands, 3 wgmma MMAs per product: index-exact mode)",
                       "fp32": "f32"}[args.precision] +
                      " linears / fp16 attention operands / fp32 accumulate, softmax, LayerNorm, residual",
             "data": "synthetic",
             "config": {"workload": WORKLOAD, "pairs_per_step_per_gpu": B, "keypoints": N_KPTS, "descriptor_dim": DESC,
                        "layers": LAYERS, "precision": args.precision, "parallelism": f"pairs sharded over {world} GPU(s)", "numa_binding": numa,
-                       "l2": "inputs (134 MB/step) + workspace (GBs) exceed the 126 MB L2; no explicit flush",
+                       "l2": "inputs (134 MB/step) + workspace (GBs) exceed the 50 MB L2; no explicit flush",
                        "host_pipelining": {"forwards_in_flight": in_flight, "warmup_ms_per_step_sync": mode_ms[0],
                                            "warmup_ms_per_step_one_in_flight": mode_ms[1],
                                            "note": "every step's stop / match lists are resolved inside the timed region"}},
@@ -659,7 +673,7 @@ def main():
             "kernel_ms": kernel_ms,
             "whole_forward": {"algorithmic_flops_per_pair": flops,
                               "achieved_tflops": flops * value / world / 1e12,
-                              "frac_of_peak": flops * value / world / 1e12 / peaks.get("bf16_tflops_sustained", 1400.0)},
+                              "frac_of_peak": flops * value / world / 1e12 / peaks["bf16_tflops"], "peak_source": how},
         }
         print(json.dumps(line), flush=True)
     if world > 1:

@@ -1,5 +1,5 @@
 /*
- * lightglue_b200.h -- C ABI of the B200-native LightGlue matcher forward path.
+ * lightglue_b200.h -- C ABI of the H100-native LightGlue matcher forward path.
  *
  * The reference (cvg/LightGlue) is pure Python: it has no FFI / plugin interface, its boundary is
  * the Python class `LightGlue` (lightglue/lightglue.py:321-662).  This header is the C-ABI a
@@ -36,8 +36,8 @@ extern "C" {
  * reductions are always fp32). */
 enum {
   LG_PREC_FP32 = 0,   /* fp32 CUDA-core path: reference-grade, used for index-exact parity      */
-  LG_PREC_BF16 = 1,   /* tcgen05 tensor cores, bf16 operands (fp16 inside attention), fp32 accum */
-  LG_PREC_BF16X3 = 2  /* tcgen05, split-bf16 (hi+lo, 3 MMAs) linears: ~fp32 accuracy            */
+  LG_PREC_BF16 = 1,   /* wgmma tensor cores, bf16 operands (fp16 inside attention), fp32 accum   */
+  LG_PREC_BF16X3 = 2  /* wgmma, split-bf16 (hi+lo, 3 MMAs) linears: ~fp32 accuracy              */
 };
 
 /* Mirrors LightGlue.default_conf (lightglue.py:322-335). */

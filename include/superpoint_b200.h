@@ -32,7 +32,7 @@ typedef struct SpConfig {
   int32_t remove_borders;      /* conf.remove_borders (4) */
   float detection_threshold;   /* conf.detection_threshold (0.0005) */
   int32_t precision;           /* arithmetic of the twelve convolutions (superpoint.py:137-153): 0 = fp32 on the CUDA
-                                  cores (the checker), 1 = tcgen05 tensor cores, split-bf16 operands (hi + lo, 3 MMAs per
+                                  cores (the checker), 1 = wgmma tensor cores, split-bf16 operands (hi + lo, 3 MMAs per
                                   product), fp32 accumulate */
 } SpConfig;
 

@@ -1,4 +1,4 @@
-"""lightglue_b200 -- a B200-native (sm_100a) implementation of the LightGlue matcher forward path.
+"""lightglue_b200 -- an H100-native (sm_90a) implementation of the LightGlue matcher forward path.
 
 ``LightGlue`` is a drop-in for ``lightglue.LightGlue`` (cvg/LightGlue): same constructor, same
 ``forward({"image0": ..., "image1": ...})`` -> output dict; the math runs in hand-written CUDA

@@ -1,4 +1,4 @@
-"""Build liblightglue_b200.so in-tree with nvcc for sm_100a (``make -C lightglue_b200/csrc``).
+"""Build liblightglue_b200.so in-tree with nvcc for sm_90a (``make -C lightglue_b200/csrc``).
 
 The library is plain CUDA C++ behind a C ABI (include/lightglue_b200.h); it does not link against
 torch.  nvcc cross-compiles without a GPU, so this runs in the CPU-only build container and the

@@ -61,19 +61,19 @@ int lg_func_smem_once(const void* func, int bytes) {
 }
 int lg_num_sms() {
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
   std::lock_guard<std::mutex> lk(g_dev_mu);
   auto it = g_sms.find(dev);
   if (it != g_sms.end()) return it->second;
   int n = 0;
-  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
   g_sms[dev] = n;
   return n;
 }
 extern "C" const char* lg_build_info(void) {
 #define LG_STR2(x) #x
 #define LG_STR(x) LG_STR2(x)
-  return "lightglue_b200 abi=" LG_STR(LG_ABI_VERSION) " arch=sm_100a (" __DATE__ " " __TIME__ ")";
+  return "lightglue_b200 abi=" LG_STR(LG_ABI_VERSION) " arch=sm_90a (" __DATE__ " " __TIME__ ")";
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -1,4 +1,4 @@
-// Tensor-core (tcgen05 / TMA) path: LG_PREC_BF16 and LG_PREC_BF16X3.
+// Tensor-core (wgmma / TMA) path: LG_PREC_BF16 and LG_PREC_BF16X3.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>

@@ -1,5 +1,5 @@
 // SuperPoint encoder + heads on the tensor cores (SURVEY.md 8f1; reference lightglue/superpoint.py:137-153, 171-190,
-// 220-221): the twelve convolutions as implicit GEMMs through the matcher's tcgen05 / TMA linear kernels
+// 220-221): the twelve convolutions as implicit GEMMs through the matcher's wgmma / TMA linear kernels
 // (k_tc_linear.cu, tc_conv), split-bf16 operands (hi + lo, three MMAs per product: ~fp32 accuracy), fp32 accumulate.
 //
 // Data layout: every feature map is a ZERO-PADDED NHWC image stored as a matrix [rows, C] of bf16 hi / lo images, row =

@@ -1,4 +1,4 @@
-"""Drop-in ``LightGlue`` matcher whose forward runs entirely in liblightglue_b200.so (sm_100a CUDA).
+"""Drop-in ``LightGlue`` matcher whose forward runs entirely in liblightglue_b200.so (sm_90a CUDA).
 
 Host-side mirror of the reference interface (reference: lightglue/lightglue.py:321-662):
 
@@ -96,7 +96,7 @@ class LightGlue(nn.Module):
             for k, v in self.features[features].items():
                 setattr(conf, k, v)
         if conf.descriptor_dim != DIM or conf.num_heads != 4:
-            raise ValueError("the sm_100a kernels are specialised for descriptor_dim=256, num_heads=4")
+            raise ValueError("the sm_90a kernels are specialised for descriptor_dim=256, num_heads=4")
         if conf.precision not in _cabi.PREC:
             raise ValueError(f"precision must be one of {sorted(_cabi.PREC)}")
         n = conf.n_layers
@@ -277,7 +277,7 @@ class LightGlue(nn.Module):
         b, n, _ = k1.shape
         device = k0.device
         if device.type != "cuda":
-            raise RuntimeError("lightglue_b200.LightGlue runs on CUDA (sm_100a) tensors only; there is no CPU path")
+            raise RuntimeError("lightglue_b200.LightGlue runs on CUDA (sm_90a) tensors only; there is no CPU path")
         x0 = d0["descriptors"].detach()
         x1 = d1["descriptors"].detach()
         assert x0.shape[-1] == self.conf.input_dim

@@ -4,7 +4,7 @@ Image pairs are independent, so the path shards with no data-path collective: on
 (torchrun), rank r takes a contiguous block of pairs, every rank holds a full replica of the
 23.7 MB weights.  The only communication is the final gather of fixed-size match indices / scores
 (``all_gather`` over NCCL on GPUs, gloo in the CPU tests).  The reference has no distributed code at
-all (SURVEY.md §2a); this module is the B200 deployment story for BASELINE config 5.
+all (SURVEY.md §2a); this module is the multi-GPU deployment story for BASELINE config 5.
 """
 from __future__ import annotations
 

@@ -35,7 +35,7 @@ class SuperPoint(nn.Module):
         "remove_borders": 4,
         # extension: None = keep the (random) initial parameters instead of looking for superpoint_v1.pth
         "weights": "superpoint_v1",
-        # extension: arithmetic of the twelve convolutions -- "bf16x3" (tcgen05 tensor cores, split-bf16 operands,
+        # extension: arithmetic of the twelve convolutions -- "bf16x3" (wgmma tensor cores, split-bf16 operands,
         # fp32 accumulate) or "fp32" (CUDA cores: the checker the tensor-core path is validated against)
         "precision": "bf16x3",
     }
@@ -122,7 +122,7 @@ class SuperPoint(nn.Module):
             assert key in data, f"Missing key {key} in data"
         image = data["image"]
         if image.device.type != "cuda":
-            raise RuntimeError("lightglue_b200.SuperPoint runs on CUDA (sm_100a) tensors only; there is no CPU path")
+            raise RuntimeError("lightglue_b200.SuperPoint runs on CUDA (sm_90a) tensors only; there is no CPU path")
         if image.shape[1] == 3:  # kornia.color.rgb_to_grayscale's weights (superpoint.py:168-169)
             wts = torch.tensor([0.299, 0.587, 0.114], device=image.device, dtype=image.dtype).view(1, 3, 1, 1)
             image = (image * wts).sum(1, keepdim=True)

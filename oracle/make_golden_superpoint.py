@@ -27,6 +27,9 @@ from oracle import superpoint_synth as sps  # noqa: E402
 
 REF = "/root/reference/lightglue/superpoint.py"
 OUT = os.path.join(ROOT, "tests", "golden")
+# CPU threads of the fixture run.  oneDNN splits a convolution's sums by thread count, so an fp32 result is reproducible
+# to the last bits only with the same count: the oracle test runs with it too.
+FIXTURE_THREADS = 8
 
 CASES = {
     "sp_240x320": dict(h=240, w=320, b=1, seed=11, conf={}),
@@ -70,6 +73,7 @@ def load_reference(weights):
 
 def main():
     torch.set_grad_enabled(False)
+    torch.set_num_threads(FIXTURE_THREADS)
     weights = sps.make_superpoint_state_dict(0)
     ref = load_reference(weights)
     os.makedirs(OUT, exist_ok=True)

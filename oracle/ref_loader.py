@@ -4,7 +4,7 @@
 container (git-ignored, travels to the GPU box with the repo snapshot).  The package ``lightglue`` itself cannot be
 imported (``__init__`` pulls in kornia, absent here) but this one file only needs torch + numpy (SURVEY.md 8c), so it is
 loaded by path.  Used by ``bench.py --impl reference`` (the reference's own CPU path), by the ``reference_gpu`` leg of
-the bench (the same file on the same B200) and by ``oracle/make_golden.py``.  Nothing under ``lightglue_b200/`` imports
+the bench (the same file on the same GPU) and by ``oracle/make_golden.py``.  Nothing under ``lightglue_b200/`` imports
 this."""
 from __future__ import annotations
 

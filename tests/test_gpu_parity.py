@@ -114,7 +114,7 @@ TC_CASES = ["c1_n512", "ragged_b2", "n2048", "disk_d128", "sift_scale_ori", "nos
 
 @pytest.mark.parametrize("name", TC_CASES)
 def test_bf16x3_path_index_exact(name):
-    """tcgen05 path with split-bf16 linears: identical match indices, scores within 1e-3."""
+    """Tensor-core path with split-bf16 linears: identical match indices, scores within 1e-3."""
     fix, data, sd = load_case(name)
     out = build(fix, sd, "bf16x3")(to_cuda(data))
     flips, dmax = compare_outputs(out, fix["out"], score_tol=1e-3)
@@ -123,7 +123,7 @@ def test_bf16x3_path_index_exact(name):
 
 @pytest.mark.parametrize("name", TC_CASES)
 def test_bf16_path_bounded_error(name):
-    """tcgen05 path with plain bf16 operands: operand rounding moves scores by O(1e-2) (SURVEY §7.3), so
+    """Tensor-core path with plain bf16 operands: operand rounding moves scores by O(1e-2) (SURVEY §7.3), so
     a few matches whose score sits at filter_threshold may flip; bounded and reported, not hidden."""
     fix, data, sd = load_case(name)
     out = build(fix, sd, "bf16")(to_cuda(data))

@@ -1,6 +1,4 @@
-"""Pairs far below one 128-row tile through the tensor-core path against the oracle.
-
-Green on the B200 since round 1's closing run (GPUTEST_r01.json)."""
+"""Pairs far below one 128-row tile through the tensor-core path against the oracle."""
 import pytest
 import torch
 

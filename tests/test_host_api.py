@@ -19,7 +19,7 @@ def test_library_exports_every_declared_symbol():
     assert sorted(declared) == sorted(_cabi.EXPORTS)
     for name in declared:
         assert hasattr(lib, name), name
-    assert b"sm_100a" in lib.lg_build_info()
+    assert b"sm_90a" in lib.lg_build_info()
 
 
 def test_blob_size_matches_parameter_count():

@@ -9,6 +9,7 @@ import torch
 from lightglue_b200 import synth
 from oracle import superpoint_oracle as sp
 from oracle import superpoint_synth as sps
+from oracle.make_golden_superpoint import FIXTURE_THREADS
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 CASES = sorted(f[:-3] for f in os.listdir(GOLDEN) if f.startswith("sp_") and f.endswith(".pt"))
@@ -23,8 +24,13 @@ def test_superpoint_oracle_matches_reference_fixture(name):
         assert synth.checksum(w[k]) == v, k
     image = sps.make_image(rc["h"], rc["w"], rc["b"], rc["seed"])
     assert synth.checksum(image) == fix["image_checksum"]
-    with torch.no_grad():
-        out = sp.forward(w, image, **fix["conf"])
+    threads = torch.get_num_threads()
+    torch.set_num_threads(FIXTURE_THREADS)  # the fixtures' summation order (see make_golden_superpoint.py)
+    try:
+        with torch.no_grad():
+            out = sp.forward(w, image, **fix["conf"])
+    finally:
+        torch.set_num_threads(threads)
     gold = fix["out"]
     assert len(out["keypoints"]) == rc["b"]
     for b in range(rc["b"]):

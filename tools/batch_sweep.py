@@ -1,5 +1,5 @@
 """Pairs/s of the resident forward against the batch size (bf16, N=2048, pruning off): does keeping the
-per-layer activations inside the 126 MB L2 (smaller batches) beat fuller waves (larger batches)?"""
+per-layer activations inside the 50 MB L2 (smaller batches) beat fuller waves (larger batches)?"""
 import os
 import sys
 
