@@ -411,6 +411,17 @@ __global__ void __launch_bounds__(LinCfg<NSLOT>::THREADS, 1) tc_linear_kernel(co
         const int yy = (int)(pp / p.conv_w2), xx = (int)(pp % p.conv_w2);
         inside = grow < p.conv_rows && yy >= 1 && yy <= p.conv_h && xx >= 1 && xx <= p.conv_w;
       }
+      // RoPE cos / sin of this row, loaded ahead of its stores (the compiler does not move a load above a store it cannot
+      // prove independent, so a load per column would pay its full latency every time); frequency index d / 2 =
+      // 4 (j % 8) + tq, the same for every head
+      float rc[8], rs[8];
+      if (use_rope) {
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+          rc[jj] = __ldg(p.cs + grow * 64 + 4 * jj + tq);
+          rs[jj] = __ldg(p.cs + grow * 64 + 32 + 4 * jj + tq);
+        }
+      }
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
         const int tcol = 8 * j + 2 * tq;        // column inside the tile (even)
@@ -430,7 +441,7 @@ __global__ void __launch_bounds__(LinCfg<NSLOT>::THREADS, 1) tc_linear_kernel(co
             continue;
           }
           if (use_rope) {  // rotary embedding on q / k (lightglue.py:58-65, 168-169); freq index = d / 2
-            const float c = __ldg(p.cs + grow * 64 + d / 2), s = __ldg(p.cs + grow * 64 + 32 + d / 2);
+            const float c = rc[j % 8], s = rs[j % 8];
             const float a = v0, b = v1;
             v0 = a * c - b * s;
             v1 = b * c + a * s;
