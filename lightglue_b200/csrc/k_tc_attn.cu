@@ -8,8 +8,6 @@
 // Warp roles (384 threads = 3 warpgroups): warpgroup 0 = TMA producer (warp 0; the warpgroup hands its registers to
 // the others), warpgroups 1 and 2 = query rows 0-63 / 64-127 of the CTA.  ~80 KB of shared memory, so two CTAs are
 // resident per SM and one CTA's exponentials overlap the other's MMAs.
-#include <stdlib.h>
-
 #include "lg_handle.h"
 #include "tc_common.cuh"
 
@@ -197,43 +195,16 @@ __global__ void __launch_bounds__(384, 2) tc_attention_kernel(const __grid_const
   }
 }
 
-struct AttnMapCache {
-  const void* q; const void* k; const void* vt; int S, Lp;
-  CUtensorMap qm, km, vm;
-};
 }  // namespace
 
 int tc_attention(LgHandle* h, const TcBuffers& b, const SeqState& st, int kv_shift, const __half* kbuf, cudaStream_t stream) {
   h->launches += 1;
-  // tensor maps depend only on (buffers, S, Lp): cache the last two sets (self: k = b.k, cross: k = b.q); the
-  // buffer addresses are unique per device (UVA), so the cache is safe with several devices in one process
-  static thread_local AttnMapCache cache[2];
-  AttnMapCache* c = nullptr;
-  for (auto& e : cache)
-    if (e.q == b.q && e.k == kbuf && e.vt == b.vt && e.S == st.S && e.Lp == st.Lp) c = &e;
-  if (!c) {
-    c = &cache[kbuf == b.q ? 1 : 0];
-    const uint64_t SH = (uint64_t)st.S * LG_HEADS, Lp = st.Lp;
-    int r;
-    if ((r = tc_make_tmap_3d(&c->qm, b.q, 2, 64, Lp, SH, 128, Lp * 128, 64, QT, 1))) return r;
-    if ((r = tc_make_tmap_3d(&c->km, kbuf, 2, 64, Lp, SH, 128, Lp * 128, 64, KB, 1))) return r;
-    if ((r = tc_make_tmap_3d(&c->vm, b.vt, 2, Lp, 64, SH, Lp * 2, 64 * Lp * 2, 64, 64, 1))) return r;
-    c->q = b.q; c->k = kbuf; c->vt = b.vt; c->S = st.S; c->Lp = st.Lp;
-  }
+  const uint64_t SH = (uint64_t)st.S * LG_HEADS, Lp = st.Lp;
   AttnParams p;
-  p.q_map = c->qm; p.k_map = c->km; p.vt_map = c->vm;
+  int r;
+  if ((r = tc_tmap(h->tc, {b.q, 3, {64, Lp, SH}, {128, Lp * 128}, {64, QT, 1}}, &p.q_map))) return r;
+  if ((r = tc_tmap(h->tc, {kbuf, 3, {64, Lp, SH}, {128, Lp * 128}, {64, KB, 1}}, &p.k_map))) return r;
+  if ((r = tc_tmap(h->tc, {b.vt, 3, {Lp, 64, SH}, {Lp * 2, 64 * Lp * 2}, {64, 64, 1}}, &p.vt_map))) return r;
   p.ctxh = b.ctxh; p.ctxl = b.ctxl; p.kv_shift = kv_shift; p.st = st; p.dbg = h->tc.dbg;
-  const dim3 grid(st.Lp / QT, LG_HEADS, st.S);
-  if (int r = lg_func_smem_once((const void*)tc_attention_kernel, SMEM_BYTES)) return r;
-  cudaLaunchConfig_t cfg{};
-  cudaLaunchAttribute at[1];
-  cfg.gridDim = grid; cfg.blockDim = dim3(384); cfg.dynamicSmemBytes = SMEM_BYTES; cfg.stream = stream;
-  if (tc_use_pdl()) {
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-  }
-  const cudaError_t e = cudaLaunchKernelEx(&cfg, tc_attention_kernel, p);
-  if (e != cudaSuccess) return lg_set_cuda_error(e, __FILE__, __LINE__);
-  return 0;
+  return tc_launch(tc_attention_kernel, dim3(st.Lp / QT, LG_HEADS, st.S), 384, SMEM_BYTES, p, stream);
 }

@@ -15,10 +15,7 @@
 // MMA warpgroup g owns the 256-column slot g and the row statistics are merged through shared memory.
 // Threads: 384 = producer warpgroup (warp 0 issues the TMA loads; the warpgroup hands its registers to the others)
 // + 2 MMA warpgroups.
-#include <stdio.h>
-#include <stdlib.h>
-
-#include <unordered_map>
+#include <map>
 
 #include "lg_handle.h"
 #include "tc_common.cuh"
@@ -30,7 +27,7 @@ namespace {
 constexpr int BN = 256, BK = 64;
 constexpr int W_TILE_BYTES = BN * BK * 2;  // 32 KB
 
-enum { TEPI_QKV = 0, TEPI_BF16 = 1, TEPI_LN_GELU = 2, TEPI_RESID = 3, TEPI_F32 = 4, TEPI_LSE = 5, TEPI_ARGMAX = 6, TEPI_CONV = 7 };
+enum { TEPI_QKV = 0, TEPI_LN_GELU = 2, TEPI_RESID = 3, TEPI_F32 = 4, TEPI_LSE = 5, TEPI_ARGMAX = 6, TEPI_CONV = 7 };
 
 struct TcLinParams {
   CUtensorMap a_hi[2], a_lo[2];  // A segment 0 / 1, box 64 x tile rows
@@ -397,7 +394,7 @@ __global__ void __launch_bounds__(LinCfg<NSLOT>::THREADS, 1) tc_linear_kernel(co
     const bool qkv_v = EPI == TEPI_QKV && (p.rope ? which == 2 : which == 1);
     const bool use_rope = EPI == TEPI_QKV && p.rope && !qkv_v;
     const bool f32out = EPI == TEPI_RESID || EPI == TEPI_F32;
-    const bool has16 = EPI == TEPI_BF16 || EPI == TEPI_CONV || EPI == TEPI_RESID || (EPI == TEPI_F32 && p.out_h != nullptr);
+    const bool has16 = EPI == TEPI_CONV || EPI == TEPI_RESID || (EPI == TEPI_F32 && p.out_h != nullptr);
     const bool haslo = has16 && p.out_l != nullptr;
 #pragma unroll
     for (int hr = 0; hr < 2; ++hr) {
@@ -498,8 +495,9 @@ __global__ void split_weights_kernel(const float* __restrict__ w, __nv_bfloat16*
 }
 
 // ------------------------------------------------------------------------------------------------
-// host: tensor maps (cached per handle), launches
+// host: the GEMM entry point, tensor maps, launches
 // ------------------------------------------------------------------------------------------------
+// cuTensorMapEncodeTiled is fetched through the runtime (no link-time dependency on libcuda).
 typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                              const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                              CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -514,150 +512,97 @@ EncodeFn get_encode() {
   }
   return fn;
 }
-}  // namespace
-
-int tc_make_tmap_2d(CUtensorMap* out, const void* base, int elem_bytes, uint64_t inner, uint64_t outer, uint64_t row_stride_bytes,
-                    uint32_t box_inner, uint32_t box_outer, bool swizzle128) {
-  EncodeFn enc = get_encode();
-  if (!enc) return lg_set_error("cuTensorMapEncodeTiled unavailable");
-  cuuint64_t dims[2] = {inner, outer};
-  cuuint64_t strides[1] = {row_stride_bytes};
-  cuuint32_t box[2] = {box_inner, box_outer};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(out, elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_UINT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2,
-                   const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return lg_set_error("cuTensorMapEncodeTiled (2d) failed");
-  return 0;
-}
-
-int tc_make_tmap_3d(CUtensorMap* out, const void* base, int elem_bytes, uint64_t d0, uint64_t d1, uint64_t d2,
-                    uint64_t stride1_bytes, uint64_t stride2_bytes, uint32_t b0, uint32_t b1, uint32_t b2) {
-  EncodeFn enc = get_encode();
-  if (!enc) return lg_set_error("cuTensorMapEncodeTiled unavailable");
-  cuuint64_t dims[3] = {d0, d1, d2};
-  cuuint64_t strides[2] = {stride1_bytes, stride2_bytes};
-  cuuint32_t box[3] = {b0, b1, b2};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(out, elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_UINT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3,
-                   const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return lg_set_error("cuTensorMapEncodeTiled (3d) failed");
-  return 0;
-}
-
-namespace {
-struct MapKey {
-  const void* p; uint64_t a, b, c, d;
-  bool operator==(const MapKey& o) const { return p == o.p && a == o.a && b == o.b && c == o.c && d == o.d; }
-};
-struct MapKeyHash {
-  size_t operator()(const MapKey& k) const {
-    size_t h = (size_t)k.p;
-    for (uint64_t v : {k.a, k.b, k.c, k.d}) h = h * 1000003u ^ (size_t)v;
-    return h;
-  }
-};
-struct MapCache {
-  std::unordered_map<MapKey, CUtensorMap, MapKeyHash> m;
-};
-
-// A operand: [rows, K] bf16 row-major, box 64 x box_rows (the tile height)
-int amap(LgHandle* h, CUtensorMap* out, const void* base, uint64_t rows, uint64_t K, uint32_t box_rows) {
-  MapCache* mc = static_cast<MapCache*>(h->tc.map_cache);
-  MapKey key{base, rows, K, 1 | ((uint64_t)box_rows << 32), 0};
-  auto it = mc->m.find(key);
-  if (it != mc->m.end()) { *out = it->second; return 0; }
-  if (mc->m.size() > 4096) mc->m.clear();
-  int r = tc_make_tmap_2d(out, base, 2, K, rows, K * 2, BK, box_rows);
-  if (r) return r;
-  mc->m.emplace(key, *out);
-  return 0;
-}
-// W operand: nsel x [Nout, K] bf16, box 64 x 256 x 1
-int wmap(LgHandle* h, CUtensorMap* out, const void* base, uint64_t Nout, uint64_t K, uint64_t nsel, uint64_t sel_stride_elems) {
-  MapCache* mc = static_cast<MapCache*>(h->tc.map_cache);
-  MapKey key{base, Nout, K, nsel, sel_stride_elems + 2};
-  auto it = mc->m.find(key);
-  if (it != mc->m.end()) { *out = it->second; return 0; }
-  if (mc->m.size() > 4096) mc->m.clear();
-  int r = tc_make_tmap_3d(out, base, 2, K, Nout, nsel, K * 2, (nsel > 1 ? sel_stride_elems : Nout * K) * 2, BK, BN, 1);
-  if (r) return r;
-  mc->m.emplace(key, *out);
-  return 0;
-}
 
 template <int NSLOT, int EPI>
-int launch_linear_t(TcLinParams& p, int n_tiles, cudaStream_t stream) {
+int launch_linear_t(const TcLinParams& p, cudaStream_t stream) {
   using C = LinCfg<NSLOT>;
-  constexpr int smem = C::SMEM;
-  if (int r = lg_func_smem_once((const void*)tc_linear_kernel<NSLOT, EPI>, smem)) return r;
   const int num_sms = lg_num_sms();
-  p.n_tiles = n_tiles;
-  const int total = n_tiles * p.st.S * (p.st.Lp / C::TBM);
+  const int total = p.n_tiles * p.st.S * (p.st.Lp / C::TBM);
   const int grid = total < num_sms ? total : num_sms;
-  cudaLaunchConfig_t cfg{};
-  cudaLaunchAttribute at[1];
-  if (tc_use_pdl()) {
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-  }
-  cfg.gridDim = dim3(grid); cfg.blockDim = dim3(C::THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, tc_linear_kernel<NSLOT, EPI>, p);
-  if (e != cudaSuccess) return lg_set_cuda_error(e, __FILE__, __LINE__);
-  return 0;
+  return tc_launch(tc_linear_kernel<NSLOT, EPI>, dim3(grid), C::THREADS, C::SMEM, p, stream);
 }
-int launch_linear(TcLinParams& p, int n_tiles, cudaStream_t stream) {
+int launch_linear(const TcLinParams& p, cudaStream_t stream) {
   switch (p.epi) {
-    case TEPI_QKV: return launch_linear_t<1, TEPI_QKV>(p, n_tiles, stream);
-    case TEPI_BF16: return launch_linear_t<1, TEPI_BF16>(p, n_tiles, stream);
-    case TEPI_LN_GELU: return launch_linear_t<2, TEPI_LN_GELU>(p, 1, stream);
-    case TEPI_RESID: return launch_linear_t<1, TEPI_RESID>(p, n_tiles, stream);
-    case TEPI_F32: return launch_linear_t<1, TEPI_F32>(p, n_tiles, stream);
-    case TEPI_CONV: return launch_linear_t<1, TEPI_CONV>(p, n_tiles, stream);
-    case TEPI_LSE: return launch_linear_t<1, TEPI_LSE>(p, n_tiles, stream);
-    case TEPI_ARGMAX: return launch_linear_t<1, TEPI_ARGMAX>(p, n_tiles, stream);
+    case TEPI_QKV: return launch_linear_t<1, TEPI_QKV>(p, stream);
+    case TEPI_LN_GELU: return launch_linear_t<2, TEPI_LN_GELU>(p, stream);
+    case TEPI_RESID: return launch_linear_t<1, TEPI_RESID>(p, stream);
+    case TEPI_F32: return launch_linear_t<1, TEPI_F32>(p, stream);
+    case TEPI_CONV: return launch_linear_t<1, TEPI_CONV>(p, stream);
+    case TEPI_LSE: return launch_linear_t<1, TEPI_LSE>(p, stream);
+    case TEPI_ARGMAX: return launch_linear_t<1, TEPI_ARGMAX>(p, stream);
   }
   return lg_set_error("launch_linear: bad epilogue");
 }
 
-struct LinDesc {
-  const __nv_bfloat16 *a0h, *a0l; int k0;   // segment 0
-  const __nv_bfloat16 *a1h, *a1l; int k1;   // segment 1 (k1 = 0: none)
-  size_t w_off; int nout;                   // offset (elements) into the split weight arrays
+// Operands of one GEMM.  A = [A0 | A1] along K, each [st.S * st.Lp rows, k] bf16 row-major; W = nsel matrices [nout, K]
+// bf16 (K = k0 + k1, or 9 k0 for a 3x3 convolution), sel_stride elements apart.  The lo images are read in bf16x3 only.
+struct TcOperands {
+  const __nv_bfloat16 *a0h, *a0l; int k0;
+  const __nv_bfloat16 *a1h, *a1l; int k1;  // k1 = 0: one segment
+  const __nv_bfloat16 *wh, *wl; int nout;
   int nsel; size_t sel_stride;
 };
 
-int run_linear(LgHandle* h, const SeqState& st, const LinDesc& d, TcLinParams& p, cudaStream_t stream) {
-  const bool x3 = h->cfg.precision == LG_PREC_BF16X3;
+// The one host entry point of tc_linear_kernel: p carries the epilogue fields (and w_select / conv_* / mma_n where they
+// apply); this adds the tensor maps, the K-block and pass counts, and launches n_tiles column tiles per row tile.
+int tc_gemm(TcEngine& e, const SeqState& st, const TcOperands& d, int n_tiles, TcLinParams& p, cudaStream_t stream) {
   const uint64_t rows = (uint64_t)st.S * st.Lp;
   const uint32_t tbm = p.epi == TEPI_LN_GELU ? LinCfg<2>::TBM : LinCfg<1>::TBM;
-  const int K = d.k0 + d.k1;
+  const uint64_t K = p.conv_cb ? 9 * d.k0 : d.k0 + d.k1, nout = d.nout, nsel = d.nsel;
+  const uint64_t sel_bytes = (nsel > 1 ? d.sel_stride : nout * K) * 2;
+  auto amap = [&](CUtensorMap* out, const void* a, uint64_t k) {  // box 64 x the tile height
+    return tc_tmap(e, {a, 2, {k, rows}, {k * 2}, {BK, tbm}}, out);
+  };
+  auto wmap = [&](CUtensorMap* out, const void* w) { return tc_tmap(e, {w, 3, {K, nout, nsel}, {K * 2, sel_bytes}, {BK, BN, 1}}, out); };
+  // maps the kernel does not read repeat a map it does (segment 1 of a one-segment A, every lo map in bf16)
   int r;
-  if ((r = amap(h, &p.a_hi[0], d.a0h, rows, d.k0, tbm))) return r;
+  if ((r = amap(&p.a_hi[0], d.a0h, d.k0))) return r;
   p.a_hi[1] = p.a_hi[0];
-  if (d.k1 && (r = amap(h, &p.a_hi[1], d.a1h, rows, d.k1, tbm))) return r;
+  if (d.k1 && (r = amap(&p.a_hi[1], d.a1h, d.k1))) return r;
   p.a_lo[0] = p.a_hi[0]; p.a_lo[1] = p.a_hi[1];
-  if (x3) {
-    if ((r = amap(h, &p.a_lo[0], d.a0l, rows, d.k0, tbm))) return r;
+  if (e.x3) {
+    if ((r = amap(&p.a_lo[0], d.a0l, d.k0))) return r;
     p.a_lo[1] = p.a_lo[0];
-    if (d.k1 && (r = amap(h, &p.a_lo[1], d.a1l, rows, d.k1, tbm))) return r;
+    if (d.k1 && (r = amap(&p.a_lo[1], d.a1l, d.k1))) return r;
   }
-  if ((r = wmap(h, &p.w_hi, h->tc.w_hi + d.w_off, d.nout, K, d.nsel, d.sel_stride))) return r;
+  if ((r = wmap(&p.w_hi, d.wh))) return r;
   p.w_lo = p.w_hi;
-  if (x3 && (r = wmap(h, &p.w_lo, h->tc.w_lo + d.w_off, d.nout, K, d.nsel, d.sel_stride))) return r;
-  p.kb0 = d.k0 / BK;
-  p.kb_total = K / BK;
-  p.passes = x3 ? 3 : 1;
+  if (e.x3 && (r = wmap(&p.w_lo, d.wl))) return r;
+  p.kb_total = (int)(K / BK);
+  p.kb0 = d.k1 ? d.k0 / BK : p.kb_total;
+  p.passes = e.x3 ? 3 : 1;
+  p.n_tiles = n_tiles;
   p.st = st;
-  if (p.w_select != 2) p.w_select = d.nsel > 1;
-  p.dbg = h->tc.dbg;
+  p.dbg = e.dbg;
+  return launch_linear(p, stream);
+}
+
+// a matcher GEMM: one launch of the handle's count
+int run_linear(LgHandle* h, const SeqState& st, const TcOperands& d, int n_tiles, TcLinParams& p, cudaStream_t stream) {
   h->launches += 1;
-  return launch_linear(p, d.nout / BN, stream);
+  return tc_gemm(h->tc, st, d, n_tiles, p, stream);
 }
 }  // namespace
+
+struct TcMapCache {
+  std::map<TmapArgs, CUtensorMap> m;
+};
+
+int tc_tmap(TcEngine& e, const TmapArgs& a, CUtensorMap* out) {
+  auto& m = e.maps->m;
+  auto it = m.find(a);
+  if (it != m.end()) { *out = it->second; return 0; }
+  if (m.size() > 4096) m.clear();
+  EncodeFn enc = get_encode();
+  if (!enc) return lg_set_error("cuTensorMapEncodeTiled unavailable");
+  const cuuint32_t estr[3] = {1, 1, 1};
+  if (enc(out, a.dtype, a.rank, const_cast<void*>(a.base), a.dims.data(), a.strides.data(), a.box.data(), estr,
+          CU_TENSOR_MAP_INTERLEAVE_NONE, a.swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
+    return lg_set_error("cuTensorMapEncodeTiled failed");
+  m.emplace(a, *out);
+  return 0;
+}
 
 // ------------------------------------------------------------------------------------------------
 // entry points used by lg_api.cu
@@ -672,6 +617,8 @@ int tc_assign_sweeps(LgHandle* h, const TcBuffers& b, const SeqState& st, const 
   float* logmat = a.log_assignment;
   const int M = a.M, N = a.N;
   const int ntc = (st.Lp + BN - 1) / BN;
+  // A = p of every sequence, W = p of its partner sequence (w_select 2)
+  const TcOperands ops{b.msgh, b.msgl, LG_DIM, nullptr, nullptr, 0, b.msgh, b.msgl, st.Lp, st.S, (size_t)st.Lp * LG_DIM};
   for (int sweep = 0; sweep < 2; ++sweep) {
     TcLinParams p{};
     p.epi = sweep == 0 ? TEPI_LSE : TEPI_ARGMAX;
@@ -679,21 +626,10 @@ int tc_assign_sweeps(LgHandle* h, const TcBuffers& b, const SeqState& st, const 
     p.part = part; p.part_arg = part_arg; p.part_stride = 2 * ntc; p.term = term;
     p.logmat = sweep == 1 ? logmat : nullptr; p.mat_m = M; p.mat_n = N;
     p.w_select = 2;
-    const bool x3 = h->cfg.precision == LG_PREC_BF16X3;
-    const uint64_t rows = (uint64_t)st.S * st.Lp;
     int r;
-    if ((r = amap(h, &p.a_hi[0], b.msgh, rows, LG_DIM, LinCfg<1>::TBM))) return r;
-    p.a_hi[1] = p.a_hi[0]; p.a_lo[0] = p.a_hi[0]; p.a_lo[1] = p.a_hi[0];
-    if (x3) { if ((r = amap(h, &p.a_lo[0], b.msgl, rows, LG_DIM, LinCfg<1>::TBM))) return r; p.a_lo[1] = p.a_lo[0]; }
-    if ((r = wmap(h, &p.w_hi, b.msgh, st.Lp, LG_DIM, st.S, (uint64_t)st.Lp * LG_DIM))) return r;
-    p.w_lo = p.w_hi;
-    if (x3 && (r = wmap(h, &p.w_lo, b.msgl, st.Lp, LG_DIM, st.S, (uint64_t)st.Lp * LG_DIM))) return r;
-    p.kb0 = LG_DIM / BK; p.kb_total = LG_DIM / BK; p.passes = x3 ? 3 : 1;
-    p.st = st; p.dbg = h->tc.dbg;
-    h->launches += 1;
     {
       Timer tm(h, LG_K_ASSIGN_MATRIX, stream, sweep == 1 && logmat != nullptr);  // the matrix-writing sweep on its own
-      if ((r = launch_linear(p, ntc, stream))) return r;
+      if ((r = run_linear(h, st, ops, ntc, p, stream))) return r;
     }
     if (sweep == 0) {
       if ((r = misc_assign_term(a, st, part, 2 * ntc, BN / 2, term, stream))) return r;
@@ -706,44 +642,41 @@ int tc_assign_sweeps(LgHandle* h, const TcBuffers& b, const SeqState& st, const 
   return r;
 }
 
-unsigned int tc_debug_timeout_code(LgHandle* h, unsigned int* words32) {
+unsigned int tc_debug_timeout_code(const TcEngine& e, unsigned int* words32) {
   unsigned int v[32] = {0};
-  if (!h->tc.dbg) return 0;
-  if (cudaMemcpy(v, h->tc.dbg, sizeof(v), cudaMemcpyDeviceToHost) != cudaSuccess) return 0xffffffffu;
+  if (!e.dbg) return 0;
+  if (cudaMemcpy(v, e.dbg, sizeof(v), cudaMemcpyDeviceToHost) != cudaSuccess) return 0xffffffffu;
   unsigned int first = 0;
   for (int i = 0; i < 32; ++i) {
     if (words32) words32[i] = v[i];
     if (v[i] && !first) first = (unsigned)i << 24 | (v[i] & 0x80ffffffu);
   }
-  if (first) cudaMemset(h->tc.dbg, 0, sizeof(v));
+  if (first) cudaMemset(e.dbg, 0, sizeof(v));
   return first;
 }
 
-int tc_pack_weights(LgHandle* h, cudaStream_t stream) {
-  TcWeights& w = h->tc;
-  const size_t n = h->wpk_floats;
-  cudaError_t e = cudaMalloc(&w.w_hi, n * sizeof(__nv_bfloat16));
-  if (e != cudaSuccess) return lg_set_cuda_error(e, __FILE__, __LINE__);
-  e = cudaMalloc(&w.w_lo, n * sizeof(__nv_bfloat16));
-  if (e != cudaSuccess) return lg_set_cuda_error(e, __FILE__, __LINE__);
-  split_weights_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(h->wpk, w.w_hi, w.w_lo, n);
+int tc_engine_create(TcEngine* e, const float* w, size_t n, bool x3, cudaStream_t stream) {
+  e->x3 = x3;
+  cudaError_t err = cudaMalloc(&e->w_hi, n * sizeof(__nv_bfloat16));
+  if (err != cudaSuccess) return lg_set_cuda_error(err, __FILE__, __LINE__);
+  err = cudaMalloc(&e->w_lo, n * sizeof(__nv_bfloat16));
+  if (err != cudaSuccess) return lg_set_cuda_error(err, __FILE__, __LINE__);
+  split_weights_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(w, e->w_hi, e->w_lo, n);
   LG_CHECK_LAUNCH();
-  w.map_cache = new MapCache();
-  e = cudaMalloc(&w.dbg, 32 * sizeof(unsigned int));
-  if (e != cudaSuccess) return lg_set_cuda_error(e, __FILE__, __LINE__);
-  cudaMemsetAsync(w.dbg, 0, 32 * sizeof(unsigned int), stream);
+  e->maps = new TcMapCache();
+  err = cudaMalloc(&e->dbg, 32 * sizeof(unsigned int));
+  if (err != cudaSuccess) return lg_set_cuda_error(err, __FILE__, __LINE__);
+  cudaMemsetAsync(e->dbg, 0, 32 * sizeof(unsigned int), stream);
   if (!get_encode()) return lg_set_error("cuTensorMapEncodeTiled unavailable (driver too old?)");
   return 0;
 }
 
-void tc_free_weights(TcWeights* w) {
-  if (w->w_hi) cudaFree(w->w_hi);
-  if (w->w_lo) cudaFree(w->w_lo);
-  if (w->map_cache) delete static_cast<MapCache*>(w->map_cache);
-  if (w->dbg) cudaFree(w->dbg);
-  w->dbg = nullptr;
-  w->w_hi = w->w_lo = nullptr;
-  w->map_cache = nullptr;
+void tc_engine_destroy(TcEngine* e) {
+  if (e->w_hi) cudaFree(e->w_hi);
+  if (e->w_lo) cudaFree(e->w_lo);
+  delete e->maps;
+  if (e->dbg) cudaFree(e->dbg);
+  *e = TcEngine{};
 }
 
 void tc_carve(size_t* off, char* base, size_t S, int Lp, const LgHandle* h, TcBuffers* b) {
@@ -783,47 +716,37 @@ int tc_input_proj(LgHandle* h, const TcBuffers& b, const SeqState& st, const flo
   TcLinParams p{};
   p.epi = TEPI_F32; p.scale = 1.f; p.bias = h->wpk + h->o_inb;
   p.out_f32 = x; p.ldo = LG_DIM; p.out_h = b.xh; p.out_l = b.xl; p.ldb = LG_DIM;
-  LinDesc ld{b.hh, b.hl, d, nullptr, nullptr, 0, h->o_inw, LG_DIM, 1, 0};
-  return run_linear(h, st, ld, p, stream);
+  const TcOperands ops{b.hh, b.hl, d, nullptr, nullptr, 0, h->tc.w_hi + h->o_inw, h->tc.w_lo + h->o_inw, LG_DIM, 1, 0};
+  return run_linear(h, st, ops, 1, p, stream);
 }
 
 int tc_final_proj(LgHandle* h, const TcBuffers& b, const SeqState& st, float* p_out, cudaStream_t stream) {
   TcLinParams p{};
   p.epi = TEPI_F32; p.scale = 0.25f;  // / 256^(1/4) (lightglue.py:291)
+  p.w_select = 1;  // final_proj of the layer each pair stopped at
   p.bias = h->wpk + h->o_assign + AO_FB; p.bias_sel_stride = ASSIGN_BLOB_PAD;
   p.out_f32 = p_out; p.ldo = LG_DIM; p.out_h = b.msgh; p.out_l = b.msgl; p.ldb = LG_DIM;  // bf16 images feed the sweeps
-  LinDesc ld{b.xh, b.xl, LG_DIM, nullptr, nullptr, 0, h->o_assign + AO_FW, LG_DIM, h->cfg.n_layers, ASSIGN_BLOB_PAD};
-  return run_linear(h, st, ld, p, stream);
+  const size_t w = h->o_assign + AO_FW;
+  const TcOperands ops{b.xh, b.xl, LG_DIM, nullptr, nullptr, 0, h->tc.w_hi + w, h->tc.w_lo + w, LG_DIM, h->cfg.n_layers,
+                       ASSIGN_BLOB_PAD};
+  return run_linear(h, st, ops, 1, p, stream);
 }
 
-int tc_conv(LgHandle* h, const SeqState& st, const __nv_bfloat16* in_h, const __nv_bfloat16* in_l, int cin, int taps, size_t w_off,
+int tc_conv(TcEngine& e, const SeqState& st, const __nv_bfloat16* in_h, const __nv_bfloat16* in_l, int cin, int taps, size_t w_off,
             const float* bias, int relu, int B, int H, int W, __nv_bfloat16* out_h, __nv_bfloat16* out_l, int cout, float* out_f32,
             int ldo, cudaStream_t stream) {
-  const bool x3 = h->cfg.precision == LG_PREC_BF16X3;
-  const uint64_t rows = (uint64_t)st.S * st.Lp;
-  const int K = taps * cin;
   if (cin % BK != 0 || (taps != 1 && taps != 9)) return lg_set_error("tc_conv: Cin must be a multiple of 64, 1x1 or 3x3");
   TcLinParams p{};
   p.epi = out_f32 ? TEPI_F32 : TEPI_CONV;
   p.scale = 1.f; p.bias = bias; p.relu = relu;
-  p.out_f32 = out_f32; p.ldo = ldo; p.out_h = out_h; p.out_l = x3 ? out_l : nullptr; p.ldb = cout;
-  int r;
-  if ((r = amap(h, &p.a_hi[0], in_h, rows, cin, LinCfg<1>::TBM))) return r;
-  p.a_hi[1] = p.a_hi[0]; p.a_lo[0] = p.a_hi[0]; p.a_lo[1] = p.a_hi[0];
-  if (x3) { if ((r = amap(h, &p.a_lo[0], in_l, rows, cin, LinCfg<1>::TBM))) return r; p.a_lo[1] = p.a_lo[0]; }
-  if ((r = wmap(h, &p.w_hi, h->tc.w_hi + w_off, BN, K, 1, 0))) return r;
-  p.w_lo = p.w_hi;
-  if (x3 && (r = wmap(h, &p.w_lo, h->tc.w_lo + w_off, BN, K, 1, 0))) return r;
+  p.out_f32 = out_f32; p.ldo = ldo; p.out_h = out_h; p.out_l = e.x3 ? out_l : nullptr; p.ldb = cout;
   const int mma_n = cout <= 64 ? 64 : cout <= 128 ? 128 : BN;  // no MMA columns for the zero rows of a narrow layer
   p.mma_n = mma_n == BN ? 0 : mma_n;
-  p.kb0 = p.kb_total = K / BK;
-  p.passes = x3 ? 3 : 1;
-  p.st = st; p.w_select = 0; p.dbg = h->tc.dbg;
   p.conv_cb = taps == 9 ? cin / BK : 0;
   p.conv_w2 = W + 2; p.conv_h = H; p.conv_w = W;
   p.conv_plane = (long)(H + 2) * (W + 2); p.conv_rows = (long)B * p.conv_plane;
-  h->launches += 1;
-  return launch_linear(p, 1, stream);
+  const TcOperands ops{in_h, in_l, cin, nullptr, nullptr, 0, e.w_hi + w_off, e.w_lo + w_off, BN, 1, 0};
+  return tc_gemm(e, st, ops, 1, p, stream);
 }
 
 int tc_block(LgHandle* h, const TcBuffers& b, const SeqState& st, int layer, int blk, float* x, const float* cs,
@@ -831,19 +754,20 @@ int tc_block(LgHandle* h, const TcBuffers& b, const SeqState& st, int layer, int
   const BlockOff& o = blk == 0 ? h->bself : h->bcross;
   const size_t base = h->o_layers + (size_t)layer * h->layer_stride + (blk == 0 ? 0 : h->bself.total);
   const float* bw = h->wpk + base;
+  const __nv_bfloat16 *wh = h->tc.w_hi + base, *wl = h->tc.w_lo + base;
   // Tile order against the 50 MB L2: every kernel of the chain reads what its predecessor wrote, and only the part written
   // LAST is still resident.  QKV and ffn.0 walk their tile lists backwards, ffn.3 (and the attention grid) forwards: ffn.3
   // starts on the hidden tiles ffn.0 finished with, the next QKV on the x images ffn.3 finished with, attention on the
   // q / k / v of the sequences QKV wrote last, ffn.0 on the context of the sequences attention wrote last.
-  static const bool no_rev = getenv("LG_TC_NO_REVERSE") && atoi(getenv("LG_TC_NO_REVERSE")) != 0;
   {  // QKV (+RoPE) / [to_qk | to_v] projection
     Timer t(h, LG_K_LINEAR, stream);
     Timer t2(h, LG_K_QKV, stream);
     TcLinParams p{};
-    p.epi = TEPI_QKV; p.rope = blk == 0; p.scale = 1.f; p.bias = bw + o.bp; p.reverse = no_rev ? 0 : 1;
+    p.epi = TEPI_QKV; p.rope = blk == 0; p.scale = 1.f; p.bias = bw + o.bp; p.reverse = 1;
     p.q = b.q; p.k = b.k; p.vt = b.vt; p.cs = cs;
-    LinDesc ld{b.xh, b.xl, LG_DIM, nullptr, nullptr, 0, base + o.wp, blk == 0 ? 3 * LG_DIM : 2 * LG_DIM, 1, 0};
-    int r = run_linear(h, st, ld, p, stream);
+    const int nout = blk == 0 ? 3 * LG_DIM : 2 * LG_DIM;
+    const TcOperands ops{b.xh, b.xl, LG_DIM, nullptr, nullptr, 0, wh + o.wp, wl + o.wp, nout, 1, 0};
+    int r = run_linear(h, st, ops, nout / BN, p, stream);
     if (r) return r;
   }
   {
@@ -852,33 +776,24 @@ int tc_block(LgHandle* h, const TcBuffers& b, const SeqState& st, int layer, int
     if (r) return r;
   }
   Timer t(h, LG_K_LINEAR, stream);
-  static const bool no_fold = getenv("LG_TC_NO_FOLD") && atoi(getenv("LG_TC_NO_FOLD")) != 0;  // debug: separate out_proj launch
-  if (no_fold) {  // out_proj / to_out -> msg
-    TcLinParams p{};
-    p.epi = TEPI_BF16; p.scale = 1.f; p.bias = bw + o.bo; p.out_h = b.msgh; p.out_l = b.msgl; p.ldb = LG_DIM;
-    LinDesc ld{b.ctxh, b.ctxl, LG_DIM, nullptr, nullptr, 0, base + o.wo, LG_DIM, 1, 0};
-    int r = run_linear(h, st, ld, p, stream);
-    if (r) return r;
-  }
   {  // ffn.0 on cat([x, msg]) + LayerNorm + GELU -> h; the output projection is folded into the weights (W1f, b1f:
      // lg_handle.h), so the GEMM reads cat([x, ctx]) and `msg` is never formed
     TcLinParams p{};
-    p.epi = TEPI_LN_GELU; p.scale = 1.f; p.bias = bw + (no_fold ? o.b1 : o.b1f); p.ln_g = bw + o.g; p.ln_b = bw + o.be;
-    p.reverse = no_rev ? 0 : 1;
+    p.epi = TEPI_LN_GELU; p.scale = 1.f; p.bias = bw + o.b1f; p.ln_g = bw + o.g; p.ln_b = bw + o.be;
+    p.reverse = 1;
     p.out_h = b.hh; p.out_l = b.hl; p.ldb = LG_FFN;
-    LinDesc ld{b.xh, b.xl, LG_DIM, no_fold ? b.msgh : b.ctxh, no_fold ? b.msgl : b.ctxl, LG_DIM, base + (no_fold ? o.w1 : o.w1f),
-               LG_FFN, 1, 0};
+    const TcOperands ops{b.xh, b.xl, LG_DIM, b.ctxh, b.ctxl, LG_DIM, wh + o.w1f, wl + o.w1f, LG_FFN, 1, 0};
     Timer t2(h, LG_K_FFN0, stream);
-    int r = run_linear(h, st, ld, p, stream);
+    int r = run_linear(h, st, ops, 1, p, stream);  // one 512-column tile: the whole LayerNorm row
     if (r) return r;
   }
   {  // ffn.3 + residual -> x (fp32 master + bf16 shadows)
     TcLinParams p{};
     p.epi = TEPI_RESID; p.scale = 1.f; p.bias = bw + o.b2; p.out_f32 = x; p.ldo = LG_DIM;
     p.out_h = b.xh; p.out_l = b.xl; p.ldb = LG_DIM;
-    LinDesc ld{b.hh, b.hl, LG_FFN, nullptr, nullptr, 0, base + o.w2, LG_DIM, 1, 0};
+    const TcOperands ops{b.hh, b.hl, LG_FFN, nullptr, nullptr, 0, wh + o.w2, wl + o.w2, LG_DIM, 1, 0};
     Timer t2(h, LG_K_FFN3, stream);
-    int r = run_linear(h, st, ld, p, stream);
+    int r = run_linear(h, st, ops, 1, p, stream);
     if (r) return r;
   }
   return 0;

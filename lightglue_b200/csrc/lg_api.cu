@@ -227,7 +227,7 @@ extern "C" int lg_create(const LgConfig* cfg, const float* blob, size_t n_floats
     h->thr[i] = (float)t;
   }
   if (cfg->precision != LG_PREC_FP32) {
-    int r = tc_pack_weights(h, stream);
+    int r = tc_engine_create(&h->tc, h->wpk, h->wpk_floats, cfg->precision == LG_PREC_BF16X3, stream);
     if (r) return r;
   }
   guard.h = nullptr;
@@ -238,14 +238,14 @@ extern "C" int lg_create(const LgConfig* cfg, const float* blob, size_t n_floats
 extern "C" int lg_destroy(LgHandle* h) {
   if (!h) return 0;
   if (h->wpk) cudaFree(h->wpk);
-  tc_free_weights(&h->tc);
+  tc_engine_destroy(&h->tc);
   for (int i = 0; i < LG_K_CLASSES; ++i)
     for (cudaEvent_t e : h->ev[i]) cudaEventDestroy(e);
   delete h;
   return 0;
 }
 
-extern "C" uint32_t lg_debug_timeout_code(LgHandle* h, uint32_t* words32) { return h ? tc_debug_timeout_code(h, words32) : 0; }
+extern "C" uint32_t lg_debug_timeout_code(LgHandle* h, uint32_t* words32) { return h ? tc_debug_timeout_code(h->tc, words32) : 0; }
 
 extern "C" int64_t lg_last_launch_count(const LgHandle* h) { return h ? h->launches : 0; }
 

@@ -42,7 +42,7 @@ struct LgHandle {
   BlockOff bself, bcross;
   size_t layer_stride;
   float thr[64];  // confidence_thresholds (lightglue.py:631-634)
-  TcWeights tc;   // bf16 hi/lo copies for the tensor-core path (unused in fp32 mode)
+  TcEngine tc;    // tensor-core path: bf16 hi/lo copies of wpk, tensor maps (all zero in fp32 mode)
   int64_t launches;
   float* dbg_layers; size_t dbg_layers_floats;  // lg_debug_capture_layers
   bool timing;

@@ -1,6 +1,7 @@
 // SuperPoint encoder + heads on the tensor cores (SURVEY.md 8f1; reference lightglue/superpoint.py:137-153, 171-190,
-// 220-221): the twelve convolutions as implicit GEMMs through the matcher's wgmma / TMA linear kernels
-// (k_tc_linear.cu, tc_conv), split-bf16 operands (hi + lo, three MMAs per product: ~fp32 accuracy), fp32 accumulate.
+// 220-221): the twelve convolutions as implicit GEMMs through the wgmma / TMA linear kernel the matcher uses, on an
+// engine of their own (k_tc_linear.cu, tc_conv), split-bf16 operands (hi + lo, three MMAs per product: ~fp32
+// accuracy), fp32 accumulate.
 //
 // Data layout: every feature map is a ZERO-PADDED NHWC image stored as a matrix [rows, C] of bf16 hi / lo images, row =
 // padded pixel b (H+2)(W+2) + y (W+2) + x.  A 3x3 tap (dy, dx) of such a map is the same matrix shifted by
@@ -13,7 +14,8 @@
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 
-#include "lg_handle.h"
+#include <new>
+
 #include "sp_pipeline.h"
 #include "sp_tc.h"
 
@@ -394,47 +396,39 @@ size_t sp_tc_workspace_bytes(int B, int H, int W) {
 int sp_tc_create(SpTc** out, const float* wts_dev, cudaStream_t stream) {
   SpTc* t = new (std::nothrow) SpTc();
   if (!t) return lg_set_error("sp_tc_create: out of host memory");
-  LgHandle& h = t->lg;
-  memset(&h.cfg, 0, sizeof(h.cfg));
-  h.cfg.precision = LG_PREC_BF16X3;
-  h.launches = 0; h.timing = false; h.dbg_layers = nullptr; h.dbg_layers_floats = 0;
-  for (int i = 0; i < LG_K_CLASSES; ++i) h.ev_used[i] = 0;
-  memset(&h.tc, 0, sizeof(h.tc));
   size_t c = 0;
   for (int l = 0; l < 12; ++l) {
     const SpLayer& L = SP_LAYERS[l];
     t->w_off[l] = c; c += (size_t)256 * L.k * L.k * (L.cin < 64 ? 64 : L.cin);
     t->b_off[l] = c; c += 256;
   }
-  h.wpk_floats = c;
-  cudaError_t e = cudaMalloc(&h.wpk, c * sizeof(float));
+  cudaError_t e = cudaMalloc(&t->wpk, c * sizeof(float));
   if (e != cudaSuccess) { delete t; return lg_set_cuda_error(e, __FILE__, __LINE__); }
-  cudaMemsetAsync(h.wpk, 0, c * sizeof(float), stream);
+  cudaMemsetAsync(t->wpk, 0, c * sizeof(float), stream);
   for (int l = 1; l < 12; ++l) {  // conv1a (Cin = 1) runs on the CUDA cores from the reference layout
     const SpLayer& L = SP_LAYERS[l];
     const float* w = wts_dev + sp_layer_offset(l);
-    sp_repack_kernel<<<256, 256, 0, stream>>>(w, w + (size_t)L.cout * L.cin * L.k * L.k, h.wpk + t->w_off[l], h.wpk + t->b_off[l],
+    sp_repack_kernel<<<256, 256, 0, stream>>>(w, w + (size_t)L.cout * L.cin * L.k * L.k, t->wpk + t->w_off[l], t->wpk + t->b_off[l],
                                              L.cout, L.cin, L.k * L.k);
   }
   e = cudaGetLastError();
-  if (e != cudaSuccess) { cudaFree(h.wpk); delete t; return lg_set_cuda_error(e, __FILE__, __LINE__); }
-  int r = tc_pack_weights(&h, stream);  // bf16 hi / lo images of the packed weights, tensor-map cache, debug words
-  if (r) { tc_free_weights(&h.tc); cudaFree(h.wpk); delete t; return r; }
+  if (e != cudaSuccess) { sp_tc_destroy(t); return lg_set_cuda_error(e, __FILE__, __LINE__); }
+  int r = tc_engine_create(&t->tc, t->wpk, c, true, stream);
+  if (r) { sp_tc_destroy(t); return r; }
   *out = t;
   return 0;
 }
 
 void sp_tc_destroy(SpTc* t) {
   if (!t) return;
-  tc_free_weights(&t->lg.tc);
-  if (t->lg.wpk) cudaFree(t->lg.wpk);
+  tc_engine_destroy(&t->tc);
+  if (t->wpk) cudaFree(t->wpk);
   delete t;
 }
 
 // image [B,1,H,W] fp32 -> logits_nchw [B,65,H/8,W/8], dense_nchw [B,256,H/8,W/8] (un-normalised), fp32
 int sp_tc_backbone(SpTc* t, const float* wts_dev, const float* image, int B, int H, int W, void* workspace, float* logits_nchw,
                    float* dense_nchw, cudaStream_t stream) {
-  LgHandle* h = &t->lg;
   const Level lv[4] = {level(B, H, W), level(B, H / 2, W / 2), level(B, H / 4, W / 4), level(B, H / 8, W / 8)};
   char* base = (char*)workspace;
   size_t off = 0;
@@ -453,7 +447,7 @@ int sp_tc_backbone(SpTc* t, const float* wts_dev, const float* image, int B, int
   auto state = [&](int i) { return SeqState{2, 1, lv[i].Lp, stw + 4 * i, stw + 4 * i + 2}; };
   auto conv = [&](int l, int li, __nv_bfloat16** in, __nv_bfloat16** out, float* out_f32, int ldo, int relu) {
     const SpLayer& L = SP_LAYERS[l];
-    return tc_conv(h, state(li), in[0], in[1], L.cin, L.k * L.k, t->w_off[l], h->wpk + t->b_off[l], relu, B, lv[li].H, lv[li].W,
+    return tc_conv(t->tc, state(li), in[0], in[1], L.cin, L.k * L.k, t->w_off[l], t->wpk + t->b_off[l], relu, B, lv[li].H, lv[li].W,
                    out ? out[0] : nullptr, out ? out[1] : nullptr, L.cout, out_f32, ldo, stream);
   };
   auto pool = [&](int li, int C, __nv_bfloat16** in, __nv_bfloat16** out) {  // level li -> li + 1

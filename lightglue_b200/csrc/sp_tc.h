@@ -3,13 +3,13 @@
 #include <cuda_runtime.h>
 #include <stddef.h>
 
-#include "lg_handle.h"
+#include "lg_tc.h"
 #include "sp_pipeline.h"
 
 struct SpTc {
-  LgHandle lg;        // carrier for the shared tensor-core linear kernels: precision, packed weights (fp32 + bf16 hi / lo),
-                      // tensor-map cache, debug words -- no matcher state
-  size_t w_off[12];   // float offsets into lg.wpk: weights repacked to [256, k*k*Cin] ...
+  TcEngine tc;        // bf16x3 GEMMs over the bf16 hi / lo images of wpk
+  float* wpk;         // packed fp32 weights (device)
+  size_t w_off[12];   // float offsets into wpk: weights repacked to [256, k*k*Cin] ...
   size_t b_off[12];   // ... and biases padded to [256]
 };
 

@@ -6,7 +6,11 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <stdlib.h>
+
+#include <array>
+#include <tuple>
+
+#include "lg_internal.h"
 
 namespace tc {
 
@@ -81,11 +85,6 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
 // global memory a predecessor writes; both are no-ops in a plain launch.
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-// host: launch attribute for such kernels (LG_NO_PDL=1 falls back to plain stream order)
-inline bool tc_use_pdl() {
-  static const bool on = !(getenv("LG_NO_PDL") && atoi(getenv("LG_NO_PDL")) != 0);
-  return on;
-}
 
 // ---------------------------------------------------------------- warpgroup MMA (wgmma)
 // Accumulators live in the registers of the issuing warpgroup (128 threads).  Layout of an m64nN fp32 accumulator d[]:
@@ -200,9 +199,38 @@ __device__ __forceinline__ void regs_inc() { asm volatile("setmaxnreg.inc.sync.a
 
 }  // namespace tc
 
-// ---------------------------------------------------------------- host: tensor maps
-// cuTensorMapEncodeTiled is fetched through the runtime (no link-time dependency on libcuda).
-int tc_make_tmap_2d(CUtensorMap* out, const void* base, int elem_bytes, uint64_t inner, uint64_t outer, uint64_t row_stride_bytes,
-                    uint32_t box_inner, uint32_t box_outer, bool swizzle128 = true);
-int tc_make_tmap_3d(CUtensorMap* out, const void* base, int elem_bytes, uint64_t d0, uint64_t d1, uint64_t d2,
-                    uint64_t stride1_bytes, uint64_t stride2_bytes, uint32_t b0, uint32_t b1, uint32_t b2);
+// ---------------------------------------------------------------- host: tensor maps, launches
+// The arguments of one cuTensorMapEncodeTiled call (entries past `rank` are zero); also the key of the engine's
+// tensor-map cache, so two maps share an entry only if every argument matches.
+struct TmapArgs {
+  const void* base;
+  uint32_t rank;
+  std::array<uint64_t, 3> dims;     // elements, innermost first
+  std::array<uint64_t, 2> strides;  // bytes, of dims 1 and 2
+  std::array<uint32_t, 3> box;
+  CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B;
+  CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_UINT16;
+  bool operator<(const TmapArgs& o) const {
+    return std::tie(base, rank, dims, strides, box, swizzle, dtype) <
+           std::tie(o.base, o.rank, o.dims, o.strides, o.box, o.swizzle, o.dtype);
+  }
+};
+struct TcEngine;
+// `out` = the map `a` describes, from the engine's cache (encoded on a miss)
+int tc_tmap(TcEngine& e, const TmapArgs& a, CUtensorMap* out);
+
+// Launches a tensor-core kernel with programmatic dependent launch, after opting it in to `smem` bytes of dynamic
+// shared memory on the current device.
+template <class P>
+int tc_launch(void (*kernel)(P), dim3 grid, int threads, int smem, const P& p, cudaStream_t stream) {
+  if (int r = lg_func_smem_once((const void*)kernel, smem)) return r;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  at[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = grid; cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
+  cfg.attrs = at; cfg.numAttrs = 1;
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, p);
+  if (e != cudaSuccess) return lg_set_cuda_error(e, __FILE__, __LINE__);
+  return 0;
+}

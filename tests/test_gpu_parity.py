@@ -345,6 +345,23 @@ def test_disk_n4096_against_oracle():
     assert flips == 0 and dmax < 1e-3
 
 
+def test_single_layer_model_tensor_core_assignment():
+    """A one-layer model on the tensor-core path: final_proj takes the weights of the layer every pair stopped at, which
+    is the only one, so the log-assignment matrix matches the oracle's."""
+    torch.manual_seed(7)
+    sd = synth.make_state_dict(n_layers=1)
+    m = LightGlue(features=None, n_layers=1, precision="bf16x3", depth_confidence=-1, width_confidence=-1)
+    m.load_state_dict(sd, strict=False)
+    m = m.cuda()
+    x0 = torch.randn(2, 300, 256)
+    x1 = torch.randn(2, 517, 256)
+    full, m0, m1, _, _ = m.log_assignment_matrix(0, x0.cuda(), x1.cuda())
+    ref = oracle.log_assignment(sd, 0, x0, x1)
+    assert float((full.cpu() - ref).abs().max()) < 2e-3
+    r0, r1, _, _ = oracle.filter_matches(ref, 0.1)
+    assert torch.equal(m0.cpu(), r0) and torch.equal(m1.cpu(), r1)
+
+
 def test_adaptive_n2048_default_flash_threshold():
     """Adaptive depth/width at N=2048 with the reference's default CUDA+flash pruning threshold (1536, lightglue.py:
     339-344, 658-662): pruning only runs while an image has more than 1536 points.  fp32 path vs the oracle."""
