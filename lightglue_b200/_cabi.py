@@ -18,6 +18,9 @@ EXPORTS = (
 # include/superpoint_b200.h (same library)
 SP_ABI_VERSION = 2
 SP_EXPORTS = ("sp_weight_blob_floats", "sp_create", "sp_destroy", "sp_max_keypoints", "sp_workspace_bytes", "sp_forward")
+# include/aliked_b200.h (same library)
+AL_ABI_VERSION = 1
+AL_EXPORTS = ("al_weight_blob_floats", "al_create", "al_destroy", "al_max_keypoints", "al_workspace_bytes", "al_forward")
 
 
 class LgConfig(C.Structure):
@@ -32,6 +35,14 @@ class SpConfig(C.Structure):
     _fields_ = [
         ("abi_version", C.c_int32), ("nms_radius", C.c_int32), ("max_num_keypoints", C.c_int32),
         ("remove_borders", C.c_int32), ("detection_threshold", C.c_float), ("precision", C.c_int32),
+    ]
+
+
+class AlConfig(C.Structure):
+    _fields_ = [
+        ("abi_version", C.c_int32), ("c1", C.c_int32), ("c2", C.c_int32), ("c3", C.c_int32), ("c4", C.c_int32),
+        ("dim", C.c_int32), ("K", C.c_int32), ("M", C.c_int32), ("nms_radius", C.c_int32),
+        ("max_num_keypoints", C.c_int32), ("detection_threshold", C.c_float),
     ]
 
 
@@ -102,6 +113,19 @@ def load():
     lib.sp_forward.restype = C.c_int
     lib.sp_forward.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64] + [C.c_void_p] * 5 + [
         C.c_size_t, C.c_void_p]
+    lib.al_weight_blob_floats.restype = C.c_size_t
+    lib.al_weight_blob_floats.argtypes = [C.POINTER(AlConfig)]
+    lib.al_create.restype = C.c_int
+    lib.al_create.argtypes = [C.POINTER(AlConfig), C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_void_p)]
+    lib.al_destroy.restype = C.c_int
+    lib.al_destroy.argtypes = [C.c_void_p]
+    lib.al_max_keypoints.restype = C.c_int64
+    lib.al_max_keypoints.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
+    lib.al_workspace_bytes.restype = C.c_size_t
+    lib.al_workspace_bytes.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32]
+    lib.al_forward.restype = C.c_int
+    lib.al_forward.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64] + [
+        C.c_void_p] * 5 + [C.c_size_t, C.c_void_p]
     lib.lg_last_launch_count.restype = C.c_int64
     lib.lg_last_launch_count.argtypes = [C.c_void_p]
     lib.lg_timing_enable.restype = C.c_int

@@ -22,6 +22,7 @@ def _stale() -> bool:
     srcs = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cu", ".h", ".cuh")) or f == "Makefile"]
     srcs.append(os.path.join(os.path.dirname(HERE), "include", "lightglue_b200.h"))
     srcs.append(os.path.join(os.path.dirname(HERE), "include", "superpoint_b200.h"))
+    srcs.append(os.path.join(os.path.dirname(HERE), "include", "aliked_b200.h"))
     return any(os.path.getmtime(s) > t for s in srcs)
 
 

@@ -178,10 +178,12 @@ struct SpRowWrite {
 };
 
 // top-k by score, sorted descending (71-76); ties: lower candidate index first.  Rank by counting: no sort network,
-// no synchronisation.  If an image has <= k candidates they keep their row-major order (the reference returns early).
+// no synchronisation.  If an image has <= k candidates they keep their row-major order (the reference returns early),
+// unless rank_all is set (ALIKED's top-k mode sorts whatever it keeps).
 struct SpSelect {
   const int* n_cand; const int* cand_pos; const float* cand_score; int* sel_pos; float* sel_score; int* n_sel;
   int B, k; long cap, out_cap;  // k <= 0: no limit
+  int rank_all;                 // with k > 0: rank the candidates even when there are no more than k
   SP_HD long count() const { return (long)B * cap; }
   SP_HD void operator()(long i) const {
     const long b = i / cap, j = i % cap;
@@ -190,7 +192,7 @@ struct SpSelect {
     if (j >= n) return;
     const float* s = cand_score + b * cap;
     long rank = j;
-    if (k > 0 && n > k) {
+    if (k > 0 && (n > k || rank_all)) {
       const float me = s[j];
       rank = 0;
       for (int t = 0; t < n; ++t) rank += (s[t] > me || (s[t] == me && t < j)) ? 1 : 0;
@@ -362,8 +364,8 @@ struct SpFunctorStages {
   }
   // top-k by score, descending, ties by candidate index (71-76, 210-218)
   template <class Exec>
-  int select(Exec& exec, const SpWorkspace& ws, int B, int k, long cap, long out_cap) const {
-    SpSelect s{ws.n_cand, ws.cand_pos, ws.cand_score, ws.sel_pos, ws.sel_score, ws.n_sel, B, k, cap, out_cap};
+  int select(Exec& exec, const SpWorkspace& ws, int B, int k, long cap, long out_cap, int rank_all = 0) const {
+    SpSelect s{ws.n_cand, ws.cand_pos, ws.cand_score, ws.sel_pos, ws.sel_score, ws.n_sel, B, k, cap, out_cap, rank_all};
     return exec.run(s);
   }
   // keypoints, scores, bilinearly sampled + normalised descriptors (79-96, 217-226)

@@ -221,7 +221,7 @@ __device__ __forceinline__ unsigned sp_key(float f) {  // order-preserving map f
 __global__ void __launch_bounds__(1024) sp_select_kernel(const int* __restrict__ n_cand, const int* __restrict__ cand_pos,
                                                          const float* __restrict__ cand_score, int* __restrict__ sel_pos,
                                                          float* __restrict__ sel_score, int* __restrict__ n_sel, int k, long cap,
-                                                         long out_cap) {
+                                                         long out_cap, int rank_all) {
   __shared__ float ss[SP_SEL_KMAX];
   __shared__ int sj[SP_SEL_KMAX];
   __shared__ int hist[256];
@@ -232,12 +232,13 @@ __global__ void __launch_bounds__(1024) sp_select_kernel(const int* __restrict__
   const int n = n_cand[b];
   const float* s = cand_score + (long)b * cap;
   const int* pos = cand_pos + (long)b * cap;
-  if (!(k > 0 && n > k)) {  // nothing to drop: row-major order is kept (the reference returns early)
+  if (!(k > 0 && (n > k || (rank_all && n > 0)))) {  // nothing to drop or rank: row-major order is kept (the reference returns early)
     const int m = n < out_cap ? n : (int)out_cap;
     if (tid == 0) n_sel[b] = m;
     for (int j = tid; j < m; j += 1024) { sel_pos[(long)b * out_cap + j] = pos[j]; sel_score[(long)b * out_cap + j] = s[j]; }
     return;
   }
+  if (n < k) k = n;  // rank_all with fewer candidates than k: keep (and rank) them all
   if (tid == 0) { s_prefix = 0u; s_remaining = k; s_count = 0; s_carry = 0; n_sel[b] = k; }
   __syncthreads();
   for (int pass = 3; pass >= 0; --pass) {
@@ -369,8 +370,9 @@ int SpCudaStages::compact_impl(const SpWorkspace& ws, int B, int H, int W, float
                                                                       thr, cap);
   return cudaGetLastError() == cudaSuccess ? 0 : lg_set_error("superpoint: candidate compaction launch failed");
 }
-int SpCudaStages::select_impl(const SpWorkspace& ws, int B, int k, long cap, long out_cap) const {
-  sp_select_kernel<<<B, 1024, 0, stream>>>(ws.n_cand, ws.cand_pos, ws.cand_score, ws.sel_pos, ws.sel_score, ws.n_sel, k, cap, out_cap);
+int SpCudaStages::select_impl(const SpWorkspace& ws, int B, int k, long cap, long out_cap, int rank_all) const {
+  sp_select_kernel<<<B, 1024, 0, stream>>>(ws.n_cand, ws.cand_pos, ws.cand_score, ws.sel_pos, ws.sel_score, ws.n_sel, k, cap, out_cap,
+                                           rank_all);
   return cudaGetLastError() == cudaSuccess ? 0 : lg_set_error("superpoint: top-k launch failed");
 }
 int SpCudaStages::sample_impl(const SpWorkspace& ws, float* kpts, float* kscores, float* desc, int B, int Hc, int Wc,

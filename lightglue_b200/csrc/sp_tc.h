@@ -24,14 +24,15 @@ int sp_tc_backbone(SpTc* t, const float* wts_dev, const float* image, int B, int
 struct SpCudaStages {
   cudaStream_t stream;
   int compact_impl(const SpWorkspace& ws, int B, int H, int W, float thr, long cap) const;
-  int select_impl(const SpWorkspace& ws, int B, int k, long cap, long out_cap) const;
+  int select_impl(const SpWorkspace& ws, int B, int k, long cap, long out_cap, int rank_all) const;
   int sample_impl(const SpWorkspace& ws, float* kpts, float* kscores, float* desc, int B, int Hc, int Wc, long out_cap) const;
   template <class Exec>
   int compact(Exec&, const SpWorkspace& ws, int B, int H, int W, float thr, long cap) const { return compact_impl(ws, B, H, W, thr, cap); }
+  // rank_all: see SpSelect (ALIKED's top-k mode)
   template <class Exec>
-  int select(Exec& exec, const SpWorkspace& ws, int B, int k, long cap, long out_cap) const {
-    if (k > 4096) return SpFunctorStages().select(exec, ws, B, k, cap, out_cap);
-    return select_impl(ws, B, k, cap, out_cap);
+  int select(Exec& exec, const SpWorkspace& ws, int B, int k, long cap, long out_cap, int rank_all = 0) const {
+    if (k > 4096) return SpFunctorStages().select(exec, ws, B, k, cap, out_cap, rank_all);
+    return select_impl(ws, B, k, cap, out_cap, rank_all);
   }
   template <class Exec>
   int sample(Exec&, const SpWorkspace& ws, float* kpts, float* kscores, float* desc, int B, int Hc, int Wc, long out_cap) const {

@@ -10,14 +10,13 @@ optional resize of ``extract`` (the reference uses kornia's antialiased resize, 
 from __future__ import annotations
 
 import ctypes as C
-import os
-from pathlib import Path
 from types import SimpleNamespace
 
 import torch
 from torch import nn
 
 from . import _cabi
+from . import extractor as _extractor
 
 LAYERS = (  # name, out channels, in channels, kernel   (superpoint.py:137-153)
     ("conv1a", 64, 1, 3), ("conv1b", 64, 64, 3), ("conv2a", 64, 64, 3), ("conv2b", 64, 64, 3),
@@ -62,18 +61,7 @@ class SuperPoint(nn.Module):
 
     def _find_checkpoint(self, fname: str):
         """The reference downloads the checkpoint (155-156); offline we look in the usual caches."""
-        cands = [
-            Path(os.environ["LIGHTGLUE_WEIGHTS_DIR"]) / fname if os.environ.get("LIGHTGLUE_WEIGHTS_DIR") else None,
-            Path(torch.hub.get_dir()) / "checkpoints" / fname,
-            Path(__file__).parent / "weights" / fname,
-        ]
-        for c in cands:
-            if c is not None and c.exists():
-                return torch.load(str(c), map_location="cpu")
-        raise FileNotFoundError(
-            f"{fname} not found (no network access: put it under $LIGHTGLUE_WEIGHTS_DIR or torch hub's checkpoints, "
-            f"or construct SuperPoint(weights=None)); upstream URL: {self.url}"
-        )
+        return _extractor.find_checkpoint(fname, self.url, "SuperPoint")
 
     # ------------------------------------------------------------------ C handle
     def _blob(self) -> torch.Tensor:
@@ -163,23 +151,6 @@ class SuperPoint(nn.Module):
 
     @torch.no_grad()
     def extract(self, img: torch.Tensor, **conf) -> dict:
-        """``Extractor.extract`` (utils.py:136-147): add the batch dimension, resize the longer side to ``resize``
-        (``ImagePreprocessor``, utils.py:26-38: ``kornia.geometry.transform.resize(side="long", antialias=True)``: the long
-        side becomes ``resize`` and the other ``int(resize / aspect)`` -- truncated, kornia's ``_side_to_image_size``; kornia
-        itself is not a dependency here), run ``forward``, map keypoints back to the original pixels."""
-        if img.dim() == 3:
-            img = img[None]
-        assert img.dim() == 4 and img.shape[0] == 1
-        h, w = img.shape[-2:]
-        resize = {**self.preprocess_conf, **conf}.get("resize")
-        nh, nw = h, w
-        if resize is not None:
-            aspect = w / h
-            nh, nw = (int(resize / aspect), int(resize)) if aspect >= 1.0 else (int(resize), int(resize * aspect))
-        if (nh, nw) != (h, w):
-            img = torch.nn.functional.interpolate(img, size=(nh, nw), mode="bilinear", antialias=True, align_corners=False)
-        scales = torch.tensor([nw / w, nh / h], device=img.device, dtype=torch.float32)
-        feats = self.forward({"image": img})
-        feats["image_size"] = torch.tensor([[w, h]], device=img.device, dtype=torch.float32)
-        feats["keypoints"] = (feats["keypoints"] + 0.5) / scales[None] - 0.5
-        return feats
+        """``Extractor.extract`` (utils.py:136-147): resize, ``forward``, keypoints back in the original pixels
+        (lightglue_b200/extractor.py)."""
+        return _extractor.extract(self, img, **conf)
