@@ -5,5 +5,6 @@
 kernels behind the C ABI declared in ``include/lightglue_b200.h``.
 """
 from .matcher import LightGlue  # noqa: F401
+from .sift import SIFT  # noqa: F401
 
-__all__ = ["LightGlue"]
+__all__ = ["LightGlue", "SIFT"]

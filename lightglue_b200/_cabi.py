@@ -21,6 +21,9 @@ SP_EXPORTS = ("sp_weight_blob_floats", "sp_create", "sp_destroy", "sp_max_keypoi
 # include/aliked_b200.h (same library)
 AL_ABI_VERSION = 1
 AL_EXPORTS = ("al_weight_blob_floats", "al_create", "al_destroy", "al_max_keypoints", "al_workspace_bytes", "al_forward")
+# include/sift_b200.h (same library)
+SIFT_ABI_VERSION = 1
+SIFT_EXPORTS = ("sift_create", "sift_destroy", "sift_max_keypoints", "sift_workspace_bytes", "sift_forward")
 
 
 class LgConfig(C.Structure):
@@ -43,6 +46,14 @@ class AlConfig(C.Structure):
         ("abi_version", C.c_int32), ("c1", C.c_int32), ("c2", C.c_int32), ("c3", C.c_int32), ("c4", C.c_int32),
         ("dim", C.c_int32), ("K", C.c_int32), ("M", C.c_int32), ("nms_radius", C.c_int32),
         ("max_num_keypoints", C.c_int32), ("detection_threshold", C.c_float),
+    ]
+
+
+class SiftConfig(C.Structure):
+    _fields_ = [
+        ("abi_version", C.c_int32), ("num_octave_layers", C.c_int32), ("nms_radius", C.c_int32),
+        ("max_num_keypoints", C.c_int32), ("rootsift", C.c_int32), ("reserved", C.c_int32),
+        ("detection_threshold", C.c_double), ("edge_threshold", C.c_double),
     ]
 
 
@@ -126,6 +137,17 @@ def load():
     lib.al_forward.restype = C.c_int
     lib.al_forward.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64] + [
         C.c_void_p] * 5 + [C.c_size_t, C.c_void_p]
+    lib.sift_create.restype = C.c_int
+    lib.sift_create.argtypes = [C.POINTER(SiftConfig), C.c_void_p, C.POINTER(C.c_void_p)]
+    lib.sift_destroy.restype = C.c_int
+    lib.sift_destroy.argtypes = [C.c_void_p]
+    lib.sift_max_keypoints.restype = C.c_int64
+    lib.sift_max_keypoints.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
+    lib.sift_workspace_bytes.restype = C.c_size_t
+    lib.sift_workspace_bytes.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32]
+    lib.sift_forward.restype = C.c_int
+    lib.sift_forward.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64] + [
+        C.c_void_p] * 6 + [C.c_void_p, C.c_size_t, C.c_void_p]
     lib.lg_last_launch_count.restype = C.c_int64
     lib.lg_last_launch_count.argtypes = [C.c_void_p]
     lib.lg_timing_enable.restype = C.c_int

@@ -23,6 +23,7 @@ def _stale() -> bool:
     srcs.append(os.path.join(os.path.dirname(HERE), "include", "lightglue_b200.h"))
     srcs.append(os.path.join(os.path.dirname(HERE), "include", "superpoint_b200.h"))
     srcs.append(os.path.join(os.path.dirname(HERE), "include", "aliked_b200.h"))
+    srcs.append(os.path.join(os.path.dirname(HERE), "include", "sift_b200.h"))
     return any(os.path.getmtime(s) > t for s in srcs)
 
 
