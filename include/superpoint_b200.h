@@ -59,6 +59,20 @@ LG_API size_t sp_workspace_bytes(const SpHandle* h, int32_t B, int32_t H, int32_
 LG_API int sp_forward(SpHandle* h, const float* image, int32_t B, int32_t H, int32_t W, int64_t cap, float* keypoints,
                float* scores, float* descriptors, int32_t* counts, void* workspace, size_t workspace_bytes, void* stream);
 
+/* The convolution stack alone, exactly as sp_forward runs it for this handle (either precision): the raw detector logits
+ * [B, 65, H/8, W/8] (superpoint.py:185) and the un-normalised descriptor map [B, 256, H/8, W/8] (221), fp32 NCHW.
+ * Same image and workspace (sp_workspace_bytes) as sp_forward. */
+LG_API int sp_backbone(SpHandle* h, const float* image, int32_t B, int32_t H, int32_t W, float* logits, float* dense,
+                       void* workspace, size_t workspace_bytes, void* stream);
+
+/* Host-only introspection (no handle, no device): the workspace plan of the tensor-core backbone (precision 1) for a
+ * [B, 1, H, W] batch.  Writes, when non-null, the byte offset (from the start of the backbone's part of the workspace) and
+ * the size of each of its SP_TC_BUFFERS buffers, in this order: activations X hi, X lo, Y hi, Y lo (the ping-pong maps),
+ * features hi, lo (conv4b), logits, dense descriptors (fp32, padded NHWC), tile state.  Returns the part's total size in
+ * bytes, 0 for B < 1 or H, W < 8. */
+#define SP_TC_BUFFERS 9
+LG_API int64_t sp_tc_layout(int32_t B, int32_t H, int32_t W, int64_t* offsets, int64_t* bytes);
+
 #ifdef __cplusplus
 }
 #endif

@@ -17,7 +17,9 @@ EXPORTS = (
 )
 # include/superpoint_b200.h (same library)
 SP_ABI_VERSION = 2
-SP_EXPORTS = ("sp_weight_blob_floats", "sp_create", "sp_destroy", "sp_max_keypoints", "sp_workspace_bytes", "sp_forward")
+SP_EXPORTS = ("sp_weight_blob_floats", "sp_create", "sp_destroy", "sp_max_keypoints", "sp_workspace_bytes", "sp_forward",
+              "sp_backbone", "sp_tc_layout")
+SP_TC_BUFFERS = 9  # buffers of the tensor-core backbone's workspace plan (sp_tc_layout)
 # include/aliked_b200.h (same library)
 AL_ABI_VERSION = 1
 AL_EXPORTS = ("al_weight_blob_floats", "al_create", "al_destroy", "al_max_keypoints", "al_workspace_bytes", "al_forward")
@@ -124,6 +126,11 @@ def load():
     lib.sp_forward.restype = C.c_int
     lib.sp_forward.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64] + [C.c_void_p] * 5 + [
         C.c_size_t, C.c_void_p]
+    lib.sp_backbone.restype = C.c_int
+    lib.sp_backbone.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                C.c_size_t, C.c_void_p]
+    lib.sp_tc_layout.restype = C.c_int64
+    lib.sp_tc_layout.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     lib.al_weight_blob_floats.restype = C.c_size_t
     lib.al_weight_blob_floats.argtypes = [C.POINTER(AlConfig)]
     lib.al_create.restype = C.c_int

@@ -41,6 +41,16 @@ int64_t max_keypoints(const SpConfig& c, int H, int W) {
   const int step = c.nms_radius + 1;  // no two NMS survivors lie within `nms_radius` of each other (Chebyshev)
   return (int64_t)((H + step - 1) / step) * ((W + step - 1) / step);
 }
+
+// The convolution stack of this handle's precision -> logits [B,65,Hc,Wc], dense [B,256,Hc,Wc] (fp32 NCHW); `w` is the
+// carve of `workspace`, whose tensor-core part follows the functor buffers
+int run_backbone(SpHandle* h, CudaExec& ex, const float* image, int B, int H, int W, SpWorkspace w, char* workspace,
+                 float* logits, float* dense) {
+  if (h->tc) return sp_tc_backbone(h->tc, h->wts, image, B, H, W, workspace + w.bytes, logits, dense, ex.stream);
+  w.logits = logits;
+  w.dense = dense;
+  return sp_run_backbone(ex, h->wts, image, B, H, W, w);
+}
 }  // namespace
 
 extern "C" size_t sp_weight_blob_floats(void) { return sp_blob_floats(); }
@@ -78,7 +88,18 @@ extern "C" size_t sp_workspace_bytes(const SpHandle* h, int32_t B, int32_t H, in
   if (!h || B <= 0 || H <= 0 || W <= 0) return 0;
   SpWorkspace w;
   sp_carve(nullptr, B, H, W, max_keypoints(h->cfg, H, W), &w);
-  return w.bytes + (h->tc ? sp_tc_workspace_bytes(B, H, W) : 0);
+  return w.bytes + (h->tc ? sp_tc_plan(B, H, W).total : 0);
+}
+
+extern "C" int64_t sp_tc_layout(int32_t B, int32_t H, int32_t W, int64_t* offsets, int64_t* bytes) {
+  static_assert(SPT_NBUF == SP_TC_BUFFERS, "superpoint_b200.h documents the buffers of SpTcPlan");
+  if (B <= 0 || H < SP_CELL || W < SP_CELL) return 0;
+  const SpTcPlan p = sp_tc_plan(B, H, W);
+  for (int i = 0; i < SPT_NBUF; ++i) {
+    if (offsets) offsets[i] = (int64_t)p.off[i];
+    if (bytes) bytes[i] = (int64_t)p.bytes[i];
+  }
+  return (int64_t)p.total;
 }
 
 extern "C" int sp_forward(SpHandle* h, const float* image, int32_t B, int32_t H, int32_t W, int64_t cap, float* keypoints,
@@ -89,26 +110,30 @@ extern "C" int sp_forward(SpHandle* h, const float* image, int32_t B, int32_t H,
   if (cap < max_keypoints(h->cfg, H, W)) return lg_set_error("sp_forward: output capacity below sp_max_keypoints()");
   SpWorkspace w;
   sp_carve((char*)workspace, B, H, W, cap, &w);
-  const size_t need = w.bytes + (h->tc ? sp_tc_workspace_bytes(B, H, W) : 0);
+  const size_t need = w.bytes + (h->tc ? sp_tc_plan(B, H, W).total : 0);
   if (!workspace || workspace_bytes < need) return lg_set_error("sp_forward: workspace too small");
   cudaStream_t stream = (cudaStream_t)stream_;
   CudaExec ex{stream};
   const SpParams prm{h->cfg.nms_radius, h->cfg.max_num_keypoints, h->cfg.remove_borders, h->cfg.detection_threshold};
-  int rc;
-  // Thumbnails (fewer than 64 x 64 pixels) take the CUDA-core path in either precision mode: the 128-row tensor-core tiles
-  // would be mostly padding, and at 9 x 15 / 17 x 33 the tensor-core scores were measured up to 8e-4 off the oracle (same
-  // keypoint sets; 8 x 8, 24 x 131, 67 x 45 and every fixture within 1.5e-4; split-bf16 rounding alone predicts <= 6e-6)
-  // -- an open defect at those shapes, so the path is not used for thumbnails.
-  const bool use_tc = h->tc && (long)H * W >= 64L * 64L;
-  if (use_tc) {  // convolutions on the tensor cores, then the shared post-processing functors
-    rc = sp_tc_backbone(h->tc, h->wts, image, B, H, W, (char*)workspace + w.bytes, w.logits, w.dense, stream);
-    if (!rc) rc = sp_run_post(ex, prm, B, H / SP_CELL * SP_CELL, W / SP_CELL * SP_CELL, cap, w, keypoints, scores, descriptors,
-                              SpCudaStages{stream});
-  } else {
-    rc = sp_run(ex, h->wts, prm, image, B, H, W, cap, w, keypoints, scores, descriptors);
-  }
+  int rc = run_backbone(h, ex, image, B, H, W, w, (char*)workspace, w.logits, w.dense);
+  if (rc) return rc;
+  const int Hs = H / SP_CELL * SP_CELL, Ws = W / SP_CELL * SP_CELL;  // the score map's extents
+  // the tensor-core mode also runs the post-processing's heavy stages as warp / block kernels (same results)
+  rc = h->tc ? sp_run_post(ex, prm, B, Hs, Ws, cap, w, keypoints, scores, descriptors, SpCudaStages{stream})
+             : sp_run_post(ex, prm, B, Hs, Ws, cap, w, keypoints, scores, descriptors);
   if (rc) return rc;
   cudaError_t e = cudaMemcpyAsync(counts, w.n_sel, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToDevice, stream);
   if (e != cudaSuccess) return lg_set_cuda_error(e, __FILE__, __LINE__);
   return 0;
+}
+
+extern "C" int sp_backbone(SpHandle* h, const float* image, int32_t B, int32_t H, int32_t W, float* logits, float* dense,
+                           void* workspace, size_t workspace_bytes, void* stream_) {
+  if (!h || !image || !logits || !dense) return lg_set_error("sp_backbone: null argument");
+  if (B <= 0 || H < SP_CELL || W < SP_CELL) return lg_set_error("sp_backbone: H and W must be at least 8");
+  if (!workspace || workspace_bytes < sp_workspace_bytes(h, B, H, W)) return lg_set_error("sp_backbone: workspace too small");
+  SpWorkspace w;
+  sp_carve((char*)workspace, B, H, W, max_keypoints(h->cfg, H, W), &w);
+  CudaExec ex{(cudaStream_t)stream_};
+  return run_backbone(h, ex, image, B, H, W, w, (char*)workspace, logits, dense);
 }

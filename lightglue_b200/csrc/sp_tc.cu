@@ -14,6 +14,7 @@
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <new>
 
 #include "sp_pipeline.h"
@@ -383,16 +384,33 @@ int SpCudaStages::sample_impl(const SpWorkspace& ws, float* kpts, float* kscores
   return cudaGetLastError() == cudaSuccess ? 0 : lg_set_error("superpoint: descriptor sampling launch failed");
 }
 
-size_t sp_tc_workspace_bytes(int B, int H, int W) {
-  const Level l0 = level(B, H, W), l3 = level(B, H / 8, W / 8);
+SpTcPlan sp_tc_plan(int B, int H, int W) {
+  const Level lv[4] = {level(B, H, W), level(B, H / 2, W / 2), level(B, H / 4, W / 4), level(B, H / 8, W / 8)};
+  // Every write into the ping-pong images X / Y (conv1a, the poolings, the 3x3 convolutions) covers all 2 Lp rows of its
+  // level, padding rows included, with Cout channels; the widest map at each level is 64, 64, 128 (conv3a, conv3b, the
+  // third pooling, conv4a) and 256 channels (convPa, convDa).  On large images the full-resolution map is the largest, but
+  // on small ones every level pads up to the same 256 rows and the 1/4- and 1/8-resolution maps outgrow it.
+  const int xy_channels[4] = {64, 64, 128, 256};
+  size_t xy = 0;
+  for (int i = 0; i < 4; ++i) xy = std::max(xy, (size_t)lv[i].rows * xy_channels[i] * 2);
+  const size_t bytes[SPT_NBUF] = {
+      xy, xy, xy, xy,                    // X hi / lo, Y hi / lo
+      (size_t)lv[3].rows * 128 * 2,      // features hi / lo (conv4b)
+      (size_t)lv[3].rows * 128 * 2,
+      (size_t)lv[3].rows * 96 * 4,       // logits fp32 [rows, 96] (convPb)
+      (size_t)lv[3].rows * 256 * 4,      // dense descriptors fp32 [rows, 256] (convDb)
+      64 * sizeof(int),                  // per-level (len[2], stop_layer[1])
+  };
+  SpTcPlan p{};
   size_t n = 0;
-  auto add = [&](size_t bytes) { n = (n + 1023) & ~(size_t)1023; n += bytes; };
-  for (int i = 0; i < 4; ++i) add((size_t)l0.rows * 64 * 2);   // X hi / lo, Y hi / lo (sized for the full-resolution maps)
-  for (int i = 0; i < 2; ++i) add((size_t)l3.rows * 128 * 2);  // feat hi / lo
-  add((size_t)l3.rows * 96 * 4);                               // logits fp32 [rows, 96]
-  add((size_t)l3.rows * 256 * 4);                              // dense descriptors fp32 [rows, 256]
-  add(64 * sizeof(int));                                       // per-level (len[2], stop_layer[1])
-  return (n + 1023) & ~(size_t)1023;
+  for (int i = 0; i < SPT_NBUF; ++i) {
+    n = (n + 1023) & ~(size_t)1023;
+    p.off[i] = n;
+    p.bytes[i] = bytes[i];
+    n += bytes[i];
+  }
+  p.total = (n + 1023) & ~(size_t)1023;
+  return p;
 }
 
 int sp_tc_create(SpTc** out, const float* wts_dev, cudaStream_t stream) {
@@ -432,16 +450,15 @@ void sp_tc_destroy(SpTc* t) {
 int sp_tc_backbone(SpTc* t, const float* wts_dev, const float* image, int B, int H, int W, void* workspace, float* logits_nchw,
                    float* dense_nchw, cudaStream_t stream) {
   const Level lv[4] = {level(B, H, W), level(B, H / 2, W / 2), level(B, H / 4, W / 4), level(B, H / 8, W / 8)};
+  const SpTcPlan plan = sp_tc_plan(B, H, W);
   char* base = (char*)workspace;
-  size_t off = 0;
-  auto take = [&](size_t bytes) { off = (off + 1023) & ~(size_t)1023; char* p = base + off; off += bytes; return p; };
-  __nv_bfloat16* X[2]; __nv_bfloat16* Y[2]; __nv_bfloat16* F[2];
-  X[0] = (__nv_bfloat16*)take((size_t)lv[0].rows * 64 * 2); X[1] = (__nv_bfloat16*)take((size_t)lv[0].rows * 64 * 2);
-  Y[0] = (__nv_bfloat16*)take((size_t)lv[0].rows * 64 * 2); Y[1] = (__nv_bfloat16*)take((size_t)lv[0].rows * 64 * 2);
-  F[0] = (__nv_bfloat16*)take((size_t)lv[3].rows * 128 * 2); F[1] = (__nv_bfloat16*)take((size_t)lv[3].rows * 128 * 2);
-  float* logits_f = (float*)take((size_t)lv[3].rows * 96 * 4);
-  float* dense_f = (float*)take((size_t)lv[3].rows * 256 * 4);
-  int* stw = (int*)take(64 * sizeof(int));
+  auto at = [&](int buf) { return (__nv_bfloat16*)(base + plan.off[buf]); };
+  __nv_bfloat16* X[2] = {at(SPT_XH), at(SPT_XL)};
+  __nv_bfloat16* Y[2] = {at(SPT_YH), at(SPT_YL)};
+  __nv_bfloat16* F[2] = {at(SPT_FH), at(SPT_FL)};
+  float* logits_f = (float*)(base + plan.off[SPT_LOGITS]);
+  float* dense_f = (float*)(base + plan.off[SPT_DENSE]);
+  int* stw = (int*)(base + plan.off[SPT_STATE]);
   int host_st[16];
   for (int i = 0; i < 4; ++i) { host_st[4 * i] = lv[i].Lp; host_st[4 * i + 1] = lv[i].Lp; host_st[4 * i + 2] = 0; host_st[4 * i + 3] = 0; }
   cudaError_t e = cudaMemcpyAsync(stw, host_st, sizeof(host_st), cudaMemcpyHostToDevice, stream);

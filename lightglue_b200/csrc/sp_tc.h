@@ -13,9 +13,17 @@ struct SpTc {
   size_t b_off[12];   // ... and biases padded to [256]
 };
 
+// The backbone's workspace: one buffer plan shared by its sizing (sp_workspace_bytes), its carving (sp_tc_backbone) and
+// its host-side export (sp_tc_layout).  Buffers in workspace order; offsets are from the start of the backbone's part.
+enum SpTcBuffer { SPT_XH, SPT_XL, SPT_YH, SPT_YL, SPT_FH, SPT_FL, SPT_LOGITS, SPT_DENSE, SPT_STATE, SPT_NBUF };
+struct SpTcPlan {
+  size_t off[SPT_NBUF], bytes[SPT_NBUF];
+  size_t total;
+};
+SpTcPlan sp_tc_plan(int B, int H, int W);
+
 int sp_tc_create(SpTc** out, const float* wts_dev, cudaStream_t stream);
 void sp_tc_destroy(SpTc* t);
-size_t sp_tc_workspace_bytes(int B, int H, int W);
 int sp_tc_backbone(SpTc* t, const float* wts_dev, const float* image, int B, int H, int W, void* workspace, float* logits_nchw,
                    float* dense_nchw, cudaStream_t stream);
 

@@ -103,32 +103,41 @@ class SuperPoint(nn.Module):
         self._release()
 
     # ------------------------------------------------------------------ forward
-    @torch.no_grad()
-    def forward(self, data: dict) -> dict:
-        """Keypoints, scores and descriptors of an image batch (superpoint.py:163-227)."""
-        for key in self.required_data_keys:
-            assert key in data, f"Missing key {key} in data"
-        image = data["image"]
+    @staticmethod
+    def _gray(image: torch.Tensor) -> torch.Tensor:
+        """[B, 1 or 3, H, W] CUDA image -> contiguous fp32 [B, 1, H, W]."""
         if image.device.type != "cuda":
             raise RuntimeError("lightglue_b200.SuperPoint runs on CUDA (sm_90a) tensors only; there is no CPU path")
         if image.shape[1] == 3:  # kornia.color.rgb_to_grayscale's weights (superpoint.py:168-169)
             wts = torch.tensor([0.299, 0.587, 0.114], device=image.device, dtype=image.dtype).view(1, 3, 1, 1)
             image = (image * wts).sum(1, keepdim=True)
-        b, c, hh, ww = image.shape
+        _, c, hh, ww = image.shape
         assert c == 1
         if hh < 8 or ww < 8:
             raise ValueError(f"image size {ww}x{hh}: height and width must be at least 8 (one detector cell)")
+        return image.detach().to(torch.float32).contiguous()
+
+    def _workspace(self, lib, handle, device: torch.device, b: int, hh: int, ww: int) -> torch.Tensor:
+        key = (device.index, b, hh, ww)
+        ws = self._ws.get(key)
+        if ws is None:
+            self._ws.clear()
+            ws = self._ws[key] = torch.empty(int(lib.sp_workspace_bytes(handle, b, hh, ww)), dtype=torch.uint8, device=device)
+        return ws
+
+    @torch.no_grad()
+    def forward(self, data: dict) -> dict:
+        """Keypoints, scores and descriptors of an image batch (superpoint.py:163-227)."""
+        for key in self.required_data_keys:
+            assert key in data, f"Missing key {key} in data"
+        image = self._gray(data["image"])
+        b, _, hh, ww = image.shape
         device = image.device
-        image = image.detach().to(torch.float32).contiguous()
         with torch.cuda.device(device):
             lib = _cabi.load()
             handle = self._get_handle(device)
             cap = int(lib.sp_max_keypoints(handle, hh, ww))
-            key = (device.index, b, hh, ww)
-            ws = self._ws.get(key)
-            if ws is None:
-                self._ws.clear()
-                ws = self._ws[key] = torch.empty(int(lib.sp_workspace_bytes(handle, b, hh, ww)), dtype=torch.uint8, device=device)
+            ws = self._workspace(lib, handle, device, b, hh, ww)
             kpts = torch.empty(b, cap, 2, dtype=torch.float32, device=device)
             scores = torch.empty(b, cap, dtype=torch.float32, device=device)
             desc = torch.empty(b, cap, 256, dtype=torch.float32, device=device)
@@ -148,6 +157,25 @@ class SuperPoint(nn.Module):
             "keypoint_scores": scores[:, :k].contiguous(),
             "descriptors": desc[:, :k].contiguous(),
         }
+
+    @torch.no_grad()
+    def backbone_heads(self, image: torch.Tensor):
+        """Block-level parity (``sp_backbone``): the convolution stack alone, as ``forward`` runs it in this precision --
+        the detector logits ``[B, 65, H/8, W/8]`` (superpoint.py:185) and the un-normalised descriptor map
+        ``[B, 256, H/8, W/8]`` (221), fp32."""
+        image = self._gray(image)
+        b, _, hh, ww = image.shape
+        device = image.device
+        with torch.cuda.device(device):
+            lib = _cabi.load()
+            handle = self._get_handle(device)
+            ws = self._workspace(lib, handle, device, b, hh, ww)
+            logits = torch.empty(b, 65, hh // 8, ww // 8, dtype=torch.float32, device=device)
+            dense = torch.empty(b, 256, hh // 8, ww // 8, dtype=torch.float32, device=device)
+            stream = torch.cuda.current_stream(device).cuda_stream
+            _cabi.check(lib.sp_backbone(handle, image.data_ptr(), b, hh, ww, logits.data_ptr(), dense.data_ptr(), ws.data_ptr(),
+                                        ws.numel(), stream), "sp_backbone")
+        return logits, dense
 
     @torch.no_grad()
     def extract(self, img: torch.Tensor, **conf) -> dict:
