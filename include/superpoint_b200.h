@@ -1,7 +1,7 @@
 /* superpoint_b200 -- C ABI of the SuperPoint extractor forward (SURVEY.md 8f1: the caller-side row next to the
- * matcher), first CUDA path: fp32 on CUDA cores, no tensor cores yet.  Same library (liblightglue_b200.so), same
- * conventions as lightglue_b200.h: plain pointers and sizes, device memory owned by the caller, asynchronous on the
- * given stream, int status (0 = ok, message via lg_last_error()).
+ * matcher); the convolutions run on tensor cores (SpConfig.precision = 1) or in fp32 on CUDA cores.  Same library
+ * (liblightglue_b200.so), same conventions as lightglue_b200.h: plain pointers and sizes, device memory owned by the
+ * caller, asynchronous on the given stream, int status (0 = ok, message via lg_last_error()).
  *
  * Reference interface replaced: lightglue/superpoint.py  SuperPoint.__init__ (126-160) and SuperPoint.forward
  * (163-227) -- encoder, detector head + soft-max, simple_nms (52-68), border removal, threshold, top-k (71-76),

@@ -1,4 +1,4 @@
-"""ctypes binding of include/lightglue_b200.h -- the thin layer between Python and the C ABI."""
+"""ctypes binding of include/*.h -- the thin layer between Python and the C ABI."""
 from __future__ import annotations
 
 import ctypes as C
@@ -10,22 +10,11 @@ PREC = {"fp32": 0, "bf16": 1, "bf16x3": 2}
 K_ATTENTION, K_LINEAR, K_ASSIGN, K_OTHER = 0, 1, 2, 3
 ABI_VERSION = 3
 
-EXPORTS = (
-    "lg_weight_blob_floats", "lg_create", "lg_destroy", "lg_workspace_bytes", "lg_forward", "lg_assign", "lg_attention",
-    "lg_last_launch_count", "lg_timing_enable", "lg_kernel_time_ms", "lg_last_error", "lg_build_info",
-    "lg_debug_timeout_code", "lg_debug_capture_layers", "lg_padded_length",
-)
-# include/superpoint_b200.h (same library)
+# include/superpoint_b200.h, include/aliked_b200.h and include/sift_b200.h: same library
 SP_ABI_VERSION = 2
-SP_EXPORTS = ("sp_weight_blob_floats", "sp_create", "sp_destroy", "sp_max_keypoints", "sp_workspace_bytes", "sp_forward",
-              "sp_backbone", "sp_tc_layout")
 SP_TC_BUFFERS = 9  # buffers of the tensor-core backbone's workspace plan (sp_tc_layout)
-# include/aliked_b200.h (same library)
 AL_ABI_VERSION = 1
-AL_EXPORTS = ("al_weight_blob_floats", "al_create", "al_destroy", "al_max_keypoints", "al_workspace_bytes", "al_forward")
-# include/sift_b200.h (same library)
 SIFT_ABI_VERSION = 1
-SIFT_EXPORTS = ("sift_create", "sift_destroy", "sift_max_keypoints", "sift_workspace_bytes", "sift_forward")
 
 
 class LgConfig(C.Structure):
@@ -79,6 +68,55 @@ class LgOutputs(C.Structure):
     ]
 
 
+
+# name: (restype, argtypes), one table per header.  The export lists are the tables' keys.
+_VP, _I32, _I64, _SZ = C.c_void_p, C.c_int32, C.c_int64, C.c_size_t
+_HANDLE_OUT = C.POINTER(C.c_void_p)
+LG_PROTOTYPES = {  # include/lightglue_b200.h
+    "lg_weight_blob_floats": (_SZ, [_I32, _I32, _I32]),
+    "lg_create": (C.c_int, [C.POINTER(LgConfig), _VP, _SZ, _VP, _HANDLE_OUT]),
+    "lg_destroy": (C.c_int, [_VP]),
+    "lg_workspace_bytes": (_SZ, [_VP, _I32, _I32, _I32]),
+    "lg_forward": (C.c_int, [_VP, C.POINTER(LgInputs), C.POINTER(LgOutputs), _VP, _SZ, _VP]),
+    "lg_assign": (C.c_int, [_VP, _I32, _I32, _I32, _I32, _VP, _VP, C.POINTER(LgOutputs), _VP, _SZ, _VP]),
+    "lg_attention": (C.c_int, [_VP] + [_I32] * 4 + [_VP] * 8 + [_VP, _SZ, _VP]),
+    "lg_last_launch_count": (_I64, [_VP]),
+    "lg_timing_enable": (C.c_int, [_VP, _I32]),
+    "lg_kernel_time_ms": (C.c_int, [_VP, _I32, C.POINTER(C.c_double), C.POINTER(C.c_int64)]),
+    "lg_last_error": (C.c_char_p, []),
+    "lg_build_info": (C.c_char_p, []),
+    "lg_debug_timeout_code": (C.c_uint32, [_VP, C.POINTER(C.c_uint32)]),
+    "lg_debug_capture_layers": (C.c_int, [_VP, _VP, _SZ]),
+    "lg_padded_length": (_I32, [_I32, _I32]),
+}
+SP_PROTOTYPES = {  # include/superpoint_b200.h
+    "sp_weight_blob_floats": (_SZ, []),
+    "sp_create": (C.c_int, [C.POINTER(SpConfig), _VP, _SZ, _VP, _HANDLE_OUT]),
+    "sp_destroy": (C.c_int, [_VP]),
+    "sp_max_keypoints": (_I64, [_VP, _I32, _I32]),
+    "sp_workspace_bytes": (_SZ, [_VP, _I32, _I32, _I32]),
+    "sp_forward": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _I64] + [_VP] * 5 + [_SZ, _VP]),
+    "sp_backbone": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _VP, _VP, _VP, _SZ, _VP]),
+    "sp_tc_layout": (_I64, [_I32, _I32, _I32, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+}
+AL_PROTOTYPES = {  # include/aliked_b200.h
+    "al_weight_blob_floats": (_SZ, [C.POINTER(AlConfig)]),
+    "al_create": (C.c_int, [C.POINTER(AlConfig), _VP, _SZ, _VP, _HANDLE_OUT]),
+    "al_destroy": (C.c_int, [_VP]),
+    "al_max_keypoints": (_I64, [_VP, _I32, _I32]),
+    "al_workspace_bytes": (_SZ, [_VP, _I32, _I32, _I32]),
+    "al_forward": (C.c_int, [_VP, _VP, _VP, _I32, _I32, _I32, _I64] + [_VP] * 5 + [_SZ, _VP]),
+}
+SIFT_PROTOTYPES = {  # include/sift_b200.h
+    "sift_create": (C.c_int, [C.POINTER(SiftConfig), _VP, _HANDLE_OUT]),
+    "sift_destroy": (C.c_int, [_VP]),
+    "sift_max_keypoints": (_I64, [_VP, _I32, _I32]),
+    "sift_workspace_bytes": (_SZ, [_VP, _I32, _I32, _I32]),
+    "sift_forward": (C.c_int, [_VP, _VP, _I32, _VP, _I32, _I32, _I32, _I64] + [_VP] * 7 + [_SZ, _VP]),
+}
+EXPORTS, SP_EXPORTS, AL_EXPORTS, SIFT_EXPORTS = (
+    tuple(t) for t in (LG_PROTOTYPES, SP_PROTOTYPES, AL_PROTOTYPES, SIFT_PROTOTYPES))
+
 _lib = None
 
 
@@ -96,79 +134,10 @@ def load():
     if not os.path.exists(path):
         raise RuntimeError(f"{path} is missing: the CUDA library must be built (python -m lightglue_b200.build)")
     lib = C.CDLL(path)
-    lib.lg_weight_blob_floats.restype = C.c_size_t
-    lib.lg_weight_blob_floats.argtypes = [C.c_int32, C.c_int32, C.c_int32]
-    lib.lg_create.restype = C.c_int
-    lib.lg_create.argtypes = [C.POINTER(LgConfig), C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_void_p)]
-    lib.lg_destroy.restype = C.c_int
-    lib.lg_destroy.argtypes = [C.c_void_p]
-    lib.lg_workspace_bytes.restype = C.c_size_t
-    lib.lg_workspace_bytes.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32]
-    lib.lg_forward.restype = C.c_int
-    lib.lg_forward.argtypes = [C.c_void_p, C.POINTER(LgInputs), C.POINTER(LgOutputs), C.c_void_p, C.c_size_t, C.c_void_p]
-    lib.lg_assign.restype = C.c_int
-    lib.lg_assign.argtypes = [
-        C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(LgOutputs),
-        C.c_void_p, C.c_size_t, C.c_void_p,
-    ]
-    lib.lg_attention.restype = C.c_int
-    lib.lg_attention.argtypes = [C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p] * 8 + [C.c_void_p, C.c_size_t, C.c_void_p]
-    lib.sp_weight_blob_floats.restype = C.c_size_t
-    lib.sp_weight_blob_floats.argtypes = []
-    lib.sp_create.restype = C.c_int
-    lib.sp_create.argtypes = [C.POINTER(SpConfig), C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_void_p)]
-    lib.sp_destroy.restype = C.c_int
-    lib.sp_destroy.argtypes = [C.c_void_p]
-    lib.sp_max_keypoints.restype = C.c_int64
-    lib.sp_max_keypoints.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
-    lib.sp_workspace_bytes.restype = C.c_size_t
-    lib.sp_workspace_bytes.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32]
-    lib.sp_forward.restype = C.c_int
-    lib.sp_forward.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64] + [C.c_void_p] * 5 + [
-        C.c_size_t, C.c_void_p]
-    lib.sp_backbone.restype = C.c_int
-    lib.sp_backbone.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
-                                C.c_size_t, C.c_void_p]
-    lib.sp_tc_layout.restype = C.c_int64
-    lib.sp_tc_layout.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
-    lib.al_weight_blob_floats.restype = C.c_size_t
-    lib.al_weight_blob_floats.argtypes = [C.POINTER(AlConfig)]
-    lib.al_create.restype = C.c_int
-    lib.al_create.argtypes = [C.POINTER(AlConfig), C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_void_p)]
-    lib.al_destroy.restype = C.c_int
-    lib.al_destroy.argtypes = [C.c_void_p]
-    lib.al_max_keypoints.restype = C.c_int64
-    lib.al_max_keypoints.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
-    lib.al_workspace_bytes.restype = C.c_size_t
-    lib.al_workspace_bytes.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32]
-    lib.al_forward.restype = C.c_int
-    lib.al_forward.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64] + [
-        C.c_void_p] * 5 + [C.c_size_t, C.c_void_p]
-    lib.sift_create.restype = C.c_int
-    lib.sift_create.argtypes = [C.POINTER(SiftConfig), C.c_void_p, C.POINTER(C.c_void_p)]
-    lib.sift_destroy.restype = C.c_int
-    lib.sift_destroy.argtypes = [C.c_void_p]
-    lib.sift_max_keypoints.restype = C.c_int64
-    lib.sift_max_keypoints.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
-    lib.sift_workspace_bytes.restype = C.c_size_t
-    lib.sift_workspace_bytes.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32]
-    lib.sift_forward.restype = C.c_int
-    lib.sift_forward.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64] + [
-        C.c_void_p] * 6 + [C.c_void_p, C.c_size_t, C.c_void_p]
-    lib.lg_last_launch_count.restype = C.c_int64
-    lib.lg_last_launch_count.argtypes = [C.c_void_p]
-    lib.lg_timing_enable.restype = C.c_int
-    lib.lg_timing_enable.argtypes = [C.c_void_p, C.c_int32]
-    lib.lg_kernel_time_ms.restype = C.c_int
-    lib.lg_kernel_time_ms.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_double), C.POINTER(C.c_int64)]
-    lib.lg_last_error.restype = C.c_char_p
-    lib.lg_debug_timeout_code.restype = C.c_uint32
-    lib.lg_debug_timeout_code.argtypes = [C.c_void_p, C.POINTER(C.c_uint32)]
-    lib.lg_build_info.restype = C.c_char_p
-    lib.lg_debug_capture_layers.restype = C.c_int
-    lib.lg_debug_capture_layers.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
-    lib.lg_padded_length.restype = C.c_int32
-    lib.lg_padded_length.argtypes = [C.c_int32, C.c_int32]
+    for table in (LG_PROTOTYPES, SP_PROTOTYPES, AL_PROTOTYPES, SIFT_PROTOTYPES):
+        for name, (restype, argtypes) in table.items():
+            fn = getattr(lib, name)
+            fn.restype, fn.argtypes = restype, argtypes
     _lib = lib
     return lib
 

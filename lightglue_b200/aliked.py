@@ -4,7 +4,7 @@ The forward runs in CUDA (``csrc/al_api.cu``, fp32 on CUDA cores): padding, enco
 head, DKD and SDDH.  This module holds the parameters under the reference's names (an official ``{model_name}.pth``
 loads with ``strict=True``), passes them to the library as one blob, and does the host glue outside ``forward``'s
 math: gray -> RGB (``kornia.color.grayscale_to_rgb``: the channel repeated, on the device) and ``extract``'s resize
-(lightglue_b200/extractor.py, shared with ``SuperPoint``).  CUDA tensors only, no CPU path.
+(lightglue_b200/extractor.py, shared with the other extractors).  CUDA tensors only, no CPU path.
 
 Deviations from the reference, both in cases where its result is not well defined:
   * top-k mode (``detection_threshold <= 0``, ``max_num_keypoints = k > 0``) on an image with fewer than k NMS maxima:
@@ -17,7 +17,6 @@ Deviations from the reference, both in cases where its result is not well define
 """
 from __future__ import annotations
 
-import ctypes as C
 from types import SimpleNamespace
 
 import torch
@@ -49,7 +48,8 @@ def _block(ci, co, dcn, res):
     return m
 
 
-class ALIKED(nn.Module):
+class ALIKED(_extractor.CudaExtractor):
+    _abi = "al"
     default_conf = {
         "model_name": "aliked-n16",
         "max_num_keypoints": -1,
@@ -99,8 +99,6 @@ class ALIKED(nn.Module):
                 _extractor.find_checkpoint(f"{name}.pth", self.checkpoint_url.format(name), "ALIKED"), strict=True)
         self.requires_grad_(False)
         self.eval()
-        self._handle = None  # (C handle, signature)
-        self._ws = {}
 
     # ------------------------------------------------------------------ C handle
     def _config(self) -> _cabi.AlConfig:
@@ -114,34 +112,9 @@ class ALIKED(nn.Module):
                  if not k.endswith("num_batches_tracked")]
         return torch.cat(parts).contiguous()
 
-    def _get_handle(self, device: torch.device):
-        lib = _cabi.load()
-        tensors = list(self.parameters()) + list(self.buffers())
-        sig = (device.index, tuple(int(t._version) for t in tensors), tuple(t.data_ptr() for t in tensors),
-               self.conf.model_name, self.conf.nms_radius, self.conf.max_num_keypoints, self.conf.detection_threshold)
-        if self._handle is not None and self._handle[1] == sig:
-            return self._handle[0]
-        self._release()
-        cfg = self._config()
-        blob = self._blob().to(device)
-        assert blob.numel() == lib.al_weight_blob_floats(C.byref(cfg))
-        h = C.c_void_p()
-        stream = torch.cuda.current_stream(device).cuda_stream
-        _cabi.check(lib.al_create(C.byref(cfg), blob.data_ptr(), blob.numel(), stream, C.byref(h)), "al_create")
-        torch.cuda.current_stream(device).synchronize()  # the blob may be freed once the copy has run
-        self._handle = (h, sig)
-        return h
-
-    def _release(self):
-        try:
-            if getattr(self, "_handle", None) is not None:  # (the constructor may have raised before the attribute exists)
-                _cabi.load().al_destroy(self._handle[0])
-                object.__setattr__(self, "_handle", None)
-        except Exception:  # noqa: BLE001  (interpreter shutdown: modules may already be torn down)
-            pass
-
-    def __del__(self):
-        self._release()
+    def _create(self, lib, cfg, blob, stream, out):
+        assert blob.numel() == lib.al_weight_blob_floats(cfg)
+        _cabi.check(lib.al_create(cfg, blob.data_ptr(), blob.numel(), stream, out), "al_create")
 
     # ------------------------------------------------------------------ forward
     @torch.no_grad()
@@ -149,52 +122,21 @@ class ALIKED(nn.Module):
         """Keypoints (pixels), descriptors and keypoint_scores of an image batch [B, 1 or 3, H, W], H, W >= 8."""
         for key in self.required_data_keys:
             assert key in data, f"Missing key {key} in data"
-        image = data["image"]
-        if image.device.type != "cuda":
-            raise RuntimeError("lightglue_b200.ALIKED runs on CUDA (sm_90a) tensors only; there is no CPU path")
+        image = self._cuda_image(data["image"])
         if image.shape[1] == 1:  # kornia.color.grayscale_to_rgb
             image = image.expand(-1, 3, -1, -1)
         b, c, hh, ww = image.shape
         assert c == 3
         if hh < 8 or ww < 8:
             raise ValueError(f"image size {ww}x{hh}: height and width must be at least 8")
-        device = image.device
         image = image.detach().to(torch.float32).contiguous()
         size = data.get("image_size")
         if size is not None:
-            size = torch.as_tensor(size).to(device=device, dtype=torch.float32).reshape(b, 2).contiguous()
-        with torch.cuda.device(device):
-            lib = _cabi.load()
-            handle = self._get_handle(device)
-            cap = int(lib.al_max_keypoints(handle, hh, ww))
-            key = (device.index, b, hh, ww)
-            ws = self._ws.get(key)
-            if ws is None:
-                self._ws.clear()
-                ws = self._ws[key] = torch.empty(int(lib.al_workspace_bytes(handle, b, hh, ww)), dtype=torch.uint8, device=device)
-            dim = self.cfgs[self.conf.model_name][4]
-            kpts = torch.empty(b, cap, 2, dtype=torch.float32, device=device)
-            scores = torch.empty(b, cap, dtype=torch.float32, device=device)
-            desc = torch.empty(b, cap, dim, dtype=torch.float32, device=device)
-            counts = torch.empty(b, dtype=torch.int32, device=device)
-            stream = torch.cuda.current_stream(device).cuda_stream
-            _cabi.check(
-                lib.al_forward(handle, image.data_ptr(), size.data_ptr() if size is not None else None, b, hh, ww, cap,
-                               kpts.data_ptr(), scores.data_ptr(), desc.data_ptr(), counts.data_ptr(), ws.data_ptr(),
-                               ws.numel(), stream),
-                "al_forward",
-            )
-            n = counts.cpu().tolist()  # the one host read-back: keypoint counts
-        if len(set(n)) != 1:  # the reference stacks the per-image results, which needs equal counts
-            raise ValueError(f"images of the batch have different keypoint counts {n}; set max_num_keypoints or batch 1")
-        k = n[0]
-        return {
-            "keypoints": kpts[:, :k].contiguous(),
-            "descriptors": desc[:, :k].contiguous(),
-            "keypoint_scores": scores[:, :k].contiguous(),
-        }
+            size = torch.as_tensor(size).to(device=image.device, dtype=torch.float32).reshape(b, 2).contiguous()
 
-    @torch.no_grad()
-    def extract(self, img: torch.Tensor, **conf) -> dict:
-        """``Extractor.extract``: resize, ``forward``, keypoints back in the original pixels (lightglue_b200/extractor.py)."""
-        return _extractor.extract(self, img, **conf)
+        def call(lib, handle, cap, p, tail):
+            return lib.al_forward(handle, image.data_ptr(), size.data_ptr() if size is not None else None, b, hh, ww, cap,
+                                  p["keypoints"], p["keypoint_scores"], p["descriptors"], *tail)
+
+        dim = self.cfgs[self.conf.model_name][4]
+        return self._run(image, {"keypoints": (2,), "descriptors": (dim,), "keypoint_scores": ()}, call)

@@ -7,6 +7,7 @@ resulting .so travels to the GPU box with the repo snapshot.
 from __future__ import annotations
 
 import fcntl
+import glob
 import os
 import subprocess
 
@@ -20,10 +21,7 @@ def _stale() -> bool:
         return True
     t = os.path.getmtime(LIB)
     srcs = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cu", ".h", ".cuh")) or f == "Makefile"]
-    srcs.append(os.path.join(os.path.dirname(HERE), "include", "lightglue_b200.h"))
-    srcs.append(os.path.join(os.path.dirname(HERE), "include", "superpoint_b200.h"))
-    srcs.append(os.path.join(os.path.dirname(HERE), "include", "aliked_b200.h"))
-    srcs.append(os.path.join(os.path.dirname(HERE), "include", "sift_b200.h"))
+    srcs += glob.glob(os.path.join(os.path.dirname(HERE), "include", "*.h"))
     return any(os.path.getmtime(s) > t for s in srcs)
 
 

@@ -566,24 +566,6 @@ __global__ void __launch_bounds__(128) al_sddh_kernel(Sddh s, const int* __restr
   if (t < dim) dd[t] = d / fmaxf(sqrtf(tot), 1e-12f);
 }
 
-// executor of the sp_pipeline.h functors (one thread per logical index)
-template <class F>
-__global__ void __launch_bounds__(256) al_for_each_kernel(F f, long n) {
-  const long i = blockIdx.x * (long)blockDim.x + threadIdx.x;
-  if (i < n) f(i);
-}
-struct CudaExec {
-  cudaStream_t stream;
-  template <class F>
-  int run(const F& f) {
-    const long n = f.count();
-    if (n <= 0) return 0;
-    al_for_each_kernel<F><<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(f, n);
-    LG_CHECK_LAUNCH();
-    return 0;
-  }
-};
-
 unsigned blocks(long n, int t) { return (unsigned)((n + t - 1) / t); }
 
 struct Geo {
@@ -606,51 +588,45 @@ struct Ws {
   size_t bytes;
 };
 void carve(char* base, const AlConfig& c, int B, int H, int W, long cap, Ws* w) {
-  size_t o = 0;
-  auto take = [&](size_t n) { o = (o + 255) & ~(size_t)255; char* p = base ? base + o : nullptr; o += n * 4; return p; };
+  WsBump bp{base, 0};
+  auto take = [&](size_t n) { return bp.take<float>(n); };
   const Geo g = geometry(H, W);
   const size_t P0 = (size_t)B * g.Hp * g.Wp, P1 = P0 / 4, P2 = P0 / 64, P3 = P0 / 1024, PX = (size_t)B * H * W;
   const int q = c.dim / 4;
-  w->img = (float*)take(3 * P0);
-  w->ta = (float*)take((size_t)(c.c1 > 8 ? c.c1 : 8) * P0);
-  w->x1 = (float*)take((size_t)c.c1 * P0);
-  w->s1 = (float*)take(8 * P0);
-  w->invn = (float*)take(P0);
-  w->p1 = (float*)take(c.c1 * P1); w->t2 = (float*)take(c.c2 * P1); w->d2 = (float*)take(c.c2 * P1);
-  w->x2 = (float*)take(c.c2 * P1); w->a2 = (float*)take(q * P1);
-  w->p2 = (float*)take(c.c2 * P2); w->o3 = (float*)take(18 * P2); w->t3 = (float*)take(c.c3 * P2);
-  w->d3 = (float*)take(c.c3 * P2); w->x3 = (float*)take(c.c3 * P2); w->a3 = (float*)take(q * P2);
-  w->p3 = (float*)take(c.c3 * P3); w->o4 = (float*)take(18 * P3); w->t4 = (float*)take(c.c4 * P3);
-  w->d4 = (float*)take(c.c4 * P3); w->x4 = (float*)take(c.c4 * P3); w->a4 = (float*)take(q * P3);
-  w->score = (float*)take(PX); w->nms = (float*)take(PX);
-  w->n1 = (float*)take(PX); w->n2 = (float*)take(PX); w->n3 = (float*)take(PX);
-  w->kpn = (float*)take((size_t)B * cap * 2);
-  w->mean = (float*)take(B);
-  w->cnt = (int*)take(B);
+  w->img = take(3 * P0);
+  w->ta = take((size_t)(c.c1 > 8 ? c.c1 : 8) * P0);
+  w->x1 = take((size_t)c.c1 * P0);
+  w->s1 = take(8 * P0);
+  w->invn = take(P0);
+  w->p1 = take(c.c1 * P1); w->t2 = take(c.c2 * P1); w->d2 = take(c.c2 * P1);
+  w->x2 = take(c.c2 * P1); w->a2 = take(q * P1);
+  w->p2 = take(c.c2 * P2); w->o3 = take(18 * P2); w->t3 = take(c.c3 * P2);
+  w->d3 = take(c.c3 * P2); w->x3 = take(c.c3 * P2); w->a3 = take(q * P2);
+  w->p3 = take(c.c3 * P3); w->o4 = take(18 * P3); w->t4 = take(c.c4 * P3);
+  w->d4 = take(c.c4 * P3); w->x4 = take(c.c4 * P3); w->a4 = take(q * P3);
+  w->score = take(PX); w->nms = take(PX);
+  w->n1 = take(PX); w->n2 = take(PX); w->n3 = take(PX);
+  w->kpn = take((size_t)B * cap * 2);
+  w->mean = take(B);
+  w->cnt = bp.take<int>(B);
   SpWorkspace& s = w->sp;
   s = SpWorkspace{};
   s.t0 = w->nms;
-  s.cand_score = (float*)take(PX);
-  s.cand_pos = (int*)take(PX);
-  s.sel_score = (float*)take((size_t)B * cap);
-  s.sel_pos = (int*)take((size_t)B * cap);
-  s.row_count = (int*)take((size_t)B * H);
-  s.row_start = (int*)take((size_t)B * H);
-  s.n_cand = (int*)take(B);
-  s.n_sel = (int*)take(B);
-  w->bytes = (o + 255) & ~(size_t)255;
+  s.cand_score = take(PX);
+  s.cand_pos = bp.take<int>(PX);
+  s.sel_score = take((size_t)B * cap);
+  s.sel_pos = bp.take<int>((size_t)B * cap);
+  s.row_count = bp.take<int>((size_t)B * H);
+  s.row_start = bp.take<int>((size_t)B * H);
+  s.n_cand = bp.take<int>(B);
+  s.n_sel = bp.take<int>(B);
+  w->bytes = bp.bytes();
 }
 
 int64_t max_keypoints(const AlConfig& c, int H, int W) {
   const int64_t k = c.max_num_keypoints > 0 ? c.max_num_keypoints : AL_N_LIMIT_MAX;
   return k < (int64_t)H * W ? k : (int64_t)H * W;
 }
-
-#define AL_LAUNCH()                                                   \
-  do {                                                                    \
-    cudaError_t e_ = cudaGetLastError();                                  \
-    if (e_ != cudaSuccess) return lg_set_cuda_error(e_, __FILE__, __LINE__); \
-  } while (0)
 
 }  // namespace
 
@@ -671,20 +647,23 @@ extern "C" int al_create(const AlConfig* cfg, const float* weights_dev, size_t n
   if (n_floats != L.total) return lg_set_error("al_create: weight blob has the wrong size");
   cudaStream_t stream = (cudaStream_t)stream_;
   AlHandle* h = new AlHandle{*cfg, L, nullptr, nullptr};
-  cudaError_t e = cudaMalloc(&h->wts, (L.total + L.fold_total) * sizeof(float));
-  if (e != cudaSuccess) { delete h; return lg_set_cuda_error(e, __FILE__, __LINE__); }
+  struct Guard {  // every failure path below releases the handle and what it owns
+    AlHandle* h;
+    ~Guard() { if (h) al_destroy(h); }
+  } guard{h};
+  LG_CU(cudaMalloc(&h->wts, (L.total + L.fold_total) * sizeof(float)));
   h->fold = h->wts + L.total;
-  e = cudaMemcpyAsync(h->wts, weights_dev, L.total * sizeof(float), cudaMemcpyDeviceToDevice, stream);
-  for (int b = 0; b < 4 && e == cudaSuccess; ++b)
+  LG_CU(cudaMemcpyAsync(h->wts, weights_dev, L.total * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+  for (int b = 0; b < 4; ++b)
     for (int cv = 0; cv < 2; ++cv) {
       const BlockIdx& k = L.blk[b];
       const int ci = cv == 0 ? k.cin : k.cout, per = ci * 9;
       al_fold_bn_kernel<<<blocks((long)k.cout * per, 256), 256, 0, stream>>>(
           h->wts + (cv == 0 ? k.w1 : k.w2), h->wts + (cv == 0 ? k.bn1 : k.bn2), h->fold + L.fold_w[2 * b + cv],
           h->fold + L.fold_b[2 * b + cv], k.cout, per);
-      e = cudaGetLastError();
+      LG_CHECK_LAUNCH();
     }
-  if (e != cudaSuccess) { cudaFree(h->wts); delete h; return lg_set_cuda_error(e, __FILE__, __LINE__); }
+  guard.h = nullptr;
   *out = h;
   return 0;
 }
@@ -773,54 +752,36 @@ extern "C" int al_forward(AlHandle* h, const float* image, const float* image_si
   conv(s2, wb + L.head[T_SH4], nullptr, nullptr, s3, 4, 4, g.Hp, g.Wp, 3, ACT_SELU, 0.f);
   conv(s3, wb + L.head[T_SH6], nullptr, nullptr, w.img, 4, 1, g.Hp, g.Wp, 3, ACT_SIGMOID, 0.f);
   al_crop_kernel<<<blocks((long)B * H * W, 256), 256, 0, st>>>(w.img, w.score, B, H, W, g.Hp, g.Wp, g.top, g.left);
-  AL_LAUNCH();
+  LG_CHECK_LAUNCH();
 
-  // ---- DKD: simple_nms with SuperPoint's functors (window maxima of radius r along x then y)
-  CudaExec ex{st};
+  // ---- DKD: simple_nms with SuperPoint's functors; cand_score is scratch until the compaction
+  SpCudaExec ex{st};
   const long n = (long)B * H * W;
   const int r = c.nms_radius;
-  int rc;
-  auto wmax = [&](const float* in, float* out) {
-    SpWindowMax a{in, w.n3, B, H, W, r, 0};
-    int e = ex.run(a);
-    if (e) return e;
-    SpWindowMax bb{w.n3, out, B, H, W, r, 1};
-    return ex.run(bb);
-  };
-  float *mask = w.n1, *tmp = w.n2, *mp = w.sp.cand_score;  // cand_score is scratch until the compaction
-  if ((rc = wmax(w.score, tmp))) return rc;
-  { SpNmsStep s{w.score, tmp, nullptr, mask, n, 0}; if ((rc = ex.run(s))) return rc; }
-  for (int it = 0; it < 2; ++it) {
-    if ((rc = wmax(mask, tmp))) return rc;                                                      // max_pool(max_mask)
-    { SpNmsStep s{w.score, tmp, nullptr, w.nms, n, 1}; if ((rc = ex.run(s))) return rc; }       // supp_scores
-    if ((rc = wmax(w.nms, mp))) return rc;                                                      // max_pool(supp_scores)
-    { SpNmsStep s{w.nms, mp, tmp, mask, n, 2}; if ((rc = ex.run(s))) return rc; }
-  }
-  { SpNmsStep s{w.score, mask, nullptr, w.nms, n, 3}; if ((rc = ex.run(s))) return rc; }       // nms scores
+  LG_RC(sp_simple_nms(ex, w.score, w.nms, B, H, W, r, w.n2, w.n1, w.nms, w.sp.cand_score, w.n3));
   al_borders_kernel<<<blocks(n, 256), 256, 0, st>>>(w.nms, image_size, B, H, W, r);
   const SpCudaStages stages{st};
   const long pcap = (long)H * W;
   if (topk) {
-    if ((rc = stages.compact(ex, w.sp, B, H, W, 0.f, pcap))) return rc;  // the positive NMS maxima
-    if ((rc = stages.select(ex, w.sp, B, c.max_num_keypoints, pcap, cap, 1))) return rc;
+    LG_RC(stages.compact(ex, w.sp, B, H, W, 0.f, pcap));  // the positive NMS maxima
+    LG_RC(stages.select(ex, w.sp, B, c.max_num_keypoints, pcap, cap, 1));
     al_fill_topk_kernel<<<blocks(B, 32), 32, 0, st>>>(w.nms, w.sp.sel_pos, w.sp.sel_score, w.sp.n_sel, B, pcap,
                                                       c.max_num_keypoints, cap);
   } else {
     al_stats_kernel<<<B, 512, 0, st>>>(w.nms, w.score, w.cnt, w.mean, pcap, c.detection_threshold);
     al_mask_kernel<<<blocks(n, 256), 256, 0, st>>>(w.nms, w.cnt, w.mean, B, pcap, c.detection_threshold);
     const int n_limit = c.max_num_keypoints > 0 ? c.max_num_keypoints : AL_N_LIMIT_MAX;
-    if ((rc = stages.compact(ex, w.sp, B, H, W, 0.f, pcap))) return rc;
-    if ((rc = stages.select(ex, w.sp, B, n_limit, pcap, cap, 0))) return rc;
+    LG_RC(stages.compact(ex, w.sp, B, H, W, 0.f, pcap));
+    LG_RC(stages.select(ex, w.sp, B, n_limit, pcap, cap, 0));
   }
-  AL_LAUNCH();
+  LG_CHECK_LAUNCH();
   al_refine_kernel<<<blocks((long)B * cap, 128), 128, 0, st>>>(w.score, w.sp.n_sel, w.sp.sel_pos, w.kpn, keypoints, scores, B, H,
                                                                W, r, cap);
   // ---- SDDH
   const Sddh sd{f, w.invn, wb + L.head[T_SOC0W], wb + L.head[T_SOC0B], wb + L.head[T_SOC2W], wb + L.head[T_SOC2B],
                 wb + L.head[T_SFW], wb + L.head[T_AGG], c.dim, c.M, H, W, g.top, g.left};
   if (cap > 0) al_sddh_kernel<<<dim3((unsigned)cap, B), 128, 0, st>>>(sd, w.sp.n_sel, w.kpn, descriptors, cap);
-  AL_LAUNCH();
-  cudaError_t e = cudaMemcpyAsync(counts, w.sp.n_sel, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToDevice, st);
-  if (e != cudaSuccess) return lg_set_cuda_error(e, __FILE__, __LINE__);
+  LG_CHECK_LAUNCH();
+  LG_CU(cudaMemcpyAsync(counts, w.sp.n_sel, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
   return 0;
 }

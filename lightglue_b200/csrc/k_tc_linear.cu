@@ -679,26 +679,21 @@ void tc_engine_destroy(TcEngine* e) {
   *e = TcEngine{};
 }
 
-void tc_carve(size_t* off, char* base, size_t S, int Lp, const LgHandle* h, TcBuffers* b) {
+void tc_carve(WsBump& w, size_t S, int Lp, const LgHandle* h, TcBuffers* b) {
   const size_t R = S * Lp;
   const bool x3 = h->cfg.precision == LG_PREC_BF16X3;
-  auto take = [&](size_t bytes) -> void* {
-    *off = (*off + 1023) & ~(size_t)1023;
-    void* p = base ? base + *off : nullptr;
-    *off += bytes;
-    return p;
-  };
-  b->xh = (__nv_bfloat16*)take(R * 256 * 2);
-  b->xl = x3 ? (__nv_bfloat16*)take(R * 256 * 2) : nullptr;
-  b->ctxh = (__nv_bfloat16*)take(R * 256 * 2);
-  b->ctxl = x3 ? (__nv_bfloat16*)take(R * 256 * 2) : nullptr;
-  b->msgh = (__nv_bfloat16*)take(R * 256 * 2);
-  b->msgl = x3 ? (__nv_bfloat16*)take(R * 256 * 2) : nullptr;
-  b->hh = (__nv_bfloat16*)take(R * 512 * 2);
-  b->hl = x3 ? (__nv_bfloat16*)take(R * 512 * 2) : nullptr;
-  b->q = (__half*)take(R * 256 * 2);
-  b->k = (__half*)take(R * 256 * 2);
-  b->vt = (__half*)take(R * 256 * 2);
+  constexpr size_t A = 1024;  // every buffer on a 1024-byte boundary
+  b->xh = w.take<__nv_bfloat16>(R * 256, A);
+  b->xl = x3 ? w.take<__nv_bfloat16>(R * 256, A) : nullptr;
+  b->ctxh = w.take<__nv_bfloat16>(R * 256, A);
+  b->ctxl = x3 ? w.take<__nv_bfloat16>(R * 256, A) : nullptr;
+  b->msgh = w.take<__nv_bfloat16>(R * 256, A);
+  b->msgl = x3 ? w.take<__nv_bfloat16>(R * 256, A) : nullptr;
+  b->hh = w.take<__nv_bfloat16>(R * 512, A);
+  b->hl = x3 ? w.take<__nv_bfloat16>(R * 512, A) : nullptr;
+  b->q = w.take<__half>(R * 256, A);
+  b->k = w.take<__half>(R * 256, A);
+  b->vt = w.take<__half>(R * 256, A);
 }
 
 int tc_refresh_shadow(LgHandle* h, const TcBuffers& b, const float* x, const SeqState& st, cudaStream_t stream) {

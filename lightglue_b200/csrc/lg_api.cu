@@ -24,16 +24,6 @@ int lg_set_cuda_error(cudaError_t e, const char* file, int line) {
   snprintf(g_err, sizeof(g_err), "CUDA error %d (%s) at %s:%d", (int)e, cudaGetErrorString(e), file, line);
   return 2;
 }
-#define CU(x)                                                      \
-  do {                                                             \
-    cudaError_t e__ = (x);                                         \
-    if (e__ != cudaSuccess) return lg_set_cuda_error(e__, __FILE__, __LINE__); \
-  } while (0)
-#define RC(x)            \
-  do {                   \
-    int r__ = (x);       \
-    if (r__) return r__; \
-  } while (0)
 
 extern "C" const char* lg_last_error(void) { return g_err; }
 
@@ -49,13 +39,11 @@ std::map<int, int> g_sms;
 }  // namespace
 int lg_func_smem_once(const void* func, int bytes) {
   int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
-  if (e != cudaSuccess) return lg_set_cuda_error(e, __FILE__, __LINE__);
+  LG_CU(cudaGetDevice(&dev));
   std::lock_guard<std::mutex> lk(g_dev_mu);
   auto it = g_smem_done.find({dev, func});
   if (it != g_smem_done.end() && it->second >= bytes) return 0;
-  e = cudaFuncSetAttribute(func, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  if (e != cudaSuccess) return lg_set_cuda_error(e, __FILE__, __LINE__);
+  LG_CU(cudaFuncSetAttribute(func, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
   g_smem_done[{dev, func}] = bytes;
   return 0;
 }
@@ -147,7 +135,7 @@ extern "C" int lg_create(const LgConfig* cfg, const float* blob, size_t n_floats
   h->timing = false;
   h->dbg_layers = nullptr; h->dbg_layers_floats = 0;
   for (int i = 0; i < LG_K_CLASSES; ++i) h->ev_used[i] = 0;
-  CU(cudaGetDevice(&h->device));
+  LG_CU(cudaGetDevice(&h->device));
   const int L = cfg->n_layers;
   h->bself = block_off(3 * D);
   h->bcross = block_off(2 * D);
@@ -161,64 +149,64 @@ extern "C" int lg_create(const LgConfig* cfg, const float* blob, size_t n_floats
   h->o_assign = c; c += (size_t)L * ASSIGN_BLOB_PAD;
   h->o_token = c; c += (size_t)L * TOKEN_BLOB_PAD;
   h->wpk_floats = c;
-  CU(cudaMalloc(&h->wpk, c * sizeof(float)));
-  CU(cudaMemsetAsync(h->wpk, 0, c * sizeof(float), stream));
+  LG_CU(cudaMalloc(&h->wpk, c * sizeof(float)));
+  LG_CU(cudaMemsetAsync(h->wpk, 0, c * sizeof(float), stream));
   auto cp = [&](size_t dst, const float* src, size_t n) {
     return cudaMemcpyAsync(h->wpk + dst, src, n * sizeof(float), cudaMemcpyDeviceToDevice, stream);
   };
   const float* p = blob;
-  CU(cp(h->o_wr, p, 32 * (size_t)cfg->pos_dim)); p += 32 * (size_t)cfg->pos_dim;
+  LG_CU(cp(h->o_wr, p, 32 * (size_t)cfg->pos_dim)); p += 32 * (size_t)cfg->pos_dim;
   if (cfg->input_dim != (int)D) {
-    CU(cp(h->o_inw, p, D * (size_t)cfg->input_dim)); p += D * (size_t)cfg->input_dim;
-    CU(cp(h->o_inb, p, D)); p += D;
+    LG_CU(cp(h->o_inw, p, D * (size_t)cfg->input_dim)); p += D * (size_t)cfg->input_dim;
+    LG_CU(cp(h->o_inb, p, D)); p += D;
   }
   for (int l = 0; l < L; ++l) {
     float* base = h->wpk + h->o_layers + (size_t)l * h->layer_stride;
     // self block
     permute_qkv_kernel<<<768, 128, 0, stream>>>(p, p + 3 * D * D, base + h->bself.wp, base + h->bself.bp);
-    CU(cudaGetLastError());
+    LG_CU(cudaGetLastError());
     p += 3 * D * D + 3 * D;
     size_t bo = h->o_layers + (size_t)l * h->layer_stride;
-    CU(cp(bo + h->bself.wo, p, D * D)); p += D * D;
-    CU(cp(bo + h->bself.bo, p, D)); p += D;
-    CU(cp(bo + h->bself.w1, p, F * F)); p += F * F;
-    CU(cp(bo + h->bself.b1, p, F)); p += F;
-    CU(cp(bo + h->bself.g, p, F)); p += F;
-    CU(cp(bo + h->bself.be, p, F)); p += F;
-    CU(cp(bo + h->bself.w2, p, D * F)); p += D * F;
-    CU(cp(bo + h->bself.b2, p, D)); p += D;
+    LG_CU(cp(bo + h->bself.wo, p, D * D)); p += D * D;
+    LG_CU(cp(bo + h->bself.bo, p, D)); p += D;
+    LG_CU(cp(bo + h->bself.w1, p, F * F)); p += F * F;
+    LG_CU(cp(bo + h->bself.b1, p, F)); p += F;
+    LG_CU(cp(bo + h->bself.g, p, F)); p += F;
+    LG_CU(cp(bo + h->bself.be, p, F)); p += F;
+    LG_CU(cp(bo + h->bself.w2, p, D * F)); p += D * F;
+    LG_CU(cp(bo + h->bself.b2, p, D)); p += D;
     // cross block: [to_qk ; to_v] stacked into one [512, 256] projection
     bo += h->bself.total;
-    CU(cp(bo + h->bcross.wp, p, D * D)); p += D * D;
-    CU(cp(bo + h->bcross.bp, p, D)); p += D;
-    CU(cp(bo + h->bcross.wp + D * D, p, D * D)); p += D * D;
-    CU(cp(bo + h->bcross.bp + D, p, D)); p += D;
-    CU(cp(bo + h->bcross.wo, p, D * D)); p += D * D;
-    CU(cp(bo + h->bcross.bo, p, D)); p += D;
-    CU(cp(bo + h->bcross.w1, p, F * F)); p += F * F;
-    CU(cp(bo + h->bcross.b1, p, F)); p += F;
-    CU(cp(bo + h->bcross.g, p, F)); p += F;
-    CU(cp(bo + h->bcross.be, p, F)); p += F;
-    CU(cp(bo + h->bcross.w2, p, D * F)); p += D * F;
-    CU(cp(bo + h->bcross.b2, p, D)); p += D;
+    LG_CU(cp(bo + h->bcross.wp, p, D * D)); p += D * D;
+    LG_CU(cp(bo + h->bcross.bp, p, D)); p += D;
+    LG_CU(cp(bo + h->bcross.wp + D * D, p, D * D)); p += D * D;
+    LG_CU(cp(bo + h->bcross.bp + D, p, D)); p += D;
+    LG_CU(cp(bo + h->bcross.wo, p, D * D)); p += D * D;
+    LG_CU(cp(bo + h->bcross.bo, p, D)); p += D;
+    LG_CU(cp(bo + h->bcross.w1, p, F * F)); p += F * F;
+    LG_CU(cp(bo + h->bcross.b1, p, F)); p += F;
+    LG_CU(cp(bo + h->bcross.g, p, F)); p += F;
+    LG_CU(cp(bo + h->bcross.be, p, F)); p += F;
+    LG_CU(cp(bo + h->bcross.w2, p, D * F)); p += D * F;
+    LG_CU(cp(bo + h->bcross.b2, p, D)); p += D;
     for (int blk = 0; blk < 2; ++blk) {
       const BlockOff& o = blk == 0 ? h->bself : h->bcross;
       float* bw = base + (blk == 0 ? 0 : h->bself.total);
       fold_out_proj_kernel<<<(unsigned)F, 256, 0, stream>>>(bw + o.w1, bw + o.b1, bw + o.wo, bw + o.bo, bw + o.w1f, bw + o.b1f);
-      CU(cudaGetLastError());
+      LG_CU(cudaGetLastError());
     }
   }
   for (int l = 0; l < L; ++l) {  // packed: final_proj.w [256,256] | final_proj.b [256] | matchability.w [256] | .b [1] (+pad)
     const size_t dst = h->o_assign + (size_t)l * ASSIGN_BLOB_PAD;
-    CU(cp(dst + AO_MW, p, D)); p += D;
-    CU(cp(dst + AO_MB, p, 1)); p += 1;
-    CU(cp(dst + AO_FW, p, D * D)); p += D * D;
-    CU(cp(dst + AO_FB, p, D)); p += D;
+    LG_CU(cp(dst + AO_MW, p, D)); p += D;
+    LG_CU(cp(dst + AO_MB, p, 1)); p += 1;
+    LG_CU(cp(dst + AO_FW, p, D * D)); p += D * D;
+    LG_CU(cp(dst + AO_FB, p, D)); p += D;
   }
   for (int l = 0; l < L - 1; ++l) {
     const size_t dst = h->o_token + (size_t)l * TOKEN_BLOB_PAD;
-    CU(cp(dst, p, D)); p += D;
-    CU(cp(dst + D, p, 1)); p += 1;
+    LG_CU(cp(dst, p, D)); p += D;
+    LG_CU(cp(dst + D, p, 1)); p += 1;
   }
   if ((size_t)(p - blob) != n_floats) return lg_set_error("lg_create: internal blob walk mismatch");
   for (int i = 0; i < L; ++i) {
@@ -271,9 +259,9 @@ extern "C" int lg_kernel_time_ms(LgHandle* h, int32_t kc, double* ms, int64_t* l
   if (!h || kc < 0 || kc >= LG_K_CLASSES) return lg_set_error("lg_kernel_time_ms: bad argument");
   double tot = 0;
   for (size_t i = 0; i + 1 < h->ev_used[kc]; i += 2) {
-    CU(cudaEventSynchronize(h->ev[kc][i + 1]));
+    LG_CU(cudaEventSynchronize(h->ev[kc][i + 1]));
     float t = 0;
-    CU(cudaEventElapsedTime(&t, h->ev[kc][i], h->ev[kc][i + 1]));
+    LG_CU(cudaEventElapsedTime(&t, h->ev[kc][i], h->ev[kc][i + 1]));
     tot += t;
   }
   if (ms) *ms = tot;
@@ -286,16 +274,6 @@ namespace {
 // ---------------------------------------------------------------------------------------------
 // workspace
 // ---------------------------------------------------------------------------------------------
-struct Bump {
-  char* base; size_t off;
-  template <typename T> T* take(size_t n) {
-    off = (off + 255) & ~(size_t)255;
-    T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
-    off += n * sizeof(T);
-    return p;
-  }
-};
-
 struct Workspace {
   int Lp, nt;
   float *xa, *xb, *csa, *csb, *q, *k, *v, *ctx, *msg, *hbuf, *z, *term;
@@ -311,7 +289,7 @@ struct Workspace {
 int round_up(int x, int m) { return (x + m - 1) / m * m; }
 
 void carve(const LgHandle* h, int B, int M, int N, char* base, Workspace* w) {
-  Bump b{base, 0};
+  WsBump b{base, 0};
   const int mx = M > N ? M : N;
   const int Lp = round_up(mx > 0 ? mx : 1, LG_TILE);
   const size_t S = 2 * (size_t)B, R = S * Lp;
@@ -335,7 +313,7 @@ void carve(const LgHandle* h, int B, int M, int N, char* base, Workspace* w) {
     w->q = w->k = w->v = w->msg = nullptr;
     w->ctx = b.take<float>(R * D);   // projected descriptors for the assignment sweeps (fp32)
     w->hbuf = b.take<float>(R * (size_t)(h->cfg.input_dim > (int)D ? h->cfg.input_dim : (int)D));
-    tc_carve(&b.off, base, S, Lp, h, &w->tc);
+    tc_carve(b, S, Lp, h, &w->tc);
   }
   w->z = b.take<float>(R);
   w->term = b.take<float>(R);
@@ -367,7 +345,7 @@ void carve(const LgHandle* h, int B, int M, int N, char* base, Workspace* w) {
   w->pos = b.take<int>(R);
   w->did_prune = b.take<int>(S);
   w->keep = b.take<unsigned char>(R);
-  w->bytes = (b.off + 255) & ~(size_t)255;
+  w->bytes = b.bytes();
 }
 
 __global__ void fill_empty_kernel(int64_t* m0, int64_t* m1, float* s0, float* s1, int* stop, int* p0, int* p1, int* nm,
@@ -401,9 +379,9 @@ static int run_assign(LgHandle* h, const Workspace& w, const SeqState& st, const
       g.w_sel_stride = ASSIGN_BLOB_PAD; g.b_sel_stride = ASSIGN_BLOB_PAD;
       g.K = D; g.Nout = D; g.epi = EPI_STORE; g.scale = 0.25f;  // / 256^(1/4) (lightglue.py:291)
       g.out = w.ctx; g.ldo = D;
-      RC(simt_gemm(g, st, stream));
+      LG_RC(simt_gemm(g, st, stream));
     } else {
-      RC(tc_final_proj(h, w.tc, st, w.ctx, stream));
+      LG_RC(tc_final_proj(h, w.tc, st, w.ctx, stream));
     }
     h->launches += 1;
   }
@@ -422,9 +400,9 @@ static int run_assign(LgHandle* h, const Workspace& w, const SeqState& st, const
     Timer t(h, out->log_assignment ? LG_K_OTHER : LG_K_ASSIGN, stream);
     if (h->cfg.precision != LG_PREC_FP32 && st.Lp >= 256) {
       // both similarity sweeps on the tensor cores; the N x M matrix reaches HBM only if the caller asked for it
-      RC(tc_assign_sweeps(h, w.tc, st, a, w.tc_part, w.tc_parg, w.term, stream));
+      LG_RC(tc_assign_sweeps(h, w.tc, st, a, w.tc_part, w.tc_parg, w.term, stream));
     } else {
-      RC(misc_assign(a, st, stream, &h->launches));
+      LG_RC(misc_assign(a, st, stream, &h->launches));
     }
   }
   return 0;
@@ -458,11 +436,11 @@ extern "C" int lg_forward(LgHandle* h, const LgInputs* in, const LgOutputs* out,
     fill_empty_kernel<<<(unsigned)((mx + 255) / 256), 256, 0, stream>>>(out->matches0, out->matches1, out->matching_scores0,
                                                                        out->matching_scores1, out->stop, out->prune0,
                                                                        out->prune1, out->n_matches, n0, n1, B);
-    CU(cudaGetLastError());
+    LG_CU(cudaGetLastError());
     h->launches = 1;
     return 0;
   }
-  RC(check_outputs(out));
+  LG_RC(check_outputs(out));
   if (!in->kpts0 || !in->kpts1 || !in->desc0 || !in->desc1) return lg_set_error("lg_forward: null input tensor");
   Workspace w;
   carve(h, B, M, N, (char*)workspace, &w);
@@ -472,7 +450,7 @@ extern "C" int lg_forward(LgHandle* h, const LgInputs* in, const LgOutputs* out,
 
   if (out->log_assignment && (in->lens0 || in->lens1))
     return lg_set_error("lg_forward: log_assignment is defined for dense batches only (no lens0/lens1)");
-  RC(misc_init_state(w.lena, w.inda, w.prune, w.stop_layer, w.below, L * B, B, M, N, Lp, in->lens0, in->lens1, stream));
+  LG_RC(misc_init_state(w.lena, w.inda, w.prune, w.stop_layer, w.below, L * B, B, M, N, Lp, in->lens0, in->lens1, stream));
   h->launches += 1;
   float *x = w.xa, *x_alt = w.xb, *cs = w.csa, *cs_alt = w.csb;
   int *len = w.lena, *len_alt = w.lenb, *ind = w.inda, *ind_alt = w.indb;
@@ -482,16 +460,16 @@ extern "C" int lg_forward(LgHandle* h, const LgInputs* in, const LgOutputs* out,
     Timer t(h, LG_K_OTHER, stream);
     PosencArgs pa{in->kpts0, in->kpts1, in->size0, in->size1, in->scales0, in->oris0, in->scales1, in->oris1,
                   h->wpk + h->o_wr, h->cfg.pos_dim, B, M, N, Lp, cs, in->lens0, in->lens1};
-    RC(misc_posenc(pa, stream));
+    LG_RC(misc_posenc(pa, stream));
     h->launches += 1;
   }
   // descriptors -> residual stream (optionally through input_proj, lightglue.py:521-522)
   if (h->cfg.input_dim == (int)D) {
-    RC(misc_pack_desc(in->desc0, in->desc1, x, B, M, N, Lp, D, in->lens0, in->lens1, stream, fp32 ? nullptr : (void*)w.tc.xh,
+    LG_RC(misc_pack_desc(in->desc0, in->desc1, x, B, M, N, Lp, D, in->lens0, in->lens1, stream, fp32 ? nullptr : (void*)w.tc.xh,
                       fp32 ? nullptr : (void*)w.tc.xl));
     h->launches += 1;
   } else {
-    RC(misc_pack_desc(in->desc0, in->desc1, w.hbuf, B, M, N, Lp, h->cfg.input_dim, in->lens0, in->lens1, stream));
+    LG_RC(misc_pack_desc(in->desc0, in->desc1, w.hbuf, B, M, N, Lp, h->cfg.input_dim, in->lens0, in->lens1, stream));
     h->launches += 1;
     Timer t(h, LG_K_LINEAR, stream);
     if (fp32) {
@@ -499,10 +477,10 @@ extern "C" int lg_forward(LgHandle* h, const LgInputs* in, const LgOutputs* out,
       g.A0 = w.hbuf; g.lda0 = h->cfg.input_dim; g.K0 = h->cfg.input_dim;
       g.W = h->wpk + h->o_inw; g.bias = h->wpk + h->o_inb;
       g.K = h->cfg.input_dim; g.Nout = D; g.epi = EPI_STORE; g.scale = 1.f; g.out = x; g.ldo = D;
-      RC(simt_gemm(g, st, stream));
+      LG_RC(simt_gemm(g, st, stream));
       h->launches += 1;
     } else {
-      RC(tc_input_proj(h, w.tc, st, w.hbuf, x, stream));
+      LG_RC(tc_input_proj(h, w.tc, st, w.hbuf, x, stream));
     }
   }
 
@@ -518,35 +496,35 @@ extern "C" int lg_forward(LgHandle* h, const LgInputs* in, const LgOutputs* out,
         g.q = w.q; g.k = w.k; g.v = w.v; g.cs = cs;
         g.Nout = blk == 0 ? 3 * D : 2 * D;
         g.epi = blk == 0 ? EPI_QKV_ROPE : EPI_QK_V;
-        { Timer t(h, LG_K_LINEAR, stream); RC(simt_gemm(g, st, stream)); }
+        { Timer t(h, LG_K_LINEAR, stream); LG_RC(simt_gemm(g, st, stream)); }
         {
           Timer t(h, LG_K_ATTENTION, stream);
-          if (blk == 0) RC(simt_attention(w.q, w.k, w.v, w.ctx, 0, st, stream));
-          else RC(simt_attention(w.q, w.q, w.v, w.ctx, B, st, stream));
+          if (blk == 0) LG_RC(simt_attention(w.q, w.k, w.v, w.ctx, 0, st, stream));
+          else LG_RC(simt_attention(w.q, w.q, w.v, w.ctx, B, st, stream));
         }
         Timer t(h, LG_K_LINEAR, stream);
         GemmArgs go{};  // out_proj / to_out
         go.A0 = w.ctx; go.lda0 = D; go.K0 = D; go.K = D; go.W = bw + o.wo; go.bias = bw + o.bo; go.Nout = D;
         go.epi = EPI_STORE; go.scale = 1.f; go.out = w.msg; go.ldo = D;
-        RC(simt_gemm(go, st, stream));
+        LG_RC(simt_gemm(go, st, stream));
         GemmArgs g1{};  // ffn.0 on cat([x, msg])
         g1.A0 = x; g1.lda0 = D; g1.K0 = D; g1.A1 = w.msg; g1.lda1 = D; g1.K = F; g1.W = bw + o.w1; g1.bias = bw + o.b1;
         g1.Nout = F; g1.epi = EPI_STORE; g1.scale = 1.f; g1.out = w.hbuf; g1.ldo = F;
-        RC(simt_gemm(g1, st, stream));
-        RC(simt_layernorm_gelu(w.hbuf, bw + o.g, bw + o.be, st, stream));
+        LG_RC(simt_gemm(g1, st, stream));
+        LG_RC(simt_layernorm_gelu(w.hbuf, bw + o.g, bw + o.be, st, stream));
         GemmArgs g2{};  // ffn.3 + residual
         g2.A0 = w.hbuf; g2.lda0 = F; g2.K0 = F; g2.K = F; g2.W = bw + o.w2; g2.bias = bw + o.b2; g2.Nout = D;
         g2.epi = EPI_RESID; g2.scale = 1.f; g2.out = x; g2.ldo = D;
-        RC(simt_gemm(g2, st, stream));
+        LG_RC(simt_gemm(g2, st, stream));
         h->launches += 6;
       } else {
-        RC(tc_block(h, w.tc, st, i, blk, x, cs, stream));
+        LG_RC(tc_block(h, w.tc, st, i, blk, x, cs, stream));
       }
     }
     if (h->dbg_layers) {
       const size_t per = (size_t)2 * B * Lp * D;
       if ((size_t)(i + 1) * per > h->dbg_layers_floats) return lg_set_error("lg_debug_capture_layers: buffer too small");
-      CU(cudaMemcpyAsync(h->dbg_layers + (size_t)i * per, x, per * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+      LG_CU(cudaMemcpyAsync(h->dbg_layers + (size_t)i * per, x, per * sizeof(float), cudaMemcpyDeviceToDevice, stream));
     }
     if (i == L - 1) break;  // no early stopping or adaptive width at the last layer (544-545)
     if (!early && !prune) continue;
@@ -562,25 +540,25 @@ extern "C" int lg_forward(LgHandle* h, const LgInputs* in, const LgOutputs* out,
     a.lens0 = in->lens0; a.lens1 = in->lens1;
     a.keep = w.keep; a.below = w.below + (size_t)i * B; a.stop_layer = w.stop_layer;
     a.len_in = len; a.len_out = prune ? len_alt : len; a.pos = w.pos; a.did_prune = w.did_prune;
-    RC(misc_adapt_score(a, st, stream));
-    RC(misc_adapt_decide(a, st, stream));
+    LG_RC(misc_adapt_score(a, st, stream));
+    LG_RC(misc_adapt_decide(a, st, stream));
     h->launches += 2;
     if (prune) {
       GatherArgs ga{x, x_alt, cs, cs_alt, ind, ind_alt, w.prune, w.keep, w.pos, w.did_prune, len, len_alt, w.stop_layer, i};
-      RC(misc_adapt_gather(ga, st, stream));
+      LG_RC(misc_adapt_gather(ga, st, stream));
       h->launches += 1;
       float* tf = x; x = x_alt; x_alt = tf;
       tf = cs; cs = cs_alt; cs_alt = tf;
       int* ti = ind; ind = ind_alt; ind_alt = ti;
       ti = len; len = len_alt; len_alt = ti;
       st.len = len;
-      if (!fp32) { RC(tc_refresh_shadow(h, w.tc, x, st, stream)); h->launches += 1; }
+      if (!fp32) { LG_RC(tc_refresh_shadow(h, w.tc, x, st, stream)); h->launches += 1; }
     }
   }
-  RC(misc_finalize_stop(w.stop_layer, B, L, stream));
+  LG_RC(misc_finalize_stop(w.stop_layer, B, L, stream));
   h->launches += 1;
-  RC(run_assign(h, w, st, x, ind, M, N, out, stream));
-  RC(misc_export_stop_prune(w.stop_layer, w.prune, out->stop, out->prune0, out->prune1, B, M, N, Lp, stream));
+  LG_RC(run_assign(h, w, st, x, ind, M, N, out, stream));
+  LG_RC(misc_export_stop_prune(w.stop_layer, w.prune, out->stop, out->prune0, out->prune1, B, M, N, Lp, stream));
   h->launches += 1;
   return 0;
 }
@@ -588,20 +566,20 @@ extern "C" int lg_forward(LgHandle* h, const LgInputs* in, const LgOutputs* out,
 extern "C" int lg_assign(LgHandle* h, int32_t layer, int32_t B, int32_t M, int32_t N, const float* x0, const float* x1,
                          const LgOutputs* out, void* workspace, size_t ws_bytes, void* stream_) {
   if (!h || !x0 || !x1) return lg_set_error("lg_assign: null argument");
-  RC(check_outputs(out));
+  LG_RC(check_outputs(out));
   if (B <= 0 || M <= 0 || N <= 0 || layer < 0 || layer >= h->cfg.n_layers) return lg_set_error("lg_assign: bad shape/layer");
   cudaStream_t stream = (cudaStream_t)stream_;
   Workspace w;
   carve(h, B, M, N, (char*)workspace, &w);
   if (!workspace || ws_bytes < w.bytes) return lg_set_error("lg_assign: workspace too small");
   h->launches = 0;
-  RC(misc_init_state(w.lena, w.inda, w.prune, w.stop_layer, w.below, h->cfg.n_layers * B, B, M, N, w.Lp, nullptr, nullptr,
+  LG_RC(misc_init_state(w.lena, w.inda, w.prune, w.stop_layer, w.below, h->cfg.n_layers * B, B, M, N, w.Lp, nullptr, nullptr,
                      stream));
-  RC(misc_finalize_stop(w.stop_layer, B, layer + 1, stream));  // selects log_assignment[layer] for every pair
-  RC(misc_pack_desc(x0, x1, w.xa, B, M, N, w.Lp, D, nullptr, nullptr, stream));
+  LG_RC(misc_finalize_stop(w.stop_layer, B, layer + 1, stream));  // selects log_assignment[layer] for every pair
+  LG_RC(misc_pack_desc(x0, x1, w.xa, B, M, N, w.Lp, D, nullptr, nullptr, stream));
   h->launches += 3;
   SeqState st{2 * B, B, w.Lp, w.lena, w.stop_layer};
-  if (h->cfg.precision != LG_PREC_FP32) { RC(tc_refresh_shadow(h, w.tc, w.xa, st, stream)); h->launches += 1; }
+  if (h->cfg.precision != LG_PREC_FP32) { LG_RC(tc_refresh_shadow(h, w.tc, w.xa, st, stream)); h->launches += 1; }
   return run_assign(h, w, st, w.xa, w.inda, M, N, out, stream);
 }
 
@@ -615,7 +593,7 @@ extern "C" int lg_attention(LgHandle* h, int32_t B, int32_t M, int32_t N, int32_
   carve(h, B, M, N, (char*)workspace, &w);
   if (!workspace || ws_bytes < w.bytes) return lg_set_error("lg_attention: workspace too small");
   h->launches = 0;
-  RC(misc_init_state(w.lena, w.inda, w.prune, w.stop_layer, w.below, h->cfg.n_layers * B, B, M, N, w.Lp, nullptr, nullptr,
+  LG_RC(misc_init_state(w.lena, w.inda, w.prune, w.stop_layer, w.below, h->cfg.n_layers * B, B, M, N, w.Lp, nullptr, nullptr,
                      stream));
   SeqState st{2 * B, B, w.Lp, w.lena, w.stop_layer};
   const bool fp32 = h->cfg.precision == LG_PREC_FP32;
@@ -625,13 +603,13 @@ extern "C" int lg_attention(LgHandle* h, int32_t B, int32_t M, int32_t N, int32_
   if (fp32) { a.qf = w.q; a.kf = w.k; a.vf = w.v; a.ctxf = w.ctx; }
   else { a.qh = w.tc.q; a.kh = w.tc.k; a.vth = w.tc.vt; a.ctxh = w.tc.ctxh; a.ctxl = w.tc.ctxl; }
   a.out0 = ctx0; a.out1 = ctx1;
-  RC(misc_attn_pack(a, stream));
+  LG_RC(misc_attn_pack(a, stream));
   {
     Timer t(h, LG_K_ATTENTION, stream);
-    if (fp32) RC(simt_attention(w.q, w.k, w.v, w.ctx, cross ? B : 0, st, stream));
-    else RC(tc_attention(h, w.tc, st, cross ? B : 0, w.tc.k, stream));
+    if (fp32) LG_RC(simt_attention(w.q, w.k, w.v, w.ctx, cross ? B : 0, st, stream));
+    else LG_RC(tc_attention(h, w.tc, st, cross ? B : 0, w.tc.k, stream));
   }
-  RC(misc_attn_unpack(a, stream));
+  LG_RC(misc_attn_unpack(a, stream));
   h->launches += fp32 ? 4 : 3;  // init + pack + (attention counted by tc_attention) + unpack
   return 0;
 }

@@ -12,10 +12,18 @@
 #define LG_FFN 512
 #define LG_TILE 128
 
-#define LG_CHECK_LAUNCH()                                     \
-  do {                                                        \
-    cudaError_t e__ = cudaGetLastError();                     \
-    if (e__ != cudaSuccess) return lg_set_cuda_error(e__, __FILE__, __LINE__); \
+// Error returns of the C-ABI code: a failed CUDA call records its error and returns it (LG_CU; LG_CHECK_LAUNCH after a
+// kernel launch), a non-zero return code is passed on (LG_RC).
+#define LG_CU(x)                                                                 \
+  do {                                                                           \
+    cudaError_t e__ = (x);                                                       \
+    if (e__ != cudaSuccess) return lg_set_cuda_error(e__, __FILE__, __LINE__);   \
+  } while (0)
+#define LG_CHECK_LAUNCH() LG_CU(cudaGetLastError())
+#define LG_RC(x)         \
+  do {                   \
+    int r__ = (x);       \
+    if (r__) return r__; \
   } while (0)
 
 int lg_set_cuda_error(cudaError_t e, const char* file, int line);

@@ -6,6 +6,7 @@
 #include <stdint.h>
 
 #include "lg_internal.h"
+#include "ws_bump.h"
 
 struct LgHandle;
 struct TcMapCache;
@@ -33,7 +34,7 @@ struct TcBuffers {
   __half* vt;                  // [S, H, 64, Lp] fp16, V transposed
 };
 
-void tc_carve(size_t* off, char* base, size_t S, int Lp, const LgHandle* h, TcBuffers* out);
+void tc_carve(WsBump& b, size_t S, int Lp, const LgHandle* h, TcBuffers* out);
 // x fp32 [S, Lp, 256] -> bf16 (hi / lo) shadow copies the linears consume
 int tc_refresh_shadow(LgHandle* h, const TcBuffers& b, const float* x, const SeqState& st, cudaStream_t stream);
 int tc_input_proj(LgHandle* h, const TcBuffers& b, const SeqState& st, const float* desc_packed, float* x, cudaStream_t stream);

@@ -36,30 +36,16 @@ struct CudaExec {
     const int threads = F::SCRATCH > 64 ? 32 : 128;
     const size_t smem = sizeof(float) * F::SCRATCH * threads;
     sift_stage<F><<<(unsigned)((n + threads - 1) / threads), threads, smem, s>>>(f, n);
-    const cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : lg_set_cuda_error(e, __FILE__, __LINE__);
+    LG_CHECK_LAUNCH();
+    return 0;
   }
   int zero(int* p, int n) {
-    const cudaError_t e = cudaMemsetAsync(p, 0, sizeof(int) * n, s);
-    return e == cudaSuccess ? 0 : lg_set_cuda_error(e, __FILE__, __LINE__);
+    LG_CU(cudaMemsetAsync(p, 0, sizeof(int) * n, s));
+    return 0;
   }
 };
 
 __global__ void sift_count_kernel(const int* counters, int32_t* count) { *count = counters[3] ? -1 : counters[2]; }
-
-SiftParams params(const SiftConfig& c) {
-  SiftParams p{};
-  p.L = c.num_octave_layers;
-  p.contrast = (float)c.detection_threshold;
-  p.edge = (float)c.edge_threshold;
-  p.sigma = 1.6f;
-  p.threshold = (int)floor(0.5 * c.detection_threshold / c.num_octave_layers * 255);
-  p.nfeatures = c.max_num_keypoints;
-  p.nms_radius = c.nms_radius;
-  p.max_kpts = c.max_num_keypoints;
-  p.rootsift = c.rootsift;
-  return p;
-}
 
 }  // namespace
 
@@ -109,16 +95,15 @@ extern "C" int sift_forward(SiftHandle* h, const float* image, int32_t channels,
   SiftWs w;
   sift_carve(base, H, W, h->cfg.num_octave_layers, h->cfg.max_num_keypoints, &w);
   CudaExec ex{(cudaStream_t)stream_};
-  const SiftParams p = params(h->cfg);
+  const SiftConfig& c = h->cfg;
+  const SiftParams p = sift_params(c.num_octave_layers, c.detection_threshold, c.edge_threshold, c.nms_radius,
+                                   c.max_num_keypoints, c.rootsift);
   for (int b = 0; b < B; ++b) {
     const int iw = image_size ? image_size[2 * b] : W, ih = image_size ? image_size[2 * b + 1] : H;
-    const int rc = sift_run(ex, p, image + (long)b * channels * H * W, channels, H, W, ih, iw, w, (int)cap,
-                            keypoints + b * cap * 2, scales + b * cap, oris + b * cap, scores + b * cap,
-                            descriptors + b * cap * SIFT_DESC);
-    if (rc) return rc;
+    LG_RC(sift_run(ex, p, image + (long)b * channels * H * W, channels, H, W, ih, iw, w, (int)cap, keypoints + b * cap * 2,
+                   scales + b * cap, oris + b * cap, scores + b * cap, descriptors + b * cap * SIFT_DESC));
     sift_count_kernel<<<1, 1, 0, ex.s>>>(w.counters, counts + b);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return lg_set_cuda_error(e, __FILE__, __LINE__);
+    LG_CHECK_LAUNCH();
   }
   return 0;
 }

@@ -23,6 +23,8 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include "ws_bump.h"
+
 #if defined(__CUDACC__)
 #define SIFT_HD __host__ __device__ __forceinline__
 #else
@@ -214,6 +216,22 @@ struct SiftParams {
   int max_kpts;             // top-k after filter_dog_point (max_num_keypoints)
   int rootsift;
 };
+
+// The parameters of a conf (include/sift_b200.h SiftConfig): L = num_octaves, contrast = detection_threshold,
+// edge = edge_threshold, max_kpts = max_num_keypoints (> 0), nms_radius (-1 = None), rootsift.
+inline SiftParams sift_params(int L, double contrast, double edge, int nms_radius, int max_kpts, int rootsift) {
+  SiftParams p{};
+  p.L = L;
+  p.contrast = (float)contrast;
+  p.edge = (float)edge;
+  p.sigma = 1.6f;
+  p.threshold = (int)floor(0.5 * contrast / L * 255);
+  p.nfeatures = max_kpts;
+  p.nms_radius = nms_radius;
+  p.max_kpts = max_kpts;
+  p.rootsift = rootsift;
+  return p;
+}
 
 // adjustLocalExtrema: up to five Newton steps on the DoG cube, then the contrast and edge tests.
 SIFT_HD bool sift_adjust(const SiftOctave& oc, int o, const SiftParams& p, int& layer, int& r, int& c, SiftCand& out) {
@@ -706,8 +724,6 @@ struct SiftWs {  // workspace carve for one image at most H x W (images are proc
   size_t bytes;
 };
 
-inline size_t sift_align(size_t v) { return (v + 255) & ~(size_t)255; }
-
 inline size_t sift_pyr_floats(int H, int W, int L) {
   size_t f = 0;
   int h = 2 * H, w = 2 * W;
@@ -719,20 +735,19 @@ inline size_t sift_pyr_floats(int H, int W, int L) {
 }
 
 inline void sift_carve(char* base, int H, int W, int L, int max_kpts, SiftWs* w) {
-  size_t o = 0;
-  auto take = [&](size_t n) { char* p = base ? base + o : nullptr; o += sift_align(n); return p; };
+  WsBump b{base, 0};
   w->raw_cap = sift_raw_cap(H, W);
-  w->counters = (int*)take(sizeof(int) * 8);
-  w->q = (float*)take(sizeof(float) * H * W);
-  w->tmp = (float*)take(sizeof(float) * 4 * H * W);
-  w->pyr = (float*)take(sizeof(float) * sift_pyr_floats(H, W, L));
-  w->cand = (SiftCand*)take(sizeof(SiftCand) * w->raw_cap);
-  w->kpt = (SiftKpt*)take(sizeof(SiftKpt) * w->raw_cap);
-  w->order = (int*)take(sizeof(int) * w->raw_cap);
-  w->flags = (int*)take(sizeof(int) * w->raw_cap);
-  w->pix = (int*)take(sizeof(int) * w->raw_cap);
-  w->out_src = (int*)take(sizeof(int) * (max_kpts > 0 ? max_kpts : 1));
-  w->bytes = o;
+  w->counters = b.take<int>(8);
+  w->q = b.take<float>((size_t)H * W);
+  w->tmp = b.take<float>((size_t)4 * H * W);
+  w->pyr = b.take<float>(sift_pyr_floats(H, W, L));
+  w->cand = b.take<SiftCand>(w->raw_cap);
+  w->kpt = b.take<SiftKpt>(w->raw_cap);
+  w->order = b.take<int>(w->raw_cap);
+  w->flags = b.take<int>(w->raw_cap);
+  w->pix = b.take<int>(w->raw_cap);
+  w->out_src = b.take<int>(max_kpts > 0 ? max_kpts : 1);
+  w->bytes = b.bytes();
 }
 
 // Host-side layout of one image's pyramid inside w.pyr: gauss[o][i] and dog[o][i] pointers and octave sizes.

@@ -1,18 +1,21 @@
-// SuperPoint extractor forward (SURVEY.md 8f1; reference lightglue/superpoint.py:163-227), first CUDA path.
+// SuperPoint extractor forward (SURVEY.md 8f1; reference lightglue/superpoint.py:163-227).
 //
 // Every stage is a small functor with `operator()(long i)` = the work of ONE logical thread, and the whole forward
 // is one template `sp_run(Exec&, ...)` that hands those functors to an executor.  The CUDA build (sp_api.cu)
 // executes them with a generic grid-stride-free kernel (one thread per index); the test-only build under oracle/
 // (sp_emul.cpp, plain g++) executes THE SAME functors and THE SAME orchestration in a host loop, which is how the
 // kernel logic is checked against the reference-generated fixtures on a machine without a GPU.  There is no
-// shared memory, no warp intrinsic and no atomics in this path: it is the correctness baseline for the extractor
-// (fp32, CUDA cores); the tensor-core implicit-GEMM convolutions replace `SpConv` later.
+// shared memory, no warp intrinsic and no atomics in this path: it is the fp32 (CUDA-core) forward and the
+// correctness baseline for the extractor.  precision "bf16x3" replaces the convolutions with the tensor-core backbone
+// (sp_tc.cu) and the heavy post-processing stages with warp / block kernels (SpCudaStages); the rest runs from here.
 //
 // Layouts: feature maps NCHW fp32, weights as in the reference state_dict ([Cout, Cin, k, k] row-major).
 #pragma once
 #include <math.h>
 #include <stddef.h>
 #include <stdint.h>
+
+#include "ws_bump.h"
 
 #if defined(__CUDACC__)
 #define SP_HD __host__ __device__ __forceinline__
@@ -285,27 +288,59 @@ struct SpWorkspace {
   size_t bytes;
 };
 inline void sp_carve(char* base, int B, int H, int W, long out_cap, SpWorkspace* w) {
-  size_t off = 0;
-  auto take = [&](size_t n, size_t elt) { off = (off + 255) & ~(size_t)255; char* p = base ? base + off : nullptr; off += n * elt; return p; };
+  WsBump b{base, 0};
   const size_t px = (size_t)B * H * W, Hc = H / SP_CELL, Wc = W / SP_CELL;
-  w->bufA = (float*)take(px * 64, 4);
-  w->bufB = (float*)take(px * 64, 4);
-  w->logits = (float*)take((size_t)B * 65 * Hc * Wc, 4);
-  w->scores = (float*)take(px, 4);
-  w->t0 = (float*)take(px, 4);
-  w->t1 = (float*)take(px, 4);
-  w->t2 = (float*)take(px, 4);
-  w->mask = (float*)take(px, 4);
-  w->dense = (float*)take((size_t)B * SP_DESC * Hc * Wc, 4);
-  w->cand_score = (float*)take(px, 4);
-  w->sel_score = (float*)take((size_t)B * out_cap, 4);
-  w->row_count = (int*)take((size_t)B * H, 4);
-  w->row_start = (int*)take((size_t)B * H, 4);
-  w->n_cand = (int*)take(B, 4);
-  w->cand_pos = (int*)take(px, 4);
-  w->sel_pos = (int*)take((size_t)B * out_cap, 4);
-  w->n_sel = (int*)take(B, 4);
-  w->bytes = (off + 255) & ~(size_t)255;
+  w->bufA = b.take<float>(px * 64);
+  w->bufB = b.take<float>(px * 64);
+  w->logits = b.take<float>((size_t)B * 65 * Hc * Wc);
+  w->scores = b.take<float>(px);
+  w->t0 = b.take<float>(px);
+  w->t1 = b.take<float>(px);
+  w->t2 = b.take<float>(px);
+  w->mask = b.take<float>(px);
+  w->dense = b.take<float>((size_t)B * SP_DESC * Hc * Wc);
+  w->cand_score = b.take<float>(px);
+  w->sel_score = b.take<float>((size_t)B * out_cap);
+  w->row_count = b.take<int>((size_t)B * H);
+  w->row_start = b.take<int>((size_t)B * H);
+  w->n_cand = b.take<int>(B);
+  w->cand_pos = b.take<int>(px);
+  w->sel_pos = b.take<int>((size_t)B * out_cap);
+  w->n_sel = b.take<int>(B);
+  w->bytes = b.bytes();
+}
+
+// Keypoints per image at most (sp_max_keypoints): max_num_keypoints, or else the most NMS survivors the image can hold
+inline int64_t sp_keypoint_cap(int nms_radius, int max_num_keypoints, int H, int W) {
+  if (max_num_keypoints > 0) return max_num_keypoints;
+  const int step = nms_radius + 1;  // no two NMS survivors lie within `nms_radius` of each other (Chebyshev)
+  return (int64_t)((H + step - 1) / step) * ((W + step - 1) / step);
+}
+
+// simple_nms (52-68) of `scores` [B,H,W] into `out` (which may be `tmp`): window maxima of radius r along x then y
+// (`line` holds the x pass), and the elementwise steps.  `tmp`, `mask`, `supp` and `pooled` are [B,H,W] scratch.
+template <class Exec>
+int sp_simple_nms(Exec& exec, const float* scores, float* out, int B, int H, int W, int r, float* tmp, float* mask,
+                  float* supp, float* pooled, float* line) {
+  const long n = (long)B * H * W;
+  auto wmax = [&](const float* in, float* o) {
+    SpWindowMax a{in, line, B, H, W, r, 0};
+    int e = exec.run(a);
+    if (e) return e;
+    SpWindowMax b{line, o, B, H, W, r, 1};
+    return exec.run(b);
+  };
+  int rc;
+  if ((rc = wmax(scores, tmp))) return rc;
+  { SpNmsStep s{scores, tmp, nullptr, mask, n, 0}; if ((rc = exec.run(s))) return rc; }
+  for (int it = 0; it < 2; ++it) {
+    if ((rc = wmax(mask, tmp))) return rc;                                                     // tmp = max_pool(max_mask)
+    { SpNmsStep s{scores, tmp, nullptr, supp, n, 1}; if ((rc = exec.run(s))) return rc; }     // supp = supp_scores
+    if ((rc = wmax(supp, pooled))) return rc;                                                  // pooled = max_pool(supp)
+    { SpNmsStep s{supp, pooled, tmp, mask, n, 2}; if ((rc = exec.run(s))) return rc; }
+  }
+  { SpNmsStep s{scores, mask, nullptr, out, n, 3}; if ((rc = exec.run(s))) return rc; }       // nms scores
+  return 0;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -385,25 +420,9 @@ int sp_run_post(Exec& exec, const SpParams& prm, int B, int H, int W, long out_c
   const int Hc = H / SP_CELL, Wc = W / SP_CELL;
   // detector scores (186-190)
   { SpScores s{ws.logits, ws.scores, B, Hc, Wc}; if ((rc = exec.run(s))) return rc; }
-  // simple_nms (52-68)
-  const long n = (long)B * H * W;
-  const int r = prm.nms_radius;
-  auto wmax = [&](const float* in, float* out) {
-    SpWindowMax a{in, ws.t2, B, H, W, r, 0};
-    int e = exec.run(a);
-    if (e) return e;
-    SpWindowMax b{ws.t2, out, B, H, W, r, 1};
-    return exec.run(b);
-  };
-  if ((rc = wmax(ws.scores, ws.t0))) return rc;
-  { SpNmsStep s{ws.scores, ws.t0, nullptr, ws.mask, n, 0}; if ((rc = exec.run(s))) return rc; }
-  for (int it = 0; it < 2; ++it) {
-    if ((rc = wmax(ws.mask, ws.t0))) return rc;                                                   // t0 = max_pool(max_mask)
-    { SpNmsStep s{ws.scores, ws.t0, nullptr, ws.t1, n, 1}; if ((rc = exec.run(s))) return rc; }   // t1 = supp_scores
-    if ((rc = wmax(ws.t1, ws.cand_score))) return rc;                                             // cand_score (scratch) = max_pool(supp_scores)
-    { SpNmsStep s{ws.t1, ws.cand_score, ws.t0, ws.mask, n, 2}; if ((rc = exec.run(s))) return rc; }
-  }
-  { SpNmsStep s{ws.scores, ws.mask, nullptr, ws.t0, n, 3}; if ((rc = exec.run(s))) return rc; }   // t0 = nms scores
+  // simple_nms (52-68) -> t0; cand_score is scratch until the compaction
+  if ((rc = sp_simple_nms(exec, ws.scores, ws.t0, B, H, W, prm.nms_radius, ws.t0, ws.mask, ws.t1, ws.cand_score, ws.t2)))
+    return rc;
   if (prm.remove_borders > 0) { SpBorders s{ws.t0, B, H, W, prm.remove_borders}; if ((rc = exec.run(s))) return rc; }
   // keypoints (201-218)
   const long cap = (long)H * W;

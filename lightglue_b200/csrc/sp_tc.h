@@ -27,6 +27,28 @@ void sp_tc_destroy(SpTc* t);
 int sp_tc_backbone(SpTc* t, const float* wts_dev, const float* image, int B, int H, int W, void* workspace, float* logits_nchw,
                    float* dense_nchw, cudaStream_t stream);
 
+namespace {
+// Executor of the sp_pipeline.h functors on `stream`, one thread per logical index (SuperPoint and ALIKED's DKD)
+template <class F>
+__global__ void __launch_bounds__(256) sp_for_each_kernel(F f, long n) {
+  const long i = blockIdx.x * (long)blockDim.x + threadIdx.x;
+  if (i < n) f(i);
+}
+struct SpCudaExec {
+  cudaStream_t stream;
+  template <class F>
+  int run(const F& f) {
+    const long n = f.count();
+    if (n <= 0) return 0;
+    const long blocks = (n + 255) / 256;
+    if (blocks > 0x7fffffffL) return lg_set_error("sp_pipeline functor: grid too large");
+    sp_for_each_kernel<F><<<(unsigned)blocks, 256, 0, stream>>>(f, n);
+    LG_CHECK_LAUNCH();
+    return 0;
+  }
+};
+}  // namespace
+
 // Stages policy of sp_run_post (sp_pipeline.h): warp / block kernels for candidate compaction, top-k and descriptor
 // sampling; top-k beyond SP_SEL_KMAX (4096) falls back to the functor.
 struct SpCudaStages {

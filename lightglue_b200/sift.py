@@ -22,17 +22,16 @@ Deviations from the reference:
 """
 from __future__ import annotations
 
-import ctypes as C
 from types import SimpleNamespace
 
 import torch
-from torch import nn
 
 from . import _cabi
 from . import extractor as _extractor
 
 
-class SIFT(nn.Module):
+class SIFT(_extractor.CudaExtractor):
+    _abi = "sift"
     default_conf = {
         "rootsift": True,
         "nms_radius": 0,  # None to disable filtering entirely.
@@ -62,8 +61,6 @@ class SIFT(nn.Module):
             raise ValueError(f"nms_radius={self.conf.nms_radius!r}: must be >= 0 or None")
         if not 1 <= int(self.conf.num_octaves) <= 8:
             raise ValueError(f"num_octaves={self.conf.num_octaves!r}: must be in [1, 8]")
-        self._handles = {}
-        self._ws = {}
 
     def _config(self) -> _cabi.SiftConfig:
         c = self.conf
@@ -74,76 +71,26 @@ class SIFT(nn.Module):
             edge_threshold=float(c.edge_threshold),
         )
 
-    def _get_handle(self, device):
-        h = self._handles.get(device.index)
-        if h is None:
-            lib = _cabi.load()
-            h = C.c_void_p()
-            cfg = self._config()
-            _cabi.check(lib.sift_create(C.byref(cfg), None, C.byref(h)), "sift_create")
-            self._handles[device.index] = h
-        return h
-
-    def __del__(self):
-        if getattr(self, "_handles", None) and _cabi._lib is not None:
-            for h in self._handles.values():
-                _cabi._lib.sift_destroy(h)
-            self._handles = {}
+    def _create(self, lib, cfg, blob, stream, out):
+        _cabi.check(lib.sift_create(cfg, None, out), "sift_create")
 
     @torch.no_grad()
     def forward(self, data: dict) -> dict:
         for key in self.required_data_keys:
             assert key in data, f"Missing key {key} in data"
-        image = data["image"]
-        if image.device.type != "cuda":
-            raise RuntimeError("lightglue_b200.SIFT runs on CUDA (sm_90a) tensors only; there is no CPU path")
+        image = self._cuda_image(data["image"])
         b, c, hh, ww = image.shape
         if c not in (1, 3):
             raise ValueError(f"image has {c} channels: expected 1 (gray) or 3 (RGB)")
-        device = image.device
         image = image.detach().to(torch.float32).contiguous()
         size = data.get("image_size")
         if size is not None:  # host copy: the pyramid's shapes depend on it
             size = torch.as_tensor(size).reshape(b, 2).cpu().to(torch.int32).contiguous()
-        with torch.cuda.device(device):
-            lib = _cabi.load()
-            handle = self._get_handle(device)
-            cap = int(lib.sift_max_keypoints(handle, hh, ww))
-            key = (device.index, hh, ww)
-            ws = self._ws.get(key)
-            if ws is None:
-                self._ws.clear()
-                ws = self._ws[key] = torch.empty(int(lib.sift_workspace_bytes(handle, b, hh, ww)), dtype=torch.uint8,
-                                                 device=device)
-            kpts = torch.empty(b, cap, 2, dtype=torch.float32, device=device)
-            scales = torch.empty(b, cap, dtype=torch.float32, device=device)
-            oris = torch.empty(b, cap, dtype=torch.float32, device=device)
-            scores = torch.empty(b, cap, dtype=torch.float32, device=device)
-            desc = torch.empty(b, cap, 128, dtype=torch.float32, device=device)
-            counts = torch.empty(b, dtype=torch.int32, device=device)
-            stream = torch.cuda.current_stream(device).cuda_stream
-            _cabi.check(
-                lib.sift_forward(handle, image.data_ptr(), c, size.data_ptr() if size is not None else None, b, hh, ww,
-                                 cap, kpts.data_ptr(), scales.data_ptr(), oris.data_ptr(), scores.data_ptr(),
-                                 desc.data_ptr(), counts.data_ptr(), ws.data_ptr(), ws.numel(), stream),
-                "sift_forward",
-            )
-            n = counts.cpu().tolist()  # the one host read-back: keypoint counts
-        if min(n) < 0:
-            raise RuntimeError(f"sift_forward: an image has more raw keypoints than the internal list holds (counts {n})")
-        if len(set(n)) != 1:  # the reference stacks the per-image results, which needs equal counts
-            raise ValueError(f"images of the batch have different keypoint counts {n}; lower max_num_keypoints or batch 1")
-        k = n[0]
-        return {
-            "keypoints": kpts[:, :k].contiguous(),
-            "scales": scales[:, :k].contiguous(),
-            "oris": oris[:, :k].contiguous(),
-            "keypoint_scores": scores[:, :k].contiguous(),
-            "descriptors": desc[:, :k].contiguous(),
-        }
 
-    @torch.no_grad()
-    def extract(self, img: torch.Tensor, **conf) -> dict:
-        """``Extractor.extract``: resize, ``forward``, keypoints back in the original pixels (lightglue_b200/extractor.py);
-        ``scales`` are returned as ``forward`` gives them, as in the reference."""
-        return _extractor.extract(self, img, **conf)
+        def call(lib, handle, cap, p, tail):
+            return lib.sift_forward(handle, image.data_ptr(), c, size.data_ptr() if size is not None else None, b, hh, ww,
+                                    cap, p["keypoints"], p["scales"], p["oris"], p["keypoint_scores"], p["descriptors"],
+                                    *tail)
+
+        return self._run(image, {"keypoints": (2,), "scales": (), "oris": (), "keypoint_scores": (), "descriptors": (128,)},
+                         call)

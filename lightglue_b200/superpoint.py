@@ -1,15 +1,15 @@
 """Drop-in host mirror of ``lightglue.SuperPoint`` (reference lightglue/superpoint.py:99-227) over the C ABI in
 ``include/superpoint_b200.h`` -- the caller-side row next to the matcher (SURVEY.md 8f1).
 
-First CUDA path: fp32 on CUDA cores (``csrc/sp_pipeline.h``), no tensor cores yet.  Same parameter names, conf keys
-and output dict as the reference; CUDA tensors only, no CPU path.  What is host glue here and not kernels: the
-RGB -> gray weighting the reference takes from kornia (``rgb_to_grayscale``: 0.299 R + 0.587 G + 0.114 B) and the
-optional resize of ``extract`` (the reference uses kornia's antialiased resize, utils.py:17-38; here
+The twelve convolutions run on tensor cores (``precision="bf16x3"``, ``csrc/sp_tc.cu``) or in fp32 on CUDA cores
+(``precision="fp32"``, ``csrc/sp_pipeline.h``); the rest of the forward is ``csrc/sp_pipeline.h``.  Same parameter
+names, conf keys and output dict as the reference; CUDA tensors only, no CPU path.  What is host glue here and not
+kernels: the RGB -> gray weighting the reference takes from kornia (``rgb_to_grayscale``: 0.299 R + 0.587 G + 0.114 B)
+and the optional resize of ``extract`` (the reference uses kornia's antialiased resize, utils.py:17-38; here
 ``F.interpolate(..., mode="bilinear", antialias=True)``).
 """
 from __future__ import annotations
 
-import ctypes as C
 from types import SimpleNamespace
 
 import torch
@@ -25,7 +25,8 @@ LAYERS = (  # name, out channels, in channels, kernel   (superpoint.py:137-153)
 )
 
 
-class SuperPoint(nn.Module):
+class SuperPoint(_extractor.CudaExtractor):
+    _abi = "sp"
     default_conf = {  # superpoint.py:112-118
         "descriptor_dim": 256,
         "nms_radius": 4,
@@ -56,14 +57,17 @@ class SuperPoint(nn.Module):
         if self.conf.weights is not None:
             self.load_state_dict(self._find_checkpoint(f"{self.conf.weights}.pth"))
         self.requires_grad_(False)
-        self._handle = None  # (C handle, device index, weight signature)
-        self._ws = {}
 
     def _find_checkpoint(self, fname: str):
         """The reference downloads the checkpoint (155-156); offline we look in the usual caches."""
         return _extractor.find_checkpoint(fname, self.url, "SuperPoint")
 
     # ------------------------------------------------------------------ C handle
+    def _config(self) -> _cabi.SpConfig:
+        c = self.conf
+        return _cabi.SpConfig(_cabi.SP_ABI_VERSION, int(c.nms_radius), int(c.max_num_keypoints or 0),
+                              int(c.remove_borders), float(c.detection_threshold), 1 if c.precision == "bf16x3" else 0)
+
     def _blob(self) -> torch.Tensor:
         parts = []
         for name, *_ in LAYERS:
@@ -71,43 +75,14 @@ class SuperPoint(nn.Module):
             parts += [m.weight.detach().reshape(-1), m.bias.detach().reshape(-1)]
         return torch.cat(parts).to(torch.float32).contiguous()
 
-    def _get_handle(self, device: torch.device):
-        lib = _cabi.load()
-        sig = (device.index, tuple(int(getattr(self, n).weight._version) for n, *_ in LAYERS),
-               self.conf.nms_radius, self.conf.max_num_keypoints, self.conf.remove_borders, self.conf.detection_threshold,
-               self.conf.precision)
-        if self._handle is not None and self._handle[1] == sig:
-            return self._handle[0]
-        self._release()
-        blob = self._blob().to(device)
+    def _create(self, lib, cfg, blob, stream, out):
         assert blob.numel() == lib.sp_weight_blob_floats()
-        cfg = _cabi.SpConfig(_cabi.SP_ABI_VERSION, int(self.conf.nms_radius), int(self.conf.max_num_keypoints or 0),
-                             int(self.conf.remove_borders), float(self.conf.detection_threshold),
-                             1 if self.conf.precision == "bf16x3" else 0)
-        h = C.c_void_p()
-        stream = torch.cuda.current_stream(device).cuda_stream
-        _cabi.check(lib.sp_create(C.byref(cfg), blob.data_ptr(), blob.numel(), stream, C.byref(h)), "sp_create")
-        torch.cuda.current_stream(device).synchronize()  # the blob may be freed once the copy has run
-        self._handle = (h, sig)
-        return h
-
-    def _release(self):
-        try:
-            if getattr(self, "_handle", None) is not None:  # (the constructor may have raised before the attribute exists)
-                _cabi.load().sp_destroy(self._handle[0])
-                object.__setattr__(self, "_handle", None)
-        except Exception:  # noqa: BLE001  (interpreter shutdown: modules may already be torn down)
-            pass
-
-    def __del__(self):
-        self._release()
+        _cabi.check(lib.sp_create(cfg, blob.data_ptr(), blob.numel(), stream, out), "sp_create")
 
     # ------------------------------------------------------------------ forward
-    @staticmethod
-    def _gray(image: torch.Tensor) -> torch.Tensor:
+    def _gray(self, image: torch.Tensor) -> torch.Tensor:
         """[B, 1 or 3, H, W] CUDA image -> contiguous fp32 [B, 1, H, W]."""
-        if image.device.type != "cuda":
-            raise RuntimeError("lightglue_b200.SuperPoint runs on CUDA (sm_90a) tensors only; there is no CPU path")
+        image = self._cuda_image(image)
         if image.shape[1] == 3:  # kornia.color.rgb_to_grayscale's weights (superpoint.py:168-169)
             wts = torch.tensor([0.299, 0.587, 0.114], device=image.device, dtype=image.dtype).view(1, 3, 1, 1)
             image = (image * wts).sum(1, keepdim=True)
@@ -117,14 +92,6 @@ class SuperPoint(nn.Module):
             raise ValueError(f"image size {ww}x{hh}: height and width must be at least 8 (one detector cell)")
         return image.detach().to(torch.float32).contiguous()
 
-    def _workspace(self, lib, handle, device: torch.device, b: int, hh: int, ww: int) -> torch.Tensor:
-        key = (device.index, b, hh, ww)
-        ws = self._ws.get(key)
-        if ws is None:
-            self._ws.clear()
-            ws = self._ws[key] = torch.empty(int(lib.sp_workspace_bytes(handle, b, hh, ww)), dtype=torch.uint8, device=device)
-        return ws
-
     @torch.no_grad()
     def forward(self, data: dict) -> dict:
         """Keypoints, scores and descriptors of an image batch (superpoint.py:163-227)."""
@@ -132,31 +99,12 @@ class SuperPoint(nn.Module):
             assert key in data, f"Missing key {key} in data"
         image = self._gray(data["image"])
         b, _, hh, ww = image.shape
-        device = image.device
-        with torch.cuda.device(device):
-            lib = _cabi.load()
-            handle = self._get_handle(device)
-            cap = int(lib.sp_max_keypoints(handle, hh, ww))
-            ws = self._workspace(lib, handle, device, b, hh, ww)
-            kpts = torch.empty(b, cap, 2, dtype=torch.float32, device=device)
-            scores = torch.empty(b, cap, dtype=torch.float32, device=device)
-            desc = torch.empty(b, cap, 256, dtype=torch.float32, device=device)
-            counts = torch.empty(b, dtype=torch.int32, device=device)
-            stream = torch.cuda.current_stream(device).cuda_stream
-            _cabi.check(
-                lib.sp_forward(handle, image.data_ptr(), b, hh, ww, cap, kpts.data_ptr(), scores.data_ptr(), desc.data_ptr(),
-                               counts.data_ptr(), ws.data_ptr(), ws.numel(), stream),
-                "sp_forward",
-            )
-            n = counts.cpu().tolist()  # the one host read-back: keypoint counts
-        if len(set(n)) != 1:  # the reference stacks the per-image results (223-227), which needs equal counts
-            raise ValueError(f"images of the batch have different keypoint counts {n}; set max_num_keypoints or batch 1")
-        k = n[0]
-        return {
-            "keypoints": kpts[:, :k].contiguous(),
-            "keypoint_scores": scores[:, :k].contiguous(),
-            "descriptors": desc[:, :k].contiguous(),
-        }
+
+        def call(lib, handle, cap, p, tail):
+            return lib.sp_forward(handle, image.data_ptr(), b, hh, ww, cap, p["keypoints"], p["keypoint_scores"],
+                                  p["descriptors"], *tail)
+
+        return self._run(image, {"keypoints": (2,), "keypoint_scores": (), "descriptors": (256,)}, call)
 
     @torch.no_grad()
     def backbone_heads(self, image: torch.Tensor):
@@ -176,9 +124,3 @@ class SuperPoint(nn.Module):
             _cabi.check(lib.sp_backbone(handle, image.data_ptr(), b, hh, ww, logits.data_ptr(), dense.data_ptr(), ws.data_ptr(),
                                         ws.numel(), stream), "sp_backbone")
         return logits, dense
-
-    @torch.no_grad()
-    def extract(self, img: torch.Tensor, **conf) -> dict:
-        """``Extractor.extract`` (utils.py:136-147): resize, ``forward``, keypoints back in the original pixels
-        (lightglue_b200/extractor.py)."""
-        return _extractor.extract(self, img, **conf)

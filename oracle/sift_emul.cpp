@@ -61,16 +61,7 @@ int sift_emul_forward(int L, double contrast, double edge, int nms_radius, int m
   if (!base) return 2;
   char* aligned = (char*)(((uintptr_t)base + 255) & ~(uintptr_t)255);
   sift_carve(aligned, H, W, L, max_kpts, &w);
-  SiftParams p{};
-  p.L = L;
-  p.contrast = (float)contrast;
-  p.edge = (float)edge;
-  p.sigma = 1.6f;
-  p.threshold = (int)floor(0.5 * contrast / L * 255);
-  p.nfeatures = max_kpts;
-  p.nms_radius = nms_radius;
-  p.max_kpts = max_kpts;
-  p.rootsift = rootsift;
+  const SiftParams p = sift_params(L, contrast, edge, nms_radius, max_kpts, rootsift);
   HostExec ex;
   int rc = 0;
   for (int b = 0; b < B && !rc; ++b) {

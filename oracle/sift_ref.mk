@@ -15,7 +15,7 @@ SIFT_REF := _ref/sift_ref.py
 
 sift-all: $(SIFT_EMUL) sift-ref
 
-$(SIFT_EMUL): sift_emul.cpp ../lightglue_b200/csrc/sift_pipeline.h
+$(SIFT_EMUL): sift_emul.cpp ../lightglue_b200/csrc/sift_pipeline.h ../lightglue_b200/csrc/ws_bump.h
 	@mkdir -p _build
 	$(CXX) -O2 -std=c++17 -fPIC -shared -pthread -ffp-contract=off -o $@ sift_emul.cpp -lm
 

@@ -43,9 +43,7 @@ extern "C" {
 size_t sp_emul_blob_floats(void) { return sp_blob_floats(); }
 
 long sp_emul_max_keypoints(int nms_radius, int max_num_keypoints, int H, int W) {
-  if (max_num_keypoints > 0) return max_num_keypoints;
-  const int step = nms_radius + 1;
-  return (long)((H + step - 1) / step) * ((W + step - 1) / step);
+  return (long)sp_keypoint_cap(nms_radius, max_num_keypoints, H, W);
 }
 
 // returns 0 on success; outputs as sp_forward (include/superpoint_b200.h)

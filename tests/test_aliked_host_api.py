@@ -22,6 +22,7 @@ def test_header_symbols_equal_exports_and_are_exported():
     lib = _cabi.load()
     for s in _cabi.AL_EXPORTS:
         assert hasattr(lib, s), s
+        assert getattr(lib, s).argtypes is not None, s
 
 
 @pytest.mark.parametrize("model_name", sorted(ALIKED.cfgs))

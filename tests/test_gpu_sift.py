@@ -125,3 +125,17 @@ def test_sift_feeds_the_matcher():
     out = lg({"image0": {**f0, "image_size": size}, "image1": {**f1, "image_size": size}})
     assert out["matches0"].shape == (1, n0) and out["matches1"].shape == (1, n1)
     assert out["matching_scores0"].shape == (1, n0)
+
+
+def test_conf_change_after_the_first_call_takes_effect():
+    """Setting ``conf.max_num_keypoints`` on a module that has run rebuilds its C handle, as a fresh module would.  (The
+    ``nfeatures`` cut comes before filter_dog_point, so the count may end below the cap.)"""
+    image = sift_synth.make_image(240, 320, 1, 13).cuda()
+    s = SIFT()
+    assert s({"image": image})["keypoints"].shape[1] > 100
+    s.conf.max_num_keypoints = 100
+    out = s({"image": image})
+    want = SIFT(max_num_keypoints=100)({"image": image})
+    assert 0 < out["keypoints"].shape[1] <= 100
+    for k in KEYS:
+        assert torch.equal(out[k], want[k]), k

@@ -19,6 +19,7 @@ def test_library_exports_every_declared_symbol():
     assert sorted(declared) == sorted(_cabi.EXPORTS)
     for name in declared:
         assert hasattr(lib, name), name
+        assert getattr(lib, name).argtypes is not None, name
     assert b"sm_90a" in lib.lg_build_info()
 
 
@@ -78,8 +79,12 @@ def test_ctypes_structs_match_the_header_layout(tmp_path):
     src = tmp_path / "layout.c"
     src.write_text(
         '#include <stdio.h>\n#include <stddef.h>\n#include "lightglue_b200.h"\n#include "superpoint_b200.h"\n'
+        '#include "aliked_b200.h"\n#include "sift_b200.h"\n'
         "int main(void) {\n"
         '  printf("%zu %zu %d ", sizeof(SpConfig), offsetof(SpConfig, detection_threshold), SP_ABI_VERSION);\n'
+        '  printf("%zu %zu %d ", sizeof(AlConfig), offsetof(AlConfig, detection_threshold), AL_ABI_VERSION);\n'
+        '  printf("%zu %zu %zu %d ", sizeof(SiftConfig), offsetof(SiftConfig, detection_threshold),\n'
+        '         offsetof(SiftConfig, edge_threshold), SIFT_ABI_VERSION);\n'
         '  printf("%zu %zu %zu %zu %zu %zu %zu %d\\n", sizeof(LgConfig), sizeof(LgInputs), sizeof(LgOutputs),\n'
         "         offsetof(LgInputs, pruning_threshold), offsetof(LgInputs, lens0), offsetof(LgInputs, lens1),\n"
         "         offsetof(LgOutputs, log_assignment), LG_ABI_VERSION);\n"
@@ -90,11 +95,56 @@ def test_ctypes_structs_match_the_header_layout(tmp_path):
     got = [int(v) for v in subprocess.check_output([str(exe)]).split()]
     want = [
         C.sizeof(_cabi.SpConfig), _cabi.SpConfig.detection_threshold.offset, _cabi.SP_ABI_VERSION,
+        C.sizeof(_cabi.AlConfig), _cabi.AlConfig.detection_threshold.offset, _cabi.AL_ABI_VERSION,
+        C.sizeof(_cabi.SiftConfig), _cabi.SiftConfig.detection_threshold.offset, _cabi.SiftConfig.edge_threshold.offset,
+        _cabi.SIFT_ABI_VERSION,
         C.sizeof(_cabi.LgConfig), C.sizeof(_cabi.LgInputs), C.sizeof(_cabi.LgOutputs),
         _cabi.LgInputs.pruning_threshold.offset, _cabi.LgInputs.lens0.offset, _cabi.LgInputs.lens1.offset,
         _cabi.LgOutputs.log_assignment.offset, _cabi.ABI_VERSION,
     ]
     assert got == want
+
+
+def test_extractor_handle_signature_covers_conf_parameters_and_device():
+    """The C handle is rebuilt whenever its signature changes: every conf value that reaches the config struct, the
+    identity and in-place version of every parameter and buffer, and the device."""
+    from lightglue_b200.aliked import ALIKED
+    from lightglue_b200.sift import SIFT
+    from lightglue_b200.superpoint import SuperPoint
+
+    dev = torch.device("cuda", 0)
+    sp = SuperPoint(weights=None)
+    sig = sp._signature(dev)
+    assert sp._signature(dev) == sig
+    assert sp._signature(torch.device("cuda", 1)) != sig
+    sp.convDa.bias.mul_(2)  # in-place change of a bias
+    assert sp._signature(dev) != sig
+    sig = sp._signature(dev)
+    sp.convPb.weight = torch.nn.Parameter(sp.convPb.weight.clone(), requires_grad=False)  # a new tensor, same values
+    assert sp._signature(dev) != sig
+    sig = sp._signature(dev)
+    sp.conf.max_num_keypoints = 100
+    assert sp._signature(dev) != sig
+    sig = sp._signature(dev)
+    sp.conf.precision = "fp32"
+    assert sp._signature(dev) != sig
+
+    al = ALIKED(weights=None)
+    sig = al._signature(dev)
+    al.block1.bn1.running_mean.add_(1)  # in-place change of a buffer
+    assert al._signature(dev) != sig
+    sig = al._signature(dev)
+    al.conf.detection_threshold = 0.5
+    assert al._signature(dev) != sig
+
+    s = SIFT()
+    sig = s._signature(dev)
+    s.conf.max_num_keypoints = 100
+    assert s._signature(dev) != sig
+    sig = s._signature(dev)
+    s.conf.edge_threshold = 12
+    assert s._signature(dev) != sig
+    assert s._signature(torch.device("cuda", 1)) != s._signature(dev)
 
 
 def test_ragged_padding_and_splitting_host_logic():

@@ -19,6 +19,7 @@ def test_header_symbols_equal_exports_and_are_exported():
     lib = _cabi.load()
     for s in _cabi.SIFT_EXPORTS:
         assert hasattr(lib, s), s
+        assert getattr(lib, s).argtypes is not None, s
 
 
 def test_conf_defaults_equal_the_reference():

@@ -83,6 +83,7 @@ def test_superpoint_header_symbols_are_exported_and_host_mirror_contract():
     assert sorted(declared) == sorted(_cabi.SP_EXPORTS)
     for name in declared:
         assert hasattr(lib, name), name
+        assert getattr(lib, name).argtypes is not None, name
     m = SuperPoint(weights=None, max_num_keypoints=512)
     assert lib.sp_weight_blob_floats() == m._blob().numel() == sum(p.numel() for p in m.parameters())
     ref_keys = {f"{n}.{s}" for n, *_ in LAYERS for s in ("weight", "bias")}  # superpoint.py:137-153
