@@ -55,7 +55,13 @@ struct TcLinParams {
   int conv_cb, conv_w2, conv_h, conv_w, relu;
   long conv_plane, conv_rows;
   int mma_n;  // N of the MMAs when fewer than 256 output columns exist (64 / 128; 0 = 256): the weight rows beyond are zero
+  // TMA stores of the staged epilogues, 64-row boxes (one MMA warpgroup's rows): TEPI_QKV: q, k ([S H Lp, 64], box 64 x 64)
+  // and vt ([S H 64, Lp], box 64 rows x 64 d); TEPI_RESID / F32 / CONV: out_f32 (box 16 x 64, also the residual's
+  // load map), out_h, out_l (box 16 x 64)
+  CUtensorMap out_map[3];
 };
+
+constexpr int STG_BOX = 8192;  // one staged output box: 64 rows x 128 bytes, or 16 fp32 + 2 x 16 bf16 columns of 64 rows
 
 template <int NSLOT>
 struct LinCfg {
@@ -64,8 +70,10 @@ struct LinCfg {
   static constexpr int STAGE_BYTES = A_TILE_BYTES + NSLOT * W_TILE_BYTES;
   static constexpr int THREADS = 384;
   static constexpr int MMA_WARPS = 8;
+  static constexpr int STG_BYTES = NSLOT == 1 ? 2 * 2 * STG_BOX : 0;     // two output boxes per MMA warpgroup
+  static constexpr int PAR_BYTES = NSLOT == 1 ? BN * 4 : 3 * 2 * BN * 4;  // the tile's bias / LayerNorm bias, gamma, beta
   static constexpr int RED_BYTES = NSLOT == 2 ? 2 * 2 * 64 * 4 : 0;  // LayerNorm: [pass][slot][row] partial sums
-  static constexpr int FIXED_BYTES = RED_BYTES + 1024 + 256;         // + alignment slack + barriers
+  static constexpr int FIXED_BYTES = STG_BYTES + PAR_BYTES + RED_BYTES + 1024 + 256;  // + alignment slack + barriers
   static constexpr int SMEM_MAX = 232448;                            // 227 KB per CTA
   static constexpr int FIT = (SMEM_MAX - FIXED_BYTES) / STAGE_BYTES;
   static constexpr int STAGES = FIT > 5 ? 5 : FIT;
@@ -95,6 +103,7 @@ __device__ __forceinline__ float gelu_erf(float y) {
   return fmaf(copysignf(erf_abs, y), hy, hy);
 }
 __device__ __forceinline__ void mma_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }  // the two MMA warpgroups
+__device__ __forceinline__ void wg_bar(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory"); }  // one of them
 
 struct TileInfo {
   int s, r0, n_tile, sel, len;
@@ -141,13 +150,19 @@ template <int NSLOT, int EPI>
 __global__ void __launch_bounds__(LinCfg<NSLOT>::THREADS, 1) tc_linear_kernel(const __grid_constant__ TcLinParams p) {
   using C = LinCfg<NSLOT>;
   constexpr int TBM = C::TBM, STAGES = C::STAGES, STAGE_BYTES = C::STAGE_BYTES;
+  // element-wise epilogues: results are staged in shared memory and written by TMA stores that drain while the next
+  // tile's MMAs run
+  constexpr bool STAGED = EPI == TEPI_QKV || EPI == TEPI_RESID || EPI == TEPI_F32 || EPI == TEPI_CONV;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // align by OFFSETTING the shared array (not by rebuilding a pointer from an integer): the compiler keeps the
   // shared address space and emits LDS / STS instead of generic LD / ST for everything derived from it
   uint8_t* smem = smem_raw + ((1024u - (static_cast<uint32_t>(reinterpret_cast<uintptr_t>(smem_raw)) & 1023u)) & 1023u);
-  float* s_red = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);  // LayerNorm: [pass][slot][64 rows]
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + C::RED_BYTES);
+  uint8_t* s_stg = smem + STAGES * STAGE_BYTES;                        // [MMA warpgroup][2 boxes of STG_BOX bytes]
+  float* s_par = reinterpret_cast<float*>(s_stg + C::STG_BYTES);      // tile bias [256] / LayerNorm b, gamma, beta [3][512]
+  float* s_red = reinterpret_cast<float*>(s_stg + C::STG_BYTES + C::PAR_BYTES);  // LayerNorm: [pass][slot][64 rows]
+  uint64_t* full = reinterpret_cast<uint64_t*>(s_stg + C::STG_BYTES + C::PAR_BYTES + C::RED_BYTES);
   uint64_t* empty = full + STAGES;
+  uint64_t* xfull = empty + STAGES;  // TEPI_RESID: [MMA warpgroup][box] the residual x has landed in the box
 
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
   const int n_tiles = p.n_tiles;
@@ -158,7 +173,10 @@ __global__ void __launch_bounds__(LinCfg<NSLOT>::THREADS, 1) tc_linear_kernel(co
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&p.a_hi[0]);
     tma_prefetch_desc(&p.w_hi);
+    if (STAGED)
+      for (int i = 0; i < 3; ++i) tma_prefetch_desc(&p.out_map[i]);
     for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], C::MMA_WARPS); }
+    for (int i = 0; i < 4; ++i) mbar_init(&xfull[i], 1);
     fence_barrier_init();
   }
   __syncthreads();
@@ -174,6 +192,9 @@ __global__ void __launch_bounds__(LinCfg<NSLOT>::THREADS, 1) tc_linear_kernel(co
       TileWalk<TBM> walk(total_tiles, n_tiles);
       TileInfo ti;
       while (walk.next(p, ti)) {
+        if (EPI == TEPI_RESID)  // the epilogue's residual (x does not fit in L2) comes from HBM while the MMAs run
+          for (int c = 0; c < 2 * BN / 16; ++c)
+            tma_prefetch_l2_2d(&p.out_map[0], ti.n_tile * BN + (c % 16) * 16, (int)ti.grow0 + (c / 16) * 64);
         for (int it = 0; it < iters; ++it, ++g) {
           const int stage = g % STAGES, round = g / STAGES;
           mbar_wait(&empty[stage], (round & 1) ^ 1, p.dbg, 17, it);
@@ -216,11 +237,42 @@ __global__ void __launch_bounds__(LinCfg<NSLOT>::THREADS, 1) tc_linear_kernel(co
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty[stage]);
   };
+  const int mt = threadIdx.x - 128;                // 0 .. 255 over the MMA warpgroups
+  const bool issuer = (threadIdx.x & 127) == 0;   // issues this warpgroup's TMA stores (and residual loads)
+  const int rw = wq * 16 + tr;                      // box row of registers 4 j, 4 j + 1 (+8: 4 j + 2, 4 j + 3)
+  uint8_t* stg = s_stg + wg * 2 * STG_BOX;
+  uint64_t* xf = xfull + 2 * wg;
+  uint32_t u = 0;  // boxes this warpgroup has staged: box u uses buffer u & 1
+  // output columns the staged epilogues write
+  const int ocols = EPI == TEPI_QKV ? n_tiles * BN
+                    : EPI == TEPI_CONV ? p.ldb
+                                       : max(p.ldo, p.out_h != nullptr ? p.ldb : 0);
+  if (EPI == TEPI_LN_GELU) {  // bias, gamma, beta of the 512 LayerNorm columns: the same for every tile
+    for (int i = mt; i < 2 * BN; i += 256) {
+      s_par[i] = p.bias[i]; s_par[2 * BN + i] = p.ln_g[i]; s_par[4 * BN + i] = p.ln_b[i];
+    }
+    mma_bar();
+  }
   int g = 0;
   float acc[128];
   TileWalk<TBM> walk(total_tiles, n_tiles);
   TileInfo ti;
   while (walk.next(p, ti)) {
+    // TEPI_RESID: TMA load of the residual x (16 columns of this warpgroup's 64 rows) into buffer v & 1
+    auto load_x = [&](uint32_t v, int box) {
+      mbar_arrive_expect_tx(&xf[v & 1], 64 * 16 * 4);
+      tma_load_2d(stg + (v & 1) * STG_BOX, &p.out_map[0], ti.n_tile * BN + box * 16, (int)ti.grow0 + wg * 64, &xf[v & 1]);
+    };
+    float bias_r = 0.f;  // bias of column mt of this tile, moved to shared memory after the main loop
+    if (STAGED) {
+      const int col = ti.n_tile * BN + mt;
+      if (col < ocols) bias_r = __ldg(p.bias + (p.w_select == 1 ? (long)ti.sel * p.bias_sel_stride : 0) + col);
+    }
+    if (EPI == TEPI_RESID && issuer) {  // the first two boxes of x land while the MMAs run
+      bulk_wait_read<0>();
+      load_x(u, 0);
+      load_x(u + 1, 1);
+    }
 #pragma unroll
     for (int i = 0; i < 128; ++i) acc[i] = 0.f;
     int prev = -1;
@@ -250,16 +302,21 @@ __global__ void __launch_bounds__(LinCfg<NSLOT>::THREADS, 1) tc_linear_kernel(co
     wgmma_wait<0>();
     fence_regs(acc);
     if (prev >= 0) release(prev);
+    if (STAGED) {  // both warpgroups are done with the previous tile's bias
+      mma_bar();
+      s_par[mt] = bias_r;
+      mma_bar();
+    }
 
     if (EPI == TEPI_LN_GELU) {
       // ---------------------------------------------------------------- LayerNorm(512) + GELU
       // Every row of the tile lies in one quad of lanes per warpgroup (256 columns each): quad shuffles give the
       // warpgroup's share, shared memory merges the two slots.  Two-pass statistics (mean, then squared deviations).
-      const float* bias = p.bias + wg * BN;
+      const float* bias = s_par + wg * BN;
       float sum[2] = {0.f, 0.f};
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
-        const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + 8 * j + 2 * tq));
+        const float2 bb = *reinterpret_cast<const float2*>(bias + 8 * j + 2 * tq);
 #pragma unroll
         for (int hr = 0; hr < 2; ++hr) {
           acc[4 * j + 2 * hr] += bb.x; acc[4 * j + 2 * hr + 1] += bb.y;
@@ -303,8 +360,8 @@ __global__ void __launch_bounds__(LinCfg<NSLOT>::THREADS, 1) tc_linear_kernel(co
 #pragma unroll
         for (int j = 0; j < 32; ++j) {
           const int c = 8 * j + 2 * tq;
-          const float2 gg = __ldg(reinterpret_cast<const float2*>(p.ln_g + wg * BN + c));
-          const float2 be = __ldg(reinterpret_cast<const float2*>(p.ln_b + wg * BN + c));
+          const float2 gg = *reinterpret_cast<const float2*>(s_par + 2 * BN + wg * BN + c);
+          const float2 be = *reinterpret_cast<const float2*>(s_par + 4 * BN + wg * BN + c);
           const float a = gelu_erf(fmaf((acc[4 * j + 2 * hr] - mean[hr]) * rstd[hr], gg.x, be.x));
           const float b = gelu_erf(fmaf((acc[4 * j + 2 * hr + 1] - mean[hr]) * rstd[hr], gg.y, be.y));
           const uint32_t hi = pack_bf16x2(a, b);
@@ -387,84 +444,151 @@ __global__ void __launch_bounds__(LinCfg<NSLOT>::THREADS, 1) tc_linear_kernel(co
       continue;
     }
 
-    // ------------------------------------------------------------------ element-wise epilogues
-    const float* bias = p.bias + (p.w_select == 1 ? (long)ti.sel * p.bias_sel_stride : 0) + ti.n_tile * BN;
-    // which output a QKV tile feeds: packed channel order [q | k | v] (self) or [qk | v] (cross)
-    const int which = ti.n_tile;
-    const bool qkv_v = EPI == TEPI_QKV && (p.rope ? which == 2 : which == 1);
-    const bool use_rope = EPI == TEPI_QKV && p.rope && !qkv_v;
+    // ------------------------------------------------------------------ element-wise epilogues, staged
+    // Each warpgroup writes its 64 rows into shared-memory boxes laid out as their TMA store maps declare them (128 / 64
+    // / 32-byte swizzle: the fragment writes are free of bank conflicts); its issuer thread stores a box once every
+    // writer has fenced it, and a box is rewritten only after the store that read it two boxes earlier has finished
+    // reading.  Box loops are unrolled so that the accumulators stay in registers.
+    auto claim = [&]() {  // the next box: the store that last read its buffer is done with it
+      if (issuer) bulk_wait_read<1>();
+      wg_bar(wg);
+      return stg + (u & 1) * STG_BOX;
+    };
+    auto publish = [&]() {  // the box is complete: hand it to the TMA engine
+      fence_proxy_async();
+      wg_bar(wg);
+    };
+    const int row0 = (int)ti.grow0 + wg * 64;  // first row of this warpgroup's boxes
+    if (EPI == TEPI_QKV) {
+      // which output a QKV tile feeds: packed channel order [q | k | v] (self) or [qk | v] (cross)
+      const int which = ti.n_tile;
+      const bool qkv_v = p.rope ? which == 2 : which == 1;
+      const bool use_rope = p.rope && !qkv_v;
+      // RoPE cos / sin of the two rows, loaded before the stores; frequency index d / 2 = 4 (j % 8) + tq, the same for
+      // every head
+      float rc[2][8], rs[2][8];
+      if (use_rope) {
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr)
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const long grow = ti.grow0 + rl_a + 8 * hr;
+            rc[hr][jj] = __ldg(p.cs + grow * 64 + 4 * jj + tq);
+            rs[hr][jj] = __ldg(p.cs + grow * 64 + 32 + 4 * jj + tq);
+          }
+      }
+#pragma unroll
+      for (int hh = 0; hh < BN / LG_HDIM; ++hh) {  // one box per head
+        uint8_t* box = claim();
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          const int row = rw + 8 * hr;
+          const bool live = ti.r0 + wg * 64 + row < ti.len;
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const int j = 8 * hh + jj, d = 8 * jj + 2 * tq;
+            const float2 bb = *reinterpret_cast<const float2*>(s_par + 8 * j + 2 * tq);
+            float v0 = acc[4 * j + 2 * hr] + bb.x, v1 = acc[4 * j + 2 * hr + 1] + bb.y;
+            if (qkv_v) {
+              // V is stored transposed [S, H, 64, Lp] (K-major B operand of P*V); box [64 d][64 rows].  Padding rows
+              // are written as zeros: attention multiplies them by P = 0, which stays 0 whatever x held there.
+              if (!live) v0 = v1 = 0.f;
+              *reinterpret_cast<__half*>(box + swz(d * 128 + row * 2, 0x70)) = __float2half_rn(v0);
+              *reinterpret_cast<__half*>(box + swz((d + 1) * 128 + row * 2, 0x70)) = __float2half_rn(v1);
+              continue;
+            }
+            if (use_rope) {  // rotary embedding on q / k (lightglue.py:58-65, 168-169); freq index = d / 2
+              const float c = rc[hr][jj], s = rs[hr][jj];
+              const float a = v0, b = v1;
+              v0 = a * c - b * s;
+              v1 = b * c + a * s;
+            }
+            *reinterpret_cast<__half2*>(box + swz(row * 128 + d * 2, 0x70)) = __floats2half2_rn(v0, v1);  // [64 rows][64 d]
+          }
+        }
+        publish();
+        if (issuer) {
+          const int bh = ti.s * LG_HEADS + hh;
+          if (qkv_v) tma_store_2d(&p.out_map[2], box, ti.r0 + wg * 64, bh * LG_HDIM);
+          else tma_store_2d(&p.out_map[which], box, 0, bh * p.st.Lp + ti.r0 + wg * 64);
+          bulk_commit();
+        }
+        ++u;
+      }
+      continue;
+    }
+
+    // bias (* scale) (+ ReLU) (+ residual) -> fp32 and / or bf16 hi (/ lo); boxes of 16 columns: fp32 [64][16] (64-byte
+    // swizzle) at 0, hi / lo [64][16] (32-byte swizzle) at 4096 / 6144.  Map bounds clip the columns >= ldo / ldb and the
+    // rows >= S Lp.
     const bool f32out = EPI == TEPI_RESID || EPI == TEPI_F32;
     const bool has16 = EPI == TEPI_CONV || EPI == TEPI_RESID || (EPI == TEPI_F32 && p.out_h != nullptr);
     const bool haslo = has16 && p.out_l != nullptr;
+    const int nbox = (min(BN, ocols - ti.n_tile * BN) + 15) / 16;
+    bool inside[2] = {true, true};
+    if (EPI == TEPI_CONV) {  // the padding pixels of the NHWC image stay zero for the next layer's taps
 #pragma unroll
-    for (int hr = 0; hr < 2; ++hr) {
-      const int rl = rl_a + 8 * hr;
-      const int r = ti.r0 + rl;
-      const long grow = ti.grow0 + rl;
-      const bool live = r < ti.len;
-      bool inside = true;
-      if (EPI == TEPI_CONV) {  // the padding pixels of the NHWC image stay zero for the next layer's taps
+      for (int hr = 0; hr < 2; ++hr) {
+        const long grow = ti.grow0 + rl_a + 8 * hr;
         const long pp = grow % p.conv_plane;
         const int yy = (int)(pp / p.conv_w2), xx = (int)(pp % p.conv_w2);
-        inside = grow < p.conv_rows && yy >= 1 && yy <= p.conv_h && xx >= 1 && xx <= p.conv_w;
-      }
-      // RoPE cos / sin of this row, loaded ahead of its stores (the compiler does not move a load above a store it cannot
-      // prove independent, so a load per column would pay its full latency every time); frequency index d / 2 =
-      // 4 (j % 8) + tq, the same for every head
-      float rc[8], rs[8];
-      if (use_rope) {
-#pragma unroll
-        for (int jj = 0; jj < 8; ++jj) {
-          rc[jj] = __ldg(p.cs + grow * 64 + 4 * jj + tq);
-          rs[jj] = __ldg(p.cs + grow * 64 + 32 + 4 * jj + tq);
-        }
-      }
-#pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        const int tcol = 8 * j + 2 * tq;        // column inside the tile (even)
-        const int col = ti.n_tile * BN + tcol;  // output channel
-        if (EPI == TEPI_CONV && col >= p.ldb) continue;  // Cout < 256: the weight rows beyond it are zero padding
-        const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + tcol));
-        float v0 = acc[4 * j + 2 * hr] + bb.x, v1 = acc[4 * j + 2 * hr + 1] + bb.y;
-        if (EPI == TEPI_QKV) {
-          const int hh = tcol / LG_HDIM, d = tcol % LG_HDIM;
-          if (qkv_v) {
-            // V is stored transposed [S, H, 64, Lp] (K-major B operand of P*V)
-            if (live) {
-              __half* dst = p.vt + (((long)ti.s * LG_HEADS + hh) * LG_HDIM + d) * p.st.Lp + r;
-              dst[0] = __float2half_rn(v0);
-              dst[p.st.Lp] = __float2half_rn(v1);
-            }
-            continue;
-          }
-          if (use_rope) {  // rotary embedding on q / k (lightglue.py:58-65, 168-169); freq index = d / 2
-            const float c = rc[j % 8], s = rs[j % 8];
-            const float a = v0, b = v1;
-            v0 = a * c - b * s;
-            v1 = b * c + a * s;
-          }
-          __half* dst = (which == 0 ? p.q : p.k) + (((long)ti.s * LG_HEADS + hh) * p.st.Lp + r) * LG_HDIM + d;
-          *reinterpret_cast<__half2*>(dst) = __floats2half2_rn(v0, v1);
-          continue;
-        }
-        if (p.scale != 1.f) { v0 *= p.scale; v1 *= p.scale; }
-        if (EPI == TEPI_CONV) {
-          v0 = inside ? ((p.relu && v0 < 0.f) ? 0.f : v0) : 0.f;
-          v1 = inside ? ((p.relu && v1 < 0.f) ? 0.f : v1) : 0.f;
-        }
-        if (EPI == TEPI_RESID) {  // x + ffn(...) (lightglue.py:172 / 228-229)
-          const float2 xr = *reinterpret_cast<const float2*>(p.out_f32 + grow * p.ldo + col);
-          v0 += xr.x; v1 += xr.y;
-        }
-        if (f32out && col < p.ldo) *reinterpret_cast<float2*>(p.out_f32 + grow * p.ldo + col) = make_float2(v0, v1);
-        if (has16 && col < p.ldb) {
-          const uint32_t hi = pack_bf16x2(v0, v1);
-          *reinterpret_cast<uint32_t*>(p.out_h + grow * p.ldb + col) = hi;
-          if (haslo) *reinterpret_cast<uint32_t*>(p.out_l + grow * p.ldb + col) = pack_bf16x2_lo(v0, v1, hi);
-        }
+        inside[hr] = grow < p.conv_rows && yy >= 1 && yy <= p.conv_h && xx >= 1 && xx <= p.conv_w;
       }
     }
+#pragma unroll
+    for (int bx = 0; bx < BN / 16; ++bx) {
+      if (bx >= nbox) break;
+      uint8_t* box;
+      if (EPI == TEPI_RESID) {  // x of this box, loaded two boxes ahead
+        box = stg + (u & 1) * STG_BOX;
+        mbar_wait(&xf[u & 1], (u >> 1) & 1, p.dbg, 19, bx);
+      } else {
+        box = claim();
+      }
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
+        const int row = rw + 8 * hr;
+#pragma unroll
+        for (int jl = 0; jl < 2; ++jl) {
+          const int j = 2 * bx + jl, c = 8 * jl + 2 * tq;  // accumulator column pair, column inside the box
+          const float2 bb = *reinterpret_cast<const float2*>(s_par + 8 * j + 2 * tq);
+          float v0 = acc[4 * j + 2 * hr] + bb.x, v1 = acc[4 * j + 2 * hr + 1] + bb.y;
+          if (p.scale != 1.f) { v0 *= p.scale; v1 *= p.scale; }
+          if (EPI == TEPI_CONV) {
+            v0 = inside[hr] ? ((p.relu && v0 < 0.f) ? 0.f : v0) : 0.f;
+            v1 = inside[hr] ? ((p.relu && v1 < 0.f) ? 0.f : v1) : 0.f;
+          }
+          float2* px = reinterpret_cast<float2*>(box + swz(row * 64 + c * 4, 0x30));
+          if (EPI == TEPI_RESID) {  // x + ffn(...) (lightglue.py:172 / 228-229)
+            const float2 xr = *px;
+            v0 += xr.x; v1 += xr.y;
+          }
+          if (f32out) *px = make_float2(v0, v1);
+          if (has16) {
+            const uint32_t o = swz(row * 32 + c * 2, 0x10);
+            const uint32_t hi = pack_bf16x2(v0, v1);
+            *reinterpret_cast<uint32_t*>(box + 4096 + o) = hi;
+            if (haslo) *reinterpret_cast<uint32_t*>(box + 6144 + o) = pack_bf16x2_lo(v0, v1, hi);
+          }
+        }
+      }
+      publish();
+      if (issuer) {
+        const int col = ti.n_tile * BN + bx * 16;
+        if (f32out) tma_store_2d(&p.out_map[0], box, col, row0);
+        if (has16) tma_store_2d(&p.out_map[1], box + 4096, col, row0);
+        if (haslo) tma_store_2d(&p.out_map[2], box + 6144, col, row0);
+        bulk_commit();
+        if (EPI == TEPI_RESID && bx + 2 < nbox) {  // the buffer's next box: once this store has read it
+          bulk_wait_read<0>();
+          load_x(u, bx + 2);
+        }
+      }
+      ++u;
+    }
   }
+  // the stores must be complete (not only read) when the grid ends: the next kernel's griddepcontrol.wait relies on it
+  if (STAGED && issuer) bulk_wait_all();
 }
 
 // fp32 -> bf16 hi (/ lo) for rows < len
@@ -568,6 +692,23 @@ int tc_gemm(TcEngine& e, const SeqState& st, const TcOperands& d, int n_tiles, T
   if ((r = wmap(&p.w_hi, d.wh))) return r;
   p.w_lo = p.w_hi;
   if (e.x3 && (r = wmap(&p.w_lo, d.wl))) return r;
+  // output maps of the staged epilogues (64-row boxes)
+  if (p.epi == TEPI_QKV) {
+    const uint64_t sh = (uint64_t)st.S * LG_HEADS;
+    if ((r = tc_tmap(e, {p.q, 2, {LG_HDIM, sh * st.Lp}, {LG_HDIM * 2}, {LG_HDIM, 64}}, &p.out_map[0]))) return r;
+    if ((r = tc_tmap(e, {p.k, 2, {LG_HDIM, sh * st.Lp}, {LG_HDIM * 2}, {LG_HDIM, 64}}, &p.out_map[1]))) return r;
+    if ((r = tc_tmap(e, {p.vt, 2, {(uint64_t)st.Lp, sh * LG_HDIM}, {(uint64_t)st.Lp * 2}, {64, LG_HDIM}}, &p.out_map[2])))
+      return r;
+  } else if (p.epi == TEPI_RESID || p.epi == TEPI_F32 || p.epi == TEPI_CONV) {
+    const uint64_t ldo = p.ldo, ldb = p.ldb;
+    if (p.out_f32 && (r = tc_tmap(e, {p.out_f32, 2, {ldo, rows}, {ldo * 4}, {16, 64}, CU_TENSOR_MAP_SWIZZLE_64B,
+                                      CU_TENSOR_MAP_DATA_TYPE_FLOAT32}, &p.out_map[0])))
+      return r;
+    const __nv_bfloat16* o16[2] = {p.out_h, p.out_l};
+    for (int i = 0; i < 2; ++i)
+      if (o16[i] && (r = tc_tmap(e, {o16[i], 2, {ldb, rows}, {ldb * 2}, {16, 64}, CU_TENSOR_MAP_SWIZZLE_32B}, &p.out_map[1 + i])))
+        return r;
+  }
   p.kb_total = (int)(K / BK);
   p.kb0 = d.k1 ? d.k0 / BK : p.kb_total;
   p.passes = e.x3 ? 3 : 1;

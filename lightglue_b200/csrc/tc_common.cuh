@@ -78,6 +78,27 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
       "l"(m), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
+// TMA store of a shared-memory box to global memory (rows / columns outside the map's bounds are not written), tracked
+// by the issuing thread's bulk async-groups
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* smem_src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(m),
+               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's bulk groups still read their shared-memory source
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// every bulk group of this thread has completed: its writes are visible in global memory
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// orders this thread's generic-proxy shared-memory writes before later TMA (async-proxy) reads of them
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void tma_prefetch_l2_2d(const CUtensorMap* m, int c0, int c1) {
+  asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global [%0, {%1, %2}];" ::"l"(m), "r"(c0), "r"(c1) : "memory");
+}
+// byte offset `off` inside a box written by TMA with the 32 / 64 / 128-byte swizzle (mask 0x10 / 0x30 / 0x70): the
+// 16-byte chunk index is XORed with the address bits 7.. (the box must start on a 256 / 512 / 1024-byte boundary)
+__device__ __forceinline__ uint32_t swz(uint32_t off, uint32_t mask) { return off ^ ((off >> 3) & mask); }
 
 // Programmatic dependent launch (kernels launched with cudaLaunchAttributeProgrammaticStreamSerialization):
 // `pdl_launch_dependents` lets the next kernel of the stream become resident as SMs drain, `pdl_wait` blocks until
