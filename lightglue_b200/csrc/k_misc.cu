@@ -6,6 +6,9 @@
 #include <cuda_fp16.h>
 
 #include "lg_internal.h"
+#include "tc_common.cuh"
+
+using tc::cluster_sync_all;
 
 // ------------------------------------------------------------------------------------------------
 // normalize_keypoints (31-43) + LearnableFourierPositionalEncoding (76-81)
@@ -681,10 +684,6 @@ __global__ void __launch_bounds__(256) assign_term_kernel(AssignArgs a, SeqState
 //   phase C (CTA 0)     ordered compaction into the `matches` / `scores` lists
 // cluster barriers (release/acquire at cluster scope) order the global-memory hand-offs between the phases.
 constexpr int TAIL_CLUSTER = 8;
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
 __global__ void __cluster_dims__(TAIL_CLUSTER, 1, 1) __launch_bounds__(1024)
 assign_tail_kernel(AssignArgs a, SeqState st, const float* __restrict__ part, const int* __restrict__ part_arg, int pstride,
                    int slot_cols) {

@@ -11,8 +11,9 @@
 // * fused epilogues: bias (+ RoPE, head split, V transpose) for the QKV projections, bias + LayerNorm(512) + exact
 //   GELU for ffn.0, bias + residual for ffn.3, bias * scale for input_proj / final_proj, the row reductions of the
 //   assignment's similarity sweeps, bias + ReLU for the SuperPoint convolutions.
-// Tiles: 128 rows x 256 columns, MMA warpgroup g owns rows 64 g .. +63; the LayerNorm variant: 64 rows x 512 columns,
-// MMA warpgroup g owns the 256-column slot g and the row statistics are merged through shared memory.
+// Tiles: 128 rows x 256 columns, MMA warpgroup g owns rows 64 g .. +63.  The LayerNorm variant runs in clusters of two
+// CTAs: a cluster owns a 128-row tile of all 512 columns, CTA rank r columns 256 r .. +255, and the two CTAs exchange
+// their row partial sums through distributed shared memory.
 // Threads: 384 = producer warpgroup (warp 0 issues the TMA loads; the warpgroup hands its registers to the others)
 // + 2 MMA warpgroups.
 #include <map>
@@ -56,23 +57,28 @@ struct TcLinParams {
   long conv_plane, conv_rows;
   int mma_n;  // N of the MMAs when fewer than 256 output columns exist (64 / 128; 0 = 256): the weight rows beyond are zero
   // TMA stores of the staged epilogues, 64-row boxes (one MMA warpgroup's rows): TEPI_QKV: q, k ([S H Lp, 64], box 64 x 64)
-  // and vt ([S H 64, Lp], box 64 rows x 64 d); TEPI_RESID / F32 / CONV: out_f32 (box 16 x 64, also the residual's
-  // load map), out_h, out_l (box 16 x 64)
+  // and vt ([S H 64, Lp], box 64 rows x 64 d); TEPI_RESID / F32 / CONV / LN_GELU: out_f32 (box 16 x 64, also the
+  // residual's load map), out_h, out_l (box 16 x 64)
   CUtensorMap out_map[3];
 };
 
-constexpr int STG_BOX = 8192;  // one staged output box: 64 rows x 128 bytes, or 16 fp32 + 2 x 16 bf16 columns of 64 rows
+constexpr int TBM = 128;  // rows per tile
 
-template <int NSLOT>
+template <int EPI>
 struct LinCfg {
-  static constexpr int TBM = NSLOT == 1 ? 128 : 64;     // rows per tile
+  static constexpr bool LN = EPI == TEPI_LN_GELU;
+  static constexpr int CLUSTER = LN ? 2 : 1;  // CTAs per 128-row tile: the LayerNorm needs all 512 columns of a row
   static constexpr int A_TILE_BYTES = TBM * BK * 2;
-  static constexpr int STAGE_BYTES = A_TILE_BYTES + NSLOT * W_TILE_BYTES;
+  static constexpr int STAGE_BYTES = A_TILE_BYTES + W_TILE_BYTES;
   static constexpr int THREADS = 384;
   static constexpr int MMA_WARPS = 8;
-  static constexpr int STG_BYTES = NSLOT == 1 ? 2 * 2 * STG_BOX : 0;     // two output boxes per MMA warpgroup
-  static constexpr int PAR_BYTES = NSLOT == 1 ? BN * 4 : 3 * 2 * BN * 4;  // the tile's bias / LayerNorm bias, gamma, beta
-  static constexpr int RED_BYTES = NSLOT == 2 ? 2 * 2 * 64 * 4 : 0;  // LayerNorm: [pass][slot][row] partial sums
+  // one staged output box: 64 rows x 128 bytes, or 16 fp32 + 2 x 16 bf16 columns of 64 rows; LayerNorm: 2 x 16 bf16
+  // columns (hi / lo), which leaves room for a 4-stage ring
+  static constexpr int STG_BOX = LN ? 4096 : 8192;
+  static constexpr int H16 = LN ? 0 : 4096;  // offset of the bf16 hi image in a box (lo: + 2048)
+  static constexpr int STG_BYTES = 2 * 2 * STG_BOX;  // two output boxes per MMA warpgroup
+  static constexpr int PAR_BYTES = (LN ? 3 : 1) * BN * 4;  // the tile's bias / LayerNorm bias, gamma, beta
+  static constexpr int RED_BYTES = LN ? 2 * TBM * 4 : 0;  // LayerNorm: [pass][row] the peer CTA's row partial sums
   static constexpr int FIXED_BYTES = STG_BYTES + PAR_BYTES + RED_BYTES + 1024 + 256;  // + alignment slack + barriers
   static constexpr int SMEM_MAX = 232448;                            // 227 KB per CTA
   static constexpr int FIT = (SMEM_MAX - FIXED_BYTES) / STAGE_BYTES;
@@ -110,7 +116,6 @@ struct TileInfo {
   long grow0;
 };
 // decode tile t (n-tile fastest, so neighbouring CTAs share A tiles in L2); returns false for tiles with nothing to do
-template <int TBM>
 __device__ __forceinline__ bool decode_tile(const TcLinParams& p, int t, int n_tiles, TileInfo& ti) {
   const int tiles_per_seq = p.st.Lp / TBM;
   ti.n_tile = t % n_tiles;
@@ -131,43 +136,49 @@ __device__ __forceinline__ bool decode_tile(const TcLinParams& p, int t, int n_t
   return live;
 }
 
-// Persistent tile schedule: CTA c walks tiles c, c + grid, ... (skipping tiles with nothing to do)
-template <int TBM>
+// Persistent tile schedule: CTA c walks tiles c, c + grid, ... (skipping tiles with nothing to do).  In clusters of CL
+// CTAs (n_tiles == CL), cluster c walks the row tiles c, c + grid / CL, ... and CTA rank r takes column tile r of each.
+template <int CL>
 struct TileWalk {
-  int cur, step, end, n_tiles;
-  __device__ TileWalk(int total_tiles, int n_tiles_) : cur(blockIdx.x), step(gridDim.x), end(total_tiles), n_tiles(n_tiles_) {}
+  int cur, step, end, n_tiles, rank;
+  __device__ TileWalk(int total_tiles, int n_tiles_, int rank_)
+      : cur(blockIdx.x / CL), step(gridDim.x / CL), end(total_tiles / CL), n_tiles(n_tiles_), rank(rank_) {}
   __device__ bool next(const TcLinParams& p, TileInfo& ti) {
     while (cur < end) {
-      const int id = p.reverse ? end - 1 - cur : cur;
+      const int id = (p.reverse ? end - 1 - cur : cur) * CL + rank;
       cur += step;
-      if (decode_tile<TBM>(p, id, n_tiles, ti)) return true;
+      if (decode_tile(p, id, n_tiles, ti)) return true;
     }
     return false;
   }
 };
 
-template <int NSLOT, int EPI>
-__global__ void __launch_bounds__(LinCfg<NSLOT>::THREADS, 1) tc_linear_kernel(const __grid_constant__ TcLinParams p) {
-  using C = LinCfg<NSLOT>;
-  constexpr int TBM = C::TBM, STAGES = C::STAGES, STAGE_BYTES = C::STAGE_BYTES;
+template <int EPI>
+__global__ void __launch_bounds__(LinCfg<EPI>::THREADS, 1) tc_linear_kernel(const __grid_constant__ TcLinParams p) {
+  using C = LinCfg<EPI>;
+  constexpr int STAGES = C::STAGES, STAGE_BYTES = C::STAGE_BYTES, STG_BOX = C::STG_BOX;
+  constexpr bool LN = C::LN;
   // element-wise epilogues: results are staged in shared memory and written by TMA stores that drain while the next
   // tile's MMAs run
-  constexpr bool STAGED = EPI == TEPI_QKV || EPI == TEPI_RESID || EPI == TEPI_F32 || EPI == TEPI_CONV;
+  constexpr bool STAGED = EPI == TEPI_QKV || EPI == TEPI_RESID || EPI == TEPI_F32 || EPI == TEPI_CONV || LN;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // align by OFFSETTING the shared array (not by rebuilding a pointer from an integer): the compiler keeps the
-  // shared address space and emits LDS / STS instead of generic LD / ST for everything derived from it
+  // shared address space and emits LDS / STS instead of generic LD / ST for everything derived from it.  The offset is
+  // the same in both CTAs of a cluster, so a shared address maps to the same variable in the peer (mapa).
   uint8_t* smem = smem_raw + ((1024u - (static_cast<uint32_t>(reinterpret_cast<uintptr_t>(smem_raw)) & 1023u)) & 1023u);
   uint8_t* s_stg = smem + STAGES * STAGE_BYTES;                        // [MMA warpgroup][2 boxes of STG_BOX bytes]
-  float* s_par = reinterpret_cast<float*>(s_stg + C::STG_BYTES);      // tile bias [256] / LayerNorm b, gamma, beta [3][512]
-  float* s_red = reinterpret_cast<float*>(s_stg + C::STG_BYTES + C::PAR_BYTES);  // LayerNorm: [pass][slot][64 rows]
+  float* s_par = reinterpret_cast<float*>(s_stg + C::STG_BYTES);      // tile bias [256] / LayerNorm b, gamma, beta [3][256]
+  float* s_red = reinterpret_cast<float*>(s_stg + C::STG_BYTES + C::PAR_BYTES);  // LayerNorm: [pass][128 rows]
   uint64_t* full = reinterpret_cast<uint64_t*>(s_stg + C::STG_BYTES + C::PAR_BYTES + C::RED_BYTES);
   uint64_t* empty = full + STAGES;
   uint64_t* xfull = empty + STAGES;  // TEPI_RESID: [MMA warpgroup][box] the residual x has landed in the box
+  uint64_t* lnbar = xfull + 4;       // LayerNorm: [MMA warpgroup][pass] the peer's partial sums have landed in s_red
 
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
   const int n_tiles = p.n_tiles;
   const int total_tiles = n_tiles * p.st.S * (p.st.Lp / TBM);
   const int iters = p.passes * p.kb_total;  // ring iterations per tile: (pass, K block)
+  const uint32_t rank = C::CLUSTER > 1 ? cluster_ctarank() : 0;
 
   pdl_launch_dependents();  // the next kernel's CTAs may take this SM as soon as this CTA has left it
   if (threadIdx.x == 0) {
@@ -177,9 +188,14 @@ __global__ void __launch_bounds__(LinCfg<NSLOT>::THREADS, 1) tc_linear_kernel(co
       for (int i = 0; i < 3; ++i) tma_prefetch_desc(&p.out_map[i]);
     for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], C::MMA_WARPS); }
     for (int i = 0; i < 4; ++i) mbar_init(&xfull[i], 1);
+    if (LN)  // one arrival per row-owning lane (lane % 4 == 0) of the peer's warpgroup
+      for (int i = 0; i < 4; ++i) mbar_init(&lnbar[i], 32);
     fence_barrier_init();
   }
-  __syncthreads();
+  // LayerNorm: the peer writes into this CTA's shared memory and arrives on its barriers only once both CTAs have
+  // initialised theirs.  Every thread of every CTA reaches this barrier, whether or not its cluster gets a tile.
+  if (C::CLUSTER > 1) cluster_sync_all();
+  else __syncthreads();
   // everything above overlapped the tail of the previous kernel; activations, lengths and stop flags are only read
   // from here on
   pdl_wait();
@@ -189,7 +205,7 @@ __global__ void __launch_bounds__(LinCfg<NSLOT>::THREADS, 1) tc_linear_kernel(co
     regs_dec<40>();
     if (warp == 0 && elect_one()) {
       int g = 0;  // global k-block counter across tiles (ring position)
-      TileWalk<TBM> walk(total_tiles, n_tiles);
+      TileWalk<C::CLUSTER> walk(total_tiles, n_tiles, rank);
       TileInfo ti;
       while (walk.next(p, ti)) {
         if (EPI == TEPI_RESID)  // the epilogue's residual (x does not fit in L2) comes from HBM while the MMAs run
@@ -214,12 +230,13 @@ __global__ void __launch_bounds__(LinCfg<NSLOT>::THREADS, 1) tc_linear_kernel(co
           }
           mbar_arrive_expect_tx(&full[stage], STAGE_BYTES);
           tma_load_2d(sa, a_lo ? &p.a_lo[seg] : &p.a_hi[seg], kc, arow, &full[stage]);
-#pragma unroll
-          for (int sl_ = 0; sl_ < NSLOT; ++sl_)
-            tma_load_3d(sa + C::A_TILE_BYTES + sl_ * W_TILE_BYTES, w_lo ? &p.w_lo : &p.w_hi, kb * BK,
-                        (ti.n_tile * NSLOT + sl_) * BN, ti.sel, &full[stage]);
+          tma_load_3d(sa + C::A_TILE_BYTES, w_lo ? &p.w_lo : &p.w_hi, kb * BK, ti.n_tile * BN, ti.sel, &full[stage]);
         }
       }
+    }
+    if (C::CLUSTER > 1) {  // the exit barrier (below): the peer may still write into this CTA's shared memory
+      __syncwarp();
+      cluster_sync_all();
     }
     return;
   }
@@ -229,10 +246,10 @@ __global__ void __launch_bounds__(LinCfg<NSLOT>::THREADS, 1) tc_linear_kernel(co
   const int wg = warp / 4 - 1;   // MMA warpgroup 0 / 1
   const int wq = warp % 4;       // warp inside it: accumulator rows 16 wq .. +15
   const int tq = lane & 3, tr = lane >> 2;
-  const uint32_t a_off = NSLOT == 1 ? wg * 64 * 128 : 0;                                   // this warpgroup's 64 A rows
-  const uint32_t b_off = C::A_TILE_BYTES + (NSLOT == 2 ? wg * W_TILE_BYTES : 0);          // and its W slot
+  const uint32_t a_off = wg * 64 * 128;  // this warpgroup's 64 A rows
+  const uint32_t b_off = C::A_TILE_BYTES;
   const int mma_n = p.mma_n ? p.mma_n : BN;
-  const int rl_a = (NSLOT == 1 ? wg * 64 : 0) + wq * 16 + tr;  // tile row of accumulator registers 4 j, 4 j + 1 (+8: 4 j + 2, 4 j + 3)
+  const int rl_a = wg * 64 + wq * 16 + tr;  // tile row of accumulator registers 4 j, 4 j + 1 (+8: 4 j + 2, 4 j + 3)
   auto release = [&](int stage) {  // this warp's MMAs have finished reading the stage
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty[stage]);
@@ -247,15 +264,15 @@ __global__ void __launch_bounds__(LinCfg<NSLOT>::THREADS, 1) tc_linear_kernel(co
   const int ocols = EPI == TEPI_QKV ? n_tiles * BN
                     : EPI == TEPI_CONV ? p.ldb
                                        : max(p.ldo, p.out_h != nullptr ? p.ldb : 0);
-  if (EPI == TEPI_LN_GELU) {  // bias, gamma, beta of the 512 LayerNorm columns: the same for every tile
-    for (int i = mt; i < 2 * BN; i += 256) {
-      s_par[i] = p.bias[i]; s_par[2 * BN + i] = p.ln_g[i]; s_par[4 * BN + i] = p.ln_b[i];
-    }
+  if (LN) {  // bias, gamma, beta of this CTA's 256 LayerNorm columns: the same for every tile
+    const int col = rank * BN + mt;
+    s_par[mt] = p.bias[col]; s_par[BN + mt] = p.ln_g[col]; s_par[2 * BN + mt] = p.ln_b[col];
     mma_bar();
   }
   int g = 0;
+  uint32_t lt = 0;  // tiles this CTA has finished: the phase of the LayerNorm exchange barriers
   float acc[128];
-  TileWalk<TBM> walk(total_tiles, n_tiles);
+  TileWalk<C::CLUSTER> walk(total_tiles, n_tiles, rank);
   TileInfo ti;
   while (walk.next(p, ti)) {
     // TEPI_RESID: TMA load of the residual x (16 columns of this warpgroup's 64 rows) into buffer v & 1
@@ -264,7 +281,7 @@ __global__ void __launch_bounds__(LinCfg<NSLOT>::THREADS, 1) tc_linear_kernel(co
       tma_load_2d(stg + (v & 1) * STG_BOX, &p.out_map[0], ti.n_tile * BN + box * 16, (int)ti.grow0 + wg * 64, &xf[v & 1]);
     };
     float bias_r = 0.f;  // bias of column mt of this tile, moved to shared memory after the main loop
-    if (STAGED) {
+    if (STAGED && !LN) {
       const int col = ti.n_tile * BN + mt;
       if (col < ocols) bias_r = __ldg(p.bias + (p.w_select == 1 ? (long)ti.sel * p.bias_sel_stride : 0) + col);
     }
@@ -302,21 +319,45 @@ __global__ void __launch_bounds__(LinCfg<NSLOT>::THREADS, 1) tc_linear_kernel(co
     wgmma_wait<0>();
     fence_regs(acc);
     if (prev >= 0) release(prev);
-    if (STAGED) {  // both warpgroups are done with the previous tile's bias
+    if (STAGED && !LN) {  // both warpgroups are done with the previous tile's bias
       mma_bar();
       s_par[mt] = bias_r;
       mma_bar();
     }
 
-    if (EPI == TEPI_LN_GELU) {
-      // ---------------------------------------------------------------- LayerNorm(512) + GELU
-      // Every row of the tile lies in one quad of lanes per warpgroup (256 columns each): quad shuffles give the
-      // warpgroup's share, shared memory merges the two slots.  Two-pass statistics (mean, then squared deviations).
-      const float* bias = s_par + wg * BN;
+    float mean[2] = {0.f, 0.f}, rstd[2] = {0.f, 0.f};  // LayerNorm statistics of rows rl_a, rl_a + 8
+    if (LN) {
+      // ---------------------------------------------------------------- LayerNorm(512) statistics
+      // Two-pass statistics (mean, then squared deviations) over the 512 columns of a row: this CTA's 256 (the quad of
+      // lanes that holds the row sums them with two shuffles), plus the peer CTA's.  The quad's lane 0 stores its sum
+      // into the peer's s_red[pass][row] through distributed shared memory, arrives on the peer's lnbar[wg][pass]
+      // (release at cluster scope), waits on its own (acquire at cluster scope), reads the peer's sum and hands it to
+      // its quad.  s_red has a single buffer per pass.  That is safe because the peer overwrites s_red[pass][row] for
+      // tile t + 1 only after lane 0 of this quad has read it for tile t:
+      //   pass 0 of t + 1 is written after the peer's wait for this lane's pass-1 arrival of tile t,
+      //   pass 1 of t + 1 is written after the peer's wait for this lane's pass-0 arrival of tile t + 1,
+      // and this lane makes each of those arrivals after its read, in program order.  The same chain keeps each
+      // barrier at most one phase ahead of the lanes that wait on it.
+      auto exchange = [&](float (&v)[2], int pass) {  // v: this CTA's partial -> slot 0 + slot 1
+        float o[2] = {0.f, 0.f};
+        if (tq == 0) {
+#pragma unroll
+          for (int hr = 0; hr < 2; ++hr) st_cluster_f32(mapa(s_red + pass * TBM + rl_a + 8 * hr, rank ^ 1), v[hr]);
+          mbar_arrive_cluster(mapa(&lnbar[2 * wg + pass], rank ^ 1));
+          mbar_wait<true>(&lnbar[2 * wg + pass], lt & 1, p.dbg, 20 + pass, lt);
+#pragma unroll
+          for (int hr = 0; hr < 2; ++hr) o[hr] = s_red[pass * TBM + rl_a + 8 * hr];
+        }
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          o[hr] = __shfl_sync(0xffffffffu, o[hr], lane & ~3);
+          v[hr] = rank == 0 ? v[hr] + o[hr] : o[hr] + v[hr];
+        }
+      };
       float sum[2] = {0.f, 0.f};
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
-        const float2 bb = *reinterpret_cast<const float2*>(bias + 8 * j + 2 * tq);
+        const float2 bb = *reinterpret_cast<const float2*>(s_par + 8 * j + 2 * tq);
 #pragma unroll
         for (int hr = 0; hr < 2; ++hr) {
           acc[4 * j + 2 * hr] += bb.x; acc[4 * j + 2 * hr + 1] += bb.y;
@@ -327,12 +368,11 @@ __global__ void __launch_bounds__(LinCfg<NSLOT>::THREADS, 1) tc_linear_kernel(co
       for (int hr = 0; hr < 2; ++hr) {
         sum[hr] += __shfl_xor_sync(0xffffffffu, sum[hr], 1);
         sum[hr] += __shfl_xor_sync(0xffffffffu, sum[hr], 2);
-        if (tq == 0) s_red[wg * 64 + rl_a + 8 * hr] = sum[hr];
       }
-      mma_bar();
-      float mean[2], sq[2] = {0.f, 0.f};
+      exchange(sum, 0);
+      float sq[2] = {0.f, 0.f};
 #pragma unroll
-      for (int hr = 0; hr < 2; ++hr) mean[hr] = (s_red[rl_a + 8 * hr] + s_red[64 + rl_a + 8 * hr]) * (1.f / LG_FFN);
+      for (int hr = 0; hr < 2; ++hr) mean[hr] = sum[hr] * (1.f / LG_FFN);
 #pragma unroll
       for (int j = 0; j < 32; ++j)
 #pragma unroll
@@ -344,32 +384,11 @@ __global__ void __launch_bounds__(LinCfg<NSLOT>::THREADS, 1) tc_linear_kernel(co
       for (int hr = 0; hr < 2; ++hr) {
         sq[hr] += __shfl_xor_sync(0xffffffffu, sq[hr], 1);
         sq[hr] += __shfl_xor_sync(0xffffffffu, sq[hr], 2);
-        if (tq == 0) s_red[128 + wg * 64 + rl_a + 8 * hr] = sq[hr];
       }
-      mma_bar();
-      float rstd[2];
+      exchange(sq, 1);
 #pragma unroll
-      for (int hr = 0; hr < 2; ++hr)
-        rstd[hr] = rsqrtf((s_red[128 + rl_a + 8 * hr] + s_red[192 + rl_a + 8 * hr]) * (1.f / LG_FFN) + 1e-5f);
-      const bool haslo = p.out_l != nullptr;
-#pragma unroll
-      for (int hr = 0; hr < 2; ++hr) {
-        const long grow = ti.grow0 + rl_a + 8 * hr;
-        __nv_bfloat16* oh = p.out_h + grow * p.ldb + wg * BN;
-        __nv_bfloat16* ol = haslo ? p.out_l + grow * p.ldb + wg * BN : nullptr;
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const int c = 8 * j + 2 * tq;
-          const float2 gg = *reinterpret_cast<const float2*>(s_par + 2 * BN + wg * BN + c);
-          const float2 be = *reinterpret_cast<const float2*>(s_par + 4 * BN + wg * BN + c);
-          const float a = gelu_erf(fmaf((acc[4 * j + 2 * hr] - mean[hr]) * rstd[hr], gg.x, be.x));
-          const float b = gelu_erf(fmaf((acc[4 * j + 2 * hr + 1] - mean[hr]) * rstd[hr], gg.y, be.y));
-          const uint32_t hi = pack_bf16x2(a, b);
-          *reinterpret_cast<uint32_t*>(oh + c) = hi;
-          if (haslo) *reinterpret_cast<uint32_t*>(ol + c) = pack_bf16x2_lo(a, b, hi);
-        }
-      }
-      continue;
+      for (int hr = 0; hr < 2; ++hr) rstd[hr] = rsqrtf(sq[hr] * (1.f / LG_FFN) + 1e-5f);
+      ++lt;
     }
 
     if (EPI == TEPI_LSE || EPI == TEPI_ARGMAX) {
@@ -518,11 +537,11 @@ __global__ void __launch_bounds__(LinCfg<NSLOT>::THREADS, 1) tc_linear_kernel(co
       continue;
     }
 
-    // bias (* scale) (+ ReLU) (+ residual) -> fp32 and / or bf16 hi (/ lo); boxes of 16 columns: fp32 [64][16] (64-byte
-    // swizzle) at 0, hi / lo [64][16] (32-byte swizzle) at 4096 / 6144.  Map bounds clip the columns >= ldo / ldb and the
-    // rows >= S Lp.
+    // bias (* scale) (+ ReLU) (+ residual) -> fp32 and / or bf16 hi (/ lo), or LayerNorm + GELU -> bf16 hi (/ lo); boxes
+    // of 16 columns: fp32 [64][16] (64-byte swizzle) at 0, hi / lo [64][16] (32-byte swizzle) at H16 / H16 + 2048 (4096 /
+    // 6144; LayerNorm: 0 / 2048).  Map bounds clip the columns >= ldo / ldb and the rows >= S Lp.
     const bool f32out = EPI == TEPI_RESID || EPI == TEPI_F32;
-    const bool has16 = EPI == TEPI_CONV || EPI == TEPI_RESID || (EPI == TEPI_F32 && p.out_h != nullptr);
+    const bool has16 = EPI == TEPI_CONV || EPI == TEPI_RESID || LN || (EPI == TEPI_F32 && p.out_h != nullptr);
     const bool haslo = has16 && p.out_l != nullptr;
     const int nbox = (min(BN, ocols - ti.n_tile * BN) + 15) / 16;
     bool inside[2] = {true, true};
@@ -551,9 +570,17 @@ __global__ void __launch_bounds__(LinCfg<NSLOT>::THREADS, 1) tc_linear_kernel(co
 #pragma unroll
         for (int jl = 0; jl < 2; ++jl) {
           const int j = 2 * bx + jl, c = 8 * jl + 2 * tq;  // accumulator column pair, column inside the box
-          const float2 bb = *reinterpret_cast<const float2*>(s_par + 8 * j + 2 * tq);
-          float v0 = acc[4 * j + 2 * hr] + bb.x, v1 = acc[4 * j + 2 * hr + 1] + bb.y;
-          if (p.scale != 1.f) { v0 *= p.scale; v1 *= p.scale; }
+          float v0, v1;
+          if (LN) {  // the bias is in acc already (statistics above)
+            const float2 gg = *reinterpret_cast<const float2*>(s_par + BN + 8 * j + 2 * tq);
+            const float2 be = *reinterpret_cast<const float2*>(s_par + 2 * BN + 8 * j + 2 * tq);
+            v0 = gelu_erf(fmaf((acc[4 * j + 2 * hr] - mean[hr]) * rstd[hr], gg.x, be.x));
+            v1 = gelu_erf(fmaf((acc[4 * j + 2 * hr + 1] - mean[hr]) * rstd[hr], gg.y, be.y));
+          } else {
+            const float2 bb = *reinterpret_cast<const float2*>(s_par + 8 * j + 2 * tq);
+            v0 = acc[4 * j + 2 * hr] + bb.x; v1 = acc[4 * j + 2 * hr + 1] + bb.y;
+            if (p.scale != 1.f) { v0 *= p.scale; v1 *= p.scale; }
+          }
           if (EPI == TEPI_CONV) {
             v0 = inside[hr] ? ((p.relu && v0 < 0.f) ? 0.f : v0) : 0.f;
             v1 = inside[hr] ? ((p.relu && v1 < 0.f) ? 0.f : v1) : 0.f;
@@ -567,8 +594,8 @@ __global__ void __launch_bounds__(LinCfg<NSLOT>::THREADS, 1) tc_linear_kernel(co
           if (has16) {
             const uint32_t o = swz(row * 32 + c * 2, 0x10);
             const uint32_t hi = pack_bf16x2(v0, v1);
-            *reinterpret_cast<uint32_t*>(box + 4096 + o) = hi;
-            if (haslo) *reinterpret_cast<uint32_t*>(box + 6144 + o) = pack_bf16x2_lo(v0, v1, hi);
+            *reinterpret_cast<uint32_t*>(box + C::H16 + o) = hi;
+            if (haslo) *reinterpret_cast<uint32_t*>(box + C::H16 + 2048 + o) = pack_bf16x2_lo(v0, v1, hi);
           }
         }
       }
@@ -576,8 +603,8 @@ __global__ void __launch_bounds__(LinCfg<NSLOT>::THREADS, 1) tc_linear_kernel(co
       if (issuer) {
         const int col = ti.n_tile * BN + bx * 16;
         if (f32out) tma_store_2d(&p.out_map[0], box, col, row0);
-        if (has16) tma_store_2d(&p.out_map[1], box + 4096, col, row0);
-        if (haslo) tma_store_2d(&p.out_map[2], box + 6144, col, row0);
+        if (has16) tma_store_2d(&p.out_map[1], box + C::H16, col, row0);
+        if (haslo) tma_store_2d(&p.out_map[2], box + C::H16 + 2048, col, row0);
         bulk_commit();
         if (EPI == TEPI_RESID && bx + 2 < nbox) {  // the buffer's next box: once this store has read it
           bulk_wait_read<0>();
@@ -589,6 +616,10 @@ __global__ void __launch_bounds__(LinCfg<NSLOT>::THREADS, 1) tc_linear_kernel(co
   }
   // the stores must be complete (not only read) when the grid ends: the next kernel's griddepcontrol.wait relies on it
   if (STAGED && issuer) bulk_wait_all();
+  if (C::CLUSTER > 1) {  // neither CTA of a cluster exits while the other may still write into its shared memory
+    __syncwarp();
+    cluster_sync_all();
+  }
 }
 
 // fp32 -> bf16 hi (/ lo) for rows < len
@@ -637,23 +668,28 @@ EncodeFn get_encode() {
   return fn;
 }
 
-template <int NSLOT, int EPI>
+template <int EPI>
 int launch_linear_t(const TcLinParams& p, cudaStream_t stream) {
-  using C = LinCfg<NSLOT>;
-  const int num_sms = lg_num_sms();
-  const int total = p.n_tiles * p.st.S * (p.st.Lp / C::TBM);
-  const int grid = total < num_sms ? total : num_sms;
-  return tc_launch(tc_linear_kernel<NSLOT, EPI>, dim3(grid), C::THREADS, C::SMEM, p, stream);
+  using C = LinCfg<EPI>;
+  const int total = p.n_tiles * p.st.S * (p.st.Lp / TBM);
+  int slots = lg_num_sms();  // co-resident CTAs, or clusters: how the SMs of the device split into clusters varies
+  if (C::CLUSTER > 1) {
+    if (p.n_tiles != C::CLUSTER) return lg_set_error("launch_linear: a cluster kernel needs one column tile per CTA");
+    if (int r = lg_max_clusters((const void*)tc_linear_kernel<EPI>, C::THREADS, C::SMEM, C::CLUSTER, &slots)) return r;
+  }
+  const int units = total / C::CLUSTER;
+  const int grid = (units < slots ? units : slots) * C::CLUSTER;
+  return tc_launch(tc_linear_kernel<EPI>, dim3(grid), C::THREADS, C::SMEM, p, stream, C::CLUSTER);
 }
 int launch_linear(const TcLinParams& p, cudaStream_t stream) {
   switch (p.epi) {
-    case TEPI_QKV: return launch_linear_t<1, TEPI_QKV>(p, stream);
-    case TEPI_LN_GELU: return launch_linear_t<2, TEPI_LN_GELU>(p, stream);
-    case TEPI_RESID: return launch_linear_t<1, TEPI_RESID>(p, stream);
-    case TEPI_F32: return launch_linear_t<1, TEPI_F32>(p, stream);
-    case TEPI_CONV: return launch_linear_t<1, TEPI_CONV>(p, stream);
-    case TEPI_LSE: return launch_linear_t<1, TEPI_LSE>(p, stream);
-    case TEPI_ARGMAX: return launch_linear_t<1, TEPI_ARGMAX>(p, stream);
+    case TEPI_QKV: return launch_linear_t<TEPI_QKV>(p, stream);
+    case TEPI_LN_GELU: return launch_linear_t<TEPI_LN_GELU>(p, stream);
+    case TEPI_RESID: return launch_linear_t<TEPI_RESID>(p, stream);
+    case TEPI_F32: return launch_linear_t<TEPI_F32>(p, stream);
+    case TEPI_CONV: return launch_linear_t<TEPI_CONV>(p, stream);
+    case TEPI_LSE: return launch_linear_t<TEPI_LSE>(p, stream);
+    case TEPI_ARGMAX: return launch_linear_t<TEPI_ARGMAX>(p, stream);
   }
   return lg_set_error("launch_linear: bad epilogue");
 }
@@ -671,11 +707,10 @@ struct TcOperands {
 // apply); this adds the tensor maps, the K-block and pass counts, and launches n_tiles column tiles per row tile.
 int tc_gemm(TcEngine& e, const SeqState& st, const TcOperands& d, int n_tiles, TcLinParams& p, cudaStream_t stream) {
   const uint64_t rows = (uint64_t)st.S * st.Lp;
-  const uint32_t tbm = p.epi == TEPI_LN_GELU ? LinCfg<2>::TBM : LinCfg<1>::TBM;
   const uint64_t K = p.conv_cb ? 9 * d.k0 : d.k0 + d.k1, nout = d.nout, nsel = d.nsel;
   const uint64_t sel_bytes = (nsel > 1 ? d.sel_stride : nout * K) * 2;
   auto amap = [&](CUtensorMap* out, const void* a, uint64_t k) {  // box 64 x the tile height
-    return tc_tmap(e, {a, 2, {k, rows}, {k * 2}, {BK, tbm}}, out);
+    return tc_tmap(e, {a, 2, {k, rows}, {k * 2}, {BK, TBM}}, out);
   };
   auto wmap = [&](CUtensorMap* out, const void* w) { return tc_tmap(e, {w, 3, {K, nout, nsel}, {K * 2, sel_bytes}, {BK, BN, 1}}, out); };
   // maps the kernel does not read repeat a map it does (segment 1 of a one-segment A, every lo map in bf16)
@@ -699,7 +734,7 @@ int tc_gemm(TcEngine& e, const SeqState& st, const TcOperands& d, int n_tiles, T
     if ((r = tc_tmap(e, {p.k, 2, {LG_HDIM, sh * st.Lp}, {LG_HDIM * 2}, {LG_HDIM, 64}}, &p.out_map[1]))) return r;
     if ((r = tc_tmap(e, {p.vt, 2, {(uint64_t)st.Lp, sh * LG_HDIM}, {(uint64_t)st.Lp * 2}, {64, LG_HDIM}}, &p.out_map[2])))
       return r;
-  } else if (p.epi == TEPI_RESID || p.epi == TEPI_F32 || p.epi == TEPI_CONV) {
+  } else if (p.epi == TEPI_RESID || p.epi == TEPI_F32 || p.epi == TEPI_CONV || p.epi == TEPI_LN_GELU) {
     const uint64_t ldo = p.ldo, ldb = p.ldb;
     if (p.out_f32 && (r = tc_tmap(e, {p.out_f32, 2, {ldo, rows}, {ldo * 4}, {16, 64}, CU_TENSOR_MAP_SWIZZLE_64B,
                                       CU_TENSOR_MAP_DATA_TYPE_FLOAT32}, &p.out_map[0])))
@@ -920,7 +955,7 @@ int tc_block(LgHandle* h, const TcBuffers& b, const SeqState& st, int layer, int
     p.out_h = b.hh; p.out_l = b.hl; p.ldb = LG_FFN;
     const TcOperands ops{b.xh, b.xl, LG_DIM, b.ctxh, b.ctxl, LG_DIM, wh + o.w1f, wl + o.w1f, LG_FFN, 1, 0};
     Timer t2(h, LG_K_FFN0, stream);
-    int r = run_linear(h, st, ops, 1, p, stream);  // one 512-column tile: the whole LayerNorm row
+    int r = run_linear(h, st, ops, LG_FFN / BN, p, stream);  // one 2-CTA cluster per 128 rows: the whole LayerNorm row
     if (r) return r;
   }
   {  // ffn.3 + residual -> x (fp32 master + bf16 shadows)

@@ -36,6 +36,7 @@ namespace {
 std::mutex g_dev_mu;
 std::map<std::pair<int, const void*>, int> g_smem_done;  // (device, kernel) -> bytes opted in
 std::map<int, int> g_sms;
+std::map<std::pair<int, const void*>, int> g_clusters;  // (device, kernel) -> co-resident clusters
 }  // namespace
 int lg_func_smem_once(const void* func, int bytes) {
   int dev = 0;
@@ -57,6 +58,26 @@ int lg_num_sms() {
   if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
   g_sms[dev] = n;
   return n;
+}
+int lg_max_clusters(const void* func, int threads, int smem, int cluster, int* out) {
+  if (int r = lg_func_smem_once(func, smem)) return r;
+  int dev = 0;
+  LG_CU(cudaGetDevice(&dev));
+  std::lock_guard<std::mutex> lk(g_dev_mu);
+  auto it = g_clusters.find({dev, func});
+  if (it != g_clusters.end()) { *out = it->second; return 0; }
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeClusterDimension;
+  at[0].val.clusterDim.x = cluster; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(cluster); cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = smem;
+  cfg.attrs = at; cfg.numAttrs = 1;
+  int n = 0;
+  LG_CU(cudaOccupancyMaxActiveClusters(&n, func, &cfg));
+  if (n <= 0) return lg_set_error("lg_max_clusters: the kernel's clusters do not fit on this device");
+  g_clusters[{dev, func}] = n;
+  *out = n;
+  return 0;
 }
 extern "C" const char* lg_build_info(void) {
 #define LG_STR2(x) #x

@@ -33,6 +33,9 @@ int lg_set_error(const char* msg);
 int lg_func_smem_once(const void* func, int bytes);
 // SM count of the current device (queried once per device).
 int lg_num_sms();
+// *out = how many clusters of `cluster` CTAs of `func` (`threads` threads, `smem` bytes of dynamic shared memory) can be
+// resident at once on the current device (queried once per device and kernel); opts `func` in to `smem` bytes.
+int lg_max_clusters(const void* func, int threads, int smem, int cluster, int* out);
 
 // Device-side view of the adaptive state; all arrays live in the workspace.
 struct SeqState {

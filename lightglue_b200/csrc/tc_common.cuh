@@ -27,15 +27,26 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t by
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
+// CLUSTER: acquire at cluster scope, for phases completed by arrivals from another CTA of the cluster
+template <bool CLUSTER = false>
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
+  if (CLUSTER)
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
+        "selp.u32 %0, 1, 0, p;\n\t}"
+        : "=r"(ok)
+        : "r"(smem_u32(bar)), "r"(parity)
+        : "memory");
+  else
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+        "selp.u32 %0, 1, 0, p;\n\t}"
+        : "=r"(ok)
+        : "r"(smem_u32(bar)), "r"(parity)
+        : "memory");
   return ok != 0;
 }
 // Bounded spin: a protocol bug must never hang the GPU.  After ~2^18 failed probes the waiter records
@@ -44,10 +55,11 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
 // dbg points at 32 words; word `site` keeps the first code recorded there: 0x80000000 | extra << 12 | thread;
 // word 31 is the "some wait has timed out" flag: once it is set every other long wait gives up after 64 probes,
 // so a broken pipeline drains in milliseconds instead of minutes.
+template <bool CLUSTER = false>
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, unsigned int* dbg, uint32_t site,
                                           uint32_t extra = 0) {
   uint32_t spins = 0;
-  while (!mbar_try_wait(bar, parity)) {
+  while (!mbar_try_wait<CLUSTER>(bar, parity)) {
     ++spins;
     if (spins == 64 && dbg && *reinterpret_cast<volatile unsigned int*>(dbg + 31) != 0u) return;
     if (spins > (1u << 18)) {
@@ -58,6 +70,32 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, unsign
       return;
     }
   }
+}
+
+// ---------------------------------------------------------------- thread-block clusters
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+// the address of the same shared-memory location in CTA `rank` of the cluster (a shared::cluster address)
+__device__ __forceinline__ uint32_t mapa(const void* p, uint32_t rank) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_u32(p)), "r"(rank));
+  return r;
+}
+__device__ __forceinline__ void st_cluster_f32(uint32_t addr, float v) {
+  asm volatile("st.shared::cluster.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory");
+}
+// arrive on an mbarrier of another CTA of the cluster (`addr` from mapa); releases this thread's earlier writes and reads
+// at cluster scope
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t addr) {
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(addr) : "memory");
+}
+// every thread of every CTA of the cluster; orders memory at cluster scope
+__device__ __forceinline__ void cluster_sync_all() {
+  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
+  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
 // ---------------------------------------------------------------- TMA
@@ -241,16 +279,18 @@ struct TcEngine;
 int tc_tmap(TcEngine& e, const TmapArgs& a, CUtensorMap* out);
 
 // Launches a tensor-core kernel with programmatic dependent launch, after opting it in to `smem` bytes of dynamic
-// shared memory on the current device.
+// shared memory on the current device; `cluster` > 1: in clusters of that many CTAs along x.
 template <class P>
-int tc_launch(void (*kernel)(P), dim3 grid, int threads, int smem, const P& p, cudaStream_t stream) {
+int tc_launch(void (*kernel)(P), dim3 grid, int threads, int smem, const P& p, cudaStream_t stream, int cluster = 1) {
   if (int r = lg_func_smem_once((const void*)kernel, smem)) return r;
-  cudaLaunchAttribute at[1];
+  cudaLaunchAttribute at[2];
   at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   at[0].val.programmaticStreamSerializationAllowed = 1;
+  at[1].id = cudaLaunchAttributeClusterDimension;
+  at[1].val.clusterDim.x = cluster; at[1].val.clusterDim.y = 1; at[1].val.clusterDim.z = 1;
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = grid; cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
-  cfg.attrs = at; cfg.numAttrs = 1;
+  cfg.attrs = at; cfg.numAttrs = cluster > 1 ? 2 : 1;
   const cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, p);
   if (e != cudaSuccess) return lg_set_cuda_error(e, __FILE__, __LINE__);
   return 0;
