@@ -4,7 +4,8 @@
 ``forward({"image0": ..., "image1": ...})`` -> output dict; the math runs in hand-written CUDA
 kernels behind the C ABI declared in ``include/lightglue_b200.h``.
 """
+from .disk import DISK  # noqa: F401
 from .matcher import LightGlue  # noqa: F401
 from .sift import SIFT  # noqa: F401
 
-__all__ = ["LightGlue", "SIFT"]
+__all__ = ["DISK", "LightGlue", "SIFT"]

@@ -10,11 +10,12 @@ PREC = {"fp32": 0, "bf16": 1, "bf16x3": 2}
 K_ATTENTION, K_LINEAR, K_ASSIGN, K_OTHER = 0, 1, 2, 3
 ABI_VERSION = 3
 
-# include/superpoint_b200.h, include/aliked_b200.h and include/sift_b200.h: same library
+# include/superpoint_b200.h, include/aliked_b200.h, include/sift_b200.h and include/disk_b200.h: same library
 SP_ABI_VERSION = 2
 SP_TC_BUFFERS = 9  # buffers of the tensor-core backbone's workspace plan (sp_tc_layout)
 AL_ABI_VERSION = 1
 SIFT_ABI_VERSION = 1
+DISK_ABI_VERSION = 1
 
 
 class LgConfig(C.Structure):
@@ -45,6 +46,13 @@ class SiftConfig(C.Structure):
         ("abi_version", C.c_int32), ("num_octave_layers", C.c_int32), ("nms_radius", C.c_int32),
         ("max_num_keypoints", C.c_int32), ("rootsift", C.c_int32), ("reserved", C.c_int32),
         ("detection_threshold", C.c_double), ("edge_threshold", C.c_double),
+    ]
+
+
+class DiskConfig(C.Structure):
+    _fields_ = [
+        ("abi_version", C.c_int32), ("max_num_keypoints", C.c_int32), ("nms_window_size", C.c_int32),
+        ("pad_if_not_divisible", C.c_int32), ("detection_threshold", C.c_float),
     ]
 
 
@@ -114,8 +122,17 @@ SIFT_PROTOTYPES = {  # include/sift_b200.h
     "sift_workspace_bytes": (_SZ, [_VP, _I32, _I32, _I32]),
     "sift_forward": (C.c_int, [_VP, _VP, _I32, _VP, _I32, _I32, _I32, _I64] + [_VP] * 7 + [_SZ, _VP]),
 }
-EXPORTS, SP_EXPORTS, AL_EXPORTS, SIFT_EXPORTS = (
-    tuple(t) for t in (LG_PROTOTYPES, SP_PROTOTYPES, AL_PROTOTYPES, SIFT_PROTOTYPES))
+DISK_PROTOTYPES = {  # include/disk_b200.h
+    "disk_weight_blob_floats": (_SZ, []),
+    "disk_create": (C.c_int, [C.POINTER(DiskConfig), _VP, _SZ, _VP, _HANDLE_OUT]),
+    "disk_destroy": (C.c_int, [_VP]),
+    "disk_max_keypoints": (_I64, [_VP, _I32, _I32]),
+    "disk_workspace_bytes": (_SZ, [_VP, _I32, _I32, _I32]),
+    "disk_forward": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _I32, _I64] + [_VP] * 5 + [_SZ, _VP]),
+    "disk_heads": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _I32, _VP, _I32, _VP, _VP, _VP, _SZ, _VP]),
+}
+EXPORTS, SP_EXPORTS, AL_EXPORTS, SIFT_EXPORTS, DISK_EXPORTS = (
+    tuple(t) for t in (LG_PROTOTYPES, SP_PROTOTYPES, AL_PROTOTYPES, SIFT_PROTOTYPES, DISK_PROTOTYPES))
 
 _lib = None
 
@@ -134,7 +151,7 @@ def load():
     if not os.path.exists(path):
         raise RuntimeError(f"{path} is missing: the CUDA library must be built (python -m lightglue_b200.build)")
     lib = C.CDLL(path)
-    for table in (LG_PROTOTYPES, SP_PROTOTYPES, AL_PROTOTYPES, SIFT_PROTOTYPES):
+    for table in (LG_PROTOTYPES, SP_PROTOTYPES, AL_PROTOTYPES, SIFT_PROTOTYPES, DISK_PROTOTYPES):
         for name, (restype, argtypes) in table.items():
             fn = getattr(lib, name)
             fn.restype, fn.argtypes = restype, argtypes

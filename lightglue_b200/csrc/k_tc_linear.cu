@@ -49,11 +49,12 @@ struct TcLinParams {
   __half* q; __half* k; __half* vt; const float* cs;
   const float* ln_g; const float* ln_b;
   unsigned int* dbg;
-  // 3x3 convolution as a GEMM over a zero-padded NHWC image [rows = B (H+2) (W+2), Cin] (SuperPoint encoder): K block kb
-  // = (tap, 64-channel block); the A tile of a tap is the same matrix shifted by (dy (W+2) + dx) rows (TMA fills the
-  // rows outside the tensor with zeros).  conv_cb = Cin / 64 (0: not a convolution).  TEPI_CONV zeroes the padding
-  // pixels again on the way out (conv_w2 = W + 2, conv_plane = (H+2)(W+2), conv_rows = B conv_plane) and applies ReLU.
-  int conv_cb, conv_w2, conv_h, conv_w, relu;
+  // k x k convolution (k = 3: SuperPoint encoder, k = 5: DISK) as a GEMM over a zero-padded NHWC image [rows = B (H+2q)
+  // (W+2q), Cin] with a border of q = k / 2 pixels: K block kb = (tap, 64-channel block); the A tile of a tap is the same
+  // matrix shifted by (dy (W+2q) + dx) rows, dy, dx in [-q, q] (TMA fills the rows outside the tensor with zeros).
+  // conv_cb = Cin / 64 (0: not a convolution).  TEPI_CONV zeroes the padding pixels again on the way out (conv_w2 = W + 2q,
+  // conv_plane = (H+2q)(W+2q), conv_rows = B conv_plane) and applies ReLU.
+  int conv_cb, conv_k, conv_pad, conv_w2, conv_h, conv_w, relu;
   long conv_plane, conv_rows;
   int mma_n;  // N of the MMAs when fewer than 256 output columns exist (64 / 128; 0 = 256): the weight rows beyond are zero
   // TMA stores of the staged epilogues, 64-row boxes (one MMA warpgroup's rows): TEPI_QKV: q, k ([S H Lp, 64], box 64 x 64)
@@ -224,7 +225,7 @@ __global__ void __launch_bounds__(LinCfg<EPI>::THREADS, 1) tc_linear_kernel(cons
           int arow = (int)ti.grow0;
           if (p.conv_cb) {  // convolution tap: shifted rows of the padded image, channel block kb % conv_cb
             const int tap = kb / p.conv_cb;
-            arow += (tap / 3 - 1) * p.conv_w2 + (tap % 3 - 1);
+            arow += (tap / p.conv_k - p.conv_pad) * p.conv_w2 + (tap % p.conv_k - p.conv_pad);
             kc = (kb % p.conv_cb) * BK;
             seg = 0;
           }
@@ -551,7 +552,8 @@ __global__ void __launch_bounds__(LinCfg<EPI>::THREADS, 1) tc_linear_kernel(cons
         const long grow = ti.grow0 + rl_a + 8 * hr;
         const long pp = grow % p.conv_plane;
         const int yy = (int)(pp / p.conv_w2), xx = (int)(pp % p.conv_w2);
-        inside[hr] = grow < p.conv_rows && yy >= 1 && yy <= p.conv_h && xx >= 1 && xx <= p.conv_w;
+        inside[hr] = grow < p.conv_rows && yy >= p.conv_pad && yy < p.conv_h + p.conv_pad && xx >= p.conv_pad &&
+                     xx < p.conv_w + p.conv_pad;
       }
     }
 #pragma unroll
@@ -695,7 +697,7 @@ int launch_linear(const TcLinParams& p, cudaStream_t stream) {
 }
 
 // Operands of one GEMM.  A = [A0 | A1] along K, each [st.S * st.Lp rows, k] bf16 row-major; W = nsel matrices [nout, K]
-// bf16 (K = k0 + k1, or 9 k0 for a 3x3 convolution), sel_stride elements apart.  The lo images are read in bf16x3 only.
+// bf16 (K = k0 + k1, or k^2 k0 for a k x k convolution), sel_stride elements apart.  The lo images are read in bf16x3 only.
 struct TcOperands {
   const __nv_bfloat16 *a0h, *a0l; int k0;
   const __nv_bfloat16 *a1h, *a1l; int k1;  // k1 = 0: one segment
@@ -707,7 +709,7 @@ struct TcOperands {
 // apply); this adds the tensor maps, the K-block and pass counts, and launches n_tiles column tiles per row tile.
 int tc_gemm(TcEngine& e, const SeqState& st, const TcOperands& d, int n_tiles, TcLinParams& p, cudaStream_t stream) {
   const uint64_t rows = (uint64_t)st.S * st.Lp;
-  const uint64_t K = p.conv_cb ? 9 * d.k0 : d.k0 + d.k1, nout = d.nout, nsel = d.nsel;
+  const uint64_t K = p.conv_cb ? (uint64_t)p.conv_k * p.conv_k * d.k0 : d.k0 + d.k1, nout = d.nout, nsel = d.nsel;
   const uint64_t sel_bytes = (nsel > 1 ? d.sel_stride : nout * K) * 2;
   auto amap = [&](CUtensorMap* out, const void* a, uint64_t k) {  // box 64 x the tile height
     return tc_tmap(e, {a, 2, {k, rows}, {k * 2}, {BK, TBM}}, out);
@@ -906,16 +908,19 @@ int tc_final_proj(LgHandle* h, const TcBuffers& b, const SeqState& st, float* p_
 int tc_conv(TcEngine& e, const SeqState& st, const __nv_bfloat16* in_h, const __nv_bfloat16* in_l, int cin, int taps, size_t w_off,
             const float* bias, int relu, int B, int H, int W, __nv_bfloat16* out_h, __nv_bfloat16* out_l, int cout, float* out_f32,
             int ldo, cudaStream_t stream) {
-  if (cin % BK != 0 || (taps != 1 && taps != 9)) return lg_set_error("tc_conv: Cin must be a multiple of 64, 1x1 or 3x3");
+  if (cin % BK != 0 || (taps != 1 && taps != 9 && taps != 25))
+    return lg_set_error("tc_conv: Cin must be a multiple of 64, 1x1, 3x3 or 5x5");
   TcLinParams p{};
   p.epi = out_f32 ? TEPI_F32 : TEPI_CONV;
   p.scale = 1.f; p.bias = bias; p.relu = relu;
   p.out_f32 = out_f32; p.ldo = ldo; p.out_h = out_h; p.out_l = e.x3 ? out_l : nullptr; p.ldb = cout;
   const int mma_n = cout <= 64 ? 64 : cout <= 128 ? 128 : BN;  // no MMA columns for the zero rows of a narrow layer
   p.mma_n = mma_n == BN ? 0 : mma_n;
-  p.conv_cb = taps == 9 ? cin / BK : 0;
-  p.conv_w2 = W + 2; p.conv_h = H; p.conv_w = W;
-  p.conv_plane = (long)(H + 2) * (W + 2); p.conv_rows = (long)B * p.conv_plane;
+  p.conv_cb = taps > 1 ? cin / BK : 0;
+  p.conv_k = taps == 25 ? 5 : 3;
+  p.conv_pad = p.conv_k / 2;  // 1x1: the 3x3 layout (SuperPoint's heads read the padded maps of their 3x3 inputs)
+  p.conv_w2 = W + 2 * p.conv_pad; p.conv_h = H; p.conv_w = W;
+  p.conv_plane = (long)(H + 2 * p.conv_pad) * p.conv_w2; p.conv_rows = (long)B * p.conv_plane;
   const TcOperands ops{in_h, in_l, cin, nullptr, nullptr, 0, e.w_hi + w_off, e.w_lo + w_off, BN, 1, 0};
   return tc_gemm(e, st, ops, 1, p, stream);
 }

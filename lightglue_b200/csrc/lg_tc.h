@@ -48,11 +48,13 @@ int tc_assign_sweeps(LgHandle* h, const TcBuffers& b, const SeqState& st, const 
 // softmax(q k^T / 8) v per (sequence, head): q from b.q, keys from kbuf, values from b.vt; key/value
 // sequence = (s + kv_shift) % S; writes b.ctxh (/ b.ctxl)
 int tc_attention(LgHandle* h, const TcBuffers& b, const SeqState& st, int kv_shift, const __half* kbuf, cudaStream_t stream);
-// k x k convolution (k = 1: `taps` = 1, k = 3: `taps` = 9, zero padding 1) + bias (+ ReLU) as a tensor-core GEMM over a
-// zero-padded NHWC image stored as a [st.S * st.Lp rows, Cin] matrix, row = padded pixel b (H+2)(W+2) + y (W+2) + x
-// (SuperPoint encoder, superpoint.py:137-153).  Weights: [256 rows (Cout, zero padded), taps * Cin] at e.w_hi/w_lo +
-// w_off; bias padded to 256.  Output: the same padded layout with `cout` channels as bf16 hi (/ lo), padding pixels
-// zeroed -- or, if out_f32 is given, fp32 [rows, ldo] without ReLU / zeroing (the 1x1 heads).
+// k x k convolution (k = 1: `taps` = 1 and k = 3: `taps` = 9, zero padding q = 1; k = 5: `taps` = 25, q = 2) + bias
+// (+ ReLU) as a tensor-core GEMM over a zero-padded NHWC image stored as a [st.S * st.Lp rows, Cin] matrix, row = padded
+// pixel b (H+2q)(W+2q) + y (W+2q) + x (SuperPoint encoder, superpoint.py:137-153; DISK's U-Net).  Weights: [256 rows
+// (Cout, zero padded), taps * Cin] (column tap * Cin + ci) at e.w_hi/w_lo + w_off; bias padded to 256.  Output: the same
+// padded layout with `cout` channels as bf16 hi (/ lo), padding pixels zeroed -- or, if out_f32 is given, fp32
+// [rows, ldo] without ReLU / zeroing (SuperPoint's 1x1 heads, DISK's convolutions: their padding rows hold garbage).
+// With taps = 1 it is a plain GEMM [rows, Cin] x [Cout, Cin]^T (DISK's descriptor head on gathered im2col rows).
 int tc_conv(TcEngine& e, const SeqState& st, const __nv_bfloat16* in_h, const __nv_bfloat16* in_l, int cin, int taps, size_t w_off,
             const float* bias, int relu, int B, int H, int W, __nv_bfloat16* out_h, __nv_bfloat16* out_l, int cout, float* out_f32,
             int ldo, cudaStream_t stream);

@@ -219,6 +219,33 @@ __device__ __forceinline__ unsigned sp_key(float f) {  // order-preserving map f
   const unsigned u = __float_as_uint(f);
   return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
+// radix select over the n scores s (blockDim 1024, 4 x 8 bits): on entry s_prefix = 0 and s_remaining = k; on exit
+// s_prefix is the key of the k-th largest score and s_remaining how many candidates with exactly that key rank <= k
+__device__ void radix_kth_largest(const float* s, int n, int* hist, unsigned& s_prefix, int& s_remaining) {
+  const int tid = threadIdx.x;
+  for (int pass = 3; pass >= 0; --pass) {
+    for (int i = tid; i < 256; i += 1024) hist[i] = 0;
+    __syncthreads();
+    const unsigned prefix = s_prefix;
+    const unsigned himask = pass == 3 ? 0u : (0xffffffffu << (8 * (pass + 1)));
+    for (int j = tid; j < n; j += 1024) {
+      const unsigned key = sp_key(s[j]);
+      if ((key & himask) == (prefix & himask)) atomicAdd(&hist[(key >> (8 * pass)) & 255], 1);
+    }
+    __syncthreads();
+    if (tid == 0) {
+      int rem = s_remaining, d = 255;
+      for (; d > 0; --d) {
+        if (hist[d] >= rem) break;
+        rem -= hist[d];
+      }
+      s_prefix = prefix | ((unsigned)d << (8 * pass));
+      s_remaining = rem;
+    }
+    __syncthreads();
+  }
+}
+
 __global__ void __launch_bounds__(1024) sp_select_kernel(const int* __restrict__ n_cand, const int* __restrict__ cand_pos,
                                                          const float* __restrict__ cand_score, int* __restrict__ sel_pos,
                                                          float* __restrict__ sel_score, int* __restrict__ n_sel, int k, long cap,
@@ -242,27 +269,7 @@ __global__ void __launch_bounds__(1024) sp_select_kernel(const int* __restrict__
   if (n < k) k = n;  // rank_all with fewer candidates than k: keep (and rank) them all
   if (tid == 0) { s_prefix = 0u; s_remaining = k; s_count = 0; s_carry = 0; n_sel[b] = k; }
   __syncthreads();
-  for (int pass = 3; pass >= 0; --pass) {
-    for (int i = tid; i < 256; i += 1024) hist[i] = 0;
-    __syncthreads();
-    const unsigned prefix = s_prefix;
-    const unsigned himask = pass == 3 ? 0u : (0xffffffffu << (8 * (pass + 1)));
-    for (int j = tid; j < n; j += 1024) {
-      const unsigned key = sp_key(s[j]);
-      if ((key & himask) == (prefix & himask)) atomicAdd(&hist[(key >> (8 * pass)) & 255], 1);
-    }
-    __syncthreads();
-    if (tid == 0) {
-      int rem = s_remaining, d = 255;
-      for (; d > 0; --d) {
-        if (hist[d] >= rem) break;
-        rem -= hist[d];
-      }
-      s_prefix = prefix | ((unsigned)d << (8 * pass));
-      s_remaining = rem;
-    }
-    __syncthreads();
-  }
+  radix_kth_largest(s, n, hist, s_prefix, s_remaining);
   const unsigned T = s_prefix;   // key of the k-th largest score
   const int take_eq = s_remaining;  // how many candidates with exactly that score are kept: the first ones
   for (int base = 0; base < n; base += 1024) {
@@ -302,6 +309,58 @@ __global__ void __launch_bounds__(1024) sp_select_kernel(const int* __restrict__
     for (int t = 0; t < cnt; ++t) rank += (ss[t] > me || (ss[t] == me && sj[t] < mj)) ? 1 : 0;
     if (rank < out_cap) { sel_pos[(long)b * out_cap + rank] = pos[mj]; sel_score[(long)b * out_cap + rank] = me; }
   }
+}
+
+// kornia's DISK top-k (n = k_max >= 0): k = min(n + 1, count), keep the candidates strictly above the k-th largest score,
+// then the first n of them, all in candidate (row-major) order.  k_max < 0: every candidate.  One block per image.
+__global__ void __launch_bounds__(1024) kp_select_above_kernel(const int* __restrict__ n_cand, const int* __restrict__ cand_pos,
+                                                               const float* __restrict__ cand_score, int* __restrict__ sel_pos,
+                                                               float* __restrict__ sel_score, int* __restrict__ n_sel, int k_max,
+                                                               long cap, long out_cap) {
+  __shared__ int hist[256];
+  __shared__ int wsum[32];
+  __shared__ unsigned s_prefix;
+  __shared__ int s_remaining, s_carry;
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const int n = n_cand[b];
+  const float* s = cand_score + (long)b * cap;
+  const int* pos = cand_pos + (long)b * cap;
+  const long lim = k_max < 0 ? out_cap : (k_max < out_cap ? k_max : out_cap);
+  if (k_max < 0 || n == 0) {
+    const int m = n < lim ? n : (int)lim;
+    if (tid == 0) n_sel[b] = m;
+    for (int j = tid; j < m; j += 1024) { sel_pos[(long)b * out_cap + j] = pos[j]; sel_score[(long)b * out_cap + j] = s[j]; }
+    return;
+  }
+  if (tid == 0) { s_prefix = 0u; s_remaining = k_max < n ? k_max + 1 : n; s_carry = 0; }
+  __syncthreads();
+  radix_kth_largest(s, n, hist, s_prefix, s_remaining);
+  const unsigned T = s_prefix;
+  for (int base = 0; base < n; base += 1024) {
+    const int j = base + tid;
+    const bool gt = j < n && sp_key(s[j]) > T;
+    const unsigned m = __ballot_sync(0xffffffffu, gt);
+    const int in_warp = __popc(m & ((1u << (tid & 31)) - 1u));
+    if ((tid & 31) == 0) wsum[tid >> 5] = __popc(m);
+    __syncthreads();
+    if (tid < 32) {
+      int w = wsum[tid], incl = w;
+#pragma unroll
+      for (int off = 1; off < 32; off <<= 1) {
+        const int t = __shfl_up_sync(0xffffffffu, incl, off);
+        if (tid >= off) incl += t;
+      }
+      wsum[tid] = incl - w;
+      if (tid == 31) hist[0] = incl;
+    }
+    __syncthreads();
+    const int rank = s_carry + wsum[tid >> 5] + in_warp;
+    if (gt && rank < lim) { sel_pos[(long)b * out_cap + rank] = pos[j]; sel_score[(long)b * out_cap + rank] = s[j]; }
+    __syncthreads();
+    if (tid == 0) s_carry += hist[0];
+    __syncthreads();
+  }
+  if (tid == 0) n_sel[b] = s_carry < lim ? s_carry : (int)lim;
 }
 
 // one block (256 threads = the 256 descriptor channels) per keypoint slot: bilinear sample + L2 normalisation (79-96)
@@ -362,14 +421,23 @@ Level level(int B, int H, int W) {
 
 }  // namespace
 
+int kp_compact(const float* scores, int B, int H, int W, float thr, long cap, int* row_count, int* row_start, int* n_cand,
+               int* cand_pos, float* cand_score, cudaStream_t stream) {
+  const long rows = (long)B * H;
+  sp_row_count_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, stream>>>(scores, row_count, rows, W, thr);
+  sp_row_scan_kernel<<<B, 1024, 0, stream>>>(row_count, row_start, n_cand, H);
+  sp_row_write_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, stream>>>(scores, row_start, cand_pos, cand_score, rows, H, W, thr, cap);
+  return cudaGetLastError() == cudaSuccess ? 0 : lg_set_error("candidate compaction launch failed");
+}
+int kp_select_above_kth(const int* n_cand, const int* cand_pos, const float* cand_score, int* sel_pos, float* sel_score, int* n_sel,
+                        int B, int k_max, long cap, long out_cap, cudaStream_t stream) {
+  kp_select_above_kernel<<<B, 1024, 0, stream>>>(n_cand, cand_pos, cand_score, sel_pos, sel_score, n_sel, k_max, cap, out_cap);
+  return cudaGetLastError() == cudaSuccess ? 0 : lg_set_error("top-k launch failed");
+}
+
 // SpCudaStages: the Stages policy of sp_run_post for the CUDA build of the tensor-core mode
 int SpCudaStages::compact_impl(const SpWorkspace& ws, int B, int H, int W, float thr, long cap) const {
-  const long rows = (long)B * H;
-  sp_row_count_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, stream>>>(ws.t0, ws.row_count, rows, W, thr);
-  sp_row_scan_kernel<<<B, 1024, 0, stream>>>(ws.row_count, ws.row_start, ws.n_cand, H);
-  sp_row_write_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, stream>>>(ws.t0, ws.row_start, ws.cand_pos, ws.cand_score, rows, H, W,
-                                                                      thr, cap);
-  return cudaGetLastError() == cudaSuccess ? 0 : lg_set_error("superpoint: candidate compaction launch failed");
+  return kp_compact(ws.t0, B, H, W, thr, cap, ws.row_count, ws.row_start, ws.n_cand, ws.cand_pos, ws.cand_score, stream);
 }
 int SpCudaStages::select_impl(const SpWorkspace& ws, int B, int k, long cap, long out_cap, int rank_all) const {
   sp_select_kernel<<<B, 1024, 0, stream>>>(ws.n_cand, ws.cand_pos, ws.cand_score, ws.sel_pos, ws.sel_score, ws.n_sel, k, cap, out_cap,

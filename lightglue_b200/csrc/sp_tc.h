@@ -23,6 +23,15 @@ struct SpTcPlan {
 SpTcPlan sp_tc_plan(int B, int H, int W);
 
 int sp_tc_create(SpTc** out, const float* wts_dev, cudaStream_t stream);
+
+// Post-processing kernels shared with DISK.  kp_compact: the pixels of scores [B, H, W] above thr, row-major, per image
+// at cand_* + b cap (row_count / row_start: [B H] scratch, n_cand [B]).  kp_select_above_kth: kornia's top-k of n =
+// k_max (k_max < 0: none): with k = min(n + 1, count), the candidates strictly above the k-th largest score, the first
+// n of them, in candidate order, into sel_* + b out_cap, counts into n_sel [B].
+int kp_compact(const float* scores, int B, int H, int W, float thr, long cap, int* row_count, int* row_start, int* n_cand,
+               int* cand_pos, float* cand_score, cudaStream_t stream);
+int kp_select_above_kth(const int* n_cand, const int* cand_pos, const float* cand_score, int* sel_pos, float* sel_score, int* n_sel,
+                        int B, int k_max, long cap, long out_cap, cudaStream_t stream);
 void sp_tc_destroy(SpTc* t);
 int sp_tc_backbone(SpTc* t, const float* wts_dev, const float* image, int B, int H, int W, void* workspace, float* logits_nchw,
                    float* dense_nchw, cudaStream_t stream);

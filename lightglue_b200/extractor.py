@@ -1,4 +1,4 @@
-"""Host shell shared by the extractors (``SuperPoint``, ``ALIKED``, ``SIFT``): checkpoint lookup, the C handle and
+"""Host shell shared by the extractors (``SuperPoint``, ``ALIKED``, ``SIFT``, ``DISK``): checkpoint lookup, the C handle and
 workspace caches, the forward call with its output allocation and count read-back, and ``Extractor.extract``."""
 from __future__ import annotations
 
