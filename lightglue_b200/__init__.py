@@ -5,7 +5,8 @@
 kernels behind the C ABI declared in ``include/lightglue_b200.h``.
 """
 from .disk import DISK  # noqa: F401
+from .dog_hardnet import DoGHardNet  # noqa: F401
 from .matcher import LightGlue  # noqa: F401
 from .sift import SIFT  # noqa: F401
 
-__all__ = ["DISK", "LightGlue", "SIFT"]
+__all__ = ["DISK", "DoGHardNet", "LightGlue", "SIFT"]

@@ -10,12 +10,14 @@ PREC = {"fp32": 0, "bf16": 1, "bf16x3": 2}
 K_ATTENTION, K_LINEAR, K_ASSIGN, K_OTHER = 0, 1, 2, 3
 ABI_VERSION = 3
 
-# include/superpoint_b200.h, include/aliked_b200.h, include/sift_b200.h and include/disk_b200.h: same library
+# include/superpoint_b200.h, include/aliked_b200.h, include/sift_b200.h, include/disk_b200.h and
+# include/doghardnet_b200.h: same library
 SP_ABI_VERSION = 2
 SP_TC_BUFFERS = 9  # buffers of the tensor-core backbone's workspace plan (sp_tc_layout)
 AL_ABI_VERSION = 1
 SIFT_ABI_VERSION = 1
 DISK_ABI_VERSION = 1
+DHN_ABI_VERSION = 1
 
 
 class LgConfig(C.Structure):
@@ -53,6 +55,13 @@ class DiskConfig(C.Structure):
     _fields_ = [
         ("abi_version", C.c_int32), ("max_num_keypoints", C.c_int32), ("nms_window_size", C.c_int32),
         ("pad_if_not_divisible", C.c_int32), ("detection_threshold", C.c_float),
+    ]
+
+
+class DhnConfig(C.Structure):
+    _fields_ = [
+        ("abi_version", C.c_int32), ("num_octave_layers", C.c_int32), ("nms_radius", C.c_int32),
+        ("max_num_keypoints", C.c_int32), ("detection_threshold", C.c_double), ("edge_threshold", C.c_double),
     ]
 
 
@@ -131,8 +140,17 @@ DISK_PROTOTYPES = {  # include/disk_b200.h
     "disk_forward": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _I32, _I64] + [_VP] * 5 + [_SZ, _VP]),
     "disk_heads": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _I32, _VP, _I32, _VP, _VP, _VP, _SZ, _VP]),
 }
-EXPORTS, SP_EXPORTS, AL_EXPORTS, SIFT_EXPORTS, DISK_EXPORTS = (
-    tuple(t) for t in (LG_PROTOTYPES, SP_PROTOTYPES, AL_PROTOTYPES, SIFT_PROTOTYPES, DISK_PROTOTYPES))
+DHN_PROTOTYPES = {  # include/doghardnet_b200.h
+    "dhn_weight_blob_floats": (_SZ, []),
+    "dhn_create": (C.c_int, [C.POINTER(DhnConfig), _VP, _SZ, _VP, _HANDLE_OUT]),
+    "dhn_destroy": (C.c_int, [_VP]),
+    "dhn_max_keypoints": (_I64, [_VP, _I32, _I32]),
+    "dhn_workspace_bytes": (_SZ, [_VP, _I32, _I32, _I32]),
+    "dhn_forward": (C.c_int, [_VP, _VP, _I32, _VP, _I32, _I32, _I32, _I64] + [_VP] * 7 + [_SZ, _VP]),
+    "dhn_describe": (C.c_int, [_VP, _VP, _I32, _VP, _I32, _I32, _I32, _I64] + [_VP] * 6 + [_SZ, _VP]),
+}
+EXPORTS, SP_EXPORTS, AL_EXPORTS, SIFT_EXPORTS, DISK_EXPORTS, DHN_EXPORTS = (
+    tuple(t) for t in (LG_PROTOTYPES, SP_PROTOTYPES, AL_PROTOTYPES, SIFT_PROTOTYPES, DISK_PROTOTYPES, DHN_PROTOTYPES))
 
 _lib = None
 
@@ -151,7 +169,7 @@ def load():
     if not os.path.exists(path):
         raise RuntimeError(f"{path} is missing: the CUDA library must be built (python -m lightglue_b200.build)")
     lib = C.CDLL(path)
-    for table in (LG_PROTOTYPES, SP_PROTOTYPES, AL_PROTOTYPES, SIFT_PROTOTYPES, DISK_PROTOTYPES):
+    for table in (LG_PROTOTYPES, SP_PROTOTYPES, AL_PROTOTYPES, SIFT_PROTOTYPES, DISK_PROTOTYPES, DHN_PROTOTYPES):
         for name, (restype, argtypes) in table.items():
             fn = getattr(lib, name)
             fn.restype, fn.argtypes = restype, argtypes

@@ -56,6 +56,12 @@ struct TcLinParams {
   // conv_plane = (H+2q)(W+2q), conv_rows = B conv_plane) and applies ReLU.
   int conv_cb, conv_k, conv_pad, conv_w2, conv_h, conv_w, relu;
   long conv_plane, conv_rows;
+  // stride-2 3x3 convolution by phase split (conv_pstride > 0): A holds the four polyphase images of the padded input,
+  // phase (py, px) = padded pixels (2i + py, 2j + px) at the output's padded position (i + 1, j + 1), phase 2 py + px
+  // starting at row (2 py + px) conv_pstride; tap (dy, dx) reads phase (dy & 1, dx & 1) shifted by (dy >> 1) conv_w2 +
+  // (dx >> 1) rows.  The A map then spans 4 conv_pstride rows (conv_arows), more than the output's.
+  int conv_pstride;
+  long conv_arows;
   int mma_n;  // N of the MMAs when fewer than 256 output columns exist (64 / 128; 0 = 256): the weight rows beyond are zero
   // TMA stores of the staged epilogues, 64-row boxes (one MMA warpgroup's rows): TEPI_QKV: q, k ([S H Lp, 64], box 64 x 64)
   // and vt ([S H 64, Lp], box 64 rows x 64 d); TEPI_RESID / F32 / CONV / LN_GELU: out_f32 (box 16 x 64, also the
@@ -225,7 +231,12 @@ __global__ void __launch_bounds__(LinCfg<EPI>::THREADS, 1) tc_linear_kernel(cons
           int arow = (int)ti.grow0;
           if (p.conv_cb) {  // convolution tap: shifted rows of the padded image, channel block kb % conv_cb
             const int tap = kb / p.conv_cb;
-            arow += (tap / p.conv_k - p.conv_pad) * p.conv_w2 + (tap % p.conv_k - p.conv_pad);
+            if (p.conv_pstride) {
+              const int dy = tap / 3, dx = tap % 3;
+              arow += ((dy & 1) * 2 + (dx & 1)) * p.conv_pstride + (dy >> 1) * p.conv_w2 + (dx >> 1);
+            } else {
+              arow += (tap / p.conv_k - p.conv_pad) * p.conv_w2 + (tap % p.conv_k - p.conv_pad);
+            }
             kc = (kb % p.conv_cb) * BK;
             seg = 0;
           }
@@ -711,8 +722,9 @@ int tc_gemm(TcEngine& e, const SeqState& st, const TcOperands& d, int n_tiles, T
   const uint64_t rows = (uint64_t)st.S * st.Lp;
   const uint64_t K = p.conv_cb ? (uint64_t)p.conv_k * p.conv_k * d.k0 : d.k0 + d.k1, nout = d.nout, nsel = d.nsel;
   const uint64_t sel_bytes = (nsel > 1 ? d.sel_stride : nout * K) * 2;
+  const uint64_t arows = p.conv_arows ? (uint64_t)p.conv_arows : rows;
   auto amap = [&](CUtensorMap* out, const void* a, uint64_t k) {  // box 64 x the tile height
-    return tc_tmap(e, {a, 2, {k, rows}, {k * 2}, {BK, TBM}}, out);
+    return tc_tmap(e, {a, 2, {k, arows}, {k * 2}, {BK, TBM}}, out);
   };
   auto wmap = [&](CUtensorMap* out, const void* w) { return tc_tmap(e, {w, 3, {K, nout, nsel}, {K * 2, sel_bytes}, {BK, BN, 1}}, out); };
   // maps the kernel does not read repeat a map it does (segment 1 of a one-segment A, every lo map in bf16)
@@ -905,12 +917,13 @@ int tc_final_proj(LgHandle* h, const TcBuffers& b, const SeqState& st, float* p_
   return run_linear(h, st, ops, 1, p, stream);
 }
 
-int tc_conv(TcEngine& e, const SeqState& st, const __nv_bfloat16* in_h, const __nv_bfloat16* in_l, int cin, int taps, size_t w_off,
-            const float* bias, int relu, int B, int H, int W, __nv_bfloat16* out_h, __nv_bfloat16* out_l, int cout, float* out_f32,
-            int ldo, cudaStream_t stream) {
-  if (cin % BK != 0 || (taps != 1 && taps != 9 && taps != 25))
-    return lg_set_error("tc_conv: Cin must be a multiple of 64, 1x1, 3x3 or 5x5");
+namespace {
+int conv_launch(TcEngine& e, const SeqState& st, const __nv_bfloat16* in_h, const __nv_bfloat16* in_l, int cin, int taps,
+                size_t w_off, const float* bias, int relu, int B, int H, int W, __nv_bfloat16* out_h, __nv_bfloat16* out_l, int cout,
+                float* out_f32, int ldo, int pstride, cudaStream_t stream) {
   TcLinParams p{};
+  p.conv_pstride = pstride;
+  p.conv_arows = pstride ? 4L * pstride : 0;
   p.epi = out_f32 ? TEPI_F32 : TEPI_CONV;
   p.scale = 1.f; p.bias = bias; p.relu = relu;
   p.out_f32 = out_f32; p.ldo = ldo; p.out_h = out_h; p.out_l = e.x3 ? out_l : nullptr; p.ldb = cout;
@@ -923,6 +936,22 @@ int tc_conv(TcEngine& e, const SeqState& st, const __nv_bfloat16* in_h, const __
   p.conv_plane = (long)(H + 2 * p.conv_pad) * p.conv_w2; p.conv_rows = (long)B * p.conv_plane;
   const TcOperands ops{in_h, in_l, cin, nullptr, nullptr, 0, e.w_hi + w_off, e.w_lo + w_off, BN, 1, 0};
   return tc_gemm(e, st, ops, 1, p, stream);
+}
+}  // namespace
+
+int tc_conv(TcEngine& e, const SeqState& st, const __nv_bfloat16* in_h, const __nv_bfloat16* in_l, int cin, int taps, size_t w_off,
+            const float* bias, int relu, int B, int H, int W, __nv_bfloat16* out_h, __nv_bfloat16* out_l, int cout, float* out_f32,
+            int ldo, cudaStream_t stream) {
+  if (cin % BK != 0 || (taps != 1 && taps != 9 && taps != 25))
+    return lg_set_error("tc_conv: Cin must be a multiple of 64, 1x1, 3x3 or 5x5");
+  return conv_launch(e, st, in_h, in_l, cin, taps, w_off, bias, relu, B, H, W, out_h, out_l, cout, out_f32, ldo, 0, stream);
+}
+
+int tc_conv_s2(TcEngine& e, const SeqState& st, const __nv_bfloat16* in_h, const __nv_bfloat16* in_l, int cin, int pstride,
+               size_t w_off, const float* bias, int relu, int B, int H, int W, __nv_bfloat16* out_h, __nv_bfloat16* out_l, int cout,
+               cudaStream_t stream) {
+  if (cin % BK != 0 || pstride <= 0) return lg_set_error("tc_conv_s2: Cin must be a multiple of 64 and the phase stride positive");
+  return conv_launch(e, st, in_h, in_l, cin, 9, w_off, bias, relu, B, H, W, out_h, out_l, cout, nullptr, 0, pstride, stream);
 }
 
 int tc_block(LgHandle* h, const TcBuffers& b, const SeqState& st, int layer, int blk, float* x, const float* cs,

@@ -58,3 +58,10 @@ int tc_attention(LgHandle* h, const TcBuffers& b, const SeqState& st, int kv_shi
 int tc_conv(TcEngine& e, const SeqState& st, const __nv_bfloat16* in_h, const __nv_bfloat16* in_l, int cin, int taps, size_t w_off,
             const float* bias, int relu, int B, int H, int W, __nv_bfloat16* out_h, __nv_bfloat16* out_l, int cout, float* out_f32,
             int ldo, cudaStream_t stream);
+// 3x3 convolution with stride 2 and zero padding 1 (HardNet) -> the padded layout of tc_conv at the OUTPUT size H x W.
+// in_h / in_l hold the four polyphase images of the padded input, each in the output's padded frame (W + 2 columns),
+// phase 2 py + px (padded input pixel (2i + py, 2j + px) at frame position (i + 1, j + 1)) starting at row
+// (2 py + px) pstride: tap (dy, dx) reads phase (dy & 1, dx & 1) shifted by (dy >> 1) (W + 2) + (dx >> 1) rows.
+int tc_conv_s2(TcEngine& e, const SeqState& st, const __nv_bfloat16* in_h, const __nv_bfloat16* in_l, int cin, int pstride,
+               size_t w_off, const float* bias, int relu, int B, int H, int W, __nv_bfloat16* out_h, __nv_bfloat16* out_l, int cout,
+               cudaStream_t stream);

@@ -107,3 +107,26 @@ extern "C" int sift_forward(SiftHandle* h, const float* image, int32_t channels,
   }
   return 0;
 }
+
+// DoG-HardNet's detection (dhn_api.cu): sift_forward's stages for one image, without the descriptor histograms.  The
+// functors stay compiled here only, with this file's -fmad=false.
+size_t sift_detect_workspace_bytes(const SiftConfig& c, int H, int W) {
+  SiftWs w;
+  sift_carve(nullptr, H, W, c.num_octave_layers, c.max_num_keypoints, &w);
+  return w.bytes + 256;
+}
+
+int sift_detect_image(const SiftConfig& c, const float* image, int channels, int H, int W, int h, int w, void* workspace,
+                      int64_t cap, float* keypoints, float* scales, float* oris, float* scores, int32_t* count,
+                      cudaStream_t stream) {
+  char* base = (char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  SiftWs ws;
+  sift_carve(base, H, W, c.num_octave_layers, c.max_num_keypoints, &ws);
+  CudaExec ex{stream};
+  const SiftParams p = sift_params(c.num_octave_layers, c.detection_threshold, c.edge_threshold, c.nms_radius,
+                                   c.max_num_keypoints, 0);
+  LG_RC(sift_run(ex, p, image, channels, H, W, h, w, ws, (int)cap, keypoints, scales, oris, scores, nullptr));
+  sift_count_kernel<<<1, 1, 0, stream>>>(ws.counters, count);
+  LG_CHECK_LAUNCH();
+  return 0;
+}

@@ -571,21 +571,22 @@ struct SiftDescribe {
   SiftPost s; SiftParams p;
   const int* out_src;
   int cap_out;
-  float* kpts; float* scales; float* oris; float* scores; float* desc;  // this image's rows
+  float* kpts; float* scales; float* oris; float* scores; float* desc;  // this image's rows; desc null: no descriptors
   static constexpr int SCRATCH = SIFT_DESC_HIST;
   SIFT_HD long count() const { return cap_out; }
   SIFT_HD void operator()(long slot, float* hist) const {
     const int n_out = s.counters[2];
-    float* dst = desc + slot * SIFT_DESC;
     if (slot >= n_out) {
       kpts[2 * slot] = kpts[2 * slot + 1] = 0.f;
       scales[slot] = oris[slot] = scores[slot] = 0.f;
-      for (int k = 0; k < SIFT_DESC; ++k) dst[k] = 0.f;
+      for (int k = 0; desc && k < SIFT_DESC; ++k) desc[slot * SIFT_DESC + k] = 0.f;
       return;
     }
     const SiftKpt kp = s.kpt[s.order[out_src[slot]]];
     kpts[2 * slot] = kp.x; kpts[2 * slot + 1] = kp.y;
     scales[slot] = kp.size; oris[slot] = sift_deg2rad(kp.angle); scores[slot] = kp.response;
+    if (!desc) return;
+    float* dst = desc + slot * SIFT_DESC;
 
     // unpackOctave: scale = 1 / 2^octave (2 for octave -1)
     const int octave = kp.o - 1;

@@ -1,5 +1,6 @@
-"""Host shell shared by the extractors (``SuperPoint``, ``ALIKED``, ``SIFT``, ``DISK``): checkpoint lookup, the C handle and
-workspace caches, the forward call with its output allocation and count read-back, and ``Extractor.extract``."""
+"""Host shell shared by the extractors (``SuperPoint``, ``ALIKED``, ``SIFT``, ``DISK``, ``DoGHardNet``): checkpoint
+lookup, the C handle and workspace caches, the forward call with its output allocation and count read-back, and
+``Extractor.extract``."""
 from __future__ import annotations
 
 import ctypes as C
