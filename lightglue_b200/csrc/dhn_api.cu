@@ -12,11 +12,12 @@
 //     std normalisation, conv 0 (1 -> 32, K = 9, fp32, folded BatchNorm + ReLU) -> padded NHWC bf16 hi / lo, 34 x 34
 //     per patch, 32 channels zero-padded to 64
 //     conv 1 (3x3) / conv 3 (3x3) / conv 5 (3x3) on the tensor cores (tc_conv); conv 2 and conv 4 (stride 2) as
-//     tc_conv_s2 over the four polyphase images of their padded input (dhn_phase_kernel), each held in the output's
-//     padded frame (18 x 18, 10 x 10)
+//     tc_conv by phase split over the four polyphase images of their padded input (dhn_phase_kernel), each held in the
+//     output's padded frame (18 x 18, 10 x 10)
 //     dhn_gather_kernel: the 8 x 8 x 128 output of conv 5 of every keypoint -> one [8192] row
 //   conv 6 (8 x 8, K = 8192) as one tensor-core GEMM over the image's gathered rows (fp32 out), then F.normalize.
-// Every BatchNorm (eval, affine=False) is folded into its convolution's weights and a bias at dhn_create, in double.
+// Every BatchNorm (eval, affine=False) is folded into its convolution's weights and a bias at dhn_create, in double
+// (tc_conv_weights_create).
 // GEMM rows past the device-side keypoint count are skipped through SeqState.len: nothing is read back to the host.
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -54,14 +55,6 @@ size_t layer_blob_off(int l) {  // weight [cout, cin, k, k], running_mean [cout]
   return o;
 }
 
-struct Lvl { int Lp; long rows; };
-Lvl rows_level(long used) {  // two 128-row tile sequences of Lp rows (as sp_tc.cu / disk_api.cu)
-  Lvl l;
-  l.Lp = (int)std::max<long>(LG_TILE, ((used + 1) / 2 + LG_TILE - 1) / LG_TILE * LG_TILE);
-  l.rows = 2L * l.Lp;
-  return l;
-}
-
 struct PyrTab {  // levels of one image's pyramid: float offset in the pyramid buffer, height, width
   int n;
   long off[MAXLV];
@@ -87,16 +80,16 @@ long pyr_floats(int h, int w) {
 struct Geo {
   int cap;  // keypoints per image (max_num_keypoints)
   int nchunk;
-  Lvl A, B, C, D;  // 32 x 32, 16 x 16, 8 x 8 levels of one chunk; conv 6 rows of one image
+  TcRows A, B, C, D;  // 32 x 32, 16 x 16, 8 x 8 levels of one chunk; conv 6 rows of one image
 };
 Geo geometry(int cap) {
   Geo g;
   g.cap = cap;
   g.nchunk = (cap + NP - 1) / NP;
-  g.A = rows_level((long)NP * RA);
-  g.B = rows_level((long)NP * RB);
-  g.C = rows_level((long)NP * RC);
-  g.D = rows_level(cap);
+  g.A = tc_rows((long)NP * RA);
+  g.B = tc_rows((long)NP * RB);
+  g.C = tc_rows((long)NP * RC);
+  g.D = tc_rows(cap);
   return g;
 }
 
@@ -180,7 +173,7 @@ __global__ void __launch_bounds__(256) dhn_pyrdown_kernel(const float* __restric
   out[i] = (1.f - ly) * ((1.f - lx) * blur(y0, x0) + lx * blur(y0, x1)) + ly * ((1.f - lx) * blur(y1, x0) + lx * blur(y1, x1));
 }
 
-// SeqState words of every chunk and level, and of conv 6, from the device-side keypoint count
+// the tc_rows_state words of every chunk and level, and of conv 6, from the device-side keypoint count
 __global__ void dhn_state_kernel(const int* __restrict__ count, long cap, int nchunk, int lpa, int lpb, int lpc, int lpd,
                                  int* __restrict__ st) {
   const int n = n_valid(count, cap);
@@ -203,14 +196,16 @@ __global__ void dhn_state_kernel(const int* __restrict__ count, long cap, int nc
 __global__ void __launch_bounds__(256) dhn_patch_kernel(const float* __restrict__ pyr, const PyrTab t, const float* __restrict__ kpts,
                                                         const float* __restrict__ scales, const float* __restrict__ oris,
                                                         const int* __restrict__ count, long cap, int k0, const float* __restrict__ w0,
-                                                        __nv_bfloat16* __restrict__ oh, __nv_bfloat16* __restrict__ ol) {
+                                                        const float* __restrict__ b0, __nv_bfloat16* __restrict__ oh,
+                                                        __nv_bfloat16* __restrict__ ol) {
   __shared__ float sp[34 * 34];  // normalised patch, pixel (i, j) at (i + 1, j + 1), zero border
   __shared__ float sw[32 * 9 + 32];
   __shared__ float red[8];
   const int p = blockIdx.x, tid = threadIdx.x;
   const int k = k0 + p;
   if (k >= n_valid(count, cap)) return;
-  for (int i = tid; i < 32 * 9 + 32; i += 256) sw[i] = w0[i];
+  for (int i = tid; i < 32 * 9; i += 256) sw[i] = w0[i];
+  if (tid < 32) sw[32 * 9 + tid] = b0[tid];
   for (int i = tid; i < 34 * 34; i += 256) sp[i] = 0.f;
   // LAF = [[s cos, s sin, x], [-s sin, s cos, y]], s = 6 size; its level: floor(clamp(log2(2 sqrt(|det| + 1e-10) / 32),
   // 0, max(0, min(h, w) // 32 - 1))), computed in double
@@ -289,8 +284,9 @@ __global__ void __launch_bounds__(256) dhn_patch_kernel(const float* __restrict_
     uint32_t hv[4], lv4[4];
 #pragma unroll
     for (int c = 0; c < 4; ++c) {
-      const __nv_bfloat162 h2 = __floats2bfloat162_rn(o[2 * c], o[2 * c + 1]);
-      const __nv_bfloat162 l2 = __floats2bfloat162_rn(o[2 * c] - __bfloat162float(h2.x), o[2 * c + 1] - __bfloat162float(h2.y));
+      __nv_bfloat162 h2, l2;
+      tc_split(o[2 * c], h2.x, l2.x);
+      tc_split(o[2 * c + 1], h2.y, l2.y);
       hv[c] = *reinterpret_cast<const uint32_t*>(&h2);
       lv4[c] = *reinterpret_cast<const uint32_t*>(&l2);
     }
@@ -359,28 +355,12 @@ __global__ void __launch_bounds__(DESC) dhn_finish_kernel(const float* __restric
   desc[j * DESC + c] = v / fmaxf(sqrtf(red[0] + red[1] + red[2] + red[3]), 1e-12f);
 }
 
-// BatchNorm (eval, eps 1e-5) folded into conv weights [cout, cin, taps] -> [rows, K] (column tap cpad + ci; zero past
-// cin / taps / cout) and bias [rows], in double
-__global__ void dhn_fold_kernel(const float* __restrict__ w, const float* __restrict__ mean, const float* __restrict__ var, int cin,
-                                int cpad, int taps, int cout, int K, float* __restrict__ wo, float* __restrict__ bo) {
-  const int r = blockIdx.x;
-  const double rs = r < cout ? 1.0 / sqrt((double)var[r] + 1e-5) : 0.0;
-  for (int idx = threadIdx.x; idx < K; idx += blockDim.x) {
-    const int tp = idx / cpad, ci = idx % cpad;
-    wo[(size_t)r * K + idx] = (r < cout && tp < taps && ci < cin) ? (float)((double)w[((size_t)r * cin + ci) * taps + tp] * rs) : 0.f;
-  }
-  if (threadIdx.x == 0) bo[r] = r < cout ? (float)(-(double)mean[r] * rs) : 0.f;
-}
-
 }  // namespace
 
 struct DhnHandle {
   DhnConfig cfg;
   SiftConfig sift;
-  float* wts;  // device copy of the weight blob
-  float* wpk;  // folded fp32 weights: conv 0 [32, 9] + [32]; convs 1..6 [256, K] + [256]
-  TcEngine tc;
-  size_t w_off[NL], b_off[NL];
+  TcConvWeights* cw;  // region l = conv l, BatchNorm folded: conv 0 [32, 9] (CUDA cores); convs 1..6 [256, K]
 };
 
 namespace {
@@ -406,32 +386,34 @@ int run_hardnet(DhnHandle* h, const Geo& g, const DhnWs& w, const float* image, 
   const int nchunk = (int)((ncap + NP - 1) / NP);
   dhn_state_kernel<<<1, 1, 0, s>>>(count, ncap, nchunk, g.A.Lp, g.B.Lp, g.C.Lp, g.D.Lp, w.state);
   LG_CHECK_LAUNCH();
-  auto st = [&](int c, int lev, const Lvl& L) {
-    int* p = w.state + (c * 3 + lev) * 4;
-    return SeqState{2, 1, L.Lp, p, p + 2};
-  };
-  const float* wp = h->wpk;
+  TcConvWeights& cw = *h->cw;
   for (int c = 0; c < nchunk; ++c) {
     const int k0 = c * NP;
-    dhn_patch_kernel<<<NP, 256, 0, s>>>(w.pyr, t, kpts, scales, oris, count, ncap, k0, wp + h->w_off[0], w.uh, w.ul);
+    const int* sw = w.state + c * 12;  // levels A, B, C of this chunk
+    dhn_patch_kernel<<<NP, 256, 0, s>>>(w.pyr, t, kpts, scales, oris, count, ncap, k0, cw.wpk + cw.w_off[0], cw.wpk + cw.b_off[0],
+                                        w.uh, w.ul);
     LG_CHECK_LAUNCH();
-    LG_RC(tc_conv(h->tc, st(c, 0, g.A), w.uh, w.ul, 64, 9, h->w_off[1], wp + h->b_off[1], 1, NP, PS, PS, w.vh, w.vl, 64, nullptr, 0, s));
+    LG_RC(tc_conv(cw, tc_rows_state(g.A, sw), {.in_h = w.uh, .in_l = w.ul, .cin = 64, .taps = 9, .region = 1, .relu = 1, .B = NP,
+                  .H = PS, .W = PS, .out_h = w.vh, .out_l = w.vl, .cout = 64}, s));
     const long nb = 4L * NP * RB * 8;
     dhn_phase_kernel<<<(unsigned)((nb + 255) / 256), 256, 0, s>>>(w.vh, w.vl, 34, 18, count, ncap, k0, g.B.rows, w.uh, w.ul);
     LG_CHECK_LAUNCH();
-    LG_RC(tc_conv_s2(h->tc, st(c, 1, g.B), w.uh, w.ul, 64, (int)g.B.rows, h->w_off[2], wp + h->b_off[2], 1, NP, 16, 16, w.bh, w.bl, 64, s));
-    LG_RC(tc_conv(h->tc, st(c, 1, g.B), w.bh, w.bl, 64, 9, h->w_off[3], wp + h->b_off[3], 1, NP, 16, 16, w.b2h, w.b2l, 64, nullptr, 0, s));
+    LG_RC(tc_conv(cw, tc_rows_state(g.B, sw + 4), {.in_h = w.uh, .in_l = w.ul, .cin = 64, .taps = 9, .pstride = (int)g.B.rows,
+                  .region = 2, .relu = 1, .B = NP, .H = 16, .W = 16, .out_h = w.bh, .out_l = w.bl, .cout = 64}, s));
+    LG_RC(tc_conv(cw, tc_rows_state(g.B, sw + 4), {.in_h = w.bh, .in_l = w.bl, .cin = 64, .taps = 9, .region = 3, .relu = 1,
+                  .B = NP, .H = 16, .W = 16, .out_h = w.b2h, .out_l = w.b2l, .cout = 64}, s));
     const long nc = 4L * NP * RC * 8;
     dhn_phase_kernel<<<(unsigned)((nc + 255) / 256), 256, 0, s>>>(w.b2h, w.b2l, 18, 10, count, ncap, k0, g.C.rows, w.vh, w.vl);
     LG_CHECK_LAUNCH();
-    LG_RC(tc_conv_s2(h->tc, st(c, 2, g.C), w.vh, w.vl, 64, (int)g.C.rows, h->w_off[4], wp + h->b_off[4], 1, NP, 8, 8, w.ch, w.cl, 128, s));
-    LG_RC(tc_conv(h->tc, st(c, 2, g.C), w.ch, w.cl, 128, 9, h->w_off[5], wp + h->b_off[5], 1, NP, 8, 8, w.c2h, w.c2l, 128, nullptr, 0, s));
+    LG_RC(tc_conv(cw, tc_rows_state(g.C, sw + 8), {.in_h = w.vh, .in_l = w.vl, .cin = 64, .taps = 9, .pstride = (int)g.C.rows,
+                  .region = 4, .relu = 1, .B = NP, .H = 8, .W = 8, .out_h = w.ch, .out_l = w.cl, .cout = 128}, s));
+    LG_RC(tc_conv(cw, tc_rows_state(g.C, sw + 8), {.in_h = w.ch, .in_l = w.cl, .cin = 128, .taps = 9, .region = 5, .relu = 1,
+                  .B = NP, .H = 8, .W = 8, .out_h = w.c2h, .out_l = w.c2l, .cout = 128}, s));
     dhn_gather_kernel<<<NP, 256, 0, s>>>(w.c2h, w.c2l, count, ncap, k0, w.gh, w.gl);
     LG_CHECK_LAUNCH();
   }
-  int* sd = w.state + nchunk * 12;
-  LG_RC(tc_conv(h->tc, SeqState{2, 1, g.D.Lp, sd, sd + 2}, w.gh, w.gl, K6, 1, h->w_off[6], wp + h->b_off[6], 0, 1, 1, 1, nullptr,
-                nullptr, DESC, w.dout, DESC, s));
+  LG_RC(tc_conv(cw, tc_rows_state(g.D, w.state + nchunk * 12),
+                {.in_h = w.gh, .in_l = w.gl, .cin = K6, .taps = 1, .region = 6, .cout = DESC, .out_f32 = w.dout, .ldo = DESC}, s));
   if (out_rows > 0) {
     dhn_finish_kernel<<<(unsigned)out_rows, DESC, 0, s>>>(w.dout, count, ncap, desc);
     LG_CHECK_LAUNCH();
@@ -472,26 +454,16 @@ extern "C" int dhn_create(const DhnConfig* cfg, const float* weights_dev, size_t
     DhnHandle* h;
     ~Guard() { if (h) dhn_destroy(h); }
   } guard{h};
-  LG_CU(cudaMalloc(&h->wts, n_floats * sizeof(float)));
-  LG_CU(cudaMemcpyAsync(h->wts, weights_dev, n_floats * sizeof(float), cudaMemcpyDeviceToDevice, stream));
-  size_t c = 0;
-  int rows[NL], kld[NL], cpd[NL];
+  TcConvRegion reg[NL];
   for (int l = 0; l < NL; ++l) {
-    rows[l] = l == 0 ? 32 : 256;
-    cpd[l] = l == 0 ? 1 : (l == NL - 1 ? HL[l].cin : (HL[l].cin + 63) / 64 * 64);
-    kld[l] = HL[l].k * HL[l].k * cpd[l];
-    h->w_off[l] = c; c += (size_t)rows[l] * kld[l];
-    h->b_off[l] = c; c += rows[l];
+    const HLayer& L = HL[l];
+    const int taps = L.k * L.k, cp = l == 0 ? 1 : (l == NL - 1 ? L.cin : (L.cin + 63) / 64 * 64);
+    const float* w = weights_dev + layer_blob_off(l);
+    const float* mean = w + (size_t)L.cout * L.cin * taps;
+    reg[l] = {.w = w, .bn_mean = mean, .bn_var = mean + L.cout, .cin = L.cin, .cpad = cp, .taps = taps, .rows = l == 0 ? 32 : 256,
+              .K = taps * cp, .ncopy = L.cout};
   }
-  LG_CU(cudaMalloc(&h->wpk, c * sizeof(float)));
-  for (int l = 0; l < NL; ++l) {
-    const float* w = h->wts + layer_blob_off(l);
-    const float* mean = w + (size_t)HL[l].cout * HL[l].cin * HL[l].k * HL[l].k;
-    dhn_fold_kernel<<<rows[l], 256, 0, stream>>>(w, mean, mean + HL[l].cout, HL[l].cin, cpd[l], HL[l].k * HL[l].k, HL[l].cout, kld[l],
-                                                 h->wpk + h->w_off[l], h->wpk + h->b_off[l]);
-  }
-  LG_CHECK_LAUNCH();
-  LG_RC(tc_engine_create(&h->tc, h->wpk, c, true, stream));
+  LG_RC(tc_conv_weights_create(&h->cw, reg, NL, stream));
   guard.h = nullptr;
   *out = h;
   return 0;
@@ -499,9 +471,7 @@ extern "C" int dhn_create(const DhnConfig* cfg, const float* weights_dev, size_t
 
 extern "C" int dhn_destroy(DhnHandle* h) {
   if (!h) return 0;
-  tc_engine_destroy(&h->tc);
-  cudaFree(h->wpk);
-  cudaFree(h->wts);
+  tc_conv_weights_destroy(h->cw);
   delete h;
   return 0;
 }

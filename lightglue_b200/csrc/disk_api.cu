@@ -13,7 +13,7 @@
 // over gathered im2col rows (K = 2000, padded to 2048).
 //
 // Feature maps: fp32 or bf16, NHWC with a 2-pixel zero border, row = b (H+4)(W+4) + (y+2)(W+4) + (x+2), as tc_conv
-// reads them; each level holds 2 Lp rows (two 128-row tile sequences, as sp_tc.cu).
+// reads them; each level holds the rows of its tc_rows plan (lg_tc.h).
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 
@@ -36,6 +36,7 @@ constexpr DLayer DL[NL] = {{3, 16, 0},   {16, 32, 1},  {32, 64, 2},  {64, 64, 3}
 constexpr int TAPS = 25;
 constexpr int DESC = 128, X3C = 80, DK = TAPS * X3C, DKP = 2048;  // descriptor head: K = 2000, padded to 32 blocks of 64
 constexpr int MAXC = 128;       // widest layer input
+constexpr int HEAT = NL - 1;    // packed region of the heatmap channel
 constexpr int STAT_CHUNK = 1024;  // pixels per partial-statistics block
 
 int cpad(int c) { return (c + 63) / 64 * 64; }
@@ -45,26 +46,11 @@ size_t layer_blob_off(int l) {  // slope [cin], weight [cout, cin, 5, 5], bias [
   return o;
 }
 
-struct Level { int H, W, Lp; long rows; };
-Level level(int B, int H, int W) {
-  Level l{H, W, 0, 0};
-  const long used = (long)B * (H + 4) * (W + 4);
-  l.Lp = (int)(((used + 1) / 2 + LG_TILE - 1) / LG_TILE * LG_TILE);
-  l.rows = 2L * l.Lp;
-  return l;
-}
-Level rows_level(long used) {  // a plain GEMM over `used` rows
-  Level l{0, 0, 0, 0};
-  l.Lp = (int)std::max<long>(LG_TILE, ((used + 1) / 2 + LG_TILE - 1) / LG_TILE * LG_TILE);
-  l.rows = 2L * l.Lp;
-  return l;
-}
-
 struct Geo {
   int B, H, W, Hp, Wp;
-  Level lv[5];
+  TcRows lv[5];     // level i: Hp >> i by Wp >> i
   long ccap, ocap;  // candidates per image (NMS packing bound), output rows per image
-  Level ld;         // descriptor GEMM rows (B ocap)
+  TcRows ld;        // descriptor GEMM rows (B ocap)
 };
 
 long nms_bound(int w, int H, int W) {
@@ -80,10 +66,10 @@ Geo geometry(const DiskConfig& c, int B, int H, int W) {
   g.B = B; g.H = H; g.W = W;
   g.Hp = c.pad_if_not_divisible ? (H + 15) / 16 * 16 : H;
   g.Wp = c.pad_if_not_divisible ? (W + 15) / 16 * 16 : W;
-  for (int i = 0; i < 5; ++i) g.lv[i] = level(B, g.Hp >> i, g.Wp >> i);
+  for (int i = 0; i < 5; ++i) g.lv[i] = tc_rows((long)B * ((g.Hp >> i) + 4) * ((g.Wp >> i) + 4));
   g.ccap = nms_bound(c.nms_window_size, H, W);
   g.ocap = out_cap(c, H, W);
-  g.ld = rows_level((long)B * g.ocap);
+  g.ld = tc_rows((long)B * g.ocap);
   return g;
 }
 
@@ -239,13 +225,8 @@ __global__ void __launch_bounds__(256) disk_apply_kernel(const Prep p, const flo
   float v = 0.f;
   if (c < p.C && b < p.B && y >= 0 && y < p.H && x >= 0 && x < p.W)
     v = prelu((prep_val(p, (int)b, y, x, c) - mean[b * MAXC + c]) * rstd[b * MAXC + c], slope[c]);
-  if (of) {
-    of[i] = v;
-  } else {
-    const __nv_bfloat16 h = __float2bfloat16_rn(v);
-    oh[i] = h;
-    ol[i] = __float2bfloat16_rn(v - __bfloat162float(h));
-  }
+  if (of) of[i] = v;
+  else tc_split(v, oh[i], ol[i]);
 }
 
 // down0: the image's instance norm and PReLU fused into the 3 -> 16 convolution (K = 75), fp32; one thread per pixel of
@@ -342,9 +323,7 @@ __global__ void __launch_bounds__(256) disk_gather_kernel(const float* __restric
       const int t = col / X3C, ci = col % X3C;
       v = base[((long)(t / 5) * (Wp + 4) + t % 5) * X3C + ci];
     }
-    const __nv_bfloat16 h = __float2bfloat16_rn(v);
-    oh[row * DKP + col] = h;
-    ol[row * DKP + col] = __float2bfloat16_rn(v - __bfloat162float(h));
+    tc_split(v, oh[row * DKP + col], ol[row * DKP + col]);
   }
 }
 
@@ -385,26 +364,14 @@ __global__ void disk_fill_kernel(int* p, int n, int v) {
   if ((int)threadIdx.x < n) p[threadIdx.x] = v;
 }
 
-// [cout, cin, 5, 5] rows co0 .. co0 + ncopy - 1 -> [rows, K_ld] (column tap cpad + ci; zero past cin / tap 25 / ncopy), bias
-__global__ void disk_repack_kernel(const float* __restrict__ w, const float* __restrict__ b, float* __restrict__ wo,
-                                   float* __restrict__ bo, int cin, int cpad_, int K_ld, int co0, int ncopy) {
-  const int r = blockIdx.x;
-  for (int idx = threadIdx.x; idx < K_ld; idx += blockDim.x) {
-    const int t = idx / cpad_, ci = idx % cpad_;
-    wo[(size_t)r * K_ld + idx] = (r < ncopy && t < TAPS && ci < cin) ? w[((size_t)(co0 + r) * cin + ci) * TAPS + t] : 0.f;
-  }
-  if (threadIdx.x == 0) bo[r] = r < ncopy ? b[co0 + r] : 0.f;
-}
-
 }  // namespace
 
 struct DiskHandle {
   DiskConfig cfg;
   float* wts;  // device copy of the weight blob
-  float* wpk;  // packed fp32 weights: tensor-core layers, descriptor head, heatmap channel
-  TcEngine tc;
-  size_t w_off[NL], b_off[NL];  // layers 1..7: [256, 25 cpad(cin)], [256]; layer 8: descriptor head [256, 2048], [256]
-  size_t hw_off, hb_off;        // heatmap channel: [2000] (tap 80 + ci), [1]
+  // packed regions: l - 1 = layer l (1..7) [256, 25 cpad(cin)]; NL - 2 = up3's descriptor head [256, 2048]; HEAT = up3's
+  // heatmap channel [1, 2000] (tap 80 + ci)
+  TcConvWeights* cw;
 };
 
 namespace {
@@ -419,27 +386,23 @@ int launch_stats(const Prep& p, const DiskWs& w, cudaStream_t s) {
 // the input of layer l >= 1 (kornia's Unet.forward)
 Prep layer_input(const Geo& g, const DiskWs& w, int l) {
   Prep p{};
-  const Level& L = g.lv[DL[l].level];
-  p.B = g.B; p.H = L.H; p.W = L.W; p.C = DL[l].cin;
+  const int L = DL[l].level, S = DL[l - 1].level;
+  p.B = g.B; p.H = g.Hp >> L; p.W = g.Wp >> L; p.C = DL[l].cin;
   if (l <= 4) {  // avg_pool2d(2) of the previous down block's output
-    const Level& S = g.lv[DL[l - 1].level];
-    p.s[0] = Seg{w.raw[l - 1], DL[l - 1].cout, DL[l - 1].cout, SRC_POOL, S.H, S.W};
+    p.s[0] = Seg{w.raw[l - 1], DL[l - 1].cout, DL[l - 1].cout, SRC_POOL, g.Hp >> S, g.Wp >> S};
   } else {  // cat([upsample(bottom), horizontal])
     const int hl = 8 - l;  // horizontal: down block 3, 2, 1, 0
-    const Level& S = g.lv[DL[l - 1].level];
-    const Level& Hz = g.lv[DL[hl].level];
-    p.s[0] = Seg{w.raw[l - 1], DL[l - 1].cout, DL[l - 1].cout, SRC_UP, S.H, S.W};
-    p.s[1] = Seg{w.raw[hl], DL[hl].cout, DL[hl].cout, SRC_DIRECT, Hz.H, Hz.W};
+    const int Hz = DL[hl].level;
+    p.s[0] = Seg{w.raw[l - 1], DL[l - 1].cout, DL[l - 1].cout, SRC_UP, g.Hp >> S, g.Wp >> S};
+    p.s[1] = Seg{w.raw[hl], DL[hl].cout, DL[hl].cout, SRC_DIRECT, g.Hp >> Hz, g.Wp >> Hz};
   }
   return p;
 }
 
 // the U-Net up to the heatmap: writes w.x3 (up3 input) and heat [B, H, W]
 int run_unet(DiskHandle* h, const float* image, int Cimg, const Geo& g, const DiskWs& w, float* heat, cudaStream_t s) {
-  int host_st[24] = {0};
-  for (int i = 0; i < 5; ++i) { host_st[4 * i] = g.lv[i].Lp; host_st[4 * i + 1] = g.lv[i].Lp; }
-  host_st[20] = g.ld.Lp; host_st[21] = g.ld.Lp;
-  LG_CU(cudaMemcpyAsync(w.state, host_st, sizeof(host_st), cudaMemcpyHostToDevice, s));
+  const TcRows plans[6] = {g.lv[0], g.lv[1], g.lv[2], g.lv[3], g.lv[4], g.ld};
+  LG_RC(tc_rows_words(plans, 6, w.state, s));
   {  // down0
     Prep p{};
     p.B = g.B; p.H = g.Hp; p.W = g.Wp; p.C = 3;
@@ -452,7 +415,7 @@ int run_unet(DiskHandle* h, const float* image, int Cimg, const Geo& g, const Di
   }
   for (int l = 1; l < NL; ++l) {
     const Prep p = layer_input(g, w, l);
-    const Level& L = g.lv[DL[l].level];
+    const TcRows& L = g.lv[DL[l].level];
     LG_RC(launch_stats(p, w, s));
     const float* slope = h->wts + layer_blob_off(l);
     const int cp = l < NL - 1 ? cpad(DL[l].cin) : X3C;
@@ -461,14 +424,13 @@ int run_unet(DiskHandle* h, const float* image, int Cimg, const Geo& g, const Di
                                                                   l < NL - 1 ? nullptr : w.x3);
     LG_CHECK_LAUNCH();
     if (l == NL - 1) break;
-    const int li = DL[l].level;
-    const SeqState st{2, 1, L.Lp, w.state + 4 * li, w.state + 4 * li + 2};
-    LG_RC(tc_conv(h->tc, st, w.ah, w.al, cp, TAPS, h->w_off[l], h->wpk + h->b_off[l], 0, g.B, L.H, L.W, nullptr, nullptr,
-                  DL[l].cout, w.raw[l], DL[l].cout, s));
+    LG_RC(tc_conv(*h->cw, tc_rows_state(L, w.state + 4 * DL[l].level), {.in_h = w.ah, .in_l = w.al, .cin = cp, .taps = TAPS,
+                  .region = l - 1, .B = g.B, .H = p.H, .W = p.W, .cout = DL[l].cout, .out_f32 = w.raw[l], .ldo = DL[l].cout}, s));
   }
   const long n = (long)g.B * g.H * g.W;
-  disk_heatmap_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(w.x3, h->wpk + h->hw_off, h->wpk + h->hb_off, g.B, g.H, g.W,
-                                                                  g.Hp, g.Wp, heat);
+  const TcConvWeights& cw = *h->cw;
+  disk_heatmap_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(w.x3, cw.wpk + cw.w_off[HEAT], cw.wpk + cw.b_off[HEAT], g.B, g.H,
+                                                                  g.W, g.Hp, g.Wp, heat);
   LG_CHECK_LAUNCH();
   return 0;
 }
@@ -477,12 +439,11 @@ int run_unet(DiskHandle* h, const float* image, int Cimg, const Geo& g, const Di
 int run_desc(DiskHandle* h, const Geo& g, const DiskWs& w, const int* n_sel, const int* sel_pos, const float* sel_score, long oc,
              long out_stride, int normalize, float* kpts, float* scores, float* desc, cudaStream_t s) {
   if (oc <= 0 || out_stride <= 0) return 0;
-  const Level ld = rows_level((long)g.B * oc);
+  const TcRows ld = tc_rows((long)g.B * oc);
   disk_gather_kernel<<<(unsigned)ld.rows, 256, 0, s>>>(w.x3, n_sel, sel_pos, g.B, g.W, g.Hp, g.Wp, oc, w.dh, w.dl);
   LG_CHECK_LAUNCH();
-  const SeqState st{2, 1, ld.Lp, w.state + 20, w.state + 22};
-  LG_RC(tc_conv(h->tc, st, w.dh, w.dl, DKP, 1, h->w_off[NL - 1], h->wpk + h->b_off[NL - 1], 0, 1, 1, 1, nullptr, nullptr, DESC,
-                w.dout, DESC, s));
+  LG_RC(tc_conv(*h->cw, tc_rows_state(ld, w.state + 20), {.in_h = w.dh, .in_l = w.dl, .cin = DKP, .taps = 1, .region = NL - 2,
+                .cout = DESC, .out_f32 = w.dout, .ldo = DESC}, s));
   disk_finish_kernel<<<dim3((unsigned)out_stride, g.B), DESC, 0, s>>>(w.dout, n_sel, sel_pos, sel_score, g.W, oc, out_stride,
                                                                       normalize, kpts, scores, desc);
   LG_CHECK_LAUNCH();
@@ -519,27 +480,19 @@ extern "C" int disk_create(const DiskConfig* cfg, const float* weights_dev, size
   } guard{h};
   LG_CU(cudaMalloc(&h->wts, n_floats * sizeof(float)));
   LG_CU(cudaMemcpyAsync(h->wts, weights_dev, n_floats * sizeof(float), cudaMemcpyDeviceToDevice, stream));
-  size_t c = 0;
-  for (int l = 1; l < NL; ++l) {
-    h->w_off[l] = c; c += (size_t)256 * (l < NL - 1 ? TAPS * cpad(DL[l].cin) : DKP);
-    h->b_off[l] = c; c += 256;
-  }
-  h->hw_off = c; c += DK;
-  h->hb_off = c; c += 256;
-  LG_CU(cudaMalloc(&h->wpk, c * sizeof(float)));
-  for (int l = 1; l < NL; ++l) {
+  TcConvRegion reg[NL];
+  for (int l = 1; l < NL; ++l) {  // up3 (l = NL - 1): the descriptor head, then the heatmap channel
     const float* w = h->wts + layer_blob_off(l) + DL[l].cin;
     const float* b = w + (size_t)DL[l].cout * DL[l].cin * TAPS;
-    if (l < NL - 1)
-      disk_repack_kernel<<<256, 256, 0, stream>>>(w, b, h->wpk + h->w_off[l], h->wpk + h->b_off[l], DL[l].cin, cpad(DL[l].cin),
-                                                 TAPS * cpad(DL[l].cin), 0, DL[l].cout);
-    else {
-      disk_repack_kernel<<<256, 256, 0, stream>>>(w, b, h->wpk + h->w_off[l], h->wpk + h->b_off[l], X3C, X3C, DKP, 0, DESC);
-      disk_repack_kernel<<<1, 256, 0, stream>>>(w, b, h->wpk + h->hw_off, h->wpk + h->hb_off, X3C, X3C, DK, DESC, 1);
+    const int cin = DL[l].cin, cp = cpad(cin);
+    if (l < NL - 1) {
+      reg[l - 1] = {.w = w, .b = b, .cin = cin, .cpad = cp, .taps = TAPS, .rows = 256, .K = TAPS * cp, .ncopy = DL[l].cout};
+    } else {
+      reg[l - 1] = {.w = w, .b = b, .cin = X3C, .cpad = X3C, .taps = TAPS, .rows = 256, .K = DKP, .ncopy = DESC};
+      reg[HEAT] = {.w = w, .b = b, .cin = X3C, .cpad = X3C, .taps = TAPS, .rows = 1, .K = DK, .co0 = DESC, .ncopy = 1};
     }
   }
-  LG_CHECK_LAUNCH();
-  LG_RC(tc_engine_create(&h->tc, h->wpk, c, true, stream));
+  LG_RC(tc_conv_weights_create(&h->cw, reg, NL, stream));
   guard.h = nullptr;
   *out = h;
   return 0;
@@ -547,8 +500,7 @@ extern "C" int disk_create(const DiskConfig* cfg, const float* weights_dev, size
 
 extern "C" int disk_destroy(DiskHandle* h) {
   if (!h) return 0;
-  tc_engine_destroy(&h->tc);
-  cudaFree(h->wpk);
+  tc_conv_weights_destroy(h->cw);
   cudaFree(h->wts);
   delete h;
   return 0;

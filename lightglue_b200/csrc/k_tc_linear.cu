@@ -939,19 +939,13 @@ int conv_launch(TcEngine& e, const SeqState& st, const __nv_bfloat16* in_h, cons
 }
 }  // namespace
 
-int tc_conv(TcEngine& e, const SeqState& st, const __nv_bfloat16* in_h, const __nv_bfloat16* in_l, int cin, int taps, size_t w_off,
-            const float* bias, int relu, int B, int H, int W, __nv_bfloat16* out_h, __nv_bfloat16* out_l, int cout, float* out_f32,
-            int ldo, cudaStream_t stream) {
-  if (cin % BK != 0 || (taps != 1 && taps != 9 && taps != 25))
+int tc_conv(TcConvWeights& cw, const SeqState& st, const TcConvArgs& a, cudaStream_t stream) {
+  if (a.cin % BK != 0 || (a.taps != 1 && a.taps != 9 && a.taps != 25))
     return lg_set_error("tc_conv: Cin must be a multiple of 64, 1x1, 3x3 or 5x5");
-  return conv_launch(e, st, in_h, in_l, cin, taps, w_off, bias, relu, B, H, W, out_h, out_l, cout, out_f32, ldo, 0, stream);
-}
-
-int tc_conv_s2(TcEngine& e, const SeqState& st, const __nv_bfloat16* in_h, const __nv_bfloat16* in_l, int cin, int pstride,
-               size_t w_off, const float* bias, int relu, int B, int H, int W, __nv_bfloat16* out_h, __nv_bfloat16* out_l, int cout,
-               cudaStream_t stream) {
-  if (cin % BK != 0 || pstride <= 0) return lg_set_error("tc_conv_s2: Cin must be a multiple of 64 and the phase stride positive");
-  return conv_launch(e, st, in_h, in_l, cin, 9, w_off, bias, relu, B, H, W, out_h, out_l, cout, nullptr, 0, pstride, stream);
+  if (a.pstride < 0 || (a.pstride > 0 && a.taps != 9))
+    return lg_set_error("tc_conv: a stride-2 convolution is 3x3 and its phase stride positive");
+  return conv_launch(cw.tc, st, a.in_h, a.in_l, a.cin, a.taps, cw.w_off[a.region], cw.wpk + cw.b_off[a.region], a.relu, a.B, a.H,
+                     a.W, a.out_h, a.out_l, a.cout, a.out_f32, a.ldo, a.pstride, stream);
 }
 
 int tc_block(LgHandle* h, const TcBuffers& b, const SeqState& st, int layer, int blk, float* x, const float* cs,

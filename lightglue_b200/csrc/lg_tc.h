@@ -11,7 +11,7 @@
 struct LgHandle;
 struct TcMapCache;
 
-// What the tensor-core GEMMs need from their owner (the matcher's handle, SuperPoint's SpTc); all zero = none
+// What the tensor-core GEMMs need from their owner (the matcher's handle, a TcConvWeights); all zero = none
 struct TcEngine {
   bool x3;             // LG_PREC_BF16X3: three passes over K (hi / lo split operands)
   __nv_bfloat16* w_hi; // bf16 hi / lo images of the owner's packed fp32 weights (same element offsets)
@@ -48,20 +48,63 @@ int tc_assign_sweeps(LgHandle* h, const TcBuffers& b, const SeqState& st, const 
 // softmax(q k^T / 8) v per (sequence, head): q from b.q, keys from kbuf, values from b.vt; key/value
 // sequence = (s + kv_shift) % S; writes b.ctxh (/ b.ctxl)
 int tc_attention(LgHandle* h, const TcBuffers& b, const SeqState& st, int kv_shift, const __half* kbuf, cudaStream_t stream);
+
+// ---------------------------------------------------------------- convolution owners: SuperPoint, DISK, HardNet
+// fp32 -> split-bf16 operand: hi = bf16(v), lo = bf16(v - hi)
+__device__ __forceinline__ void tc_split(float v, __nv_bfloat16& hi, __nv_bfloat16& lo) {
+  hi = __float2bfloat16_rn(v);
+  lo = __float2bfloat16_rn(v - __bfloat162float(hi));
+}
+
+// Row plan of a tc_conv operand: `used` rows stored as two "sequences" of Lp rows (the GEMM kernel walks 128-row tiles
+// per sequence), Lp the smallest multiple of LG_TILE (at least one) that holds half of them.
+struct TcRows { int Lp; long rows; };
+TcRows tc_rows(long used);
+// Its SeqState, read from four device words: len[2] (live rows of each sequence), stop_layer (0), unused.
+inline SeqState tc_rows_state(const TcRows& r, const int* words) { return SeqState{2, 1, r.Lp, words, words + 2}; }
+// The words of n matrices ([n][4], every row live) with one copy (n <= 8)
+int tc_rows_words(const TcRows* r, int n, int* words, cudaStream_t stream);
+
+// One region of packed convolution weights: [rows, K], column tap * cpad + ci, from a source [cout, cin, taps]
+// (nn.Conv2d) whose output channels co0 .. co0 + ncopy - 1 become rows 0 .. ncopy - 1, and a bias [rows]; zero past cin,
+// taps and ncopy.  The bias is copied from b, or, with bn_var set, an eval BatchNorm (eps 1e-5) is folded in, in double:
+// w rs and -bn_mean rs, rs = 1 / sqrt(bn_var + 1e-5).
+struct TcConvRegion {
+  const float *w, *b;
+  const float *bn_mean, *bn_var;
+  int cin, cpad, taps, rows, K;
+  int co0, ncopy;
+};
+#define TC_CONV_MAX_REGIONS 12
+// The packed fp32 weights of a convolution owner and the bf16x3 engine over their bf16 images.  Every region starts on
+// a 64-float boundary: the bf16 images are TMA bases (16 bytes) and fp32 regions may be read as float4.
+struct TcConvWeights {
+  float* wpk;
+  size_t w_off[TC_CONV_MAX_REGIONS], b_off[TC_CONV_MAX_REGIONS];  // float offsets of each region's weights and bias
+  TcEngine tc;
+};
+// Packs the n regions on `stream`; the sources are read there, so they must stay alive until the stream has run it.
+int tc_conv_weights_create(TcConvWeights** out, const TcConvRegion* reg, int n, cudaStream_t stream);
+void tc_conv_weights_destroy(TcConvWeights* cw);
+
 // k x k convolution (k = 1: `taps` = 1 and k = 3: `taps` = 9, zero padding q = 1; k = 5: `taps` = 25, q = 2) + bias
 // (+ ReLU) as a tensor-core GEMM over a zero-padded NHWC image stored as a [st.S * st.Lp rows, Cin] matrix, row = padded
-// pixel b (H+2q)(W+2q) + y (W+2q) + x (SuperPoint encoder, superpoint.py:137-153; DISK's U-Net).  Weights: [256 rows
-// (Cout, zero padded), taps * Cin] (column tap * Cin + ci) at e.w_hi/w_lo + w_off; bias padded to 256.  Output: the same
-// padded layout with `cout` channels as bf16 hi (/ lo), padding pixels zeroed -- or, if out_f32 is given, fp32
-// [rows, ldo] without ReLU / zeroing (SuperPoint's 1x1 heads, DISK's convolutions: their padding rows hold garbage).
-// With taps = 1 it is a plain GEMM [rows, Cin] x [Cout, Cin]^T (DISK's descriptor head on gathered im2col rows).
-int tc_conv(TcEngine& e, const SeqState& st, const __nv_bfloat16* in_h, const __nv_bfloat16* in_l, int cin, int taps, size_t w_off,
-            const float* bias, int relu, int B, int H, int W, __nv_bfloat16* out_h, __nv_bfloat16* out_l, int cout, float* out_f32,
-            int ldo, cudaStream_t stream);
-// 3x3 convolution with stride 2 and zero padding 1 (HardNet) -> the padded layout of tc_conv at the OUTPUT size H x W.
-// in_h / in_l hold the four polyphase images of the padded input, each in the output's padded frame (W + 2 columns),
+// pixel b (H+2q)(W+2q) + y (W+2q) + x (SuperPoint encoder, superpoint.py:137-153; DISK's U-Net; HardNet).  Weights and
+// bias: region `region` of the TcConvWeights, [256 rows (Cout, zero padded), taps * Cin].  Output: the same padded layout
+// with `cout` channels as bf16 hi (/ lo), padding pixels zeroed -- or, if out_f32 is given, fp32 [rows, ldo] without
+// ReLU / zeroing (SuperPoint's 1x1 heads, DISK's convolutions: their padding rows hold garbage).  With taps = 1 it is a
+// plain GEMM [rows, Cin] x [Cout, Cin]^T (the descriptor heads on gathered rows; B, H, W unused).
+// pstride > 0: 3x3 convolution with stride 2 and zero padding 1 (HardNet) -> the padded layout at the OUTPUT size H x W.
+// in_h / in_l then hold the four polyphase images of the padded input, each in the output's padded frame (W + 2 columns),
 // phase 2 py + px (padded input pixel (2i + py, 2j + px) at frame position (i + 1, j + 1)) starting at row
 // (2 py + px) pstride: tap (dy, dx) reads phase (dy & 1, dx & 1) shifted by (dy >> 1) (W + 2) + (dx >> 1) rows.
-int tc_conv_s2(TcEngine& e, const SeqState& st, const __nv_bfloat16* in_h, const __nv_bfloat16* in_l, int cin, int pstride,
-               size_t w_off, const float* bias, int relu, int B, int H, int W, __nv_bfloat16* out_h, __nv_bfloat16* out_l, int cout,
-               cudaStream_t stream);
+struct TcConvArgs {
+  const __nv_bfloat16 *in_h, *in_l;
+  int cin, taps, pstride, region, relu;  // pstride 0: stride 1
+  int B, H, W;
+  __nv_bfloat16 *out_h, *out_l;
+  int cout;
+  float* out_f32;
+  int ldo;
+};
+int tc_conv(TcConvWeights& cw, const SeqState& st, const TcConvArgs& a, cudaStream_t stream);

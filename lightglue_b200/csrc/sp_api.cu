@@ -10,7 +10,7 @@
 struct SpHandle {
   SpConfig cfg;
   float* wts;  // device copy of the weight blob
-  SpTc* tc;    // tensor-core backbone (cfg.precision == 1), else null
+  TcConvWeights* tc;  // tensor-core backbone (cfg.precision == 1), else null
 };
 
 namespace {
@@ -48,7 +48,7 @@ extern "C" int sp_create(const SpConfig* cfg, const float* weights_dev, size_t n
 
 extern "C" int sp_destroy(SpHandle* h) {
   if (!h) return 0;
-  sp_tc_destroy(h->tc);
+  tc_conv_weights_destroy(h->tc);
   cudaFree(h->wts);
   delete h;
   return 0;

@@ -1,7 +1,7 @@
 // SuperPoint encoder + heads on the tensor cores (SURVEY.md 8f1; reference lightglue/superpoint.py:137-153, 171-190,
-// 220-221): the twelve convolutions as implicit GEMMs through the wgmma / TMA linear kernel the matcher uses, on an
-// engine of their own (k_tc_linear.cu, tc_conv), split-bf16 operands (hi + lo, three MMAs per product: ~fp32
-// accuracy), fp32 accumulate.
+// 220-221): the twelve convolutions as implicit GEMMs through the wgmma / TMA linear kernel the matcher uses (tc_conv,
+// on the packed weights of a TcConvWeights and the row plan of lg_tc.h), split-bf16 operands (hi + lo, three MMAs per
+// product: ~fp32 accuracy), fp32 accumulate.
 //
 // Data layout: every feature map is a ZERO-PADDED NHWC image stored as a matrix [rows, C] of bf16 hi / lo images, row =
 // padded pixel b (H+2)(W+2) + y (W+2) + x.  A 3x3 tap (dy, dx) of such a map is the same matrix shifted by
@@ -15,29 +15,11 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
-#include <new>
 
 #include "sp_pipeline.h"
 #include "sp_tc.h"
 
 namespace {
-
-__device__ __forceinline__ void split2(float a, float b, __nv_bfloat162& hi, __nv_bfloat162& lo) {
-  hi = __floats2bfloat162_rn(a, b);
-  lo = __floats2bfloat162_rn(a - __bfloat162float(hi.x), b - __bfloat162float(hi.y));
-}
-
-// [Cout, Cin, k, k] -> [256, k*k*Cin] (row co, column tap * Cin + ci; rows >= Cout zero), bias -> [256]
-__global__ void sp_repack_kernel(const float* __restrict__ w, const float* __restrict__ b, float* __restrict__ wo,
-                                 float* __restrict__ bo, int cout, int cin, int kk) {
-  const int co = blockIdx.x;
-  const int K = kk * cin;
-  for (int idx = threadIdx.x; idx < K; idx += blockDim.x) {
-    const int tap = idx / cin, ci = idx % cin;
-    wo[(size_t)co * K + idx] = co < cout ? w[((size_t)co * cin + ci) * kk + tap] : 0.f;
-  }
-  if (threadIdx.x == 0) bo[co] = co < cout ? b[co] : 0.f;
-}
 
 // conv1a (1 -> 64, 3x3, zero padding) + bias + ReLU from the fp32 image into the padded NHWC hi / lo layout; eight threads
 // per padded pixel (eight channels each: one 16-byte store per image), weights in shared memory; padding pixels and the
@@ -77,14 +59,17 @@ __global__ void __launch_bounds__(256) sp_conv1a_kernel(const float* __restrict_
       v[c] = fmaxf(a, 0.f);
     }
   }
-  uint4 hv, lv;
-  __nv_bfloat162 h2, l2;
-  split2(v[0], v[1], h2, l2); hv.x = *reinterpret_cast<uint32_t*>(&h2); lv.x = *reinterpret_cast<uint32_t*>(&l2);
-  split2(v[2], v[3], h2, l2); hv.y = *reinterpret_cast<uint32_t*>(&h2); lv.y = *reinterpret_cast<uint32_t*>(&l2);
-  split2(v[4], v[5], h2, l2); hv.z = *reinterpret_cast<uint32_t*>(&h2); lv.z = *reinterpret_cast<uint32_t*>(&l2);
-  split2(v[6], v[7], h2, l2); hv.w = *reinterpret_cast<uint32_t*>(&h2); lv.w = *reinterpret_cast<uint32_t*>(&l2);
-  *reinterpret_cast<uint4*>(oh + row * 64 + c0) = hv;
-  *reinterpret_cast<uint4*>(ol + row * 64 + c0) = lv;
+  uint32_t hv[4], lv[4];
+#pragma unroll
+  for (int c = 0; c < 4; ++c) {
+    __nv_bfloat162 h2, l2;
+    tc_split(v[2 * c], h2.x, l2.x);
+    tc_split(v[2 * c + 1], h2.y, l2.y);
+    hv[c] = *reinterpret_cast<const uint32_t*>(&h2);
+    lv[c] = *reinterpret_cast<const uint32_t*>(&l2);
+  }
+  *reinterpret_cast<uint4*>(oh + row * 64 + c0) = make_uint4(hv[0], hv[1], hv[2], hv[3]);
+  *reinterpret_cast<uint4*>(ol + row * 64 + c0) = make_uint4(lv[0], lv[1], lv[2], lv[3]);
 }
 
 // 2x2 max pooling, stride 2 (superpoint.py:135), padded NHWC (H, W) -> padded NHWC (H/2, W/2); one thread per (output
@@ -410,13 +395,9 @@ __global__ void __launch_bounds__(256) sp_sample_kernel(const int* __restrict__ 
   dd[c] = v * (1.f / fmaxf(sqrtf(tot), 1e-12f));
 }
 
-struct Level { int H, W, Lp; long rows; };
-Level level(int B, int H, int W) {
-  Level l{H, W, 0, 0};
-  const long used = (long)B * (H + 2) * (W + 2);
-  l.Lp = (int)(((used + 1) / 2 + LG_TILE - 1) / LG_TILE * LG_TILE);  // two "sequences" of Lp rows (the kernels pair row tiles)
-  l.rows = 2L * l.Lp;
-  return l;
+// the padded maps of the four resolutions H >> i, W >> i (1-pixel border)
+void sp_levels(int B, int H, int W, TcRows lv[4]) {
+  for (int i = 0; i < 4; ++i) lv[i] = tc_rows((long)B * ((H >> i) + 2) * ((W >> i) + 2));
 }
 
 }  // namespace
@@ -453,7 +434,8 @@ int SpCudaStages::sample_impl(const SpWorkspace& ws, float* kpts, float* kscores
 }
 
 SpTcPlan sp_tc_plan(int B, int H, int W) {
-  const Level lv[4] = {level(B, H, W), level(B, H / 2, W / 2), level(B, H / 4, W / 4), level(B, H / 8, W / 8)};
+  TcRows lv[4];
+  sp_levels(B, H, W, lv);
   // Every write into the ping-pong images X / Y (conv1a, the poolings, the 3x3 convolutions) covers all 2 Lp rows of its
   // level, padding rows included, with Cout channels; the widest map at each level is 64, 64, 128 (conv3a, conv3b, the
   // third pooling, conv4a) and 256 channels (convPa, convDa).  On large images the full-resolution map is the largest, but
@@ -481,43 +463,23 @@ SpTcPlan sp_tc_plan(int B, int H, int W) {
   return p;
 }
 
-int sp_tc_create(SpTc** out, const float* wts_dev, cudaStream_t stream) {
-  SpTc* t = new (std::nothrow) SpTc();
-  if (!t) return lg_set_error("sp_tc_create: out of host memory");
-  size_t c = 0;
-  for (int l = 0; l < 12; ++l) {
+int sp_tc_create(TcConvWeights** out, const float* wts_dev, cudaStream_t stream) {
+  TcConvRegion reg[11];
+  for (int l = 1; l < 12; ++l) {
     const SpLayer& L = SP_LAYERS[l];
-    t->w_off[l] = c; c += (size_t)256 * L.k * L.k * (L.cin < 64 ? 64 : L.cin);
-    t->b_off[l] = c; c += 256;
-  }
-  cudaError_t e = cudaMalloc(&t->wpk, c * sizeof(float));
-  if (e != cudaSuccess) { delete t; return lg_set_cuda_error(e, __FILE__, __LINE__); }
-  cudaMemsetAsync(t->wpk, 0, c * sizeof(float), stream);
-  for (int l = 1; l < 12; ++l) {  // conv1a (Cin = 1) runs on the CUDA cores from the reference layout
-    const SpLayer& L = SP_LAYERS[l];
+    const int taps = L.k * L.k;
     const float* w = wts_dev + sp_layer_offset(l);
-    sp_repack_kernel<<<256, 256, 0, stream>>>(w, w + (size_t)L.cout * L.cin * L.k * L.k, t->wpk + t->w_off[l], t->wpk + t->b_off[l],
-                                             L.cout, L.cin, L.k * L.k);
+    reg[l - 1] = {.w = w, .b = w + (size_t)L.cout * L.cin * taps, .cin = L.cin, .cpad = L.cin, .taps = taps, .rows = 256,
+                  .K = taps * L.cin, .ncopy = L.cout};
   }
-  e = cudaGetLastError();
-  if (e != cudaSuccess) { sp_tc_destroy(t); return lg_set_cuda_error(e, __FILE__, __LINE__); }
-  int r = tc_engine_create(&t->tc, t->wpk, c, true, stream);
-  if (r) { sp_tc_destroy(t); return r; }
-  *out = t;
-  return 0;
-}
-
-void sp_tc_destroy(SpTc* t) {
-  if (!t) return;
-  tc_engine_destroy(&t->tc);
-  if (t->wpk) cudaFree(t->wpk);
-  delete t;
+  return tc_conv_weights_create(out, reg, 11, stream);
 }
 
 // image [B,1,H,W] fp32 -> logits_nchw [B,65,H/8,W/8], dense_nchw [B,256,H/8,W/8] (un-normalised), fp32
-int sp_tc_backbone(SpTc* t, const float* wts_dev, const float* image, int B, int H, int W, void* workspace, float* logits_nchw,
-                   float* dense_nchw, cudaStream_t stream) {
-  const Level lv[4] = {level(B, H, W), level(B, H / 2, W / 2), level(B, H / 4, W / 4), level(B, H / 8, W / 8)};
+int sp_tc_backbone(TcConvWeights* t, const float* wts_dev, const float* image, int B, int H, int W, void* workspace,
+                   float* logits_nchw, float* dense_nchw, cudaStream_t stream) {
+  TcRows lv[4];
+  sp_levels(B, H, W, lv);
   const SpTcPlan plan = sp_tc_plan(B, H, W);
   char* base = (char*)workspace;
   auto at = [&](int buf) { return (__nv_bfloat16*)(base + plan.off[buf]); };
@@ -527,19 +489,16 @@ int sp_tc_backbone(SpTc* t, const float* wts_dev, const float* image, int B, int
   float* logits_f = (float*)(base + plan.off[SPT_LOGITS]);
   float* dense_f = (float*)(base + plan.off[SPT_DENSE]);
   int* stw = (int*)(base + plan.off[SPT_STATE]);
-  int host_st[16];
-  for (int i = 0; i < 4; ++i) { host_st[4 * i] = lv[i].Lp; host_st[4 * i + 1] = lv[i].Lp; host_st[4 * i + 2] = 0; host_st[4 * i + 3] = 0; }
-  cudaError_t e = cudaMemcpyAsync(stw, host_st, sizeof(host_st), cudaMemcpyHostToDevice, stream);
-  if (e != cudaSuccess) return lg_set_cuda_error(e, __FILE__, __LINE__);
-  auto state = [&](int i) { return SeqState{2, 1, lv[i].Lp, stw + 4 * i, stw + 4 * i + 2}; };
+  LG_RC(tc_rows_words(lv, 4, stw, stream));
   auto conv = [&](int l, int li, __nv_bfloat16** in, __nv_bfloat16** out, float* out_f32, int ldo, int relu) {
     const SpLayer& L = SP_LAYERS[l];
-    return tc_conv(t->tc, state(li), in[0], in[1], L.cin, L.k * L.k, t->w_off[l], t->wpk + t->b_off[l], relu, B, lv[li].H, lv[li].W,
-                   out ? out[0] : nullptr, out ? out[1] : nullptr, L.cout, out_f32, ldo, stream);
+    return tc_conv(*t, tc_rows_state(lv[li], stw + 4 * li), {.in_h = in[0], .in_l = in[1], .cin = L.cin, .taps = L.k * L.k,
+                   .region = l - 1, .relu = relu, .B = B, .H = H >> li, .W = W >> li, .out_h = out ? out[0] : nullptr,
+                   .out_l = out ? out[1] : nullptr, .cout = L.cout, .out_f32 = out_f32, .ldo = ldo}, stream);
   };
   auto pool = [&](int li, int C, __nv_bfloat16** in, __nv_bfloat16** out) {  // level li -> li + 1
     const long n = lv[li + 1].rows * (C / 2);
-    sp_pool_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(in[0], in[1], out[0], out[1], B, lv[li].H, lv[li].W, C,
+    sp_pool_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(in[0], in[1], out[0], out[1], B, H >> li, W >> li, C,
                                                                    lv[li + 1].rows);
     return cudaGetLastError() == cudaSuccess ? 0 : lg_set_error("sp_pool_kernel launch failed");
   };

@@ -6,13 +6,6 @@
 #include "lg_tc.h"
 #include "sp_pipeline.h"
 
-struct SpTc {
-  TcEngine tc;        // bf16x3 GEMMs over the bf16 hi / lo images of wpk
-  float* wpk;         // packed fp32 weights (device)
-  size_t w_off[12];   // float offsets into wpk: weights repacked to [256, k*k*Cin] ...
-  size_t b_off[12];   // ... and biases padded to [256]
-};
-
 // The backbone's workspace: one buffer plan shared by its sizing (sp_workspace_bytes), its carving (sp_tc_backbone) and
 // its host-side export (sp_tc_layout).  Buffers in workspace order; offsets are from the start of the backbone's part.
 enum SpTcBuffer { SPT_XH, SPT_XL, SPT_YH, SPT_YL, SPT_FH, SPT_FL, SPT_LOGITS, SPT_DENSE, SPT_STATE, SPT_NBUF };
@@ -22,7 +15,8 @@ struct SpTcPlan {
 };
 SpTcPlan sp_tc_plan(int B, int H, int W);
 
-int sp_tc_create(SpTc** out, const float* wts_dev, cudaStream_t stream);
+// packs layers 1 .. 11 of the weight blob as regions 0 .. 10 (conv1a runs on the CUDA cores from the blob)
+int sp_tc_create(TcConvWeights** out, const float* wts_dev, cudaStream_t stream);
 
 // Post-processing kernels shared with DISK.  kp_compact: the pixels of scores [B, H, W] above thr, row-major, per image
 // at cand_* + b cap (row_count / row_start: [B H] scratch, n_cand [B]).  kp_select_above_kth: kornia's top-k of n =
@@ -32,9 +26,8 @@ int kp_compact(const float* scores, int B, int H, int W, float thr, long cap, in
                int* cand_pos, float* cand_score, cudaStream_t stream);
 int kp_select_above_kth(const int* n_cand, const int* cand_pos, const float* cand_score, int* sel_pos, float* sel_score, int* n_sel,
                         int B, int k_max, long cap, long out_cap, cudaStream_t stream);
-void sp_tc_destroy(SpTc* t);
-int sp_tc_backbone(SpTc* t, const float* wts_dev, const float* image, int B, int H, int W, void* workspace, float* logits_nchw,
-                   float* dense_nchw, cudaStream_t stream);
+int sp_tc_backbone(TcConvWeights* t, const float* wts_dev, const float* image, int B, int H, int W, void* workspace,
+                   float* logits_nchw, float* dense_nchw, cudaStream_t stream);
 
 namespace {
 // Executor of the sp_pipeline.h functors on `stream`, one thread per logical index (SuperPoint and ALIKED's DKD)
