@@ -750,7 +750,7 @@ int misc_assign_tail(const AssignArgs& a, const SeqState& st, const float* part,
   return 0;
 }
 
-int misc_assign(const AssignArgs& a, const SeqState& st, cudaStream_t stream, int64_t* launches) {
+int misc_assign(const AssignArgs& a, const SeqState& st, cudaStream_t stream) {
   const int B = st.B;
   const int tiles = st.Lp / 64;
   assign_z_kernel<<<dim3(st.Lp / 8, st.S), 256, 0, stream>>>(a, st);
@@ -765,16 +765,13 @@ int misc_assign(const AssignArgs& a, const SeqState& st, cudaStream_t stream, in
   LG_CHECK_LAUNCH();
   assign_filter_kernel<<<dim3((st.Lp + 255) / 256, B), 256, 0, stream>>>(a, st);
   LG_CHECK_LAUNCH();
-  *launches += 6;
   if (a.log_assignment) {
     const int mx = a.M > a.N ? a.M : a.N;
     assign_dustbin_kernel<<<dim3((mx + 256) / 256, B), 256, 0, stream>>>(a, st);
     LG_CHECK_LAUNCH();
-    *launches += 1;
   }
   assign_output_kernel<<<B, 1024, 0, stream>>>(a, st);
   LG_CHECK_LAUNCH();
-  *launches += 1;
   return 0;
 }
 

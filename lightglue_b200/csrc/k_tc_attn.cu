@@ -198,7 +198,6 @@ __global__ void __launch_bounds__(384, 2) tc_attention_kernel(const __grid_const
 }  // namespace
 
 int tc_attention(LgHandle* h, const TcBuffers& b, const SeqState& st, int kv_shift, const __half* kbuf, cudaStream_t stream) {
-  h->launches += 1;
   const uint64_t SH = (uint64_t)st.S * LG_HEADS, Lp = st.Lp;
   AttnParams p;
   int r;

@@ -766,12 +766,6 @@ int tc_gemm(TcEngine& e, const SeqState& st, const TcOperands& d, int n_tiles, T
   p.dbg = e.dbg;
   return launch_linear(p, stream);
 }
-
-// a matcher GEMM: one launch of the handle's count
-int run_linear(LgHandle* h, const SeqState& st, const TcOperands& d, int n_tiles, TcLinParams& p, cudaStream_t stream) {
-  h->launches += 1;
-  return tc_gemm(h->tc, st, d, n_tiles, p, stream);
-}
 }  // namespace
 
 struct TcMapCache {
@@ -819,17 +813,12 @@ int tc_assign_sweeps(LgHandle* h, const TcBuffers& b, const SeqState& st, const 
     int r;
     {
       Timer tm(h, LG_K_ASSIGN_MATRIX, stream, sweep == 1 && logmat != nullptr);  // the matrix-writing sweep on its own
-      if ((r = run_linear(h, st, ops, ntc, p, stream))) return r;
+      if ((r = tc_gemm(h->tc, st, ops, ntc, p, stream))) return r;
     }
-    if (sweep == 0) {
-      if ((r = misc_assign_term(a, st, part, 2 * ntc, BN / 2, term, stream))) return r;
-      h->launches += 1;
-    }
+    if (sweep == 0 && (r = misc_assign_term(a, st, part, 2 * ntc, BN / 2, term, stream))) return r;
   }
-  if (logmat) { if (int rd = misc_assign_dustbin(a, st, stream)) return rd; h->launches += 1; }
-  int r = misc_assign_tail(a, st, part, part_arg, 2 * ntc, BN / 2, stream);
-  h->launches += 1;
-  return r;
+  if (logmat) LG_RC(misc_assign_dustbin(a, st, stream));
+  return misc_assign_tail(a, st, part, part_arg, 2 * ntc, BN / 2, stream);
 }
 
 unsigned int tc_debug_timeout_code(const TcEngine& e, unsigned int* words32) {
@@ -897,12 +886,11 @@ int tc_input_proj(LgHandle* h, const TcBuffers& b, const SeqState& st, const flo
   if (d % BK != 0) return lg_set_error("tensor-core input_proj needs input_dim % 64 == 0");
   shadow_kernel<<<st.S * st.Lp, 256, 0, stream>>>(desc_packed, b.hh, b.hl, d, st);
   LG_CHECK_LAUNCH();
-  h->launches += 1;
   TcLinParams p{};
   p.epi = TEPI_F32; p.scale = 1.f; p.bias = h->wpk + h->o_inb;
   p.out_f32 = x; p.ldo = LG_DIM; p.out_h = b.xh; p.out_l = b.xl; p.ldb = LG_DIM;
   const TcOperands ops{b.hh, b.hl, d, nullptr, nullptr, 0, h->tc.w_hi + h->o_inw, h->tc.w_lo + h->o_inw, LG_DIM, 1, 0};
-  return run_linear(h, st, ops, 1, p, stream);
+  return tc_gemm(h->tc, st, ops, 1, p, stream);
 }
 
 int tc_final_proj(LgHandle* h, const TcBuffers& b, const SeqState& st, float* p_out, cudaStream_t stream) {
@@ -914,7 +902,7 @@ int tc_final_proj(LgHandle* h, const TcBuffers& b, const SeqState& st, float* p_
   const size_t w = h->o_assign + AO_FW;
   const TcOperands ops{b.xh, b.xl, LG_DIM, nullptr, nullptr, 0, h->tc.w_hi + w, h->tc.w_lo + w, LG_DIM, h->cfg.n_layers,
                        ASSIGN_BLOB_PAD};
-  return run_linear(h, st, ops, 1, p, stream);
+  return tc_gemm(h->tc, st, ops, 1, p, stream);
 }
 
 namespace {
@@ -966,7 +954,7 @@ int tc_block(LgHandle* h, const TcBuffers& b, const SeqState& st, int layer, int
     p.q = b.q; p.k = b.k; p.vt = b.vt; p.cs = cs;
     const int nout = blk == 0 ? 3 * LG_DIM : 2 * LG_DIM;
     const TcOperands ops{b.xh, b.xl, LG_DIM, nullptr, nullptr, 0, wh + o.wp, wl + o.wp, nout, 1, 0};
-    int r = run_linear(h, st, ops, nout / BN, p, stream);
+    int r = tc_gemm(h->tc, st, ops, nout / BN, p, stream);
     if (r) return r;
   }
   {
@@ -983,7 +971,7 @@ int tc_block(LgHandle* h, const TcBuffers& b, const SeqState& st, int layer, int
     p.out_h = b.hh; p.out_l = b.hl; p.ldb = LG_FFN;
     const TcOperands ops{b.xh, b.xl, LG_DIM, b.ctxh, b.ctxl, LG_DIM, wh + o.w1f, wl + o.w1f, LG_FFN, 1, 0};
     Timer t2(h, LG_K_FFN0, stream);
-    int r = run_linear(h, st, ops, LG_FFN / BN, p, stream);  // one 2-CTA cluster per 128 rows: the whole LayerNorm row
+    int r = tc_gemm(h->tc, st, ops, LG_FFN / BN, p, stream);  // one 2-CTA cluster per 128 rows: the whole LayerNorm row
     if (r) return r;
   }
   {  // ffn.3 + residual -> x (fp32 master + bf16 shadows)
@@ -992,7 +980,7 @@ int tc_block(LgHandle* h, const TcBuffers& b, const SeqState& st, int layer, int
     p.out_h = b.xh; p.out_l = b.xl; p.ldb = LG_DIM;
     const TcOperands ops{b.hh, b.hl, LG_FFN, nullptr, nullptr, 0, wh + o.w2, wl + o.w2, LG_DIM, 1, 0};
     Timer t2(h, LG_K_FFN3, stream);
-    int r = run_linear(h, st, ops, 1, p, stream);
+    int r = tc_gemm(h->tc, st, ops, 1, p, stream);
     if (r) return r;
   }
   return 0;

@@ -16,6 +16,7 @@
 // errors
 // ------------------------------------------------------------------------------------------------
 static thread_local char g_err[512] = "";
+thread_local int64_t lg_launches;
 int lg_set_error(const char* msg) {
   snprintf(g_err, sizeof(g_err), "%s", msg);
   return 1;
@@ -152,7 +153,6 @@ extern "C" int lg_create(const LgConfig* cfg, const float* blob, size_t n_floats
   h->wpk = nullptr;
   memset(&h->tc, 0, sizeof(h->tc));
   h->cfg = *cfg;
-  h->launches = 0;
   h->timing = false;
   h->dbg_layers = nullptr; h->dbg_layers_floats = 0;
   for (int i = 0; i < LG_K_CLASSES; ++i) h->ev_used[i] = 0;
@@ -185,7 +185,7 @@ extern "C" int lg_create(const LgConfig* cfg, const float* blob, size_t n_floats
     float* base = h->wpk + h->o_layers + (size_t)l * h->layer_stride;
     // self block
     permute_qkv_kernel<<<768, 128, 0, stream>>>(p, p + 3 * D * D, base + h->bself.wp, base + h->bself.bp);
-    LG_CU(cudaGetLastError());
+    LG_CHECK_LAUNCH();
     p += 3 * D * D + 3 * D;
     size_t bo = h->o_layers + (size_t)l * h->layer_stride;
     LG_CU(cp(bo + h->bself.wo, p, D * D)); p += D * D;
@@ -214,7 +214,7 @@ extern "C" int lg_create(const LgConfig* cfg, const float* blob, size_t n_floats
       const BlockOff& o = blk == 0 ? h->bself : h->bcross;
       float* bw = base + (blk == 0 ? 0 : h->bself.total);
       fold_out_proj_kernel<<<(unsigned)F, 256, 0, stream>>>(bw + o.w1, bw + o.b1, bw + o.wo, bw + o.bo, bw + o.w1f, bw + o.b1f);
-      LG_CU(cudaGetLastError());
+      LG_CHECK_LAUNCH();
     }
   }
   for (int l = 0; l < L; ++l) {  // packed: final_proj.w [256,256] | final_proj.b [256] | matchability.w [256] | .b [1] (+pad)
@@ -376,6 +376,66 @@ __global__ void fill_empty_kernel(int64_t* m0, int64_t* m1, float* s0, float* s1
   if (i < n1) { m1[i] = -1; s1[i] = 0.f; if (p1) p1[i] = 1; }
   if (i < B) { if (stop) stop[i] = 1; if (nm) nm[i] = 0; }
 }
+
+// What lg_forward, lg_assign and lg_attention start from: the carved workspace, the sequence state and the launch count
+// before their first launch (each reports the count's increase over the call).
+struct Call {
+  Workspace w;
+  SeqState st;
+  int64_t launches0;
+};
+
+// Carves the workspace and checks its size (the error starts with `who`), starts the launch count, and runs the first
+// launch, misc_init_state (lens0 / lens1 null: M / N rows per pair).
+int begin_call(LgHandle* h, const char* who, int B, int M, int N, const int* lens0, const int* lens1, void* workspace,
+               size_t ws_bytes, cudaStream_t stream, Call* c) {
+  Workspace& w = c->w;
+  carve(h, B, M, N, (char*)workspace, &w);
+  if (!workspace || ws_bytes < w.bytes) {
+    char msg[64];
+    snprintf(msg, sizeof(msg), "%s: workspace too small", who);
+    return lg_set_error(msg);
+  }
+  c->launches0 = lg_launches;
+  LG_RC(misc_init_state(w.lena, w.inda, w.prune, w.stop_layer, w.below, h->cfg.n_layers * B, B, M, N, w.Lp, lens0, lens1,
+                        stream));
+  c->st = SeqState{2 * B, B, w.Lp, w.lena, w.stop_layer};
+  return 0;
+}
+
+// tc_block's counterpart on the CUDA cores (fp32): QKV, attention, out_proj, ffn.0, LayerNorm + GELU, ffn.3 + residual
+int simt_block(LgHandle* h, const Workspace& w, const SeqState& st, int layer, int blk, float* x, const float* cs,
+               cudaStream_t stream) {
+  const BlockOff& o = blk == 0 ? h->bself : h->bcross;
+  const float* bw = h->wpk + h->o_layers + (size_t)layer * h->layer_stride + (blk == 0 ? 0 : h->bself.total);
+  GemmArgs g{};
+  g.A0 = x; g.lda0 = D; g.K0 = D; g.K = D;
+  g.W = bw + o.wp; g.bias = bw + o.bp; g.scale = 1.f;
+  g.q = w.q; g.k = w.k; g.v = w.v; g.cs = cs;
+  g.Nout = blk == 0 ? 3 * D : 2 * D;
+  g.epi = blk == 0 ? EPI_QKV_ROPE : EPI_QK_V;
+  { Timer t(h, LG_K_LINEAR, stream); LG_RC(simt_gemm(g, st, stream)); }
+  {
+    Timer t(h, LG_K_ATTENTION, stream);
+    if (blk == 0) LG_RC(simt_attention(w.q, w.k, w.v, w.ctx, 0, st, stream));
+    else LG_RC(simt_attention(w.q, w.q, w.v, w.ctx, st.B, st, stream));
+  }
+  Timer t(h, LG_K_LINEAR, stream);
+  GemmArgs go{};  // out_proj / to_out
+  go.A0 = w.ctx; go.lda0 = D; go.K0 = D; go.K = D; go.W = bw + o.wo; go.bias = bw + o.bo; go.Nout = D;
+  go.epi = EPI_STORE; go.scale = 1.f; go.out = w.msg; go.ldo = D;
+  LG_RC(simt_gemm(go, st, stream));
+  GemmArgs g1{};  // ffn.0 on cat([x, msg])
+  g1.A0 = x; g1.lda0 = D; g1.K0 = D; g1.A1 = w.msg; g1.lda1 = D; g1.K = F; g1.W = bw + o.w1; g1.bias = bw + o.b1;
+  g1.Nout = F; g1.epi = EPI_STORE; g1.scale = 1.f; g1.out = w.hbuf; g1.ldo = F;
+  LG_RC(simt_gemm(g1, st, stream));
+  LG_RC(simt_layernorm_gelu(w.hbuf, bw + o.g, bw + o.be, st, stream));
+  GemmArgs g2{};  // ffn.3 + residual
+  g2.A0 = w.hbuf; g2.lda0 = F; g2.K0 = F; g2.K = F; g2.W = bw + o.w2; g2.bias = bw + o.b2; g2.Nout = D;
+  g2.epi = EPI_RESID; g2.scale = 1.f; g2.out = x; g2.ldo = D;
+  LG_RC(simt_gemm(g2, st, stream));
+  return 0;
+}
 }  // namespace
 
 extern "C" size_t lg_workspace_bytes(const LgHandle* h, int32_t B, int32_t M, int32_t N) {
@@ -404,7 +464,6 @@ static int run_assign(LgHandle* h, const Workspace& w, const SeqState& st, const
     } else {
       LG_RC(tc_final_proj(h, w.tc, st, w.ctx, stream));
     }
-    h->launches += 1;
   }
   AssignArgs a{};
   a.p = w.ctx; a.x = x;
@@ -423,7 +482,7 @@ static int run_assign(LgHandle* h, const Workspace& w, const SeqState& st, const
       // both similarity sweeps on the tensor cores; the N x M matrix reaches HBM only if the caller asked for it
       LG_RC(tc_assign_sweeps(h, w.tc, st, a, w.tc_part, w.tc_parg, w.term, stream));
     } else {
-      LG_RC(misc_assign(a, st, stream, &h->launches));
+      LG_RC(misc_assign(a, st, stream));
     }
   }
   return 0;
@@ -444,7 +503,6 @@ extern "C" int lg_forward(LgHandle* h, const LgInputs* in, const LgOutputs* out,
   if (h->cfg.pos_dim == 4 && (M > 0 && N > 0) && (!in->scales0 || !in->oris0 || !in->scales1 || !in->oris1))
     return lg_set_error("lg_forward: scales/oris required when pos_dim == 4");
   cudaStream_t stream = (cudaStream_t)stream_;
-  h->launches = 0;
   const bool early = h->cfg.depth_confidence > 0, prune = h->cfg.width_confidence > 0;
   if (out->log_assignment && (early || prune)) return lg_set_error("lg_forward: log_assignment needs adaptivity off");
   if (M == 0 || N == 0) {  // lightglue.py:568-588: no keypoints -> nothing matched, stop = 1
@@ -454,44 +512,39 @@ extern "C" int lg_forward(LgHandle* h, const LgInputs* in, const LgOutputs* out,
     const long n0 = (long)B * M, n1 = (long)B * N;
     long mx = n0 > n1 ? n0 : n1;
     if (mx < B) mx = B;
+    const int64_t launches0 = lg_launches;
     fill_empty_kernel<<<(unsigned)((mx + 255) / 256), 256, 0, stream>>>(out->matches0, out->matches1, out->matching_scores0,
                                                                        out->matching_scores1, out->stop, out->prune0,
                                                                        out->prune1, out->n_matches, n0, n1, B);
-    LG_CU(cudaGetLastError());
-    h->launches = 1;
+    LG_CHECK_LAUNCH();
+    h->launches = lg_launches - launches0;
     return 0;
   }
   LG_RC(check_outputs(out));
   if (!in->kpts0 || !in->kpts1 || !in->desc0 || !in->desc1) return lg_set_error("lg_forward: null input tensor");
-  Workspace w;
-  carve(h, B, M, N, (char*)workspace, &w);
-  if (!workspace || ws_bytes < w.bytes) return lg_set_error("lg_forward: workspace too small");
-  const int L = h->cfg.n_layers, Lp = w.Lp;
-  const bool fp32 = h->cfg.precision == LG_PREC_FP32;
-
   if (out->log_assignment && (in->lens0 || in->lens1))
     return lg_set_error("lg_forward: log_assignment is defined for dense batches only (no lens0/lens1)");
-  LG_RC(misc_init_state(w.lena, w.inda, w.prune, w.stop_layer, w.below, L * B, B, M, N, Lp, in->lens0, in->lens1, stream));
-  h->launches += 1;
+  Call c;
+  LG_RC(begin_call(h, "lg_forward", B, M, N, in->lens0, in->lens1, workspace, ws_bytes, stream, &c));
+  const Workspace& w = c.w;
+  SeqState& st = c.st;
+  const int L = h->cfg.n_layers, Lp = w.Lp;
+  const bool fp32 = h->cfg.precision == LG_PREC_FP32;
   float *x = w.xa, *x_alt = w.xb, *cs = w.csa, *cs_alt = w.csb;
   int *len = w.lena, *len_alt = w.lenb, *ind = w.inda, *ind_alt = w.indb;
-  SeqState st{2 * B, B, Lp, len, w.stop_layer};
 
   {  // positional encoding, cached for all layers (lightglue.py:523-525)
     Timer t(h, LG_K_OTHER, stream);
     PosencArgs pa{in->kpts0, in->kpts1, in->size0, in->size1, in->scales0, in->oris0, in->scales1, in->oris1,
                   h->wpk + h->o_wr, h->cfg.pos_dim, B, M, N, Lp, cs, in->lens0, in->lens1};
     LG_RC(misc_posenc(pa, stream));
-    h->launches += 1;
   }
   // descriptors -> residual stream (optionally through input_proj, lightglue.py:521-522)
   if (h->cfg.input_dim == (int)D) {
     LG_RC(misc_pack_desc(in->desc0, in->desc1, x, B, M, N, Lp, D, in->lens0, in->lens1, stream, fp32 ? nullptr : (void*)w.tc.xh,
                       fp32 ? nullptr : (void*)w.tc.xl));
-    h->launches += 1;
   } else {
     LG_RC(misc_pack_desc(in->desc0, in->desc1, w.hbuf, B, M, N, Lp, h->cfg.input_dim, in->lens0, in->lens1, stream));
-    h->launches += 1;
     Timer t(h, LG_K_LINEAR, stream);
     if (fp32) {
       GemmArgs g{};
@@ -499,49 +552,14 @@ extern "C" int lg_forward(LgHandle* h, const LgInputs* in, const LgOutputs* out,
       g.W = h->wpk + h->o_inw; g.bias = h->wpk + h->o_inb;
       g.K = h->cfg.input_dim; g.Nout = D; g.epi = EPI_STORE; g.scale = 1.f; g.out = x; g.ldo = D;
       LG_RC(simt_gemm(g, st, stream));
-      h->launches += 1;
     } else {
       LG_RC(tc_input_proj(h, w.tc, st, w.hbuf, x, stream));
     }
   }
 
   for (int i = 0; i < L; ++i) {
-    const float* lw = h->wpk + h->o_layers + (size_t)i * h->layer_stride;
-    for (int blk = 0; blk < 2; ++blk) {  // 0: SelfBlock (159-172), 1: CrossBlock (201-230)
-      const BlockOff& o = blk == 0 ? h->bself : h->bcross;
-      const float* bw = lw + (blk == 0 ? 0 : h->bself.total);
-      if (fp32) {
-        GemmArgs g{};
-        g.A0 = x; g.lda0 = D; g.K0 = D; g.K = D;
-        g.W = bw + o.wp; g.bias = bw + o.bp; g.scale = 1.f;
-        g.q = w.q; g.k = w.k; g.v = w.v; g.cs = cs;
-        g.Nout = blk == 0 ? 3 * D : 2 * D;
-        g.epi = blk == 0 ? EPI_QKV_ROPE : EPI_QK_V;
-        { Timer t(h, LG_K_LINEAR, stream); LG_RC(simt_gemm(g, st, stream)); }
-        {
-          Timer t(h, LG_K_ATTENTION, stream);
-          if (blk == 0) LG_RC(simt_attention(w.q, w.k, w.v, w.ctx, 0, st, stream));
-          else LG_RC(simt_attention(w.q, w.q, w.v, w.ctx, B, st, stream));
-        }
-        Timer t(h, LG_K_LINEAR, stream);
-        GemmArgs go{};  // out_proj / to_out
-        go.A0 = w.ctx; go.lda0 = D; go.K0 = D; go.K = D; go.W = bw + o.wo; go.bias = bw + o.bo; go.Nout = D;
-        go.epi = EPI_STORE; go.scale = 1.f; go.out = w.msg; go.ldo = D;
-        LG_RC(simt_gemm(go, st, stream));
-        GemmArgs g1{};  // ffn.0 on cat([x, msg])
-        g1.A0 = x; g1.lda0 = D; g1.K0 = D; g1.A1 = w.msg; g1.lda1 = D; g1.K = F; g1.W = bw + o.w1; g1.bias = bw + o.b1;
-        g1.Nout = F; g1.epi = EPI_STORE; g1.scale = 1.f; g1.out = w.hbuf; g1.ldo = F;
-        LG_RC(simt_gemm(g1, st, stream));
-        LG_RC(simt_layernorm_gelu(w.hbuf, bw + o.g, bw + o.be, st, stream));
-        GemmArgs g2{};  // ffn.3 + residual
-        g2.A0 = w.hbuf; g2.lda0 = F; g2.K0 = F; g2.K = F; g2.W = bw + o.w2; g2.bias = bw + o.b2; g2.Nout = D;
-        g2.epi = EPI_RESID; g2.scale = 1.f; g2.out = x; g2.ldo = D;
-        LG_RC(simt_gemm(g2, st, stream));
-        h->launches += 6;
-      } else {
-        LG_RC(tc_block(h, w.tc, st, i, blk, x, cs, stream));
-      }
-    }
+    for (int blk = 0; blk < 2; ++blk)  // 0: SelfBlock (159-172), 1: CrossBlock (201-230)
+      LG_RC(fp32 ? simt_block(h, w, st, i, blk, x, cs, stream) : tc_block(h, w.tc, st, i, blk, x, cs, stream));
     if (h->dbg_layers) {
       const size_t per = (size_t)2 * B * Lp * D;
       if ((size_t)(i + 1) * per > h->dbg_layers_floats) return lg_set_error("lg_debug_capture_layers: buffer too small");
@@ -563,24 +581,21 @@ extern "C" int lg_forward(LgHandle* h, const LgInputs* in, const LgOutputs* out,
     a.len_in = len; a.len_out = prune ? len_alt : len; a.pos = w.pos; a.did_prune = w.did_prune;
     LG_RC(misc_adapt_score(a, st, stream));
     LG_RC(misc_adapt_decide(a, st, stream));
-    h->launches += 2;
     if (prune) {
       GatherArgs ga{x, x_alt, cs, cs_alt, ind, ind_alt, w.prune, w.keep, w.pos, w.did_prune, len, len_alt, w.stop_layer, i};
       LG_RC(misc_adapt_gather(ga, st, stream));
-      h->launches += 1;
       float* tf = x; x = x_alt; x_alt = tf;
       tf = cs; cs = cs_alt; cs_alt = tf;
       int* ti = ind; ind = ind_alt; ind_alt = ti;
       ti = len; len = len_alt; len_alt = ti;
       st.len = len;
-      if (!fp32) { LG_RC(tc_refresh_shadow(h, w.tc, x, st, stream)); h->launches += 1; }
+      if (!fp32) LG_RC(tc_refresh_shadow(h, w.tc, x, st, stream));
     }
   }
   LG_RC(misc_finalize_stop(w.stop_layer, B, L, stream));
-  h->launches += 1;
   LG_RC(run_assign(h, w, st, x, ind, M, N, out, stream));
   LG_RC(misc_export_stop_prune(w.stop_layer, w.prune, out->stop, out->prune0, out->prune1, B, M, N, Lp, stream));
-  h->launches += 1;
+  h->launches = lg_launches - c.launches0;
   return 0;
 }
 
@@ -590,18 +605,15 @@ extern "C" int lg_assign(LgHandle* h, int32_t layer, int32_t B, int32_t M, int32
   LG_RC(check_outputs(out));
   if (B <= 0 || M <= 0 || N <= 0 || layer < 0 || layer >= h->cfg.n_layers) return lg_set_error("lg_assign: bad shape/layer");
   cudaStream_t stream = (cudaStream_t)stream_;
-  Workspace w;
-  carve(h, B, M, N, (char*)workspace, &w);
-  if (!workspace || ws_bytes < w.bytes) return lg_set_error("lg_assign: workspace too small");
-  h->launches = 0;
-  LG_RC(misc_init_state(w.lena, w.inda, w.prune, w.stop_layer, w.below, h->cfg.n_layers * B, B, M, N, w.Lp, nullptr, nullptr,
-                     stream));
+  Call c;
+  LG_RC(begin_call(h, "lg_assign", B, M, N, nullptr, nullptr, workspace, ws_bytes, stream, &c));
+  const Workspace& w = c.w;
   LG_RC(misc_finalize_stop(w.stop_layer, B, layer + 1, stream));  // selects log_assignment[layer] for every pair
   LG_RC(misc_pack_desc(x0, x1, w.xa, B, M, N, w.Lp, D, nullptr, nullptr, stream));
-  h->launches += 3;
-  SeqState st{2 * B, B, w.Lp, w.lena, w.stop_layer};
-  if (h->cfg.precision != LG_PREC_FP32) { LG_RC(tc_refresh_shadow(h, w.tc, w.xa, st, stream)); h->launches += 1; }
-  return run_assign(h, w, st, w.xa, w.inda, M, N, out, stream);
+  if (h->cfg.precision != LG_PREC_FP32) LG_RC(tc_refresh_shadow(h, w.tc, w.xa, c.st, stream));
+  LG_RC(run_assign(h, w, c.st, w.xa, w.inda, M, N, out, stream));
+  h->launches = lg_launches - c.launches0;
+  return 0;
 }
 
 extern "C" int lg_attention(LgHandle* h, int32_t B, int32_t M, int32_t N, int32_t cross, const float* q0, const float* k0,
@@ -610,13 +622,9 @@ extern "C" int lg_attention(LgHandle* h, int32_t B, int32_t M, int32_t N, int32_
   if (!h || !q0 || !k0 || !v0 || !q1 || !k1 || !v1 || !ctx0 || !ctx1) return lg_set_error("lg_attention: null argument");
   if (B <= 0 || M <= 0 || N <= 0) return lg_set_error("lg_attention: bad shape");
   cudaStream_t stream = (cudaStream_t)stream_;
-  Workspace w;
-  carve(h, B, M, N, (char*)workspace, &w);
-  if (!workspace || ws_bytes < w.bytes) return lg_set_error("lg_attention: workspace too small");
-  h->launches = 0;
-  LG_RC(misc_init_state(w.lena, w.inda, w.prune, w.stop_layer, w.below, h->cfg.n_layers * B, B, M, N, w.Lp, nullptr, nullptr,
-                     stream));
-  SeqState st{2 * B, B, w.Lp, w.lena, w.stop_layer};
+  Call c;
+  LG_RC(begin_call(h, "lg_attention", B, M, N, nullptr, nullptr, workspace, ws_bytes, stream, &c));
+  const Workspace& w = c.w;
   const bool fp32 = h->cfg.precision == LG_PREC_FP32;
   AttnIoArgs a{};
   a.q0 = q0; a.k0 = k0; a.v0 = v0; a.q1 = q1; a.k1 = k1; a.v1 = v1;
@@ -627,10 +635,10 @@ extern "C" int lg_attention(LgHandle* h, int32_t B, int32_t M, int32_t N, int32_
   LG_RC(misc_attn_pack(a, stream));
   {
     Timer t(h, LG_K_ATTENTION, stream);
-    if (fp32) LG_RC(simt_attention(w.q, w.k, w.v, w.ctx, cross ? B : 0, st, stream));
-    else LG_RC(tc_attention(h, w.tc, st, cross ? B : 0, w.tc.k, stream));
+    if (fp32) LG_RC(simt_attention(w.q, w.k, w.v, w.ctx, cross ? B : 0, c.st, stream));
+    else LG_RC(tc_attention(h, w.tc, c.st, cross ? B : 0, w.tc.k, stream));
   }
   LG_RC(misc_attn_unpack(a, stream));
-  h->launches += fp32 ? 4 : 3;  // init + pack + (attention counted by tc_attention) + unpack
+  h->launches = lg_launches - c.launches0;
   return 0;
 }

@@ -12,14 +12,22 @@
 #define LG_FFN 512
 #define LG_TILE 128
 
+// Kernel launches issued by this thread.  Every launch bumps it once it has succeeded (LG_CHECK_LAUNCH, tc_launch), so
+// an entry point reports its own launches as the difference over the call (lg_last_launch_count).
+extern thread_local int64_t lg_launches;
+
 // Error returns of the C-ABI code: a failed CUDA call records its error and returns it (LG_CU; LG_CHECK_LAUNCH after a
-// kernel launch), a non-zero return code is passed on (LG_RC).
+// kernel launch, which also counts it), a non-zero return code is passed on (LG_RC).
 #define LG_CU(x)                                                                 \
   do {                                                                           \
     cudaError_t e__ = (x);                                                       \
     if (e__ != cudaSuccess) return lg_set_cuda_error(e__, __FILE__, __LINE__);   \
   } while (0)
-#define LG_CHECK_LAUNCH() LG_CU(cudaGetLastError())
+#define LG_CHECK_LAUNCH()        \
+  do {                           \
+    LG_CU(cudaGetLastError());   \
+    ++lg_launches;               \
+  } while (0)
 #define LG_RC(x)         \
   do {                   \
     int r__ = (x);       \
@@ -157,7 +165,7 @@ struct AssignArgs {
   int* n_matches; int64_t* matches; float* match_scores; int cap;  // cap = min(M, N)
   float* log_assignment; // optional [B, M+1, N+1]
 };
-int misc_assign(const AssignArgs& a, const SeqState& st, cudaStream_t stream, int64_t* launches);
+int misc_assign(const AssignArgs& a, const SeqState& st, cudaStream_t stream);
 // companions of the tensor-core sweeps: z + LSE combine (after sweep 1), slot reduce + filter + outputs (after sweep 2)
 int misc_assign_term(const AssignArgs& a, const SeqState& st, const float* part, int pstride, int slot_cols, float* term,
                      cudaStream_t stream);

@@ -279,7 +279,7 @@ struct TcEngine;
 int tc_tmap(TcEngine& e, const TmapArgs& a, CUtensorMap* out);
 
 // Launches a tensor-core kernel with programmatic dependent launch, after opting it in to `smem` bytes of dynamic
-// shared memory on the current device; `cluster` > 1: in clusters of that many CTAs along x.
+// shared memory on the current device; `cluster` > 1: in clusters of that many CTAs along x.  Counts it in lg_launches.
 template <class P>
 int tc_launch(void (*kernel)(P), dim3 grid, int threads, int smem, const P& p, cudaStream_t stream, int cluster = 1) {
   if (int r = lg_func_smem_once((const void*)kernel, smem)) return r;
@@ -293,5 +293,6 @@ int tc_launch(void (*kernel)(P), dim3 grid, int threads, int smem, const P& p, c
   cfg.attrs = at; cfg.numAttrs = cluster > 1 ? 2 : 1;
   const cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, p);
   if (e != cudaSuccess) return lg_set_cuda_error(e, __FILE__, __LINE__);
+  ++lg_launches;
   return 0;
 }
