@@ -10,14 +10,16 @@ PREC = {"fp32": 0, "bf16": 1, "bf16x3": 2}
 K_ATTENTION, K_LINEAR, K_ASSIGN, K_OTHER = 0, 1, 2, 3
 ABI_VERSION = 3
 
-# include/superpoint_b200.h, include/aliked_b200.h, include/sift_b200.h, include/disk_b200.h and
-# include/doghardnet_b200.h: same library
+# include/superpoint_b200.h, include/aliked_b200.h, include/sift_b200.h, include/disk_b200.h,
+# include/doghardnet_b200.h and include/geometry_b200.h: same library
 SP_ABI_VERSION = 2
 SP_TC_BUFFERS = 9  # buffers of the tensor-core backbone's workspace plan (sp_tc_layout)
 AL_ABI_VERSION = 1
 SIFT_ABI_VERSION = 1
 DISK_ABI_VERSION = 1
 DHN_ABI_VERSION = 1
+GEO_ABI_VERSION = 1  # include/geometry_b200.h
+GEO_HOMOGRAPHY, GEO_FUNDAMENTAL = 0, 1
 
 
 class LgConfig(C.Structure):
@@ -85,6 +87,26 @@ class LgOutputs(C.Structure):
     ]
 
 
+class GeoConfig(C.Structure):
+    _fields_ = [
+        ("abi_version", C.c_int32), ("model", C.c_int32), ("max_iters", C.c_int32), ("seed", C.c_uint32),
+        ("threshold", C.c_double), ("confidence", C.c_double),
+    ]
+
+
+class GeoInputs(C.Structure):
+    _fields_ = [
+        ("B", C.c_int32), ("M", C.c_int32), ("N", C.c_int32),
+        ("kpts0", C.c_void_p), ("kpts1", C.c_void_p), ("matches0", C.c_void_p),
+    ]
+
+
+class GeoOutputs(C.Structure):
+    _fields_ = [
+        ("model", C.c_void_p), ("inliers", C.c_void_p), ("num_inliers", C.c_void_p), ("success", C.c_void_p),
+        ("best_hypothesis", C.c_void_p), ("num_hypotheses", C.c_void_p),
+    ]
+
 
 # name: (restype, argtypes), one table per header.  The export lists are the tables' keys.
 _VP, _I32, _I64, _SZ = C.c_void_p, C.c_int32, C.c_int64, C.c_size_t
@@ -149,8 +171,12 @@ DHN_PROTOTYPES = {  # include/doghardnet_b200.h
     "dhn_forward": (C.c_int, [_VP, _VP, _I32, _VP, _I32, _I32, _I32, _I64] + [_VP] * 7 + [_SZ, _VP]),
     "dhn_describe": (C.c_int, [_VP, _VP, _I32, _VP, _I32, _I32, _I32, _I64] + [_VP] * 6 + [_SZ, _VP]),
 }
-EXPORTS, SP_EXPORTS, AL_EXPORTS, SIFT_EXPORTS, DISK_EXPORTS, DHN_EXPORTS = (
-    tuple(t) for t in (LG_PROTOTYPES, SP_PROTOTYPES, AL_PROTOTYPES, SIFT_PROTOTYPES, DISK_PROTOTYPES, DHN_PROTOTYPES))
+GEO_PROTOTYPES = {  # include/geometry_b200.h
+    "geo_workspace_bytes": (_SZ, [_I32, _I32, _I32]),
+    "geo_estimate": (C.c_int, [C.POINTER(GeoConfig), C.POINTER(GeoInputs), C.POINTER(GeoOutputs), _VP, _SZ, _VP]),
+}
+_TABLES = (LG_PROTOTYPES, SP_PROTOTYPES, AL_PROTOTYPES, SIFT_PROTOTYPES, DISK_PROTOTYPES, DHN_PROTOTYPES, GEO_PROTOTYPES)
+EXPORTS, SP_EXPORTS, AL_EXPORTS, SIFT_EXPORTS, DISK_EXPORTS, DHN_EXPORTS, GEO_EXPORTS = (tuple(t) for t in _TABLES)
 
 _lib = None
 
@@ -169,7 +195,7 @@ def load():
     if not os.path.exists(path):
         raise RuntimeError(f"{path} is missing: the CUDA library must be built (python -m lightglue_b200.build)")
     lib = C.CDLL(path)
-    for table in (LG_PROTOTYPES, SP_PROTOTYPES, AL_PROTOTYPES, SIFT_PROTOTYPES, DISK_PROTOTYPES, DHN_PROTOTYPES):
+    for table in _TABLES:
         for name, (restype, argtypes) in table.items():
             fn = getattr(lib, name)
             fn.restype, fn.argtypes = restype, argtypes

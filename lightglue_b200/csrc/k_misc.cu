@@ -5,6 +5,7 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
+#include "block_scan.cuh"
 #include "lg_internal.h"
 #include "tc_common.cuh"
 
@@ -590,37 +591,12 @@ __device__ __forceinline__ void assign_compact_pair(const AssignArgs& a, const S
     const int i = base + tid;
     int j = -1; float sc = 0.f;
     if (i < m) { j = a.m0c[rbase + i]; sc = a.ms0c[rbase + i]; }
-    const int flag = j >= 0;
-    int incl = flag;
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {
-      const int t = __shfl_up_sync(0xffffffffu, incl, off);
-      if ((tid & 31) >= off) incl += t;
+    const int slot = block_scan_step(j >= 0, tid, warp_sums, &carry);
+    if (j >= 0 && slot < a.cap) {
+      a.matches[((long)b * a.cap + slot) * 2] = ind0[i];
+      a.matches[((long)b * a.cap + slot) * 2 + 1] = ind1[j];
+      a.match_scores[(long)b * a.cap + slot] = sc;
     }
-    if ((tid & 31) == 31) warp_sums[tid >> 5] = incl;
-    __syncthreads();
-    if (tid < 32) {
-      int w = warp_sums[tid];
-#pragma unroll
-      for (int off = 1; off < 32; off <<= 1) {
-        const int t = __shfl_up_sync(0xffffffffu, w, off);
-        if (tid >= off) w += t;
-      }
-      warp_sums[tid] = w;
-    }
-    __syncthreads();
-    const int c = carry;
-    if (flag) {
-      const int slot = c + ((tid >> 5) ? warp_sums[(tid >> 5) - 1] : 0) + incl - 1;
-      if (slot < a.cap) {
-        a.matches[((long)b * a.cap + slot) * 2] = ind0[i];
-        a.matches[((long)b * a.cap + slot) * 2 + 1] = ind1[j];
-        a.match_scores[(long)b * a.cap + slot] = sc;
-      }
-    }
-    __syncthreads();
-    if (tid == 0) carry = c + warp_sums[31];
-    __syncthreads();
   }
   if (tid == 0) a.n_matches[b] = carry;
 }

@@ -1,0 +1,95 @@
+"""Geometric verification on the GPU: batched RANSAC homography and fundamental-matrix estimation on the matcher's output
+(C ABI ``include/geometry_b200.h``, CUDA ``csrc/geo_api.cu``).
+
+Both functions take ``matches0`` [B, M] int64 exactly as ``LightGlue.forward``, ``PendingMatch.tensors`` and
+``match_ragged`` give it (-1 or any index outside [0, N) is unmatched), run every pair of the batch in one call on the
+current stream, and return device tensors of fixed shapes without synchronising with the host, so a call can follow a
+matcher forward with no read-back in between, or be captured in a CUDA graph.  Parameter names and defaults are those of
+``cv2.findHomography(RANSAC)`` and ``cv2.findFundamentalMat(FM_RANSAC)``.
+
+Returns a dict: ``H`` or ``F`` [B, 3, 3] float64 (H scaled to H[2, 2] = 1; F to unit Frobenius norm with its largest
+entry positive), ``inliers`` [B, M] bool, ``num_inliers`` [B] int32, ``success`` [B] bool, and the diagnostics
+``best_hypothesis`` [B] int32 (-1 without one) and ``num_hypotheses`` [B] int32.  A failed pair (fewer valid matches than
+the sample size, 4 or 8, or no non-degenerate hypothesis) has ``success`` False, a zero model and no inliers.
+"""
+from __future__ import annotations
+
+import ctypes as C
+
+import torch
+
+from . import _cabi
+
+
+def _check_params(threshold, max_iters, confidence, seed) -> None:
+    if not isinstance(max_iters, int) or isinstance(max_iters, bool) or not 1 <= max_iters <= 1 << 24:
+        raise ValueError(f"max_iters={max_iters!r}: an int in [1, 2**24]")
+    if not float(threshold) > 0.0 or float(threshold) == float("inf"):
+        raise ValueError(f"ransac_reproj_threshold={threshold!r}: a positive number of pixels")
+    if not 0.0 <= float(confidence) <= 1.0:
+        raise ValueError(f"confidence={confidence!r}: in [0, 1]")
+    if not isinstance(seed, int) or isinstance(seed, bool) or not 0 <= seed < 1 << 32:
+        raise ValueError(f"seed={seed!r}: an int in [0, 2**32)")
+
+
+def _estimate(kind: int, key: str, kpts0, kpts1, matches0, threshold, max_iters, confidence, seed) -> dict:
+    for name, t in (("kpts0", kpts0), ("kpts1", kpts1), ("matches0", matches0)):
+        if not isinstance(t, torch.Tensor):
+            raise ValueError(f"{name} must be a torch.Tensor")
+        if t.device.type != "cuda":
+            raise RuntimeError("lightglue_b200.geometry runs on CUDA (sm_90a) tensors only; there is no CPU path")
+    if kpts0.dim() != 3 or kpts0.shape[-1] != 2 or kpts1.dim() != 3 or kpts1.shape[-1] != 2:
+        raise ValueError(f"kpts0 {tuple(kpts0.shape)} and kpts1 {tuple(kpts1.shape)}: expected [B, M, 2] and [B, N, 2]")
+    if matches0.dim() != 2 or matches0.shape != kpts0.shape[:2] or kpts1.shape[0] != kpts0.shape[0]:
+        raise ValueError(f"matches0 {tuple(matches0.shape)}: expected [B, M] of kpts0 {tuple(kpts0.shape)} with the "
+                         f"batch of kpts1 {tuple(kpts1.shape)}")
+    if not kpts0.is_floating_point() or not kpts1.is_floating_point():
+        raise ValueError("kpts0 and kpts1 must be floating point pixels")
+    if matches0.dtype != torch.int64:
+        raise ValueError(f"matches0 must be int64, not {matches0.dtype}")
+    if kpts1.device != kpts0.device or matches0.device != kpts0.device:
+        raise ValueError("kpts0, kpts1 and matches0 must be on one device")
+    _check_params(threshold, max_iters, confidence, seed)
+    device = kpts0.device
+    b, m, n = kpts0.shape[0], kpts0.shape[1], kpts1.shape[1]
+    k0 = kpts0.detach().to(torch.float32).contiguous()
+    k1 = kpts1.detach().to(torch.float32).contiguous()
+    m0 = matches0.detach().contiguous()
+    out = {
+        key: torch.empty(b, 3, 3, dtype=torch.float64, device=device),
+        "inliers": torch.empty(b, m, dtype=torch.bool, device=device),
+        "num_inliers": torch.empty(b, dtype=torch.int32, device=device),
+        "success": torch.empty(b, dtype=torch.bool, device=device),
+        "best_hypothesis": torch.empty(b, dtype=torch.int32, device=device),
+        "num_hypotheses": torch.empty(b, dtype=torch.int32, device=device),
+    }
+    if b == 0:
+        return out
+    with torch.cuda.device(device):
+        lib = _cabi.load()
+        ws = torch.empty(lib.geo_workspace_bytes(b, m, max_iters), dtype=torch.uint8, device=device)
+        cfg = _cabi.GeoConfig(_cabi.GEO_ABI_VERSION, kind, max_iters, seed, float(threshold), float(confidence))
+        ins = _cabi.GeoInputs(b, m, n, k0.data_ptr(), k1.data_ptr(), m0.data_ptr())
+        outs = _cabi.GeoOutputs(*(out[k].data_ptr() for k in (key, "inliers", "num_inliers", "success",
+                                                                "best_hypothesis", "num_hypotheses")))
+        stream = torch.cuda.current_stream(device).cuda_stream
+        _cabi.check(lib.geo_estimate(C.byref(cfg), C.byref(ins), C.byref(outs), ws.data_ptr(), ws.numel(), stream),
+                    "geo_estimate")
+    return out
+
+
+def find_homography(kpts0: torch.Tensor, kpts1: torch.Tensor, matches0: torch.Tensor, ransac_reproj_threshold: float = 3.0,
+                    max_iters: int = 2000, confidence: float = 0.995, seed: int = 0) -> dict:
+    """RANSAC homography per pair, mapping kpts0 to kpts1: an inlier has a squared forward transfer error below
+    ``ransac_reproj_threshold ** 2``.  Defaults of ``cv2.findHomography(method=cv2.RANSAC)``."""
+    return _estimate(_cabi.GEO_HOMOGRAPHY, "H", kpts0, kpts1, matches0, ransac_reproj_threshold, max_iters, confidence,
+                     seed)
+
+
+def find_fundamental(kpts0: torch.Tensor, kpts1: torch.Tensor, matches0: torch.Tensor, ransac_reproj_threshold: float = 3.0,
+                     max_iters: int = 1000, confidence: float = 0.99, seed: int = 0) -> dict:
+    """RANSAC fundamental matrix per pair (x1^T F x0 = 0) by the normalised 8-point method: an inlier's larger distance
+    to its two epipolar lines is below ``ransac_reproj_threshold``.  Defaults of
+    ``cv2.findFundamentalMat(method=cv2.FM_RANSAC)``."""
+    return _estimate(_cabi.GEO_FUNDAMENTAL, "F", kpts0, kpts1, matches0, ransac_reproj_threshold, max_iters, confidence,
+                     seed)
