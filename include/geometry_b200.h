@@ -1,5 +1,5 @@
-/* geometry_b200 -- C ABI of batched RANSAC on the matcher's output: a homography or a fundamental matrix per pair, for
- * every pair of a batch in one call.  Same library (liblightglue_b200.so), same conventions as lightglue_b200.h: plain
+/* geometry_b200 -- C ABI of batched RANSAC on the matcher's output: a homography, a fundamental matrix or a relative
+ * pose (E, R, t) per pair, for every pair of a batch in one call.  Same library (liblightglue_b200.so), same conventions as lightglue_b200.h: plain
  * pointers and sizes, device memory owned by the caller, asynchronous on the given stream, int status (0 = ok, message
  * via lg_last_error()).  No handle: there are no weights.  No host synchronisation, fixed output shapes, and a launch
  * sequence that depends on (B, M, max_iters) only, so a call can be captured in a CUDA graph.
@@ -66,6 +66,66 @@
  *
  * A pair fails (success 0, model all zero, no inliers, best_hypothesis -1) when n < s, when its normalisation fails, or
  * when every hypothesis is degenerate.
+ *
+ * Relative pose (geo_relative_pose; oracle/pose_oracle.py restates it bit for bit): an essential matrix E with
+ * x1^T E x0 = 0 on calibrated coordinates, and the (R, t) of x1 = R x0 + t that recoverPose would choose.
+ *
+ * P1. Compaction as step 1.  K = [[fx, s, cx], [0, fy, cy], [0, 0, 1]] per pair and image (K[1][0] is not read);
+ *     y = ((double)v - cy) / fy, x = (((double)u - cx) - s*y) / fx, rounded to float.  The solver, the refit and the
+ *     triangulation read these floats widened to double.  No Hartley step.  A K with a non-finite entry, fx <= 0, fy <= 0
+ *     or a bottom row other than (0, 0, 1) fails its pair.  The threshold is t = threshold / f with
+ *     f = (((fx0 + fy0) + fx1) + fy1) / 4, compared as (float)(t*t).
+ * P2. Sampling as step 3 with s = 5.
+ * P3. Five-point solver, in double.  Rows [u*x, u*y, u, v*x, v*y, v, x, y, 1] (as F) in sample order; the 5x9 system is
+ *     reduced as in step 4 (5 pivots, GEO_PIVOT_EPS).  For free column f = 5..8 a null vector has x_f = 1, the other
+ *     free entries 0 and x[k] = -(a[k][f] + a[k][k+1]*x[k+1] + ... + a[k][4]*x[4]) / a[k][k] for k = 4..0, summed left
+ *     to right: X, Y, Z, W.  Modified Gram-Schmidt in that order (d = running dot product, b_i = b_i - d*b_j for
+ *     j < i, then b_i / sqrt(running sum of squares)).  E = x X + y Y + z Z + W: each entry a polynomial over the
+ *     graded monomials 1 | x y z | xx xy xz yy yz zz | xxx xxy xxz xyy xyz xzz yyy yyz yzz zzz.  A product of two
+ *     polynomials adds a_i*b_j into its monomial for i, then j, ascending, starting from 0.  Constraint 0 is
+ *     (E0*d0 - E1*d1) + E2*d2 with d0 = E4*E8 - E5*E7, d1 = E3*E8 - E5*E6, d2 = E3*E7 - E4*E6 (row-major E0..E8).
+ *     S_ij = (E_i0*E_j0 + E_i1*E_j1) + E_i2*E_j2, tr = (S_00 + S_11) + S_22, and constraint 1 + 3i + j is
+ *     2*((S_i0*E_0j + S_i1*E_1j) + S_i2*E_2j) - tr*E_ij.  The 10x20 matrix has the monomial columns
+ *     xxx yyy xxy xyy xxz xx yyz yy xyz xy | xzz xz x yzz yz y zzz zz z 1.  It is degenerate with a non-finite entry;
+ *     else Gauss-Jordan for k = 0..9: the first row r >= k of largest |g[r][k]| is the pivot (degenerate unless
+ *     > GEO_PIVOT_EPS * max|g|), swapped in, g[k][c] = g[k][c] / g[k][k] and then g[r][c] = g[r][c] - g[r][k]*g[k][c]
+ *     for every r != k in ascending order, c > k.  With R_r = g[r][10..19], rows (4, 5), (6, 7), (8, 9) give
+ *     e - z*f = x*px(z) + y*py(z) + p1(z) with px = [e2, e1 - f2, e0 - f1, -f0], py = [e5, e4 - f5, e3 - f4, -f3],
+ *     p1 = [e9, e8 - f9, e7 - f8, e6 - f7, -f6] (ascending powers): the rows (k, l, m) of a 3x3 B(z).
+ *     det B = (kx*c0 - ky*c1) + k1*c2, c0 = ly*m1 - l1*my, c1 = lx*m1 - l1*mx, c2 = lx*my - ly*mx (univariate
+ *     products in ascending (i, j) from 0): p(z) of degree 10.  Degenerate with a non-finite coefficient or
+ *     |p10| <= GEO_LEAD_EPS * max|p_i|.  q = p / p10; r_b = 1 + max_{i<10} |q_i|.  Sturm sequence: s0 = q,
+ *     s1_i = (i + 1) * q_(i+1); s_k = -r / max|r| with r = s_(k-2) mod s_(k-1) (r_i = a_i - (a_da/b_db)*b_(i-1), then
+ *     r_i = r_i - (r_(da-1)/b_db)*b_i); the sequence ends before a remainder with a non-finite entry or a zero leading
+ *     coefficient.  V(z): sign changes over the members (Horner, zeros skipped); V(-inf), V(+inf) from the leading
+ *     signs; n = max(V(-inf) - V(+inf), 0) roots.  Root k = 1..n: lo = -r_b, hi = r_b and GEO_STURM_STEPS bisections
+ *     (mid = 0.5*(lo + hi); hi = mid when V(-inf) - V(mid) >= k, else lo = mid), then from z = 0.5*(lo + hi)
+ *     GEO_NEWTON_STEPS Newton steps on q (Horner for q and q' together), a non-finite step leaving z.  No real root is
+ *     a degenerate sample.  Per root: B(z) by Horner; of the cross products r0 x r1, r0 x r2, r1 x r2 the first of
+ *     largest |third entry| w gives x = c0 / w, y = c1 / w; E = ((x*X + y*Y) + z*Z) + W is kept when its running sum of
+ *     squares f is finite and positive, scaled to unit Frobenius norm and negated if its first entry of largest
+ *     magnitude is negative.  Solution r is the r-th kept one, in ascending z; a sample has at most
+ *     GEO_MAX_SOLUTIONS.
+ * P4. Scoring in fp32 without fused multiply-adds, every solution of every sample, OpenCV's squared Sampson error:
+ *     (a0, a1, a2) = E x0 row by row as in step 5, d = (u*a0 + v*a1) + a2, b0 = (e0*u + e3*v) + e6,
+ *     b1 = (e1*u + e4*v) + e7, err = (d*d) / (((a0*a0 + a1*a1) + b0*b0) + b1*b1); an inlier has err < (float)(t*t).
+ *     Ties go to the lowest (sample h, solution r): the key packs ~(h*16 + r).  max_iters counts samples.
+ * P5. Stopping as step 6 with s = 5.
+ * P6. Refit.  With at least GEO_REFIT_MIN inliers, the upper triangle of A^T A over the best solution's inliers as
+ *     step 7 (rows of P3), its least eigenvector by the 9x9 cyclic Jacobi, then U diag(1, 1, 0) V^T: one-sided Jacobi
+ *     of step 4 on the 3x3, column m of least squared norm dropped, the other two (i < j) give u1 = a_i / sqrt(n_i),
+ *     u2 = a_j / sqrt(n_j), v1, v2 (columns of V), E_ab = u1_a*v1_b + u2_a*v2_b, scaled as in P3.  The refit replaces
+ *     the solution unless it has fewer inliers.
+ * P7. Pose.  u1, u2, v1, v2 of the final E as in P6, u3 = u1 x u2, v3 = v1 x v2 (so U and V are proper rotations),
+ *     R1_ab = (u2_a*v1_b - u1_a*v2_b) + u3_a*v3_b (U W V^T, W = [[0, -1, 0], [1, 0, 0], [0, 0, 1]]),
+ *     R2_ab = (u1_a*v2_b - u2_a*v1_b) + u3_a*v3_b, candidates (R1, u3), (R2, u3), (R1, -u3), (R2, -u3).  Each inlier
+ *     is triangulated per candidate with P0 = [I | 0], P1 = [R | t]: rows [-1, 0, x, 0], [0, -1, y, 0],
+ *     u*P1_2 - P1_0, v*P1_2 - P1_1, N_ij = ((r0_i*r0_j + r1_i*r1_j) + r2_i*r2_j) + r3_i*r3_j, Q its least eigenvector
+ *     by the same cyclic Jacobi (4x4).  It passes when Q2*Q3 > 0, Z = Q2/Q3 < distance_threshold and
+ *     z1 = ((R_20*X + R_21*Y) + R_22*Z) + t2 lies in (0, distance_threshold), X = Q0/Q3, Y = Q1/Q3.  The candidate
+ *     with most passing points wins (ties: the lowest); its passing points are pose_inliers.
+ * P8. A pair fails (success 0, E, R and t zero, no inliers, best_hypothesis = best_solution = -1) when n < 5, a K is
+ *     invalid, or every sample is degenerate.
  */
 #ifndef GEOMETRY_B200_H
 #define GEOMETRY_B200_H
@@ -92,6 +152,12 @@ extern "C" {
 #define GEO_PIVOT_EPS 1e-10
 #define GEO_SVD_SWEEPS 8
 #define GEO_EIG_SWEEPS 12
+#define GEO_ESSENTIAL 2       /* the relative pose's model, for geo_relative_pose */
+#define GEO_MAX_SOLUTIONS 10
+#define GEO_LEAD_EPS 1e-12
+#define GEO_STURM_STEPS 40
+#define GEO_NEWTON_STEPS 8
+#define GEO_REFIT_MIN 8
 
 typedef struct GeoConfig {
   int32_t abi_version; /* GEO_ABI_VERSION */
@@ -121,6 +187,43 @@ typedef struct GeoOutputs {
 LG_API size_t geo_workspace_bytes(int32_t B, int32_t M, int32_t max_iters);
 LG_API int geo_estimate(const GeoConfig* cfg, const GeoInputs* in, GeoOutputs* out, void* workspace,
                         size_t workspace_bytes, void* stream);
+
+typedef struct GeoPoseConfig {
+  int32_t abi_version;        /* GEO_ABI_VERSION */
+  int32_t max_iters;          /* samples per pair, in [1, GEO_MAX_ITERS] */
+  uint32_t seed;
+  int32_t reserved;
+  double threshold;           /* pixels, > 0: Sampson distance, divided by the pair's mean focal length */
+  double confidence;          /* in [0, 1] */
+  double distance_threshold;  /* > 0: triangulated depth bound of the cheirality test */
+} GeoPoseConfig;
+
+typedef struct GeoPoseInputs {
+  int32_t B, M, N;
+  const float* kpts0;      /* [B, M, 2] */
+  const float* kpts1;      /* [B, N, 2] */
+  const int64_t* matches0; /* [B, M]; indices outside [0, N) are unmatched */
+  const double* K0;        /* [B, 9] row-major intrinsics of image 0 */
+  const double* K1;        /* [B, 9] of image 1 */
+} GeoPoseInputs;
+
+typedef struct GeoPoseOutputs {
+  double* E;                 /* [B, 3, 3] */
+  double* R;                 /* [B, 3, 3] */
+  double* t;                 /* [B, 3], unit */
+  uint8_t* inliers;          /* [B, M] */
+  int32_t* num_inliers;      /* [B] */
+  uint8_t* pose_inliers;     /* [B, M] inliers that pass the chosen pose's cheirality test */
+  int32_t* num_pose_inliers; /* [B] */
+  uint8_t* success;          /* [B] */
+  int32_t* best_hypothesis;  /* [B], -1 without one */
+  int32_t* best_solution;    /* [B], -1 without one */
+  int32_t* num_hypotheses;   /* [B] */
+} GeoPoseOutputs;
+
+LG_API size_t geo_pose_workspace_bytes(int32_t B, int32_t M, int32_t max_iters);
+LG_API int geo_relative_pose(const GeoPoseConfig* cfg, const GeoPoseInputs* in, GeoPoseOutputs* out, void* workspace,
+                             size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }

@@ -19,7 +19,7 @@ SIFT_ABI_VERSION = 1
 DISK_ABI_VERSION = 1
 DHN_ABI_VERSION = 1
 GEO_ABI_VERSION = 1  # include/geometry_b200.h
-GEO_HOMOGRAPHY, GEO_FUNDAMENTAL = 0, 1
+GEO_HOMOGRAPHY, GEO_FUNDAMENTAL, GEO_ESSENTIAL = 0, 1, 2
 
 
 class LgConfig(C.Structure):
@@ -108,6 +108,28 @@ class GeoOutputs(C.Structure):
     ]
 
 
+class GeoPoseConfig(C.Structure):
+    _fields_ = [
+        ("abi_version", C.c_int32), ("max_iters", C.c_int32), ("seed", C.c_uint32), ("reserved", C.c_int32),
+        ("threshold", C.c_double), ("confidence", C.c_double), ("distance_threshold", C.c_double),
+    ]
+
+
+class GeoPoseInputs(C.Structure):
+    _fields_ = [
+        ("B", C.c_int32), ("M", C.c_int32), ("N", C.c_int32),
+        ("kpts0", C.c_void_p), ("kpts1", C.c_void_p), ("matches0", C.c_void_p), ("K0", C.c_void_p), ("K1", C.c_void_p),
+    ]
+
+
+class GeoPoseOutputs(C.Structure):
+    _fields_ = [
+        ("E", C.c_void_p), ("R", C.c_void_p), ("t", C.c_void_p), ("inliers", C.c_void_p), ("num_inliers", C.c_void_p),
+        ("pose_inliers", C.c_void_p), ("num_pose_inliers", C.c_void_p), ("success", C.c_void_p),
+        ("best_hypothesis", C.c_void_p), ("best_solution", C.c_void_p), ("num_hypotheses", C.c_void_p),
+    ]
+
+
 # name: (restype, argtypes), one table per header.  The export lists are the tables' keys.
 _VP, _I32, _I64, _SZ = C.c_void_p, C.c_int32, C.c_int64, C.c_size_t
 _HANDLE_OUT = C.POINTER(C.c_void_p)
@@ -174,6 +196,9 @@ DHN_PROTOTYPES = {  # include/doghardnet_b200.h
 GEO_PROTOTYPES = {  # include/geometry_b200.h
     "geo_workspace_bytes": (_SZ, [_I32, _I32, _I32]),
     "geo_estimate": (C.c_int, [C.POINTER(GeoConfig), C.POINTER(GeoInputs), C.POINTER(GeoOutputs), _VP, _SZ, _VP]),
+    "geo_pose_workspace_bytes": (_SZ, [_I32, _I32, _I32]),
+    "geo_relative_pose": (C.c_int, [C.POINTER(GeoPoseConfig), C.POINTER(GeoPoseInputs), C.POINTER(GeoPoseOutputs), _VP,
+                                    _SZ, _VP]),
 }
 _TABLES = (LG_PROTOTYPES, SP_PROTOTYPES, AL_PROTOTYPES, SIFT_PROTOTYPES, DISK_PROTOTYPES, DHN_PROTOTYPES, GEO_PROTOTYPES)
 EXPORTS, SP_EXPORTS, AL_EXPORTS, SIFT_EXPORTS, DISK_EXPORTS, DHN_EXPORTS, GEO_EXPORTS = (tuple(t) for t in _TABLES)

@@ -11,18 +11,13 @@
 //            outputs
 // A stopped pair's CTAs return at once.  This file is compiled with -fmad=false: every multiply and add rounds on its
 // own, as numpy's do in oracle/geometry_oracle.py.
-#include <cuda_runtime.h>
-#include <float.h>
-#include <math.h>
-
-#include "../../include/geometry_b200.h"
 #include "block_scan.cuh"
+#include "geo_common.cuh"
 #include "lg_internal.h"
 #include "ws_bump.h"
 
 namespace {
 
-constexpr int RED = 256;    // partial sums of the fixed summation order (header step 2)
 constexpr int TILE = 1024;  // points per shared-memory tile of the score kernel
 
 struct GeoPair {
@@ -64,64 +59,17 @@ struct GeoArgs {
   GeoOutputs out;
 };
 
-__device__ __forceinline__ unsigned geo_mix(unsigned x) {
-  x ^= x >> 16;
-  x *= 0x7feb352du;
-  x ^= x >> 15;
-  x *= 0x846ca68bu;
-  x ^= x >> 16;
-  return x;
-}
-
-// The fixed-order sum of the block's RED partials (threads tid < RED hold one each).  Every thread of the block calls
-// it; every thread gets the sum.
-__device__ double tree_sum(double p, double* red, int tid) {
-  if (tid < RED) red[tid] = p;
-  __syncthreads();
-  for (int h = RED / 2; h > 0; h >>= 1) {
-    if (tid < h) red[tid] = red[tid] + red[tid + h];
-    __syncthreads();
-  }
-  const double r = red[0];
-  __syncthreads();
-  return r;
-}
-
 // (A B)_ij = (A_i0 B_0j + A_i1 B_1j) + A_i2 B_2j, row-major 3x3
 __device__ void mm3(const double* A, const double* B, double* C) {
   for (int i = 0; i < 3; ++i)
     for (int j = 0; j < 3; ++j) C[i * 3 + j] = (A[i * 3] * B[j] + A[i * 3 + 1] * B[3 + j]) + A[i * 3 + 2] * B[6 + j];
 }
 
-__device__ __forceinline__ double sgn1(double z) { return z >= 0.0 ? 1.0 : -1.0; }
-
 // Rank 2 by one-sided Jacobi on the columns (header step 4), in place on a row-major 3x3.
 __device__ void rank2(double* F) {
   double A[9], V[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
   for (int i = 0; i < 9; ++i) A[i] = F[i];
-  const int PQ[3][2] = {{0, 1}, {0, 2}, {1, 2}};
-  for (int sweep = 0; sweep < GEO_SVD_SWEEPS; ++sweep)
-    for (int r = 0; r < 3; ++r) {
-      const int p = PQ[r][0], q = PQ[r][1];
-      double al = 0.0, be = 0.0, ga = 0.0;
-      for (int i = 0; i < 3; ++i) {
-        al = al + A[i * 3 + p] * A[i * 3 + p];
-        be = be + A[i * 3 + q] * A[i * 3 + q];
-        ga = ga + A[i * 3 + p] * A[i * 3 + q];
-      }
-      if (fabs(ga) <= 1e-15 * sqrt(al * be)) continue;
-      const double z = (be - al) / (2.0 * ga);
-      const double t = sgn1(z) / (fabs(z) + sqrt(1.0 + z * z));
-      const double c = 1.0 / sqrt(1.0 + t * t), s = c * t;
-      for (int i = 0; i < 3; ++i) {
-        const double ap = A[i * 3 + p], aq = A[i * 3 + q];
-        A[i * 3 + p] = c * ap - s * aq;
-        A[i * 3 + q] = s * ap + c * aq;
-        const double vp = V[i * 3 + p], vq = V[i * 3 + q];
-        V[i * 3 + p] = c * vp - s * vq;
-        V[i * 3 + q] = s * vp + c * vq;
-      }
-    }
+  jacobi_columns3(A, V);
   int m = 0;
   double nm = 0.0;
   for (int j = 0; j < 3; ++j) {
@@ -270,22 +218,6 @@ __device__ __forceinline__ float geo_err(int kind, const float* h, float4 p) {
   return fmaxf(d1 * d1 * s1, d2 * d2 * s2);
 }
 
-// OpenCV's RANSACUpdateNumIters, with pow(1 - ep, s) as repeated products (header step 6)
-__device__ int update_num_iters(double p, double ep, int s, int max_iters) {
-  if (p >= 1.0) return max_iters;
-  p = fmin(fmax(p, 0.0), 1.0);
-  ep = fmin(fmax(ep, 0.0), 1.0);
-  double num = fmax(1.0 - p, DBL_MIN);
-  const double q = 1.0 - ep;
-  double pw = q;
-  for (int i = 1; i < s; ++i) pw = pw * q;
-  double denom = 1.0 - pw;
-  if (denom < DBL_MIN) return 0;
-  num = log(num);
-  denom = log(denom);
-  return (denom >= 0.0 || -num >= max_iters * (-denom)) ? max_iters : __double2int_rn(num / denom);
-}
-
 // Folds chunk c's counts into the pair's best and decides whether the pair stops.  Called by every thread of a
 // GEO_CHUNK-thread CTA; thread t owns hypothesis c * GEO_CHUNK + t.
 __device__ void geo_fold(const GeoArgs& a, int b, int c) {
@@ -413,41 +345,6 @@ __device__ __forceinline__ int geo_rows(int kind, const GeoPair& P, float4 p, do
   return 1;
 }
 
-// Smallest-eigenvalue eigenvector of a symmetric 9x9 by cyclic Jacobi (header step 7)
-__device__ void smallest_eigvec(double (*A)[9], double* out) {
-  double V[9][9];
-  for (int i = 0; i < 9; ++i)
-    for (int j = 0; j < 9; ++j) V[i][j] = i == j ? 1.0 : 0.0;
-  for (int sweep = 0; sweep < GEO_EIG_SWEEPS; ++sweep)
-    for (int p = 0; p < 8; ++p)
-      for (int q = p + 1; q < 9; ++q) {
-        const double apq = A[p][q];
-        if (apq == 0.0) continue;
-        const double z = (A[q][q] - A[p][p]) / (2.0 * apq);
-        const double t = sgn1(z) / (fabs(z) + sqrt(z * z + 1.0));
-        const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
-        for (int k = 0; k < 9; ++k) {
-          const double akp = A[k][p], akq = A[k][q];
-          A[k][p] = c * akp - s * akq;
-          A[k][q] = s * akp + c * akq;
-        }
-        for (int k = 0; k < 9; ++k) {
-          const double apk = A[p][k], aqk = A[q][k];
-          A[p][k] = c * apk - s * aqk;
-          A[q][k] = s * apk + c * aqk;
-        }
-        for (int k = 0; k < 9; ++k) {
-          const double vkp = V[k][p], vkq = V[k][q];
-          V[k][p] = c * vkp - s * vkq;
-          V[k][q] = s * vkp + c * vkq;
-        }
-      }
-  int m = 0;
-  for (int k = 1; k < 9; ++k)
-    if (A[k][k] < A[m][m]) m = k;
-  for (int k = 0; k < 9; ++k) out[k] = V[k][m];
-}
-
 __global__ void __launch_bounds__(RED, 1) geo_refit_kernel(GeoArgs a) {
   const int b = blockIdx.x, t = threadIdx.x;
   geo_fold(a, b, a.chunks - 1);
@@ -507,7 +404,7 @@ __global__ void __launch_bounds__(RED, 1) geo_refit_kernel(GeoArgs a) {
       double A[9][9], v[9];
       for (int i = 0, e = 0; i < 9; ++i)
         for (int j = i; j < 9; ++j, ++e) A[i][j] = A[j][i] = ata[e];
-      smallest_eigvec(A, v);
+      smallest_eigvec<9>(A, v);
       if (a.kind == GEO_FUNDAMENTAL) rank2(v);
       denormalise(a.kind, P, v, model[1]);
       for (int i = 0; i < 9; ++i) fm[1][i] = (float)model[1][i];

@@ -1,13 +1,14 @@
-"""Geometric verification on the GPU: batched RANSAC homography and fundamental-matrix estimation on the matcher's output
-(C ABI ``include/geometry_b200.h``, CUDA ``csrc/geo_api.cu``).
+"""Geometric verification on the GPU: batched RANSAC homography, fundamental-matrix and relative-pose estimation on the
+matcher's output (C ABI ``include/geometry_b200.h``, CUDA ``csrc/geo_api.cu`` and ``csrc/pose_api.cu``).
 
-Both functions take ``matches0`` [B, M] int64 exactly as ``LightGlue.forward``, ``PendingMatch.tensors`` and
+All three functions take ``matches0`` [B, M] int64 exactly as ``LightGlue.forward``, ``PendingMatch.tensors`` and
 ``match_ragged`` give it (-1 or any index outside [0, N) is unmatched), run every pair of the batch in one call on the
 current stream, and return device tensors of fixed shapes without synchronising with the host, so a call can follow a
 matcher forward with no read-back in between, or be captured in a CUDA graph.  Parameter names and defaults are those of
-``cv2.findHomography(RANSAC)`` and ``cv2.findFundamentalMat(FM_RANSAC)``.
+``cv2.findHomography(RANSAC)``, ``cv2.findFundamentalMat(FM_RANSAC)`` and ``cv2.findEssentialMat(RANSAC)`` with
+``cv2.recoverPose``.
 
-Returns a dict: ``H`` or ``F`` [B, 3, 3] float64 (H scaled to H[2, 2] = 1; F to unit Frobenius norm with its largest
+``find_homography`` and ``find_fundamental`` return a dict: ``H`` or ``F`` [B, 3, 3] float64 (H scaled to H[2, 2] = 1; F to unit Frobenius norm with its largest
 entry positive), ``inliers`` [B, M] bool, ``num_inliers`` [B] int32, ``success`` [B] bool, and the diagnostics
 ``best_hypothesis`` [B] int32 (-1 without one) and ``num_hypotheses`` [B] int32.  A failed pair (fewer valid matches than
 the sample size, 4 or 8, or no non-degenerate hypothesis) has ``success`` False, a zero model and no inliers.
@@ -32,7 +33,7 @@ def _check_params(threshold, max_iters, confidence, seed) -> None:
         raise ValueError(f"seed={seed!r}: an int in [0, 2**32)")
 
 
-def _estimate(kind: int, key: str, kpts0, kpts1, matches0, threshold, max_iters, confidence, seed) -> dict:
+def _check_inputs(kpts0, kpts1, matches0) -> None:
     for name, t in (("kpts0", kpts0), ("kpts1", kpts1), ("matches0", matches0)):
         if not isinstance(t, torch.Tensor):
             raise ValueError(f"{name} must be a torch.Tensor")
@@ -49,6 +50,10 @@ def _estimate(kind: int, key: str, kpts0, kpts1, matches0, threshold, max_iters,
         raise ValueError(f"matches0 must be int64, not {matches0.dtype}")
     if kpts1.device != kpts0.device or matches0.device != kpts0.device:
         raise ValueError("kpts0, kpts1 and matches0 must be on one device")
+
+
+def _estimate(kind: int, key: str, kpts0, kpts1, matches0, threshold, max_iters, confidence, seed) -> dict:
+    _check_inputs(kpts0, kpts1, matches0)
     _check_params(threshold, max_iters, confidence, seed)
     device = kpts0.device
     b, m, n = kpts0.shape[0], kpts0.shape[1], kpts1.shape[1]
@@ -93,3 +98,67 @@ def find_fundamental(kpts0: torch.Tensor, kpts1: torch.Tensor, matches0: torch.T
     ``cv2.findFundamentalMat(method=cv2.FM_RANSAC)``."""
     return _estimate(_cabi.GEO_FUNDAMENTAL, "F", kpts0, kpts1, matches0, ransac_reproj_threshold, max_iters, confidence,
                      seed)
+
+
+def _intrinsics(name: str, K, b: int, device) -> torch.Tensor:
+    if not isinstance(K, torch.Tensor):
+        raise ValueError(f"{name} must be a torch.Tensor")
+    if K.device.type != "cuda":
+        raise RuntimeError("lightglue_b200.geometry runs on CUDA (sm_90a) tensors only; there is no CPU path")
+    if not K.is_floating_point():
+        raise ValueError(f"{name} must be floating point")
+    if K.shape == (3, 3):
+        K = K.expand(b, 3, 3)
+    elif K.dim() != 3 or K.shape != (b, 3, 3):
+        raise ValueError(f"{name} {tuple(K.shape)}: expected [3, 3] or [B, 3, 3] with B = {b}")
+    if K.device != device:
+        raise ValueError(f"{name} must be on the device of kpts0")
+    return K.detach().to(torch.float64).contiguous()
+
+
+def estimate_relative_pose(kpts0: torch.Tensor, kpts1: torch.Tensor, matches0: torch.Tensor, K0: torch.Tensor,
+                           K1: torch.Tensor | None = None, ransac_reproj_threshold: float = 1.0, max_iters: int = 1000,
+                           confidence: float = 0.999, distance_threshold: float = 50.0, seed: int = 0) -> dict:
+    """Relative pose per pair: a five-point RANSAC essential matrix on calibrated coordinates, then the (R, t) of
+    ``cv2.recoverPose`` by its cheirality test.  ``K0`` and ``K1`` are [3, 3] or [B, 3, 3] (``K1=None``: K0); the pixel
+    threshold is divided by the pair's mean focal length (fx0 + fy0 + fx1 + fy1) / 4.  Defaults of
+    ``cv2.findEssentialMat(method=cv2.RANSAC)`` and ``cv2.recoverPose``.
+
+    Returns ``E``, ``R`` [B, 3, 3] and ``t`` [B, 3] float64 with x1 = R x0 + t, |t| = 1 and E of unit Frobenius norm
+    with its largest entry positive; ``inliers`` [B, M] bool and ``num_inliers`` [B] int32 of the RANSAC;
+    ``pose_inliers`` and ``num_pose_inliers``, the inliers that pass the chosen pose's cheirality test; ``success``
+    [B] bool; and the diagnostics ``best_hypothesis``, ``best_solution`` and ``num_hypotheses`` [B] int32.  A pair
+    with fewer than 5 valid matches, an invalid K (a non-finite entry, fx or fy <= 0, or a bottom row other than
+    [0, 0, 1]) or no non-degenerate sample has ``success`` False, zero E, R and t, and no inliers."""
+    _check_inputs(kpts0, kpts1, matches0)
+    _check_params(ransac_reproj_threshold, max_iters, confidence, seed)
+    if not float(distance_threshold) > 0.0 or float(distance_threshold) == float("inf"):
+        raise ValueError(f"distance_threshold={distance_threshold!r}: a positive number")
+    device = kpts0.device
+    b, m, n = kpts0.shape[0], kpts0.shape[1], kpts1.shape[1]
+    k0 = _intrinsics("K0", K0, b, device)
+    k1 = k0 if K1 is None else _intrinsics("K1", K1, b, device)
+    p0 = kpts0.detach().to(torch.float32).contiguous()
+    p1 = kpts1.detach().to(torch.float32).contiguous()
+    m0 = matches0.detach().contiguous()
+    keys = ("E", "R", "t", "inliers", "num_inliers", "pose_inliers", "num_pose_inliers", "success", "best_hypothesis",
+            "best_solution", "num_hypotheses")
+    f64, i32, bl = torch.float64, torch.int32, torch.bool
+    shapes = {"E": ((b, 3, 3), f64), "R": ((b, 3, 3), f64), "t": ((b, 3), f64), "inliers": ((b, m), bl),
+              "num_inliers": ((b,), i32), "pose_inliers": ((b, m), bl), "num_pose_inliers": ((b,), i32),
+              "success": ((b,), bl), "best_hypothesis": ((b,), i32), "best_solution": ((b,), i32),
+              "num_hypotheses": ((b,), i32)}
+    out = {k: torch.empty(*shapes[k][0], dtype=shapes[k][1], device=device) for k in keys}
+    if b == 0:
+        return out
+    with torch.cuda.device(device):
+        lib = _cabi.load()
+        ws = torch.empty(lib.geo_pose_workspace_bytes(b, m, max_iters), dtype=torch.uint8, device=device)
+        cfg = _cabi.GeoPoseConfig(_cabi.GEO_ABI_VERSION, max_iters, seed, 0, float(ransac_reproj_threshold),
+                                  float(confidence), float(distance_threshold))
+        ins = _cabi.GeoPoseInputs(b, m, n, p0.data_ptr(), p1.data_ptr(), m0.data_ptr(), k0.data_ptr(), k1.data_ptr())
+        outs = _cabi.GeoPoseOutputs(*(out[k].data_ptr() for k in keys))
+        stream = torch.cuda.current_stream(device).cuda_stream
+        _cabi.check(lib.geo_relative_pose(C.byref(cfg), C.byref(ins), C.byref(outs), ws.data_ptr(), ws.numel(), stream),
+                    "geo_relative_pose")
+    return out

@@ -1,0 +1,104 @@
+"""Batched GPU relative pose (lightglue_b200.geometry.estimate_relative_pose) against OpenCV on the host, and its cost
+behind the matcher.
+
+Prints one JSON line:
+  * the card's name and power limit, read in this run;
+  * GPU ms per batch (CUDA events) at B pairs of M putative matches and 20 / 50 / 70 % outliers, with OpenCV's
+    adaptive stopping ("adaptive") and with confidence 1 ("full", every sample);
+  * cv2.findEssentialMat(RANSAC) + cv2.recoverPose on the host for the same pairs, one after another and in a thread
+    pool (null without cv2);
+  * pairs/s of LightGlue (bf16x3, N = 2048, synthetic weights) alone and followed by estimate_relative_pose on one
+    stream.
+The scenes come from oracle/pose_oracle.calibrated_two_view (0.5 px noise, 640x480, f = 500); nothing is written to disk.
+"""
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import sys
+import time
+from concurrent.futures import ThreadPoolExecutor
+
+import numpy as np
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+from lightglue_b200 import LightGlue, synth  # noqa: E402
+from lightglue_b200.geometry import estimate_relative_pose  # noqa: E402
+from oracle import pose_oracle as po  # noqa: E402
+from tools.geometry_bench import gpu_info, time_gpu  # noqa: E402
+
+
+def opencv_times(k0, k1, m0, K, threads):
+    try:
+        import cv2
+    except ImportError:
+        return None
+    cv2.setNumThreads(1)
+
+    def one(b):
+        v = m0[b] >= 0
+        a, c = k0[b][v].astype(np.float64), k1[b][m0[b][v]].astype(np.float64)
+        E, mask = cv2.findEssentialMat(a, c, K, cv2.RANSAC, 0.999, 1.0, maxIters=1000)
+        cv2.recoverPose(E[:3], a, c, K, mask=mask)
+
+    t = time.perf_counter()
+    for b in range(len(m0)):
+        one(b)
+    seq = (time.perf_counter() - t) * 1e3
+    with ThreadPoolExecutor(threads) as ex:
+        t = time.perf_counter()
+        list(ex.map(one, range(len(m0))))
+        pool = (time.perf_counter() - t) * 1e3
+    return {"sequential_ms": round(seq, 2), "pool_ms": round(pool, 2), "threads": threads}
+
+
+def main() -> None:
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--batch", type=int, default=32)
+    ap.add_argument("--matches", type=int, default=2048)
+    ap.add_argument("--reps", type=int, default=10)
+    ap.add_argument("--steps", type=int, default=20, help="matcher steps per pairs/s measurement")
+    args = ap.parse_args()
+    torch.set_grad_enabled(False)
+    res = {"tool": "pose_bench", **gpu_info(), "B": args.batch, "matches": args.matches, "pose": {}}
+    threads = os.cpu_count() or 1
+    for o in (0.2, 0.5, 0.7):
+        pairs = [po.calibrated_two_view(args.matches, o, 1000 + b, unmatched=0.0) for b in range(args.batch)]
+        k0, k1, m0, _, K, _, _, _ = (np.stack([p[i] for p in pairs]) for i in range(8))
+        t0, t1, tm, tk = (torch.from_numpy(x).cuda() for x in (k0, k1, m0, K[0]))
+        row = {}
+        for mode, c in (("adaptive", 0.999), ("full", 1.0)):
+            out = estimate_relative_pose(t0, t1, tm, tk, confidence=c)
+            row[mode] = {"gpu_ms": round(time_gpu(lambda: estimate_relative_pose(t0, t1, tm, tk, confidence=c),
+                                                  args.reps), 3),
+                         "mean_samples": float(out["num_hypotheses"].float().mean()),
+                         "mean_inliers": float(out["num_inliers"].float().mean())}
+        row["opencv"] = opencv_times(k0, k1, m0, K[0], threads)
+        res["pose"][f"outliers{o}"] = row
+    # the matcher alone, and followed by the relative pose on its device output (no host read-back in between)
+    data, _ = synth.make_pair(2048, b=args.batch, seed=7)
+    cuda = {k: {kk: vv.cuda() for kk, vv in v.items()} for k, v in data.items()}
+    m = LightGlue(features=None, depth_confidence=-1, width_confidence=-1, precision="bf16x3")
+    m.load_state_dict(synth.make_state_dict(), strict=False)
+    m = m.eval().cuda()
+    Kc = torch.tensor([[800.0, 0.0, 512.0], [0.0, 800.0, 384.0], [0.0, 0.0, 1.0]], dtype=torch.float64, device="cuda")
+
+    def matcher_only():
+        return m.forward_async(cuda).tensors["matches0"]
+
+    def matcher_pose():
+        m0 = m.forward_async(cuda).tensors["matches0"]
+        return estimate_relative_pose(cuda["image0"]["keypoints"], cuda["image1"]["keypoints"], m0, Kc)
+
+    for name, f in (("lightglue", matcher_only), ("lightglue_plus_pose", matcher_pose),
+                    ("lightglue_again", matcher_only)):
+        ms = time_gpu(f, args.steps)
+        res[f"{name}_pairs_per_s"] = round(args.batch / ms * 1e3, 1)
+    print(json.dumps(res))
+
+
+if __name__ == "__main__":
+    main()
