@@ -1,7 +1,8 @@
-/* geometry_b200 -- C ABI of batched RANSAC on the matcher's output: a homography, a fundamental matrix or a relative
- * pose (E, R, t) per pair, for every pair of a batch in one call.  Same library (liblightglue_b200.so), same conventions as lightglue_b200.h: plain
- * pointers and sizes, device memory owned by the caller, asynchronous on the given stream, int status (0 = ok, message
- * via lg_last_error()).  No handle: there are no weights.  No host synchronisation, fixed output shapes, and a launch
+/* geometry_b200 -- C ABI of batched RANSAC on the matcher's output: a homography, a fundamental matrix, a relative
+ * pose (E, R, t) or an absolute pose (R, t from 2D-3D matches) per pair, for every pair of a batch in one call.  Same
+ * library (liblightglue_b200.so), same conventions as lightglue_b200.h: plain pointers and sizes, device memory owned
+ * by the caller, asynchronous on the given stream, int status (0 = ok, message via lg_last_error()).  No handle: there
+ * are no weights.  No host synchronisation, fixed output shapes, and a launch
  * sequence that depends on (B, M, max_iters) only, so a call can be captured in a CUDA graph.
  *
  * The algorithm, exactly (oracle/geometry_oracle.py restates it in numpy and matches it bit for bit):
@@ -126,6 +127,80 @@
  *     with most passing points wins (ties: the lowest); its passing points are pose_inliers.
  * P8. A pair fails (success 0, E, R and t zero, no inliers, best_hypothesis = best_solution = -1) when n < 5, a K is
  *     invalid, or every sample is degenerate.
+ *
+ * Absolute pose (geo_absolute_pose; oracle/pnp_oracle.py restates it bit for bit): the (R, t) of x_cam = R X + t that
+ * maps the world points of image 1's keypoints into the query camera 0, OpenCV's rvec/tvec convention.  Expressions
+ * below evaluate left to right as written (a + b + c is (a + b) + c); no step whose result must match bit for bit calls
+ * cbrt, acos, atan2, sin, cos or pow: + - * / and sqrt round alike everywhere.
+ *
+ * A1. Compaction as step 1, where match i is valid when also the float point X = points3d1[b, matches0[b, i]] has three
+ *     finite coordinates.  Point k is the pixel (u, v) = kpts0[b, i_k] and the world point X_k, both float.
+ * A2. Calibrated coordinates of the pixels through K0 as P1 (K0 checked as P1).  The solver reads them and the world
+ *     points widened to double.
+ * A3. Sampling as step 3 with s = 3.
+ * A4. Lambda Twist P3P (Persson & Nordberg, ECCV 2018), in double.  Bearings y_k = (x, y, 1) / sqrt(x*x + y*y + 1.0);
+ *     b12 = -2.0 * y0.y1, b13 = -2.0 * y0.y2, b23 = -2.0 * y1.y2 (a.b = a0*b0 + a1*b1 + a2*b2); d12 = X0 - X1,
+ *     d13 = X0 - X2, d23 = X1 - X2, a12 = d12.d12, a13 = d13.d13, a23 = d23.d23, n = d12 x d13.  The sample is degenerate
+ *     (collinear or coincident points) unless n.n > GEO_PNP_COLLINEAR_EPS * (a12 * a13).  With c31 = -0.5 * b13,
+ *     c23 = -0.5 * b23, c12 = -0.5 * b12, blob = c12 * c23 * c31 - 1.0, sij = 1.0 - cij * cij:
+ *       p3 = a13 * (a23 * s31 - a13 * s23)
+ *       p2 = 2.0 * blob * a23 * a13 + a13 * (2.0 * a12 + a13) * s23 + a23 * (a23 - a12) * s31
+ *       p1 = a23 * (a13 - a23) * s12 - a12 * a12 * s23 - 2.0 * a12 * (blob * a23 + a13 * s23)
+ *       p0 = a12 * (a12 * s23 - a23 * s12)
+ *     h(g) = ((g + cb) * g + cc) * g + cd with cb = p2 / p3, cc = p1 / p3, cd = p0 / p3 (degenerate unless all finite).
+ *     Root: rb = 1.0 + max(|cb|, |cc|, |cd|), bracket [-rb, rb]; when disc = cb * cb - 3.0 * cc >= 0, v = sqrt(disc),
+ *     t1 = (-cb - v) / 3.0: [-rb, t1] if h(t1) > 0 (the leftmost root), else [(-cb + v) / 3.0, rb] (the rightmost).
+ *     GEO_PNP_BISECT_STEPS bisections (mid = 0.5 * (lo + hi); hi = mid when h(mid) > 0, else lo = mid), then from
+ *     g = 0.5 * (lo + hi) GEO_PNP_NEWTON_STEPS steps g - h(g) / ((3.0 * g + 2.0 * cb) * g + cc), a non-finite step
+ *     leaving g.  Then A00 = a23 * (1.0 - g), A01 = a23 * b12 * 0.5, A02 = a23 * b13 * g * -0.5,
+ *     A11 = a23 - a12 + a13 * g, A12 = b23 * (a13 * g - a12) * 0.5, A22 = g * (a13 - a23) - a12.
+ *     root2(b, c): y = sqrt(fmax(b * b - 4.0 * c, 0.0)), q = -0.5 * (b + (b >= 0 ? y : -y)), roots (q, c / q).
+ *     (e1, e2) = root2(-A00 - A11 - A22, -(A01 * A01) - A02 * A02 - A12 * A12 + A00 * (A11 + A22) + A11 * A22),
+ *     swapped when |e1| < |e2|.  For e = e1, e2: tmp = 1.0 / (e * (A00 + A11) + mx - e * e + A01 * A01) with
+ *     mx = -(A00 * A11), a1 = -(e * A02 + pr0) * tmp, a2 = -(e * A12 + pr1) * tmp with pr0 = A01 * A12 - A02 * A11,
+ *     pr1 = A01 * A02 - A00 * A12, rn = 1.0 / sqrt(a1 * a1 + a2 * a2 + 1.0): the vectors v1 (of e1), v2 (of e2) =
+ *     (a1 * rn, a2 * rn, rn).  sv = sqrt(fmax(0.0, -e2 / e1)).  For s = sv, then -sv: w2 = 1.0 / (s * v2_0 - v1_0),
+ *     w0 = (v1_1 - s * v2_1) * w2, w1 = (v1_2 - s * v2_2) * w2,
+ *       ia = 1.0 / ((a13 - a12) * w1 * w1 - a12 * b13 * w1 - a12)
+ *       qb = (a13 * b12 * w1 - a12 * b13 * w0 - 2.0 * w0 * w1 * (a12 - a13)) * ia
+ *       qc = ((a13 - a12) * w0 * w0 + a13 * b12 * w0 + a13) * ia;
+ *     when qb * qb - 4.0 * qc >= 0, for tau of root2(qb, qc) in order: with tau > 0, d = a23 / (tau * (b23 + tau) + 1.0)
+ *     > 0, l2 = sqrt(d), l3 = tau * l2, l1 = w0 * l2 + w1 * l3 >= 0, the lambdas take GEO_PNP_GN_STEPS Gauss-Newton
+ *     steps: r1 = l1 * l1 + l2 * l2 + b12 * l1 * l2 - a12, r2 (l1, l3, b13, a13), r3 (l2, l3, b23, a23);
+ *     v0 = 2.0 * l1 + b12 * l2, v1 = 2.0 * l2 + b12 * l1, v3 = 2.0 * l1 + b13 * l3, v5 = 2.0 * l3 + b13 * l1,
+ *     v7 = 2.0 * l2 + b23 * l3, v8 = 2.0 * l3 + b23 * l2, det = -(v0 * v5 * v7) - v1 * v3 * v8,
+ *     j0 = -(v5 * v7) * r1 - v1 * v8 * r2 + v1 * v5 * r3, j1 = -(v3 * v8) * r1 + v0 * v8 * r2 - v0 * v5 * r3,
+ *     j2 = v3 * v7 * r1 - v0 * v7 * r2 - v1 * v3 * r3, l_i = l_i - j_(i-1) / det unless a new l is non-finite.
+ *     Pose: ry_k = y_k * l_k, e1 = ry0 - ry1, e2 = ry0 - ry2, e3 = e1 x e2; R_ij = e1_i * Xi_0j + e2_i * Xi_1j +
+ *     e3_i * Xi_2j with Xi the inverse of [d12 d13 n] (columns) by cofactors (C_ij of row i, column j,
+ *     det = x00 * C00 + x01 * C01 + x02 * C02, Xi_ij = C_ji / det); t_i = ry0_i - (R_i0 * X0_0 + R_i1 * X0_1 +
+ *     R_i2 * X0_2).  A solution is kept when its R and t are finite; solution r is the r-th kept one, at most
+ *     GEO_PNP_MAX_SOLUTIONS.  A sample without one is degenerate.
+ * A5. Scoring in fp32 without fused multiply-adds, every solution of every sample: P = K0 [R | t], P_ij = K_i0 * M_0j +
+ *     K_i1 * M_1j + K_i2 * M_2j in double with M = [R | t], rounded to float (p0..p11 row-major);
+ *     w = p8 * X + p9 * Y + p10 * Z + p11, iw = 1 / w, du = u - (p0 * X + p1 * Y + p2 * Z + p3) * iw, dv likewise with
+ *     p4..p7.  An inlier has w > 0 (in front of the camera) and du * du + dv * dv < (float)(threshold * threshold).
+ *     Ties go to the lowest (sample h, solution r): the key packs ~(h*16 + r).  max_iters counts samples.
+ * A6. Stopping as step 6 with s = 3.
+ * A7. Refit.  With at least GEO_PNP_REFIT_MIN inliers, GEO_PNP_LM_STEPS Levenberg-Marquardt steps in double on the
+ *     squared pixel error of the best solution's inliers, from that solution's (R, t); no convergence test.  At a pose,
+ *     per inlier: Xc_i = R_i0 * X + R_i1 * Y + R_i2 * Z + t_i, iz = 1.0 / Xc2, a = Xc0 * iz, b = Xc1 * iz,
+ *     pu = fx * a + s * b, ru = pu + cx - u, rv = fy * b + cy - v (fx = K0[0], s = K0[1], cx = K0[2], fy = K0[4],
+ *     cy = K0[5]); gu = (fx * iz, s * iz, -(pu * iz)), gv = (0.0, fy * iz, -(fy * b * iz)); for g = gu, gv the Jacobian
+ *     row (g2 * Xc1 - g1 * Xc2, g0 * Xc2 - g2 * Xc0, g1 * Xc0 - g0 * Xc1, g0, g1, g2) = ju, jv.  The 28 terms
+ *     ju_i * ju_j + jv_i * jv_j (i <= j in row order), ju_i * ru + jv_i * rv and ru * ru + rv * rv are each summed over
+ *     the points in the order of step 2, other points adding 0: H, g and the cost.  A step: H with its diagonal times
+ *     (1.0 + lambda), Cholesky (for j: d = A_jj - L_j0^2 - ... left to right, failing unless d > 0, L_jj = sqrt(d),
+ *     L_ij = (A_ij - L_i0 * L_j0 - ...) / L_jj for i > j), forward then back substitution for delta with right-hand
+ *     side -g, failing on a non-finite delta.  q = (1.0, delta0 * 0.5, delta1 * 0.5, delta2 * 0.5) / sqrt(w*w + x*x +
+ *     y*y + z*z), Q its rotation ([1.0 - 2.0 * (y*y + z*z), 2.0 * (x*y - w*z), 2.0 * (x*z + w*y)], [2.0 * (x*y + w*z),
+ *     1.0 - 2.0 * (x*x + z*z), 2.0 * (y*z - w*x)], [2.0 * (x*z - w*y), 2.0 * (y*z + w*x), 1.0 - 2.0 * (x*x + y*y)]),
+ *     R' = Q R (3x3 product as in step 4), t'_i = Q_i0 * t0 + Q_i1 * t1 + Q_i2 * t2 + delta_(3+i).  The step is taken
+ *     only if the cost at (R', t') is strictly lower, then lambda = lambda / 10.0; a failed or rejected step sets
+ *     lambda = lambda * 10.0.  lambda starts at GEO_PNP_LM_LAMBDA0.  The refit is re-scored as A5 and replaces the
+ *     solution unless it has fewer inliers; inliers and num_inliers are the final pose's.
+ * A8. A pair fails (success 0, R and t zero, no inliers, best_hypothesis = best_solution = -1, num_hypotheses the
+ *     samples drawn) when n < 3, K0 is invalid, or every sample is degenerate.
  */
 #ifndef GEOMETRY_B200_H
 #define GEOMETRY_B200_H
@@ -223,6 +298,47 @@ typedef struct GeoPoseOutputs {
 
 LG_API size_t geo_pose_workspace_bytes(int32_t B, int32_t M, int32_t max_iters);
 LG_API int geo_relative_pose(const GeoPoseConfig* cfg, const GeoPoseInputs* in, GeoPoseOutputs* out, void* workspace,
+                             size_t workspace_bytes, void* stream);
+
+#define GEO_PNP_MAX_SOLUTIONS 4
+#define GEO_PNP_COLLINEAR_EPS 1e-10
+#define GEO_PNP_BISECT_STEPS 60
+#define GEO_PNP_NEWTON_STEPS 4
+#define GEO_PNP_GN_STEPS 3
+#define GEO_PNP_LM_STEPS 10
+#define GEO_PNP_LM_LAMBDA0 1e-3
+#define GEO_PNP_REFIT_MIN 6
+
+typedef struct GeoPnpConfig {
+  int32_t abi_version; /* GEO_ABI_VERSION */
+  int32_t max_iters;   /* samples per pair, in [1, GEO_MAX_ITERS] */
+  uint32_t seed;
+  int32_t reserved;
+  double threshold;    /* pixels, > 0: reprojection error in image 0 */
+  double confidence;   /* in [0, 1] */
+} GeoPnpConfig;
+
+typedef struct GeoPnpInputs {
+  int32_t B, M, N;
+  const float* kpts0;      /* [B, M, 2] query pixels */
+  const float* points3d1;  /* [B, N, 3] world point of each keypoint of image 1; a non-finite coordinate: none */
+  const int64_t* matches0; /* [B, M]; indices outside [0, N) are unmatched */
+  const double* K0;        /* [B, 9] row-major intrinsics of image 0 */
+} GeoPnpInputs;
+
+typedef struct GeoPnpOutputs {
+  double* R;                /* [B, 3, 3] world to camera: x_cam = R X + t */
+  double* t;                /* [B, 3] */
+  uint8_t* inliers;         /* [B, M] */
+  int32_t* num_inliers;     /* [B] */
+  uint8_t* success;         /* [B] */
+  int32_t* best_hypothesis; /* [B], -1 without one */
+  int32_t* best_solution;   /* [B], -1 without one */
+  int32_t* num_hypotheses;  /* [B] */
+} GeoPnpOutputs;
+
+LG_API size_t geo_pnp_workspace_bytes(int32_t B, int32_t M, int32_t max_iters);
+LG_API int geo_absolute_pose(const GeoPnpConfig* cfg, const GeoPnpInputs* in, GeoPnpOutputs* out, void* workspace,
                              size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus

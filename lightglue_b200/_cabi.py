@@ -130,6 +130,28 @@ class GeoPoseOutputs(C.Structure):
     ]
 
 
+class GeoPnpConfig(C.Structure):
+    _fields_ = [
+        ("abi_version", C.c_int32), ("max_iters", C.c_int32), ("seed", C.c_uint32), ("reserved", C.c_int32),
+        ("threshold", C.c_double), ("confidence", C.c_double),
+    ]
+
+
+class GeoPnpInputs(C.Structure):
+    _fields_ = [
+        ("B", C.c_int32), ("M", C.c_int32), ("N", C.c_int32),
+        ("kpts0", C.c_void_p), ("points3d1", C.c_void_p), ("matches0", C.c_void_p), ("K0", C.c_void_p),
+    ]
+
+
+class GeoPnpOutputs(C.Structure):
+    _fields_ = [
+        ("R", C.c_void_p), ("t", C.c_void_p), ("inliers", C.c_void_p), ("num_inliers", C.c_void_p),
+        ("success", C.c_void_p), ("best_hypothesis", C.c_void_p), ("best_solution", C.c_void_p),
+        ("num_hypotheses", C.c_void_p),
+    ]
+
+
 # name: (restype, argtypes), one table per header.  The export lists are the tables' keys.
 _VP, _I32, _I64, _SZ = C.c_void_p, C.c_int32, C.c_int64, C.c_size_t
 _HANDLE_OUT = C.POINTER(C.c_void_p)
@@ -198,6 +220,9 @@ GEO_PROTOTYPES = {  # include/geometry_b200.h
     "geo_estimate": (C.c_int, [C.POINTER(GeoConfig), C.POINTER(GeoInputs), C.POINTER(GeoOutputs), _VP, _SZ, _VP]),
     "geo_pose_workspace_bytes": (_SZ, [_I32, _I32, _I32]),
     "geo_relative_pose": (C.c_int, [C.POINTER(GeoPoseConfig), C.POINTER(GeoPoseInputs), C.POINTER(GeoPoseOutputs), _VP,
+                                    _SZ, _VP]),
+    "geo_pnp_workspace_bytes": (_SZ, [_I32, _I32, _I32]),
+    "geo_absolute_pose": (C.c_int, [C.POINTER(GeoPnpConfig), C.POINTER(GeoPnpInputs), C.POINTER(GeoPnpOutputs), _VP,
                                     _SZ, _VP]),
 }
 _TABLES = (LG_PROTOTYPES, SP_PROTOTYPES, AL_PROTOTYPES, SIFT_PROTOTYPES, DISK_PROTOTYPES, DHN_PROTOTYPES, GEO_PROTOTYPES)

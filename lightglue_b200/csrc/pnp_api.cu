@@ -1,0 +1,660 @@
+// Batched absolute pose on the matcher's 2D-3D matches: Lambda Twist P3P RANSAC, then Levenberg-Marquardt on the
+// inliers (include/geometry_b200.h, steps A1-A8).
+//
+// Launches, all fixed by (B, M, max_iters):
+//   prepare  one 1024-thread CTA per pair: ordered compaction of the valid matches, calibrated coordinates, K check
+//   per chunk of GEO_CHUNK samples:
+//     hyp    one CTA per pair: folds the previous chunk's counts into the pair's best (packed (count + 1, ~(h*16 + r)),
+//            atomic max), decides the adaptive stop, then one thread per sample solves it: up to 4 fp32 projections
+//     score  (splits, B) CTAs: each streams a slice of the pair's points through shared memory against every solution
+//            of the chunk, one thread per sample, and adds the inlier counts
+//   refit    one CTA per pair: folds the last chunk, Levenberg-Marquardt from the best solution, recount, R and t
+//   mask     one thread per row of matches0: the final inlier mask
+// A stopped pair's CTAs return at once.  Compiled with -fmad=false, like geo_api.cu: oracle/pnp_oracle.py takes the same
+// steps in numpy.
+#include <stdint.h>
+
+#include "block_scan.cuh"
+#include "geo_common.cuh"
+#include "lg_internal.h"
+#include "ws_bump.h"
+
+namespace {
+
+constexpr int S = 3;                   // points per sample
+constexpr int SOLS = GEO_PNP_MAX_SOLUTIONS;
+constexpr int TILE = 512;              // points per shared-memory tile of the score kernel
+constexpr int MASK_THREADS = 256;
+
+struct PnpPair {
+  float P[12];               // the final K0 [R | t], fp32 (refit -> mask)
+  unsigned long long best;   // (count + 1) << 32 | ~(h * 16 + r) of the best solution so far; 0: none
+  float thr2;                // threshold^2
+  int n;                     // valid matches
+  int ok;                    // n >= 3 and K0 valid
+  int stop;                  // no further samples are drawn
+  int drawn;                 // samples drawn so far
+  int success;               // set by the refit kernel
+};
+
+struct PnpWs {
+  PnpPair* pair;   // [B]
+  float4* pts;     // [B, M] compacted (u, v, x, y): pixel and calibrated coordinates
+  float4* wld;     // [B, M] compacted world point (X, Y, Z, 0)
+  int* slot;       // [B, M] compacted slot of each row of matches0, -1 for an invalid match
+  float* hyp;      // [B, GEO_CHUNK, SOLS, 12] the current chunk's projections, fp32
+  int* nsol;       // [B, GEO_CHUNK] their number; 0: degenerate or not drawn
+  int* count;      // [B, GEO_CHUNK, SOLS] their inlier counts
+  uint8_t* inl;    // [B, M] the best solution's inliers, per compacted point (refit)
+};
+
+size_t carve(char* base, int B, int M, PnpWs* w) {
+  WsBump b{base, 0};
+  w->pair = b.take<PnpPair>(B);
+  w->pts = b.take<float4>((size_t)B * M);
+  w->wld = b.take<float4>((size_t)B * M);
+  w->slot = b.take<int>((size_t)B * M);
+  w->hyp = b.take<float>((size_t)B * GEO_CHUNK * SOLS * 12);
+  w->nsol = b.take<int>((size_t)B * GEO_CHUNK);
+  w->count = b.take<int>((size_t)B * GEO_CHUNK * SOLS);
+  w->inl = b.take<uint8_t>((size_t)B * M);
+  return b.bytes();
+}
+
+struct PnpArgs {
+  int B, M, N, max_iters, chunks;
+  unsigned seed;
+  double threshold, confidence;
+  const float* kpts0;
+  const float* points3d1;
+  const int64_t* matches0;
+  const double* K0;
+  PnpWs w;
+  GeoPnpOutputs out;
+};
+
+__device__ __forceinline__ double dot3(const double* a, const double* b) { return a[0] * b[0] + a[1] * b[1] + a[2] * b[2]; }
+
+__device__ __forceinline__ void cross3(const double* a, const double* b, double* c) {
+  c[0] = a[1] * b[2] - a[2] * b[1];
+  c[1] = a[2] * b[0] - a[0] * b[2];
+  c[2] = a[0] * b[1] - a[1] * b[0];
+}
+
+// Both roots of z^2 + b z + c, the larger-magnitude one first; a negative discriminant counts as 0 (header step A4)
+__device__ __forceinline__ void root2(double b, double c, double* r1, double* r2) {
+  const double y = sqrt(fmax(b * b - 4.0 * c, 0.0));
+  const double q = -0.5 * (b + (b >= 0.0 ? y : -y));
+  *r1 = q;
+  *r2 = c / q;
+}
+
+__device__ __forceinline__ double cubic(double g, double cb, double cc, double cd) { return ((g + cb) * g + cc) * g + cd; }
+
+// Lambda Twist P3P on the calibrated (x, y) in pts[id[k]].z/w and the world points wlds[id[k]] (header step A4).
+// Writes the kept solutions' R (row-major) and t in the solver's order; returns their number.
+__device__ __noinline__ int p3p(const float4* pts, const float4* wlds, const int* id, double (*Rs)[9], double (*ts)[3]) {
+  double y[3][3], X[3][3];
+  for (int k = 0; k < 3; ++k) {
+    const float4 p = pts[id[k]], q = wlds[id[k]];
+    const double xx = p.z, yy = p.w;
+    const double n = sqrt(xx * xx + yy * yy + 1.0);
+    y[k][0] = xx / n;
+    y[k][1] = yy / n;
+    y[k][2] = 1.0 / n;
+    X[k][0] = q.x;
+    X[k][1] = q.y;
+    X[k][2] = q.z;
+  }
+  const double b12 = -2.0 * dot3(y[0], y[1]), b13 = -2.0 * dot3(y[0], y[2]), b23 = -2.0 * dot3(y[1], y[2]);
+  double d12[3], d13[3], d23[3], nrm[3];
+  for (int i = 0; i < 3; ++i) {
+    d12[i] = X[0][i] - X[1][i];
+    d13[i] = X[0][i] - X[2][i];
+    d23[i] = X[1][i] - X[2][i];
+  }
+  const double a12 = dot3(d12, d12), a13 = dot3(d13, d13), a23 = dot3(d23, d23);
+  cross3(d12, d13, nrm);
+  if (!(dot3(nrm, nrm) > GEO_PNP_COLLINEAR_EPS * (a12 * a13))) return 0;
+  const double c31 = -0.5 * b13, c23 = -0.5 * b23, c12 = -0.5 * b12;
+  const double blob = c12 * c23 * c31 - 1.0;
+  const double s31 = 1.0 - c31 * c31, s23 = 1.0 - c23 * c23, s12 = 1.0 - c12 * c12;
+  const double p3 = a13 * (a23 * s31 - a13 * s23);
+  const double p2 = 2.0 * blob * a23 * a13 + a13 * (2.0 * a12 + a13) * s23 + a23 * (a23 - a12) * s31;
+  const double p1 = a23 * (a13 - a23) * s12 - a12 * a12 * s23 - 2.0 * a12 * (blob * a23 + a13 * s23);
+  const double p0 = a12 * (a12 * s23 - a23 * s12);
+  const double cb = p2 / p3, cc = p1 / p3, cd = p0 / p3;
+  if (!(isfinite(cb) && isfinite(cc) && isfinite(cd))) return 0;
+  // one real root of the monic cubic: bisection on a bracket holding exactly one root, then Newton
+  const double rb = 1.0 + fmax(fmax(fabs(cb), fabs(cc)), fabs(cd));
+  double lo = -rb, hi = rb;
+  const double disc = cb * cb - 3.0 * cc;
+  if (disc >= 0.0) {
+    const double v = sqrt(fmax(disc, 0.0));
+    const double t1 = (-cb - v) / 3.0;
+    if (cubic(t1, cb, cc, cd) > 0.0) hi = t1; else lo = (-cb + v) / 3.0;
+  }
+  for (int s = 0; s < GEO_PNP_BISECT_STEPS; ++s) {
+    const double mid = 0.5 * (lo + hi);
+    if (cubic(mid, cb, cc, cd) > 0.0) hi = mid; else lo = mid;
+  }
+  double g = 0.5 * (lo + hi);
+  for (int s = 0; s < GEO_PNP_NEWTON_STEPS; ++s) {
+    const double gn = g - cubic(g, cb, cc, cd) / ((3.0 * g + 2.0 * cb) * g + cc);
+    if (isfinite(gn)) g = gn;
+  }
+  // the degenerate conic A = D1 + g D2 and its two eigenvectors of nonzero eigenvalue
+  const double A00 = a23 * (1.0 - g);
+  const double A01 = a23 * b12 * 0.5;
+  const double A02 = a23 * b13 * g * -0.5;
+  const double A11 = a23 - a12 + a13 * g;
+  const double A12 = b23 * (a13 * g - a12) * 0.5;
+  const double A22 = g * (a13 - a23) - a12;
+  double e1, e2;
+  root2(-A00 - A11 - A22, -(A01 * A01) - A02 * A02 - A12 * A12 + A00 * (A11 + A22) + A11 * A22, &e1, &e2);
+  if (fabs(e1) < fabs(e2)) { const double tmp = e1; e1 = e2; e2 = tmp; }
+  const double mx = -(A00 * A11);
+  const double pr0 = A01 * A12 - A02 * A11;
+  const double pr1 = A01 * A02 - A00 * A12;
+  double V[2][3];
+  for (int k = 0; k < 2; ++k) {
+    const double e = k == 0 ? e1 : e2;
+    const double tmp = 1.0 / (e * (A00 + A11) + mx - e * e + A01 * A01);
+    const double a1 = -(e * A02 + pr0) * tmp;
+    const double a2 = -(e * A12 + pr1) * tmp;
+    const double rn = 1.0 / sqrt(a1 * a1 + a2 * a2 + 1.0);
+    V[k][0] = a1 * rn;
+    V[k][1] = a2 * rn;
+    V[k][2] = rn;
+  }
+  const double sv = sqrt(fmax(0.0, -e2 / e1));
+  // the inverse of X = [d12 d13 d12 x d13] by cofactors
+  const double x[3][3] = {{d12[0], d13[0], nrm[0]}, {d12[1], d13[1], nrm[1]}, {d12[2], d13[2], nrm[2]}};
+  const double C[3][3] = {
+      {x[1][1] * x[2][2] - x[1][2] * x[2][1], x[1][2] * x[2][0] - x[1][0] * x[2][2], x[1][0] * x[2][1] - x[1][1] * x[2][0]},
+      {x[0][2] * x[2][1] - x[0][1] * x[2][2], x[0][0] * x[2][2] - x[0][2] * x[2][0], x[0][1] * x[2][0] - x[0][0] * x[2][1]},
+      {x[0][1] * x[1][2] - x[0][2] * x[1][1], x[0][2] * x[1][0] - x[0][0] * x[1][2], x[0][0] * x[1][1] - x[0][1] * x[1][0]}};
+  const double det = x[0][0] * C[0][0] + x[0][1] * C[0][1] + x[0][2] * C[0][2];
+  double Xi[3][3];
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 3; ++j) Xi[i][j] = C[j][i] / det;
+  int ns = 0;
+  for (int sg = 0; sg < 2; ++sg) {
+    const double s = sg == 0 ? sv : -sv;
+    const double w2 = 1.0 / (s * V[1][0] - V[0][0]);
+    const double w0 = (V[0][1] - s * V[1][1]) * w2;
+    const double w1 = (V[0][2] - s * V[1][2]) * w2;
+    const double ia = 1.0 / ((a13 - a12) * w1 * w1 - a12 * b13 * w1 - a12);
+    const double qb = (a13 * b12 * w1 - a12 * b13 * w0 - 2.0 * w0 * w1 * (a12 - a13)) * ia;
+    const double qc = ((a13 - a12) * w0 * w0 + a13 * b12 * w0 + a13) * ia;
+    if (!(qb * qb - 4.0 * qc >= 0.0)) continue;
+    double taus[2];
+    root2(qb, qc, &taus[0], &taus[1]);
+    for (int k = 0; k < 2; ++k) {
+      const double tau = taus[k];
+      if (!(tau > 0.0)) continue;
+      const double d = a23 / (tau * (b23 + tau) + 1.0);
+      if (!(d > 0.0)) continue;
+      double l2 = sqrt(d);
+      double l3 = tau * l2;
+      double l1 = w0 * l2 + w1 * l3;
+      if (!(l1 >= 0.0)) continue;
+      for (int it = 0; it < GEO_PNP_GN_STEPS; ++it) {
+        const double r1 = l1 * l1 + l2 * l2 + b12 * l1 * l2 - a12;
+        const double r2 = l1 * l1 + l3 * l3 + b13 * l1 * l3 - a13;
+        const double r3 = l2 * l2 + l3 * l3 + b23 * l2 * l3 - a23;
+        const double v0 = 2.0 * l1 + b12 * l2, v1 = 2.0 * l2 + b12 * l1;
+        const double v3 = 2.0 * l1 + b13 * l3, v5 = 2.0 * l3 + b13 * l1;
+        const double v7 = 2.0 * l2 + b23 * l3, v8 = 2.0 * l3 + b23 * l2;
+        const double dt = -(v0 * v5 * v7) - v1 * v3 * v8;
+        const double j0 = -(v5 * v7) * r1 - v1 * v8 * r2 + v1 * v5 * r3;
+        const double j1 = -(v3 * v8) * r1 + v0 * v8 * r2 - v0 * v5 * r3;
+        const double j2 = v3 * v7 * r1 - v0 * v7 * r2 - v1 * v3 * r3;
+        const double n1 = l1 - j0 / dt, n2 = l2 - j1 / dt, n3 = l3 - j2 / dt;
+        if (isfinite(n1) && isfinite(n2) && isfinite(n3)) { l1 = n1; l2 = n2; l3 = n3; }
+      }
+      const double lam[3] = {l1, l2, l3};
+      double ry[3][3];
+      for (int q = 0; q < 3; ++q)
+        for (int i = 0; i < 3; ++i) ry[q][i] = y[q][i] * lam[q];
+      double yd1[3], yd2[3], yc[3];
+      for (int i = 0; i < 3; ++i) {
+        yd1[i] = ry[0][i] - ry[1][i];
+        yd2[i] = ry[0][i] - ry[2][i];
+      }
+      cross3(yd1, yd2, yc);
+      double* R = Rs[ns];
+      double* t = ts[ns];
+      bool fin = true;
+      for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) {
+          R[i * 3 + j] = yd1[i] * Xi[0][j] + yd2[i] * Xi[1][j] + yc[i] * Xi[2][j];
+          fin = fin && isfinite(R[i * 3 + j]);
+        }
+      for (int i = 0; i < 3; ++i) {
+        t[i] = ry[0][i] - (R[i * 3] * X[0][0] + R[i * 3 + 1] * X[0][1] + R[i * 3 + 2] * X[0][2]);
+        fin = fin && isfinite(t[i]);
+      }
+      if (fin) ++ns;
+    }
+  }
+  return ns;
+}
+
+// P = K [R | t] (header step A5), P_ij = (K_i0*M_0j + K_i1*M_1j) + K_i2*M_2j
+__device__ __forceinline__ void projection(const double* K, const double* R, const double* t, double* P) {
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 4; ++j) {
+      const double m0 = j < 3 ? R[j] : t[0], m1 = j < 3 ? R[3 + j] : t[1], m2 = j < 3 ? R[6 + j] : t[2];
+      P[i * 4 + j] = K[3 * i] * m0 + K[3 * i + 1] * m1 + K[3 * i + 2] * m2;
+    }
+}
+
+// fp32 inlier test of one point (header step A5): depth w > 0 and squared reprojection error below thr2
+__device__ __forceinline__ bool reproj_inlier(const float* g, float4 p, float4 q, float thr2) {
+  const float w = g[8] * q.x + g[9] * q.y + g[10] * q.z + g[11];
+  const float iw = 1.f / w;
+  const float du = p.x - (g[0] * q.x + g[1] * q.y + g[2] * q.z + g[3]) * iw;
+  const float dv = p.y - (g[4] * q.x + g[5] * q.y + g[6] * q.z + g[7]) * iw;
+  return w > 0.f && du * du + dv * dv < thr2;
+}
+
+__device__ bool k_valid(const double* K) {
+  bool finite = true;
+  for (int i = 0; i < 9; ++i) finite = finite && isfinite(K[i]);
+  return finite && K[0] > 0.0 && K[4] > 0.0 && K[6] == 0.0 && K[7] == 0.0 && K[8] == 1.0;
+}
+
+// Folds chunk c's counts into the pair's best and decides whether the pair stops.  Called by every thread of a
+// GEO_CHUNK-thread CTA; thread t owns sample c * GEO_CHUNK + t.
+__device__ void pnp_fold(const PnpArgs& a, int b, int c) {
+  __shared__ unsigned long long best;
+  PnpPair* P = a.w.pair + b;
+  const int t = threadIdx.x;
+  const bool live = P->stop == 0;
+  if (t == 0) best = P->best;
+  __syncthreads();
+  const int ns = a.w.nsol[(long)b * GEO_CHUNK + t];
+  const unsigned h = c * GEO_CHUNK + t;
+  for (int r = 0; live && r < ns; ++r) {
+    const int k = a.w.count[((long)b * GEO_CHUNK + t) * SOLS + r];
+    atomicMax(&best, ((unsigned long long)(k + 1) << 32) | (unsigned)~(h * 16u + (unsigned)r));
+  }
+  __syncthreads();
+  if (t == 0 && live) {
+    const int drawn = min((c + 1) * GEO_CHUNK, a.max_iters);
+    const int cnt = best ? (int)(best >> 32) - 1 : 0;
+    P->best = best;
+    P->drawn = drawn;
+    P->stop = drawn >= a.max_iters || drawn >= update_num_iters(a.confidence, 1.0 - (double)cnt / P->n, S, a.max_iters);
+  }
+  __syncthreads();
+}
+
+__global__ void __launch_bounds__(1024) pnp_prepare_kernel(PnpArgs a) {
+  const int b = blockIdx.x, tid = threadIdx.x;
+  __shared__ int warp_sums[32];
+  __shared__ int carry;
+  if (tid == 0) carry = 0;
+  __syncthreads();
+  const double* K = a.K0 + (long)b * 9;
+  const int64_t* m0 = a.matches0 + (long)b * a.M;
+  float4* pts = a.w.pts + (long)b * a.M;
+  float4* wld = a.w.wld + (long)b * a.M;
+  int* slot = a.w.slot + (long)b * a.M;
+  for (int base = 0; base < a.M; base += 1024) {
+    const int i = base + tid;
+    const int64_t j = i < a.M ? m0[i] : -1;
+    float X = 0.f, Y = 0.f, Z = 0.f;
+    if (j >= 0 && j < a.N) {
+      const float* q = a.points3d1 + ((long)b * a.N + j) * 3;
+      X = q[0];
+      Y = q[1];
+      Z = q[2];
+    }
+    const bool valid = j >= 0 && j < a.N && isfinite(X) && isfinite(Y) && isfinite(Z);
+    const int k = block_scan_step(valid, tid, warp_sums, &carry);
+    if (i < a.M) slot[i] = valid ? k : -1;
+    if (valid) {
+      const float2 p = reinterpret_cast<const float2*>(a.kpts0)[(long)b * a.M + i];
+      const double yy = ((double)p.y - K[5]) / K[4], xx = (((double)p.x - K[2]) - K[1] * yy) / K[0];
+      pts[k] = make_float4(p.x, p.y, (float)xx, (float)yy);
+      wld[k] = make_float4(X, Y, Z, 0.f);
+    }
+  }
+  __syncthreads();
+  if (tid == 0) {
+    PnpPair& P = a.w.pair[b];
+    P.thr2 = (float)(a.threshold * a.threshold);
+    P.best = 0;
+    P.n = carry;
+    P.ok = carry >= S && k_valid(K);
+    P.stop = !P.ok;
+    P.drawn = 0;
+    P.success = 0;
+  }
+}
+
+__global__ void __launch_bounds__(GEO_CHUNK, 1) pnp_hyp_kernel(PnpArgs a, int c) {
+  const int b = blockIdx.x, t = threadIdx.x;
+  if (c > 0) pnp_fold(a, b, c - 1);
+  const PnpPair& P = a.w.pair[b];
+  const int h = c * GEO_CHUNK + t;
+  int ns = 0;
+  int id[S];
+  if (P.stop == 0 && h < a.max_iters && geo_sample(a.seed, h, P.n, S, id) == S) {
+    double Rs[SOLS][9], ts[SOLS][3];
+    ns = p3p(a.w.pts + (long)b * a.M, a.w.wld + (long)b * a.M, id, Rs, ts);
+    const double* K = a.K0 + (long)b * 9;
+    float* hm = a.w.hyp + ((long)b * GEO_CHUNK + t) * SOLS * 12;
+    for (int r = 0; r < ns; ++r) {
+      double Pm[12];
+      projection(K, Rs[r], ts[r], Pm);
+      for (int i = 0; i < 12; ++i) hm[r * 12 + i] = (float)Pm[i];
+      a.w.count[((long)b * GEO_CHUNK + t) * SOLS + r] = 0;
+    }
+  }
+  a.w.nsol[(long)b * GEO_CHUNK + t] = ns;
+}
+
+__global__ void __launch_bounds__(GEO_CHUNK) pnp_score_kernel(PnpArgs a) {
+  const int b = blockIdx.y, split = blockIdx.x, t = threadIdx.x;
+  const PnpPair& P = a.w.pair[b];
+  if (P.stop) return;
+  const int lo = (int)((long)P.n * split / gridDim.x), hi = (int)((long)P.n * (split + 1) / gridDim.x);
+  const int ns = a.w.nsol[(long)b * GEO_CHUNK + t];
+  const float* hm = a.w.hyp + ((long)b * GEO_CHUNK + t) * SOLS * 12;
+  const float thr2 = P.thr2;
+  float g[SOLS][12];
+  int k[SOLS];
+#pragma unroll
+  for (int r = 0; r < SOLS; ++r) {
+    k[r] = 0;
+#pragma unroll
+    for (int i = 0; i < 12; ++i) g[r][i] = r < ns ? hm[r * 12 + i] : 0.f;
+  }
+  const float4* pts = a.w.pts + (long)b * a.M;
+  const float4* wld = a.w.wld + (long)b * a.M;
+  __shared__ float4 tp[TILE], tw[TILE];
+  for (int base = lo; base < hi; base += TILE) {
+    const int m = min(TILE, hi - base);
+    __syncthreads();
+    for (int i = t; i < m; i += GEO_CHUNK) {
+      tp[i] = pts[base + i];
+      tw[i] = wld[base + i];
+    }
+    __syncthreads();
+    for (int i = 0; i < m; ++i) {
+      const float4 p = tp[i], q = tw[i];
+#pragma unroll
+      for (int r = 0; r < SOLS; ++r)
+        if (r < ns) k[r] += reproj_inlier(g[r], p, q, thr2);
+    }
+  }
+#pragma unroll
+  for (int r = 0; r < SOLS; ++r)
+    if (r < ns && k[r]) atomicAdd(a.w.count + ((long)b * GEO_CHUNK + t) * SOLS + r, k[r]);
+}
+
+constexpr int LM_TERMS = 28;  // J^T J upper triangle (21), J^T r (6), cost
+
+// This thread's partial sums of the refit's terms at (R, t) over the inliers k = t, t + RED, ... (header step A7)
+__device__ void lm_partials(const double* K, const double* R, const double* t, const float4* pts, const float4* wld,
+                            const uint8_t* inl, int n, int tid, double* acc) {
+  const double fx = K[0], s = K[1], cx = K[2], fy = K[4], cy = K[5];
+  for (int i = 0; i < LM_TERMS; ++i) acc[i] = 0.0;
+  for (int k = tid; k < n; k += RED) {
+    if (!inl[k]) continue;
+    const float4 p = pts[k], q = wld[k];
+    const double u = p.x, v = p.y, W[3] = {q.x, q.y, q.z};
+    double Xc[3];
+    for (int i = 0; i < 3; ++i) Xc[i] = R[3 * i] * W[0] + R[3 * i + 1] * W[1] + R[3 * i + 2] * W[2] + t[i];
+    const double iz = 1.0 / Xc[2];
+    const double ax = Xc[0] * iz, bx = Xc[1] * iz;
+    const double pu = fx * ax + s * bx;
+    const double ru = pu + cx - u, rv = fy * bx + cy - v;
+    const double gu[3] = {fx * iz, s * iz, -(pu * iz)};
+    const double gv[3] = {0.0, fy * iz, -(fy * bx * iz)};
+    const double ju[6] = {gu[2] * Xc[1] - gu[1] * Xc[2], gu[0] * Xc[2] - gu[2] * Xc[0], gu[1] * Xc[0] - gu[0] * Xc[1],
+                          gu[0], gu[1], gu[2]};
+    const double jv[6] = {gv[2] * Xc[1] - gv[1] * Xc[2], gv[0] * Xc[2] - gv[2] * Xc[0], gv[1] * Xc[0] - gv[0] * Xc[1],
+                          gv[0], gv[1], gv[2]};
+    int e = 0;
+#pragma unroll
+    for (int i = 0; i < 6; ++i)
+#pragma unroll
+      for (int j = i; j < 6; ++j, ++e) acc[e] = acc[e] + (ju[i] * ju[j] + jv[i] * jv[j]);
+#pragma unroll
+    for (int i = 0; i < 6; ++i) acc[21 + i] = acc[21 + i] + (ju[i] * ru + jv[i] * rv);
+    acc[27] = acc[27] + (ru * ru + rv * rv);
+  }
+}
+
+// delta of (J^T J, its diagonal times (1 + lam)) delta = -J^T r by Cholesky; false on a pivot <= 0 or a non-finite delta
+__device__ bool lm_solve(const double* Hu, const double* g, double lam, double* x) {
+  double A[6][6], L[6][6], yv[6];
+  for (int i = 0, e = 0; i < 6; ++i)
+    for (int j = i; j < 6; ++j, ++e) A[i][j] = A[j][i] = Hu[e];
+  for (int i = 0; i < 6; ++i) A[i][i] = A[i][i] * (1.0 + lam);
+  for (int j = 0; j < 6; ++j) {
+    double d = A[j][j];
+    for (int k = 0; k < j; ++k) d = d - L[j][k] * L[j][k];
+    if (!(d > 0.0)) return false;
+    L[j][j] = sqrt(d);
+    for (int i = j + 1; i < 6; ++i) {
+      double e = A[i][j];
+      for (int k = 0; k < j; ++k) e = e - L[i][k] * L[j][k];
+      L[i][j] = e / L[j][j];
+    }
+  }
+  for (int i = 0; i < 6; ++i) {
+    double e = -g[i];
+    for (int k = 0; k < i; ++k) e = e - L[i][k] * yv[k];
+    yv[i] = e / L[i][i];
+  }
+  bool fin = true;
+  for (int i = 5; i >= 0; --i) {
+    double e = yv[i];
+    for (int k = i + 1; k < 6; ++k) e = e - L[k][i] * x[k];
+    x[i] = e / L[i][i];
+    fin = fin && isfinite(x[i]);
+  }
+  return fin;
+}
+
+// R' = Q R, t' = Q t + d[3..5], Q of the unit quaternion (1, d[0..2] / 2) / norm
+__device__ void lm_update(const double* R, const double* t, const double* d, double* Rn, double* tn) {
+  double qw = 1.0, qx = d[0] * 0.5, qy = d[1] * 0.5, qz = d[2] * 0.5;
+  const double n = sqrt(qw * qw + qx * qx + qy * qy + qz * qz);
+  qw = qw / n;
+  qx = qx / n;
+  qy = qy / n;
+  qz = qz / n;
+  const double Q[9] = {1.0 - 2.0 * (qy * qy + qz * qz), 2.0 * (qx * qy - qw * qz), 2.0 * (qx * qz + qw * qy),
+                       2.0 * (qx * qy + qw * qz), 1.0 - 2.0 * (qx * qx + qz * qz), 2.0 * (qy * qz - qw * qx),
+                       2.0 * (qx * qz - qw * qy), 2.0 * (qy * qz + qw * qx), 1.0 - 2.0 * (qx * qx + qy * qy)};
+  for (int i = 0; i < 3; ++i) {
+    for (int j = 0; j < 3; ++j) Rn[3 * i + j] = Q[3 * i] * R[j] + Q[3 * i + 1] * R[3 + j] + Q[3 * i + 2] * R[6 + j];
+    tn[i] = Q[3 * i] * t[0] + Q[3 * i + 1] * t[1] + Q[3 * i + 2] * t[2] + d[3 + i];
+  }
+}
+
+__global__ void __launch_bounds__(RED, 1) pnp_refit_kernel(PnpArgs a) {
+  const int b = blockIdx.x, t = threadIdx.x;
+  pnp_fold(a, b, a.chunks - 1);
+  PnpPair& P = a.w.pair[b];
+  const float4* pts = a.w.pts + (long)b * a.M;
+  const float4* wld = a.w.wld + (long)b * a.M;
+  const double* K = a.K0 + (long)b * 9;
+  __shared__ double red[RED];
+  __shared__ double pose[2][12];  // R, t of the best solution and of the refit
+  __shared__ double cand[12];     // the LM step's candidate
+  __shared__ double sums[LM_TERMS], csum[LM_TERMS];
+  __shared__ float fm[2][12];
+  __shared__ int count[2];
+  __shared__ int step_ok;
+  const unsigned long long key = P.best;
+  if (!P.ok || key == 0) {
+    if (t < 9) a.out.R[(long)b * 9 + t] = 0.0;
+    if (t < 3) a.out.t[(long)b * 3 + t] = 0.0;
+    if (t == 0) {
+      a.out.num_inliers[b] = 0;
+      a.out.success[b] = 0;
+      a.out.best_hypothesis[b] = a.out.best_solution[b] = -1;
+      a.out.num_hypotheses[b] = P.drawn;
+    }
+    return;
+  }
+  const unsigned hr = ~(unsigned)(key & 0xffffffffu);
+  const int hcount = (int)(key >> 32) - 1;
+  const float thr2 = P.thr2;
+  if (t == 0) {
+    int id[S];
+    double Rs[SOLS][9], ts[SOLS][3], Pm[12];
+    geo_sample(a.seed, hr >> 4, P.n, S, id);
+    p3p(pts, wld, id, Rs, ts);
+    for (int i = 0; i < 9; ++i) pose[0][i] = pose[1][i] = Rs[hr & 15][i];
+    for (int i = 0; i < 3; ++i) pose[0][9 + i] = pose[1][9 + i] = ts[hr & 15][i];
+    projection(K, pose[0], pose[0] + 9, Pm);
+    for (int i = 0; i < 12; ++i) fm[0][i] = (float)Pm[i];
+    count[0] = hcount;
+    count[1] = -1;
+  }
+  __syncthreads();
+  if (hcount >= GEO_PNP_REFIT_MIN) {
+    uint8_t* inl = a.w.inl + (long)b * a.M;
+    for (int k = t; k < P.n; k += RED) inl[k] = reproj_inlier(fm[0], pts[k], wld[k], thr2);
+    __syncthreads();
+    double acc[LM_TERMS];
+    lm_partials(K, pose[1], pose[1] + 9, pts, wld, inl, P.n, t, acc);
+    for (int i = 0; i < LM_TERMS; ++i) {
+      const double s = tree_sum(acc[i], red, t);
+      if (t == 0) sums[i] = s;
+    }
+    double lam = GEO_PNP_LM_LAMBDA0;  // every thread keeps the same schedule
+    for (int it = 0; it < GEO_PNP_LM_STEPS; ++it) {
+      if (t == 0) {
+        double d[6];
+        step_ok = lm_solve(sums, sums + 21, lam, d);
+        if (step_ok) lm_update(pose[1], pose[1] + 9, d, cand, cand + 9);
+      }
+      __syncthreads();
+      if (!step_ok) {
+        lam = lam * 10.0;
+        __syncthreads();
+        continue;
+      }
+      lm_partials(K, cand, cand + 9, pts, wld, inl, P.n, t, acc);
+      for (int i = 0; i < LM_TERMS; ++i) {
+        const double s = tree_sum(acc[i], red, t);
+        if (t == 0) csum[i] = s;
+      }
+      __syncthreads();
+      const bool better = csum[27] < sums[27];
+      __syncthreads();
+      if (better) {
+        if (t < 12) pose[1][t] = cand[t];
+        if (t < LM_TERMS) sums[t] = csum[t];
+        lam = lam / 10.0;
+      } else {
+        lam = lam * 10.0;
+      }
+      __syncthreads();
+    }
+    if (t == 0) {
+      double Pm[12];
+      projection(K, pose[1], pose[1] + 9, Pm);
+      for (int i = 0; i < 12; ++i) fm[1][i] = (float)Pm[i];
+      count[1] = 0;
+    }
+    __syncthreads();
+    int k1 = 0;
+    for (int k = t; k < P.n; k += RED) k1 += reproj_inlier(fm[1], pts[k], wld[k], thr2);
+    if (k1) atomicAdd(&count[1], k1);
+    __syncthreads();
+  }
+  const int u = count[1] >= count[0] ? 1 : 0;
+  if (t < 12) P.P[t] = fm[u][t];
+  if (t < 9) a.out.R[(long)b * 9 + t] = pose[u][t];
+  if (t < 3) a.out.t[(long)b * 3 + t] = pose[u][9 + t];
+  if (t == 0) {
+    a.out.num_inliers[b] = count[u];
+    a.out.success[b] = 1;
+    a.out.best_hypothesis[b] = (int)(hr >> 4);
+    a.out.best_solution[b] = (int)(hr & 15);
+    a.out.num_hypotheses[b] = P.drawn;
+    P.success = 1;
+  }
+}
+
+__global__ void __launch_bounds__(MASK_THREADS) pnp_mask_kernel(PnpArgs a) {
+  const int b = blockIdx.y, i = blockIdx.x * MASK_THREADS + threadIdx.x;
+  if (i >= a.M) return;
+  const PnpPair& P = a.w.pair[b];
+  const int k = a.w.slot[(long)b * a.M + i];
+  bool in = false;
+  if (P.success && k >= 0) in = reproj_inlier(P.P, a.w.pts[(long)b * a.M + k], a.w.wld[(long)b * a.M + k], P.thr2);
+  a.out.inliers[(long)b * a.M + i] = in;
+}
+
+}  // namespace
+
+extern "C" size_t geo_pnp_workspace_bytes(int32_t B, int32_t M, int32_t) {
+  if (B < 0 || M < 0) return 0;
+  PnpWs w;
+  return carve(nullptr, B, M, &w) + 256;
+}
+
+extern "C" int geo_absolute_pose(const GeoPnpConfig* cfg, const GeoPnpInputs* in, GeoPnpOutputs* out, void* workspace,
+                                 size_t workspace_bytes, void* stream_) {
+  if (!cfg || !in || !out) return lg_set_error("geo_absolute_pose: null argument");
+  if (cfg->abi_version != GEO_ABI_VERSION) return lg_set_error("geo_absolute_pose: ABI version mismatch");
+  if (cfg->max_iters < 1 || cfg->max_iters > GEO_MAX_ITERS)
+    return lg_set_error("geo_absolute_pose: max_iters outside [1, 2^24]");
+  if (!(cfg->threshold > 0.0) || !isfinite(cfg->threshold))
+    return lg_set_error("geo_absolute_pose: threshold must be positive");
+  if (!(cfg->confidence >= 0.0 && cfg->confidence <= 1.0))
+    return lg_set_error("geo_absolute_pose: confidence outside [0, 1]");
+  if (in->B < 0 || in->M < 0 || in->N < 0) return lg_set_error("geo_absolute_pose: negative size");
+  if (in->B == 0) return 0;
+  if (!out->R || !out->t || !out->inliers || !out->num_inliers || !out->success || !out->best_hypothesis ||
+      !out->best_solution || !out->num_hypotheses)
+    return lg_set_error("geo_absolute_pose: null output");
+  if (!in->K0) return lg_set_error("geo_absolute_pose: null intrinsics");
+  if (in->M > 0 && (!in->kpts0 || !in->matches0 || (in->N > 0 && !in->points3d1)))
+    return lg_set_error("geo_absolute_pose: null input");
+  if (!workspace || workspace_bytes < geo_pnp_workspace_bytes(in->B, in->M, cfg->max_iters))
+    return lg_set_error("geo_absolute_pose: workspace too small");
+  PnpArgs a{};
+  carve((char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255), in->B, in->M, &a.w);
+  a.B = in->B; a.M = in->M; a.N = in->N;
+  a.max_iters = cfg->max_iters;
+  a.chunks = (cfg->max_iters + GEO_CHUNK - 1) / GEO_CHUNK;
+  a.seed = cfg->seed;
+  a.threshold = cfg->threshold;
+  a.confidence = cfg->confidence;
+  a.kpts0 = in->kpts0; a.points3d1 = in->points3d1; a.matches0 = in->matches0;
+  a.K0 = in->K0;
+  a.out = *out;
+  // enough score CTAs to cover the SMs twice, with at least 128 points per slice
+  const int want = (2 * lg_num_sms() + a.B - 1) / a.B;
+  int splits = (a.M + 127) / 128;
+  if (splits > want) splits = want;
+  if (splits < 1) splits = 1;
+  const cudaStream_t stream = (cudaStream_t)stream_;
+  pnp_prepare_kernel<<<a.B, 1024, 0, stream>>>(a);
+  LG_CHECK_LAUNCH();
+  for (int c = 0; c < a.chunks; ++c) {
+    pnp_hyp_kernel<<<a.B, GEO_CHUNK, 0, stream>>>(a, c);
+    LG_CHECK_LAUNCH();
+    pnp_score_kernel<<<dim3(splits, a.B), GEO_CHUNK, 0, stream>>>(a);
+    LG_CHECK_LAUNCH();
+  }
+  pnp_refit_kernel<<<a.B, RED, 0, stream>>>(a);
+  LG_CHECK_LAUNCH();
+  if (a.M > 0) {
+    pnp_mask_kernel<<<dim3((a.M + MASK_THREADS - 1) / MASK_THREADS, a.B), MASK_THREADS, 0, stream>>>(a);
+    LG_CHECK_LAUNCH();
+  }
+  return 0;
+}

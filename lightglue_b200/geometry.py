@@ -1,12 +1,13 @@
-"""Geometric verification on the GPU: batched RANSAC homography, fundamental-matrix and relative-pose estimation on the
-matcher's output (C ABI ``include/geometry_b200.h``, CUDA ``csrc/geo_api.cu`` and ``csrc/pose_api.cu``).
+"""Geometric verification on the GPU: batched RANSAC homography, fundamental-matrix, relative-pose and absolute-pose
+estimation on the matcher's output (C ABI ``include/geometry_b200.h``, CUDA ``csrc/geo_api.cu``, ``csrc/pose_api.cu``
+and ``csrc/pnp_api.cu``).
 
-All three functions take ``matches0`` [B, M] int64 exactly as ``LightGlue.forward``, ``PendingMatch.tensors`` and
+All four functions take ``matches0`` [B, M] int64 exactly as ``LightGlue.forward``, ``PendingMatch.tensors`` and
 ``match_ragged`` give it (-1 or any index outside [0, N) is unmatched), run every pair of the batch in one call on the
 current stream, and return device tensors of fixed shapes without synchronising with the host, so a call can follow a
 matcher forward with no read-back in between, or be captured in a CUDA graph.  Parameter names and defaults are those of
-``cv2.findHomography(RANSAC)``, ``cv2.findFundamentalMat(FM_RANSAC)`` and ``cv2.findEssentialMat(RANSAC)`` with
-``cv2.recoverPose``.
+``cv2.findHomography(RANSAC)``, ``cv2.findFundamentalMat(FM_RANSAC)``, ``cv2.findEssentialMat(RANSAC)`` with
+``cv2.recoverPose``, and ``cv2.solvePnPRansac``.
 
 ``find_homography`` and ``find_fundamental`` return a dict: ``H`` or ``F`` [B, 3, 3] float64 (H scaled to H[2, 2] = 1; F to unit Frobenius norm with its largest
 entry positive), ``inliers`` [B, M] bool, ``num_inliers`` [B] int32, ``success`` [B] bool, and the diagnostics
@@ -33,23 +34,24 @@ def _check_params(threshold, max_iters, confidence, seed) -> None:
         raise ValueError(f"seed={seed!r}: an int in [0, 2**32)")
 
 
-def _check_inputs(kpts0, kpts1, matches0) -> None:
-    for name, t in (("kpts0", kpts0), ("kpts1", kpts1), ("matches0", matches0)):
+def _check_inputs(kpts0, kpts1, matches0, name1="kpts1", dim1=2) -> None:
+    for name, t in (("kpts0", kpts0), (name1, kpts1), ("matches0", matches0)):
         if not isinstance(t, torch.Tensor):
             raise ValueError(f"{name} must be a torch.Tensor")
         if t.device.type != "cuda":
             raise RuntimeError("lightglue_b200.geometry runs on CUDA (sm_90a) tensors only; there is no CPU path")
-    if kpts0.dim() != 3 or kpts0.shape[-1] != 2 or kpts1.dim() != 3 or kpts1.shape[-1] != 2:
-        raise ValueError(f"kpts0 {tuple(kpts0.shape)} and kpts1 {tuple(kpts1.shape)}: expected [B, M, 2] and [B, N, 2]")
+    if kpts0.dim() != 3 or kpts0.shape[-1] != 2 or kpts1.dim() != 3 or kpts1.shape[-1] != dim1:
+        raise ValueError(f"kpts0 {tuple(kpts0.shape)} and {name1} {tuple(kpts1.shape)}: expected [B, M, 2] and "
+                         f"[B, N, {dim1}]")
     if matches0.dim() != 2 or matches0.shape != kpts0.shape[:2] or kpts1.shape[0] != kpts0.shape[0]:
         raise ValueError(f"matches0 {tuple(matches0.shape)}: expected [B, M] of kpts0 {tuple(kpts0.shape)} with the "
-                         f"batch of kpts1 {tuple(kpts1.shape)}")
+                         f"batch of {name1} {tuple(kpts1.shape)}")
     if not kpts0.is_floating_point() or not kpts1.is_floating_point():
-        raise ValueError("kpts0 and kpts1 must be floating point pixels")
+        raise ValueError(f"kpts0 and {name1} must be floating point" + (" pixels" if dim1 == 2 else ""))
     if matches0.dtype != torch.int64:
         raise ValueError(f"matches0 must be int64, not {matches0.dtype}")
     if kpts1.device != kpts0.device or matches0.device != kpts0.device:
-        raise ValueError("kpts0, kpts1 and matches0 must be on one device")
+        raise ValueError(f"kpts0, {name1} and matches0 must be on one device")
 
 
 def _estimate(kind: int, key: str, kpts0, kpts1, matches0, threshold, max_iters, confidence, seed) -> dict:
@@ -161,4 +163,48 @@ def estimate_relative_pose(kpts0: torch.Tensor, kpts1: torch.Tensor, matches0: t
         stream = torch.cuda.current_stream(device).cuda_stream
         _cabi.check(lib.geo_relative_pose(C.byref(cfg), C.byref(ins), C.byref(outs), ws.data_ptr(), ws.numel(), stream),
                     "geo_relative_pose")
+    return out
+
+
+def estimate_absolute_pose(kpts0: torch.Tensor, points3d1: torch.Tensor, matches0: torch.Tensor, K0: torch.Tensor,
+                           ransac_reproj_threshold: float = 8.0, max_iters: int = 100, confidence: float = 0.99,
+                           seed: int = 0) -> dict:
+    """Absolute pose per pair from 2D-3D matches: Lambda Twist P3P RANSAC on the query pixels ``kpts0`` [B, M, 2] and
+    the world points ``points3d1`` [B, N, 3] of image 1's keypoints (a row with a non-finite coordinate has no 3D point,
+    so its matches are invalid), then Levenberg-Marquardt on the inliers.  An inlier lies in front of the camera with a
+    squared reprojection error through ``K0`` ([3, 3] or [B, 3, 3], no distortion) below
+    ``ransac_reproj_threshold ** 2``.  Defaults of ``cv2.solvePnPRansac``.
+
+    Returns ``R`` [B, 3, 3] and ``t`` [B, 3] float64 with x_cam = R X + t (OpenCV's rvec/tvec convention);
+    ``inliers`` [B, M] bool and ``num_inliers`` [B] int32 of the final pose; ``success`` [B] bool; and the
+    diagnostics ``best_hypothesis``, ``best_solution`` and ``num_hypotheses`` [B] int32.  A pair with fewer than 3
+    valid matches, an invalid K0 (a non-finite entry, fx or fy <= 0, or a bottom row other than [0, 0, 1]) or no
+    non-degenerate sample has ``success`` False, zero R and t, no inliers and -1 for ``best_hypothesis`` and
+    ``best_solution``."""
+    _check_inputs(kpts0, points3d1, matches0, "points3d1", 3)
+    _check_params(ransac_reproj_threshold, max_iters, confidence, seed)
+    device = kpts0.device
+    b, m, n = kpts0.shape[0], kpts0.shape[1], points3d1.shape[1]
+    k0 = _intrinsics("K0", K0, b, device)
+    p0 = kpts0.detach().to(torch.float32).contiguous()
+    x1 = points3d1.detach().to(torch.float32).contiguous()
+    m0 = matches0.detach().contiguous()
+    keys = ("R", "t", "inliers", "num_inliers", "success", "best_hypothesis", "best_solution", "num_hypotheses")
+    f64, i32, bl = torch.float64, torch.int32, torch.bool
+    shapes = {"R": ((b, 3, 3), f64), "t": ((b, 3), f64), "inliers": ((b, m), bl), "num_inliers": ((b,), i32),
+              "success": ((b,), bl), "best_hypothesis": ((b,), i32), "best_solution": ((b,), i32),
+              "num_hypotheses": ((b,), i32)}
+    out = {k: torch.empty(*shapes[k][0], dtype=shapes[k][1], device=device) for k in keys}
+    if b == 0:
+        return out
+    with torch.cuda.device(device):
+        lib = _cabi.load()
+        ws = torch.empty(lib.geo_pnp_workspace_bytes(b, m, max_iters), dtype=torch.uint8, device=device)
+        cfg = _cabi.GeoPnpConfig(_cabi.GEO_ABI_VERSION, max_iters, seed, 0, float(ransac_reproj_threshold),
+                                 float(confidence))
+        ins = _cabi.GeoPnpInputs(b, m, n, p0.data_ptr(), x1.data_ptr(), m0.data_ptr(), k0.data_ptr())
+        outs = _cabi.GeoPnpOutputs(*(out[k].data_ptr() for k in keys))
+        stream = torch.cuda.current_stream(device).cuda_stream
+        _cabi.check(lib.geo_absolute_pose(C.byref(cfg), C.byref(ins), C.byref(outs), ws.data_ptr(), ws.numel(), stream),
+                    "geo_absolute_pose")
     return out
