@@ -1,0 +1,100 @@
+/* nn_b200 -- C ABI of the nearest-neighbour matcher: mutual nearest neighbours with Lowe's ratio test and a distance
+ * threshold on unit-norm descriptors, for every pair of a batch in one call, on the tensor cores in split-bf16.  Same
+ * library (liblightglue_b200.so) and conventions as lightglue_b200.h: plain pointers and sizes, device memory owned by
+ * the caller, asynchronous on the given stream, int status (0 = ok, message via lg_last_error()).  No host
+ * synchronisation and a launch sequence that depends on (B, M, N, D) only, so a call can be captured in a CUDA graph.
+ * The B x M x N similarity matrix is never written to memory.
+ *
+ * Semantics (oracle/nn_oracle.py restates them in float64).  Pair b has image 0 rows i < m_b and image 1 rows j < n_b,
+ * m_b = lens0[b] and n_b = lens1[b] (clamped to [0, M] / [0, N]) when given, M and N otherwise.
+ *   s_ij = d0_i . d1_j, the dot product of the descriptors.  They are expected to be unit-norm, as every extractor of
+ *        this library returns them; the matcher does not re-normalise them.
+ *   Image 0 -> image 1, per row i:
+ *     j1 = the j with the largest s_ij (on a tie the lowest j), s1 = s_i,j1;
+ *     s2 = the largest s_ij over j != j1 (it may equal s1; -inf when n_b = 1);
+ *     D1 = 2 (1 - s1), D2 = 2 (1 - s2) (+inf when s2 = -inf): the squared L2 distances of unit vectors;
+ *     row i keeps j1 when n_b >= 1 and (ratio_thresh <= 0 or D1 <= r2 * D2) and (distance_thresh <= 0 or D1 <= t2),
+ *     with r2 = (float)(ratio_thresh^2) and t2 = (float)(distance_thresh^2) formed in double, and D1, D2, the product
+ *     and the comparisons in fp32.
+ *   Image 1 -> image 0 likewise, per row j.
+ *   mutual_check != 0: a kept i -> j survives only if j -> i is kept as well, and the same from the other side.
+ *   Outputs: matches0[b, i] = the surviving j or -1, matching_scores0[b, i] = (s1 + 1) / 2 for a matched row (in [0, 1]
+ *   for unit descriptors, like LightGlue's scores) and 0 otherwise; matches1 / matching_scores1 from image 1's side.
+ *   Rows past a pair's count get -1 and 0.  A pair with m_b = 0 or n_b = 0 matches nothing.  matches[b] lists the
+ *   pairs (i, matches0[b, i]) of the matched rows in ascending i, match_scores[b] their scores, n_matches[b] how many.
+ *   Without the mutual check these come from image 0's side only, and several rows of image 0 may name the same j.
+ *
+ * Arithmetic: s_ij comes from three bf16 tensor-core products with fp32 accumulation, d = hi + lo with hi = bf16(d) and
+ * lo = bf16(d - hi): hi0 hi1 + hi0 lo1 + lo0 hi1 (lo0 lo1 is dropped).  For unit descriptors and D <= 512 it differs
+ * from the exact dot product by about 5e-5 at most; it is exact when every descriptor entry is a bf16 value and the sums
+ * are exact in fp32.
+ *
+ * Work: the pairs run in groups of G pairs (G * Lp <= NN_GROUP_ROWS rows per image, at least one pair; Lp = max(M, N)
+ * rounded up to a multiple of 128), three launches per group: the split into bf16 hi / lo images, one tensor-core
+ * sweep that computes every S tile of both directions and keeps, per row and per 128 columns, the best two similarities
+ * and the arg-max, and one CTA per pair that merges them, applies the tests and writes the outputs.
+ */
+#ifndef NN_B200_H
+#define NN_B200_H
+
+#include <stddef.h>
+#include <stdint.h>
+
+#ifdef __cplusplus
+extern "C" {
+#endif
+
+#ifndef LG_API
+#define LG_API __attribute__((visibility("default")))
+#endif
+
+#define NN_ABI_VERSION 1
+#define NN_MIN_DIM 64       /* dim: a multiple of 64 in [NN_MIN_DIM, NN_MAX_DIM] */
+#define NN_MAX_DIM 512
+#define NN_GROUP_ROWS 32768 /* rows of one image's side the pairs of one group hold together */
+
+/* Mirrors NearestNeighborMatcher.default_conf; thresholds <= 0 switch their test off. */
+typedef struct NnConfig {
+  int32_t abi_version;   /* NN_ABI_VERSION */
+  int32_t dim;           /* descriptor size D */
+  int32_t mutual_check;  /* non-zero: keep mutual nearest neighbours only */
+  float ratio_thresh;    /* Lowe's ratio r on distances, in (0, 1]; <= 0: off */
+  float distance_thresh; /* t on the L2 distance; <= 0: off */
+} NnConfig;
+
+typedef struct NnInputs {
+  int32_t B, M, N;
+  const float* desc0;   /* [B, M, D] fp32, 16-byte aligned */
+  const float* desc1;   /* [B, N, D] */
+  const int32_t* lens0; /* optional DEVICE [B]: pair b uses the first lens0[b] rows of desc0; NULL = M */
+  const int32_t* lens1; /* optional DEVICE [B]; NULL = N */
+} NnInputs;
+
+typedef struct NnOutputs {
+  int64_t* matches0;       /* [B, M] -1 = unmatched */
+  int64_t* matches1;       /* [B, N] */
+  float* matching_scores0; /* [B, M] */
+  float* matching_scores1; /* [B, N] */
+  int32_t* n_matches;      /* [B] */
+  int64_t* matches;        /* [B, M, 2] (i, j), ascending i; the first n_matches[b] rows are valid.  M rows: without
+                              the mutual check every row of image 0 may match */
+  float* match_scores;     /* [B, M] */
+} NnOutputs;
+
+typedef struct NnHandle NnHandle;
+
+/* The handle holds the tensor-map cache of the tensor-core sweep; it has no weights. */
+LG_API int nn_create(void* stream, NnHandle** out);
+LG_API int nn_destroy(NnHandle* h);
+
+/* Scratch bytes of nn_match for a (B, M, N, D) problem (0 for invalid sizes): the bf16 images and the per-slot
+ * partials of one group of pairs, O(G Lp (D + Lp / 128 * 3) * 8) bytes.  No zero fill is needed. */
+LG_API size_t nn_workspace_bytes(int32_t B, int32_t M, int32_t N, int32_t D);
+
+LG_API int nn_match(NnHandle* h, const NnConfig* cfg, const NnInputs* in, const NnOutputs* out, void* workspace,
+                    size_t workspace_bytes, void* stream);
+
+#ifdef __cplusplus
+}
+#endif
+#endif /* NN_B200_H */

@@ -7,6 +7,7 @@ kernels behind the C ABI declared in ``include/lightglue_b200.h``.
 from .disk import DISK  # noqa: F401
 from .dog_hardnet import DoGHardNet  # noqa: F401
 from .matcher import LightGlue  # noqa: F401
+from .nn_matcher import NearestNeighborMatcher  # noqa: F401
 from .sift import SIFT  # noqa: F401
 
-__all__ = ["DISK", "DoGHardNet", "LightGlue", "SIFT"]
+__all__ = ["DISK", "DoGHardNet", "LightGlue", "NearestNeighborMatcher", "SIFT"]

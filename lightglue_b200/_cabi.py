@@ -11,7 +11,7 @@ K_ATTENTION, K_LINEAR, K_ASSIGN, K_OTHER = 0, 1, 2, 3
 ABI_VERSION = 3
 
 # include/superpoint_b200.h, include/aliked_b200.h, include/sift_b200.h, include/disk_b200.h,
-# include/doghardnet_b200.h and include/geometry_b200.h: same library
+# include/doghardnet_b200.h, include/geometry_b200.h and include/nn_b200.h: same library
 SP_ABI_VERSION = 2
 SP_TC_BUFFERS = 9  # buffers of the tensor-core backbone's workspace plan (sp_tc_layout)
 AL_ABI_VERSION = 1
@@ -20,6 +20,8 @@ DISK_ABI_VERSION = 1
 DHN_ABI_VERSION = 1
 GEO_ABI_VERSION = 1  # include/geometry_b200.h
 GEO_HOMOGRAPHY, GEO_FUNDAMENTAL, GEO_ESSENTIAL = 0, 1, 2
+NN_ABI_VERSION = 1  # include/nn_b200.h
+NN_MIN_DIM, NN_MAX_DIM, NN_GROUP_ROWS = 64, 512, 32768
 
 
 class LgConfig(C.Structure):
@@ -152,6 +154,28 @@ class GeoPnpOutputs(C.Structure):
     ]
 
 
+class NnConfig(C.Structure):
+    _fields_ = [
+        ("abi_version", C.c_int32), ("dim", C.c_int32), ("mutual_check", C.c_int32), ("ratio_thresh", C.c_float),
+        ("distance_thresh", C.c_float),
+    ]
+
+
+class NnInputs(C.Structure):
+    _fields_ = [
+        ("B", C.c_int32), ("M", C.c_int32), ("N", C.c_int32),
+        ("desc0", C.c_void_p), ("desc1", C.c_void_p), ("lens0", C.c_void_p), ("lens1", C.c_void_p),
+    ]
+
+
+class NnOutputs(C.Structure):
+    _fields_ = [
+        ("matches0", C.c_void_p), ("matches1", C.c_void_p), ("matching_scores0", C.c_void_p),
+        ("matching_scores1", C.c_void_p), ("n_matches", C.c_void_p), ("matches", C.c_void_p),
+        ("match_scores", C.c_void_p),
+    ]
+
+
 # name: (restype, argtypes), one table per header.  The export lists are the tables' keys.
 _VP, _I32, _I64, _SZ = C.c_void_p, C.c_int32, C.c_int64, C.c_size_t
 _HANDLE_OUT = C.POINTER(C.c_void_p)
@@ -225,8 +249,16 @@ GEO_PROTOTYPES = {  # include/geometry_b200.h
     "geo_absolute_pose": (C.c_int, [C.POINTER(GeoPnpConfig), C.POINTER(GeoPnpInputs), C.POINTER(GeoPnpOutputs), _VP,
                                     _SZ, _VP]),
 }
-_TABLES = (LG_PROTOTYPES, SP_PROTOTYPES, AL_PROTOTYPES, SIFT_PROTOTYPES, DISK_PROTOTYPES, DHN_PROTOTYPES, GEO_PROTOTYPES)
-EXPORTS, SP_EXPORTS, AL_EXPORTS, SIFT_EXPORTS, DISK_EXPORTS, DHN_EXPORTS, GEO_EXPORTS = (tuple(t) for t in _TABLES)
+NN_PROTOTYPES = {  # include/nn_b200.h
+    "nn_create": (C.c_int, [_VP, _HANDLE_OUT]),
+    "nn_destroy": (C.c_int, [_VP]),
+    "nn_workspace_bytes": (_SZ, [_I32, _I32, _I32, _I32]),
+    "nn_match": (C.c_int, [_VP, C.POINTER(NnConfig), C.POINTER(NnInputs), C.POINTER(NnOutputs), _VP, _SZ, _VP]),
+}
+_TABLES = (LG_PROTOTYPES, SP_PROTOTYPES, AL_PROTOTYPES, SIFT_PROTOTYPES, DISK_PROTOTYPES, DHN_PROTOTYPES, GEO_PROTOTYPES,
+           NN_PROTOTYPES)
+EXPORTS, SP_EXPORTS, AL_EXPORTS, SIFT_EXPORTS, DISK_EXPORTS, DHN_EXPORTS, GEO_EXPORTS, NN_EXPORTS = (
+    tuple(t) for t in _TABLES)
 
 _lib = None
 

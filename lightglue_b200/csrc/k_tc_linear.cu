@@ -10,7 +10,7 @@
 // * A may be the concatenation of two sources along K (the FFN input cat([x, msg]), lightglue.py:172);
 // * fused epilogues: bias (+ RoPE, head split, V transpose) for the QKV projections, bias + LayerNorm(512) + exact
 //   GELU for ffn.0, bias + residual for ffn.3, bias * scale for input_proj / final_proj, the row reductions of the
-//   assignment's similarity sweeps, bias + ReLU for the SuperPoint convolutions.
+//   assignment's similarity sweeps, the nearest-neighbour matcher's top-2 sweep, bias + ReLU for the convolutions.
 // Tiles: 128 rows x 256 columns, MMA warpgroup g owns rows 64 g .. +63.  The LayerNorm variant runs in clusters of two
 // CTAs: a cluster owns a 128-row tile of all 512 columns, CTA rank r columns 256 r .. +255, and the two CTAs exchange
 // their row partial sums through distributed shared memory.
@@ -28,7 +28,7 @@ namespace {
 constexpr int BN = 256, BK = 64;
 constexpr int W_TILE_BYTES = BN * BK * 2;  // 32 KB
 
-enum { TEPI_QKV = 0, TEPI_LN_GELU = 2, TEPI_RESID = 3, TEPI_F32 = 4, TEPI_LSE = 5, TEPI_ARGMAX = 6, TEPI_CONV = 7 };
+enum { TEPI_QKV = 0, TEPI_LN_GELU = 2, TEPI_RESID = 3, TEPI_F32 = 4, TEPI_LSE = 5, TEPI_ARGMAX = 6, TEPI_CONV = 7, TEPI_TOP2 = 8 };
 
 struct TcLinParams {
   CUtensorMap a_hi[2], a_lo[2];  // A segment 0 / 1, box 64 x tile rows
@@ -38,7 +38,8 @@ struct TcLinParams {
   SeqState st;
   int w_select;                  // 1: third TMA coordinate / bias offset = stop_layer[pair] - 1
                                  // 2: third TMA coordinate = partner sequence (similarity sweeps of the assignment)
-  float* part; int* part_arg; int part_stride;  // TEPI_LSE: (max, sumexp) pairs; TEPI_ARGMAX: best / arg, [S*Lp, part_stride]
+  float* part; int* part_arg; int part_stride;  // TEPI_LSE: (max, sumexp) pairs; TEPI_ARGMAX: best / arg; TEPI_TOP2:
+                                                // (s1, s2) pairs / j1, [S*Lp, part_stride]
   const float* term;             // TEPI_ARGMAX: logsigmoid(z) - LSE per token, [S, Lp]
   int reverse;  // walk the tile list from its end: a kernel that reads what the previous kernel wrote LAST finds it in L2
   float* logmat; int mat_m, mat_n;  // TEPI_ARGMAX, optional: materialise the [B, M+1, N+1] log-assignment matrix (core block)
@@ -403,6 +404,51 @@ __global__ void __launch_bounds__(LinCfg<EPI>::THREADS, 1) tc_linear_kernel(cons
       ++lt;
     }
 
+    if (EPI == TEPI_TOP2) {
+      // ---------------------------------------------------------------- nearest-neighbour sweep (nn_api.cu)
+      // per row and per 128-column slot of live partner columns: the best similarity s1, its column j1 (ascending
+      // columns: the first maximum wins) and the best over the slot's other columns s2 (equal to s1 on a tie)
+      const int lens = p.st.len[ti.sel];
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
+        const int rl = rl_a + 8 * hr;
+        const long grow = ti.grow0 + rl;
+        const bool live = ti.r0 + rl < ti.len;
+#pragma unroll
+        for (int half = 0; half < 2; ++half) {
+          const int col0 = ti.n_tile * BN + half * 128;
+          const int ncols = lens - col0;
+          float b1 = -INFINITY, b2 = -INFINITY;
+          int a1 = INT_MAX;
+#pragma unroll
+          for (int jj = 0; jj < 16; ++jj)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int c = 8 * jj + 2 * tq + e;
+              const float v = acc[4 * (16 * half + jj) + 2 * hr + e];
+              if (c < ncols) {
+                if (v > b1) { b2 = b1; b1 = v; a1 = col0 + c; }
+                else b2 = fmaxf(b2, v);
+              }
+            }
+          // merge over the quad of lanes that holds the row: (value descending, index ascending)
+#pragma unroll
+          for (int o = 1; o <= 2; o <<= 1) {
+            const float ob1 = __shfl_xor_sync(0xffffffffu, b1, o), ob2 = __shfl_xor_sync(0xffffffffu, b2, o);
+            const int oa1 = __shfl_xor_sync(0xffffffffu, a1, o);
+            if (ob1 > b1 || (ob1 == b1 && oa1 < a1)) { b2 = fmaxf(b1, ob2); b1 = ob1; a1 = oa1; }
+            else b2 = fmaxf(b2, ob1);
+          }
+          if (live && tq == 0) {
+            const long at = grow * p.part_stride + ti.n_tile * 2 + half;
+            reinterpret_cast<float2*>(p.part)[at] = make_float2(b1, b2);
+            p.part_arg[at] = a1;
+          }
+        }
+      }
+      continue;
+    }
+
     if (EPI == TEPI_LSE || EPI == TEPI_ARGMAX) {
       // ---------------------------------------------------------------- assignment sweeps (lightglue.py:265-277, 302-305)
       // on a 128 x 256 tile of S = p_s p_partner^T; partials per 128-column slot, reduced over the quad of lanes that
@@ -703,6 +749,7 @@ int launch_linear(const TcLinParams& p, cudaStream_t stream) {
     case TEPI_CONV: return launch_linear_t<TEPI_CONV>(p, stream);
     case TEPI_LSE: return launch_linear_t<TEPI_LSE>(p, stream);
     case TEPI_ARGMAX: return launch_linear_t<TEPI_ARGMAX>(p, stream);
+    case TEPI_TOP2: return launch_linear_t<TEPI_TOP2>(p, stream);
   }
   return lg_set_error("launch_linear: bad epilogue");
 }
@@ -821,6 +868,21 @@ int tc_assign_sweeps(LgHandle* h, const TcBuffers& b, const SeqState& st, const 
   return misc_assign_tail(a, st, part, part_arg, 2 * ntc, BN / 2, stream);
 }
 
+// Nearest-neighbour sweep: S = d_s d_partner^T of every sequence in split-bf16 (hi / lo [st.S * st.Lp, dim]), per row the
+// top-2 partials of every 128-column slot into part (float2) / part_arg, [st.S * st.Lp, pstride]
+int tc_nn_sweep(TcEngine& e, const SeqState& st, const __nv_bfloat16* hi, const __nv_bfloat16* lo, int dim, float* part,
+                int* part_arg, int pstride, cudaStream_t stream) {
+  if (dim % BK != 0) return lg_set_error("tc_nn_sweep: the descriptor size must be a multiple of 64");
+  const int ntc = (st.Lp + BN - 1) / BN;
+  if (pstride < 2 * ntc) return lg_set_error("tc_nn_sweep: slot stride too small");
+  const TcOperands ops{hi, lo, dim, nullptr, nullptr, 0, hi, lo, st.Lp, st.S, (size_t)st.Lp * dim};
+  TcLinParams p{};
+  p.epi = TEPI_TOP2; p.scale = 1.f;
+  p.part = part; p.part_arg = part_arg; p.part_stride = pstride;
+  p.w_select = 2;
+  return tc_gemm(e, st, ops, ntc, p, stream);
+}
+
 unsigned int tc_debug_timeout_code(const TcEngine& e, unsigned int* words32) {
   unsigned int v[32] = {0};
   if (!e.dbg) return 0;
@@ -836,12 +898,15 @@ unsigned int tc_debug_timeout_code(const TcEngine& e, unsigned int* words32) {
 
 int tc_engine_create(TcEngine* e, const float* w, size_t n, bool x3, cudaStream_t stream) {
   e->x3 = x3;
-  cudaError_t err = cudaMalloc(&e->w_hi, n * sizeof(__nv_bfloat16));
-  if (err != cudaSuccess) return lg_set_cuda_error(err, __FILE__, __LINE__);
-  err = cudaMalloc(&e->w_lo, n * sizeof(__nv_bfloat16));
-  if (err != cudaSuccess) return lg_set_cuda_error(err, __FILE__, __LINE__);
-  split_weights_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(w, e->w_hi, e->w_lo, n);
-  LG_CHECK_LAUNCH();
+  cudaError_t err;
+  if (n) {  // n = 0: an engine without weights (both operands are activations)
+    err = cudaMalloc(&e->w_hi, n * sizeof(__nv_bfloat16));
+    if (err != cudaSuccess) return lg_set_cuda_error(err, __FILE__, __LINE__);
+    err = cudaMalloc(&e->w_lo, n * sizeof(__nv_bfloat16));
+    if (err != cudaSuccess) return lg_set_cuda_error(err, __FILE__, __LINE__);
+    split_weights_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(w, e->w_hi, e->w_lo, n);
+    LG_CHECK_LAUNCH();
+  }
   e->maps = new TcMapCache();
   err = cudaMalloc(&e->dbg, 32 * sizeof(unsigned int));
   if (err != cudaSuccess) return lg_set_cuda_error(err, __FILE__, __LINE__);

@@ -11,7 +11,8 @@
 struct LgHandle;
 struct TcMapCache;
 
-// What the tensor-core GEMMs need from their owner (the matcher's handle, a TcConvWeights); all zero = none
+// What the tensor-core GEMMs need from their owner (the matcher's handle, a TcConvWeights, the nearest-neighbour
+// matcher's handle); all zero = none
 struct TcEngine {
   bool x3;             // LG_PREC_BF16X3: three passes over K (hi / lo split operands)
   __nv_bfloat16* w_hi; // bf16 hi / lo images of the owner's packed fp32 weights (same element offsets)
@@ -19,7 +20,8 @@ struct TcEngine {
   TcMapCache* maps;    // tensor maps of the linears and attention, keyed by every encode argument
   unsigned int* dbg;   // device words: site code of the first pipeline wait that timed out (0 = none)
 };
-// splits the n floats of the device array w into the engine's bf16 images; on failure the caller still destroys `e`
+// splits the n floats of the device array w into the engine's bf16 images (n = 0: no weights); on failure the caller
+// still destroys `e`
 int tc_engine_create(TcEngine* e, const float* w, size_t n, bool x3, cudaStream_t stream);
 void tc_engine_destroy(TcEngine* e);
 // 0, or the site code of the first mbarrier wait that timed out since the last call (synchronises)
@@ -45,6 +47,11 @@ int tc_final_proj(LgHandle* h, const TcBuffers& b, const SeqState& st, float* p_
 // (sweep 1) and row arg-max of the score (sweep 2); p (bf16 hi/lo) is read from b.msgh / b.msgl.
 int tc_assign_sweeps(LgHandle* h, const TcBuffers& b, const SeqState& st, const AssignArgs& a, float* part, int* part_arg,
                      float* term, cudaStream_t stream);
+// Nearest-neighbour sweep on the tensor cores (split-bf16, e.x3): S = d_s d_partner^T in both directions from the bf16
+// hi / lo images [st.S * st.Lp, dim]; per live row and 128-column slot of live partner columns, (s1, s2) into part
+// (float2) and j1 into part_arg, [st.S * st.Lp, pstride] with pstride >= 2 ceil(Lp / 256) (k_tc_linear.cu, TEPI_TOP2)
+int tc_nn_sweep(TcEngine& e, const SeqState& st, const __nv_bfloat16* hi, const __nv_bfloat16* lo, int dim, float* part,
+                int* part_arg, int pstride, cudaStream_t stream);
 // softmax(q k^T / 8) v per (sequence, head): q from b.q, keys from kbuf, values from b.vt; key/value
 // sequence = (s + kv_shift) % S; writes b.ctxh (/ b.ctxl)
 int tc_attention(LgHandle* h, const TcBuffers& b, const SeqState& st, int kv_shift, const __half* kbuf, cudaStream_t stream);

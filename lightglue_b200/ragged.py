@@ -71,17 +71,20 @@ def split_outputs(out: dict, lens0, lens1) -> List[Dict]:
     res = []
     lists = isinstance(out["matches"], (list, tuple))
     for b, (m, n) in enumerate(zip(lens0, lens1)):
-        res.append({
+        pair = {
             "matches0": out["matches0"][b : b + 1, :m],
             "matches1": out["matches1"][b : b + 1, :n],
             "matching_scores0": out["matching_scores0"][b : b + 1, :m],
             "matching_scores1": out["matching_scores1"][b : b + 1, :n],
             "matches": [out["matches"][b]] if lists else out["matches"][b : b + 1],
             "scores": [out["scores"][b]] if lists else out["scores"][b : b + 1],
-            "prune0": out["prune0"][b : b + 1, :m],
-            "prune1": out["prune1"][b : b + 1, :n],
-            "stop": int(out["stops"][b]) if "stops" in out else out["stop"],
-        })
+        }
+        if "prune0" in out:  # LightGlue's adaptive-depth keys; a matcher without layers has none
+            pair["prune0"] = out["prune0"][b : b + 1, :m]
+            pair["prune1"] = out["prune1"][b : b + 1, :n]
+        if "stops" in out or "stop" in out:
+            pair["stop"] = int(out["stops"][b]) if "stops" in out else out["stop"]
+        res.append(pair)
     return res
 
 
