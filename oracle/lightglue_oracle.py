@@ -172,12 +172,19 @@ def forward(
     add_scale_ori: bool = False,
     dtype: torch.dtype = torch.float32,
     return_layers: bool = False,
+    return_decisions: bool = False,
 ) -> dict:
     """lightglue/lightglue.py:483-629 (``LightGlue._forward``), eager/unpadded path, any device -> CPU.
 
     ``pruning_threshold`` plays the role of ``pruning_min_kpts(device)`` (658-662): point pruning
     runs on an image only while it still has more keypoints than this.  The reference's adaptive
     bookkeeping (549, 554) is only meaningful for batch size 1; the oracle asserts that.
+
+    ``return_decisions`` adds ``out["decisions"]``: one dict per executed layer below the last with the values its
+    adaptive decisions were taken from -- ``thr`` and ``size`` (m + n, original sizes) always; with early exit on,
+    ``tok0`` / ``tok1`` (token confidences of the live points) and ``below`` (how many are < ``thr``); for each image
+    that is pruned at that layer, ``mat0`` / ``mat1`` (matchability of its live points).  ``certificate`` turns
+    them into the pair's smallest margins.
     """
     w = {k: v.to(dtype) for k, v in w.items()}
     d0, d1 = data["image0"], data["image1"]
@@ -210,6 +217,7 @@ def forward(
     pr0 = torch.ones(b, m, dtype=torch.long)
     pr1 = torch.ones(b, n, dtype=torch.long)
     layers: List[tuple] = []
+    decisions: List[dict] = []
     last = 0
     tok0 = tok1 = None
     for i in range(n_layers):
@@ -223,20 +231,26 @@ def forward(
             layers.append((x0.clone(), x1.clone()))
         if i == n_layers - 1:  # 544-545
             continue
+        dec = {"thr": float(thr[i]), "size": m + n}
+        if return_decisions:
+            decisions.append(dec)
         if early:  # 547-550, 645-656
             tok0, tok1 = token_confidence(w, i, x0), token_confidence(w, i, x1)
             below = (torch.cat([tok0, tok1], -1) < thr[i]).to(dtype).sum()
+            dec.update(tok0=tok0[0], tok1=tok1[0], below=int(below))
             if 1.0 - below / (m + n) > depth_confidence:
                 break
         if prune and x0.shape[1] > pruning_threshold:  # 551-558, 636-643
-            keep = matchability(w, i, x0) > (1 - width_confidence)
+            dec["mat0"] = matchability(w, i, x0)[0]
+            keep = dec["mat0"][None] > (1 - width_confidence)
             if tok0 is not None:
                 keep |= tok0 <= thr[i]
             kk = torch.where(keep)[1]
             ind0, x0, c0, s0 = ind0[:, kk], x0[:, kk], c0[:, kk], s0[:, kk]
             pr0[:, ind0[0]] += 1
         if prune and x1.shape[1] > pruning_threshold:  # 559-566
-            keep = matchability(w, i, x1) > (1 - width_confidence)
+            dec["mat1"] = matchability(w, i, x1)[0]
+            keep = dec["mat1"][None] > (1 - width_confidence)
             if tok1 is not None:
                 keep |= tok1 <= thr[i]
             kk = torch.where(keep)[1]
@@ -255,6 +269,8 @@ def forward(
             "prune0": pr0 if prune else torch.full((b, m), float(n_layers), dtype=dtype),
             "prune1": pr1 if prune else torch.full((b, n), float(n_layers), dtype=dtype),
         }
+        if return_decisions:
+            out["decisions"] = decisions
         return out
 
     scores = log_assignment(w, last, x0, x1)  # 591
@@ -296,4 +312,37 @@ def forward(
     if return_layers:
         out["layers"] = layers
         out["log_assignment"] = scores
+    if return_decisions:
+        out["decisions"] = decisions
     return out
+
+
+def certificate(decisions: List[dict], *, depth_confidence: float, width_confidence: float):
+    """A pair's smallest decision margins over ``forward(..., return_decisions=True)["decisions"]``:
+    ``(margin, slack)`` where
+
+    * ``margin`` is the least of |token confidence - thr_i| over the live points and |matchability - (1 -
+      width_confidence)| over the points a pruning step could drop (confidence > thr_i; every point when early exit
+      is off);
+    * ``slack`` is the least distance, in points, between the below-threshold count and the stop boundary
+      (1 - depth_confidence)(m + n).  The stop ratio is evaluated in fp32 on both sides, so a count on the
+      boundary has slack 0 and is never certified.
+
+    Both are ``inf`` where no such decision was taken."""
+    margin = slack = math.inf
+    for d in decisions:
+        thr = d["thr"]
+        if "below" in d:
+            for t in (d["tok0"], d["tok1"]):
+                if t.numel():
+                    margin = min(margin, float((t.double() - thr).abs().min()))
+            slack = min(slack, abs((1.0 - depth_confidence) * d["size"] - d["below"]))
+        for k, t in (("mat0", d.get("tok0")), ("mat1", d.get("tok1"))):
+            if k not in d:
+                continue
+            mt = d[k].double()
+            if t is not None:
+                mt = mt[t > thr]
+            if mt.numel():
+                margin = min(margin, float((mt - (1.0 - width_confidence)).abs().min()))
+    return margin, slack

@@ -19,109 +19,10 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 import torch  # noqa: E402
-import torch.nn.functional as F  # noqa: E402
 
 from lightglue_b200 import synth  # noqa: E402
 from oracle import lightglue_oracle as oracle  # noqa: E402
-
-
-def rnd(x: torch.Tensor, bits: int) -> torch.Tensor:
-    """round-to-nearest-even to `bits` explicit mantissa bits (7 = bf16, 10 = fp16 ignoring its range)."""
-    if bits == 7:
-        return x.to(torch.bfloat16).to(torch.float32)
-    if bits == 10:
-        return x.to(torch.float16).to(torch.float32)
-    raise ValueError(bits)
-
-
-def split(x, bits):
-    hi = rnd(x, bits)
-    return hi, rnd(x - hi, bits)
-
-
-def gemm(a, w, mode):
-    """a [.., K] x w [N, K]^T with the operand formats of `mode`."""
-    if mode == "f32":
-        return a @ w.t()
-    if mode in ("bf16", "fp16"):
-        b = 7 if mode == "bf16" else 10
-        return rnd(a, b) @ rnd(w, b).t()
-    b = 7 if mode.startswith("bf16") else 10
-    ah, al = split(a, b)
-    wh, wl = split(w, b)
-    if mode.endswith("x3"):
-        return al @ wh.t() + ah @ wl.t() + ah @ wh.t()
-    if mode.endswith("x2a"):  # activations split, weights hi only
-        return al @ wh.t() + ah @ wh.t()
-    if mode.endswith("x2w"):  # weights split, activations hi only
-        return ah @ wl.t() + ah @ wh.t()
-    raise ValueError(mode)
-
-
-class Shim:
-    """Stands in for torch.nn.functional inside the oracle: routes F.linear by weight name."""
-
-    def __init__(self, sd, pmap):
-        self.cls = {}
-        for k, v in sd.items():
-            if not k.endswith("weight"):
-                continue
-            c = None
-            if "Wqkv" in k or "to_qk" in k or "to_v" in k:
-                c = "qkv"
-            elif "out_proj" in k or "to_out" in k:
-                c = "out"
-            elif "ffn.0" in k:
-                c = "ffn0"
-            elif "ffn.3" in k:
-                c = "ffn3"
-            elif "final_proj" in k:
-                c = "final"
-            elif "input_proj" in k:
-                c = "qkv"
-            if c:
-                self.cls[id(v)] = c
-        self.pmap = pmap
-
-    def linear(self, x, w, b=None):
-        c = self.cls.get(id(w))
-        if c == "ffn0" and self.pmap.get("msg") == "hi":  # msg half of cat([x, msg]) kept as a single 16-bit image
-            mode = self.pmap.get(c, "f32")
-            x = torch.cat([x[..., :256], rnd(x[..., 256:], 7 if mode.startswith("bf16") else 10)], -1)
-        y = gemm(x, w, self.pmap.get(c, "f32")) if c else x @ w.t()
-        return y if b is None else y + b
-
-    def __getattr__(self, name):
-        return getattr(F, name)
-
-
-def attention_fp16(q, k, v):
-    """fp16 q, k, v operands, fp32 scores / softmax statistics, fp16 P for the numerator (k_tc_attn.cu)."""
-    q, k, v = rnd(q, 10), rnd(k, 10), rnd(v, 10)
-    s = (q @ k.transpose(-1, -2)) * 0.125
-    e = torch.exp(s - s.amax(-1, keepdim=True))
-    return (rnd(e, 10) @ v) / e.sum(-1, keepdim=True)
-
-
-def make_log_assignment(pmap):
-    def log_assignment(w, i, x0, x1):
-        p = f"log_assignment.{i}."
-        b, m, _ = x0.shape
-        n = x1.shape[1]
-        fm = pmap.get("final", "f32")
-        p0 = (gemm(x0, w[p + "final_proj.weight"], fm) + w[p + "final_proj.bias"]) / 4.0
-        p1 = (gemm(x1, w[p + "final_proj.weight"], fm) + w[p + "final_proj.bias"]) / 4.0
-        sm = pmap.get("sim", "f32")
-        sim = torch.stack([gemm(p0[i_], p1[i_], sm) for i_ in range(b)])
-        z0 = F.linear(x0, w[p + "matchability.weight"], w[p + "matchability.bias"])
-        z1 = F.linear(x1, w[p + "matchability.weight"], w[p + "matchability.bias"])
-        out = sim.new_zeros(b, m + 1, n + 1)
-        out[:, :m, :n] = (torch.log_softmax(sim, 2) + torch.log_softmax(sim, 1) + F.logsigmoid(z0)
-                          + F.logsigmoid(z1).transpose(1, 2))
-        out[:, :m, n] = F.logsigmoid(-z0.squeeze(-1))
-        out[:, m, :n] = F.logsigmoid(-z1.squeeze(-1))
-        return out
-    return log_assignment
+from oracle.tc_emulation import emulated  # noqa: E402
 
 
 MAPS2 = {
@@ -155,24 +56,18 @@ def main():
     torch.set_grad_enabled(False)
     sd = synth.make_state_dict()
     pairs = [synth.make_pair(args.n, seed=1000 + i)[0] for i in range(args.pairs)]
-    orig_F, orig_attn, orig_la = oracle.F, oracle.attention, oracle.log_assignment
     refs = [oracle.forward(sd, d) for d in pairs]
     print(f"# {args.pairs} pairs, N={args.n}; attention operands fp16 in every map; flips over {2 * args.n * args.pairs} indices")
     for name, pmap in (MAPS if args.set == 1 else MAPS2).items():
         if args.only and args.only not in name:
             continue
         t0 = time.time()
-        oracle.F = Shim(sd, pmap)
-        oracle.attention = attention_fp16
-        oracle.log_assignment = make_log_assignment(pmap)
-        flips, dmax, near = 0, 0.0, 0
-        try:
+        flips, dmax = 0, 0.0
+        with emulated(sd, pmap):
             for d, r in zip(pairs, refs):
                 o = oracle.forward(sd, d)
                 flips += int((o["matches0"] != r["matches0"]).sum()) + int((o["matches1"] != r["matches1"]).sum())
                 dmax = max(dmax, float((o["matching_scores0"] - r["matching_scores0"]).abs().max()))
-        finally:
-            oracle.F, oracle.attention, oracle.log_assignment = orig_F, orig_attn, orig_la
         print(f"{name:40s} flips={flips:4d}  max|dscore|={dmax:.2e}  ({time.time() - t0:.0f} s)", flush=True)
 
 
