@@ -128,6 +128,48 @@
  * P8. A pair fails (success 0, E, R and t zero, no inliers, best_hypothesis = best_solution = -1) when n < 5, a K is
  *     invalid, or every sample is degenerate.
  *
+ * LO-RANSAC relative pose (geo_relative_pose_lo; oracle/lo_pose_oracle.py restates it bit for bit): the outputs of
+ * geo_relative_pose, from an MSAC-scored five-point RANSAC with Levenberg-Marquardt local optimisation (Chum, Matas and
+ * Kittler, DAGM 2003; the schedule of PoseLib's LO-RANSAC, with the deviations below).  Expressions evaluate left to
+ * right as written; every multiply and add rounds on its own.
+ *
+ * L1. Compaction, calibration, K checks and the threshold thr2 = (float)(t*t) exactly as P1.  M <= GEO_LO_MAX_MATCHES.
+ * L2. Sampling and the five-point solutions exactly as P2 and P3: with the same seed both estimators draw the same
+ *     samples and solve the same solutions.
+ * L3. MSAC score, per solution of every sample, from P4's fp32 err (the solution rounded to float):
+ *     w = GEO_LO_QSCALE / thr2 in fp32, q = err < thr2 ? (uint32)(err * w) (fp32 product, truncated) : GEO_LO_QSCALE.
+ *     score = sum of q over the points in uint64 (exact in any order), count = the number of err < thr2.  Lower is
+ *     better; ties go to the lowest (sample h, solution r).
+ * L4. Local optimisation, after every chunk of GEO_CHUNK samples, once per pair.  Chunk c's best solution (lowest
+ *     (score, h, r)) is taken when the pair has no model yet or its score is strictly below the model's score; else
+ *     nothing happens.  Taken, it becomes the pair's model (score, count, h, r) with the (R, t) of P7's candidate choice
+ *     on its inliers (its fp32 E widened to double as P7's E).  Then GEO_LO_STEPS LM steps (below) from that (R, t)
+ *     give (R', t'), which are scored as L3 through E' = [t']x R' scaled as P3 and rounded to float; with a strictly
+ *     lower score they replace the model (keeping h and r) and num_local_optimizations counts one.
+ * L5. Stopping as P5 from the model's count (a local optimisation's count included).
+ * L6. Final refinement: GEO_LO_FINAL_STEPS LM steps from the model's (R, t), kept unless their L3 score is higher.
+ * L7. LM, in double on the calibrated points read as floats widened.  At a pose (R, t):
+ *     E = [t]x R unscaled (column j is t x R[:, j], cross products a x b = (a1*b2 - a2*b1, a2*b0 - a0*b2,
+ *     a0*b1 - a1*b0)); per point a0 = (E0*x + E1*y) + E2, a1, a2 likewise, d = (u*a0 + v*a1) + a2,
+ *     b0 = (E0*u + E3*v) + E6, b1 = (E1*u + E4*v) + E7, den = ((a0*a0 + a1*a1) + b0*b0) + b1*b1, err = (d*d) / den,
+ *     r = d / sqrt(den).  A point is an inlier at this pose when err < (double)thr2.  The tangent basis of t: m the
+ *     first index of least |t_m|, c = t x e_m, b1 = c / sqrt((c0*c0 + c1*c1) + c2*c2), b2 = t x b1.  The parameters
+ *     delta0..4 move the pose to R' = Q R with Q the quaternion rotation of A7, and t' = v / sqrt((v0*v0 + v1*v1) + v2*v2)
+ *     with v_i = (t_i + delta3*b1_i) + delta4*b2_i.  dE_k = [t]x ([e_k]x R) for k < 3 and [b_(k-2)]x R for k = 3, 4
+ *     (column-wise cross products as above); da, dd, db of dE_k as a, d, b of E,
+ *     dden = ((a0*da0 + a1*da1) + b0*db0) + b1*db1, J_k = (dd - d*dden / den) / sqrt(den).  The 21 terms J_i*J_j
+ *     (i <= j in row order) and J_i*r over the inliers, and the truncated cost (err for an inlier, else (double)thr2)
+ *     over every point, are each summed in the order of step 2.  A step solves the 5x5 system of A7 (damping, Cholesky,
+ *     right-hand side -J^T r), lambda starts at GEO_LO_LAMBDA0, and the step is taken only if the truncated cost at the
+ *     new pose, with its own inliers, is strictly lower: A7's schedule.
+ * L8. Outputs: E = [t]x R of the final (R, t) scaled as P3; R and t as they are; inliers the points with err < thr2
+ *     under that E rounded to float (num_inliers their number, cost its L3 score); pose_inliers the inliers that pass
+ *     P7's triangulation test for that single (R, t).  best_hypothesis and best_solution name the solution that seeded
+ *     the final model; num_hypotheses the samples drawn.  A pair fails as P8, with num_local_optimizations and cost 0.
+ *     Deviations from PoseLib: local optimisation runs at most once per chunk rather than at every new best, so the
+ *     launch sequence is fixed and the result is deterministic; the score is quantised to integers; there is no
+ *     non-minimal refit inside the LO and no PROSAC ordering.
+ *
  * Absolute pose (geo_absolute_pose; oracle/pnp_oracle.py restates it bit for bit): the (R, t) of x_cam = R X + t that
  * maps the world points of image 1's keypoints into the query camera 0, OpenCV's rvec/tvec convention.  Expressions
  * below evaluate left to right as written (a + b + c is (a + b) + c); no step whose result must match bit for bit calls
@@ -299,6 +341,32 @@ typedef struct GeoPoseOutputs {
 LG_API size_t geo_pose_workspace_bytes(int32_t B, int32_t M, int32_t max_iters);
 LG_API int geo_relative_pose(const GeoPoseConfig* cfg, const GeoPoseInputs* in, GeoPoseOutputs* out, void* workspace,
                              size_t workspace_bytes, void* stream);
+
+#define GEO_LO_QSCALE 65536
+#define GEO_LO_STEPS 8
+#define GEO_LO_FINAL_STEPS 16
+#define GEO_LO_LAMBDA0 1e-3
+#define GEO_LO_MAX_MATCHES (1 << 20) /* M bound: a 40-bit score and a 24-bit count share one 64-bit sum */
+
+typedef struct GeoLoPoseConfig {
+  int32_t abi_version;        /* GEO_ABI_VERSION */
+  int32_t max_iters;          /* samples per pair, in [1, GEO_MAX_ITERS] */
+  uint32_t seed;
+  int32_t reserved;
+  double threshold;           /* pixels, > 0: Sampson distance, divided by the pair's mean focal length */
+  double confidence;          /* in [0, 1] */
+  double distance_threshold;  /* > 0: triangulated depth bound of the cheirality test */
+} GeoLoPoseConfig;
+
+typedef struct GeoLoPoseOutputs {
+  GeoPoseOutputs pose;               /* as geo_relative_pose's */
+  int32_t* num_local_optimizations;  /* [B] local optimisations whose model was adopted */
+  int64_t* cost;                     /* [B] L3 score of the final model */
+} GeoLoPoseOutputs;
+
+LG_API size_t geo_lo_pose_workspace_bytes(int32_t B, int32_t M, int32_t max_iters);
+LG_API int geo_relative_pose_lo(const GeoLoPoseConfig* cfg, const GeoPoseInputs* in, GeoLoPoseOutputs* out,
+                                void* workspace, size_t workspace_bytes, void* stream);
 
 #define GEO_PNP_MAX_SOLUTIONS 4
 #define GEO_PNP_COLLINEAR_EPS 1e-10

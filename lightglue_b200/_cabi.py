@@ -20,6 +20,7 @@ DISK_ABI_VERSION = 1
 DHN_ABI_VERSION = 1
 GEO_ABI_VERSION = 1  # include/geometry_b200.h
 GEO_HOMOGRAPHY, GEO_FUNDAMENTAL, GEO_ESSENTIAL = 0, 1, 2
+GEO_LO_QSCALE, GEO_LO_MAX_MATCHES = 65536, 1 << 20
 NN_ABI_VERSION = 1  # include/nn_b200.h
 NN_MIN_DIM, NN_MAX_DIM, NN_GROUP_ROWS = 64, 512, 32768
 
@@ -130,6 +131,14 @@ class GeoPoseOutputs(C.Structure):
         ("pose_inliers", C.c_void_p), ("num_pose_inliers", C.c_void_p), ("success", C.c_void_p),
         ("best_hypothesis", C.c_void_p), ("best_solution", C.c_void_p), ("num_hypotheses", C.c_void_p),
     ]
+
+
+class GeoLoPoseConfig(C.Structure):
+    _fields_ = GeoPoseConfig._fields_
+
+
+class GeoLoPoseOutputs(C.Structure):
+    _fields_ = [("pose", GeoPoseOutputs), ("num_local_optimizations", C.c_void_p), ("cost", C.c_void_p)]
 
 
 class GeoPnpConfig(C.Structure):
@@ -245,6 +254,9 @@ GEO_PROTOTYPES = {  # include/geometry_b200.h
     "geo_pose_workspace_bytes": (_SZ, [_I32, _I32, _I32]),
     "geo_relative_pose": (C.c_int, [C.POINTER(GeoPoseConfig), C.POINTER(GeoPoseInputs), C.POINTER(GeoPoseOutputs), _VP,
                                     _SZ, _VP]),
+    "geo_lo_pose_workspace_bytes": (_SZ, [_I32, _I32, _I32]),
+    "geo_relative_pose_lo": (C.c_int, [C.POINTER(GeoLoPoseConfig), C.POINTER(GeoPoseInputs),
+                                       C.POINTER(GeoLoPoseOutputs), _VP, _SZ, _VP]),
     "geo_pnp_workspace_bytes": (_SZ, [_I32, _I32, _I32]),
     "geo_absolute_pose": (C.c_int, [C.POINTER(GeoPnpConfig), C.POINTER(GeoPnpInputs), C.POINTER(GeoPnpOutputs), _VP,
                                     _SZ, _VP]),

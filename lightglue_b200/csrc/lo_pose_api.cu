@@ -1,0 +1,536 @@
+// Batched LO-RANSAC relative pose on the matcher's output: MSAC-scored five-point sampling with Levenberg-Marquardt
+// local optimisation and a final refinement (include/geometry_b200.h, steps L1-L8).
+//
+// Launches, all fixed by (B, M, max_iters):
+//   prepare  pose_api.cu's compaction kernel (pose_common.cuh)
+//   per chunk of GEO_CHUNK samples:
+//     hyp    one CTA per pair, one thread per sample: the five-point solutions, fp32
+//     score  (splits, B) CTAs: each streams a slice of the pair's points through shared memory against every solution
+//            of the chunk, one thread per sample, and adds count << 40 | MSAC score with one 64-bit atomic per solution
+//     lo     one CTA per pair: the chunk's lowest (score, h, r); when it beats the pair's model, P7's pose choice, LM
+//            on the truncated Sampson cost and a re-score; then the adaptive stop.  Otherwise it returns at once.
+//   final    one CTA per pair: the final LM refinement, E, the inliers and the cheirality test of the chosen (R, t)
+// A stopped pair's CTAs return at once.  Compiled with -fmad=false: oracle/lo_pose_oracle.py takes the same steps.
+#include <stdint.h>
+
+#include "geo_lm.cuh"
+#include "lg_internal.h"
+#include "pose_common.cuh"
+
+namespace {
+
+// recoverPose's cheirality test of the calibrated point (x, y) <-> (u, v) for P1 = [R | t] (header step P7).
+// pose_kernel (pose_api.cu) writes the same steps inline: routed through this function its register allocation
+// changes.
+__device__ __forceinline__ bool cheirality_pass(const double (&P1)[3][4], double x, double y, double u, double v,
+                                                double distance) {
+  double r[4][4] = {{-1.0, 0.0, x, 0.0}, {0.0, -1.0, y, 0.0}};
+  for (int j = 0; j < 4; ++j) {
+    r[2][j] = u * P1[2][j] - P1[0][j];
+    r[3][j] = v * P1[2][j] - P1[1][j];
+  }
+  double Nm[4][4], Q[4];
+  for (int i = 0; i < 4; ++i)
+    for (int j = 0; j < 4; ++j) Nm[i][j] = ((r[0][i] * r[0][j] + r[1][i] * r[1][j]) + r[2][i] * r[2][j]) + r[3][i] * r[3][j];
+  smallest_eigvec<4>(Nm, Q);
+  const double X = Q[0] / Q[3], Y = Q[1] / Q[3], Z = Q[2] / Q[3];
+  const double z1 = ((P1[2][0] * X + P1[2][1] * Y) + P1[2][2] * Z) + P1[2][3];
+  return Q[2] * Q[3] > 0.0 && Z < distance && z1 > 0.0 && z1 < distance;
+}
+
+// [R | t] of a row-major R and t
+__device__ __forceinline__ void projection34(const double* R, const double* tv, double (&P1)[3][4]) {
+  for (int i = 0; i < 3; ++i) {
+    for (int j = 0; j < 3; ++j) P1[i][j] = R[3 * i + j];
+    P1[i][3] = tv[i];
+  }
+}
+
+constexpr int LO_TERMS = 21;  // J^T J upper triangle (15), J^T r (5), truncated cost
+constexpr unsigned long long LO_COUNT_ONE = 1ull << 40;  // a score sum's count field (header GEO_LO_MAX_MATCHES)
+constexpr unsigned long long LO_SCORE_MASK = LO_COUNT_ONE - 1;
+
+struct LoPair {
+  double R[9], t[3];         // the pair's model
+  unsigned long long score;  // its L3 score
+  int count;                 // its inliers
+  int hr;                    // h * 16 + r of the solution that seeded it; -1: none yet
+  int nlo;                   // local optimisations adopted
+};
+
+struct LoWs {
+  LoPair* pair;             // [B]
+  unsigned long long* acc;  // [B, GEO_CHUNK, SOLS] count << 40 | score of the current chunk's solutions
+};
+
+size_t lo_carve(char* base, int B, int M, PoseWs* w, LoWs* l) {
+  WsBump b{base, carve(base, B, M, w)};
+  l->pair = b.take<LoPair>(B);
+  l->acc = b.take<unsigned long long>((size_t)B * GEO_CHUNK * SOLS);
+  return b.bytes();
+}
+
+struct LoArgs {
+  PoseArgs p;
+  LoWs l;
+  int32_t* num_lo;
+  int64_t* cost;
+};
+
+// L3's per-point term of one fp32 error, with the count in bit 40
+__device__ __forceinline__ unsigned long long lo_term(float e, float thr2, float w) {
+  return e < thr2 ? LO_COUNT_ONE + (unsigned)(e * w) : (unsigned long long)GEO_LO_QSCALE;
+}
+
+// Column-wise cross product: column j of out is a x M[:, j] ([a]x M), M and out row-major
+__device__ __forceinline__ void cross_columns(const double* a, const double* M, double* out) {
+  for (int j = 0; j < 3; ++j) {
+    const double col[3] = {M[j], M[3 + j], M[6 + j]};
+    double c[3];
+    cross3(a, col, c);
+    for (int i = 0; i < 3; ++i) out[3 * i + j] = c[i];
+  }
+}
+
+__device__ void tangent_basis(const double* t, double* b1, double* b2) {
+  int m = 0;
+  for (int i = 1; i < 3; ++i)
+    if (fabs(t[i]) < fabs(t[m])) m = i;
+  const double e[3] = {m == 0 ? 1.0 : 0.0, m == 1 ? 1.0 : 0.0, m == 2 ? 1.0 : 0.0};
+  double c[3];
+  cross3(t, e, c);
+  const double nc = sqrt((c[0] * c[0] + c[1] * c[1]) + c[2] * c[2]);
+  for (int i = 0; i < 3; ++i) b1[i] = c[i] / nc;
+  cross3(t, b1, b2);
+}
+
+// Shared state of one pair's CTA in the LO and final kernels
+struct LoShared {
+  double red[LO_TERMS][RED];
+  double pose[12], cand[12];           // R, t of the model being refined and of the LM step's candidate
+  double sums[LO_TERMS], csum[LO_TERMS];
+  double E[9], dE[5][9];               // [t]x R and its derivatives at the pose being summed
+  double Rs[2][9], ts[3];              // P7 candidates
+  double Eo[9];                        // the scaled E of the last re-scored pose
+  float fm[9];                         // a model rounded to float
+  unsigned long long key, score;
+  int good[4], count, step_ok;
+};
+
+// The terms' fixed-order sums (header step 2), all LO_TERMS at once; every thread of the CTA calls it
+__device__ void lo_tree_sums(const double* acc, LoShared& s, double* out, int tid) {
+  for (int i = 0; i < LO_TERMS; ++i) s.red[i][tid] = acc[i];
+  __syncthreads();
+  for (int h = RED / 2; h > 0; h >>= 1) {
+    if (tid < h)
+      for (int i = 0; i < LO_TERMS; ++i) s.red[i][tid] = s.red[i][tid] + s.red[i][tid + h];
+    __syncthreads();
+  }
+  if (tid < LO_TERMS) out[tid] = s.red[tid][0];
+  __syncthreads();
+}
+
+__device__ __forceinline__ void lo_epipolar(const double* E, double x, double y, double u, double v, double* a0, double* a1,
+                                            double* b0, double* b1, double* d) {
+  *a0 = (E[0] * x + E[1] * y) + E[2];
+  *a1 = (E[3] * x + E[4] * y) + E[5];
+  const double a2 = (E[6] * x + E[7] * y) + E[8];
+  *d = (u * *a0 + v * *a1) + a2;
+  *b0 = (E[0] * u + E[3] * v) + E[6];
+  *b1 = (E[1] * u + E[4] * v) + E[7];
+}
+
+// The LO_TERMS sums at pose (R, t) (header step L7) into out
+__device__ void lo_terms(LoShared& s, const double* pose, const float4* pts, int n, double thr2, double* out, int tid) {
+  if (tid == 0) {
+    const double* R = pose;
+    const double* t = pose + 9;
+    cross_columns(t, R, s.E);
+    for (int k = 0; k < 3; ++k) {
+      const double e[3] = {k == 0 ? 1.0 : 0.0, k == 1 ? 1.0 : 0.0, k == 2 ? 1.0 : 0.0};
+      double G[9];
+      cross_columns(e, R, G);
+      cross_columns(t, G, s.dE[k]);
+    }
+    double b1[3], b2[3];
+    tangent_basis(t, b1, b2);
+    cross_columns(b1, R, s.dE[3]);
+    cross_columns(b2, R, s.dE[4]);
+  }
+  __syncthreads();
+  double acc[LO_TERMS];
+#pragma unroll
+  for (int i = 0; i < LO_TERMS; ++i) acc[i] = 0.0;
+  for (int k = tid; k < n; k += RED) {
+    const float4 p = pts[k];
+    const double x = p.x, y = p.y, u = p.z, v = p.w;
+    double a0, a1, b0, b1, d;
+    lo_epipolar(s.E, x, y, u, v, &a0, &a1, &b0, &b1, &d);
+    const double den = ((a0 * a0 + a1 * a1) + b0 * b0) + b1 * b1;
+    const double err = (d * d) / den;
+    const bool in = err < thr2;
+    acc[20] = acc[20] + (in ? err : thr2);
+    if (!in) continue;
+    const double sq = sqrt(den);
+    const double r = d / sq;
+    double J[5];
+#pragma unroll
+    for (int q = 0; q < 5; ++q) {
+      double da0, da1, db0, db1, dd;
+      lo_epipolar(s.dE[q], x, y, u, v, &da0, &da1, &db0, &db1, &dd);
+      const double dden = ((a0 * da0 + a1 * da1) + b0 * db0) + b1 * db1;
+      J[q] = (dd - d * dden / den) / sq;
+    }
+    int e = 0;
+#pragma unroll
+    for (int i = 0; i < 5; ++i)
+#pragma unroll
+      for (int j = i; j < 5; ++j, ++e) acc[e] = acc[e] + J[i] * J[j];
+#pragma unroll
+    for (int i = 0; i < 5; ++i) acc[15 + i] = acc[15 + i] + J[i] * r;
+  }
+  lo_tree_sums(acc, s, out, tid);
+}
+
+// R' = Q(d0..2) R, t' = normalize(t + d3 b1 + d4 b2) (header step L7)
+__device__ void lo_update(const double* pose, const double* d, double* out) {
+  double Q[9], b1[3], b2[3], v[3];
+  quat_rotation(d, Q);
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 3; ++j) out[3 * i + j] = Q[3 * i] * pose[j] + Q[3 * i + 1] * pose[3 + j] + Q[3 * i + 2] * pose[6 + j];
+  tangent_basis(pose + 9, b1, b2);
+  for (int i = 0; i < 3; ++i) v[i] = (pose[9 + i] + d[3] * b1[i]) + d[4] * b2[i];
+  const double nv = sqrt((v[0] * v[0] + v[1] * v[1]) + v[2] * v[2]);
+  for (int i = 0; i < 3; ++i) out[9 + i] = v[i] / nv;
+}
+
+// steps LM steps from s.pose, in place (header step L7); every thread of the CTA calls it
+__device__ void lo_refine(LoShared& s, const float4* pts, int n, double thr2, int steps, int tid) {
+  lo_terms(s, s.pose, pts, n, thr2, s.sums, tid);
+  double lam = GEO_LO_LAMBDA0;  // every thread keeps the same schedule
+  for (int it = 0; it < steps; ++it) {
+    if (tid == 0) {
+      double d[5];
+      s.step_ok = lm_solve<5>(s.sums, s.sums + 15, lam, d);
+      if (s.step_ok) lo_update(s.pose, d, s.cand);
+    }
+    __syncthreads();
+    if (!s.step_ok) {
+      lam = lam * 10.0;
+      __syncthreads();
+      continue;
+    }
+    lo_terms(s, s.cand, pts, n, thr2, s.csum, tid);
+    const bool better = s.csum[20] < s.sums[20];
+    __syncthreads();
+    if (better) {
+      if (tid < 12) s.pose[tid] = s.cand[tid];
+      if (tid < LO_TERMS) s.sums[tid] = s.csum[tid];
+      lam = lam / 10.0;
+    } else {
+      lam = lam * 10.0;
+    }
+    __syncthreads();
+  }
+}
+
+// L3 score and count of E = [t]x R of pose, scaled as P3 (s.Eo) and rounded to float (s.fm)
+__device__ void lo_rescore(LoShared& s, const double* pose, const float4* pts, int n, float thr2, int tid) {
+  if (tid == 0) {
+    cross_columns(pose + 9, pose, s.Eo);
+    unit_scale(s.Eo);
+    for (int i = 0; i < 9; ++i) s.fm[i] = (float)s.Eo[i];
+    s.score = 0;
+  }
+  __syncthreads();
+  const float w = (float)GEO_LO_QSCALE / thr2;
+  unsigned long long acc = 0;
+  for (int k = tid; k < n; k += RED) acc += lo_term(sampson(s.fm, pts[k]), thr2, w);
+  if (acc) atomicAdd(&s.score, acc);
+  __syncthreads();
+}
+
+__global__ void __launch_bounds__(GEO_CHUNK, 1) lo_hyp_kernel(LoArgs a, int c) {
+  const int b = blockIdx.x, t = threadIdx.x;
+  if (c == 0 && t == 0) {
+    LoPair& L = a.l.pair[b];
+    L.score = 0;
+    L.count = 0;
+    L.hr = -1;
+    L.nlo = 0;
+  }
+  const PosePair& P = a.p.w.pair[b];
+  const int h = c * GEO_CHUNK + t;
+  int ns = 0;
+  int id[S];
+  if (P.stop == 0 && h < a.p.max_iters && geo_sample(a.p.seed, h, P.n, S, id) == S) {
+    double sol[SOLS][9];
+    ns = five_point(a.p.w.pts + (long)b * a.p.M, id, sol);
+    float* hm = a.p.w.hyp + ((long)b * GEO_CHUNK + t) * SOLS * 9;
+    for (int r = 0; r < ns; ++r) {
+      for (int i = 0; i < 9; ++i) hm[r * 9 + i] = (float)sol[r][i];
+      a.l.acc[((long)b * GEO_CHUNK + t) * SOLS + r] = 0;
+    }
+  }
+  a.p.w.nsol[(long)b * GEO_CHUNK + t] = ns;
+}
+
+__global__ void __launch_bounds__(GEO_CHUNK) lo_score_kernel(LoArgs a) {
+  const int b = blockIdx.y, split = blockIdx.x, t = threadIdx.x;
+  const PosePair& P = a.p.w.pair[b];
+  if (P.stop) return;
+  const int lo = (int)((long)P.n * split / gridDim.x), hi = (int)((long)P.n * (split + 1) / gridDim.x);
+  const int ns = a.p.w.nsol[(long)b * GEO_CHUNK + t];
+  const float* hm = a.p.w.hyp + ((long)b * GEO_CHUNK + t) * SOLS * 9;
+  const float thr2 = P.thr2;
+  const float w = (float)GEO_LO_QSCALE / thr2;
+  float g[SOLS][9];
+  unsigned long long k[SOLS];
+#pragma unroll
+  for (int r = 0; r < SOLS; ++r) {
+    k[r] = 0;
+#pragma unroll
+    for (int i = 0; i < 9; ++i) g[r][i] = r < ns ? hm[r * 9 + i] : 0.f;
+  }
+  const float4* pts = a.p.w.pts + (long)b * a.p.M;
+  __shared__ float4 tile[TILE];
+  for (int base = lo; base < hi; base += TILE) {
+    const int m = min(TILE, hi - base);
+    __syncthreads();
+    for (int i = t; i < m; i += GEO_CHUNK) tile[i] = pts[base + i];
+    __syncthreads();
+    for (int i = 0; i < m; ++i) {
+      const float4 p = tile[i];
+#pragma unroll
+      for (int r = 0; r < SOLS; ++r)
+        if (r < ns) k[r] += lo_term(sampson(g[r], p), thr2, w);
+    }
+  }
+#pragma unroll
+  for (int r = 0; r < SOLS; ++r)
+    if (r < ns && k[r]) atomicAdd(a.l.acc + ((long)b * GEO_CHUNK + t) * SOLS + r, k[r]);
+}
+
+// P7's choice among the candidates of s.fm (widened) on s.fm's inliers, into s.pose; every thread calls it
+__device__ void lo_choose_pose(LoShared& s, const float4* pts, int n, float thr2, double distance, int tid) {
+  if (tid == 0) {
+    double E[9];
+    for (int i = 0; i < 9; ++i) E[i] = s.fm[i];
+    pose_candidates(E, s.Rs, s.ts);
+  }
+  if (tid < 4) s.good[tid] = 0;
+  __syncthreads();
+  int cnt[4] = {0, 0, 0, 0};
+  for (int k = tid; k < n; k += RED) {
+    const float4 p = pts[k];
+    if (!(sampson(s.fm, p) < thr2)) continue;
+    for (int c = 0; c < 4; ++c) {
+      const double sg = c < 2 ? 1.0 : -1.0;
+      const double tv[3] = {sg * s.ts[0], sg * s.ts[1], sg * s.ts[2]};
+      double P1[3][4];
+      projection34(s.Rs[c & 1], tv, P1);
+      cnt[c] += cheirality_pass(P1, p.x, p.y, p.z, p.w, distance);
+    }
+  }
+  for (int c = 0; c < 4; ++c)
+    if (cnt[c]) atomicAdd(&s.good[c], cnt[c]);
+  __syncthreads();
+  int best = 0;
+  for (int c = 1; c < 4; ++c)
+    if (s.good[c] > s.good[best]) best = c;
+  if (tid < 9) s.pose[tid] = s.Rs[best & 1][tid];
+  if (tid < 3) s.pose[9 + tid] = (best < 2 ? 1.0 : -1.0) * s.ts[tid];
+  __syncthreads();
+}
+
+// After chunk c: the chunk's best solution, the local optimisation when it beats the pair's model, the stop
+__global__ void __launch_bounds__(RED, 1) lo_kernel(LoArgs a, int c) {
+  const int b = blockIdx.x, t = threadIdx.x;
+  PosePair& P = a.p.w.pair[b];
+  if (P.stop) return;
+  LoPair& L = a.l.pair[b];
+  __shared__ LoShared s;
+  if (t == 0) s.key = ~0ull;
+  __syncthreads();
+  if (t < GEO_CHUNK) {
+    const int ns = a.p.w.nsol[(long)b * GEO_CHUNK + t];
+    const unsigned h = c * GEO_CHUNK + t;
+    for (int r = 0; r < ns; ++r) {
+      const unsigned long long v = a.l.acc[((long)b * GEO_CHUNK + t) * SOLS + r];
+      atomicMin(&s.key, (v & LO_SCORE_MASK) << 28 | (h * 16u + (unsigned)r));
+    }
+  }
+  __syncthreads();
+  const unsigned long long key = s.key;
+  const float4* pts = a.p.w.pts + (long)b * a.p.M;
+  if (key != ~0ull && (L.hr < 0 || (key >> 28) < L.score)) {
+    const unsigned hr = (unsigned)(key & 0xfffffffu);
+    const long slot = (long)b * GEO_CHUNK + (hr >> 4) - c * GEO_CHUNK;
+    if (t < 9) s.fm[t] = a.p.w.hyp[(slot * SOLS + (hr & 15)) * 9 + t];
+    __syncthreads();
+    lo_choose_pose(s, pts, P.n, P.thr2, a.p.distance, t);
+    if (t == 0) {
+      for (int i = 0; i < 9; ++i) L.R[i] = s.pose[i];
+      for (int i = 0; i < 3; ++i) L.t[i] = s.pose[9 + i];
+      L.score = key >> 28;
+      L.count = (int)(a.l.acc[slot * SOLS + (hr & 15)] >> 40);
+      L.hr = (int)hr;
+    }
+    lo_refine(s, pts, P.n, (double)P.thr2, GEO_LO_STEPS, t);
+    lo_rescore(s, s.pose, pts, P.n, P.thr2, t);
+    if (t == 0 && (s.score & LO_SCORE_MASK) < L.score) {
+      for (int i = 0; i < 9; ++i) L.R[i] = s.pose[i];
+      for (int i = 0; i < 3; ++i) L.t[i] = s.pose[9 + i];
+      L.score = s.score & LO_SCORE_MASK;
+      L.count = (int)(s.score >> 40);
+      L.nlo = L.nlo + 1;
+    }
+  }
+  if (t == 0) {
+    const int drawn = min((c + 1) * GEO_CHUNK, a.p.max_iters);
+    const int cnt = L.hr >= 0 ? L.count : 0;
+    P.drawn = drawn;
+    P.stop = drawn >= a.p.max_iters ||
+             drawn >= update_num_iters(a.p.confidence, 1.0 - (double)cnt / P.n, S, a.p.max_iters);
+  }
+}
+
+// Final refinement and the outputs (header steps L6, L8)
+__global__ void __launch_bounds__(RED, 1) lo_final_kernel(LoArgs a) {
+  const int b = blockIdx.x, t = threadIdx.x;
+  const PosePair& P = a.p.w.pair[b];
+  const LoPair& L = a.l.pair[b];
+  const GeoPoseOutputs& o = a.p.out;
+  uint8_t* inl = o.inliers + (long)b * a.p.M;
+  uint8_t* pinl = o.pose_inliers + (long)b * a.p.M;
+  for (int i = t; i < a.p.M; i += RED) inl[i] = pinl[i] = 0;
+  if (!P.ok || L.hr < 0) {
+    if (t < 9) o.E[(long)b * 9 + t] = o.R[(long)b * 9 + t] = 0.0;
+    if (t < 3) o.t[(long)b * 3 + t] = 0.0;
+    if (t == 0) {
+      o.num_inliers[b] = o.num_pose_inliers[b] = 0;
+      o.success[b] = 0;
+      o.best_hypothesis[b] = o.best_solution[b] = -1;
+      o.num_hypotheses[b] = P.drawn;
+      a.num_lo[b] = 0;
+      a.cost[b] = 0;
+    }
+    return;
+  }
+  __shared__ LoShared s;
+  const float4* pts = a.p.w.pts + (long)b * a.p.M;
+  const int* idx = a.p.w.idx + (long)b * a.p.M;
+  if (t < 9) s.pose[t] = L.R[t];
+  if (t < 3) s.pose[9 + t] = L.t[t];
+  __syncthreads();
+  lo_refine(s, pts, P.n, (double)P.thr2, GEO_LO_FINAL_STEPS, t);
+  lo_rescore(s, s.pose, pts, P.n, P.thr2, t);
+  const bool keep = (s.score & LO_SCORE_MASK) <= L.score;
+  __syncthreads();
+  if (!keep) {
+    if (t < 9) s.pose[t] = L.R[t];
+    if (t < 3) s.pose[9 + t] = L.t[t];
+    __syncthreads();
+    lo_rescore(s, s.pose, pts, P.n, P.thr2, t);
+  }
+  if (t == 0) s.count = 0;
+  __syncthreads();
+  int cnt = 0;
+  double P1[3][4];
+  projection34(s.pose, s.pose + 9, P1);
+  for (int k = t; k < P.n; k += RED) {
+    const float4 p = pts[k];
+    if (!(sampson(s.fm, p) < P.thr2)) continue;
+    inl[idx[k]] = 1;
+    if (cheirality_pass(P1, p.x, p.y, p.z, p.w, a.p.distance)) {
+      pinl[idx[k]] = 1;
+      ++cnt;
+    }
+  }
+  if (cnt) atomicAdd(&s.count, cnt);
+  __syncthreads();
+  if (t < 9) {
+    o.E[(long)b * 9 + t] = s.Eo[t];
+    o.R[(long)b * 9 + t] = s.pose[t];
+  }
+  if (t < 3) o.t[(long)b * 3 + t] = s.pose[9 + t];
+  if (t == 0) {
+    o.num_inliers[b] = (int)(s.score >> 40);
+    o.num_pose_inliers[b] = s.count;
+    o.success[b] = 1;
+    o.best_hypothesis[b] = L.hr >> 4;
+    o.best_solution[b] = L.hr & 15;
+    o.num_hypotheses[b] = P.drawn;
+    a.num_lo[b] = L.nlo;
+    a.cost[b] = (int64_t)(s.score & LO_SCORE_MASK);
+  }
+}
+
+}  // namespace
+
+extern "C" size_t geo_lo_pose_workspace_bytes(int32_t B, int32_t M, int32_t) {
+  if (B < 0 || M < 0) return 0;
+  PoseWs w;
+  LoWs l;
+  return lo_carve(nullptr, B, M, &w, &l) + 256;
+}
+
+extern "C" int geo_relative_pose_lo(const GeoLoPoseConfig* cfg, const GeoPoseInputs* in, GeoLoPoseOutputs* out,
+                                    void* workspace, size_t workspace_bytes, void* stream_) {
+  if (!cfg || !in || !out) return lg_set_error("geo_relative_pose_lo: null argument");
+  if (cfg->abi_version != GEO_ABI_VERSION) return lg_set_error("geo_relative_pose_lo: ABI version mismatch");
+  if (cfg->max_iters < 1 || cfg->max_iters > GEO_MAX_ITERS)
+    return lg_set_error("geo_relative_pose_lo: max_iters outside [1, 2^24]");
+  if (!(cfg->threshold > 0.0) || !isfinite(cfg->threshold))
+    return lg_set_error("geo_relative_pose_lo: threshold must be positive");
+  if (!(cfg->confidence >= 0.0 && cfg->confidence <= 1.0))
+    return lg_set_error("geo_relative_pose_lo: confidence outside [0, 1]");
+  if (!(cfg->distance_threshold > 0.0) || !isfinite(cfg->distance_threshold))
+    return lg_set_error("geo_relative_pose_lo: distance_threshold must be positive");
+  if (in->B < 0 || in->M < 0 || in->N < 0) return lg_set_error("geo_relative_pose_lo: negative size");
+  if (in->M > GEO_LO_MAX_MATCHES) return lg_set_error("geo_relative_pose_lo: M above GEO_LO_MAX_MATCHES");
+  if (in->B == 0) return 0;
+  const GeoPoseOutputs& o = out->pose;
+  if (!o.E || !o.R || !o.t || !o.inliers || !o.num_inliers || !o.pose_inliers || !o.num_pose_inliers || !o.success ||
+      !o.best_hypothesis || !o.best_solution || !o.num_hypotheses || !out->num_local_optimizations || !out->cost)
+    return lg_set_error("geo_relative_pose_lo: null output");
+  if (!in->K0 || !in->K1) return lg_set_error("geo_relative_pose_lo: null intrinsics");
+  if (in->M > 0 && (!in->kpts0 || !in->matches0 || (in->N > 0 && !in->kpts1)))
+    return lg_set_error("geo_relative_pose_lo: null input");
+  if (!workspace || workspace_bytes < geo_lo_pose_workspace_bytes(in->B, in->M, cfg->max_iters))
+    return lg_set_error("geo_relative_pose_lo: workspace too small");
+  LoArgs a{};
+  lo_carve((char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255), in->B, in->M, &a.p.w, &a.l);
+  PoseArgs& p = a.p;
+  p.B = in->B; p.M = in->M; p.N = in->N;
+  p.max_iters = cfg->max_iters;
+  p.chunks = (cfg->max_iters + GEO_CHUNK - 1) / GEO_CHUNK;
+  p.seed = cfg->seed;
+  p.threshold = cfg->threshold;
+  p.confidence = cfg->confidence;
+  p.distance = cfg->distance_threshold;
+  p.kpts0 = in->kpts0; p.kpts1 = in->kpts1; p.matches0 = in->matches0;
+  p.K0 = in->K0; p.K1 = in->K1;
+  p.out = o;
+  a.num_lo = out->num_local_optimizations;
+  a.cost = out->cost;
+  // the score CTAs of geo_relative_pose
+  const int want = (2 * lg_num_sms() + p.B - 1) / p.B;
+  int splits = (p.M + 127) / 128;
+  if (splits > want) splits = want;
+  if (splits < 1) splits = 1;
+  const cudaStream_t stream = (cudaStream_t)stream_;
+  pose_prepare_kernel<<<p.B, 1024, 0, stream>>>(p);
+  LG_CHECK_LAUNCH();
+  for (int c = 0; c < p.chunks; ++c) {
+    lo_hyp_kernel<<<p.B, GEO_CHUNK, 0, stream>>>(a, c);
+    LG_CHECK_LAUNCH();
+    lo_score_kernel<<<dim3(splits, p.B), GEO_CHUNK, 0, stream>>>(a);
+    LG_CHECK_LAUNCH();
+    lo_kernel<<<p.B, RED, 0, stream>>>(a, c);
+    LG_CHECK_LAUNCH();
+  }
+  lo_final_kernel<<<p.B, RED, 0, stream>>>(a);
+  LG_CHECK_LAUNCH();
+  return 0;
+}

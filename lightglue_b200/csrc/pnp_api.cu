@@ -16,6 +16,7 @@
 
 #include "block_scan.cuh"
 #include "geo_common.cuh"
+#include "geo_lm.cuh"
 #include "lg_internal.h"
 #include "ws_bump.h"
 
@@ -430,49 +431,10 @@ __device__ void lm_partials(const double* K, const double* R, const double* t, c
   }
 }
 
-// delta of (J^T J, its diagonal times (1 + lam)) delta = -J^T r by Cholesky; false on a pivot <= 0 or a non-finite delta
-__device__ bool lm_solve(const double* Hu, const double* g, double lam, double* x) {
-  double A[6][6], L[6][6], yv[6];
-  for (int i = 0, e = 0; i < 6; ++i)
-    for (int j = i; j < 6; ++j, ++e) A[i][j] = A[j][i] = Hu[e];
-  for (int i = 0; i < 6; ++i) A[i][i] = A[i][i] * (1.0 + lam);
-  for (int j = 0; j < 6; ++j) {
-    double d = A[j][j];
-    for (int k = 0; k < j; ++k) d = d - L[j][k] * L[j][k];
-    if (!(d > 0.0)) return false;
-    L[j][j] = sqrt(d);
-    for (int i = j + 1; i < 6; ++i) {
-      double e = A[i][j];
-      for (int k = 0; k < j; ++k) e = e - L[i][k] * L[j][k];
-      L[i][j] = e / L[j][j];
-    }
-  }
-  for (int i = 0; i < 6; ++i) {
-    double e = -g[i];
-    for (int k = 0; k < i; ++k) e = e - L[i][k] * yv[k];
-    yv[i] = e / L[i][i];
-  }
-  bool fin = true;
-  for (int i = 5; i >= 0; --i) {
-    double e = yv[i];
-    for (int k = i + 1; k < 6; ++k) e = e - L[k][i] * x[k];
-    x[i] = e / L[i][i];
-    fin = fin && isfinite(x[i]);
-  }
-  return fin;
-}
-
 // R' = Q R, t' = Q t + d[3..5], Q of the unit quaternion (1, d[0..2] / 2) / norm
 __device__ void lm_update(const double* R, const double* t, const double* d, double* Rn, double* tn) {
-  double qw = 1.0, qx = d[0] * 0.5, qy = d[1] * 0.5, qz = d[2] * 0.5;
-  const double n = sqrt(qw * qw + qx * qx + qy * qy + qz * qz);
-  qw = qw / n;
-  qx = qx / n;
-  qy = qy / n;
-  qz = qz / n;
-  const double Q[9] = {1.0 - 2.0 * (qy * qy + qz * qz), 2.0 * (qx * qy - qw * qz), 2.0 * (qx * qz + qw * qy),
-                       2.0 * (qx * qy + qw * qz), 1.0 - 2.0 * (qx * qx + qz * qz), 2.0 * (qy * qz - qw * qx),
-                       2.0 * (qx * qz - qw * qy), 2.0 * (qy * qz + qw * qx), 1.0 - 2.0 * (qx * qx + qy * qy)};
+  double Q[9];
+  quat_rotation(d, Q);
   for (int i = 0; i < 3; ++i) {
     for (int j = 0; j < 3; ++j) Rn[3 * i + j] = Q[3 * i] * R[j] + Q[3 * i + 1] * R[3 + j] + Q[3 * i + 2] * R[6 + j];
     tn[i] = Q[3 * i] * t[0] + Q[3 * i + 1] * t[1] + Q[3 * i + 2] * t[2] + d[3 + i];
@@ -535,7 +497,7 @@ __global__ void __launch_bounds__(RED, 1) pnp_refit_kernel(PnpArgs a) {
     for (int it = 0; it < GEO_PNP_LM_STEPS; ++it) {
       if (t == 0) {
         double d[6];
-        step_ok = lm_solve(sums, sums + 21, lam, d);
+        step_ok = lm_solve<6>(sums, sums + 21, lam, d);
         if (step_ok) lm_update(pose[1], pose[1] + 9, d, cand, cand + 9);
       }
       __syncthreads();

@@ -1,8 +1,8 @@
-"""Geometric verification on the GPU: batched RANSAC homography, fundamental-matrix, relative-pose and absolute-pose
-estimation on the matcher's output (C ABI ``include/geometry_b200.h``, CUDA ``csrc/geo_api.cu``, ``csrc/pose_api.cu``
-and ``csrc/pnp_api.cu``).
+"""Geometric verification on the GPU: batched RANSAC homography, fundamental-matrix, relative-pose (plain and
+LO-RANSAC) and absolute-pose estimation on the matcher's output (C ABI ``include/geometry_b200.h``, CUDA
+``csrc/geo_api.cu``, ``csrc/pose_api.cu`` and ``csrc/pnp_api.cu``).
 
-All four functions take ``matches0`` [B, M] int64 exactly as ``LightGlue.forward``, ``PendingMatch.tensors`` and
+All five functions take ``matches0`` [B, M] int64 exactly as ``LightGlue.forward``, ``PendingMatch.tensors`` and
 ``match_ragged`` give it (-1 or any index outside [0, N) is unmatched), run every pair of the batch in one call on the
 current stream, and return device tensors of fixed shapes without synchronising with the host, so a call can follow a
 matcher forward with no read-back in between, or be captured in a CUDA graph.  Parameter names and defaults are those of
@@ -132,10 +132,36 @@ def estimate_relative_pose(kpts0: torch.Tensor, kpts1: torch.Tensor, matches0: t
     [B] bool; and the diagnostics ``best_hypothesis``, ``best_solution`` and ``num_hypotheses`` [B] int32.  A pair
     with fewer than 5 valid matches, an invalid K (a non-finite entry, fx or fy <= 0, or a bottom row other than
     [0, 0, 1]) or no non-degenerate sample has ``success`` False, zero E, R and t, and no inliers."""
+    return _relative_pose(False, kpts0, kpts1, matches0, K0, K1, ransac_reproj_threshold, max_iters, confidence,
+                          distance_threshold, seed)
+
+
+def estimate_relative_pose_lo(kpts0: torch.Tensor, kpts1: torch.Tensor, matches0: torch.Tensor, K0: torch.Tensor,
+                              K1: torch.Tensor | None = None, ransac_reproj_threshold: float = 1.0, max_iters: int = 1000,
+                              confidence: float = 0.999, distance_threshold: float = 50.0, seed: int = 0) -> dict:
+    """LO-RANSAC relative pose per pair: the samples and five-point solutions of ``estimate_relative_pose``, scored by
+    a truncated (MSAC) Sampson cost, with Levenberg-Marquardt local optimisation of (R, t) after each chunk of 256
+    samples that improves the best model, and a final Levenberg-Marquardt refinement.  The accuracy of PoseLib's and
+    OpenCV's USAC LO-RANSAC, on the GPU; ``estimate_relative_pose`` stays the one that follows ``cv2.RANSAC``.
+    Arguments and defaults are ``estimate_relative_pose``'s, so the two compare like for like.
+
+    Returns the keys of ``estimate_relative_pose`` (E = [t]x R of the final pose, unit Frobenius norm with its largest
+    entry positive; ``inliers`` the points within the threshold of that E; ``best_hypothesis`` and ``best_solution``
+    the five-point solution the final model grew from) plus ``num_local_optimizations`` [B] int32, the local
+    optimisations whose model was adopted, and ``cost`` [B] int64, the final model's integer MSAC score.  Failures are
+    those of ``estimate_relative_pose``, with ``num_local_optimizations`` and ``cost`` 0."""
+    return _relative_pose(True, kpts0, kpts1, matches0, K0, K1, ransac_reproj_threshold, max_iters, confidence,
+                          distance_threshold, seed)
+
+
+def _relative_pose(lo: bool, kpts0, kpts1, matches0, K0, K1, ransac_reproj_threshold, max_iters, confidence,
+                   distance_threshold, seed) -> dict:
     _check_inputs(kpts0, kpts1, matches0)
     _check_params(ransac_reproj_threshold, max_iters, confidence, seed)
     if not float(distance_threshold) > 0.0 or float(distance_threshold) == float("inf"):
         raise ValueError(f"distance_threshold={distance_threshold!r}: a positive number")
+    if lo and kpts0.shape[1] > _cabi.GEO_LO_MAX_MATCHES:
+        raise ValueError(f"kpts0 {tuple(kpts0.shape)}: at most {_cabi.GEO_LO_MAX_MATCHES} rows per pair")
     device = kpts0.device
     b, m, n = kpts0.shape[0], kpts0.shape[1], kpts1.shape[1]
     k0 = _intrinsics("K0", K0, b, device)
@@ -150,19 +176,28 @@ def estimate_relative_pose(kpts0: torch.Tensor, kpts1: torch.Tensor, matches0: t
               "num_inliers": ((b,), i32), "pose_inliers": ((b, m), bl), "num_pose_inliers": ((b,), i32),
               "success": ((b,), bl), "best_hypothesis": ((b,), i32), "best_solution": ((b,), i32),
               "num_hypotheses": ((b,), i32)}
-    out = {k: torch.empty(*shapes[k][0], dtype=shapes[k][1], device=device) for k in keys}
+    if lo:
+        shapes.update(num_local_optimizations=((b,), i32), cost=((b,), torch.int64))
+    out = {k: torch.empty(*shape, dtype=dtype, device=device) for k, (shape, dtype) in shapes.items()}
     if b == 0:
         return out
     with torch.cuda.device(device):
         lib = _cabi.load()
-        ws = torch.empty(lib.geo_pose_workspace_bytes(b, m, max_iters), dtype=torch.uint8, device=device)
-        cfg = _cabi.GeoPoseConfig(_cabi.GEO_ABI_VERSION, max_iters, seed, 0, float(ransac_reproj_threshold),
-                                  float(confidence), float(distance_threshold))
+        args = (max_iters, seed, 0, float(ransac_reproj_threshold), float(confidence), float(distance_threshold))
         ins = _cabi.GeoPoseInputs(b, m, n, p0.data_ptr(), p1.data_ptr(), m0.data_ptr(), k0.data_ptr(), k1.data_ptr())
         outs = _cabi.GeoPoseOutputs(*(out[k].data_ptr() for k in keys))
         stream = torch.cuda.current_stream(device).cuda_stream
-        _cabi.check(lib.geo_relative_pose(C.byref(cfg), C.byref(ins), C.byref(outs), ws.data_ptr(), ws.numel(), stream),
-                    "geo_relative_pose")
+        if lo:
+            ws = torch.empty(lib.geo_lo_pose_workspace_bytes(b, m, max_iters), dtype=torch.uint8, device=device)
+            cfg = _cabi.GeoLoPoseConfig(_cabi.GEO_ABI_VERSION, *args)
+            louts = _cabi.GeoLoPoseOutputs(outs, out["num_local_optimizations"].data_ptr(), out["cost"].data_ptr())
+            _cabi.check(lib.geo_relative_pose_lo(C.byref(cfg), C.byref(ins), C.byref(louts), ws.data_ptr(), ws.numel(),
+                                                 stream), "geo_relative_pose_lo")
+        else:
+            ws = torch.empty(lib.geo_pose_workspace_bytes(b, m, max_iters), dtype=torch.uint8, device=device)
+            cfg = _cabi.GeoPoseConfig(_cabi.GEO_ABI_VERSION, *args)
+            _cabi.check(lib.geo_relative_pose(C.byref(cfg), C.byref(ins), C.byref(outs), ws.data_ptr(), ws.numel(),
+                                              stream), "geo_relative_pose")
     return out
 
 
