@@ -170,6 +170,49 @@
  *     launch sequence is fixed and the result is deterministic; the score is quantised to integers; there is no
  *     non-minimal refit inside the LO and no PROSAC ordering.
  *
+ * LO-RANSAC homography (geo_homography_lo; oracle/lo_homography_oracle.py restates it bit for bit): the outputs of
+ * geo_estimate for GEO_HOMOGRAPHY, from an MSAC-scored four-point RANSAC with Levenberg-Marquardt local optimisation,
+ * on the schedule of L1-L8.  Expressions evaluate left to right as written; every multiply and add rounds on its own.
+ *
+ * LH1. Compaction and Hartley normalisation exactly as steps 1-2; thr2 = (float)(threshold * threshold).
+ *      M <= GEO_LO_MAX_MATCHES.
+ * LH2. Sampling and the four-point DLT exactly as steps 3-4, with OpenCV's collinearity and orientation rejection and
+ *      the same scale: with the same seed both estimators draw the same samples and solve the same hypotheses.
+ * LH3. MSAC score, per hypothesis, from step 5's fp32 forward transfer error err (the model rounded to float):
+ *      w = GEO_LO_QSCALE / thr2 in fp32, q = err < thr2 ? (uint32)(err * w) (fp32 product, truncated) : GEO_LO_QSCALE,
+ *      so a non-finite err (a point mapped to infinity, w = 1/0) scores as an outlier.  score = sum of q over the
+ *      points in uint64, count = the number of err < thr2.  Lower is better; ties go to the lowest h.
+ * LH4. Local optimisation, after every chunk of GEO_CHUNK samples, once per pair.  Chunk c's best hypothesis (lowest
+ *      (score, h)) is taken when the pair has no model yet or its score is strictly below the model's score; else
+ *      nothing happens.  Taken, its double H of step 4 becomes the pair's model (score, count, h).  Then GEO_LO_STEPS
+ *      LM steps (LH7) from it give Hn', whose pixel model H' = T1^-1 Hn' T0 scaled as step 4 is scored as LH3; with a
+ *      strictly lower score H' replaces the model (keeping h) and num_local_optimizations counts one.
+ * LH5. Stopping as step 6 with s = 4 from the model's count (a local optimisation's count included).
+ * LH6. Final refinement: GEO_LO_FINAL_STEPS LM steps from the model, kept unless their LH3 score is higher.
+ * LH7. LM, in double, on the normalised model at unit Frobenius norm: from a pixel H (row-major, as everywhere here),
+ *      Hn = (T1 H) T0^-1 (3x3 products as step 4; T1 = [[s1, 0, -(s1*cx1)], [0, s1, -(s1*cy1)], [0, 0, 1]],
+ *      T0^-1 = [[1/s0, 0, cx0], [0, 1/s0, cy0], [0, 0, 1]]) divided by the square root of its running sum of squares.
+ *      Tangent basis at Hn: m the first index of least |Hn_m|, v = e_m - Hn (v_i = (i == m ? 1.0 : 0.0) - Hn_i),
+ *      vv = running sum of v_i*v_i, c = 2.0 / vv; the reflection I - c v v^T maps e_m to Hn, and its columns j != m
+ *      in ascending j are b_0..b_7: b_k,i = (i == j ? 1.0 : 0.0) - c*v_i*v_j.  The parameters delta0..7 move Hn to
+ *      Hn' = x / sqrt(running sum of x_i*x_i) with x_i = Hn_i + delta0*b_0,i + ... + delta7*b_7,i (left to right).
+ *      Residuals in pixels, on the compacted floats widened: with h = (T1^-1 Hn) T0 unscaled (T1^-1 as step 4),
+ *      w = 1.0 / ((h6*x0 + h7*y0) + h8), px = ((h0*x0 + h1*y0) + h2) * w, py = ((h3*x0 + h4*y0) + h5) * w,
+ *      dx = x1 - px, dy = y1 - py, err = dx*dx + dy*dy; an inlier at this model has err < (double)thr2.  With
+ *      g = (T1^-1 b_k) T0 and da = (g0*x0 + g1*y0) + g2, db, dc likewise (g3..g5, g6..g8): jx_k = -((da - px*dc) * w),
+ *      jy_k = -((db - py*dc) * w).  The 36 terms jx_i*jx_j + jy_i*jy_j (i <= j in row order) and the 8 terms
+ *      jx_i*dx + jy_i*dy over the inliers, and the truncated cost (err for an inlier, else (double)thr2) over every
+ *      point, are each summed in the order of step 2.  A step solves the 8x8 system of A7 (damping, Cholesky,
+ *      right-hand side -J^T r), lambda starts at GEO_LO_LAMBDA0, and the step is taken only if the truncated cost at
+ *      Hn', with its own inliers, is strictly lower: A7's schedule.
+ * LH8. Outputs: model the final H (a hypothesis's H of step 4, or T1^-1 Hn T0 scaled as step 4); inliers the points
+ *      with err < thr2 under it rounded to float, num_inliers their number and cost its LH3 score; best_hypothesis the
+ *      hypothesis that seeded it; num_hypotheses the samples drawn.  A pair fails as step 7's failures (n < 4, a failed
+ *      normalisation, every sample degenerate), with num_local_optimizations and cost 0.  Deviations from PoseLib:
+ *      local optimisation runs at most once per chunk rather than at every new best, so the launch sequence is fixed
+ *      and the result is deterministic; the score is quantised to integers; there is no non-minimal (DLT) refit inside
+ *      the LO and no PROSAC ordering.
+ *
  * Absolute pose (geo_absolute_pose; oracle/pnp_oracle.py restates it bit for bit): the (R, t) of x_cam = R X + t that
  * maps the world points of image 1's keypoints into the query camera 0, OpenCV's rvec/tvec convention.  Expressions
  * below evaluate left to right as written (a + b + c is (a + b) + c); no step whose result must match bit for bit calls
@@ -367,6 +410,17 @@ typedef struct GeoLoPoseOutputs {
 LG_API size_t geo_lo_pose_workspace_bytes(int32_t B, int32_t M, int32_t max_iters);
 LG_API int geo_relative_pose_lo(const GeoLoPoseConfig* cfg, const GeoPoseInputs* in, GeoLoPoseOutputs* out,
                                 void* workspace, size_t workspace_bytes, void* stream);
+
+typedef struct GeoLoOutputs {
+  GeoOutputs geo;                    /* as geo_estimate's; model is H */
+  int32_t* num_local_optimizations;  /* [B] local optimisations whose model was adopted */
+  int64_t* cost;                     /* [B] LH3 score of the final model */
+} GeoLoOutputs;
+
+/* LO-RANSAC homography (steps LH1-LH8): cfg->model must be GEO_HOMOGRAPHY, in->M <= GEO_LO_MAX_MATCHES. */
+LG_API size_t geo_lo_homography_workspace_bytes(int32_t B, int32_t M, int32_t max_iters);
+LG_API int geo_homography_lo(const GeoConfig* cfg, const GeoInputs* in, GeoLoOutputs* out, void* workspace,
+                             size_t workspace_bytes, void* stream);
 
 #define GEO_PNP_MAX_SOLUTIONS 4
 #define GEO_PNP_COLLINEAR_EPS 1e-10

@@ -141,6 +141,10 @@ class GeoLoPoseOutputs(C.Structure):
     _fields_ = [("pose", GeoPoseOutputs), ("num_local_optimizations", C.c_void_p), ("cost", C.c_void_p)]
 
 
+class GeoLoOutputs(C.Structure):
+    _fields_ = [("geo", GeoOutputs), ("num_local_optimizations", C.c_void_p), ("cost", C.c_void_p)]
+
+
 class GeoPnpConfig(C.Structure):
     _fields_ = [
         ("abi_version", C.c_int32), ("max_iters", C.c_int32), ("seed", C.c_uint32), ("reserved", C.c_int32),
@@ -257,6 +261,9 @@ GEO_PROTOTYPES = {  # include/geometry_b200.h
     "geo_lo_pose_workspace_bytes": (_SZ, [_I32, _I32, _I32]),
     "geo_relative_pose_lo": (C.c_int, [C.POINTER(GeoLoPoseConfig), C.POINTER(GeoPoseInputs),
                                        C.POINTER(GeoLoPoseOutputs), _VP, _SZ, _VP]),
+    "geo_lo_homography_workspace_bytes": (_SZ, [_I32, _I32, _I32]),
+    "geo_homography_lo": (C.c_int, [C.POINTER(GeoConfig), C.POINTER(GeoInputs), C.POINTER(GeoLoOutputs), _VP, _SZ,
+                                    _VP]),
     "geo_pnp_workspace_bytes": (_SZ, [_I32, _I32, _I32]),
     "geo_absolute_pose": (C.c_int, [C.POINTER(GeoPnpConfig), C.POINTER(GeoPnpInputs), C.POINTER(GeoPnpOutputs), _VP,
                                     _SZ, _VP]),

@@ -1,5 +1,5 @@
 // Levenberg-Marquardt pieces shared by the absolute pose (pnp_api.cu, header step A7) and the LO-RANSAC relative pose
-// (pose_api.cu, header step L3), both compiled with -fmad=false.
+// and homography (lo_pose_api.cu and lo_homography_api.cu, header steps L7 and LH7), all compiled with -fmad=false.
 #pragma once
 #include <cuda_runtime.h>
 #include <math.h>

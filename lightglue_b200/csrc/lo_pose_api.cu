@@ -15,6 +15,7 @@
 
 #include "geo_lm.cuh"
 #include "lg_internal.h"
+#include "lo_common.cuh"
 #include "pose_common.cuh"
 
 namespace {
@@ -47,8 +48,6 @@ __device__ __forceinline__ void projection34(const double* R, const double* tv, 
 }
 
 constexpr int LO_TERMS = 21;  // J^T J upper triangle (15), J^T r (5), truncated cost
-constexpr unsigned long long LO_COUNT_ONE = 1ull << 40;  // a score sum's count field (header GEO_LO_MAX_MATCHES)
-constexpr unsigned long long LO_SCORE_MASK = LO_COUNT_ONE - 1;
 
 struct LoPair {
   double R[9], t[3];         // the pair's model
@@ -76,11 +75,6 @@ struct LoArgs {
   int32_t* num_lo;
   int64_t* cost;
 };
-
-// L3's per-point term of one fp32 error, with the count in bit 40
-__device__ __forceinline__ unsigned long long lo_term(float e, float thr2, float w) {
-  return e < thr2 ? LO_COUNT_ONE + (unsigned)(e * w) : (unsigned long long)GEO_LO_QSCALE;
-}
 
 // Column-wise cross product: column j of out is a x M[:, j] ([a]x M), M and out row-major
 __device__ __forceinline__ void cross_columns(const double* a, const double* M, double* out) {
@@ -116,19 +110,6 @@ struct LoShared {
   unsigned long long key, score;
   int good[4], count, step_ok;
 };
-
-// The terms' fixed-order sums (header step 2), all LO_TERMS at once; every thread of the CTA calls it
-__device__ void lo_tree_sums(const double* acc, LoShared& s, double* out, int tid) {
-  for (int i = 0; i < LO_TERMS; ++i) s.red[i][tid] = acc[i];
-  __syncthreads();
-  for (int h = RED / 2; h > 0; h >>= 1) {
-    if (tid < h)
-      for (int i = 0; i < LO_TERMS; ++i) s.red[i][tid] = s.red[i][tid] + s.red[i][tid + h];
-    __syncthreads();
-  }
-  if (tid < LO_TERMS) out[tid] = s.red[tid][0];
-  __syncthreads();
-}
 
 __device__ __forceinline__ void lo_epipolar(const double* E, double x, double y, double u, double v, double* a0, double* a1,
                                             double* b0, double* b1, double* d) {
@@ -189,7 +170,7 @@ __device__ void lo_terms(LoShared& s, const double* pose, const float4* pts, int
 #pragma unroll
     for (int i = 0; i < 5; ++i) acc[15 + i] = acc[15 + i] + J[i] * r;
   }
-  lo_tree_sums(acc, s, out, tid);
+  lo_tree_sums<LO_TERMS>(acc, s.red, out, tid);
 }
 
 // R' = Q(d0..2) R, t' = normalize(t + d3 b1 + d4 b2) (header step L7)

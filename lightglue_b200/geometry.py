@@ -1,8 +1,9 @@
-"""Geometric verification on the GPU: batched RANSAC homography, fundamental-matrix, relative-pose (plain and
-LO-RANSAC) and absolute-pose estimation on the matcher's output (C ABI ``include/geometry_b200.h``, CUDA
-``csrc/geo_api.cu``, ``csrc/pose_api.cu`` and ``csrc/pnp_api.cu``).
+"""Geometric verification on the GPU: batched RANSAC homography (plain and LO-RANSAC), fundamental-matrix,
+relative-pose (plain and LO-RANSAC) and absolute-pose estimation on the matcher's output (C ABI
+``include/geometry_b200.h``, CUDA ``csrc/geo_api.cu``, ``csrc/lo_homography_api.cu``, ``csrc/pose_api.cu``,
+``csrc/lo_pose_api.cu`` and ``csrc/pnp_api.cu``).
 
-All five functions take ``matches0`` [B, M] int64 exactly as ``LightGlue.forward``, ``PendingMatch.tensors`` and
+All six functions take ``matches0`` [B, M] int64 exactly as ``LightGlue.forward``, ``PendingMatch.tensors`` and
 ``match_ragged`` give it (-1 or any index outside [0, N) is unmatched), run every pair of the batch in one call on the
 current stream, and return device tensors of fixed shapes without synchronising with the host, so a call can follow a
 matcher forward with no read-back in between, or be captured in a CUDA graph.  Parameter names and defaults are those of
@@ -13,6 +14,7 @@ matcher forward with no read-back in between, or be captured in a CUDA graph.  P
 entry positive), ``inliers`` [B, M] bool, ``num_inliers`` [B] int32, ``success`` [B] bool, and the diagnostics
 ``best_hypothesis`` [B] int32 (-1 without one) and ``num_hypotheses`` [B] int32.  A failed pair (fewer valid matches than
 the sample size, 4 or 8, or no non-degenerate hypothesis) has ``success`` False, a zero model and no inliers.
+``find_homography_lo`` returns the keys of ``find_homography`` plus ``num_local_optimizations`` and ``cost``.
 """
 from __future__ import annotations
 
@@ -54,9 +56,12 @@ def _check_inputs(kpts0, kpts1, matches0, name1="kpts1", dim1=2) -> None:
         raise ValueError(f"kpts0, {name1} and matches0 must be on one device")
 
 
-def _estimate(kind: int, key: str, kpts0, kpts1, matches0, threshold, max_iters, confidence, seed) -> dict:
+def _estimate(kind: int, key: str, kpts0, kpts1, matches0, threshold, max_iters, confidence, seed,
+              lo: bool = False) -> dict:
     _check_inputs(kpts0, kpts1, matches0)
     _check_params(threshold, max_iters, confidence, seed)
+    if lo and kpts0.shape[1] > _cabi.GEO_LO_MAX_MATCHES:
+        raise ValueError(f"kpts0 {tuple(kpts0.shape)}: at most {_cabi.GEO_LO_MAX_MATCHES} rows per pair")
     device = kpts0.device
     b, m, n = kpts0.shape[0], kpts0.shape[1], kpts1.shape[1]
     k0 = kpts0.detach().to(torch.float32).contiguous()
@@ -70,18 +75,27 @@ def _estimate(kind: int, key: str, kpts0, kpts1, matches0, threshold, max_iters,
         "best_hypothesis": torch.empty(b, dtype=torch.int32, device=device),
         "num_hypotheses": torch.empty(b, dtype=torch.int32, device=device),
     }
+    if lo:
+        out["num_local_optimizations"] = torch.empty(b, dtype=torch.int32, device=device)
+        out["cost"] = torch.empty(b, dtype=torch.int64, device=device)
     if b == 0:
         return out
     with torch.cuda.device(device):
         lib = _cabi.load()
-        ws = torch.empty(lib.geo_workspace_bytes(b, m, max_iters), dtype=torch.uint8, device=device)
         cfg = _cabi.GeoConfig(_cabi.GEO_ABI_VERSION, kind, max_iters, seed, float(threshold), float(confidence))
         ins = _cabi.GeoInputs(b, m, n, k0.data_ptr(), k1.data_ptr(), m0.data_ptr())
         outs = _cabi.GeoOutputs(*(out[k].data_ptr() for k in (key, "inliers", "num_inliers", "success",
                                                                 "best_hypothesis", "num_hypotheses")))
         stream = torch.cuda.current_stream(device).cuda_stream
-        _cabi.check(lib.geo_estimate(C.byref(cfg), C.byref(ins), C.byref(outs), ws.data_ptr(), ws.numel(), stream),
-                    "geo_estimate")
+        if lo:
+            ws = torch.empty(lib.geo_lo_homography_workspace_bytes(b, m, max_iters), dtype=torch.uint8, device=device)
+            louts = _cabi.GeoLoOutputs(outs, out["num_local_optimizations"].data_ptr(), out["cost"].data_ptr())
+            _cabi.check(lib.geo_homography_lo(C.byref(cfg), C.byref(ins), C.byref(louts), ws.data_ptr(), ws.numel(),
+                                              stream), "geo_homography_lo")
+        else:
+            ws = torch.empty(lib.geo_workspace_bytes(b, m, max_iters), dtype=torch.uint8, device=device)
+            _cabi.check(lib.geo_estimate(C.byref(cfg), C.byref(ins), C.byref(outs), ws.data_ptr(), ws.numel(),
+                                         stream), "geo_estimate")
     return out
 
 
@@ -91,6 +105,23 @@ def find_homography(kpts0: torch.Tensor, kpts1: torch.Tensor, matches0: torch.Te
     ``ransac_reproj_threshold ** 2``.  Defaults of ``cv2.findHomography(method=cv2.RANSAC)``."""
     return _estimate(_cabi.GEO_HOMOGRAPHY, "H", kpts0, kpts1, matches0, ransac_reproj_threshold, max_iters, confidence,
                      seed)
+
+
+def find_homography_lo(kpts0: torch.Tensor, kpts1: torch.Tensor, matches0: torch.Tensor,
+                       ransac_reproj_threshold: float = 3.0, max_iters: int = 2000, confidence: float = 0.995,
+                       seed: int = 0) -> dict:
+    """LO-RANSAC homography per pair: the samples and four-point hypotheses of ``find_homography``, scored by a
+    truncated (MSAC) transfer cost, with Levenberg-Marquardt local optimisation of H after each chunk of 256 samples
+    that improves the best model, and a final Levenberg-Marquardt refinement.  The accuracy of PoseLib's and OpenCV's
+    USAC LO-RANSAC, on the GPU; ``find_homography`` stays the one that follows ``cv2.RANSAC``.  Arguments and defaults
+    are ``find_homography``'s, so the two compare like for like; at most 2**20 rows of ``matches0`` per pair.
+
+    Returns the keys of ``find_homography`` (``H`` the final model with H[2, 2] = 1; ``inliers`` the points within the
+    threshold of that H; ``best_hypothesis`` the sample the final model grew from) plus ``num_local_optimizations``
+    [B] int32, the local optimisations whose model was adopted, and ``cost`` [B] int64, the final model's integer MSAC
+    score.  Failures are those of ``find_homography``, with ``num_local_optimizations`` and ``cost`` 0."""
+    return _estimate(_cabi.GEO_HOMOGRAPHY, "H", kpts0, kpts1, matches0, ransac_reproj_threshold, max_iters, confidence,
+                     seed, lo=True)
 
 
 def find_fundamental(kpts0: torch.Tensor, kpts1: torch.Tensor, matches0: torch.Tensor, ransac_reproj_threshold: float = 3.0,
