@@ -7,8 +7,9 @@
  *
  * The algorithm, exactly (oracle/geometry_oracle.py restates it in numpy and matches it bit for bit):
  *
- * 1. Compaction.  Match i of pair b is valid when 0 <= matches0[b, i] < N.  The valid matches are compacted per pair in
- *    ascending i; n is their number.  Point k of the pair is (x0, y0) = kpts0[b, i_k], (x1, y1) = kpts1[b, matches0[b, i_k]].
+ * 1. Compaction.  Match i of pair b is valid when 0 <= matches0[b, i] < N and both kpts0[b, i] and
+ *    kpts1[b, matches0[b, i]] have finite coordinates (float): a match with a NaN or infinite keypoint is never an inlier
+ *    and does not count in n.  The valid matches are compacted per pair in ascending i; n is their number.  Point k of the pair is (x0, y0) = kpts0[b, i_k], (x1, y1) = kpts1[b, matches0[b, i_k]].
  *
  * 2. Hartley normalisation, per pair and image, in double.  Sums over the n points use one fixed order: 256 partial sums,
  *    partial t adds the terms t, t + 256, t + 512, ... in that order starting from 0.0, then a halving tree
@@ -71,7 +72,7 @@
  * Relative pose (geo_relative_pose; oracle/pose_oracle.py restates it bit for bit): an essential matrix E with
  * x1^T E x0 = 0 on calibrated coordinates, and the (R, t) of x1 = R x0 + t that recoverPose would choose.
  *
- * P1. Compaction as step 1.  K = [[fx, s, cx], [0, fy, cy], [0, 0, 1]] per pair and image (K[1][0] is not read);
+ * P1. Compaction as step 1 (a non-finite keypoint invalidates its match).  K = [[fx, s, cx], [0, fy, cy], [0, 0, 1]] per pair and image (K[1][0] is not read);
  *     y = ((double)v - cy) / fy, x = (((double)u - cx) - s*y) / fx, rounded to float.  The solver, the refit and the
  *     triangulation read these floats widened to double.  No Hartley step.  A K with a non-finite entry, fx <= 0, fy <= 0
  *     or a bottom row other than (0, 0, 1) fails its pair.  The threshold is t = threshold / f with
@@ -137,8 +138,9 @@
  * L2. Sampling and the five-point solutions exactly as P2 and P3: with the same seed both estimators draw the same
  *     samples and solve the same solutions.
  * L3. MSAC score, per solution of every sample, from P4's fp32 err (the solution rounded to float):
- *     w = GEO_LO_QSCALE / thr2 in fp32, q = err < thr2 ? (uint32)(err * w) (fp32 product, truncated) : GEO_LO_QSCALE.
- *     score = sum of q over the points in uint64 (exact in any order), count = the number of err < thr2.  Lower is
+ *     w = GEO_LO_QSCALE / thr2 in fp32; for err < thr2, q = 0 when err == 0, else
+ *     (uint32)fminf(err * w, GEO_LO_QSCALE) (fp32 product, truncated), so a subnormal thr2 with w = +inf stays
+ *     defined; q = GEO_LO_QSCALE otherwise.  score = sum of q over the points in uint64 (exact in any order), count = the number of err < thr2.  Lower is
  *     better; ties go to the lowest (sample h, solution r).
  * L4. Local optimisation, after every chunk of GEO_CHUNK samples, once per pair.  Chunk c's best solution (lowest
  *     (score, h, r)) is taken when the pair has no model yet or its score is strictly below the model's score; else
@@ -179,7 +181,7 @@
  * LH2. Sampling and the four-point DLT exactly as steps 3-4, with OpenCV's collinearity and orientation rejection and
  *      the same scale: with the same seed both estimators draw the same samples and solve the same hypotheses.
  * LH3. MSAC score, per hypothesis, from step 5's fp32 forward transfer error err (the model rounded to float):
- *      w = GEO_LO_QSCALE / thr2 in fp32, q = err < thr2 ? (uint32)(err * w) (fp32 product, truncated) : GEO_LO_QSCALE,
+ *      q as L3 (0 at err == 0, else (uint32)fminf(err * w, GEO_LO_QSCALE) for err < thr2, else GEO_LO_QSCALE),
  *      so a non-finite err (a point mapped to infinity, w = 1/0) scores as an outlier.  score = sum of q over the
  *      points in uint64, count = the number of err < thr2.  Lower is better; ties go to the lowest h.
  * LH4. Local optimisation, after every chunk of GEO_CHUNK samples, once per pair.  Chunk c's best hypothesis (lowest
@@ -218,8 +220,8 @@
  * below evaluate left to right as written (a + b + c is (a + b) + c); no step whose result must match bit for bit calls
  * cbrt, acos, atan2, sin, cos or pow: + - * / and sqrt round alike everywhere.
  *
- * A1. Compaction as step 1, where match i is valid when also the float point X = points3d1[b, matches0[b, i]] has three
- *     finite coordinates.  Point k is the pixel (u, v) = kpts0[b, i_k] and the world point X_k, both float.
+ * A1. Compaction as step 1, where match i is valid when the pixel kpts0[b, i] has two and the float point
+ *     X = points3d1[b, matches0[b, i]] has three finite coordinates.  Point k is the pixel (u, v) = kpts0[b, i_k] and the world point X_k, both float.
  * A2. Calibrated coordinates of the pixels through K0 as P1 (K0 checked as P1).  The solver reads them and the world
  *     points widened to double.
  * A3. Sampling as step 3 with s = 3.
@@ -389,7 +391,7 @@ LG_API int geo_relative_pose(const GeoPoseConfig* cfg, const GeoPoseInputs* in, 
 #define GEO_LO_STEPS 8
 #define GEO_LO_FINAL_STEPS 16
 #define GEO_LO_LAMBDA0 1e-3
-#define GEO_LO_MAX_MATCHES (1 << 20) /* M bound: a 40-bit score and a 24-bit count share one 64-bit sum */
+#define GEO_LO_MAX_MATCHES ((1 << 20) - 1) /* M bound: QSCALE * M < 2^36 fits the 36 score bits of the (score, h) key */
 
 typedef struct GeoLoPoseConfig {
   int32_t abi_version;        /* GEO_ABI_VERSION */

@@ -20,7 +20,7 @@ DISK_ABI_VERSION = 1
 DHN_ABI_VERSION = 1
 GEO_ABI_VERSION = 1  # include/geometry_b200.h
 GEO_HOMOGRAPHY, GEO_FUNDAMENTAL, GEO_ESSENTIAL = 0, 1, 2
-GEO_LO_QSCALE, GEO_LO_MAX_MATCHES = 65536, 1 << 20
+GEO_LO_QSCALE, GEO_LO_MAX_MATCHES = 65536, (1 << 20) - 1
 NN_ABI_VERSION = 1  # include/nn_b200.h
 NN_MIN_DIM, NN_MAX_DIM, NN_GROUP_ROWS = 64, 512, 32768
 

@@ -5,7 +5,7 @@
 //   per chunk of GEO_CHUNK hypotheses:
 //     hyp    one CTA per pair: folds the previous chunk's counts into the pair's best (packed (count + 1, ~h), atomic
 //            max), decides the adaptive stop, then one thread per hypothesis draws and solves its sample in double
-//     score  (splits, B) CTAs: each streams a slice of the pair's points through shared memory against the chunk's
+//     score  (B, splits) CTAs: each streams a slice of the pair's points through shared memory against the chunk's
 //            fp32 models, one thread per hypothesis, and adds its inlier counts
 //   refit    one CTA per pair: folds the last chunk, least-squares refit on the best hypothesis's inliers, recount,
 //            outputs
@@ -54,10 +54,10 @@ __global__ void __launch_bounds__(GEO_CHUNK, 1) geo_hyp_kernel(GeoArgs a, int c)
 }
 
 __global__ void __launch_bounds__(GEO_CHUNK) geo_score_kernel(GeoArgs a) {
-  const int b = blockIdx.y, split = blockIdx.x, t = threadIdx.x;
+  const int b = blockIdx.x, split = blockIdx.y, t = threadIdx.x;
   const GeoPair& P = a.w.pair[b];
   if (P.stop) return;
-  const int lo = (int)((long)P.n * split / gridDim.x), hi = (int)((long)P.n * (split + 1) / gridDim.x);
+  const int lo = (int)((long)P.n * split / gridDim.y), hi = (int)((long)P.n * (split + 1) / gridDim.y);
   int* cnt = a.w.count + (long)b * GEO_CHUNK + t;
   const bool valid = *cnt >= 0;
   float h[9];
@@ -192,7 +192,8 @@ extern "C" int geo_estimate(const GeoConfig* cfg, const GeoInputs* in, GeoOutput
   if (!(cfg->confidence >= 0.0 && cfg->confidence <= 1.0)) return lg_set_error("geo_estimate: confidence outside [0, 1]");
   if (in->B < 0 || in->M < 0 || in->N < 0) return lg_set_error("geo_estimate: negative size");
   if (in->B == 0) return 0;
-  if (!out->model || !out->inliers || !out->num_inliers || !out->success || !out->best_hypothesis || !out->num_hypotheses)
+  if (!out->model || !out->num_inliers || !out->success || !out->best_hypothesis || !out->num_hypotheses ||
+      (in->M > 0 && !out->inliers))  // an empty [B, 0] mask may have no storage
     return lg_set_error("geo_estimate: null output");
   if (in->M > 0 && (!in->kpts0 || !in->matches0 || (in->N > 0 && !in->kpts1))) return lg_set_error("geo_estimate: null input");
   if (!workspace || workspace_bytes < geo_workspace_bytes(in->B, in->M, cfg->max_iters))
@@ -220,7 +221,7 @@ extern "C" int geo_estimate(const GeoConfig* cfg, const GeoInputs* in, GeoOutput
   for (int c = 0; c < a.chunks; ++c) {
     geo_hyp_kernel<<<a.B, GEO_CHUNK, 0, stream>>>(a, c);
     LG_CHECK_LAUNCH();
-    geo_score_kernel<<<dim3(splits, a.B), GEO_CHUNK, 0, stream>>>(a);
+    geo_score_kernel<<<dim3(a.B, splits), GEO_CHUNK, 0, stream>>>(a);
     LG_CHECK_LAUNCH();
   }
   geo_refit_kernel<<<a.B, RED, 0, stream>>>(a);

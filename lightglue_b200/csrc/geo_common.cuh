@@ -12,6 +12,9 @@ namespace {
 
 constexpr int RED = 256;  // partial sums of the fixed summation order (header step 2)
 
+// A keypoint with a non-finite coordinate makes its match invalid at compaction (header steps 1, P1 and A1)
+__device__ __forceinline__ bool finite2(float2 p) { return isfinite(p.x) && isfinite(p.y); }
+
 __device__ __forceinline__ unsigned geo_mix(unsigned x) {
   x ^= x >> 16;
   x *= 0x7feb352du;

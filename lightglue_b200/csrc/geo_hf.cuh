@@ -222,11 +222,14 @@ __global__ void __launch_bounds__(1024) geo_prepare_kernel(GeoArgs a) {
   for (int base = 0; base < a.M; base += 1024) {
     const int i = base + tid;
     const int64_t j = i < a.M ? m0[i] : -1;
-    const bool valid = j >= 0 && j < a.N;
+    float2 p0 = make_float2(0.f, 0.f), p1 = p0;
+    if (j >= 0 && j < a.N) {
+      p0 = reinterpret_cast<const float2*>(a.kpts0)[(long)b * a.M + i];
+      p1 = reinterpret_cast<const float2*>(a.kpts1)[(long)b * a.N + j];
+    }
+    const bool valid = j >= 0 && j < a.N && finite2(p0) && finite2(p1);
     const int slot = block_scan_step(valid, tid, warp_sums, &carry);
     if (valid) {
-      const float2 p0 = reinterpret_cast<const float2*>(a.kpts0)[(long)b * a.M + i];
-      const float2 p1 = reinterpret_cast<const float2*>(a.kpts1)[(long)b * a.N + j];
       pts[slot] = make_float4(p0.x, p0.y, p1.x, p1.y);
       a.w.idx[(long)b * a.M + slot] = i;
     }

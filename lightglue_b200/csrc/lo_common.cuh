@@ -11,9 +11,11 @@ namespace {
 constexpr unsigned long long LO_COUNT_ONE = 1ull << 40;  // a score sum's count field (header GEO_LO_MAX_MATCHES)
 constexpr unsigned long long LO_SCORE_MASK = LO_COUNT_ONE - 1;
 
-// L3's per-point term of one fp32 error, with the count in bit 40.  A non-finite error is an outlier.
+// L3's per-point term of one fp32 error, with the count in bit 40.  A non-finite error is an outlier.  An inlier's
+// product is clamped to GEO_LO_QSCALE, so a subnormal thr2 (w = +inf) stays defined, and e == 0 scores 0 (0 * inf).
 __device__ __forceinline__ unsigned long long lo_term(float e, float thr2, float w) {
-  return e < thr2 ? LO_COUNT_ONE + (unsigned)(e * w) : (unsigned long long)GEO_LO_QSCALE;
+  if (!(e < thr2)) return GEO_LO_QSCALE;
+  return LO_COUNT_ONE + (e == 0.f ? 0u : (unsigned)fminf(e * w, (float)GEO_LO_QSCALE));
 }
 
 // The fixed-order sums (header step 2) of T terms at once, through red [T][RED]; every thread of the CTA calls it

@@ -5,7 +5,7 @@
 //   prepare  geo_api.cu's compaction and Hartley normalisation kernel (geo_hf.cuh)
 //   per chunk of GEO_CHUNK samples:
 //     hyp    one CTA per pair, one thread per sample: the four-point DLT of step 4, fp32
-//     score  (splits, B) CTAs: each streams a slice of the pair's points through shared memory against the chunk's
+//     score  (B, splits) CTAs: each streams a slice of the pair's points through shared memory against the chunk's
 //            models, one thread per sample, and adds count << 40 | MSAC score with one 64-bit atomic per sample
 //     lo     one CTA per pair: the chunk's lowest (score, h); when it beats the pair's model, LM on the truncated
 //            transfer cost and a re-score; then the adaptive stop.  Otherwise it returns at once.
@@ -230,10 +230,10 @@ __global__ void __launch_bounds__(GEO_CHUNK, 1) loh_hyp_kernel(LohArgs a, int c)
 }
 
 __global__ void __launch_bounds__(GEO_CHUNK) loh_score_kernel(LohArgs a) {
-  const int b = blockIdx.y, split = blockIdx.x, t = threadIdx.x;
+  const int b = blockIdx.x, split = blockIdx.y, t = threadIdx.x;
   const GeoPair& P = a.g.w.pair[b];
   if (P.stop) return;
-  const int lo = (int)((long)P.n * split / gridDim.x), hi = (int)((long)P.n * (split + 1) / gridDim.x);
+  const int lo = (int)((long)P.n * split / gridDim.y), hi = (int)((long)P.n * (split + 1) / gridDim.y);
   const bool valid = a.g.w.count[(long)b * GEO_CHUNK + t] >= 0;
   float h[9];
   for (int i = 0; i < 9; ++i) h[i] = valid ? a.g.w.hyp[((long)b * GEO_CHUNK + t) * 9 + i] : 0.f;
@@ -369,8 +369,8 @@ extern "C" int geo_homography_lo(const GeoConfig* cfg, const GeoInputs* in, GeoL
   if (in->M > GEO_LO_MAX_MATCHES) return lg_set_error("geo_homography_lo: M above GEO_LO_MAX_MATCHES");
   if (in->B == 0) return 0;
   const GeoOutputs& o = out->geo;
-  if (!o.model || !o.inliers || !o.num_inliers || !o.success || !o.best_hypothesis || !o.num_hypotheses ||
-      !out->num_local_optimizations || !out->cost)
+  if (!o.model || !o.num_inliers || !o.success || !o.best_hypothesis || !o.num_hypotheses ||
+      !out->num_local_optimizations || !out->cost || (in->M > 0 && !o.inliers))  // an empty mask may have no storage
     return lg_set_error("geo_homography_lo: null output");
   if (in->M > 0 && (!in->kpts0 || !in->matches0 || (in->N > 0 && !in->kpts1)))
     return lg_set_error("geo_homography_lo: null input");
@@ -402,7 +402,7 @@ extern "C" int geo_homography_lo(const GeoConfig* cfg, const GeoInputs* in, GeoL
   for (int c = 0; c < g.chunks; ++c) {
     loh_hyp_kernel<<<g.B, GEO_CHUNK, 0, stream>>>(a, c);
     LG_CHECK_LAUNCH();
-    loh_score_kernel<<<dim3(splits, g.B), GEO_CHUNK, 0, stream>>>(a);
+    loh_score_kernel<<<dim3(g.B, splits), GEO_CHUNK, 0, stream>>>(a);
     LG_CHECK_LAUNCH();
     loh_kernel<<<g.B, RED, 0, stream>>>(a, c);
     LG_CHECK_LAUNCH();

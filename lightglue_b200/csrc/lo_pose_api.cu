@@ -5,7 +5,7 @@
 //   prepare  pose_api.cu's compaction kernel (pose_common.cuh)
 //   per chunk of GEO_CHUNK samples:
 //     hyp    one CTA per pair, one thread per sample: the five-point solutions, fp32
-//     score  (splits, B) CTAs: each streams a slice of the pair's points through shared memory against every solution
+//     score  (B, splits) CTAs: each streams a slice of the pair's points through shared memory against every solution
 //            of the chunk, one thread per sample, and adds count << 40 | MSAC score with one 64-bit atomic per solution
 //     lo     one CTA per pair: the chunk's lowest (score, h, r); when it beats the pair's model, P7's pose choice, LM
 //            on the truncated Sampson cost and a re-score; then the adaptive stop.  Otherwise it returns at once.
@@ -257,10 +257,10 @@ __global__ void __launch_bounds__(GEO_CHUNK, 1) lo_hyp_kernel(LoArgs a, int c) {
 }
 
 __global__ void __launch_bounds__(GEO_CHUNK) lo_score_kernel(LoArgs a) {
-  const int b = blockIdx.y, split = blockIdx.x, t = threadIdx.x;
+  const int b = blockIdx.x, split = blockIdx.y, t = threadIdx.x;
   const PosePair& P = a.p.w.pair[b];
   if (P.stop) return;
-  const int lo = (int)((long)P.n * split / gridDim.x), hi = (int)((long)P.n * (split + 1) / gridDim.x);
+  const int lo = (int)((long)P.n * split / gridDim.y), hi = (int)((long)P.n * (split + 1) / gridDim.y);
   const int ns = a.p.w.nsol[(long)b * GEO_CHUNK + t];
   const float* hm = a.p.w.hyp + ((long)b * GEO_CHUNK + t) * SOLS * 9;
   const float thr2 = P.thr2;
@@ -472,8 +472,9 @@ extern "C" int geo_relative_pose_lo(const GeoLoPoseConfig* cfg, const GeoPoseInp
   if (in->M > GEO_LO_MAX_MATCHES) return lg_set_error("geo_relative_pose_lo: M above GEO_LO_MAX_MATCHES");
   if (in->B == 0) return 0;
   const GeoPoseOutputs& o = out->pose;
-  if (!o.E || !o.R || !o.t || !o.inliers || !o.num_inliers || !o.pose_inliers || !o.num_pose_inliers || !o.success ||
-      !o.best_hypothesis || !o.best_solution || !o.num_hypotheses || !out->num_local_optimizations || !out->cost)
+  if (!o.E || !o.R || !o.t || !o.num_inliers || !o.num_pose_inliers || !o.success || !o.best_hypothesis ||
+      !o.best_solution || !o.num_hypotheses || !out->num_local_optimizations || !out->cost ||
+      (in->M > 0 && (!o.inliers || !o.pose_inliers)))  // empty [B, 0] masks may have no storage
     return lg_set_error("geo_relative_pose_lo: null output");
   if (!in->K0 || !in->K1) return lg_set_error("geo_relative_pose_lo: null intrinsics");
   if (in->M > 0 && (!in->kpts0 || !in->matches0 || (in->N > 0 && !in->kpts1)))
@@ -506,7 +507,7 @@ extern "C" int geo_relative_pose_lo(const GeoLoPoseConfig* cfg, const GeoPoseInp
   for (int c = 0; c < p.chunks; ++c) {
     lo_hyp_kernel<<<p.B, GEO_CHUNK, 0, stream>>>(a, c);
     LG_CHECK_LAUNCH();
-    lo_score_kernel<<<dim3(splits, p.B), GEO_CHUNK, 0, stream>>>(a);
+    lo_score_kernel<<<dim3(p.B, splits), GEO_CHUNK, 0, stream>>>(a);
     LG_CHECK_LAUNCH();
     lo_kernel<<<p.B, RED, 0, stream>>>(a, c);
     LG_CHECK_LAUNCH();

@@ -6,7 +6,7 @@
 //   per chunk of GEO_CHUNK samples:
 //     hyp    one CTA per pair: folds the previous chunk's counts into the pair's best (packed (count + 1, ~(h*16 + r)),
 //            atomic max), decides the adaptive stop, then one thread per sample solves it: up to 4 fp32 projections
-//     score  (splits, B) CTAs: each streams a slice of the pair's points through shared memory against every solution
+//     score  (B, splits) CTAs: each streams a slice of the pair's points through shared memory against every solution
 //            of the chunk, one thread per sample, and adds the inlier counts
 //   refit    one CTA per pair: folds the last chunk, Levenberg-Marquardt from the best solution, recount, R and t
 //   mask     one thread per row of matches0: the final inlier mask
@@ -307,17 +307,18 @@ __global__ void __launch_bounds__(1024) pnp_prepare_kernel(PnpArgs a) {
     const int i = base + tid;
     const int64_t j = i < a.M ? m0[i] : -1;
     float X = 0.f, Y = 0.f, Z = 0.f;
+    float2 p = make_float2(0.f, 0.f);
     if (j >= 0 && j < a.N) {
       const float* q = a.points3d1 + ((long)b * a.N + j) * 3;
       X = q[0];
       Y = q[1];
       Z = q[2];
+      p = reinterpret_cast<const float2*>(a.kpts0)[(long)b * a.M + i];
     }
-    const bool valid = j >= 0 && j < a.N && isfinite(X) && isfinite(Y) && isfinite(Z);
+    const bool valid = j >= 0 && j < a.N && isfinite(X) && isfinite(Y) && isfinite(Z) && finite2(p);
     const int k = block_scan_step(valid, tid, warp_sums, &carry);
     if (i < a.M) slot[i] = valid ? k : -1;
     if (valid) {
-      const float2 p = reinterpret_cast<const float2*>(a.kpts0)[(long)b * a.M + i];
       const double yy = ((double)p.y - K[5]) / K[4], xx = (((double)p.x - K[2]) - K[1] * yy) / K[0];
       pts[k] = make_float4(p.x, p.y, (float)xx, (float)yy);
       wld[k] = make_float4(X, Y, Z, 0.f);
@@ -359,10 +360,10 @@ __global__ void __launch_bounds__(GEO_CHUNK, 1) pnp_hyp_kernel(PnpArgs a, int c)
 }
 
 __global__ void __launch_bounds__(GEO_CHUNK) pnp_score_kernel(PnpArgs a) {
-  const int b = blockIdx.y, split = blockIdx.x, t = threadIdx.x;
+  const int b = blockIdx.x, split = blockIdx.y, t = threadIdx.x;
   const PnpPair& P = a.w.pair[b];
   if (P.stop) return;
-  const int lo = (int)((long)P.n * split / gridDim.x), hi = (int)((long)P.n * (split + 1) / gridDim.x);
+  const int lo = (int)((long)P.n * split / gridDim.y), hi = (int)((long)P.n * (split + 1) / gridDim.y);
   const int ns = a.w.nsol[(long)b * GEO_CHUNK + t];
   const float* hm = a.w.hyp + ((long)b * GEO_CHUNK + t) * SOLS * 12;
   const float thr2 = P.thr2;
@@ -550,7 +551,7 @@ __global__ void __launch_bounds__(RED, 1) pnp_refit_kernel(PnpArgs a) {
 }
 
 __global__ void __launch_bounds__(MASK_THREADS) pnp_mask_kernel(PnpArgs a) {
-  const int b = blockIdx.y, i = blockIdx.x * MASK_THREADS + threadIdx.x;
+  const int b = blockIdx.x, i = blockIdx.y * MASK_THREADS + threadIdx.x;
   if (i >= a.M) return;
   const PnpPair& P = a.w.pair[b];
   const int k = a.w.slot[(long)b * a.M + i];
@@ -579,8 +580,8 @@ extern "C" int geo_absolute_pose(const GeoPnpConfig* cfg, const GeoPnpInputs* in
     return lg_set_error("geo_absolute_pose: confidence outside [0, 1]");
   if (in->B < 0 || in->M < 0 || in->N < 0) return lg_set_error("geo_absolute_pose: negative size");
   if (in->B == 0) return 0;
-  if (!out->R || !out->t || !out->inliers || !out->num_inliers || !out->success || !out->best_hypothesis ||
-      !out->best_solution || !out->num_hypotheses)
+  if (!out->R || !out->t || !out->num_inliers || !out->success || !out->best_hypothesis || !out->best_solution ||
+      !out->num_hypotheses || (in->M > 0 && !out->inliers))  // an empty [B, 0] mask may have no storage
     return lg_set_error("geo_absolute_pose: null output");
   if (!in->K0) return lg_set_error("geo_absolute_pose: null intrinsics");
   if (in->M > 0 && (!in->kpts0 || !in->matches0 || (in->N > 0 && !in->points3d1)))
@@ -609,13 +610,13 @@ extern "C" int geo_absolute_pose(const GeoPnpConfig* cfg, const GeoPnpInputs* in
   for (int c = 0; c < a.chunks; ++c) {
     pnp_hyp_kernel<<<a.B, GEO_CHUNK, 0, stream>>>(a, c);
     LG_CHECK_LAUNCH();
-    pnp_score_kernel<<<dim3(splits, a.B), GEO_CHUNK, 0, stream>>>(a);
+    pnp_score_kernel<<<dim3(a.B, splits), GEO_CHUNK, 0, stream>>>(a);
     LG_CHECK_LAUNCH();
   }
   pnp_refit_kernel<<<a.B, RED, 0, stream>>>(a);
   LG_CHECK_LAUNCH();
   if (a.M > 0) {
-    pnp_mask_kernel<<<dim3((a.M + MASK_THREADS - 1) / MASK_THREADS, a.B), MASK_THREADS, 0, stream>>>(a);
+    pnp_mask_kernel<<<dim3(a.B, (a.M + MASK_THREADS - 1) / MASK_THREADS), MASK_THREADS, 0, stream>>>(a);
     LG_CHECK_LAUNCH();
   }
   return 0;

@@ -6,7 +6,7 @@
 //   per chunk of GEO_CHUNK samples:
 //     hyp    one CTA per pair: folds the previous chunk's counts into the pair's best (packed (count + 1, ~(h*16 + r)),
 //            atomic max), decides the adaptive stop, then one thread per sample solves it: up to 10 fp32 models
-//     score  (splits, B) CTAs: each streams a slice of the pair's points through shared memory against every solution
+//     score  (B, splits) CTAs: each streams a slice of the pair's points through shared memory against every solution
 //            of the chunk, one thread per sample, and adds the inlier counts
 //   refit    one CTA per pair: folds the last chunk, least-squares refit projected on the essential manifold, recount,
 //            E and the inliers
@@ -66,10 +66,10 @@ __global__ void __launch_bounds__(GEO_CHUNK, 1) pose_hyp_kernel(PoseArgs a, int 
 }
 
 __global__ void __launch_bounds__(GEO_CHUNK) pose_score_kernel(PoseArgs a) {
-  const int b = blockIdx.y, split = blockIdx.x, t = threadIdx.x;
+  const int b = blockIdx.x, split = blockIdx.y, t = threadIdx.x;
   const PosePair& P = a.w.pair[b];
   if (P.stop) return;
-  const int lo = (int)((long)P.n * split / gridDim.x), hi = (int)((long)P.n * (split + 1) / gridDim.x);
+  const int lo = (int)((long)P.n * split / gridDim.y), hi = (int)((long)P.n * (split + 1) / gridDim.y);
   const int ns = a.w.nsol[(long)b * GEO_CHUNK + t];
   const float* hm = a.w.hyp + ((long)b * GEO_CHUNK + t) * SOLS * 9;
   const float thr2 = P.thr2;
@@ -275,8 +275,9 @@ extern "C" int geo_relative_pose(const GeoPoseConfig* cfg, const GeoPoseInputs* 
     return lg_set_error("geo_relative_pose: distance_threshold must be positive");
   if (in->B < 0 || in->M < 0 || in->N < 0) return lg_set_error("geo_relative_pose: negative size");
   if (in->B == 0) return 0;
-  if (!out->E || !out->R || !out->t || !out->inliers || !out->num_inliers || !out->pose_inliers ||
-      !out->num_pose_inliers || !out->success || !out->best_hypothesis || !out->best_solution || !out->num_hypotheses)
+  if (!out->E || !out->R || !out->t || !out->num_inliers || !out->num_pose_inliers || !out->success ||
+      !out->best_hypothesis || !out->best_solution || !out->num_hypotheses ||
+      (in->M > 0 && (!out->inliers || !out->pose_inliers)))  // empty [B, 0] masks may have no storage
     return lg_set_error("geo_relative_pose: null output");
   if (!in->K0 || !in->K1) return lg_set_error("geo_relative_pose: null intrinsics");
   if (in->M > 0 && (!in->kpts0 || !in->matches0 || (in->N > 0 && !in->kpts1)))
@@ -306,7 +307,7 @@ extern "C" int geo_relative_pose(const GeoPoseConfig* cfg, const GeoPoseInputs* 
   for (int c = 0; c < a.chunks; ++c) {
     pose_hyp_kernel<<<a.B, GEO_CHUNK, 0, stream>>>(a, c);
     LG_CHECK_LAUNCH();
-    pose_score_kernel<<<dim3(splits, a.B), GEO_CHUNK, 0, stream>>>(a);
+    pose_score_kernel<<<dim3(a.B, splits), GEO_CHUNK, 0, stream>>>(a);
     LG_CHECK_LAUNCH();
   }
   pose_refit_kernel<<<a.B, RED, 0, stream>>>(a);

@@ -437,11 +437,14 @@ __global__ void __launch_bounds__(1024) pose_prepare_kernel(PoseArgs a) {
   for (int base = 0; base < a.M; base += 1024) {
     const int i = base + tid;
     const int64_t j = i < a.M ? m0[i] : -1;
-    const bool valid = j >= 0 && j < a.N;
+    float2 p0 = make_float2(0.f, 0.f), p1 = p0;
+    if (j >= 0 && j < a.N) {
+      p0 = reinterpret_cast<const float2*>(a.kpts0)[(long)b * a.M + i];
+      p1 = reinterpret_cast<const float2*>(a.kpts1)[(long)b * a.N + j];
+    }
+    const bool valid = j >= 0 && j < a.N && finite2(p0) && finite2(p1);
     const int slot = block_scan_step(valid, tid, warp_sums, &carry);
     if (valid) {
-      const float2 p0 = reinterpret_cast<const float2*>(a.kpts0)[(long)b * a.M + i];
-      const float2 p1 = reinterpret_cast<const float2*>(a.kpts1)[(long)b * a.N + j];
       const double y0 = ((double)p0.y - K0[5]) / K0[4], x0 = (((double)p0.x - K0[2]) - K0[1] * y0) / K0[0];
       const double y1 = ((double)p1.y - K1[5]) / K1[4], x1 = (((double)p1.x - K1[2]) - K1[1] * y1) / K1[0];
       pts[slot] = make_float4((float)x0, (float)y0, (float)x1, (float)y1);

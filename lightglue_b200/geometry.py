@@ -6,7 +6,9 @@ relative-pose (plain and LO-RANSAC) and absolute-pose estimation on the matcher'
 All six functions take ``matches0`` [B, M] int64 exactly as ``LightGlue.forward``, ``PendingMatch.tensors`` and
 ``match_ragged`` give it (-1 or any index outside [0, N) is unmatched), run every pair of the batch in one call on the
 current stream, and return device tensors of fixed shapes without synchronising with the host, so a call can follow a
-matcher forward with no read-back in between, or be captured in a CUDA graph.  Parameter names and defaults are those of
+matcher forward with no read-back in between, or be captured in a CUDA graph.  A match whose keypoint in either image,
+or whose 3D point, has a NaN or infinite coordinate is invalid like an unmatched row: it is never an inlier and does
+not count towards the pair's matches.  Parameter names and defaults are those of
 ``cv2.findHomography(RANSAC)``, ``cv2.findFundamentalMat(FM_RANSAC)``, ``cv2.findEssentialMat(RANSAC)`` with
 ``cv2.recoverPose``, and ``cv2.solvePnPRansac``.
 
@@ -114,7 +116,7 @@ def find_homography_lo(kpts0: torch.Tensor, kpts1: torch.Tensor, matches0: torch
     truncated (MSAC) transfer cost, with Levenberg-Marquardt local optimisation of H after each chunk of 256 samples
     that improves the best model, and a final Levenberg-Marquardt refinement.  The accuracy of PoseLib's and OpenCV's
     USAC LO-RANSAC, on the GPU; ``find_homography`` stays the one that follows ``cv2.RANSAC``.  Arguments and defaults
-    are ``find_homography``'s, so the two compare like for like; at most 2**20 rows of ``matches0`` per pair.
+    are ``find_homography``'s, so the two compare like for like; at most 2**20 - 1 rows of ``matches0`` per pair.
 
     Returns the keys of ``find_homography`` (``H`` the final model with H[2, 2] = 1; ``inliers`` the points within the
     threshold of that H; ``best_hypothesis`` the sample the final model grew from) plus ``num_local_optimizations``
@@ -174,7 +176,8 @@ def estimate_relative_pose_lo(kpts0: torch.Tensor, kpts1: torch.Tensor, matches0
     a truncated (MSAC) Sampson cost, with Levenberg-Marquardt local optimisation of (R, t) after each chunk of 256
     samples that improves the best model, and a final Levenberg-Marquardt refinement.  The accuracy of PoseLib's and
     OpenCV's USAC LO-RANSAC, on the GPU; ``estimate_relative_pose`` stays the one that follows ``cv2.RANSAC``.
-    Arguments and defaults are ``estimate_relative_pose``'s, so the two compare like for like.
+    Arguments and defaults are ``estimate_relative_pose``'s, so the two compare like for like; at most 2**20 - 1 rows of
+    ``matches0`` per pair.
 
     Returns the keys of ``estimate_relative_pose`` (E = [t]x R of the final pose, unit Frobenius norm with its largest
     entry positive; ``inliers`` the points within the threshold of that E; ``best_hypothesis`` and ``best_solution``

@@ -53,9 +53,12 @@ def fixed_sum(v: np.ndarray) -> np.ndarray:
 
 
 def compact(kpts0: np.ndarray, kpts1: np.ndarray, m0: np.ndarray):
-    """One pair: the valid matches in ascending row order, as (rows, float32 [n, 4] of x0, y0, x1, y1)."""
+    """One pair: the valid matches (index in range, both keypoints finite) in ascending row order, as (rows, float32
+    [n, 4] of x0, y0, x1, y1)."""
     n1 = kpts1.shape[0]
-    rows = np.nonzero((m0 >= 0) & (m0 < n1))[0]
+    ok = (m0 >= 0) & (m0 < n1)
+    ok[ok] = np.isfinite(kpts0[ok]).all(1) & np.isfinite(kpts1[m0[ok]]).all(1)
+    rows = np.nonzero(ok)[0]
     pts = np.concatenate([kpts0[rows], kpts1[m0[rows]]], axis=1).astype(np.float32)
     return rows, pts
 

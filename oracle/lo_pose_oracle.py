@@ -23,11 +23,15 @@ TERMS = 21           # J^T J upper triangle (15), J^T r (5), truncated cost
 
 
 def score(err: np.ndarray, thr2: np.float32):
-    """fp32 errors [..., n] -> (uint64 MSAC scores, int64 inlier counts) over the last axis (header step L3)."""
-    w = np.float32(QSCALE) / thr2
-    inl = err < thr2
+    """fp32 errors [..., n] -> (uint64 MSAC scores, int64 inlier counts) over the last axis (header step L3).  An
+    inlier's term is min(err * w, QSCALE) truncated, and 0 at err == 0, so a subnormal thr2 (w = inf) is defined."""
+    thr2 = np.float32(thr2)
     with np.errstate(all="ignore"):
-        q = np.where(inl, np.where(inl, err, np.float32(0.0)) * w, np.float32(0.0)).astype(np.uint32)
+        w = np.float32(QSCALE) / thr2
+        inl = err < thr2
+        e = np.where(inl, err, np.float32(0.0))
+        p = np.where(e == 0, np.float32(0.0), np.fmin(e * w, np.float32(QSCALE)))
+        q = p.astype(np.uint32)
     q = np.where(inl, q, np.uint32(QSCALE)).astype(np.uint64)
     return q.sum(-1, dtype=np.uint64), inl.sum(-1)
 

@@ -33,11 +33,11 @@ calibrate = po.calibrate
 
 
 def compact(kpts0, points3d1, m0):
-    """One pair: rows of the valid matches (index in range, finite 3D point) in ascending order, their float32 pixels
-    [n, 2] and float32 world points [n, 3]."""
+    """One pair: rows of the valid matches (index in range, finite pixel and 3D point) in ascending order, their
+    float32 pixels [n, 2] and float32 world points [n, 3]."""
     n1 = points3d1.shape[0]
     ok = (m0 >= 0) & (m0 < n1)
-    ok[ok] = np.isfinite(points3d1[m0[ok]]).all(1)
+    ok[ok] = np.isfinite(points3d1[m0[ok]]).all(1) & np.isfinite(kpts0[ok]).all(1)
     rows = np.nonzero(ok)[0]
     return rows, kpts0[rows].astype(np.float32), points3d1[m0[rows]].astype(np.float32)
 

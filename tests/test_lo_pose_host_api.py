@@ -27,13 +27,15 @@ def test_lo_entry_points_are_exported():
         assert getattr(lib, s).argtypes is not None, s
 
 
-def test_lo_constants_match_the_oracle_and_bindings():
+def test_lo_constants_and_row_bound_match_the_oracle_and_bindings():
     h = _header()
     for name, value in (("GEO_LO_QSCALE", lo.QSCALE), ("GEO_LO_STEPS", lo.STEPS),
                         ("GEO_LO_FINAL_STEPS", lo.FINAL_STEPS)):
         assert re.search(rf"#define {name} {value}\b", h), name
     assert re.search(r"#define GEO_LO_LAMBDA0 1e-3\b", h) and lo.LAMBDA0 == 1e-3
-    assert re.search(r"#define GEO_LO_MAX_MATCHES \(1 << 20\)", h) and _cabi.GEO_LO_MAX_MATCHES == 1 << 20
+    # the row bound keeps the largest score, QSCALE * M, below 2^36: the bits above h in the (score, h) key
+    assert re.search(r"#define GEO_LO_MAX_MATCHES \(\(1 << 20\) - 1\)", h) and _cabi.GEO_LO_MAX_MATCHES == (1 << 20) - 1
+    assert lo.QSCALE * _cabi.GEO_LO_MAX_MATCHES < 1 << 36
     assert _cabi.GEO_LO_QSCALE == lo.QSCALE
     assert re.search(r"#define GEO_ABI_VERSION 1\b", h)
 
