@@ -215,6 +215,56 @@
  *      and the result is deterministic; the score is quantised to integers; there is no non-minimal (DLT) refit inside
  *      the LO and no PROSAC ordering.
  *
+ * LO-RANSAC fundamental matrix (geo_fundamental_lo; oracle/lo_fundamental_oracle.py restates it bit for bit): the
+ * outputs of geo_estimate for GEO_FUNDAMENTAL, from an MSAC-scored eight-point RANSAC with Levenberg-Marquardt local
+ * optimisation of a rank-2 F, on the schedule of L1-L8.  Expressions evaluate left to right as written; every multiply
+ * and add rounds on its own.
+ *
+ * LF1. Compaction and Hartley normalisation exactly as steps 1-2; thr2 = (float)(threshold * threshold).
+ *      M <= GEO_LO_MAX_MATCHES.
+ * LF2. Sampling (s = 8) and the eight-point solver, rank 2, denormalisation and scale exactly as steps 3-4: with the
+ *      same seed both estimators draw the same samples and solve the same hypotheses.
+ * LF3. MSAC score, per hypothesis, from step 5's fp32 error err (the larger of the two squared point-to-epipolar-line
+ *      distances, the model rounded to float): q as L3 (0 at err == 0, else (uint32)fminf(err * w, GEO_LO_QSCALE) for
+ *      err < thr2, else GEO_LO_QSCALE), so a non-finite err scores as an outlier.  score = sum of q over the points in
+ *      uint64, count = the number of err < thr2.  Lower is better; ties go to the lowest h.
+ * LF4. Local optimisation, after every chunk of GEO_CHUNK samples, once per pair.  Chunk c's best hypothesis (lowest
+ *      (score, h)) is taken when the pair has no model yet or its score is strictly below the model's score; else
+ *      nothing happens.  Taken, its double F of step 4 becomes the pair's model (score, count, h).  Then GEO_LO_STEPS
+ *      LM steps (LF7) from it give (U', V', sig'), whose pixel model F' = T1^T Fn' T0 scaled as step 4 is scored as
+ *      LF3; with a strictly lower score F' replaces the model (keeping h) and num_local_optimizations counts one.
+ * LF5. Stopping as step 6 with s = 8 from the model's count (a local optimisation's count included).
+ * LF6. Final refinement: GEO_LO_FINAL_STEPS LM steps from the model, kept unless their LF3 score is higher.
+ * LF7. LM, in double, on the normalised model in the orthonormal representation of Bartoli and Sturm (PoseLib's
+ *      FactorizedFundamentalMatrix: 7 degrees of freedom, rank 2 by construction).  From a pixel F (row-major),
+ *      Fn = (T1^-T F) T0^-1 (3x3 products as step 4; T1^-T = [[1/s1, 0, 0], [0, 1/s1, 0], [cx1, cy1, 1]],
+ *      T0^-1 = [[1/s0, 0, cx0], [0, 1/s0, cy0], [0, 0, 1]]).  Factorisation: step 4's one-sided Jacobi on Fn, the column
+ *      m of least squared norm n_m (the first) dropped; of the two kept columns (i < j) the one of larger squared norm
+ *      (i on a tie) is p, the other q: u1 = a_p / sqrt(n_p), u2 = a_q / sqrt(n_q), v1, v2 the columns p, q of V,
+ *      u3 = u1 x u2, v3 = v1 x v2 (a x b = (a1*b2 - a2*b1, a2*b0 - a0*b2, a0*b1 - a1*b0)), sig = sqrt(n_q) / sqrt(n_p).
+ *      U = [u1 u2 u3] and V = [v1 v2 v3] are rotations, and Fn(U, V, sig)_ab = u1_a*v1_b + sig*u2_a*v2_b.  The
+ *      parameters delta0..6 move the model to U' = Q(delta0..2) U, V' = Q(delta3..5) V (3x3 products as step 4, Q the
+ *      quaternion rotation of A7) and sig' = sig + delta6; sig is not clamped.  Directions at Fn = Fn(U, V, sig):
+ *      D_k = [e_k]x Fn (column j is e_k x Fn[:, j]) for k = 0..2, D_(3+k) = -Fn [e_k]x (row i is e_k x Fn[i, :]) and
+ *      D_6_ab = u2_a*v2_b.  Residuals in pixels, on the compacted floats widened: with f = (T1^T Fn) T0 unscaled
+ *      (T1^T as step 4), a0 = (f0*x0 + f1*y0) + f2, a1 = (f3*x0 + f4*y0) + f5, a2 = (f6*x0 + f7*y0) + f8,
+ *      d = (x1*a0 + y1*a1) + a2, b0 = (f0*x1 + f3*y1) + f6, b1 = (f1*x1 + f4*y1) + f7,
+ *      den = ((a0*a0 + a1*a1) + b0*b0) + b1*b1, err = (d*d) / den and r = d / sqrt(den): L7's Sampson error with F in
+ *      place of E.  An inlier at this model has err < (double)thr2.  With g = (T1^T D_k) T0 and da, dd, db of g as a, d,
+ *      b of f, dden = ((a0*da0 + a1*da1) + b0*db0) + b1*db1 and J_k = (dd - d*dden / den) / sqrt(den).  The 28 terms
+ *      J_i*J_j (i <= j in row order) and the 7 terms J_i*r over the inliers, and the truncated cost (err for an inlier,
+ *      else (double)thr2) over every point, are each summed in the order of step 2.  A step solves the 7x7 system of
+ *      A7 (damping, Cholesky, right-hand side -J^T r), lambda starts at GEO_LO_LAMBDA0, and the step is taken only if
+ *      the truncated cost at (U', V', sig'), with its own inliers, is strictly lower: A7's schedule.
+ * LF8. Outputs: model the final F (a hypothesis's F of step 4, or T1^T Fn T0 scaled as step 4: rank 2, unit Frobenius
+ *      norm, its first entry of largest magnitude positive); inliers the points with err < thr2 under it rounded to
+ *      float (step 5's error), num_inliers their number and cost its LF3 score; best_hypothesis the hypothesis that
+ *      seeded it; num_hypotheses the samples drawn.  A pair fails as step 7's failures (n < 8, a failed
+ *      normalisation, every sample degenerate), with num_local_optimizations and cost 0.  Deviations from PoseLib:
+ *      local optimisation runs at most once per chunk rather than at every new best, so the launch sequence is fixed
+ *      and the result is deterministic; the score is quantised to integers; samples have 8 points rather than 7, so
+ *      they are find_fundamental's; there is no non-minimal refit inside the LO, and no DEGENSAC or PROSAC.
+ *
  * Absolute pose (geo_absolute_pose; oracle/pnp_oracle.py restates it bit for bit): the (R, t) of x_cam = R X + t that
  * maps the world points of image 1's keypoints into the query camera 0, OpenCV's rvec/tvec convention.  Expressions
  * below evaluate left to right as written (a + b + c is (a + b) + c); no step whose result must match bit for bit calls
@@ -414,15 +464,20 @@ LG_API int geo_relative_pose_lo(const GeoLoPoseConfig* cfg, const GeoPoseInputs*
                                 void* workspace, size_t workspace_bytes, void* stream);
 
 typedef struct GeoLoOutputs {
-  GeoOutputs geo;                    /* as geo_estimate's; model is H */
+  GeoOutputs geo;                    /* as geo_estimate's; model is H or F */
   int32_t* num_local_optimizations;  /* [B] local optimisations whose model was adopted */
-  int64_t* cost;                     /* [B] LH3 score of the final model */
+  int64_t* cost;                     /* [B] LH3 or LF3 score of the final model */
 } GeoLoOutputs;
 
 /* LO-RANSAC homography (steps LH1-LH8): cfg->model must be GEO_HOMOGRAPHY, in->M <= GEO_LO_MAX_MATCHES. */
 LG_API size_t geo_lo_homography_workspace_bytes(int32_t B, int32_t M, int32_t max_iters);
 LG_API int geo_homography_lo(const GeoConfig* cfg, const GeoInputs* in, GeoLoOutputs* out, void* workspace,
                              size_t workspace_bytes, void* stream);
+
+/* LO-RANSAC fundamental matrix (steps LF1-LF8): cfg->model must be GEO_FUNDAMENTAL, in->M <= GEO_LO_MAX_MATCHES. */
+LG_API size_t geo_lo_fundamental_workspace_bytes(int32_t B, int32_t M, int32_t max_iters);
+LG_API int geo_fundamental_lo(const GeoConfig* cfg, const GeoInputs* in, GeoLoOutputs* out, void* workspace,
+                              size_t workspace_bytes, void* stream);
 
 #define GEO_PNP_MAX_SOLUTIONS 4
 #define GEO_PNP_COLLINEAR_EPS 1e-10

@@ -264,6 +264,9 @@ GEO_PROTOTYPES = {  # include/geometry_b200.h
     "geo_lo_homography_workspace_bytes": (_SZ, [_I32, _I32, _I32]),
     "geo_homography_lo": (C.c_int, [C.POINTER(GeoConfig), C.POINTER(GeoInputs), C.POINTER(GeoLoOutputs), _VP, _SZ,
                                     _VP]),
+    "geo_lo_fundamental_workspace_bytes": (_SZ, [_I32, _I32, _I32]),
+    "geo_fundamental_lo": (C.c_int, [C.POINTER(GeoConfig), C.POINTER(GeoInputs), C.POINTER(GeoLoOutputs), _VP, _SZ,
+                                     _VP]),
     "geo_pnp_workspace_bytes": (_SZ, [_I32, _I32, _I32]),
     "geo_absolute_pose": (C.c_int, [C.POINTER(GeoPnpConfig), C.POINTER(GeoPnpInputs), C.POINTER(GeoPnpOutputs), _VP,
                                     _SZ, _VP]),

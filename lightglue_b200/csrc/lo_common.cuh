@@ -1,6 +1,6 @@
-// The LO-RANSAC pieces shared by the relative pose (lo_pose_api.cu, header steps L3 and L7) and the homography
-// (lo_homography_api.cu, LH3 and LH7), both compiled with -fmad=false: the packed MSAC score term and the fixed-order
-// sums of the Levenberg-Marquardt terms.
+// The LO-RANSAC pieces shared by the relative pose (lo_pose_api.cu, header steps L3 and L7), the homography
+// (lo_homography_api.cu, LH3 and LH7) and the fundamental matrix (lo_fundamental_api.cu, LF3 and LF7), all compiled
+// with -fmad=false: the packed MSAC score term and the fixed-order sums of the Levenberg-Marquardt terms.
 #pragma once
 #include <cuda_runtime.h>
 

@@ -4,52 +4,25 @@
 // Launches, all fixed by (B, M, max_iters):
 //   prepare  geo_api.cu's compaction and Hartley normalisation kernel (geo_hf.cuh)
 //   per chunk of GEO_CHUNK samples:
-//     hyp    one CTA per pair, one thread per sample: the four-point DLT of step 4, fp32
+//     hyp    one CTA per pair, one thread per sample: the four-point DLT of step 4, fp32 (lo_hf.cuh)
 //     score  (B, splits) CTAs: each streams a slice of the pair's points through shared memory against the chunk's
 //            models, one thread per sample, and adds count << 40 | MSAC score with one 64-bit atomic per sample
+//            (lo_hf.cuh)
 //     lo     one CTA per pair: the chunk's lowest (score, h); when it beats the pair's model, LM on the truncated
 //            transfer cost and a re-score; then the adaptive stop.  Otherwise it returns at once.
 //   final    one CTA per pair: the final LM refinement, H and its inliers
 // A stopped pair's CTAs return at once.  Compiled with -fmad=false: oracle/lo_homography_oracle.py takes the same steps.
 #include <stdint.h>
 
-#include "geo_hf.cuh"
 #include "geo_lm.cuh"
 #include "lg_internal.h"
-#include "lo_common.cuh"
+#include "lo_hf.cuh"
 
 namespace {
 
 constexpr int LOH_DOF = 8;
 constexpr int LOH_TERMS = 45;  // J^T J upper triangle (36), J^T r (8), truncated cost
 constexpr int LOH_GROUP = 15;  // terms per pass of the fixed-order sums: three passes keep red within static shared
-
-struct LohPair {
-  double H[9];               // the pair's model in pixels, scaled as step 4
-  unsigned long long score;  // its LH3 score
-  int count;                 // its inliers
-  int h;                     // the hypothesis that seeded it; -1: none yet
-  int nlo;                   // local optimisations adopted
-};
-
-struct LohWs {
-  LohPair* pair;            // [B]
-  unsigned long long* acc;  // [B, GEO_CHUNK] count << 40 | score of the current chunk's hypotheses
-};
-
-size_t loh_carve(char* base, int B, int M, GeoWs* w, LohWs* l) {
-  WsBump b{base, carve(base, B, M, w)};
-  l->pair = b.take<LohPair>(B);
-  l->acc = b.take<unsigned long long>((size_t)B * GEO_CHUNK);
-  return b.bytes();
-}
-
-struct LohArgs {
-  GeoArgs g;
-  LohWs l;
-  int32_t* num_lo;
-  int64_t* cost;
-};
 
 // Shared state of one pair's CTA in the LO and final kernels
 struct LohShared {
@@ -208,57 +181,12 @@ __device__ void loh_rescore(LohShared& s, const GeoPair& P, const float4* pts, f
   __syncthreads();
 }
 
-__global__ void __launch_bounds__(GEO_CHUNK, 1) loh_hyp_kernel(LohArgs a, int c) {
-  const int b = blockIdx.x, t = threadIdx.x;
-  if (c == 0 && t == 0) {
-    LohPair& L = a.l.pair[b];
-    L.score = 0;
-    L.count = 0;
-    L.h = -1;
-    L.nlo = 0;
-  }
-  const GeoPair& P = a.g.w.pair[b];
-  const int h = c * GEO_CHUNK + t;
-  double m[9];
-  const bool ok = P.stop == 0 && h < a.g.max_iters && geo_hypothesis(a.g, P, a.g.w.pts + (long)b * a.g.M, h, m);
-  if (ok) {
-    float* hm = a.g.w.hyp + ((long)b * GEO_CHUNK + t) * 9;
-    for (int i = 0; i < 9; ++i) hm[i] = (float)m[i];
-    a.l.acc[(long)b * GEO_CHUNK + t] = 0;
-  }
-  a.g.w.count[(long)b * GEO_CHUNK + t] = ok ? 0 : -1;
-}
-
-__global__ void __launch_bounds__(GEO_CHUNK) loh_score_kernel(LohArgs a) {
-  const int b = blockIdx.x, split = blockIdx.y, t = threadIdx.x;
-  const GeoPair& P = a.g.w.pair[b];
-  if (P.stop) return;
-  const int lo = (int)((long)P.n * split / gridDim.y), hi = (int)((long)P.n * (split + 1) / gridDim.y);
-  const bool valid = a.g.w.count[(long)b * GEO_CHUNK + t] >= 0;
-  float h[9];
-  for (int i = 0; i < 9; ++i) h[i] = valid ? a.g.w.hyp[((long)b * GEO_CHUNK + t) * 9 + i] : 0.f;
-  const float thr2 = a.g.thr2;
-  const float w = (float)GEO_LO_QSCALE / thr2;
-  const float4* pts = a.g.w.pts + (long)b * a.g.M;
-  __shared__ float4 tile[TILE];
-  unsigned long long k = 0;
-  for (int base = lo; base < hi; base += TILE) {
-    const int m = min(TILE, hi - base);
-    __syncthreads();
-    for (int i = t; i < m; i += GEO_CHUNK) tile[i] = pts[base + i];
-    __syncthreads();
-    if (valid)
-      for (int i = 0; i < m; ++i) k += lo_term(geo_err(GEO_HOMOGRAPHY, h, tile[i]), thr2, w);
-  }
-  if (k) atomicAdd(a.l.acc + (long)b * GEO_CHUNK + t, k);
-}
-
 // After chunk c: the chunk's best hypothesis, the local optimisation when it beats the pair's model, the stop
-__global__ void __launch_bounds__(RED, 1) loh_kernel(LohArgs a, int c) {
+__global__ void __launch_bounds__(RED, 1) loh_kernel(LoHfArgs a, int c) {
   const int b = blockIdx.x, t = threadIdx.x;
   GeoPair& P = a.g.w.pair[b];
   if (P.stop) return;
-  LohPair& L = a.l.pair[b];
+  LoHfPair& L = a.l.pair[b];
   __shared__ LohShared s;
   if (t == 0) s.key = ~0ull;
   __syncthreads();
@@ -272,17 +200,17 @@ __global__ void __launch_bounds__(RED, 1) loh_kernel(LohArgs a, int c) {
   if (s.take) {
     if (t == 0) {
       const unsigned h = (unsigned)(key & 0xfffffffu);
-      geo_hypothesis(a.g, P, pts, h, L.H);
+      geo_hypothesis(a.g, P, pts, h, L.model);
       L.score = key >> 28;
       L.count = (int)(a.l.acc[(long)b * GEO_CHUNK + h - c * GEO_CHUNK] >> 40);
       L.h = (int)h;
-      normalised_model(P, L.H, s.Hn);
+      normalised_model(P, L.model, s.Hn);
     }
     __syncthreads();
     loh_refine(s, P, pts, P.n, (double)a.g.thr2, GEO_LO_STEPS, t);
     loh_rescore(s, P, pts, a.g.thr2, t);
     if (t == 0 && (s.score & LO_SCORE_MASK) < L.score) {
-      for (int i = 0; i < 9; ++i) L.H[i] = s.Ho[i];
+      for (int i = 0; i < 9; ++i) L.model[i] = s.Ho[i];
       L.score = s.score & LO_SCORE_MASK;
       L.count = (int)(s.score >> 40);
       L.nlo = L.nlo + 1;
@@ -298,10 +226,10 @@ __global__ void __launch_bounds__(RED, 1) loh_kernel(LohArgs a, int c) {
 }
 
 // Final refinement and the outputs (header steps LH6, LH8)
-__global__ void __launch_bounds__(RED, 1) loh_final_kernel(LohArgs a) {
+__global__ void __launch_bounds__(RED, 1) loh_final_kernel(LoHfArgs a) {
   const int b = blockIdx.x, t = threadIdx.x;
   const GeoPair& P = a.g.w.pair[b];
-  const LohPair& L = a.l.pair[b];
+  const LoHfPair& L = a.l.pair[b];
   const GeoOutputs& o = a.g.out;
   uint8_t* inl = o.inliers + (long)b * a.g.M;
   for (int i = t; i < a.g.M; i += RED) inl[i] = 0;
@@ -320,14 +248,14 @@ __global__ void __launch_bounds__(RED, 1) loh_final_kernel(LohArgs a) {
   __shared__ LohShared s;
   const float4* pts = a.g.w.pts + (long)b * a.g.M;
   const int* idx = a.g.w.idx + (long)b * a.g.M;
-  if (t == 0) normalised_model(P, L.H, s.Hn);
+  if (t == 0) normalised_model(P, L.model, s.Hn);
   __syncthreads();
   loh_refine(s, P, pts, P.n, (double)a.g.thr2, GEO_LO_FINAL_STEPS, t);
   loh_rescore(s, P, pts, a.g.thr2, t);
   if (t == 0 && (s.score & LO_SCORE_MASK) > L.score) {  // the refinement is kept unless its score rises
     for (int i = 0; i < 9; ++i) {
-      s.Ho[i] = L.H[i];
-      s.fm[i] = (float)L.H[i];
+      s.Ho[i] = L.model[i];
+      s.fm[i] = (float)L.model[i];
     }
     s.score = (unsigned long long)L.count * LO_COUNT_ONE + L.score;
   }
@@ -350,8 +278,8 @@ __global__ void __launch_bounds__(RED, 1) loh_final_kernel(LohArgs a) {
 extern "C" size_t geo_lo_homography_workspace_bytes(int32_t B, int32_t M, int32_t) {
   if (B < 0 || M < 0) return 0;
   GeoWs w;
-  LohWs l;
-  return loh_carve(nullptr, B, M, &w, &l) + 256;
+  LoHfWs l;
+  return lohf_carve(nullptr, B, M, &w, &l) + 256;
 }
 
 extern "C" int geo_homography_lo(const GeoConfig* cfg, const GeoInputs* in, GeoLoOutputs* out, void* workspace,
@@ -376,8 +304,8 @@ extern "C" int geo_homography_lo(const GeoConfig* cfg, const GeoInputs* in, GeoL
     return lg_set_error("geo_homography_lo: null input");
   if (!workspace || workspace_bytes < geo_lo_homography_workspace_bytes(in->B, in->M, cfg->max_iters))
     return lg_set_error("geo_homography_lo: workspace too small");
-  LohArgs a{};
-  loh_carve((char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255), in->B, in->M, &a.g.w, &a.l);
+  LoHfArgs a{};
+  lohf_carve((char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255), in->B, in->M, &a.g.w, &a.l);
   GeoArgs& g = a.g;
   g.B = in->B; g.M = in->M; g.N = in->N;
   g.kind = GEO_HOMOGRAPHY;
@@ -400,9 +328,9 @@ extern "C" int geo_homography_lo(const GeoConfig* cfg, const GeoInputs* in, GeoL
   geo_prepare_kernel<<<g.B, 1024, 0, stream>>>(g);
   LG_CHECK_LAUNCH();
   for (int c = 0; c < g.chunks; ++c) {
-    loh_hyp_kernel<<<g.B, GEO_CHUNK, 0, stream>>>(a, c);
+    lohf_hyp_kernel<<<g.B, GEO_CHUNK, 0, stream>>>(a, c);
     LG_CHECK_LAUNCH();
-    loh_score_kernel<<<dim3(g.B, splits), GEO_CHUNK, 0, stream>>>(a);
+    lohf_score_kernel<GEO_HOMOGRAPHY><<<dim3(g.B, splits), GEO_CHUNK, 0, stream>>>(a);
     LG_CHECK_LAUNCH();
     loh_kernel<<<g.B, RED, 0, stream>>>(a, c);
     LG_CHECK_LAUNCH();

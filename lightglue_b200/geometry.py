@@ -1,9 +1,9 @@
-"""Geometric verification on the GPU: batched RANSAC homography (plain and LO-RANSAC), fundamental-matrix,
-relative-pose (plain and LO-RANSAC) and absolute-pose estimation on the matcher's output (C ABI
-``include/geometry_b200.h``, CUDA ``csrc/geo_api.cu``, ``csrc/lo_homography_api.cu``, ``csrc/pose_api.cu``,
-``csrc/lo_pose_api.cu`` and ``csrc/pnp_api.cu``).
+"""Geometric verification on the GPU: batched RANSAC homography and fundamental-matrix (each plain and
+LO-RANSAC), relative-pose (plain and LO-RANSAC) and absolute-pose estimation on the matcher's output (C ABI
+``include/geometry_b200.h``, CUDA ``csrc/geo_api.cu``, ``csrc/lo_homography_api.cu``, ``csrc/lo_fundamental_api.cu``,
+``csrc/pose_api.cu``, ``csrc/lo_pose_api.cu`` and ``csrc/pnp_api.cu``).
 
-All six functions take ``matches0`` [B, M] int64 exactly as ``LightGlue.forward``, ``PendingMatch.tensors`` and
+All seven functions take ``matches0`` [B, M] int64 exactly as ``LightGlue.forward``, ``PendingMatch.tensors`` and
 ``match_ragged`` give it (-1 or any index outside [0, N) is unmatched), run every pair of the batch in one call on the
 current stream, and return device tensors of fixed shapes without synchronising with the host, so a call can follow a
 matcher forward with no read-back in between, or be captured in a CUDA graph.  A match whose keypoint in either image,
@@ -16,7 +16,8 @@ not count towards the pair's matches.  Parameter names and defaults are those of
 entry positive), ``inliers`` [B, M] bool, ``num_inliers`` [B] int32, ``success`` [B] bool, and the diagnostics
 ``best_hypothesis`` [B] int32 (-1 without one) and ``num_hypotheses`` [B] int32.  A failed pair (fewer valid matches than
 the sample size, 4 or 8, or no non-degenerate hypothesis) has ``success`` False, a zero model and no inliers.
-``find_homography_lo`` returns the keys of ``find_homography`` plus ``num_local_optimizations`` and ``cost``.
+``find_homography_lo`` and ``find_fundamental_lo`` return the keys of ``find_homography`` and ``find_fundamental`` plus
+``num_local_optimizations`` and ``cost``.
 """
 from __future__ import annotations
 
@@ -90,10 +91,12 @@ def _estimate(kind: int, key: str, kpts0, kpts1, matches0, threshold, max_iters,
                                                                 "best_hypothesis", "num_hypotheses")))
         stream = torch.cuda.current_stream(device).cuda_stream
         if lo:
-            ws = torch.empty(lib.geo_lo_homography_workspace_bytes(b, m, max_iters), dtype=torch.uint8, device=device)
+            name = "homography" if kind == _cabi.GEO_HOMOGRAPHY else "fundamental"
+            ws_bytes, entry = getattr(lib, f"geo_lo_{name}_workspace_bytes"), f"geo_{name}_lo"
+            ws = torch.empty(ws_bytes(b, m, max_iters), dtype=torch.uint8, device=device)
             louts = _cabi.GeoLoOutputs(outs, out["num_local_optimizations"].data_ptr(), out["cost"].data_ptr())
-            _cabi.check(lib.geo_homography_lo(C.byref(cfg), C.byref(ins), C.byref(louts), ws.data_ptr(), ws.numel(),
-                                              stream), "geo_homography_lo")
+            _cabi.check(getattr(lib, entry)(C.byref(cfg), C.byref(ins), C.byref(louts), ws.data_ptr(), ws.numel(),
+                                            stream), entry)
         else:
             ws = torch.empty(lib.geo_workspace_bytes(b, m, max_iters), dtype=torch.uint8, device=device)
             _cabi.check(lib.geo_estimate(C.byref(cfg), C.byref(ins), C.byref(outs), ws.data_ptr(), ws.numel(),
@@ -133,6 +136,25 @@ def find_fundamental(kpts0: torch.Tensor, kpts1: torch.Tensor, matches0: torch.T
     ``cv2.findFundamentalMat(method=cv2.FM_RANSAC)``."""
     return _estimate(_cabi.GEO_FUNDAMENTAL, "F", kpts0, kpts1, matches0, ransac_reproj_threshold, max_iters, confidence,
                      seed)
+
+
+def find_fundamental_lo(kpts0: torch.Tensor, kpts1: torch.Tensor, matches0: torch.Tensor,
+                        ransac_reproj_threshold: float = 3.0, max_iters: int = 1000, confidence: float = 0.99,
+                        seed: int = 0) -> dict:
+    """LO-RANSAC fundamental matrix per pair: the samples and eight-point hypotheses of ``find_fundamental``, scored by
+    a truncated (MSAC) epipolar-distance cost, with Levenberg-Marquardt local optimisation of a rank-2 F on the Sampson
+    error after each chunk of 256 samples that improves the best model, and a final Levenberg-Marquardt refinement.
+    The accuracy of PoseLib's and OpenCV's USAC LO-RANSAC, on the GPU; ``find_fundamental`` stays the one that follows
+    ``cv2.FM_RANSAC``.  Arguments and defaults are ``find_fundamental``'s, so the two compare like for like; at most
+    2**20 - 1 rows of ``matches0`` per pair.
+
+    Returns the keys of ``find_fundamental`` (``F`` the final model: rank 2, unit Frobenius norm, largest entry
+    positive; ``inliers`` the points whose larger distance to their two epipolar lines under that F is below the
+    threshold; ``best_hypothesis`` the sample the final model grew from) plus ``num_local_optimizations`` [B] int32, the
+    local optimisations whose model was adopted, and ``cost`` [B] int64, the final model's integer MSAC score.
+    Failures are those of ``find_fundamental``, with ``num_local_optimizations`` and ``cost`` 0."""
+    return _estimate(_cabi.GEO_FUNDAMENTAL, "F", kpts0, kpts1, matches0, ransac_reproj_threshold, max_iters, confidence,
+                     seed, lo=True)
 
 
 def _intrinsics(name: str, K, b: int, device) -> torch.Tensor:

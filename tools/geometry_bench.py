@@ -2,13 +2,15 @@
 
 Prints one JSON line:
   * the card's name and power limit, read in this run;
-  * GPU ms per batch (CUDA events) for find_homography, find_homography_lo ("lo_adaptive", "lo_full") and
-    find_fundamental at B pairs of M putative matches, inlier ratios 0.8 / 0.5 / 0.3, with OpenCV's adaptive stopping
-    ("adaptive") and with confidence 1 ("full", every hypothesis);
-  * OpenCV on the host for the same pairs, one after another and in a thread pool (null without cv2); for H also
-    cv2.findHomography(USAC_ACCURATE), the LO-RANSAC that find_homography_lo is compared with ("opencv_usac_accurate");
-  * pairs/s of LightGlue (bf16x3, N = 2048, synthetic weights) alone and followed by find_fundamental or
-    find_homography_lo on one stream, the runs alternated.
+  * GPU ms per batch (CUDA events) for find_homography and find_fundamental, and for their LO-RANSAC variants
+    find_homography_lo and find_fundamental_lo ("lo_adaptive", "lo_full"), at B pairs of M putative matches, inlier
+    ratios 0.8 / 0.5 / 0.3, with OpenCV's adaptive stopping ("adaptive") and with confidence 1 ("full", every
+    hypothesis);
+  * OpenCV on the host for the same pairs, one after another and in a thread pool (null without cv2), and
+    cv2.findHomography / cv2.findFundamentalMat(USAC_ACCURATE), the LO-RANSAC the LO variants are compared with
+    ("opencv_usac_accurate");
+  * pairs/s of LightGlue (bf16x3, N = 2048, synthetic weights) alone and followed by find_fundamental,
+    find_homography_lo or find_fundamental_lo on one stream, the runs alternated.
 The scenes come from oracle/geometry_synth.py (0.5 px noise, 640x480); nothing is written to disk.
 """
 from __future__ import annotations
@@ -27,10 +29,12 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 from lightglue_b200 import LightGlue, synth  # noqa: E402
-from lightglue_b200.geometry import find_fundamental, find_homography, find_homography_lo  # noqa: E402
+from lightglue_b200.geometry import (find_fundamental, find_fundamental_lo, find_homography,  # noqa: E402
+                                     find_homography_lo)
 from oracle import geometry_synth as gs  # noqa: E402
 
 DEFAULTS = {"H": (find_homography, 2000, 0.995), "F": (find_fundamental, 1000, 0.99)}
+LO = {"H": find_homography_lo, "F": find_fundamental_lo}
 
 
 def gpu_info() -> dict:
@@ -70,7 +74,7 @@ def opencv_times(key, k0, k1, m0, threads, usac=False):
         if key == "H":
             cv2.findHomography(a, c, cv2.USAC_ACCURATE if usac else cv2.RANSAC, 3.0, maxIters=iters, confidence=conf)
         else:
-            cv2.findFundamentalMat(a, c, cv2.FM_RANSAC, 3.0, conf, iters)
+            cv2.findFundamentalMat(a, c, cv2.USAC_ACCURATE if usac else cv2.FM_RANSAC, 3.0, conf, iters)
 
     t = time.perf_counter()
     for b in range(len(m0)):
@@ -105,16 +109,15 @@ def main() -> None:
                 row[mode] = {"gpu_ms": round(time_gpu(lambda: fn(t0, t1, tm, confidence=c), args.reps), 3),
                              "mean_hypotheses": float(out["num_hypotheses"].float().mean()),
                              "mean_inliers": float(out["num_inliers"].float().mean())}
-                if key == "H":
-                    out = find_homography_lo(t0, t1, tm, confidence=c)
-                    row["lo_" + mode] = {
-                        "gpu_ms": round(time_gpu(lambda: find_homography_lo(t0, t1, tm, confidence=c), args.reps), 3),
-                        "mean_hypotheses": float(out["num_hypotheses"].float().mean()),
-                        "mean_inliers": float(out["num_inliers"].float().mean()),
-                        "mean_local_optimizations": float(out["num_local_optimizations"].float().mean())}
+                lo = LO[key]
+                out = lo(t0, t1, tm, confidence=c)
+                row["lo_" + mode] = {
+                    "gpu_ms": round(time_gpu(lambda: lo(t0, t1, tm, confidence=c), args.reps), 3),
+                    "mean_hypotheses": float(out["num_hypotheses"].float().mean()),
+                    "mean_inliers": float(out["num_inliers"].float().mean()),
+                    "mean_local_optimizations": float(out["num_local_optimizations"].float().mean())}
             row["opencv"] = opencv_times(key, k0, k1, m0, threads)
-            if key == "H":
-                row["opencv_usac_accurate"] = opencv_times(key, k0, k1, m0, threads, usac=True)
+            row["opencv_usac_accurate"] = opencv_times(key, k0, k1, m0, threads, usac=True)
             res["ransac"][f"{key}_inliers{inl}"] = row
     # the matcher alone, and followed by find_fundamental on its device output (no host read-back in between)
     data, _ = synth.make_pair(2048, b=args.batch, seed=7)
@@ -134,9 +137,14 @@ def main() -> None:
         m0 = m.forward_async(cuda).tensors["matches0"]
         return find_homography_lo(cuda["image0"]["keypoints"], cuda["image1"]["keypoints"], m0)
 
+    def matcher_lo_fundamental():
+        m0 = m.forward_async(cuda).tensors["matches0"]
+        return find_fundamental_lo(cuda["image0"]["keypoints"], cuda["image1"]["keypoints"], m0)
+
     for name, f in (("lightglue", matcher_only), ("lightglue_plus_fundamental", matcher_ransac),
                     ("lightglue_again", matcher_only), ("lightglue_plus_homography_lo", matcher_lo_homography),
-                    ("lightglue_again2", matcher_only)):
+                    ("lightglue_again2", matcher_only), ("lightglue_plus_fundamental_lo", matcher_lo_fundamental),
+                    ("lightglue_again3", matcher_only)):
         ms = time_gpu(f, args.steps)
         res[f"{name}_pairs_per_s"] = round(args.batch / ms * 1e3, 1)
     print(json.dumps(res))
