@@ -1,16 +1,26 @@
-// Device helpers shared by the H/F RANSAC (geo_api.cu) and the relative pose (pose_api.cu), both compiled with
-// -fmad=false.  include/geometry_b200.h states each step; oracle/geometry_oracle.py and oracle/pose_oracle.py restate
-// them in numpy.
+// Helpers shared by every geometry estimator (geo_api.cu, pose_api.cu, lo_pose_api.cu, lo_hf_api.cu, pnp_api.cu), all
+// compiled with -fmad=false.  include/geometry_b200.h states each step; oracle/geometry_oracle.py and
+// oracle/pose_oracle.py restate them in numpy.
 #pragma once
 #include <cuda_runtime.h>
 #include <float.h>
 #include <math.h>
 
 #include "../../include/geometry_b200.h"
+#include "lg_internal.h"
 
 namespace {
 
 constexpr int RED = 256;  // partial sums of the fixed summation order (header step 2)
+
+// Score CTAs per pair of every estimator's score kernel: enough to cover the SMs twice, with at least 128 points each
+int geo_score_splits(int B, int M) {
+  const int want = (2 * lg_num_sms() + B - 1) / B;
+  int splits = (M + 127) / 128;
+  if (splits > want) splits = want;
+  if (splits < 1) splits = 1;
+  return splits;
+}
 
 // A keypoint with a non-finite coordinate makes its match invalid at compaction (header steps 1, P1 and A1)
 __device__ __forceinline__ bool finite2(float2 p) { return isfinite(p.x) && isfinite(p.y); }

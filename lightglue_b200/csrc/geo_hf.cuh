@@ -1,7 +1,7 @@
 // The H/F RANSAC's shared pieces (include/geometry_b200.h, steps 1-5): the workspace, the compaction and Hartley
 // normalisation kernel, the sampler and minimal solvers, and the fp32 error.  Included by geo_api.cu (RANSAC, steps
-// 1-7), lo_homography_api.cu (LO-RANSAC homography, LH1-LH8) and lo_fundamental_api.cu (LO-RANSAC fundamental
-// matrix, LF1-LF8), all compiled with -fmad=false.
+// 1-7) and lo_hf_api.cu (LO-RANSAC homography and fundamental matrix, LH1-LH8 and LF1-LF8), both compiled with
+// -fmad=false.
 #pragma once
 #include <stdint.h>
 

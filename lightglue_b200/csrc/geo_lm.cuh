@@ -1,5 +1,5 @@
 // Levenberg-Marquardt pieces shared by the absolute pose (pnp_api.cu, header step A7) and the LO-RANSAC relative pose,
-// homography and fundamental matrix (lo_pose_api.cu, lo_homography_api.cu and lo_fundamental_api.cu, header steps L7,
+// homography and fundamental matrix (lo_pose_api.cu and lo_hf_api.cu through lo_common.cuh, header steps L7,
 // LH7 and LF7), all compiled with -fmad=false.
 #pragma once
 #include <cuda_runtime.h>

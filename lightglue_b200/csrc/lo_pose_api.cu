@@ -47,8 +47,6 @@ __device__ __forceinline__ void projection34(const double* R, const double* tv, 
   }
 }
 
-constexpr int LO_TERMS = 21;  // J^T J upper triangle (15), J^T r (5), truncated cost
-
 struct LoPair {
   double R[9], t[3];         // the pair's model
   unsigned long long score;  // its L3 score
@@ -98,19 +96,6 @@ __device__ void tangent_basis(const double* t, double* b1, double* b2) {
   cross3(t, b1, b2);
 }
 
-// Shared state of one pair's CTA in the LO and final kernels
-struct LoShared {
-  double red[LO_TERMS][RED];
-  double pose[12], cand[12];           // R, t of the model being refined and of the LM step's candidate
-  double sums[LO_TERMS], csum[LO_TERMS];
-  double E[9], dE[5][9];               // [t]x R and its derivatives at the pose being summed
-  double Rs[2][9], ts[3];              // P7 candidates
-  double Eo[9];                        // the scaled E of the last re-scored pose
-  float fm[9];                         // a model rounded to float
-  unsigned long long key, score;
-  int good[4], count, step_ok;
-};
-
 __device__ __forceinline__ void lo_epipolar(const double* E, double x, double y, double u, double v, double* a0, double* a1,
                                             double* b0, double* b1, double* d) {
   *a0 = (E[0] * x + E[1] * y) + E[2];
@@ -121,115 +106,89 @@ __device__ __forceinline__ void lo_epipolar(const double* E, double x, double y,
   *b1 = (E[1] * u + E[4] * v) + E[7];
 }
 
-// The LO_TERMS sums at pose (R, t) (header step L7) into out
-__device__ void lo_terms(LoShared& s, const double* pose, const float4* pts, int n, double thr2, double* out, int tid) {
-  if (tid == 0) {
-    const double* R = pose;
-    const double* t = pose + 9;
-    cross_columns(t, R, s.E);
-    for (int k = 0; k < 3; ++k) {
-      const double e[3] = {k == 0 ? 1.0 : 0.0, k == 1 ? 1.0 : 0.0, k == 2 ? 1.0 : 0.0};
-      double G[9];
-      cross_columns(e, R, G);
-      cross_columns(t, G, s.dE[k]);
-    }
-    double b1[3], b2[3];
-    tangent_basis(t, b1, b2);
-    cross_columns(b1, R, s.dE[3]);
-    cross_columns(b2, R, s.dE[4]);
-  }
-  __syncthreads();
-  double acc[LO_TERMS];
-#pragma unroll
-  for (int i = 0; i < LO_TERMS; ++i) acc[i] = 0.0;
-  for (int k = tid; k < n; k += RED) {
-    const float4 p = pts[k];
-    const double x = p.x, y = p.y, u = p.z, v = p.w;
-    double a0, a1, b0, b1, d;
-    lo_epipolar(s.E, x, y, u, v, &a0, &a1, &b0, &b1, &d);
-    const double den = ((a0 * a0 + a1 * a1) + b0 * b0) + b1 * b1;
-    const double err = (d * d) / den;
-    const bool in = err < thr2;
-    acc[20] = acc[20] + (in ? err : thr2);
-    if (!in) continue;
-    const double sq = sqrt(den);
-    const double r = d / sq;
-    double J[5];
-#pragma unroll
-    for (int q = 0; q < 5; ++q) {
-      double da0, da1, db0, db1, dd;
-      lo_epipolar(s.dE[q], x, y, u, v, &da0, &da1, &db0, &db1, &dd);
-      const double dden = ((a0 * da0 + a1 * da1) + b0 * db0) + b1 * db1;
-      J[q] = (dd - d * dden / den) / sq;
-    }
-    int e = 0;
-#pragma unroll
-    for (int i = 0; i < 5; ++i)
-#pragma unroll
-      for (int j = i; j < 5; ++j, ++e) acc[e] = acc[e] + J[i] * J[j];
-#pragma unroll
-    for (int i = 0; i < 5; ++i) acc[15 + i] = acc[15 + i] + J[i] * r;
-  }
-  lo_tree_sums<LO_TERMS>(acc, s.red, out, tid);
-}
+// The relative pose for lo_common.cuh's LM loop and re-score: x = R, t (header step L7)
+struct PoseLo {
+  static constexpr int DOF = 5, TERMS = 21, GROUP = 21, NP = 12;
+  struct Scratch {
+    double E[9], dE[5][9];   // [t]x R and its derivatives at the pose being summed
+    double Rs[2][9], ts[3];  // P7 candidates
+    int good[4], count;
+  };
 
-// R' = Q(d0..2) R, t' = normalize(t + d3 b1 + d4 b2) (header step L7)
-__device__ void lo_update(const double* pose, const double* d, double* out) {
-  double Q[9], b1[3], b2[3], v[3];
-  quat_rotation(d, Q);
-  for (int i = 0; i < 3; ++i)
-    for (int j = 0; j < 3; ++j) out[3 * i + j] = Q[3 * i] * pose[j] + Q[3 * i + 1] * pose[3 + j] + Q[3 * i + 2] * pose[6 + j];
-  tangent_basis(pose + 9, b1, b2);
-  for (int i = 0; i < 3; ++i) v[i] = (pose[9 + i] + d[3] * b1[i]) + d[4] * b2[i];
-  const double nv = sqrt((v[0] * v[0] + v[1] * v[1]) + v[2] * v[2]);
-  for (int i = 0; i < 3; ++i) out[9 + i] = v[i] / nv;
-}
-
-// steps LM steps from s.pose, in place (header step L7); every thread of the CTA calls it
-__device__ void lo_refine(LoShared& s, const float4* pts, int n, double thr2, int steps, int tid) {
-  lo_terms(s, s.pose, pts, n, thr2, s.sums, tid);
-  double lam = GEO_LO_LAMBDA0;  // every thread keeps the same schedule
-  for (int it = 0; it < steps; ++it) {
+  // The TERMS sums at pose (R, t) (header step L7) into out
+  static __device__ void terms(LoShared<PoseLo>& s, const PosePair&, const double* pose, const float4* pts, int n,
+                               double thr2, double* out, int tid) {
     if (tid == 0) {
-      double d[5];
-      s.step_ok = lm_solve<5>(s.sums, s.sums + 15, lam, d);
-      if (s.step_ok) lo_update(s.pose, d, s.cand);
+      const double* R = pose;
+      const double* t = pose + 9;
+      cross_columns(t, R, s.m.E);
+      for (int k = 0; k < 3; ++k) {
+        const double e[3] = {k == 0 ? 1.0 : 0.0, k == 1 ? 1.0 : 0.0, k == 2 ? 1.0 : 0.0};
+        double G[9];
+        cross_columns(e, R, G);
+        cross_columns(t, G, s.m.dE[k]);
+      }
+      double b1[3], b2[3];
+      tangent_basis(t, b1, b2);
+      cross_columns(b1, R, s.m.dE[3]);
+      cross_columns(b2, R, s.m.dE[4]);
     }
     __syncthreads();
-    if (!s.step_ok) {
-      lam = lam * 10.0;
-      __syncthreads();
-      continue;
+    double acc[TERMS];
+#pragma unroll
+    for (int i = 0; i < TERMS; ++i) acc[i] = 0.0;
+    for (int k = tid; k < n; k += RED) {
+      const float4 p = pts[k];
+      const double x = p.x, y = p.y, u = p.z, v = p.w;
+      double a0, a1, b0, b1, d;
+      lo_epipolar(s.m.E, x, y, u, v, &a0, &a1, &b0, &b1, &d);
+      const double den = ((a0 * a0 + a1 * a1) + b0 * b0) + b1 * b1;
+      const double err = (d * d) / den;
+      const bool in = err < thr2;
+      acc[20] = acc[20] + (in ? err : thr2);
+      if (!in) continue;
+      const double sq = sqrt(den);
+      const double r = d / sq;
+      double J[5];
+#pragma unroll
+      for (int q = 0; q < 5; ++q) {
+        double da0, da1, db0, db1, dd;
+        lo_epipolar(s.m.dE[q], x, y, u, v, &da0, &da1, &db0, &db1, &dd);
+        const double dden = ((a0 * da0 + a1 * da1) + b0 * db0) + b1 * db1;
+        J[q] = (dd - d * dden / den) / sq;
+      }
+      int e = 0;
+#pragma unroll
+      for (int i = 0; i < 5; ++i)
+#pragma unroll
+        for (int j = i; j < 5; ++j, ++e) acc[e] = acc[e] + J[i] * J[j];
+#pragma unroll
+      for (int i = 0; i < 5; ++i) acc[15 + i] = acc[15 + i] + J[i] * r;
     }
-    lo_terms(s, s.cand, pts, n, thr2, s.csum, tid);
-    const bool better = s.csum[20] < s.sums[20];
-    __syncthreads();
-    if (better) {
-      if (tid < 12) s.pose[tid] = s.cand[tid];
-      if (tid < LO_TERMS) s.sums[tid] = s.csum[tid];
-      lam = lam / 10.0;
-    } else {
-      lam = lam * 10.0;
-    }
-    __syncthreads();
+    lo_tree_sums<TERMS, GROUP>(acc, s.red, out, tid);
   }
-}
 
-// L3 score and count of E = [t]x R of pose, scaled as P3 (s.Eo) and rounded to float (s.fm)
-__device__ void lo_rescore(LoShared& s, const double* pose, const float4* pts, int n, float thr2, int tid) {
-  if (tid == 0) {
-    cross_columns(pose + 9, pose, s.Eo);
-    unit_scale(s.Eo);
-    for (int i = 0; i < 9; ++i) s.fm[i] = (float)s.Eo[i];
-    s.score = 0;
+  // R' = Q(d0..2) R, t' = normalize(t + d3 b1 + d4 b2) (header step L7)
+  static __device__ void update(LoShared<PoseLo>&, const double* pose, const double* d, double* out) {
+    double Q[9], b1[3], b2[3], v[3];
+    quat_rotation(d, Q);
+    for (int i = 0; i < 3; ++i)
+      for (int j = 0; j < 3; ++j)
+        out[3 * i + j] = Q[3 * i] * pose[j] + Q[3 * i + 1] * pose[3 + j] + Q[3 * i + 2] * pose[6 + j];
+    tangent_basis(pose + 9, b1, b2);
+    for (int i = 0; i < 3; ++i) v[i] = (pose[9 + i] + d[3] * b1[i]) + d[4] * b2[i];
+    const double nv = sqrt((v[0] * v[0] + v[1] * v[1]) + v[2] * v[2]);
+    for (int i = 0; i < 3; ++i) out[9 + i] = v[i] / nv;
   }
-  __syncthreads();
-  const float w = (float)GEO_LO_QSCALE / thr2;
-  unsigned long long acc = 0;
-  for (int k = tid; k < n; k += RED) acc += lo_term(sampson(s.fm, pts[k]), thr2, w);
-  if (acc) atomicAdd(&s.score, acc);
-  __syncthreads();
-}
+
+  // E = [t]x R scaled as P3
+  static __device__ void pixels(LoShared<PoseLo>&, const PosePair&, const double* pose, double* out) {
+    cross_columns(pose + 9, pose, out);
+    unit_scale(out);
+  }
+
+  static __device__ __forceinline__ float err(const float* h, float4 p) { return sampson(h, p); }
+};
 
 __global__ void __launch_bounds__(GEO_CHUNK, 1) lo_hyp_kernel(LoArgs a, int c) {
   const int b = blockIdx.x, t = threadIdx.x;
@@ -292,14 +251,14 @@ __global__ void __launch_bounds__(GEO_CHUNK) lo_score_kernel(LoArgs a) {
     if (r < ns && k[r]) atomicAdd(a.l.acc + ((long)b * GEO_CHUNK + t) * SOLS + r, k[r]);
 }
 
-// P7's choice among the candidates of s.fm (widened) on s.fm's inliers, into s.pose; every thread calls it
-__device__ void lo_choose_pose(LoShared& s, const float4* pts, int n, float thr2, double distance, int tid) {
+// P7's choice among the candidates of s.fm (widened) on s.fm's inliers, into s.x; every thread calls it
+__device__ void lo_choose_pose(LoShared<PoseLo>& s, const float4* pts, int n, float thr2, double distance, int tid) {
   if (tid == 0) {
     double E[9];
     for (int i = 0; i < 9; ++i) E[i] = s.fm[i];
-    pose_candidates(E, s.Rs, s.ts);
+    pose_candidates(E, s.m.Rs, s.m.ts);
   }
-  if (tid < 4) s.good[tid] = 0;
+  if (tid < 4) s.m.good[tid] = 0;
   __syncthreads();
   int cnt[4] = {0, 0, 0, 0};
   for (int k = tid; k < n; k += RED) {
@@ -307,20 +266,20 @@ __device__ void lo_choose_pose(LoShared& s, const float4* pts, int n, float thr2
     if (!(sampson(s.fm, p) < thr2)) continue;
     for (int c = 0; c < 4; ++c) {
       const double sg = c < 2 ? 1.0 : -1.0;
-      const double tv[3] = {sg * s.ts[0], sg * s.ts[1], sg * s.ts[2]};
+      const double tv[3] = {sg * s.m.ts[0], sg * s.m.ts[1], sg * s.m.ts[2]};
       double P1[3][4];
-      projection34(s.Rs[c & 1], tv, P1);
+      projection34(s.m.Rs[c & 1], tv, P1);
       cnt[c] += cheirality_pass(P1, p.x, p.y, p.z, p.w, distance);
     }
   }
   for (int c = 0; c < 4; ++c)
-    if (cnt[c]) atomicAdd(&s.good[c], cnt[c]);
+    if (cnt[c]) atomicAdd(&s.m.good[c], cnt[c]);
   __syncthreads();
   int best = 0;
   for (int c = 1; c < 4; ++c)
-    if (s.good[c] > s.good[best]) best = c;
-  if (tid < 9) s.pose[tid] = s.Rs[best & 1][tid];
-  if (tid < 3) s.pose[9 + tid] = (best < 2 ? 1.0 : -1.0) * s.ts[tid];
+    if (s.m.good[c] > s.m.good[best]) best = c;
+  if (tid < 9) s.x[tid] = s.m.Rs[best & 1][tid];
+  if (tid < 3) s.x[9 + tid] = (best < 2 ? 1.0 : -1.0) * s.m.ts[tid];
   __syncthreads();
 }
 
@@ -330,7 +289,7 @@ __global__ void __launch_bounds__(RED, 1) lo_kernel(LoArgs a, int c) {
   PosePair& P = a.p.w.pair[b];
   if (P.stop) return;
   LoPair& L = a.l.pair[b];
-  __shared__ LoShared s;
+  __shared__ LoShared<PoseLo> s;
   if (t == 0) s.key = ~0ull;
   __syncthreads();
   if (t < GEO_CHUNK) {
@@ -351,17 +310,17 @@ __global__ void __launch_bounds__(RED, 1) lo_kernel(LoArgs a, int c) {
     __syncthreads();
     lo_choose_pose(s, pts, P.n, P.thr2, a.p.distance, t);
     if (t == 0) {
-      for (int i = 0; i < 9; ++i) L.R[i] = s.pose[i];
-      for (int i = 0; i < 3; ++i) L.t[i] = s.pose[9 + i];
+      for (int i = 0; i < 9; ++i) L.R[i] = s.x[i];
+      for (int i = 0; i < 3; ++i) L.t[i] = s.x[9 + i];
       L.score = key >> 28;
       L.count = (int)(a.l.acc[slot * SOLS + (hr & 15)] >> 40);
       L.hr = (int)hr;
     }
-    lo_refine(s, pts, P.n, (double)P.thr2, GEO_LO_STEPS, t);
-    lo_rescore(s, s.pose, pts, P.n, P.thr2, t);
+    lo_refine(s, P, pts, P.n, (double)P.thr2, GEO_LO_STEPS, t);
+    lo_rescore(s, P, pts, P.n, P.thr2, t);
     if (t == 0 && (s.score & LO_SCORE_MASK) < L.score) {
-      for (int i = 0; i < 9; ++i) L.R[i] = s.pose[i];
-      for (int i = 0; i < 3; ++i) L.t[i] = s.pose[9 + i];
+      for (int i = 0; i < 9; ++i) L.R[i] = s.x[i];
+      for (int i = 0; i < 3; ++i) L.t[i] = s.x[9 + i];
       L.score = s.score & LO_SCORE_MASK;
       L.count = (int)(s.score >> 40);
       L.nlo = L.nlo + 1;
@@ -398,27 +357,27 @@ __global__ void __launch_bounds__(RED, 1) lo_final_kernel(LoArgs a) {
     }
     return;
   }
-  __shared__ LoShared s;
+  __shared__ LoShared<PoseLo> s;
   const float4* pts = a.p.w.pts + (long)b * a.p.M;
   const int* idx = a.p.w.idx + (long)b * a.p.M;
-  if (t < 9) s.pose[t] = L.R[t];
-  if (t < 3) s.pose[9 + t] = L.t[t];
+  if (t < 9) s.x[t] = L.R[t];
+  if (t < 3) s.x[9 + t] = L.t[t];
   __syncthreads();
-  lo_refine(s, pts, P.n, (double)P.thr2, GEO_LO_FINAL_STEPS, t);
-  lo_rescore(s, s.pose, pts, P.n, P.thr2, t);
+  lo_refine(s, P, pts, P.n, (double)P.thr2, GEO_LO_FINAL_STEPS, t);
+  lo_rescore(s, P, pts, P.n, P.thr2, t);
   const bool keep = (s.score & LO_SCORE_MASK) <= L.score;
   __syncthreads();
   if (!keep) {
-    if (t < 9) s.pose[t] = L.R[t];
-    if (t < 3) s.pose[9 + t] = L.t[t];
+    if (t < 9) s.x[t] = L.R[t];
+    if (t < 3) s.x[9 + t] = L.t[t];
     __syncthreads();
-    lo_rescore(s, s.pose, pts, P.n, P.thr2, t);
+    lo_rescore(s, P, pts, P.n, P.thr2, t);
   }
-  if (t == 0) s.count = 0;
+  if (t == 0) s.m.count = 0;
   __syncthreads();
   int cnt = 0;
   double P1[3][4];
-  projection34(s.pose, s.pose + 9, P1);
+  projection34(s.x, s.x + 9, P1);
   for (int k = t; k < P.n; k += RED) {
     const float4 p = pts[k];
     if (!(sampson(s.fm, p) < P.thr2)) continue;
@@ -428,16 +387,16 @@ __global__ void __launch_bounds__(RED, 1) lo_final_kernel(LoArgs a) {
       ++cnt;
     }
   }
-  if (cnt) atomicAdd(&s.count, cnt);
+  if (cnt) atomicAdd(&s.m.count, cnt);
   __syncthreads();
   if (t < 9) {
-    o.E[(long)b * 9 + t] = s.Eo[t];
-    o.R[(long)b * 9 + t] = s.pose[t];
+    o.E[(long)b * 9 + t] = s.px[t];
+    o.R[(long)b * 9 + t] = s.x[t];
   }
-  if (t < 3) o.t[(long)b * 3 + t] = s.pose[9 + t];
+  if (t < 3) o.t[(long)b * 3 + t] = s.x[9 + t];
   if (t == 0) {
     o.num_inliers[b] = (int)(s.score >> 40);
-    o.num_pose_inliers[b] = s.count;
+    o.num_pose_inliers[b] = s.m.count;
     o.success[b] = 1;
     o.best_hypothesis[b] = L.hr >> 4;
     o.best_solution[b] = L.hr & 15;
@@ -496,11 +455,7 @@ extern "C" int geo_relative_pose_lo(const GeoLoPoseConfig* cfg, const GeoPoseInp
   p.out = o;
   a.num_lo = out->num_local_optimizations;
   a.cost = out->cost;
-  // the score CTAs of geo_relative_pose
-  const int want = (2 * lg_num_sms() + p.B - 1) / p.B;
-  int splits = (p.M + 127) / 128;
-  if (splits > want) splits = want;
-  if (splits < 1) splits = 1;
+  const int splits = geo_score_splits(p.B, p.M);
   const cudaStream_t stream = (cudaStream_t)stream_;
   pose_prepare_kernel<<<p.B, 1024, 0, stream>>>(p);
   LG_CHECK_LAUNCH();

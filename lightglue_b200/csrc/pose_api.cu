@@ -296,11 +296,7 @@ extern "C" int geo_relative_pose(const GeoPoseConfig* cfg, const GeoPoseInputs* 
   a.kpts0 = in->kpts0; a.kpts1 = in->kpts1; a.matches0 = in->matches0;
   a.K0 = in->K0; a.K1 = in->K1;
   a.out = *out;
-  // enough score CTAs to cover the SMs twice, with at least 128 points per slice
-  const int want = (2 * lg_num_sms() + a.B - 1) / a.B;
-  int splits = (a.M + 127) / 128;
-  if (splits > want) splits = want;
-  if (splits < 1) splits = 1;
+  const int splits = geo_score_splits(a.B, a.M);
   const cudaStream_t stream = (cudaStream_t)stream_;
   pose_prepare_kernel<<<a.B, 1024, 0, stream>>>(a);
   LG_CHECK_LAUNCH();

@@ -1,7 +1,7 @@
 """Geometric verification on the GPU: batched RANSAC homography and fundamental-matrix (each plain and
 LO-RANSAC), relative-pose (plain and LO-RANSAC) and absolute-pose estimation on the matcher's output (C ABI
-``include/geometry_b200.h``, CUDA ``csrc/geo_api.cu``, ``csrc/lo_homography_api.cu``, ``csrc/lo_fundamental_api.cu``,
-``csrc/pose_api.cu``, ``csrc/lo_pose_api.cu`` and ``csrc/pnp_api.cu``).
+``include/geometry_b200.h``, CUDA ``csrc/geo_api.cu``, ``csrc/lo_hf_api.cu``, ``csrc/pose_api.cu``,
+``csrc/lo_pose_api.cu`` and ``csrc/pnp_api.cu``).
 
 All seven functions take ``matches0`` [B, M] int64 exactly as ``LightGlue.forward``, ``PendingMatch.tensors`` and
 ``match_ragged`` give it (-1 or any index outside [0, N) is unmatched), run every pair of the batch in one call on the

@@ -1,0 +1,132 @@
+"""numpy restatement of csrc/geo_lm.cuh and lo_common.cuh: the damped Cholesky step and A7's quaternion rotation that
+every Levenberg-Marquardt refinement takes, the LM loop of the LO-RANSAC estimators (header steps L7, LH7 and LF7),
+and the chunk driver that the LO-RANSAC homography and fundamental matrix share (steps LH1-LH8 and LF1-LF8).
+
+Python floats and elementwise numpy only, so the CUDA build compiled with -fmad=false agrees bit for bit.
+"""
+from __future__ import annotations
+
+import math
+
+import numpy as np
+
+from oracle import geometry_oracle as go
+from oracle import lo_pose_oracle as lpo
+
+
+def lm_solve(h, g, lam, n):
+    """delta of (H, its diagonal times (1 + lam)) delta = -g by Cholesky for an n x n system (header step A7), H given
+    by its row-major upper triangle h; None on a pivot <= 0 or a non-finite delta."""
+    A = [[0.0] * n for _ in range(n)]
+    e = 0
+    for i in range(n):
+        for j in range(i, n):
+            A[i][j] = A[j][i] = float(h[e])
+            e += 1
+    for i in range(n):
+        A[i][i] = A[i][i] * (1.0 + lam)
+    L = [[0.0] * n for _ in range(n)]
+    for j in range(n):
+        d = A[j][j]
+        for k in range(j):
+            d = d - L[j][k] * L[j][k]
+        if not d > 0.0:
+            return None
+        L[j][j] = math.sqrt(d)
+        for i in range(j + 1, n):
+            s = A[i][j]
+            for k in range(j):
+                s = s - L[i][k] * L[j][k]
+            L[i][j] = s / L[j][j]
+    yv = [0.0] * n
+    for i in range(n):
+        s = -float(g[i])
+        for k in range(i):
+            s = s - L[i][k] * yv[k]
+        yv[i] = s / L[i][i]
+    x = [0.0] * n
+    for i in range(n - 1, -1, -1):
+        s = yv[i]
+        for k in range(i + 1, n):
+            s = s - L[k][i] * x[k]
+        x[i] = s / L[i][i]
+    return x if all(math.isfinite(v) for v in x) else None
+
+
+def quat_rotation(d):
+    """A7's row-major rotation of the unit quaternion (1, d0/2, d1/2, d2/2) / norm."""
+    qw, qx, qy, qz = 1.0, d[0] * 0.5, d[1] * 0.5, d[2] * 0.5
+    n = math.sqrt(qw * qw + qx * qx + qy * qy + qz * qz)
+    qw, qx, qy, qz = qw / n, qx / n, qy / n, qz / n
+    return [1.0 - 2.0 * (qy * qy + qz * qz), 2.0 * (qx * qy - qw * qz), 2.0 * (qx * qz + qw * qy),
+            2.0 * (qx * qy + qw * qz), 1.0 - 2.0 * (qx * qx + qz * qz), 2.0 * (qy * qz - qw * qx),
+            2.0 * (qx * qz - qw * qy), 2.0 * (qy * qz + qw * qx), 1.0 - 2.0 * (qx * qx + qy * qy)]
+
+
+def refine(terms, update, x, dof, steps: int):
+    """steps Levenberg-Marquardt steps on a truncated cost from the model x.  terms(x) gives its fixed-order sums: the
+    J^T J upper triangle, J^T r (dof each) and the cost last; update(x, d) the candidate of the step d.  A candidate is
+    taken when its cost is lower; the damping starts at LAMBDA0 and falls or rises tenfold."""
+    nh = dof * (dof + 1) // 2
+    sums = terms(x)
+    lam = lpo.LAMBDA0
+    for _ in range(steps):
+        d = lm_solve(sums[:nh], sums[nh:nh + dof], lam, dof)
+        if d is None:
+            lam = lam * 10.0
+            continue
+        cand = update(x, d)
+        cs = terms(cand)
+        if cs[-1] < sums[-1]:
+            x, sums = cand, cs
+            lam = lam / 10.0
+        else:
+            lam = lam * 10.0
+    return x
+
+
+def lo_hf_pair(kind, s, key, start, refine_model, rescore, kpts0, kpts1, m0, threshold, max_iters, confidence,
+               seed) -> dict:
+    """One pair of the LO-RANSAC homography (LH1-LH8) or fundamental matrix (LF1-LF8), kind and s its step 4 model and
+    sample size, key the output name of the model.  start(norm, model) is the LM start of a pixel model,
+    refine_model(norm, x, pts, thr2, steps) its LM and rescore(norm, x, pts, thr2) its (pixel model, score, count)."""
+    kpts0 = np.asarray(kpts0, dtype=np.float32)
+    kpts1 = np.asarray(kpts1, dtype=np.float32)
+    m0 = np.asarray(m0, dtype=np.int64)
+    M = m0.shape[0]
+    thr2 = np.float32(threshold * threshold)
+    idx, pts = go.compact(kpts0, kpts1, m0)
+    n = pts.shape[0]
+    norm = go.normalisation(pts) if n >= s else None
+    fail = {key: np.zeros((3, 3)), "inliers": np.zeros(M, dtype=bool), "num_inliers": 0, "success": False,
+            "best_hypothesis": -1, "num_hypotheses": 0, "num_local_optimizations": 0, "cost": 0}
+    if norm is None:
+        return fail
+    best, nlo, drawn = None, 0, 0  # best: (score, count, h, model)
+    for c in range(-(-max_iters // go.CHUNK)):
+        h = np.arange(c * go.CHUNK, min((c + 1) * go.CHUNK, max_iters), dtype=np.int64)
+        models, ok = go.hypotheses(kind, seed, h, pts, norm)
+        if ok.any():
+            sc, cnt = lpo.score(go.errors(kind, models[ok], pts), thr2)
+            i = int(np.argmin(sc))  # first minimum: the lowest hypothesis
+            if best is None or sc[i] < best[0]:
+                best = (int(sc[i]), int(cnt[i]), int(h[ok][i]), models[ok][i])
+                Ml, sl, cl = rescore(norm, refine_model(norm, start(norm, best[3]), pts, float(thr2), lpo.STEPS), pts,
+                                     thr2)
+                if sl < best[0]:
+                    best = (sl, cl, best[2], Ml)
+                    nlo += 1
+        drawn = min((c + 1) * go.CHUNK, max_iters)
+        ep = 1.0 - (best[1] if best else 0) / n
+        if drawn >= max_iters or drawn >= go.update_num_iters(confidence, ep, s, max_iters):
+            break
+    if best is None:
+        return dict(fail, num_hypotheses=drawn)
+    model, cost, count = rescore(norm, refine_model(norm, start(norm, best[3]), pts, float(thr2), lpo.FINAL_STEPS),
+                                 pts, thr2)
+    if cost > best[0]:
+        cost, count, model = best[0], best[1], best[3]
+    inliers = np.zeros(M, dtype=bool)
+    inliers[idx[go.errors(kind, model[None], pts)[0] < thr2]] = True
+    return {key: model.reshape(3, 3), "inliers": inliers, "num_inliers": count, "success": True,
+            "best_hypothesis": best[2], "num_hypotheses": drawn, "num_local_optimizations": nlo, "cost": cost}

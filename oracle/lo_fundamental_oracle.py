@@ -1,11 +1,11 @@
 """numpy restatement of the LO-RANSAC fundamental matrix of include/geometry_b200.h (geo_fundamental_lo, steps LF1-LF8,
-csrc/lo_fundamental_api.cu), and the accuracy metric its tests and tools/geometry_bench.py share.
+csrc/lo_hf_api.cu), and the accuracy metric its tests and tools/geometry_bench.py share.
 
 The compaction, Hartley normalisation, samples, eight-point hypotheses, fp32 epipolar errors, denormalisation and
-fixed-order sums are geometry_oracle's; the MSAC score is lo_pose_oracle's and the Cholesky step lo_homography_oracle's.
-What is new here is the Levenberg-Marquardt refinement of a rank-2 F in the orthonormal representation
-(U, V, sigma) on the truncated Sampson cost in pixels (double, elementwise operations only, so the CUDA build compiled
-with -fmad=false agrees bit for bit).
+fixed-order sums are geometry_oracle's; the MSAC score is lo_pose_oracle's; the Cholesky step, quaternion, LM loop and
+chunk driver are lo_common's.  What is new here is the Levenberg-Marquardt refinement of a rank-2 F in the
+orthonormal representation (U, V, sigma) on the truncated Sampson cost in pixels (double, elementwise operations only,
+so the CUDA build compiled with -fmad=false agrees bit for bit).
 """
 from __future__ import annotations
 
@@ -15,7 +15,7 @@ import numpy as np
 
 from oracle import geometry_oracle as go
 from oracle import geometry_synth as gs
-from oracle import lo_homography_oracle as lh
+from oracle import lo_common as lc
 from oracle import lo_pose_oracle as lpo
 
 S = 8                # points per sample
@@ -106,19 +106,9 @@ def directions(U, V, sig):
     return out
 
 
-def _quat(d):
-    """A7's rotation of the unit quaternion (1, d0/2, d1/2, d2/2) / norm, row-major."""
-    qw, qx, qy, qz = 1.0, d[0] * 0.5, d[1] * 0.5, d[2] * 0.5
-    n = math.sqrt(qw * qw + qx * qx + qy * qy + qz * qz)
-    qw, qx, qy, qz = qw / n, qx / n, qy / n, qz / n
-    return [1.0 - 2.0 * (qy * qy + qz * qz), 2.0 * (qx * qy - qw * qz), 2.0 * (qx * qz + qw * qy),
-            2.0 * (qx * qy + qw * qz), 1.0 - 2.0 * (qx * qx + qz * qz), 2.0 * (qy * qz - qw * qx),
-            2.0 * (qx * qz - qw * qy), 2.0 * (qy * qz + qw * qx), 1.0 - 2.0 * (qx * qx + qy * qy)]
-
-
 def update(U, V, sig, d):
     """U' = Q(d0..2) U, V' = Q(d3..5) V, sig' = sig + d6."""
-    return go._mm3(_quat(d[0:3]), list(U)), go._mm3(_quat(d[3:6]), list(V)), sig + d[6]
+    return go._mm3(lc.quat_rotation(d[0:3]), list(U)), go._mm3(lc.quat_rotation(d[3:6]), list(V)), sig + d[6]
 
 
 def _epipolar(f, x, y, u, v):
@@ -164,22 +154,8 @@ def terms(norm, U, V, sig, pts: np.ndarray, thr2: float) -> np.ndarray:
 def refine(norm, model, pts: np.ndarray, thr2: float, steps: int):
     """steps Levenberg-Marquardt steps on the truncated Sampson cost from model = (U, V, sig), inliers re-selected at
     every model."""
-    U, V, sig = [float(v) for v in model[0]], [float(v) for v in model[1]], float(model[2])
-    sums = terms(norm, U, V, sig, pts, thr2)
-    lam = LAMBDA0
-    for _ in range(steps):
-        d = lh.lm_solve(sums[:28], sums[28:35], lam, DOF)
-        if d is None:
-            lam = lam * 10.0
-            continue
-        cand = update(U, V, sig, d)
-        cs = terms(norm, *cand, pts, thr2)
-        if cs[35] < sums[35]:
-            (U, V, sig), sums = cand, cs
-            lam = lam / 10.0
-        else:
-            lam = lam * 10.0
-    return U, V, sig
+    x = [float(v) for v in model[0]], [float(v) for v in model[1]], float(model[2])
+    return lc.refine(lambda m: terms(norm, *m, pts, thr2), lambda m, d: update(*m, d), x, DOF, steps)
 
 
 def rescore(norm, model, pts: np.ndarray, thr2: np.float32):
@@ -190,52 +166,14 @@ def rescore(norm, model, pts: np.ndarray, thr2: np.float32):
     return F, int(sc), int(cnt)
 
 
-def _fail(M: int, drawn: int) -> dict:
-    return {"F": np.zeros((3, 3)), "inliers": np.zeros(M, dtype=bool), "num_inliers": 0, "success": False,
-            "best_hypothesis": -1, "num_hypotheses": drawn, "num_local_optimizations": 0, "cost": 0}
+def start(norm, F):
+    """(U, V, sig) of a pixel F."""
+    return factorise(normalised_model(norm, F))
 
 
 def lo_fundamental_pair(kpts0, kpts1, m0, threshold=3.0, max_iters=1000, confidence=0.99, seed=0) -> dict:
-    kpts0 = np.asarray(kpts0, dtype=np.float32)
-    kpts1 = np.asarray(kpts1, dtype=np.float32)
-    m0 = np.asarray(m0, dtype=np.int64)
-    M = m0.shape[0]
-    thr2 = np.float32(threshold * threshold)
-    idx, pts = go.compact(kpts0, kpts1, m0)
-    n = pts.shape[0]
-    if n < S:
-        return _fail(M, 0)
-    norm = go.normalisation(pts)
-    if norm is None:
-        return _fail(M, 0)
-    best, nlo, drawn = None, 0, 0  # best: (score, count, h, F)
-    for c in range(-(-max_iters // go.CHUNK)):
-        h = np.arange(c * go.CHUNK, min((c + 1) * go.CHUNK, max_iters), dtype=np.int64)
-        models, ok = go.hypotheses(go.FUNDAMENTAL, seed, h, pts, norm)
-        if ok.any():
-            sc, cnt = lpo.score(go.errors(go.FUNDAMENTAL, models[ok], pts), thr2)
-            i = int(np.argmin(sc))  # first minimum: the lowest hypothesis
-            if best is None or sc[i] < best[0]:
-                best = (int(sc[i]), int(cnt[i]), int(h[ok][i]), models[ok][i])
-                start = factorise(normalised_model(norm, best[3]))
-                Fl, sl, cl = rescore(norm, refine(norm, start, pts, float(thr2), STEPS), pts, thr2)
-                if sl < best[0]:
-                    best = (sl, cl, best[2], Fl)
-                    nlo += 1
-        drawn = min((c + 1) * go.CHUNK, max_iters)
-        ep = 1.0 - (best[1] if best else 0) / n
-        if drawn >= max_iters or drawn >= go.update_num_iters(confidence, ep, S, max_iters):
-            break
-    if best is None:
-        return _fail(M, drawn)
-    start = factorise(normalised_model(norm, best[3]))
-    F, cost, count = rescore(norm, refine(norm, start, pts, float(thr2), FINAL_STEPS), pts, thr2)
-    if cost > best[0]:
-        cost, count, F = best[0], best[1], best[3]
-    inliers = np.zeros(M, dtype=bool)
-    inliers[idx[go.errors(go.FUNDAMENTAL, F[None], pts)[0] < thr2]] = True
-    return {"F": F.reshape(3, 3), "inliers": inliers, "num_inliers": count, "success": True, "best_hypothesis": best[2],
-            "num_hypotheses": drawn, "num_local_optimizations": nlo, "cost": cost}
+    return lc.lo_hf_pair(go.FUNDAMENTAL, S, "F", start, refine, rescore, kpts0, kpts1, m0, threshold, max_iters,
+                         confidence, seed)
 
 
 def lo_fundamental(kpts0, kpts1, matches0, threshold=3.0, max_iters=1000, confidence=0.99, seed=0) -> dict:

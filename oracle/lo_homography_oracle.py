@@ -1,10 +1,11 @@
 """numpy restatement of the LO-RANSAC homography of include/geometry_b200.h (geo_homography_lo, steps LH1-LH8,
-csrc/lo_homography_api.cu).
+csrc/lo_hf_api.cu).
 
 The compaction, Hartley normalisation, samples, four-point hypotheses, fp32 transfer errors, denormalisation and
-fixed-order sums are geometry_oracle's; the MSAC score is lo_pose_oracle's.  What is new here is the Levenberg-Marquardt
-refinement of the unit-norm normalised homography on the truncated transfer cost in pixels (double, elementwise
-operations only, so the CUDA build compiled with -fmad=false agrees bit for bit) and its tangent basis.
+fixed-order sums are geometry_oracle's; the MSAC score is lo_pose_oracle's; the Cholesky step, LM loop and chunk
+driver are lo_common's.  What is new here is the Levenberg-Marquardt refinement of the unit-norm normalised homography
+on the truncated transfer cost in pixels (double, elementwise operations only, so the CUDA build compiled with
+-fmad=false agrees bit for bit) and its tangent basis.
 """
 from __future__ import annotations
 
@@ -13,6 +14,7 @@ import math
 import numpy as np
 
 from oracle import geometry_oracle as go
+from oracle import lo_common as lc
 from oracle import lo_pose_oracle as lpo
 
 S = 4                # points per sample
@@ -108,63 +110,9 @@ def terms(norm, Hn, pts: np.ndarray, thr2: float) -> np.ndarray:
     return go.fixed_sum(np.stack(rows))
 
 
-def lm_solve(h, g, lam, n=DOF):
-    """lo_pose_oracle.lm_solve (header step A7) for an n x n system: delta of (H, its diagonal times (1 + lam)) delta
-    = -g by Cholesky; None on failure.  n = 5 is lo_pose_oracle's, operation for operation."""
-    A = [[0.0] * n for _ in range(n)]
-    e = 0
-    for i in range(n):
-        for j in range(i, n):
-            A[i][j] = A[j][i] = float(h[e])
-            e += 1
-    for i in range(n):
-        A[i][i] = A[i][i] * (1.0 + lam)
-    L = [[0.0] * n for _ in range(n)]
-    for j in range(n):
-        d = A[j][j]
-        for k in range(j):
-            d = d - L[j][k] * L[j][k]
-        if not d > 0.0:
-            return None
-        L[j][j] = math.sqrt(d)
-        for i in range(j + 1, n):
-            s = A[i][j]
-            for k in range(j):
-                s = s - L[i][k] * L[j][k]
-            L[i][j] = s / L[j][j]
-    yv = [0.0] * n
-    for i in range(n):
-        s = -float(g[i])
-        for k in range(i):
-            s = s - L[i][k] * yv[k]
-        yv[i] = s / L[i][i]
-    x = [0.0] * n
-    for i in range(n - 1, -1, -1):
-        s = yv[i]
-        for k in range(i + 1, n):
-            s = s - L[k][i] * x[k]
-        x[i] = s / L[i][i]
-    return x if all(math.isfinite(v) for v in x) else None
-
-
 def refine(norm, Hn, pts: np.ndarray, thr2: float, steps: int):
     """steps Levenberg-Marquardt steps on the truncated transfer cost from Hn, inliers re-selected at every model."""
-    Hn = [float(v) for v in Hn]
-    sums = terms(norm, Hn, pts, thr2)
-    lam = LAMBDA0
-    for _ in range(steps):
-        d = lm_solve(sums[:36], sums[36:44], lam)
-        if d is None:
-            lam = lam * 10.0
-            continue
-        cand = update(Hn, d)
-        cs = terms(norm, cand, pts, thr2)
-        if cs[44] < sums[44]:
-            Hn, sums = cand, cs
-            lam = lam / 10.0
-        else:
-            lam = lam * 10.0
-    return Hn
+    return lc.refine(lambda x: terms(norm, x, pts, thr2), update, [float(v) for v in Hn], DOF, steps)
 
 
 def rescore(norm, Hn, pts: np.ndarray, thr2: np.float32):
@@ -175,52 +123,9 @@ def rescore(norm, Hn, pts: np.ndarray, thr2: np.float32):
     return H, int(sc), int(cnt)
 
 
-def _fail(M: int, drawn: int) -> dict:
-    return {"H": np.zeros((3, 3)), "inliers": np.zeros(M, dtype=bool), "num_inliers": 0, "success": False,
-            "best_hypothesis": -1, "num_hypotheses": drawn, "num_local_optimizations": 0, "cost": 0}
-
-
 def lo_homography_pair(kpts0, kpts1, m0, threshold=3.0, max_iters=2000, confidence=0.995, seed=0) -> dict:
-    kpts0 = np.asarray(kpts0, dtype=np.float32)
-    kpts1 = np.asarray(kpts1, dtype=np.float32)
-    m0 = np.asarray(m0, dtype=np.int64)
-    M = m0.shape[0]
-    thr2 = np.float32(threshold * threshold)
-    idx, pts = go.compact(kpts0, kpts1, m0)
-    n = pts.shape[0]
-    if n < S:
-        return _fail(M, 0)
-    norm = go.normalisation(pts)
-    if norm is None:
-        return _fail(M, 0)
-    best, nlo, drawn = None, 0, 0  # best: (score, count, h, H)
-    for c in range(-(-max_iters // go.CHUNK)):
-        h = np.arange(c * go.CHUNK, min((c + 1) * go.CHUNK, max_iters), dtype=np.int64)
-        models, ok = go.hypotheses(go.HOMOGRAPHY, seed, h, pts, norm)
-        if ok.any():
-            sc, cnt = lpo.score(go.errors(go.HOMOGRAPHY, models[ok], pts), thr2)
-            i = int(np.argmin(sc))  # first minimum: the lowest hypothesis
-            if best is None or sc[i] < best[0]:
-                best = (int(sc[i]), int(cnt[i]), int(h[ok][i]), models[ok][i])
-                Hl, sl, cl = rescore(norm, refine(norm, normalised_model(norm, best[3]), pts, float(thr2), STEPS), pts,
-                                     thr2)
-                if sl < best[0]:
-                    best = (sl, cl, best[2], Hl)
-                    nlo += 1
-        drawn = min((c + 1) * go.CHUNK, max_iters)
-        ep = 1.0 - (best[1] if best else 0) / n
-        if drawn >= max_iters or drawn >= go.update_num_iters(confidence, ep, S, max_iters):
-            break
-    if best is None:
-        return _fail(M, drawn)
-    H, cost, count = rescore(norm, refine(norm, normalised_model(norm, best[3]), pts, float(thr2), FINAL_STEPS), pts,
-                             thr2)
-    if cost > best[0]:
-        cost, count, H = best[0], best[1], best[3]
-    inliers = np.zeros(M, dtype=bool)
-    inliers[idx[go.errors(go.HOMOGRAPHY, H[None], pts)[0] < thr2]] = True
-    return {"H": H.reshape(3, 3), "inliers": inliers, "num_inliers": count, "success": True, "best_hypothesis": best[2],
-            "num_hypotheses": drawn, "num_local_optimizations": nlo, "cost": cost}
+    return lc.lo_hf_pair(go.HOMOGRAPHY, S, "H", normalised_model, refine, rescore, kpts0, kpts1, m0, threshold,
+                         max_iters, confidence, seed)
 
 
 def lo_homography(kpts0, kpts1, matches0, threshold=3.0, max_iters=2000, confidence=0.995, seed=0) -> dict:

@@ -2,9 +2,9 @@
 csrc/pose_api.cu).
 
 The sampling, the five-point solutions, the fp32 Sampson error and the cheirality test are pose_oracle's; the sums are
-geometry_oracle's fixed order.  What is new here is the integer MSAC score, the Levenberg-Marquardt refinement on the
-truncated Sampson cost (double, elementwise operations only, so the CUDA build compiled with -fmad=false agrees bit for
-bit) and the once-per-chunk local optimisation schedule.
+geometry_oracle's fixed order; the Cholesky step, quaternion and LM loop are lo_common's.  What is new here is the
+integer MSAC score, the 5-DOF pose update and terms on the truncated Sampson cost (double, elementwise operations only,
+so the CUDA build compiled with -fmad=false agrees bit for bit) and the once-per-chunk local optimisation schedule.
 """
 from __future__ import annotations
 
@@ -13,6 +13,7 @@ import math
 import numpy as np
 
 from oracle import geometry_oracle as go
+from oracle import lo_common as lc
 from oracle import pose_oracle as po
 
 QSCALE = 65536       # GEO_LO_QSCALE: a point's score at or past the threshold
@@ -113,52 +114,9 @@ def terms(R, t, pts: np.ndarray, thr2: float) -> np.ndarray:
     return go.fixed_sum(np.stack(rows))
 
 
-def lm_solve(h, g, lam):
-    """delta of (H, its diagonal times (1 + lam)) delta = -g by Cholesky (header step A7, 5x5); None on failure."""
-    A = [[0.0] * 5 for _ in range(5)]
-    e = 0
-    for i in range(5):
-        for j in range(i, 5):
-            A[i][j] = A[j][i] = float(h[e])
-            e += 1
-    for i in range(5):
-        A[i][i] = A[i][i] * (1.0 + lam)
-    L = [[0.0] * 5 for _ in range(5)]
-    for j in range(5):
-        d = A[j][j]
-        for k in range(j):
-            d = d - L[j][k] * L[j][k]
-        if not d > 0.0:
-            return None
-        L[j][j] = math.sqrt(d)
-        for i in range(j + 1, 5):
-            s = A[i][j]
-            for k in range(j):
-                s = s - L[i][k] * L[j][k]
-            L[i][j] = s / L[j][j]
-    yv = [0.0] * 5
-    for i in range(5):
-        s = -float(g[i])
-        for k in range(i):
-            s = s - L[i][k] * yv[k]
-        yv[i] = s / L[i][i]
-    x = [0.0] * 5
-    for i in range(4, -1, -1):
-        s = yv[i]
-        for k in range(i + 1, 5):
-            s = s - L[k][i] * x[k]
-        x[i] = s / L[i][i]
-    return x if all(math.isfinite(v) for v in x) else None
-
-
 def update(R, t, d):
     """R' = Q(d0..2) R with A7's quaternion, t' = normalize(t + d3 b1 + d4 b2)."""
-    qw, qx, qy, qz = 1.0, d[0] * 0.5, d[1] * 0.5, d[2] * 0.5
-    n = math.sqrt(qw * qw + qx * qx + qy * qy + qz * qz)
-    qw, qx, qy, qz = qw / n, qx / n, qy / n, qz / n
-    Q = [1.0 - 2.0 * (qy * qy + qz * qz), 2.0 * (qx * qy - qw * qz), 2.0 * (qx * qz + qw * qy),
-         2.0 * (qx * qy + qw * qz), 1.0 - 2.0 * (qx * qx + qz * qz), 2.0 * (qy * qz - qw * qx),
-         2.0 * (qx * qz - qw * qy), 2.0 * (qy * qz + qw * qx), 1.0 - 2.0 * (qx * qx + qy * qy)]
+    Q = lc.quat_rotation(d)
     Rn = [Q[3 * i] * R[j] + Q[3 * i + 1] * R[3 + j] + Q[3 * i + 2] * R[6 + j] for i in range(3) for j in range(3)]
     b1, b2 = tangent_basis(t)
     v = [(t[i] + d[3] * b1[i]) + d[4] * b2[i] for i in range(3)]
@@ -168,22 +126,8 @@ def update(R, t, d):
 
 def refine(R, t, pts: np.ndarray, thr2: float, steps: int):
     """steps Levenberg-Marquardt steps on the truncated Sampson cost from (R, t), inliers re-selected at every pose."""
-    R, t = [float(v) for v in R], [float(v) for v in t]
-    sums = terms(R, t, pts, thr2)
-    lam = LAMBDA0
-    for _ in range(steps):
-        d = lm_solve(sums[:15], sums[15:20], lam)
-        if d is None:
-            lam = lam * 10.0
-            continue
-        Rc, tc = update(R, t, d)
-        cs = terms(Rc, tc, pts, thr2)
-        if cs[20] < sums[20]:
-            R, t, sums = Rc, tc, cs
-            lam = lam / 10.0
-        else:
-            lam = lam * 10.0
-    return R, t
+    x = [float(v) for v in R], [float(v) for v in t]
+    return lc.refine(lambda m: terms(*m, pts, thr2), lambda m, d: update(*m, d), x, 5, steps)
 
 
 def model_errors(R, t, pts: np.ndarray) -> np.ndarray:

@@ -10,11 +10,10 @@ pair's points, its 6x6 solve on Python floats.
 """
 from __future__ import annotations
 
-import math
-
 import numpy as np
 
 from oracle import geometry_oracle as go
+from oracle import lo_common as lc
 from oracle import pose_oracle as po
 
 S = 3               # points per sample
@@ -237,52 +236,9 @@ def _terms(R, t, K, pix, wld, inl):
     return [float(x) for x in sums[:21]], [float(x) for x in sums[21:27]], float(sums[27])
 
 
-def _cholesky_step(Hu, g, lam):
-    """delta of (J^T J with its diagonal times (1 + lam)) delta = -J^T r by Cholesky, or None."""
-    A = [[0.0] * 6 for _ in range(6)]
-    e = 0
-    for i in range(6):
-        for j in range(i, 6):
-            A[i][j] = A[j][i] = Hu[e]
-            e += 1
-    for i in range(6):
-        A[i][i] = A[i][i] * (1.0 + lam)
-    L = [[0.0] * 6 for _ in range(6)]
-    for j in range(6):
-        d = A[j][j]
-        for k in range(j):
-            d = d - L[j][k] * L[j][k]
-        if not d > 0.0:
-            return None
-        L[j][j] = math.sqrt(d)
-        for i in range(j + 1, 6):
-            e = A[i][j]
-            for k in range(j):
-                e = e - L[i][k] * L[j][k]
-            L[i][j] = e / L[j][j]
-    yv = [0.0] * 6
-    for i in range(6):
-        e = -g[i]
-        for k in range(i):
-            e = e - L[i][k] * yv[k]
-        yv[i] = e / L[i][i]
-    x = [0.0] * 6
-    for i in range(5, -1, -1):
-        e = yv[i]
-        for k in range(i + 1, 6):
-            e = e - L[k][i] * x[k]
-        x[i] = e / L[i][i]
-    return x if all(math.isfinite(c) for c in x) else None
-
-
 def _update(R, t, d):
     """R' = Q R, t' = Q t + d[3:] with Q the rotation of the unit quaternion (1, d[:3] / 2) / norm."""
-    qw, qx, qy, qz = 1.0, d[0] * 0.5, d[1] * 0.5, d[2] * 0.5
-    n = math.sqrt(qw * qw + qx * qx + qy * qy + qz * qz)
-    qw, qx, qy, qz = qw / n, qx / n, qy / n, qz / n
-    Q = [1.0 - 2.0 * (qy * qy + qz * qz), 2.0 * (qx * qy - qw * qz), 2.0 * (qx * qz + qw * qy),
-         2.0 * (qx * qy + qw * qz), 1.0 - 2.0 * (qx * qx + qz * qz), 2.0 * (qy * qz - qw * qx),
-         2.0 * (qx * qz - qw * qy), 2.0 * (qy * qz + qw * qx), 1.0 - 2.0 * (qx * qx + qy * qy)]
+    Q = lc.quat_rotation(d)
     Rn = [Q[3 * i] * R[j] + Q[3 * i + 1] * R[3 + j] + Q[3 * i + 2] * R[6 + j] for i in range(3) for j in range(3)]
     tn = [Q[3 * i] * t[0] + Q[3 * i + 1] * t[1] + Q[3 * i + 2] * t[2] + d[3 + i] for i in range(3)]
     return Rn, tn
@@ -294,7 +250,7 @@ def refine_lm(R, t, K, pix, wld, inl):
     Hu, g, cost = _terms(R, t, K, pix, wld, inl)
     lam = LM_LAMBDA0
     for _ in range(LM_STEPS):
-        d = _cholesky_step(Hu, g, lam)
+        d = lc.lm_solve(Hu, g, lam, 6)
         if d is None:
             lam = lam * 10.0
             continue

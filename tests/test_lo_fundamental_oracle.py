@@ -6,6 +6,7 @@ import pytest
 
 from oracle import geometry_oracle as go
 from oracle import geometry_synth as gs
+from oracle import lo_common as lc
 from oracle import lo_fundamental_oracle as lf
 
 
@@ -29,7 +30,7 @@ def _unit(F):
 def _rotation(rng):
     q = rng.normal(size=4)
     q = q / np.linalg.norm(q)
-    return np.array(lf._quat((q[1:] / q[0] * 2.0).tolist())).reshape(3, 3)
+    return np.array(lc.quat_rotation((q[1:] / q[0] * 2.0).tolist())).reshape(3, 3)
 
 
 def test_factorise_then_compose_returns_the_model():

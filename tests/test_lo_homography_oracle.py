@@ -35,15 +35,6 @@ def test_basis_is_an_orthonormal_tangent_basis():
         assert np.abs(B @ np.array(Hn)).max() <= 1e-14
 
 
-def test_lm_solve_is_lo_pose_oracles_at_five():
-    rng = np.random.default_rng(1)
-    for _ in range(20):
-        J = rng.normal(size=(30, 5))
-        h = [(J.T @ J)[i, j] for i in range(5) for j in range(i, 5)]
-        g = rng.normal(size=5)
-        assert lh.lm_solve(h, g, 1e-3, 5) == lpo.lm_solve(h, g, 1e-3)
-
-
 @pytest.mark.parametrize("seed", [0, 1, 2, 3])
 def test_transfer_jacobian_equals_central_differences(seed):
     rng = np.random.default_rng(seed)
