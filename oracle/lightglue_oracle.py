@@ -160,6 +160,29 @@ def filter_matches(scores: torch.Tensor, th: float):
     return torch.where(valid0, m0, -1), torch.where(valid1, m1, -1), ms0, ms1
 
 
+def encodings(w: Dict[str, torch.Tensor], data: dict, add_scale_ori: bool = False):
+    """lightglue/lightglue.py:491-501, 523-524: the rotary encodings ``(c0, s0, c1, s1)`` of both images' normalised
+    keypoints (with scale and orientation appended when ``add_scale_ori``), in the dtype and on the device of
+    ``w["posenc.Wr.weight"]``."""
+    wr = w["posenc.Wr.weight"]
+    enc = []
+    for d in (data["image0"], data["image1"]):
+        k = normalize_keypoints(d["keypoints"].to(wr), d.get("image_size"))
+        if add_scale_ori:  # 495-501
+            k = torch.cat([k, d["scales"].to(wr).unsqueeze(-1), d["oris"].to(wr).unsqueeze(-1)], -1)
+        enc += fourier_encoding(k, wr)
+    return tuple(enc)
+
+
+def layer(w: Dict[str, torch.Tensor], i: int, x0: torch.Tensor, x1: torch.Tensor, enc):
+    """lightglue/lightglue.py:541-543 (``TransformerLayer``, 233-253): transformer layer ``i`` (self blocks, then the cross block) on the residual
+    streams ``x0``, ``x1`` with the encodings ``enc = encodings(...)`` of those rows; returns the new ``(x0, x1)``."""
+    c0, s0, c1, s1 = enc
+    x0 = self_block(w, i, x0, c0, s0)
+    x1 = self_block(w, i, x1, c1, s1)
+    return cross_block(w, i, x0, x1)
+
+
 def forward(
     w: Dict[str, torch.Tensor],
     data: dict,
@@ -188,15 +211,8 @@ def forward(
     """
     w = {k: v.to(dtype) for k, v in w.items()}
     d0, d1 = data["image0"], data["image1"]
-    k0 = d0["keypoints"].to(dtype)
-    k1 = d1["keypoints"].to(dtype)
-    b, m, _ = k0.shape
-    n = k1.shape[1]
-    k0 = normalize_keypoints(k0, d0.get("image_size"))
-    k1 = normalize_keypoints(k1, d1.get("image_size"))
-    if add_scale_ori:  # 495-501
-        k0 = torch.cat([k0, d0["scales"].to(dtype).unsqueeze(-1), d0["oris"].to(dtype).unsqueeze(-1)], -1)
-        k1 = torch.cat([k1, d1["scales"].to(dtype).unsqueeze(-1), d1["oris"].to(dtype).unsqueeze(-1)], -1)
+    b, m, _ = d0["keypoints"].shape
+    n = d1["keypoints"].shape[1]
     x0 = d0["descriptors"].to(dtype)
     x1 = d1["descriptors"].to(dtype)
     if "input_proj.weight" in w:  # 388-391, 521-522
@@ -204,8 +220,7 @@ def forward(
         x1 = F.linear(x1, w["input_proj.weight"], w["input_proj.bias"])
     else:
         assert x0.shape[-1] == DIM and x1.shape[-1] == DIM
-    c0, s0 = fourier_encoding(k0, w["posenc.Wr.weight"])
-    c1, s1 = fourier_encoding(k1, w["posenc.Wr.weight"])
+    c0, s0, c1, s1 = encodings(w, data, add_scale_ori)
 
     early = depth_confidence > 0
     prune = width_confidence > 0
@@ -224,9 +239,7 @@ def forward(
         last = i
         if x0.shape[1] == 0 or x1.shape[1] == 0:  # 539-540
             break
-        x0 = self_block(w, i, x0, c0, s0)
-        x1 = self_block(w, i, x1, c1, s1)
-        x0, x1 = cross_block(w, i, x0, x1)
+        x0, x1 = layer(w, i, x0, x1, (c0, s0, c1, s1))
         if return_layers:
             layers.append((x0.clone(), x1.clone()))
         if i == n_layers - 1:  # 544-545
