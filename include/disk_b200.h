@@ -60,6 +60,23 @@ LG_API int disk_forward(DiskHandle* h, const float* image, int32_t C, int32_t B,
 LG_API int disk_heads(DiskHandle* h, const float* image, int32_t C, int32_t B, int32_t H, int32_t W, const int32_t* pos,
                       int32_t P, float* heatmap, float* descriptors, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Host-only introspection (no device work): the workspace plan of disk_forward / disk_heads for this handle and a
+ * [B, C, H, W] batch.  Writes, when non-null, the byte offset from the workspace's start and the size of each of its
+ * DISK_LAYOUT_BUFFERS buffers, in this order:
+ *   0 .. 7  raw outputs of down0 .. down4, up0 .. up2: fp32 padded NHWC (2-pixel zero border, row b (h+4)(w+4) +
+ *           (y+2)(w+4) + (x+2) at the layer's level h x w of the 16-padded image), cout channels (16, 32, 64,
+ *           64, 64, 64, 64, 64), bias included; their padding rows hold garbage;
+ *   8       x3, up3's input (normalised, PReLU'd), fp32 padded NHWC, 80 channels, padding zero;
+ *   9, 10   the descriptor GEMM's im2col rows, bf16 hi / lo [rows, 2048] (column tap 80 + ci, zero past 2000), row
+ *           b P + j for disk_heads' P (b max_keypoints + j for disk_forward);
+ *   11      the descriptor GEMM's output, fp32 [rows, 128] (bias included);
+ *   12      the row-plan state: 6 x 4 int32 words (len[2], stop_layer, unused) of levels 0 .. 4 and of the descriptor
+ *           GEMM.
+ * After a call the buffers hold that call's values.  Returns the workspace size (disk_workspace_bytes), 0 for a null
+ * handle or a non-positive size. */
+#define DISK_LAYOUT_BUFFERS 13
+LG_API int64_t disk_workspace_layout(const DiskHandle* h, int32_t B, int32_t H, int32_t W, int64_t* offsets, int64_t* bytes);
+
 #ifdef __cplusplus
 }
 #endif

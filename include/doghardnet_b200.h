@@ -68,6 +68,24 @@ LG_API int dhn_describe(DhnHandle* h, const float* image, int32_t channels, cons
                         int32_t W, int64_t cap, const float* keypoints, const float* scales, const float* oris,
                         const int32_t* counts, float* descriptors, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Host-only introspection (no device work): the workspace plan of dhn_forward / dhn_describe for this handle and an
+ * H x W image.  Patches run in chunks of 256; each level of a chunk is a padded NHWC map of 256 patches (34 x 34,
+ * 18 x 18 or 10 x 10 rows per patch, a 1-pixel zero border), stored as the rows of tc_rows(256 * rows per patch).
+ * Writes, when non-null, the byte offset from the workspace's start and the size of each of its DHN_LAYOUT_BUFFERS
+ * buffers, in this order (bf16 hi / lo pairs; after a call they hold the last chunk of the last image):
+ *   0, 1    conv 0's output (34 x 34, 64 channels, 32 live), then the four polyphase images of conv 1's output: phase
+ *           2 py + px from row (2 py + px) R, R = the rows of the 18 x 18 level, holds padded pixel
+ *           (2 (i - 1) + py, 2 (j - 1) + px) at frame position (i, j) of an 18 x 18 frame per patch, i, j >= 1;
+ *   2, 3    conv 1's output (34 x 34, 64 channels), then the polyphase images of conv 3's output (10 x 10 frames);
+ *   4, 5    conv 2's output; 6, 7 conv 3's output (18 x 18, 64 channels);
+ *   8, 9    conv 4's output; 10, 11 conv 5's output (10 x 10, 128 channels);
+ *   12, 13  conv 6's input rows [rows, 8192] (column (ky 8 + kx) 128 + ci), row k for keypoint k of the image;
+ *   14      conv 6's output, fp32 [rows, 128] (folded BatchNorm included, before F.normalize);
+ *   15      the row-plan state: int32 words (len[2], stop_layer, unused) per chunk and level, then conv 6's.
+ * Returns the workspace size (dhn_workspace_bytes), 0 for a null handle or a non-positive size. */
+#define DHN_LAYOUT_BUFFERS 16
+LG_API int64_t dhn_workspace_layout(const DhnHandle* h, int32_t H, int32_t W, int64_t* offsets, int64_t* bytes);
+
 #ifdef __cplusplus
 }
 #endif

@@ -17,7 +17,9 @@ SP_TC_BUFFERS = 9  # buffers of the tensor-core backbone's workspace plan (sp_tc
 AL_ABI_VERSION = 1
 SIFT_ABI_VERSION = 1
 DISK_ABI_VERSION = 1
+DISK_LAYOUT_BUFFERS = 13  # buffers of disk_workspace_layout
 DHN_ABI_VERSION = 1
+DHN_LAYOUT_BUFFERS = 16  # buffers of dhn_workspace_layout
 GEO_ABI_VERSION = 1  # include/geometry_b200.h
 GEO_HOMOGRAPHY, GEO_FUNDAMENTAL, GEO_ESSENTIAL = 0, 1, 2
 GEO_LO_QSCALE, GEO_LO_MAX_MATCHES = 65536, (1 << 20) - 1
@@ -242,6 +244,7 @@ DISK_PROTOTYPES = {  # include/disk_b200.h
     "disk_workspace_bytes": (_SZ, [_VP, _I32, _I32, _I32]),
     "disk_forward": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _I32, _I64] + [_VP] * 5 + [_SZ, _VP]),
     "disk_heads": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _I32, _VP, _I32, _VP, _VP, _VP, _SZ, _VP]),
+    "disk_workspace_layout": (_I64, [_VP, _I32, _I32, _I32, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
 }
 DHN_PROTOTYPES = {  # include/doghardnet_b200.h
     "dhn_weight_blob_floats": (_SZ, []),
@@ -251,6 +254,7 @@ DHN_PROTOTYPES = {  # include/doghardnet_b200.h
     "dhn_workspace_bytes": (_SZ, [_VP, _I32, _I32, _I32]),
     "dhn_forward": (C.c_int, [_VP, _VP, _I32, _VP, _I32, _I32, _I32, _I64] + [_VP] * 7 + [_SZ, _VP]),
     "dhn_describe": (C.c_int, [_VP, _VP, _I32, _VP, _I32, _I32, _I32, _I64] + [_VP] * 6 + [_SZ, _VP]),
+    "dhn_workspace_layout": (_I64, [_VP, _I32, _I32, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
 }
 GEO_PROTOTYPES = {  # include/geometry_b200.h
     "geo_workspace_bytes": (_SZ, [_I32, _I32, _I32]),

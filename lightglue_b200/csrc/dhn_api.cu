@@ -105,6 +105,7 @@ struct DhnWs {
   __nv_bfloat16 *c2h, *c2l;
   __nv_bfloat16 *gh, *gl;    // [D rows, 8192] conv 6 input rows
   float* dout;               // [D rows, 128]
+  size_t bytes[DHN_LAYOUT_BUFFERS];  // sizes of the buffers dhn_workspace_layout reports, in its order
 };
 
 size_t carve(char* base, const Geo& g, size_t sift_bytes, int H, int W, DhnWs* w) {
@@ -113,16 +114,18 @@ size_t carve(char* base, const Geo& g, size_t sift_bytes, int H, int W, DhnWs* w
   w->sift = b.take<char>(sift_bytes, A);
   w->pyr = b.take<float>((size_t)pyr_floats(H, W), A);
   w->state = b.take<int>((size_t)(g.nchunk * 3 + 1) * 4, A);
+  w->bytes[15] = b.last;
   const size_t u = (size_t)std::max(g.A.rows, 4 * g.B.rows) * 64, v = (size_t)std::max(g.A.rows, 4 * g.C.rows) * 64;
-  w->uh = b.take<__nv_bfloat16>(u, A); w->ul = b.take<__nv_bfloat16>(u, A);
-  w->vh = b.take<__nv_bfloat16>(v, A); w->vl = b.take<__nv_bfloat16>(v, A);
   const size_t bb = (size_t)g.B.rows * 64, cc = (size_t)g.C.rows * 128;
-  w->bh = b.take<__nv_bfloat16>(bb, A); w->bl = b.take<__nv_bfloat16>(bb, A);
-  w->b2h = b.take<__nv_bfloat16>(bb, A); w->b2l = b.take<__nv_bfloat16>(bb, A);
-  w->ch = b.take<__nv_bfloat16>(cc, A); w->cl = b.take<__nv_bfloat16>(cc, A);
-  w->c2h = b.take<__nv_bfloat16>(cc, A); w->c2l = b.take<__nv_bfloat16>(cc, A);
-  w->gh = b.take<__nv_bfloat16>((size_t)g.D.rows * K6, A); w->gl = b.take<__nv_bfloat16>((size_t)g.D.rows * K6, A);
-  w->dout = b.take<float>((size_t)g.D.rows * DESC, A);
+  __nv_bfloat16** maps[12] = {&w->uh, &w->ul, &w->vh, &w->vl, &w->bh, &w->bl, &w->b2h, &w->b2l, &w->ch, &w->cl, &w->c2h, &w->c2l};
+  const size_t n[12] = {u, u, v, v, bb, bb, bb, bb, cc, cc, cc, cc};
+  for (int i = 0; i < 12; ++i) {
+    *maps[i] = b.take<__nv_bfloat16>(n[i], A);
+    w->bytes[i] = b.last;
+  }
+  w->gh = b.take<__nv_bfloat16>((size_t)g.D.rows * K6, A); w->bytes[12] = b.last;
+  w->gl = b.take<__nv_bfloat16>((size_t)g.D.rows * K6, A); w->bytes[13] = b.last;
+  w->dout = b.take<float>((size_t)g.D.rows * DESC, A); w->bytes[14] = b.last;
   return b.bytes();
 }
 
@@ -481,6 +484,20 @@ extern "C" int64_t dhn_max_keypoints(const DhnHandle* h, int32_t, int32_t) { ret
 extern "C" size_t dhn_workspace_bytes(const DhnHandle* h, int32_t B, int32_t H, int32_t W) {
   if (!h || B <= 0 || H <= 0 || W <= 0) return 0;
   return ws_bytes(h, H, W);
+}
+
+extern "C" int64_t dhn_workspace_layout(const DhnHandle* h, int32_t H, int32_t W, int64_t* offsets, int64_t* bytes) {
+  if (!h || H <= 0 || W <= 0) return 0;
+  DhnWs w;
+  char* const base = reinterpret_cast<char*>(kLayoutBase);
+  const size_t total = carve(base, geometry(h->cfg.max_num_keypoints), sift_detect_workspace_bytes(h->sift, H, W), H, W, &w);
+  const void* p[DHN_LAYOUT_BUFFERS] = {w.uh, w.ul, w.vh,  w.vl,  w.bh, w.bl, w.b2h, w.b2l,
+                                       w.ch, w.cl, w.c2h, w.c2l, w.gh, w.gl, w.dout, w.state};
+  for (int i = 0; i < DHN_LAYOUT_BUFFERS; ++i) {
+    if (offsets) offsets[i] = (int64_t)((const char*)p[i] - base);
+    if (bytes) bytes[i] = (int64_t)w.bytes[i];
+  }
+  return (int64_t)total;
 }
 
 extern "C" int dhn_forward(DhnHandle* h, const float* image, int32_t channels, const int32_t* image_size, int32_t B, int32_t H,

@@ -86,6 +86,7 @@ struct DiskWs {
   float* sel_score;
   __nv_bfloat16 *dh, *dl;  // im2col rows of the descriptor head
   float* dout;             // [rows, 128]
+  size_t bytes[DISK_LAYOUT_BUFFERS];  // sizes of the buffers disk_workspace_layout reports, in its order
 };
 
 size_t carve(char* base, const Geo& g, DiskWs* w) {
@@ -93,6 +94,7 @@ size_t carve(char* base, const Geo& g, DiskWs* w) {
   constexpr size_t A = 1024;
   const int B = g.B;
   w->state = b.take<int>(24, A);
+  w->bytes[12] = b.last;
   const long nchunk0 = ((long)g.Hp * g.Wp + STAT_CHUNK - 1) / STAT_CHUNK;
   w->part = b.take<float>((size_t)B * nchunk0 * MAXC * 3, A);
   w->mean = b.take<float>((size_t)B * MAXC, A);
@@ -100,11 +102,13 @@ size_t carve(char* base, const Geo& g, DiskWs* w) {
   size_t amax = 0;
   for (int l = 0; l < NL - 1; ++l) {
     w->raw[l] = b.take<float>((size_t)g.lv[DL[l].level].rows * DL[l].cout, A);
+    w->bytes[l] = b.last;
     if (l > 0) amax = std::max(amax, (size_t)g.lv[DL[l].level].rows * cpad(DL[l].cin));
   }
   w->ah = b.take<__nv_bfloat16>(amax, A);
   w->al = b.take<__nv_bfloat16>(amax, A);
   w->x3 = b.take<float>((size_t)g.lv[0].rows * X3C, A);
+  w->bytes[8] = b.last;
   const size_t hw = (size_t)B * g.H * g.W;
   w->heat = b.take<float>(hw, A);
   w->kept = b.take<float>(hw, A);
@@ -117,8 +121,11 @@ size_t carve(char* base, const Geo& g, DiskWs* w) {
   w->sel_score = b.take<float>((size_t)B * g.ocap, A);
   w->n_sel = b.take<int>(B, A);
   w->dh = b.take<__nv_bfloat16>((size_t)g.ld.rows * DKP, A);
+  w->bytes[9] = b.last;
   w->dl = b.take<__nv_bfloat16>((size_t)g.ld.rows * DKP, A);
+  w->bytes[10] = b.last;
   w->dout = b.take<float>((size_t)g.ld.rows * DESC, A);
+  w->bytes[11] = b.last;
   return b.bytes();
 }
 
@@ -399,9 +406,11 @@ Prep layer_input(const Geo& g, const DiskWs& w, int l) {
   return p;
 }
 
-// the U-Net up to the heatmap: writes w.x3 (up3 input) and heat [B, H, W]
-int run_unet(DiskHandle* h, const float* image, int Cimg, const Geo& g, const DiskWs& w, float* heat, cudaStream_t s) {
-  const TcRows plans[6] = {g.lv[0], g.lv[1], g.lv[2], g.lv[3], g.lv[4], g.ld};
+// the U-Net up to the heatmap: writes w.x3 (up3 input) and heat [B, H, W]; the state words of the levels and of `ld`,
+// the row plan the descriptor GEMM will run on
+int run_unet(DiskHandle* h, const float* image, int Cimg, const Geo& g, const TcRows& ld, const DiskWs& w, float* heat,
+             cudaStream_t s) {
+  const TcRows plans[6] = {g.lv[0], g.lv[1], g.lv[2], g.lv[3], g.lv[4], ld};
   LG_RC(tc_rows_words(plans, 6, w.state, s));
   {  // down0
     Prep p{};
@@ -435,7 +444,8 @@ int run_unet(DiskHandle* h, const float* image, int Cimg, const Geo& g, const Di
   return 0;
 }
 
-// descriptor head at the pixels sel_pos (n_sel per image, oc selection slots per image) -> desc [B, out_stride, 128]
+// descriptor head at the pixels sel_pos (n_sel per image, oc selection slots per image) -> desc [B, out_stride, 128];
+// its state words (w.state + 20) must be those of tc_rows(B oc), written by run_unet
 int run_desc(DiskHandle* h, const Geo& g, const DiskWs& w, const int* n_sel, const int* sel_pos, const float* sel_score, long oc,
              long out_stride, int normalize, float* kpts, float* scores, float* desc, cudaStream_t s) {
   if (oc <= 0 || out_stride <= 0) return 0;
@@ -516,6 +526,21 @@ extern "C" size_t disk_workspace_bytes(const DiskHandle* h, int32_t B, int32_t H
   return carve(nullptr, geometry(h->cfg, B, H, W), &w);
 }
 
+extern "C" int64_t disk_workspace_layout(const DiskHandle* h, int32_t B, int32_t H, int32_t W, int64_t* offsets,
+                                         int64_t* bytes) {
+  if (!h || B <= 0 || H <= 0 || W <= 0) return 0;
+  DiskWs w;
+  char* const base = reinterpret_cast<char*>(kLayoutBase);
+  const size_t total = carve(base, geometry(h->cfg, B, H, W), &w);
+  const void* p[DISK_LAYOUT_BUFFERS] = {w.raw[0], w.raw[1], w.raw[2], w.raw[3], w.raw[4], w.raw[5], w.raw[6],
+                                        w.raw[7], w.x3,     w.dh,     w.dl,     w.dout,   w.state};
+  for (int i = 0; i < DISK_LAYOUT_BUFFERS; ++i) {
+    if (offsets) offsets[i] = (int64_t)((const char*)p[i] - base);
+    if (bytes) bytes[i] = (int64_t)w.bytes[i];
+  }
+  return (int64_t)total;
+}
+
 extern "C" int disk_forward(DiskHandle* h, const float* image, int32_t C, int32_t B, int32_t H, int32_t W, int64_t cap,
                             float* keypoints, float* scores, float* descriptors, int32_t* counts, void* workspace,
                             size_t workspace_bytes, void* stream_) {
@@ -527,7 +552,7 @@ extern "C" int disk_forward(DiskHandle* h, const float* image, int32_t C, int32_
   if (!workspace || workspace_bytes < carve(nullptr, g, &w)) return lg_set_error("disk_forward: workspace too small");
   carve((char*)workspace, g, &w);
   cudaStream_t s = (cudaStream_t)stream_;
-  LG_RC(run_unet(h, image, C, g, w, w.heat, s));
+  LG_RC(run_unet(h, image, C, g, g.ld, w, w.heat, s));
   const long n = (long)B * H * W;
   const int r = h->cfg.nms_window_size / 2;
   disk_nms_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(w.heat, w.kept, B, H, W, r);
@@ -552,7 +577,7 @@ extern "C" int disk_heads(DiskHandle* h, const float* image, int32_t C, int32_t 
   if (!workspace || workspace_bytes < carve(nullptr, g, &w)) return lg_set_error("disk_heads: workspace too small");
   carve((char*)workspace, g, &w);
   cudaStream_t s = (cudaStream_t)stream_;
-  LG_RC(run_unet(h, image, C, g, w, heatmap, s));
+  LG_RC(run_unet(h, image, C, g, tc_rows((long)B * P), w, heatmap, s));
   disk_fill_kernel<<<1, 1024, 0, s>>>(w.n_sel, B, P);
   LG_CHECK_LAUNCH();
   return run_desc(h, g, w, w.n_sel, pos, nullptr, P, P, 0, nullptr, nullptr, descriptors, s);

@@ -123,6 +123,36 @@ def hardnet(sd: dict, patches: torch.Tensor) -> torch.Tensor:
     return F.normalize(x.reshape(x.shape[0], -1), dim=1)
 
 
+def folded(sd: dict, li: int, like: torch.Tensor):
+    """Convolution li's weight and bias with its eval BatchNorm folded in, in double as dhn_create folds them:
+    w rs and -running_mean rs, rs = 1 / sqrt(running_var + 1e-5); returned in the dtype and on the device of `like`."""
+    i = CONVS[li]
+    rs = 1.0 / torch.sqrt(sd[f"features.{i + 1}.running_var"].double() + 1e-5)
+    w = sd[f"features.{i}.weight"].double() * rs.view(-1, 1, 1, 1)
+    b = -sd[f"features.{i + 1}.running_mean"].double() * rs
+    return w.to(like), b.to(like)
+
+
+def hardnet_layers(sd: dict, patches: torch.Tensor) -> list:
+    """HardNet layer by layer on folded weights (`folded`): the post-ReLU outputs of convs 0 .. 5 [N, C, h, w] and conv
+    6's output before F.normalize [N, 128].  Each layer l >= 1 is ``hardnet_conv(sd, l, outputs[l - 1])``."""
+    sp, mp = torch.std_mean(patches, dim=(1, 2, 3), keepdim=True)
+    x = (patches - mp) / (sp + 1e-6)
+    out = []
+    for li in range(len(CONVS)):
+        x = hardnet_conv(sd, li, x)
+        out.append(x)
+    out[-1] = out[-1].reshape(out[-1].shape[0], -1)
+    return out
+
+
+def hardnet_conv(sd: dict, li: int, x: torch.Tensor) -> torch.Tensor:
+    """Convolution li (folded BatchNorm), with its ReLU for li < 6, on the previous layer's output x [N, C, h, w]."""
+    w, b = folded(sd, li, x)
+    y = F.conv2d(x, w, b, stride=STRIDES[li], padding=1 if w.shape[-1] == 3 else 0)
+    return F.relu(y) if li < len(CONVS) - 1 else y
+
+
 # ---------------------------------------------------------------------------------------------------------- the extractor
 def gray(image: torch.Tensor) -> torch.Tensor:
     """kornia's rgb_to_grayscale of [B, 3, H, W] (0.299 r + 0.587 g + 0.114 b); gray images pass through."""

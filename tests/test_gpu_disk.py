@@ -2,7 +2,9 @@
 
 * ``heads`` (``disk_heads``): the cropped heatmap and the raw 128-d descriptors at chosen pixels -- crop corners and
   edges, pixels next to the padded frame, random ones -- against the oracle in float64 on the GPU, held to 1e-4 of
-  max|ref| per head (split-bf16 tensor-core convolutions, fp32 statistics).
+  max|ref| per head (split-bf16 tensor-core convolutions, fp32 statistics): at least 3x the emulated rounding and at
+  most 1/3 of a lost split-bf16 pass (tests/test_conv_layer_emulation.py).  A lost bias in down0 .. up2 is removed by
+  the next instance norm and invisible here; tests/test_gpu_conv_layers.py checks each layer from its own input.
 * ``forward``: against the oracle in fp32 (cuDNN, TF32 off).  The same keypoints in the same row-major order, except
   keypoints whose float64 NMS / threshold / top-k margin is below 1e-4 max|heatmap| (at most 0.5 % of them); on common
   keypoints scores within 1e-4 max|heatmap| and descriptors within 1e-4.
@@ -14,6 +16,7 @@ import torch.nn.functional as F
 from lightglue_b200 import DISK, _cabi, synth
 from oracle import disk_oracle as do
 from oracle import disk_synth as ds
+from tests.test_conv_layer_emulation import E2E_DISK
 
 pytestmark = pytest.mark.gpu
 
@@ -66,7 +69,7 @@ def test_heads_vs_float64(b, h, w):
     eh, ed = rel(heat, ref_heat), rel(desc, ref_d)
     print(f"B={b} {h}x{w}: max rel error heatmap {eh:.2e} descriptors {ed:.2e} ({pos.shape[1]} pixels)")
     assert heat.shape == (b, h, w) and desc.shape == (b, pos.shape[1], 128)
-    assert eh <= 1e-4 and ed <= 1e-4, (eh, ed)
+    assert eh <= E2E_DISK and ed <= E2E_DISK, (eh, ed)
 
 
 def _margins(h64, xy, conf, cand_vals):
