@@ -3,8 +3,8 @@
 // Launches, all fixed by (B, M, max_iters):
 //   prepare  one 1024-thread CTA per pair: ordered compaction of the valid matches, Hartley normalisation
 //   per chunk of GEO_CHUNK hypotheses:
-//     hyp    one CTA per pair: folds the previous chunk's counts into the pair's best (packed (count + 1, ~h), atomic
-//            max), decides the adaptive stop, then one thread per hypothesis draws and solves its sample in double
+//     hyp    one CTA per pair: folds the previous chunk's counts into the pair's best (geo_fold), decides the
+//            adaptive stop, then one thread per hypothesis draws and solves its sample in double
 //     score  (B, splits) CTAs: each streams a slice of the pair's points through shared memory against the chunk's
 //            fp32 models, one thread per hypothesis, and adds its inlier counts
 //   refit    one CTA per pair: folds the last chunk, least-squares refit on the best hypothesis's inliers, recount,
@@ -16,32 +16,9 @@
 
 namespace {
 
-// Folds chunk c's counts into the pair's best and decides whether the pair stops.  Called by every thread of a
-// GEO_CHUNK-thread CTA; thread t owns hypothesis c * GEO_CHUNK + t.
-__device__ void geo_fold(const GeoArgs& a, int b, int c) {
-  __shared__ unsigned long long best;
-  GeoPair* P = a.w.pair + b;
-  const int t = threadIdx.x;
-  const bool live = P->stop == 0;
-  if (t == 0) best = P->best;
-  __syncthreads();
-  const int k = a.w.count[(long)b * GEO_CHUNK + t];
-  if (live && k >= 0) atomicMax(&best, ((unsigned long long)(k + 1) << 32) | (unsigned)~(unsigned)(c * GEO_CHUNK + t));
-  __syncthreads();
-  if (t == 0 && live) {
-    const int drawn = min((c + 1) * GEO_CHUNK, a.max_iters);
-    const int cnt = best ? (int)(best >> 32) - 1 : 0;
-    P->best = best;
-    P->drawn = drawn;
-    P->stop = drawn >= a.max_iters || drawn >= update_num_iters(a.confidence, 1.0 - (double)cnt / P->n, a.s, a.max_iters);
-  }
-  __syncthreads();
-}
-
-
 __global__ void __launch_bounds__(GEO_CHUNK, 1) geo_hyp_kernel(GeoArgs a, int c) {
   const int b = blockIdx.x, t = threadIdx.x;
-  if (c > 0) geo_fold(a, b, c - 1);
+  if (c > 0) geo_fold<1>(a, a.s, b, c - 1);
   const GeoPair& P = a.w.pair[b];
   const int h = c * GEO_CHUNK + t;
   double m[9];
@@ -53,28 +30,20 @@ __global__ void __launch_bounds__(GEO_CHUNK, 1) geo_hyp_kernel(GeoArgs a, int c)
   a.w.count[(long)b * GEO_CHUNK + t] = ok ? 0 : -1;
 }
 
-__global__ void __launch_bounds__(GEO_CHUNK) geo_score_kernel(GeoArgs a) {
-  const int b = blockIdx.x, split = blockIdx.y, t = threadIdx.x;
-  const GeoPair& P = a.w.pair[b];
-  if (P.stop) return;
-  const int lo = (int)((long)P.n * split / gridDim.y), hi = (int)((long)P.n * (split + 1) / gridDim.y);
-  int* cnt = a.w.count + (long)b * GEO_CHUNK + t;
-  const bool valid = *cnt >= 0;
-  float h[9];
-  for (int i = 0; i < 9; ++i) h[i] = valid ? a.w.hyp[((long)b * GEO_CHUNK + t) * 9 + i] : 0.f;
-  const float4* pts = a.w.pts + (long)b * a.M;
-  __shared__ float4 tile[TILE];
-  int k = 0;
-  for (int base = lo; base < hi; base += TILE) {
-    const int m = min(TILE, hi - base);
-    __syncthreads();
-    for (int i = t; i < m; i += GEO_CHUNK) tile[i] = pts[base + i];
-    __syncthreads();
-    if (valid)
-      for (int i = 0; i < m; ++i) k += geo_err(a.kind, h, tile[i]) < a.thr2;
-  }
-  if (k) atomicAdd(cnt, k);
-}
+// H or F inlier counts, the model kind read at run time
+struct HfScore {
+  using Args = GeoArgs;
+  using Acc = int;
+  static constexpr int SOLS = 1, NF = 9, K = 1, TILE = ::TILE;
+  static __device__ const GeoWs& ws(const GeoArgs& a) { return a.w; }
+  const float4* src[K];
+  int* sums;
+  int kind;
+  float thr2;
+  __device__ HfScore(const GeoArgs& a, const GeoPair&, int b)
+      : src{a.w.pts + (long)b * a.M}, sums(a.w.count), kind(a.kind), thr2(a.thr2) {}
+  __device__ int term(const float* h, const float4* p) const { return geo_err(kind, h, p[0]) < thr2; }
+};
 
 // Normalised DLT / 8-point rows of one correspondence; returns the number of rows (header step 4)
 __device__ __forceinline__ int geo_rows(int kind, const GeoPair& P, float4 p, double* ra, double* rb) {
@@ -93,7 +62,7 @@ __device__ __forceinline__ int geo_rows(int kind, const GeoPair& P, float4 p, do
 
 __global__ void __launch_bounds__(RED, 1) geo_refit_kernel(GeoArgs a) {
   const int b = blockIdx.x, t = threadIdx.x;
-  geo_fold(a, b, a.chunks - 1);
+  geo_fold<1>(a, a.s, b, a.chunks - 1);
   const GeoPair& P = a.w.pair[b];
   const float4* pts = a.w.pts + (long)b * a.M;
   const int* idx = a.w.idx + (long)b * a.M;
@@ -115,7 +84,7 @@ __global__ void __launch_bounds__(RED, 1) geo_refit_kernel(GeoArgs a) {
     }
     return;
   }
-  const unsigned hb = ~(unsigned)(key & 0xffffffffu);
+  const unsigned hb = ~(unsigned)(key & 0xffffffffu) >> 4;
   const int hcount = (int)(key >> 32) - 1;
   if (t == 0) {
     geo_hypothesis(a, P, pts, hb, model[0]);
@@ -184,27 +153,22 @@ extern "C" size_t geo_workspace_bytes(int32_t B, int32_t M, int32_t) {
 
 extern "C" int geo_estimate(const GeoConfig* cfg, const GeoInputs* in, GeoOutputs* out, void* workspace,
                             size_t workspace_bytes, void* stream_) {
-  if (!cfg || !in || !out) return lg_set_error("geo_estimate: null argument");
-  if (cfg->abi_version != GEO_ABI_VERSION) return lg_set_error("geo_estimate: ABI version mismatch");
-  if (cfg->model != GEO_HOMOGRAPHY && cfg->model != GEO_FUNDAMENTAL) return lg_set_error("geo_estimate: unknown model");
-  if (cfg->max_iters < 1 || cfg->max_iters > GEO_MAX_ITERS) return lg_set_error("geo_estimate: max_iters outside [1, 2^24]");
-  if (!(cfg->threshold > 0.0) || !isfinite(cfg->threshold)) return lg_set_error("geo_estimate: threshold must be positive");
-  if (!(cfg->confidence >= 0.0 && cfg->confidence <= 1.0)) return lg_set_error("geo_estimate: confidence outside [0, 1]");
-  if (in->B < 0 || in->M < 0 || in->N < 0) return lg_set_error("geo_estimate: negative size");
-  if (in->B == 0) return 0;
-  if (!out->model || !out->num_inliers || !out->success || !out->best_hypothesis || !out->num_hypotheses ||
-      (in->M > 0 && !out->inliers))  // an empty [B, 0] mask may have no storage
-    return lg_set_error("geo_estimate: null output");
-  if (in->M > 0 && (!in->kpts0 || !in->matches0 || (in->N > 0 && !in->kpts1))) return lg_set_error("geo_estimate: null input");
-  if (!workspace || workspace_bytes < geo_workspace_bytes(in->B, in->M, cfg->max_iters))
-    return lg_set_error("geo_estimate: workspace too small");
+  const char* entry = "geo_estimate";
+  int rc = geo_check_config(entry, cfg, in, out, INT_MAX, [&] {
+    return cfg->model != GEO_HOMOGRAPHY && cfg->model != GEO_FUNDAMENTAL ? "unknown model" : nullptr;
+  }, geo_no_check);
+  if (rc == GEO_RUN)
+    rc = geo_check_buffers(entry, in, {out->model, out->num_inliers, out->success, out->best_hypothesis,
+                                       out->num_hypotheses}, {out->inliers}, {}, in->kpts1, workspace, workspace_bytes,
+                           geo_workspace_bytes(in->B, in->M, cfg->max_iters));
+  if (rc != GEO_RUN) return rc;
   GeoArgs a{};
-  carve((char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255), in->B, in->M, &a.w);
+  carve(geo_workspace_base(workspace), in->B, in->M, &a.w);
   a.B = in->B; a.M = in->M; a.N = in->N;
   a.kind = cfg->model;
   a.s = cfg->model == GEO_HOMOGRAPHY ? 4 : 8;
   a.max_iters = cfg->max_iters;
-  a.chunks = (cfg->max_iters + GEO_CHUNK - 1) / GEO_CHUNK;
+  a.chunks = geo_chunks(cfg->max_iters);
   a.seed = cfg->seed;
   a.thr2 = (float)(cfg->threshold * cfg->threshold);
   a.confidence = cfg->confidence;
@@ -217,7 +181,7 @@ extern "C" int geo_estimate(const GeoConfig* cfg, const GeoInputs* in, GeoOutput
   for (int c = 0; c < a.chunks; ++c) {
     geo_hyp_kernel<<<a.B, GEO_CHUNK, 0, stream>>>(a, c);
     LG_CHECK_LAUNCH();
-    geo_score_kernel<<<dim3(a.B, splits), GEO_CHUNK, 0, stream>>>(a);
+    geo_score_kernel<HfScore><<<dim3(a.B, splits), GEO_CHUNK, 0, stream>>>(a);
     LG_CHECK_LAUNCH();
   }
   geo_refit_kernel<<<a.B, RED, 0, stream>>>(a);

@@ -15,7 +15,7 @@ constexpr int TILE = 1024;  // points per shared-memory tile of the score kernel
 
 struct GeoPair {
   double cx0, cy0, s0, cx1, cy1, s1;  // Hartley normalisation of image 0 and image 1
-  unsigned long long best;            // (count + 1) << 32 | ~h of the best hypothesis so far; 0: none
+  unsigned long long best;            // (count + 1) << 32 | ~(h * 16) of the best hypothesis so far; 0: none
   int n;                              // valid matches
   int ok;                             // n >= sample size and the normalisation succeeded
   int stop;                           // no further hypotheses are drawn
@@ -39,6 +39,9 @@ size_t carve(char* base, int B, int M, GeoWs* w) {
   w->count = b.take<int>((size_t)B * GEO_CHUNK);
   return b.bytes();
 }
+
+// geo_fold's and geo_score_kernel's valid models of chunk slot `slot`: one, unless degenerate or not drawn
+__device__ __forceinline__ int geo_models(const GeoWs& w, long slot) { return w.count[slot] >= 0; }
 
 struct GeoArgs {
   int B, M, N, kind, s, max_iters, chunks;

@@ -15,7 +15,6 @@
 // A stopped pair's CTAs return at once.  Compiled with -fmad=false: oracle/lo_homography_oracle.py and
 // oracle/lo_fundamental_oracle.py take the same steps.
 #include <stdint.h>
-#include <stdio.h>
 
 #include "geo_hf.cuh"
 #include "lg_internal.h"
@@ -72,31 +71,22 @@ __global__ void __launch_bounds__(GEO_CHUNK, 1) lohf_hyp_kernel(LoHfArgs a, int 
   a.g.w.count[(long)b * GEO_CHUNK + t] = ok ? 0 : -1;
 }
 
-// The chunk's LH3 / LF3 scores: (B, splits) CTAs, each streams a slice of the pair's points through shared memory
+// The chunk's LH3 / LF3 scores, count << 40 | MSAC score
 template <int KIND>
-__global__ void __launch_bounds__(GEO_CHUNK) lohf_score_kernel(LoHfArgs a) {
-  const int b = blockIdx.x, split = blockIdx.y, t = threadIdx.x;
-  const GeoPair& P = a.g.w.pair[b];
-  if (P.stop) return;
-  const int lo = (int)((long)P.n * split / gridDim.y), hi = (int)((long)P.n * (split + 1) / gridDim.y);
-  const bool valid = a.g.w.count[(long)b * GEO_CHUNK + t] >= 0;
-  float h[9];
-  for (int i = 0; i < 9; ++i) h[i] = valid ? a.g.w.hyp[((long)b * GEO_CHUNK + t) * 9 + i] : 0.f;
-  const float thr2 = a.g.thr2;
-  const float w = (float)GEO_LO_QSCALE / thr2;
-  const float4* pts = a.g.w.pts + (long)b * a.g.M;
-  __shared__ float4 tile[TILE];
-  unsigned long long k = 0;
-  for (int base = lo; base < hi; base += TILE) {
-    const int m = min(TILE, hi - base);
-    __syncthreads();
-    for (int i = t; i < m; i += GEO_CHUNK) tile[i] = pts[base + i];
-    __syncthreads();
-    if (valid)
-      for (int i = 0; i < m; ++i) k += lo_term(geo_err(KIND, h, tile[i]), thr2, w);
+struct LoHfScore {
+  using Args = LoHfArgs;
+  using Acc = unsigned long long;
+  static constexpr int SOLS = 1, NF = 9, K = 1, TILE = ::TILE;
+  static __device__ const GeoWs& ws(const LoHfArgs& a) { return a.g.w; }
+  const float4* src[K];
+  unsigned long long* sums;
+  float thr2, w;
+  __device__ LoHfScore(const LoHfArgs& a, const GeoPair&, int b)
+      : src{a.g.w.pts + (long)b * a.g.M}, sums(a.l.acc), thr2(a.g.thr2), w((float)GEO_LO_QSCALE / a.g.thr2) {}
+  __device__ unsigned long long term(const float* h, const float4* p) const {
+    return lo_term(geo_err(KIND, h, p[0]), thr2, w);
   }
-  if (k) atomicAdd(a.l.acc + (long)b * GEO_CHUNK + t, k);
-}
+};
 
 // T1^-1 X T0 (H) or (T1^T X) T0 (F), unscaled: the first half of denormalise
 template <int KIND>
@@ -464,47 +454,35 @@ size_t lohf_workspace_bytes(int B, int M) {
   return lohf_carve(nullptr, B, M, &w, &l) + 256;
 }
 
-int lohf_error(const char* name, const char* what) {
-  char msg[96];
-  snprintf(msg, sizeof(msg), "%s: %s", name, what);
-  return lg_set_error(msg);
-}
-
 // geo_homography_lo and geo_fundamental_lo: name for the error strings, s the points per sample
 template <class Model>
 int lohf_estimate(const char* name, int s, const GeoConfig* cfg, const GeoInputs* in, GeoLoOutputs* out,
                   void* workspace, size_t workspace_bytes, void* stream_) {
-  if (!cfg || !in || !out) return lohf_error(name, "null argument");
-  if (cfg->abi_version != GEO_ABI_VERSION) return lohf_error(name, "ABI version mismatch");
-  if (cfg->model != Model::KIND)
-    return lohf_error(name, Model::KIND == GEO_HOMOGRAPHY ? "model must be GEO_HOMOGRAPHY"
-                                                          : "model must be GEO_FUNDAMENTAL");
-  if (cfg->max_iters < 1 || cfg->max_iters > GEO_MAX_ITERS) return lohf_error(name, "max_iters outside [1, 2^24]");
-  if (!(cfg->threshold > 0.0) || !isfinite(cfg->threshold)) return lohf_error(name, "threshold must be positive");
-  if (!(cfg->confidence >= 0.0 && cfg->confidence <= 1.0)) return lohf_error(name, "confidence outside [0, 1]");
-  if (in->B < 0 || in->M < 0 || in->N < 0) return lohf_error(name, "negative size");
-  if (in->M > GEO_LO_MAX_MATCHES) return lohf_error(name, "M above GEO_LO_MAX_MATCHES");
-  if (in->B == 0) return 0;
-  const GeoOutputs& o = out->geo;
-  if (!o.model || !o.num_inliers || !o.success || !o.best_hypothesis || !o.num_hypotheses ||
-      !out->num_local_optimizations || !out->cost || (in->M > 0 && !o.inliers))  // an empty mask may have no storage
-    return lohf_error(name, "null output");
-  if (in->M > 0 && (!in->kpts0 || !in->matches0 || (in->N > 0 && !in->kpts1))) return lohf_error(name, "null input");
-  if (!workspace || workspace_bytes < lohf_workspace_bytes(in->B, in->M))
-    return lohf_error(name, "workspace too small");
+  int rc = geo_check_config(name, cfg, in, out, GEO_LO_MAX_MATCHES, [&] {
+    return cfg->model == Model::KIND          ? nullptr
+           : Model::KIND == GEO_HOMOGRAPHY ? "model must be GEO_HOMOGRAPHY"
+                                           : "model must be GEO_FUNDAMENTAL";
+  }, geo_no_check);
+  if (rc == GEO_RUN) {
+    const GeoOutputs& o = out->geo;
+    rc = geo_check_buffers(name, in, {o.model, o.num_inliers, o.success, o.best_hypothesis, o.num_hypotheses,
+                                      out->num_local_optimizations, out->cost}, {o.inliers}, {}, in->kpts1,
+                           workspace, workspace_bytes, lohf_workspace_bytes(in->B, in->M));
+  }
+  if (rc != GEO_RUN) return rc;
   LoHfArgs a{};
-  lohf_carve((char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255), in->B, in->M, &a.g.w, &a.l);
+  lohf_carve(geo_workspace_base(workspace), in->B, in->M, &a.g.w, &a.l);
   GeoArgs& g = a.g;
   g.B = in->B; g.M = in->M; g.N = in->N;
   g.kind = Model::KIND;
   g.s = s;
   g.max_iters = cfg->max_iters;
-  g.chunks = (cfg->max_iters + GEO_CHUNK - 1) / GEO_CHUNK;
+  g.chunks = geo_chunks(cfg->max_iters);
   g.seed = cfg->seed;
   g.thr2 = (float)(cfg->threshold * cfg->threshold);
   g.confidence = cfg->confidence;
   g.kpts0 = in->kpts0; g.kpts1 = in->kpts1; g.matches0 = in->matches0;
-  g.out = o;
+  g.out = out->geo;
   a.num_lo = out->num_local_optimizations;
   a.cost = out->cost;
   const int splits = geo_score_splits(g.B, g.M);
@@ -514,7 +492,7 @@ int lohf_estimate(const char* name, int s, const GeoConfig* cfg, const GeoInputs
   for (int c = 0; c < g.chunks; ++c) {
     lohf_hyp_kernel<<<g.B, GEO_CHUNK, 0, stream>>>(a, c);
     LG_CHECK_LAUNCH();
-    lohf_score_kernel<Model::KIND><<<dim3(g.B, splits), GEO_CHUNK, 0, stream>>>(a);
+    geo_score_kernel<LoHfScore<Model::KIND>><<<dim3(g.B, splits), GEO_CHUNK, 0, stream>>>(a);
     LG_CHECK_LAUNCH();
     lohf_lo_kernel<Model><<<g.B, RED, 0, stream>>>(a, c);
     LG_CHECK_LAUNCH();

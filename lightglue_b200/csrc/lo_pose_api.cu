@@ -215,41 +215,21 @@ __global__ void __launch_bounds__(GEO_CHUNK, 1) lo_hyp_kernel(LoArgs a, int c) {
   a.p.w.nsol[(long)b * GEO_CHUNK + t] = ns;
 }
 
-__global__ void __launch_bounds__(GEO_CHUNK) lo_score_kernel(LoArgs a) {
-  const int b = blockIdx.x, split = blockIdx.y, t = threadIdx.x;
-  const PosePair& P = a.p.w.pair[b];
-  if (P.stop) return;
-  const int lo = (int)((long)P.n * split / gridDim.y), hi = (int)((long)P.n * (split + 1) / gridDim.y);
-  const int ns = a.p.w.nsol[(long)b * GEO_CHUNK + t];
-  const float* hm = a.p.w.hyp + ((long)b * GEO_CHUNK + t) * SOLS * 9;
-  const float thr2 = P.thr2;
-  const float w = (float)GEO_LO_QSCALE / thr2;
-  float g[SOLS][9];
-  unsigned long long k[SOLS];
-#pragma unroll
-  for (int r = 0; r < SOLS; ++r) {
-    k[r] = 0;
-#pragma unroll
-    for (int i = 0; i < 9; ++i) g[r][i] = r < ns ? hm[r * 9 + i] : 0.f;
+// The chunk's L3 scores of every solution, count << 40 | MSAC score
+struct LoPoseScore {
+  using Args = LoArgs;
+  using Acc = unsigned long long;
+  static constexpr int SOLS = ::SOLS, NF = 9, K = 1, TILE = ::TILE;
+  static __device__ const PoseWs& ws(const LoArgs& a) { return a.p.w; }
+  const float4* src[K];
+  unsigned long long* sums;
+  float thr2, w;
+  __device__ LoPoseScore(const LoArgs& a, const PosePair& P, int b)
+      : src{a.p.w.pts + (long)b * a.p.M}, sums(a.l.acc), thr2(P.thr2), w((float)GEO_LO_QSCALE / P.thr2) {}
+  __device__ unsigned long long term(const float* g, const float4* p) const {
+    return lo_term(sampson(g, p[0]), thr2, w);
   }
-  const float4* pts = a.p.w.pts + (long)b * a.p.M;
-  __shared__ float4 tile[TILE];
-  for (int base = lo; base < hi; base += TILE) {
-    const int m = min(TILE, hi - base);
-    __syncthreads();
-    for (int i = t; i < m; i += GEO_CHUNK) tile[i] = pts[base + i];
-    __syncthreads();
-    for (int i = 0; i < m; ++i) {
-      const float4 p = tile[i];
-#pragma unroll
-      for (int r = 0; r < SOLS; ++r)
-        if (r < ns) k[r] += lo_term(sampson(g[r], p), thr2, w);
-    }
-  }
-#pragma unroll
-  for (int r = 0; r < SOLS; ++r)
-    if (r < ns && k[r]) atomicAdd(a.l.acc + ((long)b * GEO_CHUNK + t) * SOLS + r, k[r]);
-}
+};
 
 // P7's choice among the candidates of s.fm (widened) on s.fm's inliers, into s.x; every thread calls it
 __device__ void lo_choose_pose(LoShared<PoseLo>& s, const float4* pts, int n, float thr2, double distance, int tid) {
@@ -417,42 +397,32 @@ extern "C" size_t geo_lo_pose_workspace_bytes(int32_t B, int32_t M, int32_t) {
 
 extern "C" int geo_relative_pose_lo(const GeoLoPoseConfig* cfg, const GeoPoseInputs* in, GeoLoPoseOutputs* out,
                                     void* workspace, size_t workspace_bytes, void* stream_) {
-  if (!cfg || !in || !out) return lg_set_error("geo_relative_pose_lo: null argument");
-  if (cfg->abi_version != GEO_ABI_VERSION) return lg_set_error("geo_relative_pose_lo: ABI version mismatch");
-  if (cfg->max_iters < 1 || cfg->max_iters > GEO_MAX_ITERS)
-    return lg_set_error("geo_relative_pose_lo: max_iters outside [1, 2^24]");
-  if (!(cfg->threshold > 0.0) || !isfinite(cfg->threshold))
-    return lg_set_error("geo_relative_pose_lo: threshold must be positive");
-  if (!(cfg->confidence >= 0.0 && cfg->confidence <= 1.0))
-    return lg_set_error("geo_relative_pose_lo: confidence outside [0, 1]");
-  if (!(cfg->distance_threshold > 0.0) || !isfinite(cfg->distance_threshold))
-    return lg_set_error("geo_relative_pose_lo: distance_threshold must be positive");
-  if (in->B < 0 || in->M < 0 || in->N < 0) return lg_set_error("geo_relative_pose_lo: negative size");
-  if (in->M > GEO_LO_MAX_MATCHES) return lg_set_error("geo_relative_pose_lo: M above GEO_LO_MAX_MATCHES");
-  if (in->B == 0) return 0;
-  const GeoPoseOutputs& o = out->pose;
-  if (!o.E || !o.R || !o.t || !o.num_inliers || !o.num_pose_inliers || !o.success || !o.best_hypothesis ||
-      !o.best_solution || !o.num_hypotheses || !out->num_local_optimizations || !out->cost ||
-      (in->M > 0 && (!o.inliers || !o.pose_inliers)))  // empty [B, 0] masks may have no storage
-    return lg_set_error("geo_relative_pose_lo: null output");
-  if (!in->K0 || !in->K1) return lg_set_error("geo_relative_pose_lo: null intrinsics");
-  if (in->M > 0 && (!in->kpts0 || !in->matches0 || (in->N > 0 && !in->kpts1)))
-    return lg_set_error("geo_relative_pose_lo: null input");
-  if (!workspace || workspace_bytes < geo_lo_pose_workspace_bytes(in->B, in->M, cfg->max_iters))
-    return lg_set_error("geo_relative_pose_lo: workspace too small");
+  const char* entry = "geo_relative_pose_lo";
+  int rc = geo_check_config(entry, cfg, in, out, GEO_LO_MAX_MATCHES, geo_no_check, [&] {
+    return !(cfg->distance_threshold > 0.0) || !isfinite(cfg->distance_threshold) ? "distance_threshold must be positive"
+                                                                                   : nullptr;
+  });
+  if (rc == GEO_RUN) {
+    const GeoPoseOutputs& o = out->pose;
+    rc = geo_check_buffers(entry, in, {o.E, o.R, o.t, o.num_inliers, o.num_pose_inliers, o.success, o.best_hypothesis,
+                                       o.best_solution, o.num_hypotheses, out->num_local_optimizations, out->cost},
+                           {o.inliers, o.pose_inliers}, {in->K0, in->K1}, in->kpts1, workspace, workspace_bytes,
+                           geo_lo_pose_workspace_bytes(in->B, in->M, cfg->max_iters));
+  }
+  if (rc != GEO_RUN) return rc;
   LoArgs a{};
-  lo_carve((char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255), in->B, in->M, &a.p.w, &a.l);
+  lo_carve(geo_workspace_base(workspace), in->B, in->M, &a.p.w, &a.l);
   PoseArgs& p = a.p;
   p.B = in->B; p.M = in->M; p.N = in->N;
   p.max_iters = cfg->max_iters;
-  p.chunks = (cfg->max_iters + GEO_CHUNK - 1) / GEO_CHUNK;
+  p.chunks = geo_chunks(cfg->max_iters);
   p.seed = cfg->seed;
   p.threshold = cfg->threshold;
   p.confidence = cfg->confidence;
   p.distance = cfg->distance_threshold;
   p.kpts0 = in->kpts0; p.kpts1 = in->kpts1; p.matches0 = in->matches0;
   p.K0 = in->K0; p.K1 = in->K1;
-  p.out = o;
+  p.out = out->pose;
   a.num_lo = out->num_local_optimizations;
   a.cost = out->cost;
   const int splits = geo_score_splits(p.B, p.M);
@@ -462,7 +432,7 @@ extern "C" int geo_relative_pose_lo(const GeoLoPoseConfig* cfg, const GeoPoseInp
   for (int c = 0; c < p.chunks; ++c) {
     lo_hyp_kernel<<<p.B, GEO_CHUNK, 0, stream>>>(a, c);
     LG_CHECK_LAUNCH();
-    lo_score_kernel<<<dim3(p.B, splits), GEO_CHUNK, 0, stream>>>(a);
+    geo_score_kernel<LoPoseScore><<<dim3(p.B, splits), GEO_CHUNK, 0, stream>>>(a);
     LG_CHECK_LAUNCH();
     lo_kernel<<<p.B, RED, 0, stream>>>(a, c);
     LG_CHECK_LAUNCH();

@@ -4,8 +4,8 @@
 // Launches, all fixed by (B, M, max_iters):
 //   prepare  one 1024-thread CTA per pair: ordered compaction of the valid matches, calibrated coordinates, K check
 //   per chunk of GEO_CHUNK samples:
-//     hyp    one CTA per pair: folds the previous chunk's counts into the pair's best (packed (count + 1, ~(h*16 + r)),
-//            atomic max), decides the adaptive stop, then one thread per sample solves it: up to 4 fp32 projections
+//     hyp    one CTA per pair: folds the previous chunk's counts into the pair's best (geo_fold), decides the
+//            adaptive stop, then one thread per sample solves it: up to 4 fp32 projections
 //     score  (B, splits) CTAs: each streams a slice of the pair's points through shared memory against every solution
 //            of the chunk, one thread per sample, and adds the inlier counts
 //   refit    one CTA per pair: folds the last chunk, Levenberg-Marquardt from the best solution, recount, R and t
@@ -266,32 +266,6 @@ __device__ bool k_valid(const double* K) {
   return finite && K[0] > 0.0 && K[4] > 0.0 && K[6] == 0.0 && K[7] == 0.0 && K[8] == 1.0;
 }
 
-// Folds chunk c's counts into the pair's best and decides whether the pair stops.  Called by every thread of a
-// GEO_CHUNK-thread CTA; thread t owns sample c * GEO_CHUNK + t.
-__device__ void pnp_fold(const PnpArgs& a, int b, int c) {
-  __shared__ unsigned long long best;
-  PnpPair* P = a.w.pair + b;
-  const int t = threadIdx.x;
-  const bool live = P->stop == 0;
-  if (t == 0) best = P->best;
-  __syncthreads();
-  const int ns = a.w.nsol[(long)b * GEO_CHUNK + t];
-  const unsigned h = c * GEO_CHUNK + t;
-  for (int r = 0; live && r < ns; ++r) {
-    const int k = a.w.count[((long)b * GEO_CHUNK + t) * SOLS + r];
-    atomicMax(&best, ((unsigned long long)(k + 1) << 32) | (unsigned)~(h * 16u + (unsigned)r));
-  }
-  __syncthreads();
-  if (t == 0 && live) {
-    const int drawn = min((c + 1) * GEO_CHUNK, a.max_iters);
-    const int cnt = best ? (int)(best >> 32) - 1 : 0;
-    P->best = best;
-    P->drawn = drawn;
-    P->stop = drawn >= a.max_iters || drawn >= update_num_iters(a.confidence, 1.0 - (double)cnt / P->n, S, a.max_iters);
-  }
-  __syncthreads();
-}
-
 __global__ void __launch_bounds__(1024) pnp_prepare_kernel(PnpArgs a) {
   const int b = blockIdx.x, tid = threadIdx.x;
   __shared__ int warp_sums[32];
@@ -339,7 +313,7 @@ __global__ void __launch_bounds__(1024) pnp_prepare_kernel(PnpArgs a) {
 
 __global__ void __launch_bounds__(GEO_CHUNK, 1) pnp_hyp_kernel(PnpArgs a, int c) {
   const int b = blockIdx.x, t = threadIdx.x;
-  if (c > 0) pnp_fold(a, b, c - 1);
+  if (c > 0) geo_fold<SOLS>(a, S, b, c - 1);
   const PnpPair& P = a.w.pair[b];
   const int h = c * GEO_CHUNK + t;
   int ns = 0;
@@ -359,44 +333,19 @@ __global__ void __launch_bounds__(GEO_CHUNK, 1) pnp_hyp_kernel(PnpArgs a, int c)
   a.w.nsol[(long)b * GEO_CHUNK + t] = ns;
 }
 
-__global__ void __launch_bounds__(GEO_CHUNK) pnp_score_kernel(PnpArgs a) {
-  const int b = blockIdx.x, split = blockIdx.y, t = threadIdx.x;
-  const PnpPair& P = a.w.pair[b];
-  if (P.stop) return;
-  const int lo = (int)((long)P.n * split / gridDim.y), hi = (int)((long)P.n * (split + 1) / gridDim.y);
-  const int ns = a.w.nsol[(long)b * GEO_CHUNK + t];
-  const float* hm = a.w.hyp + ((long)b * GEO_CHUNK + t) * SOLS * 12;
-  const float thr2 = P.thr2;
-  float g[SOLS][12];
-  int k[SOLS];
-#pragma unroll
-  for (int r = 0; r < SOLS; ++r) {
-    k[r] = 0;
-#pragma unroll
-    for (int i = 0; i < 12; ++i) g[r][i] = r < ns ? hm[r * 12 + i] : 0.f;
-  }
-  const float4* pts = a.w.pts + (long)b * a.M;
-  const float4* wld = a.w.wld + (long)b * a.M;
-  __shared__ float4 tp[TILE], tw[TILE];
-  for (int base = lo; base < hi; base += TILE) {
-    const int m = min(TILE, hi - base);
-    __syncthreads();
-    for (int i = t; i < m; i += GEO_CHUNK) {
-      tp[i] = pts[base + i];
-      tw[i] = wld[base + i];
-    }
-    __syncthreads();
-    for (int i = 0; i < m; ++i) {
-      const float4 p = tp[i], q = tw[i];
-#pragma unroll
-      for (int r = 0; r < SOLS; ++r)
-        if (r < ns) k[r] += reproj_inlier(g[r], p, q, thr2);
-    }
-  }
-#pragma unroll
-  for (int r = 0; r < SOLS; ++r)
-    if (r < ns && k[r]) atomicAdd(a.w.count + ((long)b * GEO_CHUNK + t) * SOLS + r, k[r]);
-}
+// Inlier counts of every projection, on a tile of pixels and world points
+struct PnpScore {
+  using Args = PnpArgs;
+  using Acc = int;
+  static constexpr int SOLS = ::SOLS, NF = 12, K = 2, TILE = ::TILE;
+  static __device__ const PnpWs& ws(const PnpArgs& a) { return a.w; }
+  const float4* src[K];
+  int* sums;
+  float thr2;
+  __device__ PnpScore(const PnpArgs& a, const PnpPair& P, int b)
+      : src{a.w.pts + (long)b * a.M, a.w.wld + (long)b * a.M}, sums(a.w.count), thr2(P.thr2) {}
+  __device__ int term(const float* g, const float4* p) const { return reproj_inlier(g, p[0], p[1], thr2); }
+};
 
 constexpr int LM_TERMS = 28;  // J^T J upper triangle (21), J^T r (6), cost
 
@@ -444,7 +393,7 @@ __device__ void lm_update(const double* R, const double* t, const double* d, dou
 
 __global__ void __launch_bounds__(RED, 1) pnp_refit_kernel(PnpArgs a) {
   const int b = blockIdx.x, t = threadIdx.x;
-  pnp_fold(a, b, a.chunks - 1);
+  geo_fold<SOLS>(a, S, b, a.chunks - 1);
   PnpPair& P = a.w.pair[b];
   const float4* pts = a.w.pts + (long)b * a.M;
   const float4* wld = a.w.wld + (long)b * a.M;
@@ -570,29 +519,19 @@ extern "C" size_t geo_pnp_workspace_bytes(int32_t B, int32_t M, int32_t) {
 
 extern "C" int geo_absolute_pose(const GeoPnpConfig* cfg, const GeoPnpInputs* in, GeoPnpOutputs* out, void* workspace,
                                  size_t workspace_bytes, void* stream_) {
-  if (!cfg || !in || !out) return lg_set_error("geo_absolute_pose: null argument");
-  if (cfg->abi_version != GEO_ABI_VERSION) return lg_set_error("geo_absolute_pose: ABI version mismatch");
-  if (cfg->max_iters < 1 || cfg->max_iters > GEO_MAX_ITERS)
-    return lg_set_error("geo_absolute_pose: max_iters outside [1, 2^24]");
-  if (!(cfg->threshold > 0.0) || !isfinite(cfg->threshold))
-    return lg_set_error("geo_absolute_pose: threshold must be positive");
-  if (!(cfg->confidence >= 0.0 && cfg->confidence <= 1.0))
-    return lg_set_error("geo_absolute_pose: confidence outside [0, 1]");
-  if (in->B < 0 || in->M < 0 || in->N < 0) return lg_set_error("geo_absolute_pose: negative size");
-  if (in->B == 0) return 0;
-  if (!out->R || !out->t || !out->num_inliers || !out->success || !out->best_hypothesis || !out->best_solution ||
-      !out->num_hypotheses || (in->M > 0 && !out->inliers))  // an empty [B, 0] mask may have no storage
-    return lg_set_error("geo_absolute_pose: null output");
-  if (!in->K0) return lg_set_error("geo_absolute_pose: null intrinsics");
-  if (in->M > 0 && (!in->kpts0 || !in->matches0 || (in->N > 0 && !in->points3d1)))
-    return lg_set_error("geo_absolute_pose: null input");
-  if (!workspace || workspace_bytes < geo_pnp_workspace_bytes(in->B, in->M, cfg->max_iters))
-    return lg_set_error("geo_absolute_pose: workspace too small");
+  const char* entry = "geo_absolute_pose";
+  int rc = geo_check_config(entry, cfg, in, out, INT_MAX, geo_no_check, geo_no_check);
+  if (rc == GEO_RUN)
+    rc = geo_check_buffers(entry, in, {out->R, out->t, out->num_inliers, out->success, out->best_hypothesis,
+                                       out->best_solution, out->num_hypotheses}, {out->inliers}, {in->K0},
+                           in->points3d1, workspace, workspace_bytes,
+                           geo_pnp_workspace_bytes(in->B, in->M, cfg->max_iters));
+  if (rc != GEO_RUN) return rc;
   PnpArgs a{};
-  carve((char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255), in->B, in->M, &a.w);
+  carve(geo_workspace_base(workspace), in->B, in->M, &a.w);
   a.B = in->B; a.M = in->M; a.N = in->N;
   a.max_iters = cfg->max_iters;
-  a.chunks = (cfg->max_iters + GEO_CHUNK - 1) / GEO_CHUNK;
+  a.chunks = geo_chunks(cfg->max_iters);
   a.seed = cfg->seed;
   a.threshold = cfg->threshold;
   a.confidence = cfg->confidence;
@@ -606,7 +545,7 @@ extern "C" int geo_absolute_pose(const GeoPnpConfig* cfg, const GeoPnpInputs* in
   for (int c = 0; c < a.chunks; ++c) {
     pnp_hyp_kernel<<<a.B, GEO_CHUNK, 0, stream>>>(a, c);
     LG_CHECK_LAUNCH();
-    pnp_score_kernel<<<dim3(a.B, splits), GEO_CHUNK, 0, stream>>>(a);
+    geo_score_kernel<PnpScore><<<dim3(a.B, splits), GEO_CHUNK, 0, stream>>>(a);
     LG_CHECK_LAUNCH();
   }
   pnp_refit_kernel<<<a.B, RED, 0, stream>>>(a);

@@ -4,8 +4,8 @@
 // Launches, all fixed by (B, M, max_iters):
 //   prepare  one 1024-thread CTA per pair: ordered compaction of the valid matches, calibrated coordinates, K checks
 //   per chunk of GEO_CHUNK samples:
-//     hyp    one CTA per pair: folds the previous chunk's counts into the pair's best (packed (count + 1, ~(h*16 + r)),
-//            atomic max), decides the adaptive stop, then one thread per sample solves it: up to 10 fp32 models
+//     hyp    one CTA per pair: folds the previous chunk's counts into the pair's best (geo_fold), decides the
+//            adaptive stop, then one thread per sample solves it: up to 10 fp32 models
 //     score  (B, splits) CTAs: each streams a slice of the pair's points through shared memory against every solution
 //            of the chunk, one thread per sample, and adds the inlier counts
 //   refit    one CTA per pair: folds the last chunk, least-squares refit projected on the essential manifold, recount,
@@ -20,35 +20,9 @@
 
 namespace {
 
-// Folds chunk c's counts into the pair's best and decides whether the pair stops.  Called by every thread of a
-// GEO_CHUNK-thread CTA; thread t owns sample c * GEO_CHUNK + t.
-__device__ void pose_fold(const PoseArgs& a, int b, int c) {
-  __shared__ unsigned long long best;
-  PosePair* P = a.w.pair + b;
-  const int t = threadIdx.x;
-  const bool live = P->stop == 0;
-  if (t == 0) best = P->best;
-  __syncthreads();
-  const int ns = a.w.nsol[(long)b * GEO_CHUNK + t];
-  const unsigned h = c * GEO_CHUNK + t;
-  for (int r = 0; live && r < ns; ++r) {
-    const int k = a.w.count[((long)b * GEO_CHUNK + t) * SOLS + r];
-    atomicMax(&best, ((unsigned long long)(k + 1) << 32) | (unsigned)~(h * 16u + (unsigned)r));
-  }
-  __syncthreads();
-  if (t == 0 && live) {
-    const int drawn = min((c + 1) * GEO_CHUNK, a.max_iters);
-    const int cnt = best ? (int)(best >> 32) - 1 : 0;
-    P->best = best;
-    P->drawn = drawn;
-    P->stop = drawn >= a.max_iters || drawn >= update_num_iters(a.confidence, 1.0 - (double)cnt / P->n, S, a.max_iters);
-  }
-  __syncthreads();
-}
-
 __global__ void __launch_bounds__(GEO_CHUNK, 1) pose_hyp_kernel(PoseArgs a, int c) {
   const int b = blockIdx.x, t = threadIdx.x;
-  if (c > 0) pose_fold(a, b, c - 1);
+  if (c > 0) geo_fold<SOLS>(a, S, b, c - 1);
   const PosePair& P = a.w.pair[b];
   const int h = c * GEO_CHUNK + t;
   int ns = 0;
@@ -65,44 +39,23 @@ __global__ void __launch_bounds__(GEO_CHUNK, 1) pose_hyp_kernel(PoseArgs a, int 
   a.w.nsol[(long)b * GEO_CHUNK + t] = ns;
 }
 
-__global__ void __launch_bounds__(GEO_CHUNK) pose_score_kernel(PoseArgs a) {
-  const int b = blockIdx.x, split = blockIdx.y, t = threadIdx.x;
-  const PosePair& P = a.w.pair[b];
-  if (P.stop) return;
-  const int lo = (int)((long)P.n * split / gridDim.y), hi = (int)((long)P.n * (split + 1) / gridDim.y);
-  const int ns = a.w.nsol[(long)b * GEO_CHUNK + t];
-  const float* hm = a.w.hyp + ((long)b * GEO_CHUNK + t) * SOLS * 9;
-  const float thr2 = P.thr2;
-  float g[SOLS][9];
-  int k[SOLS];
-#pragma unroll
-  for (int r = 0; r < SOLS; ++r) {
-    k[r] = 0;
-#pragma unroll
-    for (int i = 0; i < 9; ++i) g[r][i] = r < ns ? hm[r * 9 + i] : 0.f;
-  }
-  const float4* pts = a.w.pts + (long)b * a.M;
-  __shared__ float4 tile[TILE];
-  for (int base = lo; base < hi; base += TILE) {
-    const int m = min(TILE, hi - base);
-    __syncthreads();
-    for (int i = t; i < m; i += GEO_CHUNK) tile[i] = pts[base + i];
-    __syncthreads();
-    for (int i = 0; i < m; ++i) {
-      const float4 p = tile[i];
-#pragma unroll
-      for (int r = 0; r < SOLS; ++r)
-        if (r < ns) k[r] += sampson(g[r], p) < thr2;
-    }
-  }
-#pragma unroll
-  for (int r = 0; r < SOLS; ++r)
-    if (r < ns && k[r]) atomicAdd(a.w.count + ((long)b * GEO_CHUNK + t) * SOLS + r, k[r]);
-}
+// Inlier counts of every solution
+struct PoseScore {
+  using Args = PoseArgs;
+  using Acc = int;
+  static constexpr int SOLS = ::SOLS, NF = 9, K = 1, TILE = ::TILE;
+  static __device__ const PoseWs& ws(const PoseArgs& a) { return a.w; }
+  const float4* src[K];
+  int* sums;
+  float thr2;
+  __device__ PoseScore(const PoseArgs& a, const PosePair& P, int b)
+      : src{a.w.pts + (long)b * a.M}, sums(a.w.count), thr2(P.thr2) {}
+  __device__ int term(const float* g, const float4* p) const { return sampson(g, p[0]) < thr2; }
+};
 
 __global__ void __launch_bounds__(RED, 1) pose_refit_kernel(PoseArgs a) {
   const int b = blockIdx.x, t = threadIdx.x;
-  pose_fold(a, b, a.chunks - 1);
+  geo_fold<SOLS>(a, S, b, a.chunks - 1);
   PosePair& P = a.w.pair[b];
   const float4* pts = a.w.pts + (long)b * a.M;
   const int* idx = a.w.idx + (long)b * a.M;
@@ -263,32 +216,22 @@ extern "C" size_t geo_pose_workspace_bytes(int32_t B, int32_t M, int32_t) {
 
 extern "C" int geo_relative_pose(const GeoPoseConfig* cfg, const GeoPoseInputs* in, GeoPoseOutputs* out, void* workspace,
                                  size_t workspace_bytes, void* stream_) {
-  if (!cfg || !in || !out) return lg_set_error("geo_relative_pose: null argument");
-  if (cfg->abi_version != GEO_ABI_VERSION) return lg_set_error("geo_relative_pose: ABI version mismatch");
-  if (cfg->max_iters < 1 || cfg->max_iters > GEO_MAX_ITERS)
-    return lg_set_error("geo_relative_pose: max_iters outside [1, 2^24]");
-  if (!(cfg->threshold > 0.0) || !isfinite(cfg->threshold))
-    return lg_set_error("geo_relative_pose: threshold must be positive");
-  if (!(cfg->confidence >= 0.0 && cfg->confidence <= 1.0))
-    return lg_set_error("geo_relative_pose: confidence outside [0, 1]");
-  if (!(cfg->distance_threshold > 0.0) || !isfinite(cfg->distance_threshold))
-    return lg_set_error("geo_relative_pose: distance_threshold must be positive");
-  if (in->B < 0 || in->M < 0 || in->N < 0) return lg_set_error("geo_relative_pose: negative size");
-  if (in->B == 0) return 0;
-  if (!out->E || !out->R || !out->t || !out->num_inliers || !out->num_pose_inliers || !out->success ||
-      !out->best_hypothesis || !out->best_solution || !out->num_hypotheses ||
-      (in->M > 0 && (!out->inliers || !out->pose_inliers)))  // empty [B, 0] masks may have no storage
-    return lg_set_error("geo_relative_pose: null output");
-  if (!in->K0 || !in->K1) return lg_set_error("geo_relative_pose: null intrinsics");
-  if (in->M > 0 && (!in->kpts0 || !in->matches0 || (in->N > 0 && !in->kpts1)))
-    return lg_set_error("geo_relative_pose: null input");
-  if (!workspace || workspace_bytes < geo_pose_workspace_bytes(in->B, in->M, cfg->max_iters))
-    return lg_set_error("geo_relative_pose: workspace too small");
+  const char* entry = "geo_relative_pose";
+  int rc = geo_check_config(entry, cfg, in, out, INT_MAX, geo_no_check, [&] {
+    return !(cfg->distance_threshold > 0.0) || !isfinite(cfg->distance_threshold) ? "distance_threshold must be positive"
+                                                                                   : nullptr;
+  });
+  if (rc == GEO_RUN)
+    rc = geo_check_buffers(entry, in, {out->E, out->R, out->t, out->num_inliers, out->num_pose_inliers, out->success,
+                                       out->best_hypothesis, out->best_solution, out->num_hypotheses},
+                           {out->inliers, out->pose_inliers}, {in->K0, in->K1}, in->kpts1, workspace, workspace_bytes,
+                           geo_pose_workspace_bytes(in->B, in->M, cfg->max_iters));
+  if (rc != GEO_RUN) return rc;
   PoseArgs a{};
-  carve((char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255), in->B, in->M, &a.w);
+  carve(geo_workspace_base(workspace), in->B, in->M, &a.w);
   a.B = in->B; a.M = in->M; a.N = in->N;
   a.max_iters = cfg->max_iters;
-  a.chunks = (cfg->max_iters + GEO_CHUNK - 1) / GEO_CHUNK;
+  a.chunks = geo_chunks(cfg->max_iters);
   a.seed = cfg->seed;
   a.threshold = cfg->threshold;
   a.confidence = cfg->confidence;
@@ -303,7 +246,7 @@ extern "C" int geo_relative_pose(const GeoPoseConfig* cfg, const GeoPoseInputs* 
   for (int c = 0; c < a.chunks; ++c) {
     pose_hyp_kernel<<<a.B, GEO_CHUNK, 0, stream>>>(a, c);
     LG_CHECK_LAUNCH();
-    pose_score_kernel<<<dim3(a.B, splits), GEO_CHUNK, 0, stream>>>(a);
+    geo_score_kernel<PoseScore><<<dim3(a.B, splits), GEO_CHUNK, 0, stream>>>(a);
     LG_CHECK_LAUNCH();
   }
   pose_refit_kernel<<<a.B, RED, 0, stream>>>(a);

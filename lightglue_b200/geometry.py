@@ -59,6 +59,21 @@ def _check_inputs(kpts0, kpts1, matches0, name1="kpts1", dim1=2) -> None:
         raise ValueError(f"kpts0, {name1} and matches0 must be on one device")
 
 
+def _run(entry: str, ws_entry: str, shapes: dict, device, b: int, m: int, max_iters: int, make_args) -> dict:
+    """Allocates the outputs of ``shapes`` (key -> (shape, dtype)) and, unless the batch is empty, a workspace of
+    ``ws_entry``'s size, then calls ``entry`` on the ctypes structs ``make_args(out)`` returns."""
+    out = {k: torch.empty(*shape, dtype=dtype, device=device) for k, (shape, dtype) in shapes.items()}
+    if b == 0:
+        return out
+    with torch.cuda.device(device):
+        lib = _cabi.load()
+        ws = torch.empty(getattr(lib, ws_entry)(b, m, max_iters), dtype=torch.uint8, device=device)
+        cfg, ins, outs = make_args(out)
+        _cabi.check(getattr(lib, entry)(C.byref(cfg), C.byref(ins), C.byref(outs), ws.data_ptr(), ws.numel(),
+                                        torch.cuda.current_stream(device).cuda_stream), entry)
+    return out
+
+
 def _estimate(kind: int, key: str, kpts0, kpts1, matches0, threshold, max_iters, confidence, seed,
               lo: bool = False) -> dict:
     _check_inputs(kpts0, kpts1, matches0)
@@ -70,38 +85,24 @@ def _estimate(kind: int, key: str, kpts0, kpts1, matches0, threshold, max_iters,
     k0 = kpts0.detach().to(torch.float32).contiguous()
     k1 = kpts1.detach().to(torch.float32).contiguous()
     m0 = matches0.detach().contiguous()
-    out = {
-        key: torch.empty(b, 3, 3, dtype=torch.float64, device=device),
-        "inliers": torch.empty(b, m, dtype=torch.bool, device=device),
-        "num_inliers": torch.empty(b, dtype=torch.int32, device=device),
-        "success": torch.empty(b, dtype=torch.bool, device=device),
-        "best_hypothesis": torch.empty(b, dtype=torch.int32, device=device),
-        "num_hypotheses": torch.empty(b, dtype=torch.int32, device=device),
-    }
+    f64, i32, bl = torch.float64, torch.int32, torch.bool
+    shapes = {key: ((b, 3, 3), f64), "inliers": ((b, m), bl), "num_inliers": ((b,), i32), "success": ((b,), bl),
+              "best_hypothesis": ((b,), i32), "num_hypotheses": ((b,), i32)}
     if lo:
-        out["num_local_optimizations"] = torch.empty(b, dtype=torch.int32, device=device)
-        out["cost"] = torch.empty(b, dtype=torch.int64, device=device)
-    if b == 0:
-        return out
-    with torch.cuda.device(device):
-        lib = _cabi.load()
+        shapes.update(num_local_optimizations=((b,), i32), cost=((b,), torch.int64))
+
+    def make_args(out):
         cfg = _cabi.GeoConfig(_cabi.GEO_ABI_VERSION, kind, max_iters, seed, float(threshold), float(confidence))
         ins = _cabi.GeoInputs(b, m, n, k0.data_ptr(), k1.data_ptr(), m0.data_ptr())
-        outs = _cabi.GeoOutputs(*(out[k].data_ptr() for k in (key, "inliers", "num_inliers", "success",
-                                                                "best_hypothesis", "num_hypotheses")))
-        stream = torch.cuda.current_stream(device).cuda_stream
+        outs = _cabi.GeoOutputs(*(out[k].data_ptr() for k in list(shapes)[:6]))
         if lo:
-            name = "homography" if kind == _cabi.GEO_HOMOGRAPHY else "fundamental"
-            ws_bytes, entry = getattr(lib, f"geo_lo_{name}_workspace_bytes"), f"geo_{name}_lo"
-            ws = torch.empty(ws_bytes(b, m, max_iters), dtype=torch.uint8, device=device)
-            louts = _cabi.GeoLoOutputs(outs, out["num_local_optimizations"].data_ptr(), out["cost"].data_ptr())
-            _cabi.check(getattr(lib, entry)(C.byref(cfg), C.byref(ins), C.byref(louts), ws.data_ptr(), ws.numel(),
-                                            stream), entry)
-        else:
-            ws = torch.empty(lib.geo_workspace_bytes(b, m, max_iters), dtype=torch.uint8, device=device)
-            _cabi.check(lib.geo_estimate(C.byref(cfg), C.byref(ins), C.byref(outs), ws.data_ptr(), ws.numel(),
-                                         stream), "geo_estimate")
-    return out
+            outs = _cabi.GeoLoOutputs(outs, out["num_local_optimizations"].data_ptr(), out["cost"].data_ptr())
+        return cfg, ins, outs
+
+    if not lo:
+        return _run("geo_estimate", "geo_workspace_bytes", shapes, device, b, m, max_iters, make_args)
+    name = "homography" if kind == _cabi.GEO_HOMOGRAPHY else "fundamental"
+    return _run(f"geo_{name}_lo", f"geo_lo_{name}_workspace_bytes", shapes, device, b, m, max_iters, make_args)
 
 
 def find_homography(kpts0: torch.Tensor, kpts1: torch.Tensor, matches0: torch.Tensor, ransac_reproj_threshold: float = 3.0,
@@ -225,8 +226,6 @@ def _relative_pose(lo: bool, kpts0, kpts1, matches0, K0, K1, ransac_reproj_thres
     p0 = kpts0.detach().to(torch.float32).contiguous()
     p1 = kpts1.detach().to(torch.float32).contiguous()
     m0 = matches0.detach().contiguous()
-    keys = ("E", "R", "t", "inliers", "num_inliers", "pose_inliers", "num_pose_inliers", "success", "best_hypothesis",
-            "best_solution", "num_hypotheses")
     f64, i32, bl = torch.float64, torch.int32, torch.bool
     shapes = {"E": ((b, 3, 3), f64), "R": ((b, 3, 3), f64), "t": ((b, 3), f64), "inliers": ((b, m), bl),
               "num_inliers": ((b,), i32), "pose_inliers": ((b, m), bl), "num_pose_inliers": ((b,), i32),
@@ -234,27 +233,19 @@ def _relative_pose(lo: bool, kpts0, kpts1, matches0, K0, K1, ransac_reproj_thres
               "num_hypotheses": ((b,), i32)}
     if lo:
         shapes.update(num_local_optimizations=((b,), i32), cost=((b,), torch.int64))
-    out = {k: torch.empty(*shape, dtype=dtype, device=device) for k, (shape, dtype) in shapes.items()}
-    if b == 0:
-        return out
-    with torch.cuda.device(device):
-        lib = _cabi.load()
+
+    def make_args(out):
         args = (max_iters, seed, 0, float(ransac_reproj_threshold), float(confidence), float(distance_threshold))
         ins = _cabi.GeoPoseInputs(b, m, n, p0.data_ptr(), p1.data_ptr(), m0.data_ptr(), k0.data_ptr(), k1.data_ptr())
-        outs = _cabi.GeoPoseOutputs(*(out[k].data_ptr() for k in keys))
-        stream = torch.cuda.current_stream(device).cuda_stream
-        if lo:
-            ws = torch.empty(lib.geo_lo_pose_workspace_bytes(b, m, max_iters), dtype=torch.uint8, device=device)
-            cfg = _cabi.GeoLoPoseConfig(_cabi.GEO_ABI_VERSION, *args)
-            louts = _cabi.GeoLoPoseOutputs(outs, out["num_local_optimizations"].data_ptr(), out["cost"].data_ptr())
-            _cabi.check(lib.geo_relative_pose_lo(C.byref(cfg), C.byref(ins), C.byref(louts), ws.data_ptr(), ws.numel(),
-                                                 stream), "geo_relative_pose_lo")
-        else:
-            ws = torch.empty(lib.geo_pose_workspace_bytes(b, m, max_iters), dtype=torch.uint8, device=device)
-            cfg = _cabi.GeoPoseConfig(_cabi.GEO_ABI_VERSION, *args)
-            _cabi.check(lib.geo_relative_pose(C.byref(cfg), C.byref(ins), C.byref(outs), ws.data_ptr(), ws.numel(),
-                                              stream), "geo_relative_pose")
-    return out
+        outs = _cabi.GeoPoseOutputs(*(out[k].data_ptr() for k in list(shapes)[:11]))
+        if not lo:
+            return _cabi.GeoPoseConfig(_cabi.GEO_ABI_VERSION, *args), ins, outs
+        louts = _cabi.GeoLoPoseOutputs(outs, out["num_local_optimizations"].data_ptr(), out["cost"].data_ptr())
+        return _cabi.GeoLoPoseConfig(_cabi.GEO_ABI_VERSION, *args), ins, louts
+
+    if lo:
+        return _run("geo_relative_pose_lo", "geo_lo_pose_workspace_bytes", shapes, device, b, m, max_iters, make_args)
+    return _run("geo_relative_pose", "geo_pose_workspace_bytes", shapes, device, b, m, max_iters, make_args)
 
 
 def estimate_absolute_pose(kpts0: torch.Tensor, points3d1: torch.Tensor, matches0: torch.Tensor, K0: torch.Tensor,
@@ -280,22 +271,15 @@ def estimate_absolute_pose(kpts0: torch.Tensor, points3d1: torch.Tensor, matches
     p0 = kpts0.detach().to(torch.float32).contiguous()
     x1 = points3d1.detach().to(torch.float32).contiguous()
     m0 = matches0.detach().contiguous()
-    keys = ("R", "t", "inliers", "num_inliers", "success", "best_hypothesis", "best_solution", "num_hypotheses")
     f64, i32, bl = torch.float64, torch.int32, torch.bool
     shapes = {"R": ((b, 3, 3), f64), "t": ((b, 3), f64), "inliers": ((b, m), bl), "num_inliers": ((b,), i32),
               "success": ((b,), bl), "best_hypothesis": ((b,), i32), "best_solution": ((b,), i32),
               "num_hypotheses": ((b,), i32)}
-    out = {k: torch.empty(*shapes[k][0], dtype=shapes[k][1], device=device) for k in keys}
-    if b == 0:
-        return out
-    with torch.cuda.device(device):
-        lib = _cabi.load()
-        ws = torch.empty(lib.geo_pnp_workspace_bytes(b, m, max_iters), dtype=torch.uint8, device=device)
+
+    def make_args(out):
         cfg = _cabi.GeoPnpConfig(_cabi.GEO_ABI_VERSION, max_iters, seed, 0, float(ransac_reproj_threshold),
                                  float(confidence))
         ins = _cabi.GeoPnpInputs(b, m, n, p0.data_ptr(), x1.data_ptr(), m0.data_ptr(), k0.data_ptr())
-        outs = _cabi.GeoPnpOutputs(*(out[k].data_ptr() for k in keys))
-        stream = torch.cuda.current_stream(device).cuda_stream
-        _cabi.check(lib.geo_absolute_pose(C.byref(cfg), C.byref(ins), C.byref(outs), ws.data_ptr(), ws.numel(), stream),
-                    "geo_absolute_pose")
-    return out
+        return cfg, ins, _cabi.GeoPnpOutputs(*(out[k].data_ptr() for k in shapes))
+
+    return _run("geo_absolute_pose", "geo_pnp_workspace_bytes", shapes, device, b, m, max_iters, make_args)
