@@ -338,6 +338,43 @@
  *     solution unless it has fewer inliers; inliers and num_inliers are the final pose's.
  * A8. A pair fails (success 0, R and t zero, no inliers, best_hypothesis = best_solution = -1, num_hypotheses the
  *     samples drawn) when n < 3, K0 is invalid, or every sample is degenerate.
+ *
+ * LO-RANSAC absolute pose (geo_absolute_pose_lo; oracle/lo_pnp_oracle.py restates it bit for bit): the outputs of
+ * geo_absolute_pose, from an MSAC-scored P3P RANSAC with Levenberg-Marquardt local optimisation of (R, t), on the
+ * schedule of L1-L8.  Expressions evaluate left to right as written; every multiply and add rounds on its own.
+ *
+ * LA1. Compaction, calibration, the K0 check and thr2 = (float)(threshold * threshold) exactly as A1-A2.
+ *      M <= GEO_LO_MAX_MATCHES.
+ * LA2. Sampling and the Lambda Twist solutions exactly as A3-A4: with the same seed both estimators draw the same
+ *      samples and solve the same solutions.
+ * LA3. MSAC score, per solution of every sample, from A5's fp32 test (P = K0 [R | t] rounded to float): err =
+ *      du * du + dv * dv when w > 0, else the point is an outlier; q as L3 (0 at err == 0, else
+ *      (uint32)fminf(err * w', GEO_LO_QSCALE) with w' = GEO_LO_QSCALE / thr2 for err < thr2, else GEO_LO_QSCALE), so a
+ *      point behind the camera or with a non-finite err scores GEO_LO_QSCALE.  score = sum of q over the points in
+ *      uint64, count = the number of inliers (A5's test).  Lower is better; ties go to the lowest (sample h,
+ *      solution r).
+ * LA4. Local optimisation, after every chunk of GEO_CHUNK samples, once per pair.  Chunk c's best solution (lowest
+ *      (score, h, r)) is taken when the pair has no model yet or its score is strictly below the model's score; else
+ *      nothing happens.  Taken, sample h is drawn and solved again as LA2, and the (R, t) of its solution r in double
+ *      becomes the pair's model (score, count, h, r).  Then GEO_LO_STEPS LM steps (LA7) from it give (R', t'), which
+ *      are scored as LA3 through P = K0 [R' | t'] rounded to float; with a strictly lower score they replace the model
+ *      (keeping h and r) and num_local_optimizations counts one.
+ * LA5. Stopping as A6 (s = 3) from the model's count (a local optimisation's count included).
+ * LA6. Final refinement: GEO_LO_FINAL_STEPS LM steps from the model's (R, t), kept unless their LA3 score is higher.
+ * LA7. LM, in double on the compacted pixels and world points read as floats widened: A7's parametrisation
+ *      (R' = Q R, t'_i = Q_i0 * t0 + Q_i1 * t1 + Q_i2 * t2 + delta_(3+i)), residuals (ru, rv), err = ru * ru + rv * rv
+ *      and Jacobian rows ju, jv at each pose.  A point is an inlier at this pose when Xc2 > 0 and err < (double)thr2.
+ *      The 21 terms ju_i * ju_j + jv_i * jv_j (i <= j in row order) and the 6 terms ju_i * ru + jv_i * rv over the
+ *      inliers, and the truncated cost (err for an inlier, else (double)thr2) over every point, are each summed in the
+ *      order of step 2.  A step solves the 6x6 system of A7 (damping, Cholesky, right-hand side -J^T r), lambda starts
+ *      at GEO_LO_LAMBDA0, and the step is taken only if the truncated cost at (R', t'), with its own inliers, is
+ *      strictly lower: A7's schedule.
+ * LA8. Outputs: R and t the final pose; inliers the rows that pass A5's test under its P = K0 [R | t] rounded to float,
+ *      num_inliers their number and cost its LA3 score; best_hypothesis and best_solution the solution that seeded
+ *      the final model; num_hypotheses the samples drawn.  A pair fails as A8, with num_local_optimizations and cost
+ *      0.  Deviations from PoseLib and COLMAP: local optimisation runs at most once per chunk rather than at every new
+ *      best, so the launch sequence is fixed and the result is deterministic; the score is quantised to integers;
+ *      there is no non-minimal (EPnP) refit inside the LO and no PROSAC ordering.
  */
 #ifndef GEOMETRY_B200_H
 #define GEOMETRY_B200_H
@@ -519,6 +556,17 @@ typedef struct GeoPnpOutputs {
 LG_API size_t geo_pnp_workspace_bytes(int32_t B, int32_t M, int32_t max_iters);
 LG_API int geo_absolute_pose(const GeoPnpConfig* cfg, const GeoPnpInputs* in, GeoPnpOutputs* out, void* workspace,
                              size_t workspace_bytes, void* stream);
+
+typedef struct GeoLoPnpOutputs {
+  GeoPnpOutputs pnp;                 /* as geo_absolute_pose's */
+  int32_t* num_local_optimizations;  /* [B] local optimisations whose model was adopted */
+  int64_t* cost;                     /* [B] LA3 score of the final model */
+} GeoLoPnpOutputs;
+
+/* LO-RANSAC absolute pose (steps LA1-LA8): in->M <= GEO_LO_MAX_MATCHES. */
+LG_API size_t geo_lo_pnp_workspace_bytes(int32_t B, int32_t M, int32_t max_iters);
+LG_API int geo_absolute_pose_lo(const GeoPnpConfig* cfg, const GeoPnpInputs* in, GeoLoPnpOutputs* out,
+                                void* workspace, size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }

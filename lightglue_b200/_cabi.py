@@ -169,6 +169,10 @@ class GeoPnpOutputs(C.Structure):
     ]
 
 
+class GeoLoPnpOutputs(C.Structure):
+    _fields_ = [("pnp", GeoPnpOutputs), ("num_local_optimizations", C.c_void_p), ("cost", C.c_void_p)]
+
+
 class NnConfig(C.Structure):
     _fields_ = [
         ("abi_version", C.c_int32), ("dim", C.c_int32), ("mutual_check", C.c_int32), ("ratio_thresh", C.c_float),
@@ -274,6 +278,9 @@ GEO_PROTOTYPES = {  # include/geometry_b200.h
     "geo_pnp_workspace_bytes": (_SZ, [_I32, _I32, _I32]),
     "geo_absolute_pose": (C.c_int, [C.POINTER(GeoPnpConfig), C.POINTER(GeoPnpInputs), C.POINTER(GeoPnpOutputs), _VP,
                                     _SZ, _VP]),
+    "geo_lo_pnp_workspace_bytes": (_SZ, [_I32, _I32, _I32]),
+    "geo_absolute_pose_lo": (C.c_int, [C.POINTER(GeoPnpConfig), C.POINTER(GeoPnpInputs), C.POINTER(GeoLoPnpOutputs),
+                                       _VP, _SZ, _VP]),
 }
 NN_PROTOTYPES = {  # include/nn_b200.h
     "nn_create": (C.c_int, [_VP, _HANDLE_OUT]),

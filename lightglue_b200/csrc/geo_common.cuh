@@ -1,5 +1,5 @@
-// Helpers shared by every geometry estimator (geo_api.cu, pose_api.cu, lo_pose_api.cu, lo_hf_api.cu, pnp_api.cu), all
-// compiled with -fmad=false.  include/geometry_b200.h states each step; oracle/geometry_oracle.py and
+// Helpers shared by every geometry estimator (geo_api.cu, pose_api.cu, lo_pose_api.cu, lo_hf_api.cu, pnp_api.cu,
+// lo_pnp_api.cu), all compiled with -fmad=false.  include/geometry_b200.h states each step; oracle/geometry_oracle.py and
 // oracle/pose_oracle.py restate them in numpy.
 #pragma once
 #include <cuda_runtime.h>

@@ -1,6 +1,7 @@
 // The LO-RANSAC pieces shared by the relative pose (lo_pose_api.cu, header steps L3 and L7), the homography and the
-// fundamental matrix (lo_hf_api.cu, LH3 and LH7, LF3 and LF7), all compiled with -fmad=false: the packed MSAC score
-// term, the fixed-order sums of the Levenberg-Marquardt terms, and one LM loop and re-score over a model policy.
+// fundamental matrix (lo_hf_api.cu, LH3 and LH7, LF3 and LF7) and the absolute pose (lo_pnp_api.cu, LA3 and LA7), all
+// compiled with -fmad=false: the packed MSAC score term, the fixed-order sums of the Levenberg-Marquardt terms, and one
+// LM loop and re-score over a model policy.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -38,28 +39,30 @@ __device__ void lo_tree_sums(const double* acc, double (*red)[RED], double* out,
 
 // Shared state of one pair's CTA in an LO or final kernel.  Model is the policy of one estimator:
 //   DOF, TERMS (J^T J upper triangle, J^T r, truncated cost: DOF (DOF + 1) / 2 + DOF + 1), GROUP (the terms per pass of
-//   lo_tree_sums, which keeps red within static shared memory) and NP (the length of the parameter vector x);
+//   lo_tree_sums, which keeps red within static shared memory), NP (the length of the parameter vector x) and NF (the
+//   length of the pixel model that is scored);
 //   Scratch, the model's own shared state;
 //   terms(s, P, x, pts, n, thr2, out, tid), the TERMS sums at x (every thread);
 //   update(s, x, d, out), x moved by the LM step d (thread 0);
 //   pixels(s, P, x, out), x as the scaled pixel model that is rounded to float and scored (thread 0);
-//   err(h, p), the fp32 error of a point against a float model.
+//   err(h, pts[k]), the fp32 error of point k against a float model.
+// P, the pair's constants, and pts, its points (a pointer, or any type whose pts[k] is one point), pass through the
+// LM loop and the re-score to the model unread.
 template <class Model>
 struct LoShared {
   double red[Model::GROUP][RED];
   double x[Model::NP], cand[Model::NP];  // the model being refined and the LM step's candidate
   double sums[Model::TERMS], csum[Model::TERMS];
   typename Model::Scratch m;
-  double px[9];                          // the scaled pixel model of the last re-scored x
-  float fm[9];                           // a model rounded to float
+  double px[Model::NF];                  // the scaled pixel model of the last re-scored x
+  float fm[Model::NF];                   // a model rounded to float
   unsigned long long key, score;
   int take, step_ok;
 };
 
-// steps LM steps from s.x, in place (header steps L7, LH7, LF7); every thread of the CTA calls it
-template <class Model, class Pair>
-__device__ void lo_refine(LoShared<Model>& s, const Pair& P, const float4* pts, int n, double thr2, int steps,
-                          int tid) {
+// steps LM steps from s.x, in place (header steps L7, LH7, LF7, LA7); every thread of the CTA calls it
+template <class Model, class Pair, class Points>
+__device__ void lo_refine(LoShared<Model>& s, const Pair& P, Points pts, int n, double thr2, int steps, int tid) {
   constexpr int NH = Model::DOF * (Model::DOF + 1) / 2;
   Model::terms(s, P, s.x, pts, n, thr2, s.sums, tid);
   double lam = GEO_LO_LAMBDA0;  // every thread keeps the same schedule
@@ -89,12 +92,12 @@ __device__ void lo_refine(LoShared<Model>& s, const Pair& P, const float4* pts, 
   }
 }
 
-// L3 / LH3 / LF3 score and count of s.x in pixels (s.px), rounded to float (s.fm)
-template <class Model, class Pair>
-__device__ void lo_rescore(LoShared<Model>& s, const Pair& P, const float4* pts, int n, float thr2, int tid) {
+// L3 / LH3 / LF3 / LA3 score and count of s.x in pixels (s.px), rounded to float (s.fm)
+template <class Model, class Pair, class Points>
+__device__ void lo_rescore(LoShared<Model>& s, const Pair& P, Points pts, int n, float thr2, int tid) {
   if (tid == 0) {
     Model::pixels(s, P, s.x, s.px);
-    for (int i = 0; i < 9; ++i) s.fm[i] = (float)s.px[i];
+    for (int i = 0; i < Model::NF; ++i) s.fm[i] = (float)s.px[i];
     s.score = 0;
   }
   __syncthreads();

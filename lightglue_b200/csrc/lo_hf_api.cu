@@ -125,7 +125,7 @@ __device__ void householder_basis(const double* Hn, double (*B)[9]) {
 
 // The homography for lo_common.cuh's LM loop and re-score: x = Hn, the unit-norm normalised model (header step LH7)
 struct HomographyLo {
-  static constexpr int KIND = GEO_HOMOGRAPHY, DOF = 8, TERMS = 45, GROUP = 15, NP = 9;
+  static constexpr int KIND = GEO_HOMOGRAPHY, DOF = 8, TERMS = 45, GROUP = 15, NP = 9, NF = 9;
   struct Scratch {
     double basis[DOF][9];     // tangent basis at the model being summed or updated
     double Hu[9], G[DOF][9];  // T1^-1 Hn T0 and its derivatives along the basis
@@ -225,7 +225,7 @@ __device__ void compose(const double* x, double* Fn) {
 // The fundamental matrix for lo_common.cuh's LM loop and re-score: x = U (0-8), V (9-17) and sig (18), the orthonormal
 // representation Fn = u1 v1^T + sig u2 v2^T of the normalised model, u_k, v_k columns of U, V (header step LF7)
 struct FundamentalLo {
-  static constexpr int KIND = GEO_FUNDAMENTAL, DOF = 7, TERMS = 36, GROUP = 18, NP = 19;
+  static constexpr int KIND = GEO_FUNDAMENTAL, DOF = 7, TERMS = 36, GROUP = 18, NP = 19, NF = 9;
   struct Scratch {
     double Fu[9], G[DOF][9];  // T1^T Fn T0 and the directions at Fn in pixels
   };

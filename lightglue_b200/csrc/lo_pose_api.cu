@@ -108,7 +108,7 @@ __device__ __forceinline__ void lo_epipolar(const double* E, double x, double y,
 
 // The relative pose for lo_common.cuh's LM loop and re-score: x = R, t (header step L7)
 struct PoseLo {
-  static constexpr int DOF = 5, TERMS = 21, GROUP = 21, NP = 12;
+  static constexpr int DOF = 5, TERMS = 21, GROUP = 21, NP = 12, NF = 9;
   struct Scratch {
     double E[9], dE[5][9];   // [t]x R and its derivatives at the pose being summed
     double Rs[2][9], ts[3];  // P7 candidates

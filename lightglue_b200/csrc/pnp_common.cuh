@@ -1,0 +1,323 @@
+// The absolute-pose pieces shared by the plain (pnp_api.cu, header steps A1-A8) and the LO-RANSAC estimator
+// (lo_pnp_api.cu, LA1-LA8), both compiled with -fmad=false: the workspace, the compaction kernel, the Lambda Twist
+// solver, the projection, the fp32 reprojection test and the pose update of the Levenberg-Marquardt steps.
+#pragma once
+#include <stdint.h>
+
+#include "block_scan.cuh"
+#include "geo_common.cuh"
+#include "geo_lm.cuh"
+#include "lg_internal.h"
+#include "ws_bump.h"
+
+namespace {
+
+constexpr int S = 3;                   // points per sample
+constexpr int SOLS = GEO_PNP_MAX_SOLUTIONS;
+constexpr int TILE = 512;              // points per shared-memory tile of the score kernel
+
+struct PnpPair {
+  float P[12];               // the final K0 [R | t], fp32 (refit -> mask)
+  unsigned long long best;   // (count + 1) << 32 | ~(h * 16 + r) of the best solution so far; 0: none
+  float thr2;                // threshold^2
+  int n;                     // valid matches
+  int ok;                    // n >= 3 and K0 valid
+  int stop;                  // no further samples are drawn
+  int drawn;                 // samples drawn so far
+  int success;               // set by the refit kernel
+};
+
+struct PnpWs {
+  PnpPair* pair;   // [B]
+  float4* pts;     // [B, M] compacted (u, v, x, y): pixel and calibrated coordinates
+  float4* wld;     // [B, M] compacted world point (X, Y, Z, 0)
+  int* slot;       // [B, M] compacted slot of each row of matches0, -1 for an invalid match
+  float* hyp;      // [B, GEO_CHUNK, SOLS, 12] the current chunk's projections, fp32
+  int* nsol;       // [B, GEO_CHUNK] their number; 0: degenerate or not drawn
+  int* count;      // [B, GEO_CHUNK, SOLS] their inlier counts
+  uint8_t* inl;    // [B, M] the best solution's inliers, per compacted point (refit)
+};
+
+size_t carve(char* base, int B, int M, PnpWs* w) {
+  WsBump b{base, 0};
+  w->pair = b.take<PnpPair>(B);
+  w->pts = b.take<float4>((size_t)B * M);
+  w->wld = b.take<float4>((size_t)B * M);
+  w->slot = b.take<int>((size_t)B * M);
+  w->hyp = b.take<float>((size_t)B * GEO_CHUNK * SOLS * 12);
+  w->nsol = b.take<int>((size_t)B * GEO_CHUNK);
+  w->count = b.take<int>((size_t)B * GEO_CHUNK * SOLS);
+  w->inl = b.take<uint8_t>((size_t)B * M);
+  return b.bytes();
+}
+
+struct PnpArgs {
+  int B, M, N, max_iters, chunks;
+  unsigned seed;
+  double threshold, confidence;
+  const float* kpts0;
+  const float* points3d1;
+  const int64_t* matches0;
+  const double* K0;
+  PnpWs w;
+  GeoPnpOutputs out;
+};
+
+__device__ __forceinline__ double dot3(const double* a, const double* b) { return a[0] * b[0] + a[1] * b[1] + a[2] * b[2]; }
+
+__device__ __forceinline__ void cross3(const double* a, const double* b, double* c) {
+  c[0] = a[1] * b[2] - a[2] * b[1];
+  c[1] = a[2] * b[0] - a[0] * b[2];
+  c[2] = a[0] * b[1] - a[1] * b[0];
+}
+
+// Both roots of z^2 + b z + c, the larger-magnitude one first; a negative discriminant counts as 0 (header step A4)
+__device__ __forceinline__ void root2(double b, double c, double* r1, double* r2) {
+  const double y = sqrt(fmax(b * b - 4.0 * c, 0.0));
+  const double q = -0.5 * (b + (b >= 0.0 ? y : -y));
+  *r1 = q;
+  *r2 = c / q;
+}
+
+__device__ __forceinline__ double cubic(double g, double cb, double cc, double cd) { return ((g + cb) * g + cc) * g + cd; }
+
+// Lambda Twist P3P on the calibrated (x, y) in pts[id[k]].z/w and the world points wlds[id[k]] (header step A4).
+// Writes the kept solutions' R (row-major) and t in the solver's order; returns their number.
+__device__ __noinline__ int p3p(const float4* pts, const float4* wlds, const int* id, double (*Rs)[9], double (*ts)[3]) {
+  double y[3][3], X[3][3];
+  for (int k = 0; k < 3; ++k) {
+    const float4 p = pts[id[k]], q = wlds[id[k]];
+    const double xx = p.z, yy = p.w;
+    const double n = sqrt(xx * xx + yy * yy + 1.0);
+    y[k][0] = xx / n;
+    y[k][1] = yy / n;
+    y[k][2] = 1.0 / n;
+    X[k][0] = q.x;
+    X[k][1] = q.y;
+    X[k][2] = q.z;
+  }
+  const double b12 = -2.0 * dot3(y[0], y[1]), b13 = -2.0 * dot3(y[0], y[2]), b23 = -2.0 * dot3(y[1], y[2]);
+  double d12[3], d13[3], d23[3], nrm[3];
+  for (int i = 0; i < 3; ++i) {
+    d12[i] = X[0][i] - X[1][i];
+    d13[i] = X[0][i] - X[2][i];
+    d23[i] = X[1][i] - X[2][i];
+  }
+  const double a12 = dot3(d12, d12), a13 = dot3(d13, d13), a23 = dot3(d23, d23);
+  cross3(d12, d13, nrm);
+  if (!(dot3(nrm, nrm) > GEO_PNP_COLLINEAR_EPS * (a12 * a13))) return 0;
+  const double c31 = -0.5 * b13, c23 = -0.5 * b23, c12 = -0.5 * b12;
+  const double blob = c12 * c23 * c31 - 1.0;
+  const double s31 = 1.0 - c31 * c31, s23 = 1.0 - c23 * c23, s12 = 1.0 - c12 * c12;
+  const double p3 = a13 * (a23 * s31 - a13 * s23);
+  const double p2 = 2.0 * blob * a23 * a13 + a13 * (2.0 * a12 + a13) * s23 + a23 * (a23 - a12) * s31;
+  const double p1 = a23 * (a13 - a23) * s12 - a12 * a12 * s23 - 2.0 * a12 * (blob * a23 + a13 * s23);
+  const double p0 = a12 * (a12 * s23 - a23 * s12);
+  const double cb = p2 / p3, cc = p1 / p3, cd = p0 / p3;
+  if (!(isfinite(cb) && isfinite(cc) && isfinite(cd))) return 0;
+  // one real root of the monic cubic: bisection on a bracket holding exactly one root, then Newton
+  const double rb = 1.0 + fmax(fmax(fabs(cb), fabs(cc)), fabs(cd));
+  double lo = -rb, hi = rb;
+  const double disc = cb * cb - 3.0 * cc;
+  if (disc >= 0.0) {
+    const double v = sqrt(fmax(disc, 0.0));
+    const double t1 = (-cb - v) / 3.0;
+    if (cubic(t1, cb, cc, cd) > 0.0) hi = t1; else lo = (-cb + v) / 3.0;
+  }
+  for (int s = 0; s < GEO_PNP_BISECT_STEPS; ++s) {
+    const double mid = 0.5 * (lo + hi);
+    if (cubic(mid, cb, cc, cd) > 0.0) hi = mid; else lo = mid;
+  }
+  double g = 0.5 * (lo + hi);
+  for (int s = 0; s < GEO_PNP_NEWTON_STEPS; ++s) {
+    const double gn = g - cubic(g, cb, cc, cd) / ((3.0 * g + 2.0 * cb) * g + cc);
+    if (isfinite(gn)) g = gn;
+  }
+  // the degenerate conic A = D1 + g D2 and its two eigenvectors of nonzero eigenvalue
+  const double A00 = a23 * (1.0 - g);
+  const double A01 = a23 * b12 * 0.5;
+  const double A02 = a23 * b13 * g * -0.5;
+  const double A11 = a23 - a12 + a13 * g;
+  const double A12 = b23 * (a13 * g - a12) * 0.5;
+  const double A22 = g * (a13 - a23) - a12;
+  double e1, e2;
+  root2(-A00 - A11 - A22, -(A01 * A01) - A02 * A02 - A12 * A12 + A00 * (A11 + A22) + A11 * A22, &e1, &e2);
+  if (fabs(e1) < fabs(e2)) { const double tmp = e1; e1 = e2; e2 = tmp; }
+  const double mx = -(A00 * A11);
+  const double pr0 = A01 * A12 - A02 * A11;
+  const double pr1 = A01 * A02 - A00 * A12;
+  double V[2][3];
+  for (int k = 0; k < 2; ++k) {
+    const double e = k == 0 ? e1 : e2;
+    const double tmp = 1.0 / (e * (A00 + A11) + mx - e * e + A01 * A01);
+    const double a1 = -(e * A02 + pr0) * tmp;
+    const double a2 = -(e * A12 + pr1) * tmp;
+    const double rn = 1.0 / sqrt(a1 * a1 + a2 * a2 + 1.0);
+    V[k][0] = a1 * rn;
+    V[k][1] = a2 * rn;
+    V[k][2] = rn;
+  }
+  const double sv = sqrt(fmax(0.0, -e2 / e1));
+  // the inverse of X = [d12 d13 d12 x d13] by cofactors
+  const double x[3][3] = {{d12[0], d13[0], nrm[0]}, {d12[1], d13[1], nrm[1]}, {d12[2], d13[2], nrm[2]}};
+  const double C[3][3] = {
+      {x[1][1] * x[2][2] - x[1][2] * x[2][1], x[1][2] * x[2][0] - x[1][0] * x[2][2], x[1][0] * x[2][1] - x[1][1] * x[2][0]},
+      {x[0][2] * x[2][1] - x[0][1] * x[2][2], x[0][0] * x[2][2] - x[0][2] * x[2][0], x[0][1] * x[2][0] - x[0][0] * x[2][1]},
+      {x[0][1] * x[1][2] - x[0][2] * x[1][1], x[0][2] * x[1][0] - x[0][0] * x[1][2], x[0][0] * x[1][1] - x[0][1] * x[1][0]}};
+  const double det = x[0][0] * C[0][0] + x[0][1] * C[0][1] + x[0][2] * C[0][2];
+  double Xi[3][3];
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 3; ++j) Xi[i][j] = C[j][i] / det;
+  int ns = 0;
+  for (int sg = 0; sg < 2; ++sg) {
+    const double s = sg == 0 ? sv : -sv;
+    const double w2 = 1.0 / (s * V[1][0] - V[0][0]);
+    const double w0 = (V[0][1] - s * V[1][1]) * w2;
+    const double w1 = (V[0][2] - s * V[1][2]) * w2;
+    const double ia = 1.0 / ((a13 - a12) * w1 * w1 - a12 * b13 * w1 - a12);
+    const double qb = (a13 * b12 * w1 - a12 * b13 * w0 - 2.0 * w0 * w1 * (a12 - a13)) * ia;
+    const double qc = ((a13 - a12) * w0 * w0 + a13 * b12 * w0 + a13) * ia;
+    if (!(qb * qb - 4.0 * qc >= 0.0)) continue;
+    double taus[2];
+    root2(qb, qc, &taus[0], &taus[1]);
+    for (int k = 0; k < 2; ++k) {
+      const double tau = taus[k];
+      if (!(tau > 0.0)) continue;
+      const double d = a23 / (tau * (b23 + tau) + 1.0);
+      if (!(d > 0.0)) continue;
+      double l2 = sqrt(d);
+      double l3 = tau * l2;
+      double l1 = w0 * l2 + w1 * l3;
+      if (!(l1 >= 0.0)) continue;
+      for (int it = 0; it < GEO_PNP_GN_STEPS; ++it) {
+        const double r1 = l1 * l1 + l2 * l2 + b12 * l1 * l2 - a12;
+        const double r2 = l1 * l1 + l3 * l3 + b13 * l1 * l3 - a13;
+        const double r3 = l2 * l2 + l3 * l3 + b23 * l2 * l3 - a23;
+        const double v0 = 2.0 * l1 + b12 * l2, v1 = 2.0 * l2 + b12 * l1;
+        const double v3 = 2.0 * l1 + b13 * l3, v5 = 2.0 * l3 + b13 * l1;
+        const double v7 = 2.0 * l2 + b23 * l3, v8 = 2.0 * l3 + b23 * l2;
+        const double dt = -(v0 * v5 * v7) - v1 * v3 * v8;
+        const double j0 = -(v5 * v7) * r1 - v1 * v8 * r2 + v1 * v5 * r3;
+        const double j1 = -(v3 * v8) * r1 + v0 * v8 * r2 - v0 * v5 * r3;
+        const double j2 = v3 * v7 * r1 - v0 * v7 * r2 - v1 * v3 * r3;
+        const double n1 = l1 - j0 / dt, n2 = l2 - j1 / dt, n3 = l3 - j2 / dt;
+        if (isfinite(n1) && isfinite(n2) && isfinite(n3)) { l1 = n1; l2 = n2; l3 = n3; }
+      }
+      const double lam[3] = {l1, l2, l3};
+      double ry[3][3];
+      for (int q = 0; q < 3; ++q)
+        for (int i = 0; i < 3; ++i) ry[q][i] = y[q][i] * lam[q];
+      double yd1[3], yd2[3], yc[3];
+      for (int i = 0; i < 3; ++i) {
+        yd1[i] = ry[0][i] - ry[1][i];
+        yd2[i] = ry[0][i] - ry[2][i];
+      }
+      cross3(yd1, yd2, yc);
+      double* R = Rs[ns];
+      double* t = ts[ns];
+      bool fin = true;
+      for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) {
+          R[i * 3 + j] = yd1[i] * Xi[0][j] + yd2[i] * Xi[1][j] + yc[i] * Xi[2][j];
+          fin = fin && isfinite(R[i * 3 + j]);
+        }
+      for (int i = 0; i < 3; ++i) {
+        t[i] = ry[0][i] - (R[i * 3] * X[0][0] + R[i * 3 + 1] * X[0][1] + R[i * 3 + 2] * X[0][2]);
+        fin = fin && isfinite(t[i]);
+      }
+      if (fin) ++ns;
+    }
+  }
+  return ns;
+}
+
+// P = K [R | t] (header step A5), P_ij = (K_i0*M_0j + K_i1*M_1j) + K_i2*M_2j
+__device__ __forceinline__ void projection(const double* K, const double* R, const double* t, double* P) {
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 4; ++j) {
+      const double m0 = j < 3 ? R[j] : t[0], m1 = j < 3 ? R[3 + j] : t[1], m2 = j < 3 ? R[6 + j] : t[2];
+      P[i * 4 + j] = K[3 * i] * m0 + K[3 * i + 1] * m1 + K[3 * i + 2] * m2;
+    }
+}
+
+// fp32 inlier test of one point (header step A5): depth w > 0 and squared reprojection error below thr2
+__device__ __forceinline__ bool reproj_inlier(const float* g, float4 p, float4 q, float thr2) {
+  const float w = g[8] * q.x + g[9] * q.y + g[10] * q.z + g[11];
+  const float iw = 1.f / w;
+  const float du = p.x - (g[0] * q.x + g[1] * q.y + g[2] * q.z + g[3]) * iw;
+  const float dv = p.y - (g[4] * q.x + g[5] * q.y + g[6] * q.z + g[7]) * iw;
+  return w > 0.f && du * du + dv * dv < thr2;
+}
+
+// The same point's fp32 error for the MSAC score (header step LA3): du * du + dv * dv in front of the camera, +inf
+// behind it, so that lo_term counts it as an outlier.  e < thr2 exactly when reproj_inlier holds.
+__device__ __forceinline__ float reproj_err(const float* g, float4 p, float4 q) {
+  const float w = g[8] * q.x + g[9] * q.y + g[10] * q.z + g[11];
+  const float iw = 1.f / w;
+  const float du = p.x - (g[0] * q.x + g[1] * q.y + g[2] * q.z + g[3]) * iw;
+  const float dv = p.y - (g[4] * q.x + g[5] * q.y + g[6] * q.z + g[7]) * iw;
+  return w > 0.f ? du * du + dv * dv : INFINITY;
+}
+
+__device__ bool k_valid(const double* K) {
+  bool finite = true;
+  for (int i = 0; i < 9; ++i) finite = finite && isfinite(K[i]);
+  return finite && K[0] > 0.0 && K[4] > 0.0 && K[6] == 0.0 && K[7] == 0.0 && K[8] == 1.0;
+}
+
+__global__ void __launch_bounds__(1024) pnp_prepare_kernel(PnpArgs a) {
+  const int b = blockIdx.x, tid = threadIdx.x;
+  __shared__ int warp_sums[32];
+  __shared__ int carry;
+  if (tid == 0) carry = 0;
+  __syncthreads();
+  const double* K = a.K0 + (long)b * 9;
+  const int64_t* m0 = a.matches0 + (long)b * a.M;
+  float4* pts = a.w.pts + (long)b * a.M;
+  float4* wld = a.w.wld + (long)b * a.M;
+  int* slot = a.w.slot + (long)b * a.M;
+  for (int base = 0; base < a.M; base += 1024) {
+    const int i = base + tid;
+    const int64_t j = i < a.M ? m0[i] : -1;
+    float X = 0.f, Y = 0.f, Z = 0.f;
+    float2 p = make_float2(0.f, 0.f);
+    if (j >= 0 && j < a.N) {
+      const float* q = a.points3d1 + ((long)b * a.N + j) * 3;
+      X = q[0];
+      Y = q[1];
+      Z = q[2];
+      p = reinterpret_cast<const float2*>(a.kpts0)[(long)b * a.M + i];
+    }
+    const bool valid = j >= 0 && j < a.N && isfinite(X) && isfinite(Y) && isfinite(Z) && finite2(p);
+    const int k = block_scan_step(valid, tid, warp_sums, &carry);
+    if (i < a.M) slot[i] = valid ? k : -1;
+    if (valid) {
+      const double yy = ((double)p.y - K[5]) / K[4], xx = (((double)p.x - K[2]) - K[1] * yy) / K[0];
+      pts[k] = make_float4(p.x, p.y, (float)xx, (float)yy);
+      wld[k] = make_float4(X, Y, Z, 0.f);
+    }
+  }
+  __syncthreads();
+  if (tid == 0) {
+    PnpPair& P = a.w.pair[b];
+    P.thr2 = (float)(a.threshold * a.threshold);
+    P.best = 0;
+    P.n = carry;
+    P.ok = carry >= S && k_valid(K);
+    P.stop = !P.ok;
+    P.drawn = 0;
+    P.success = 0;
+  }
+}
+
+// R' = Q R, t' = Q t + d[3..5], Q of the unit quaternion (1, d[0..2] / 2) / norm
+__device__ void lm_update(const double* R, const double* t, const double* d, double* Rn, double* tn) {
+  double Q[9];
+  quat_rotation(d, Q);
+  for (int i = 0; i < 3; ++i) {
+    for (int j = 0; j < 3; ++j) Rn[3 * i + j] = Q[3 * i] * R[j] + Q[3 * i + 1] * R[3 + j] + Q[3 * i + 2] * R[6 + j];
+    tn[i] = Q[3 * i] * t[0] + Q[3 * i + 1] * t[1] + Q[3 * i + 2] * t[2] + d[3 + i];
+  }
+}
+
+}  // namespace

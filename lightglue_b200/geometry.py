@@ -1,9 +1,9 @@
-"""Geometric verification on the GPU: batched RANSAC homography and fundamental-matrix (each plain and
-LO-RANSAC), relative-pose (plain and LO-RANSAC) and absolute-pose estimation on the matcher's output (C ABI
-``include/geometry_b200.h``, CUDA ``csrc/geo_api.cu``, ``csrc/lo_hf_api.cu``, ``csrc/pose_api.cu``,
-``csrc/lo_pose_api.cu`` and ``csrc/pnp_api.cu``).
+"""Geometric verification on the GPU: batched RANSAC homography and fundamental-matrix, relative-pose and
+absolute-pose estimation on the matcher's output, each plain and LO-RANSAC (C ABI ``include/geometry_b200.h``, CUDA
+``csrc/geo_api.cu``, ``csrc/lo_hf_api.cu``, ``csrc/pose_api.cu``, ``csrc/lo_pose_api.cu``, ``csrc/pnp_api.cu`` and
+``csrc/lo_pnp_api.cu``).
 
-All seven functions take ``matches0`` [B, M] int64 exactly as ``LightGlue.forward``, ``PendingMatch.tensors`` and
+All eight functions take ``matches0`` [B, M] int64 exactly as ``LightGlue.forward``, ``PendingMatch.tensors`` and
 ``match_ragged`` give it (-1 or any index outside [0, N) is unmatched), run every pair of the batch in one call on the
 current stream, and return device tensors of fixed shapes without synchronising with the host, so a call can follow a
 matcher forward with no read-back in between, or be captured in a CUDA graph.  A match whose keypoint in either image,
@@ -17,7 +17,8 @@ entry positive), ``inliers`` [B, M] bool, ``num_inliers`` [B] int32, ``success``
 ``best_hypothesis`` [B] int32 (-1 without one) and ``num_hypotheses`` [B] int32.  A failed pair (fewer valid matches than
 the sample size, 4 or 8, or no non-degenerate hypothesis) has ``success`` False, a zero model and no inliers.
 ``find_homography_lo`` and ``find_fundamental_lo`` return the keys of ``find_homography`` and ``find_fundamental`` plus
-``num_local_optimizations`` and ``cost``.
+``num_local_optimizations`` and ``cost``; so do ``estimate_relative_pose_lo`` and ``estimate_absolute_pose_lo`` with
+those of ``estimate_relative_pose`` and ``estimate_absolute_pose``.
 """
 from __future__ import annotations
 
@@ -263,8 +264,34 @@ def estimate_absolute_pose(kpts0: torch.Tensor, points3d1: torch.Tensor, matches
     valid matches, an invalid K0 (a non-finite entry, fx or fy <= 0, or a bottom row other than [0, 0, 1]) or no
     non-degenerate sample has ``success`` False, zero R and t, no inliers and -1 for ``best_hypothesis`` and
     ``best_solution``."""
+    return _absolute_pose(False, kpts0, points3d1, matches0, K0, ransac_reproj_threshold, max_iters, confidence, seed)
+
+
+def estimate_absolute_pose_lo(kpts0: torch.Tensor, points3d1: torch.Tensor, matches0: torch.Tensor, K0: torch.Tensor,
+                              ransac_reproj_threshold: float = 8.0, max_iters: int = 100, confidence: float = 0.99,
+                              seed: int = 0) -> dict:
+    """LO-RANSAC absolute pose per pair: the samples and P3P solutions of ``estimate_absolute_pose``, scored by a
+    truncated (MSAC) squared reprojection error, with Levenberg-Marquardt local optimisation of (R, t) after each chunk
+    of 256 samples that improves the best model, and a final Levenberg-Marquardt refinement.  The accuracy of PoseLib's
+    and OpenCV's USAC LO-RANSAC, on the GPU: a rotation-error tail close to USAC's where ``estimate_absolute_pose``'s
+    one refit from one sample leaves outliers in the tail; ``estimate_absolute_pose`` stays the one that follows
+    ``cv2.solvePnPRansac``.  Arguments and defaults are ``estimate_absolute_pose``'s, so the two compare like for like;
+    at most 2**20 - 1 rows of ``matches0`` per pair.
+
+    Returns the keys of ``estimate_absolute_pose`` (R and t the final pose; ``inliers`` the rows in front of the camera
+    within the threshold of it; ``best_hypothesis`` and ``best_solution`` the P3P solution the final model grew from)
+    plus ``num_local_optimizations`` [B] int32, the local optimisations whose model was adopted, and ``cost`` [B]
+    int64, the final model's integer MSAC score.  Failures are those of ``estimate_absolute_pose``, with
+    ``num_local_optimizations`` and ``cost`` 0."""
+    return _absolute_pose(True, kpts0, points3d1, matches0, K0, ransac_reproj_threshold, max_iters, confidence, seed)
+
+
+def _absolute_pose(lo: bool, kpts0, points3d1, matches0, K0, ransac_reproj_threshold, max_iters, confidence,
+                   seed) -> dict:
     _check_inputs(kpts0, points3d1, matches0, "points3d1", 3)
     _check_params(ransac_reproj_threshold, max_iters, confidence, seed)
+    if lo and kpts0.shape[1] > _cabi.GEO_LO_MAX_MATCHES:
+        raise ValueError(f"kpts0 {tuple(kpts0.shape)}: at most {_cabi.GEO_LO_MAX_MATCHES} rows per pair")
     device = kpts0.device
     b, m, n = kpts0.shape[0], kpts0.shape[1], points3d1.shape[1]
     k0 = _intrinsics("K0", K0, b, device)
@@ -275,11 +302,18 @@ def estimate_absolute_pose(kpts0: torch.Tensor, points3d1: torch.Tensor, matches
     shapes = {"R": ((b, 3, 3), f64), "t": ((b, 3), f64), "inliers": ((b, m), bl), "num_inliers": ((b,), i32),
               "success": ((b,), bl), "best_hypothesis": ((b,), i32), "best_solution": ((b,), i32),
               "num_hypotheses": ((b,), i32)}
+    if lo:
+        shapes.update(num_local_optimizations=((b,), i32), cost=((b,), torch.int64))
 
     def make_args(out):
         cfg = _cabi.GeoPnpConfig(_cabi.GEO_ABI_VERSION, max_iters, seed, 0, float(ransac_reproj_threshold),
                                  float(confidence))
         ins = _cabi.GeoPnpInputs(b, m, n, p0.data_ptr(), x1.data_ptr(), m0.data_ptr(), k0.data_ptr())
-        return cfg, ins, _cabi.GeoPnpOutputs(*(out[k].data_ptr() for k in shapes))
+        outs = _cabi.GeoPnpOutputs(*(out[k].data_ptr() for k in list(shapes)[:8]))
+        if lo:
+            outs = _cabi.GeoLoPnpOutputs(outs, out["num_local_optimizations"].data_ptr(), out["cost"].data_ptr())
+        return cfg, ins, outs
 
+    if lo:
+        return _run("geo_absolute_pose_lo", "geo_lo_pnp_workspace_bytes", shapes, device, b, m, max_iters, make_args)
     return _run("geo_absolute_pose", "geo_pnp_workspace_bytes", shapes, device, b, m, max_iters, make_args)

@@ -1,0 +1,157 @@
+"""numpy restatement of the LO-RANSAC absolute pose of include/geometry_b200.h (geo_absolute_pose_lo, steps LA1-LA8,
+csrc/lo_pnp_api.cu).
+
+The compaction, calibration, samples, Lambda Twist solutions, projections and fp32 inlier test are pnp_oracle's; the
+MSAC score is lo_pose_oracle's; the Cholesky step, quaternion rotation and LM loop are lo_common's.  What is new here is
+the fp32 reprojection error that the score reads and the Levenberg-Marquardt refinement of (R, t) on the truncated
+squared reprojection error in pixels (double, elementwise operations only, so the CUDA build compiled with -fmad=false
+agrees bit for bit).
+"""
+from __future__ import annotations
+
+import numpy as np
+
+from oracle import geometry_oracle as go
+from oracle import lo_common as lc
+from oracle import lo_pose_oracle as lpo
+from oracle import pnp_oracle as pnp
+
+S = pnp.S
+DOF = 6              # parameters of an LM step: a rotation increment and a translation increment
+TERMS = 28           # J^T J upper triangle (21), J^T r (6), truncated cost
+QSCALE, STEPS, FINAL_STEPS, LAMBDA0 = lpo.QSCALE, lpo.STEPS, lpo.FINAL_STEPS, lpo.LAMBDA0
+
+
+def errors(P: np.ndarray, pix: np.ndarray, wld: np.ndarray) -> np.ndarray:
+    """fp32 errors [H, n] of projections P [H, 12] (cast to fp32) as A5: du*du + dv*dv in front of the camera (w > 0),
+    +inf behind it, so that the L3 score counts such a point as an outlier (header step LA3)."""
+    g = [P.astype(np.float32)[:, i:i + 1] for i in range(12)]
+    u, v = pix[None, :, 0], pix[None, :, 1]
+    X, Y, Z = wld[None, :, 0], wld[None, :, 1], wld[None, :, 2]
+    with np.errstate(all="ignore"):
+        w = g[8] * X + g[9] * Y + g[10] * Z + g[11]
+        iw = np.float32(1.0) / w
+        du = u - (g[0] * X + g[1] * Y + g[2] * Z + g[3]) * iw
+        dv = v - (g[4] * X + g[5] * Y + g[6] * Z + g[7]) * iw
+        return np.where(w > 0.0, du * du + dv * dv, np.float32(np.inf))
+
+
+def residuals(x, K, pix: np.ndarray, wld: np.ndarray):
+    """At x = R (9, row-major) + t (3): double residuals (ru, rv) in pixels, errors ru*ru + rv*rv, depths Xc2 and the
+    Jacobian rows ju, jv [6, n] of A7 (header step LA7)."""
+    R, t = x[:9], x[9:]
+    fx, s, cx, fy, cy = (float(K[i]) for i in (0, 1, 2, 4, 5))
+    u, v = pix[:, 0].astype(np.float64), pix[:, 1].astype(np.float64)
+    W = [wld[:, i].astype(np.float64) for i in range(3)]
+    with np.errstate(all="ignore"):
+        Xc = [R[3 * i] * W[0] + R[3 * i + 1] * W[1] + R[3 * i + 2] * W[2] + t[i] for i in range(3)]
+        iz = 1.0 / Xc[2]
+        a, b = Xc[0] * iz, Xc[1] * iz
+        pu = fx * a + s * b
+        ru, rv = pu + cx - u, fy * b + cy - v
+        gu = [fx * iz, s * iz, -(pu * iz)]
+        gv = [np.zeros_like(iz), fy * iz, -(fy * b * iz)]
+
+        def jrow(g):
+            return [g[2] * Xc[1] - g[1] * Xc[2], g[0] * Xc[2] - g[2] * Xc[0], g[1] * Xc[0] - g[0] * Xc[1], g[0], g[1], g[2]]
+        ju, jv = np.stack(jrow(gu)), np.stack(jrow(gv))
+        err = ru * ru + rv * rv
+    return ru, rv, err, Xc[2], ju, jv
+
+
+def terms(x, K, pix: np.ndarray, wld: np.ndarray, thr2: float) -> np.ndarray:
+    """The TERMS fixed-order sums at x: the points in front of the camera with err < thr2 give J^T J and J^T r, every
+    point its truncated cost (err for those, else thr2)."""
+    ru, rv, err, z, ju, jv = residuals(x, K, pix, wld)
+    with np.errstate(invalid="ignore"):
+        inl = (z > 0.0) & (err < thr2)
+    rows = []
+    with np.errstate(all="ignore"):
+        for i in range(DOF):
+            for j in range(i, DOF):
+                rows.append(np.where(inl, ju[i] * ju[j] + jv[i] * jv[j], 0.0))
+        for i in range(DOF):
+            rows.append(np.where(inl, ju[i] * ru + jv[i] * rv, 0.0))
+    rows.append(np.where(inl, err, thr2))
+    return go.fixed_sum(np.stack(rows))
+
+
+def update(x, d):
+    """R' = Q R, t' = Q t + d[3:] (A7's step)."""
+    Rn, tn = pnp._update(x[:9], x[9:], d)
+    return Rn + tn
+
+
+def refine(x, K, pix: np.ndarray, wld: np.ndarray, thr2: float, steps: int):
+    """steps Levenberg-Marquardt steps on the truncated reprojection cost from x, inliers re-selected at every pose."""
+    return lc.refine(lambda y: terms(y, K, pix, wld, thr2), update, [float(v) for v in x], DOF, steps)
+
+
+def rescore(x, K, pix: np.ndarray, wld: np.ndarray, thr2: np.float32):
+    """(LA3 score, count) of x through P = K0 [R | t] rounded to float."""
+    P = pnp.projection(np.array(x[:9]), np.array(x[9:]), K)
+    sc, cnt = lpo.score(errors(P[None], pix, wld)[0], thr2)
+    return int(sc), int(cnt)
+
+
+def _fail(M: int, drawn: int) -> dict:
+    return dict(pnp._fail(M, drawn), num_local_optimizations=0, cost=0)
+
+
+def lo_absolute_pose_pair(kpts0, points3d1, m0, K0, threshold=8.0, max_iters=100, confidence=0.99, seed=0) -> dict:
+    kpts0 = np.asarray(kpts0, dtype=np.float32)
+    points3d1 = np.asarray(points3d1, dtype=np.float32)
+    m0 = np.asarray(m0, dtype=np.int64)
+    K0 = np.asarray(K0, dtype=np.float64).reshape(9)
+    M = m0.shape[0]
+    idx, pix, wld = pnp.compact(kpts0, points3d1, m0)
+    n = pix.shape[0]
+    if n < S or not pnp.k_valid(K0):
+        return _fail(M, 0)
+    bear = pnp.calibrate(K0, pix)
+    thr2 = np.float32(threshold * threshold)
+    best, nlo, drawn = None, 0, 0  # best: (score, count, h, r, x)
+    for c in range(-(-max_iters // go.CHUNK)):
+        h = np.arange(c * go.CHUNK, min((c + 1) * go.CHUNK, max_iters), dtype=np.int64)
+        R, t, kept = pnp.solutions(seed, h, bear, wld)
+        if kept.any():
+            sc, cnt = lpo.score(errors(pnp.projection(R[kept], t[kept], K0), pix, wld), thr2)
+            i = int(np.argmin(sc))  # first minimum: the lowest (sample, solution)
+            if best is None or sc[i] < best[0]:
+                hh, rr = np.nonzero(kept)
+                x = [float(v) for v in R[hh[i], rr[i]]] + [float(v) for v in t[hh[i], rr[i]]]
+                best = (int(sc[i]), int(cnt[i]), int(h[hh[i]]), int(rr[i]), x)
+                xl = refine(x, K0, pix, wld, float(thr2), STEPS)
+                sl, cl = rescore(xl, K0, pix, wld, thr2)
+                if sl < best[0]:
+                    best = (sl, cl, best[2], best[3], xl)
+                    nlo += 1
+        drawn = min((c + 1) * go.CHUNK, max_iters)
+        ep = 1.0 - (best[1] if best else 0) / n
+        if drawn >= max_iters or drawn >= go.update_num_iters(confidence, ep, S, max_iters):
+            break
+    if best is None:
+        return _fail(M, drawn)
+    x = refine(best[4], K0, pix, wld, float(thr2), FINAL_STEPS)
+    cost, count = rescore(x, K0, pix, wld, thr2)
+    if cost > best[0]:  # the refinement is kept unless its score rises
+        x, cost, count = best[4], best[0], best[1]
+    P = pnp.projection(np.array(x[:9]), np.array(x[9:]), K0)
+    inliers = np.zeros(M, dtype=bool)
+    inliers[idx[pnp.reproj_inliers(P[None], pix, wld, thr2)[0]]] = True
+    return {"R": np.array(x[:9]).reshape(3, 3), "t": np.array(x[9:]), "inliers": inliers, "num_inliers": count,
+            "success": True, "best_hypothesis": best[2], "best_solution": best[3], "num_hypotheses": drawn,
+            "num_local_optimizations": nlo, "cost": cost}
+
+
+def lo_absolute_pose(kpts0, points3d1, matches0, K0, threshold=8.0, max_iters=100, confidence=0.99, seed=0) -> dict:
+    """Batched: [B, M, 2], [B, N, 3], [B, M], K0 [B, 3, 3] -> the outputs of geo_absolute_pose_lo as numpy arrays."""
+    outs = [lo_absolute_pose_pair(kpts0[b], points3d1[b], matches0[b], K0[b], threshold, max_iters, confidence, seed)
+            for b in range(len(matches0))]
+    return {k: np.stack([np.asarray(o[k]) for o in outs]) for k in outs[0]}
+
+
+def rotation_error(R, Rt) -> float:
+    """Angle in degrees of R Rt^T."""
+    c = (np.trace(np.asarray(R).reshape(3, 3) @ np.asarray(Rt).reshape(3, 3).T) - 1.0) / 2.0
+    return float(np.degrees(np.arccos(np.clip(c, -1.0, 1.0))))

@@ -1,12 +1,14 @@
-"""Batched GPU absolute pose (lightglue_b200.geometry.estimate_absolute_pose) against OpenCV on the host, and its cost
-behind the matcher.
+"""Batched GPU absolute pose (lightglue_b200.geometry.estimate_absolute_pose and estimate_absolute_pose_lo) against
+OpenCV on the host, and its cost behind the matcher.
 
 Prints one JSON line:
   * the card's name and power limit, read in this run;
   * GPU ms per batch (CUDA events) at B pairs of M putative 2D-3D matches and 20 / 50 / 70 % outliers, with OpenCV's
     adaptive stopping ("adaptive") and with confidence 1 ("full", every sample), at cv2.solvePnPRansac's defaults
-    (8 px, 0.99) and a budget of 100 samples (1000 at 70 %);
-  * cv2.solvePnPRansac on the host for the same pairs, one after another and in a 16-thread pool (null without cv2);
+    (8 px, 0.99) and a budget of 100 samples (1000 at 70 %), for the plain estimator and ("lo_adaptive", "lo_full")
+    the LO-RANSAC one;
+  * cv2.solvePnPRansac on the host for the same pairs, one after another and in a 16-thread pool (null without cv2),
+    with its RANSAC ("opencv") and with UsacParams of MSAC, inner + iterative LO and the LSQ polisher ("opencv_usac");
   * pairs/s of LightGlue (bf16x3, N = 2048, synthetic weights) alone and followed by estimate_absolute_pose on one
     stream, alternated.
 The scenes come from oracle/pnp_oracle.localization_scene (0.5 px noise, 640x480, f = 500); nothing is written to disk.
@@ -26,22 +28,30 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 from lightglue_b200 import LightGlue, synth  # noqa: E402
-from lightglue_b200.geometry import estimate_absolute_pose  # noqa: E402
+from lightglue_b200.geometry import estimate_absolute_pose, estimate_absolute_pose_lo  # noqa: E402
 from oracle import pnp_oracle as pp  # noqa: E402
 from tools.geometry_bench import gpu_info, time_gpu  # noqa: E402
 
 
-def opencv_times(k0, p3, m0, K, iters, threads):
+def opencv_times(k0, p3, m0, K, iters, threads, usac=False):
     try:
         import cv2
     except ImportError:
         return None
     cv2.setNumThreads(1)
+    if usac:
+        params = cv2.UsacParams()
+        params.confidence, params.maxIterations, params.threshold = 0.99, iters, 8.0
+        params.score, params.loMethod = cv2.SCORE_METHOD_MSAC, cv2.LOCAL_OPTIM_INNER_AND_ITER_LO
+        params.final_polisher = cv2.LSQ_POLISHER
 
     def one(b):
         _, pix, wld = pp.compact(k0[b], p3[b], m0[b])
-        cv2.solvePnPRansac(wld.astype(np.float64), pix.astype(np.float64), K, None, iterationsCount=iters,
-                           reprojectionError=8.0, confidence=0.99)
+        if usac:
+            cv2.solvePnPRansac(wld.astype(np.float64), pix.astype(np.float64), K, None, params=params)
+        else:
+            cv2.solvePnPRansac(wld.astype(np.float64), pix.astype(np.float64), K, None, iterationsCount=iters,
+                               reprojectionError=8.0, confidence=0.99)
 
     t = time.perf_counter()
     for b in range(len(m0)):
@@ -70,13 +80,15 @@ def main() -> None:
         k0, p3, m0, _, K, _, _ = (np.stack([p[i] for p in pairs]) for i in range(7))
         t0, t3, tm, tk = (torch.from_numpy(x).cuda() for x in (k0, p3, m0, K[0]))
         row = {"max_iters": iters}
-        for mode, c in (("adaptive", 0.99), ("full", 1.0)):
-            out = estimate_absolute_pose(t0, t3, tm, tk, max_iters=iters, confidence=c)
-            row[mode] = {"gpu_ms": round(time_gpu(lambda: estimate_absolute_pose(t0, t3, tm, tk, max_iters=iters,
-                                                                                 confidence=c), args.reps), 3),
-                         "mean_samples": float(out["num_hypotheses"].float().mean()),
-                         "mean_inliers": float(out["num_inliers"].float().mean())}
+        for prefix, fn in (("", estimate_absolute_pose), ("lo_", estimate_absolute_pose_lo)):
+            for mode, c in (("adaptive", 0.99), ("full", 1.0)):
+                out = fn(t0, t3, tm, tk, max_iters=iters, confidence=c)
+                row[prefix + mode] = {
+                    "gpu_ms": round(time_gpu(lambda: fn(t0, t3, tm, tk, max_iters=iters, confidence=c), args.reps), 3),
+                    "mean_samples": float(out["num_hypotheses"].float().mean()),
+                    "mean_inliers": float(out["num_inliers"].float().mean())}
         row["opencv"] = opencv_times(k0, p3, m0, K[0], iters, args.threads)
+        row["opencv_usac"] = opencv_times(k0, p3, m0, K[0], iters, args.threads, usac=True)
         res["pnp"][f"outliers{o}"] = row
     # the matcher alone, and followed by the absolute pose on its device output (no host read-back in between)
     data, _ = synth.make_pair(2048, b=args.batch, seed=7)
