@@ -66,6 +66,39 @@ LG_API int al_forward(AlHandle* h, const float* image, const float* image_size, 
                       float* keypoints, float* scores, float* descriptors, int32_t* counts, void* workspace,
                       size_t workspace_bytes, void* stream);
 
+/* Host-only introspection (no device work, no handle needed): the workspace plan of al_forward for a handle created
+ * with this configuration, a [B, 3, H, W] batch and cap = al_max_keypoints(H, W).  Writes, when non-null, the byte
+ * offset from the workspace's start and the size of each of its AL_LAYOUT_BUFFERS buffers, in this order, with what
+ * each holds when al_forward returns.  All fp32 NCHW unless
+ * stated; Hp x Wp is the image replicate-padded to multiples of 32 (top = (Hp - H) / 2 rows above, left = (Wp - W) / 2
+ * columns to the left), level l of the encoder is (Hp / s) x (Wp / s) with s = 1, 2, 8, 32, P0 = B Hp Wp, q = dim / 4.
+ * Only what is listed here may be relied on; the buffers are disjoint.
+ *   0      img    first P0 floats: the score head's sigmoid output on the padded frame [B, 1, Hp, Wp], before the crop
+ *                 (the padded image it held first is partly overwritten);
+ *   1      ta     first 4 P0 floats: score_head.2 + SELU [B, 4, Hp, Wp]; next 4 P0: score_head.4 + SELU (block1's
+ *                 first convolution, which this buffer held first, is lost);
+ *   2      x1     block1's output [B, c1, Hp, Wp];
+ *   3      s1     score_head.0 + SELU [B, 8, Hp, Wp];
+ *   4      invn   1 / max(|x1234|, 1e-12) per padded pixel [B, Hp, Wp];
+ *   5 .. 9   p1 t2 d2 x2 a2: 2x2 pool of x1 [B, c1, .] and at 1/2: block2's SELU(bn1(conv1 p1)) [B, c2, .], its
+ *                 downsample (1x1 + bias) of p1 [B, c2, .], block2's output x2 [B, c2, .], SELU(conv2 x2) [B, q, .];
+ *   10 .. 15 p2 o3 t3 d3 x3 a3: 4x4 pool of x2 [B, c2, .] and at 1/8: block3's *second* offset convolution (+ bias,
+ *                 clamped to +-max(h, w) / 4) of t3 [B, 18, .], t3 = SELU(bn1(deform conv1 p2)) [B, c3, .], the
+ *                 downsample of p2, x3, SELU(conv3 x3) [B, q, .];
+ *   16 .. 21 p3 o4 t4 d4 x4 a4: the same for block4 at 1/32 (c3 -> c4 channels);
+ *   22     score  the cropped score map [B, H, W];
+ *   23     nms    simple_nms of score with the borders zeroed; in threshold mode every value not above the image's
+ *                 threshold (detection_threshold, or its mean score in the fallback) is then -1 [B, H, W];
+ *   24     kpn    normalised keypoints (x, y) in [-1, 1] [B, cap, 2], zero past counts[b];
+ *   25     mean   threshold mode only: each image's mean score [B];
+ *   26     cnt    threshold mode only: int32 count of NMS values above detection_threshold per image [B];
+ *   27     sel_pos    int32 flat pixel index y W + x of each output row [B, cap] (rows < counts[b]);
+ *   28     sel_score  the NMS score of each output row, 0 for top-k filler rows [B, cap] (rows < counts[b]);
+ *   29     n_sel      int32 counts [B].
+ * Returns the workspace size (al_workspace_bytes), 0 for an invalid configuration or a non-positive size. */
+#define AL_LAYOUT_BUFFERS 30
+LG_API int64_t al_workspace_layout(const AlConfig* cfg, int32_t B, int32_t H, int32_t W, int64_t* offsets, int64_t* bytes);
+
 #ifdef __cplusplus
 }
 #endif

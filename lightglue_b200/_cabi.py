@@ -15,6 +15,7 @@ ABI_VERSION = 3
 SP_ABI_VERSION = 2
 SP_TC_BUFFERS = 9  # buffers of the tensor-core backbone's workspace plan (sp_tc_layout)
 AL_ABI_VERSION = 1
+AL_LAYOUT_BUFFERS = 30  # buffers of al_workspace_layout
 SIFT_ABI_VERSION = 1
 DISK_ABI_VERSION = 1
 DISK_LAYOUT_BUFFERS = 13  # buffers of disk_workspace_layout
@@ -232,6 +233,7 @@ AL_PROTOTYPES = {  # include/aliked_b200.h
     "al_max_keypoints": (_I64, [_VP, _I32, _I32]),
     "al_workspace_bytes": (_SZ, [_VP, _I32, _I32, _I32]),
     "al_forward": (C.c_int, [_VP, _VP, _VP, _I32, _I32, _I32, _I64] + [_VP] * 5 + [_SZ, _VP]),
+    "al_workspace_layout": (_I64, [C.POINTER(AlConfig), _I32, _I32, _I32, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
 }
 SIFT_PROTOTYPES = {  # include/sift_b200.h
     "sift_create": (C.c_int, [C.POINTER(SiftConfig), _VP, _HANDLE_OUT]),

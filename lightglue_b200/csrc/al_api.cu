@@ -586,6 +586,7 @@ struct Ws {
   int* cnt;
   SpWorkspace sp;                                   // the fields SuperPoint's compaction / selection use
   size_t bytes;
+  size_t part[AL_LAYOUT_BUFFERS];                   // sizes of the buffers al_workspace_layout reports, in its order
 };
 void carve(char* base, const AlConfig& c, int B, int H, int W, long cap, Ws* w) {
   WsBump bp{base, 0};
@@ -593,33 +594,34 @@ void carve(char* base, const AlConfig& c, int B, int H, int W, long cap, Ws* w) 
   const Geo g = geometry(H, W);
   const size_t P0 = (size_t)B * g.Hp * g.Wp, P1 = P0 / 4, P2 = P0 / 64, P3 = P0 / 1024, PX = (size_t)B * H * W;
   const int q = c.dim / 4;
-  w->img = take(3 * P0);
-  w->ta = take((size_t)(c.c1 > 8 ? c.c1 : 8) * P0);
-  w->x1 = take((size_t)c.c1 * P0);
-  w->s1 = take(8 * P0);
-  w->invn = take(P0);
-  w->p1 = take(c.c1 * P1); w->t2 = take(c.c2 * P1); w->d2 = take(c.c2 * P1);
-  w->x2 = take(c.c2 * P1); w->a2 = take(q * P1);
-  w->p2 = take(c.c2 * P2); w->o3 = take(18 * P2); w->t3 = take(c.c3 * P2);
-  w->d3 = take(c.c3 * P2); w->x3 = take(c.c3 * P2); w->a3 = take(q * P2);
-  w->p3 = take(c.c3 * P3); w->o4 = take(18 * P3); w->t4 = take(c.c4 * P3);
-  w->d4 = take(c.c4 * P3); w->x4 = take(c.c4 * P3); w->a4 = take(q * P3);
-  w->score = take(PX); w->nms = take(PX);
+  auto rec = [&](int i) { w->part[i] = bp.last; };  // index in al_workspace_layout's order
+  w->img = take(3 * P0); rec(0);
+  w->ta = take((size_t)(c.c1 > 8 ? c.c1 : 8) * P0); rec(1);
+  w->x1 = take((size_t)c.c1 * P0); rec(2);
+  w->s1 = take(8 * P0); rec(3);
+  w->invn = take(P0); rec(4);
+  w->p1 = take(c.c1 * P1); rec(5); w->t2 = take(c.c2 * P1); rec(6); w->d2 = take(c.c2 * P1); rec(7);
+  w->x2 = take(c.c2 * P1); rec(8); w->a2 = take(q * P1); rec(9);
+  w->p2 = take(c.c2 * P2); rec(10); w->o3 = take(18 * P2); rec(11); w->t3 = take(c.c3 * P2); rec(12);
+  w->d3 = take(c.c3 * P2); rec(13); w->x3 = take(c.c3 * P2); rec(14); w->a3 = take(q * P2); rec(15);
+  w->p3 = take(c.c3 * P3); rec(16); w->o4 = take(18 * P3); rec(17); w->t4 = take(c.c4 * P3); rec(18);
+  w->d4 = take(c.c4 * P3); rec(19); w->x4 = take(c.c4 * P3); rec(20); w->a4 = take(q * P3); rec(21);
+  w->score = take(PX); rec(22); w->nms = take(PX); rec(23);
   w->n1 = take(PX); w->n2 = take(PX); w->n3 = take(PX);
-  w->kpn = take((size_t)B * cap * 2);
-  w->mean = take(B);
-  w->cnt = bp.take<int>(B);
+  w->kpn = take((size_t)B * cap * 2); rec(24);
+  w->mean = take(B); rec(25);
+  w->cnt = bp.take<int>(B); rec(26);
   SpWorkspace& s = w->sp;
   s = SpWorkspace{};
   s.t0 = w->nms;
   s.cand_score = take(PX);
   s.cand_pos = bp.take<int>(PX);
-  s.sel_score = take((size_t)B * cap);
-  s.sel_pos = bp.take<int>((size_t)B * cap);
+  s.sel_score = take((size_t)B * cap); rec(28);
+  s.sel_pos = bp.take<int>((size_t)B * cap); rec(27);
   s.row_count = bp.take<int>((size_t)B * H);
   s.row_start = bp.take<int>((size_t)B * H);
   s.n_cand = bp.take<int>(B);
-  s.n_sel = bp.take<int>(B);
+  s.n_sel = bp.take<int>(B); rec(29);
   w->bytes = bp.bytes();
 }
 
@@ -682,6 +684,21 @@ extern "C" size_t al_workspace_bytes(const AlHandle* h, int32_t B, int32_t H, in
   Ws w;
   carve(nullptr, h->cfg, B, H, W, max_keypoints(h->cfg, H, W), &w);
   return w.bytes;
+}
+
+extern "C" int64_t al_workspace_layout(const AlConfig* cfg, int32_t B, int32_t H, int32_t W, int64_t* offsets, int64_t* bytes) {
+  if (!cfg || !valid(*cfg) || B <= 0 || H <= 0 || W <= 0) return 0;
+  Ws w;
+  char* const base = reinterpret_cast<char*>(kLayoutBase);
+  carve(base, *cfg, B, H, W, max_keypoints(*cfg, H, W), &w);
+  const void* p[AL_LAYOUT_BUFFERS] = {w.img, w.ta, w.x1, w.s1, w.invn, w.p1, w.t2, w.d2, w.x2, w.a2, w.p2, w.o3, w.t3,
+                                      w.d3, w.x3, w.a3, w.p3, w.o4, w.t4, w.d4, w.x4, w.a4, w.score, w.nms, w.kpn,
+                                      w.mean, w.cnt, w.sp.sel_pos, w.sp.sel_score, w.sp.n_sel};
+  for (int i = 0; i < AL_LAYOUT_BUFFERS; ++i) {
+    if (offsets) offsets[i] = (int64_t)((const char*)p[i] - base);
+    if (bytes) bytes[i] = (int64_t)w.part[i];
+  }
+  return (int64_t)w.bytes;
 }
 
 extern "C" int al_forward(AlHandle* h, const float* image, const float* image_size, int32_t B, int32_t H, int32_t W, int64_t cap,

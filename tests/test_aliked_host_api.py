@@ -71,3 +71,75 @@ def test_weights_found_in_weights_dir(tmp_path, monkeypatch):
 def test_unknown_model_name_raises():
     with pytest.raises(ValueError):
         ALIKED(model_name="aliked-x99", weights=None)
+
+
+# ---------------------------------------------------------------------------------------------- workspace layout
+LAYOUT_NAMES = ["img", "ta", "x1", "s1", "invn", "p1", "t2", "d2", "x2", "a2", "p2", "o3", "t3", "d3", "x3", "a3",
+                "p3", "o4", "t4", "d4", "x4", "a4", "score", "nms", "kpn", "mean", "cnt", "sel_pos", "sel_score", "n_sel"]
+
+
+def al_layout(cfg, b, h, w):
+    """{name: (byte offset, bytes)} of al_workspace_layout and its total."""
+    n = _cabi.AL_LAYOUT_BUFFERS
+    off, size = (C.c_int64 * n)(), (C.c_int64 * n)()
+    total = _cabi.load().al_workspace_layout(C.byref(cfg), b, h, w, off, size)
+    return {k: (off[i], size[i]) for i, k in enumerate(LAYOUT_NAMES)}, total
+
+
+def _expected_floats(model_name, b, h, w, cap):
+    c1, c2, c3, c4, dim, _, _ = ALIKED.cfgs[model_name]
+    hp, wp = -(-h // 32) * 32, -(-w // 32) * 32
+    p0, q, px = b * hp * wp, dim // 4, b * h * w
+    p1, p2, p3 = p0 // 4, p0 // 64, p0 // 1024
+    return {"img": 3 * p0, "ta": max(c1, 8) * p0, "x1": c1 * p0, "s1": 8 * p0, "invn": p0,
+            "p1": c1 * p1, "t2": c2 * p1, "d2": c2 * p1, "x2": c2 * p1, "a2": q * p1,
+            "p2": c2 * p2, "o3": 18 * p2, "t3": c3 * p2, "d3": c3 * p2, "x3": c3 * p2, "a3": q * p2,
+            "p3": c3 * p3, "o4": 18 * p3, "t4": c4 * p3, "d4": c4 * p3, "x4": c4 * p3, "a4": q * p3,
+            "score": px, "nms": px, "kpn": 2 * b * cap, "mean": b, "cnt": b, "sel_pos": b * cap, "sel_score": b * cap,
+            "n_sel": b}
+
+
+# (model, conf, B, H, W): t16 / n16 / n32, odd pads, a 1x1 level 3, top-k and threshold capacities
+LAYOUT_CASES = [("aliked-t16", {}, 1, 8, 8), ("aliked-t16", dict(max_num_keypoints=100), 2, 33, 47),
+                ("aliked-n16", {}, 3, 240, 320), ("aliked-n16", dict(max_num_keypoints=50, detection_threshold=-1), 1, 100, 37),
+                ("aliked-n32", {}, 1, 203, 317), ("aliked-n32", {}, 2, 768, 1024)]
+
+
+@pytest.mark.parametrize("model_name,conf,b,h,w", LAYOUT_CASES)
+def test_workspace_layout_buffers(model_name, conf, b, h, w):
+    """Every buffer 256-aligned, of its shape's size and disjoint from the others; the total is the bump carve of the
+    listed buffers plus DKD's scratch (three NMS planes, the candidate list and the row scan), 256-aligned."""
+    cfg = ALIKED(model_name=model_name, weights=None, **conf)._config()
+    lay, total = al_layout(cfg, b, h, w)
+    k = conf.get("max_num_keypoints", -1)
+    cap = min(k if k > 0 else 20000, h * w)
+    want = _expected_floats(model_name, b, h, w, cap)
+    for name, (o, n) in lay.items():
+        assert o % 256 == 0, name
+        assert n == 4 * want[name], (name, n, 4 * want[name])
+    spans = sorted(lay.values())
+    for (o0, n0), (o1, _) in zip(spans, spans[1:]):
+        assert o0 + n0 <= o1
+    # the carve's order, scratch (None: its float count) between the listed buffers
+    px = b * h * w
+    order = LAYOUT_NAMES[:24] + [px, px, px, "kpn", "mean", "cnt", px, px, "sel_score", "sel_pos", b * h, b * h, b,
+                                 "n_sel"]
+    at = 0
+    for item in order:
+        at = -(-at // 256) * 256
+        if isinstance(item, str):
+            assert lay[item][0] == at, item
+            at += lay[item][1]
+        else:
+            at += 4 * item
+    assert total == -(-at // 256) * 256
+
+
+def test_workspace_layout_rejects_bad_arguments():
+    cfg = ALIKED(weights=None)._config()
+    assert _cabi.load().al_workspace_layout(C.byref(cfg), 0, 64, 64, None, None) == 0
+    assert _cabi.load().al_workspace_layout(C.byref(cfg), 1, 64, 0, None, None) == 0
+    bad = ALIKED(weights=None)._config()
+    bad.M = 33
+    assert _cabi.load().al_workspace_layout(C.byref(bad), 1, 64, 64, None, None) == 0
+    assert _cabi.load().al_workspace_layout(C.byref(cfg), 1, 64, 64, None, None) > 0
