@@ -94,6 +94,44 @@ LG_API size_t nn_workspace_bytes(int32_t B, int32_t M, int32_t N, int32_t D);
 LG_API int nn_match(NnHandle* h, const NnConfig* cfg, const NnInputs* in, const NnOutputs* out, void* workspace,
                     size_t workspace_bytes, void* stream);
 
+/* Guided matching: each pair is matched again under its estimated homography H (image 0 -> image 1) or fundamental
+ * matrix F (x1^T F x0 = 0), with the conventions of geo_estimate (include/geometry_b200.h), and a candidate (i, j)
+ * counts only when it is consistent with that model (oracle/nn_guided_oracle.py restates the rules in float64).
+ *   gate(i, j) holds iff err(i, j) < t2, t2 = (float)(max_error * max_error) formed in double, where err is exactly
+ *   step 5 of include/geometry_b200.h on x0 = kpts0[b, i], x1 = kpts1[b, j]: the model rounded to float, fp32 without
+ *   fused multiply-adds; H the forward transfer error, F the larger (fmaxf) of the two squared point-to-line distances.
+ *   So (i, j) passes at max_error = t exactly when geo_estimate at threshold t counts it as an inlier of that model.  A
+ *   NaN error (a non-finite keypoint, a zero F) fails the gate.  The gate depends on the pair (i, j) only, not on the
+ *   direction of the sweep.
+ *   Pair b with valid[b] != 0 (or valid NULL) follows nn_match's rules with "every column" read as "every gated
+ *   column": j1 is the lowest gated j among the maxima, s2 the best over the other gated columns (-inf when there are
+ *   none), and a row with no gated column matches nothing; image 1's side likewise, then the mutual check.  Scores,
+ *   matches, match_scores and n_matches are defined as in nn_match.
+ *   Pair b with valid[b] == 0 is matched ungated: its outputs equal nn_match's bit for bit, so passing an estimator's
+ *   success flags as valid never loses a pair whose estimation failed.
+ * Work: nn_match's three launches per group plus one that writes a gate record per row (H: the projected point of an
+ * image-0 row, the point of an image-1 row; F: the point, its epipolar line in the other image and 1 / (a^2 + b^2));
+ * the tensor-core sweep evaluates the gate in its top-2 epilogue.  The launch sequence depends on (B, M, N, D, kind).
+ */
+#define NN_GUIDE_H 0 /* the model is a homography, as GEO_HOMOGRAPHY */
+#define NN_GUIDE_F 1 /* the model is a fundamental matrix, as GEO_FUNDAMENTAL */
+
+typedef struct NnGuide {
+  int32_t kind;         /* NN_GUIDE_H or NN_GUIDE_F */
+  const double* model;  /* DEVICE [B, 9] row-major, 8-byte aligned */
+  const uint8_t* valid; /* optional DEVICE [B]: 0 = match the pair ungated; NULL = every pair is guided */
+  const float* kpts0;   /* DEVICE [B, M, 2] pixels, 8-byte aligned */
+  const float* kpts1;   /* DEVICE [B, N, 2] */
+  double max_error;     /* pixels, positive and finite */
+} NnGuide;
+
+/* Scratch bytes of nn_match_guided for a (B, M, N, D) problem (0 for invalid sizes): nn_workspace_bytes' buffers and
+ * the gate records of one group, 24 bytes per row. */
+LG_API size_t nn_guided_workspace_bytes(int32_t B, int32_t M, int32_t N, int32_t D);
+
+LG_API int nn_match_guided(NnHandle* h, const NnConfig* cfg, const NnInputs* in, const NnGuide* guide,
+                           const NnOutputs* out, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -26,6 +26,7 @@ GEO_HOMOGRAPHY, GEO_FUNDAMENTAL, GEO_ESSENTIAL = 0, 1, 2
 GEO_LO_QSCALE, GEO_LO_MAX_MATCHES = 65536, (1 << 20) - 1
 NN_ABI_VERSION = 1  # include/nn_b200.h
 NN_MIN_DIM, NN_MAX_DIM, NN_GROUP_ROWS = 64, 512, 32768
+NN_GUIDE_H, NN_GUIDE_F = 0, 1
 
 
 class LgConfig(C.Structure):
@@ -196,6 +197,13 @@ class NnOutputs(C.Structure):
     ]
 
 
+class NnGuide(C.Structure):
+    _fields_ = [
+        ("kind", C.c_int32), ("model", C.c_void_p), ("valid", C.c_void_p), ("kpts0", C.c_void_p), ("kpts1", C.c_void_p),
+        ("max_error", C.c_double),
+    ]
+
+
 # name: (restype, argtypes), one table per header.  The export lists are the tables' keys.
 _VP, _I32, _I64, _SZ = C.c_void_p, C.c_int32, C.c_int64, C.c_size_t
 _HANDLE_OUT = C.POINTER(C.c_void_p)
@@ -289,6 +297,9 @@ NN_PROTOTYPES = {  # include/nn_b200.h
     "nn_destroy": (C.c_int, [_VP]),
     "nn_workspace_bytes": (_SZ, [_I32, _I32, _I32, _I32]),
     "nn_match": (C.c_int, [_VP, C.POINTER(NnConfig), C.POINTER(NnInputs), C.POINTER(NnOutputs), _VP, _SZ, _VP]),
+    "nn_guided_workspace_bytes": (_SZ, [_I32, _I32, _I32, _I32]),
+    "nn_match_guided": (C.c_int, [_VP, C.POINTER(NnConfig), C.POINTER(NnInputs), C.POINTER(NnGuide),
+                                  C.POINTER(NnOutputs), _VP, _SZ, _VP]),
 }
 _TABLES = (LG_PROTOTYPES, SP_PROTOTYPES, AL_PROTOTYPES, SIFT_PROTOTYPES, DISK_PROTOTYPES, DHN_PROTOTYPES, GEO_PROTOTYPES,
            NN_PROTOTYPES)

@@ -29,6 +29,8 @@ constexpr int BN = 256, BK = 64;
 constexpr int W_TILE_BYTES = BN * BK * 2;  // 32 KB
 
 enum { TEPI_QKV = 0, TEPI_LN_GELU = 2, TEPI_RESID = 3, TEPI_F32 = 4, TEPI_LSE = 5, TEPI_ARGMAX = 6, TEPI_CONV = 7, TEPI_TOP2 = 8 };
+// the guided nearest-neighbour sweeps: TEPI_TOP2 over the columns that pass a homography (H) or epipolar (F) gate
+enum { TEPI_TOP2_H = 9, TEPI_TOP2_F = 10 };
 
 struct TcLinParams {
   CUtensorMap a_hi[2], a_lo[2];  // A segment 0 / 1, box 64 x tile rows
@@ -68,6 +70,9 @@ struct TcLinParams {
   // and vt ([S H 64, Lp], box 64 rows x 64 d); TEPI_RESID / F32 / CONV / LN_GELU: out_f32 (box 16 x 64, also the
   // residual's load map), out_h, out_l (box 16 x 64)
   CUtensorMap out_map[3];
+  // TEPI_TOP2_H / F (appended, so the parameter offsets of the other epilogues stay put): gate records, field f of row
+  // r at gate_rec[f * S Lp + r] (H: 2 fields, F: 6), gate_on[pair] != 0 for a guided pair, and the squared threshold
+  const float* gate_rec; const int* gate_on; float gate_t2;
 };
 
 constexpr int TBM = 128;  // rows per tile
@@ -404,16 +409,60 @@ __global__ void __launch_bounds__(LinCfg<EPI>::THREADS, 1) tc_linear_kernel(cons
       ++lt;
     }
 
-    if (EPI == TEPI_TOP2) {
+    constexpr bool GATED = EPI == TEPI_TOP2_H || EPI == TEPI_TOP2_F;
+    constexpr int GATE_FIELDS = EPI == TEPI_TOP2_F ? 6 : 2;
+    if (EPI == TEPI_TOP2 || GATED) {
       // ---------------------------------------------------------------- nearest-neighbour sweep (nn_api.cu)
       // per row and per 128-column slot of live partner columns: the best similarity s1, its column j1 (ascending
       // columns: the first maximum wins) and the best over the slot's other columns s2 (equal to s1 on a tie)
       const int lens = p.st.len[ti.sel];
+      // Guided sweeps: only the columns whose gate passes enter the top-2.  The gate records of the tile's 256 partner
+      // columns are staged in shared memory, one array per field (the staging boxes are free in this epilogue); the
+      // tile's own rows read theirs from global memory.  A pair that is not guided takes the ungated path: the flag is
+      // uniform per tile, so both MMA warpgroups meet the same barriers.
+      float* s_rec = reinterpret_cast<float*>(s_stg);  // [GATE_FIELDS][BN]
+      const long rec_rows = (long)p.st.S * p.st.Lp;
+      bool gate_on = false;
+      if (GATED) {
+        gate_on = p.gate_on[ti.s >= p.st.B ? ti.s - p.st.B : ti.s] != 0;
+        if (gate_on) {
+          const int col = ti.n_tile * BN + mt;
+          mma_bar();  // both warpgroups are done with the previous tile's records
+#pragma unroll
+          for (int f = 0; f < GATE_FIELDS; ++f)
+            s_rec[f * BN + mt] = col < p.st.Lp ? __ldg(p.gate_rec + f * rec_rows + (long)ti.sel * p.st.Lp + col) : 0.f;
+          mma_bar();
+        }
+      }
 #pragma unroll
       for (int hr = 0; hr < 2; ++hr) {
         const int rl = rl_a + 8 * hr;
         const long grow = ti.grow0 + rl;
         const bool live = ti.r0 + rl < ti.len;
+        float rr[GATE_FIELDS];  // this row's gate record
+#pragma unroll
+        for (int f = 0; f < GATE_FIELDS; ++f) rr[f] = GATED && gate_on ? __ldg(p.gate_rec + f * rec_rows + grow) : 0.f;
+        // include/nn_b200.h: step 5 of include/geometry_b200.h in fp32 with every operation rounded on its own.  Both
+        // forms are symmetric in the two records, so the direction of the sweep does not enter: H squares the
+        // difference of the projected point and the point (b - a = -(a - b) exactly); F takes the fmaxf of the two
+        // point-to-line terms, each record holding its point and its line in the other image.
+        auto gate = [&](int cl) -> bool {
+          const float* cr = s_rec + cl;
+          float err;
+          if constexpr (EPI != TEPI_TOP2_F) {
+            const float dx = __fsub_rn(rr[0], cr[0]), dy = __fsub_rn(rr[1], cr[BN]);
+            err = __fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy));
+          } else {
+            // record: x, y, a, b, c, s = 1 / (a^2 + b^2) with (a, b, c) the point's epipolar line
+            auto term = [](float px, float py, float a, float b, float c, float s) {
+              const float d = __fadd_rn(__fadd_rn(__fmul_rn(px, a), __fmul_rn(py, b)), c);
+              return __fmul_rn(__fmul_rn(d, d), s);
+            };
+            err = fmaxf(term(cr[0], cr[BN], rr[2], rr[3], rr[4], rr[5]),
+                        term(rr[0], rr[1], cr[2 * BN], cr[3 * BN], cr[4 * BN], cr[5 * BN]));
+          }
+          return err < p.gate_t2;  // NaN fails
+        };
 #pragma unroll
         for (int half = 0; half < 2; ++half) {
           const int col0 = ti.n_tile * BN + half * 128;
@@ -426,7 +475,7 @@ __global__ void __launch_bounds__(LinCfg<EPI>::THREADS, 1) tc_linear_kernel(cons
             for (int e = 0; e < 2; ++e) {
               const int c = 8 * jj + 2 * tq + e;
               const float v = acc[4 * (16 * half + jj) + 2 * hr + e];
-              if (c < ncols) {
+              if (c < ncols && (!GATED || !gate_on || gate(half * 128 + c))) {
                 if (v > b1) { b2 = b1; b1 = v; a1 = col0 + c; }
                 else b2 = fmaxf(b2, v);
               }
@@ -750,6 +799,8 @@ int launch_linear(const TcLinParams& p, cudaStream_t stream) {
     case TEPI_LSE: return launch_linear_t<TEPI_LSE>(p, stream);
     case TEPI_ARGMAX: return launch_linear_t<TEPI_ARGMAX>(p, stream);
     case TEPI_TOP2: return launch_linear_t<TEPI_TOP2>(p, stream);
+    case TEPI_TOP2_H: return launch_linear_t<TEPI_TOP2_H>(p, stream);
+    case TEPI_TOP2_F: return launch_linear_t<TEPI_TOP2_F>(p, stream);
   }
   return lg_set_error("launch_linear: bad epilogue");
 }
@@ -871,7 +922,7 @@ int tc_assign_sweeps(LgHandle* h, const TcBuffers& b, const SeqState& st, const 
 // Nearest-neighbour sweep: S = d_s d_partner^T of every sequence in split-bf16 (hi / lo [st.S * st.Lp, dim]), per row the
 // top-2 partials of every 128-column slot into part (float2) / part_arg, [st.S * st.Lp, pstride]
 int tc_nn_sweep(TcEngine& e, const SeqState& st, const __nv_bfloat16* hi, const __nv_bfloat16* lo, int dim, float* part,
-                int* part_arg, int pstride, cudaStream_t stream) {
+                int* part_arg, int pstride, cudaStream_t stream, const TcNnGate* gate) {
   if (dim % BK != 0) return lg_set_error("tc_nn_sweep: the descriptor size must be a multiple of 64");
   const int ntc = (st.Lp + BN - 1) / BN;
   if (pstride < 2 * ntc) return lg_set_error("tc_nn_sweep: slot stride too small");
@@ -880,6 +931,10 @@ int tc_nn_sweep(TcEngine& e, const SeqState& st, const __nv_bfloat16* hi, const 
   p.epi = TEPI_TOP2; p.scale = 1.f;
   p.part = part; p.part_arg = part_arg; p.part_stride = pstride;
   p.w_select = 2;
+  if (gate) {
+    p.epi = gate->fundamental ? TEPI_TOP2_F : TEPI_TOP2_H;
+    p.gate_rec = gate->rec; p.gate_on = gate->on; p.gate_t2 = gate->t2;
+  }
   return tc_gemm(e, st, ops, ntc, p, stream);
 }
 

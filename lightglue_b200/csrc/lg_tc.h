@@ -49,9 +49,17 @@ int tc_assign_sweeps(LgHandle* h, const TcBuffers& b, const SeqState& st, const 
                      float* term, cudaStream_t stream);
 // Nearest-neighbour sweep on the tensor cores (split-bf16, e.x3): S = d_s d_partner^T in both directions from the bf16
 // hi / lo images [st.S * st.Lp, dim]; per live row and 128-column slot of live partner columns, (s1, s2) into part
-// (float2) and j1 into part_arg, [st.S * st.Lp, pstride] with pstride >= 2 ceil(Lp / 256) (k_tc_linear.cu, TEPI_TOP2)
+// (float2) and j1 into part_arg, [st.S * st.Lp, pstride] with pstride >= 2 ceil(Lp / 256) (k_tc_linear.cu, TEPI_TOP2).
+// With a gate (guided matching, include/nn_b200.h) only the columns (row record, column record) passes enter the top-2
+// of a pair with on[pair] != 0 (TEPI_TOP2_H / TEPI_TOP2_F).
+struct TcNnGate {
+  bool fundamental;  // records: H (u, v) / F (x, y, a, b, c, s), field f of row r at rec[f * st.S * st.Lp + r]
+  const float* rec;
+  const int* on;     // [st.B] 0: the pair is matched ungated
+  float t2;          // a column passes when err < t2
+};
 int tc_nn_sweep(TcEngine& e, const SeqState& st, const __nv_bfloat16* hi, const __nv_bfloat16* lo, int dim, float* part,
-                int* part_arg, int pstride, cudaStream_t stream);
+                int* part_arg, int pstride, cudaStream_t stream, const TcNnGate* gate = nullptr);
 // softmax(q k^T / 8) v per (sequence, head): q from b.q, keys from kbuf, values from b.vt; key/value
 // sequence = (s + kv_shift) % S; writes b.ctxh (/ b.ctxl)
 int tc_attention(LgHandle* h, const TcBuffers& b, const SeqState& st, int kv_shift, const __half* kbuf, cudaStream_t stream);

@@ -1,8 +1,10 @@
 // C ABI of the nearest-neighbour matcher (include/nn_b200.h): per group of pairs, the split into bf16 hi / lo images,
 // the tensor-core top-2 sweep of both directions (k_tc_linear.cu, TEPI_TOP2) and one CTA per pair for the tests and
-// the outputs.
+// the outputs.  Guided matching adds one launch per group that writes the gate records, and runs the sweep with the
+// gated epilogue (TEPI_TOP2_H / TEPI_TOP2_F).
 #include <math.h>
 #include <stdint.h>
+#include <stdio.h>
 
 #include <new>
 
@@ -31,9 +33,13 @@ struct NnWs {
   float* sbest;            // [2G Lp] s1
   int* len;                // [2G] rows of each sequence
   int* stop;               // [G] zero: the sweep's per-pair stop words
+  float* rec;              // guided only: [GATE_FIELDS][2G Lp] the rows' gate records
+  int* gate_on;            // guided only: [G] non-zero for a guided pair
 };
 
-size_t carve(char* base, int B, int M, int N, int D, NnWs* w) {
+constexpr int GATE_FIELDS = 6;  // F: x, y, a, b, c, s; H uses the first two
+
+size_t carve(char* base, int B, int M, int N, int D, NnWs* w, bool guided = false) {
   const int mx = M > N ? M : N;
   w->Lp = ((mx > 0 ? mx : 1) + LG_TILE - 1) / LG_TILE * LG_TILE;
   const int gmax = NN_GROUP_ROWS / w->Lp > 1 ? NN_GROUP_ROWS / w->Lp : 1;
@@ -50,6 +56,8 @@ size_t carve(char* base, int B, int M, int N, int D, NnWs* w) {
   w->sbest = b.take<float>(R);
   w->len = b.take<int>(2 * (size_t)w->G);
   w->stop = b.take<int>(w->G);
+  w->rec = guided ? b.take<float>(R * GATE_FIELDS) : nullptr;
+  w->gate_on = guided ? b.take<int>(w->G) : nullptr;
   return b.bytes();
 }
 
@@ -93,6 +101,55 @@ __global__ void __launch_bounds__(256) nn_pack_kernel(PackArgs a) {
     *reinterpret_cast<uint2*>(a.hi + row * a.D + c) = *reinterpret_cast<const uint2*>(h);
     *reinterpret_cast<uint2*>(a.lo + row * a.D + c) = *reinterpret_cast<const uint2*>(l);
   }
+}
+
+struct GateArgs {
+  const double* model; const uint8_t* valid;
+  const float *k0, *k1;
+  int b0, g, M, N, Lp;  // pairs b0 .. b0 + g - 1
+  int fundamental;
+  float* rec; int* on;
+};
+
+// One thread per row of the group's sequences: the row's gate record, from step 5 of include/geometry_b200.h in fp32
+// with every operation rounded on its own (this file is compiled with fused multiply-adds allowed), the model rounded
+// to float.  H: an image-0 row stores its projected point ((h0 x + h1 y) + h2) w, ((h3 x + h4 y) + h5) w with
+// w = 1 / ((h6 x + h7 y) + h8), an image-1 row its point.  F: a row stores its point, its epipolar line in the other
+// image (F x0 row by row for image 0, F^T x1 for image 1) and 1 / (a^2 + b^2).  Rows past M / N store zeros.
+__global__ void __launch_bounds__(256) nn_gate_record_kernel(GateArgs a) {
+  const long rows = 2L * a.g * a.Lp;
+  const long row = blockIdx.x * 256L + threadIdx.x;
+  if (row < a.g) a.on[row] = a.valid ? a.valid[a.b0 + row] != 0 : 1;
+  if (row >= rows) return;
+  const int s = (int)(row / a.Lp), r = (int)(row % a.Lp);
+  const bool im1 = s >= a.g;
+  const int pb = a.b0 + (im1 ? s - a.g : s);
+  const int cap = im1 ? a.N : a.M;
+  float v[GATE_FIELDS] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  if (r < cap) {
+    const float2 x = reinterpret_cast<const float2*>(im1 ? a.k1 : a.k0)[(long)pb * cap + r];
+    float h[9];
+#pragma unroll
+    for (int k = 0; k < 9; ++k) h[k] = (float)a.model[(long)pb * 9 + k];
+    // (u x + v y) + w, rounded step by step
+    auto lin = [&](float u, float vv, float w) { return __fadd_rn(__fadd_rn(__fmul_rn(u, x.x), __fmul_rn(vv, x.y)), w); };
+    v[0] = x.x; v[1] = x.y;
+    if (!a.fundamental) {
+      if (!im1) {
+        const float w = __fdiv_rn(1.f, lin(h[6], h[7], h[8]));
+        v[0] = __fmul_rn(lin(h[0], h[1], h[2]), w);
+        v[1] = __fmul_rn(lin(h[3], h[4], h[5]), w);
+      }
+    } else {
+      const float la = im1 ? lin(h[0], h[3], h[6]) : lin(h[0], h[1], h[2]);
+      const float lb = im1 ? lin(h[1], h[4], h[7]) : lin(h[3], h[4], h[5]);
+      const float lc = im1 ? lin(h[2], h[5], h[8]) : lin(h[6], h[7], h[8]);
+      v[2] = la; v[3] = lb; v[4] = lc;
+      v[5] = __fdiv_rn(1.f, __fadd_rn(__fmul_rn(la, la), __fmul_rn(lb, lb)));
+    }
+  }
+  const int fields = a.fundamental ? GATE_FIELDS : 2;
+  for (int f = 0; f < fields; ++f) a.rec[f * rows + row] = v[f];
 }
 
 struct TailArgs {
@@ -193,24 +250,50 @@ extern "C" size_t nn_workspace_bytes(int32_t B, int32_t M, int32_t N, int32_t D)
   return carve(nullptr, B, M, N, D, &w);
 }
 
-extern "C" int nn_match(NnHandle* h, const NnConfig* cfg, const NnInputs* in, const NnOutputs* out, void* workspace,
-                        size_t workspace_bytes, void* stream_) {
-  if (!h || !cfg || !in || !out) return lg_set_error("nn_match: null argument");
-  if (cfg->abi_version != NN_ABI_VERSION) return lg_set_error("nn_match: ABI version mismatch");
+extern "C" size_t nn_guided_workspace_bytes(int32_t B, int32_t M, int32_t N, int32_t D) {
+  if (B < 0 || M < 0 || N < 0 || !dim_ok(D)) return 0;
+  NnWs w;
+  return carve(nullptr, B, M, N, D, &w, true);
+}
+
+static int nn_error(const char* entry, const char* what) {
+  char msg[128];
+  snprintf(msg, sizeof(msg), "%s: %s", entry, what);
+  return lg_set_error(msg);
+}
+
+// nn_match and nn_match_guided (guide non-null): the argument checks, then per group the pack, [the gate records,] the
+// sweep and the tail
+static int nn_run(const char* entry, NnHandle* h, const NnConfig* cfg, const NnInputs* in, const NnGuide* guide,
+                  const NnOutputs* out, void* workspace, size_t workspace_bytes, void* stream_) {
+  const bool guided = guide != nullptr;
+  if (!h || !cfg || !in || !out) return nn_error(entry, "null argument");
+  if (cfg->abi_version != NN_ABI_VERSION) return nn_error(entry, "ABI version mismatch");
   const int B = in->B, M = in->M, N = in->N, D = cfg->dim;
-  if (!dim_ok(D)) return lg_set_error("nn_match: dim must be a multiple of 64 in [64, 512]");
-  if (B < 0 || M < 0 || N < 0) return lg_set_error("nn_match: negative size");
-  if (!isfinite(cfg->ratio_thresh) || cfg->ratio_thresh > 1.f) return lg_set_error("nn_match: ratio_thresh must be <= 1");
-  if (!isfinite(cfg->distance_thresh)) return lg_set_error("nn_match: distance_thresh must be finite");
+  if (!dim_ok(D)) return nn_error(entry, "dim must be a multiple of 64 in [64, 512]");
+  if (B < 0 || M < 0 || N < 0) return nn_error(entry, "negative size");
+  if (!isfinite(cfg->ratio_thresh) || cfg->ratio_thresh > 1.f) return nn_error(entry, "ratio_thresh must be <= 1");
+  if (!isfinite(cfg->distance_thresh)) return nn_error(entry, "distance_thresh must be finite");
+  if (guided) {
+    if (guide->kind != NN_GUIDE_H && guide->kind != NN_GUIDE_F) return nn_error(entry, "kind must be NN_GUIDE_H or NN_GUIDE_F");
+    if (!(guide->max_error > 0.0) || !isfinite(guide->max_error)) return nn_error(entry, "max_error must be positive and finite");
+  }
   if (B == 0) return 0;
   if ((M > 0 && (!in->desc0 || !out->matches0 || !out->matching_scores0 || !out->matches || !out->match_scores)) ||
       (N > 0 && (!in->desc1 || !out->matches1 || !out->matching_scores1)) || !out->n_matches)
-    return lg_set_error("nn_match: required pointer is null");
+    return nn_error(entry, "required pointer is null");
   if ((reinterpret_cast<uintptr_t>(in->desc0) | reinterpret_cast<uintptr_t>(in->desc1)) & 15)
-    return lg_set_error("nn_match: descriptors must be 16-byte aligned");
+    return nn_error(entry, "descriptors must be 16-byte aligned");
+  if (guided) {
+    if (!guide->model || (M > 0 && !guide->kpts0) || (N > 0 && !guide->kpts1))
+      return nn_error(entry, "model or keypoint pointer is null");
+    if ((reinterpret_cast<uintptr_t>(guide->model) | reinterpret_cast<uintptr_t>(guide->kpts0) |
+         reinterpret_cast<uintptr_t>(guide->kpts1)) & 7)
+      return nn_error(entry, "model and keypoints must be 8-byte aligned");
+  }
   NnWs w;
-  if (!workspace || workspace_bytes < carve(nullptr, B, M, N, D, &w)) return lg_set_error("nn_match: workspace too small");
-  carve(static_cast<char*>(workspace), B, M, N, D, &w);
+  if (!workspace || workspace_bytes < carve(nullptr, B, M, N, D, &w, guided)) return nn_error(entry, "workspace too small");
+  carve(static_cast<char*>(workspace), B, M, N, D, &w, guided);
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const double r = cfg->ratio_thresh, t = cfg->distance_thresh;
   TailArgs ta{};
@@ -220,6 +303,12 @@ extern "C" int nn_match(NnHandle* h, const NnConfig* cfg, const NnInputs* in, co
   ta.r2 = r > 0 ? (float)(r * r) : 0.f;
   ta.t2 = t > 0 ? (float)(t * t) : 0.f;
   ta.mutual = cfg->mutual_check != 0;
+  TcNnGate gate{};
+  if (guided) {
+    gate.fundamental = guide->kind == NN_GUIDE_F;
+    gate.rec = w.rec; gate.on = w.gate_on;
+    gate.t2 = (float)(guide->max_error * guide->max_error);
+  }
   for (int b0 = 0; b0 < B; b0 += w.G) {
     const int g = B - b0 < w.G ? B - b0 : w.G;
     PackArgs pa{in->desc0, in->desc1, in->lens0, in->lens1, b0, g, M, N, D, w.Lp, w.hi, w.lo, w.len, w.stop};
@@ -227,8 +316,14 @@ extern "C" int nn_match(NnHandle* h, const NnConfig* cfg, const NnInputs* in, co
     const long blocks = (groups4 + 255) / 256;
     nn_pack_kernel<<<(unsigned)(blocks < 8192 ? blocks : 8192), 256, 0, stream>>>(pa);
     LG_CHECK_LAUNCH();
+    if (guided) {
+      const GateArgs ga{guide->model, guide->valid, guide->kpts0, guide->kpts1, b0, g, M, N, w.Lp, gate.fundamental,
+                        w.rec, w.gate_on};
+      nn_gate_record_kernel<<<(unsigned)((2L * g * w.Lp + 255) / 256), 256, 0, stream>>>(ga);
+      LG_CHECK_LAUNCH();
+    }
     const SeqState st{2 * g, g, w.Lp, w.len, w.stop};
-    LG_RC(tc_nn_sweep(h->tc, st, w.hi, w.lo, D, w.part, w.parg, w.pstride, stream));
+    LG_RC(tc_nn_sweep(h->tc, st, w.hi, w.lo, D, w.part, w.parg, w.pstride, stream, guided ? &gate : nullptr));
     ta.g = g;
     ta.m0 = out->matches0 + (long)b0 * M; ta.ms0 = out->matching_scores0 + (long)b0 * M;
     ta.m1 = out->matches1 + (long)b0 * N; ta.ms1 = out->matching_scores1 + (long)b0 * N;
@@ -238,4 +333,15 @@ extern "C" int nn_match(NnHandle* h, const NnConfig* cfg, const NnInputs* in, co
     LG_CHECK_LAUNCH();
   }
   return 0;
+}
+
+extern "C" int nn_match(NnHandle* h, const NnConfig* cfg, const NnInputs* in, const NnOutputs* out, void* workspace,
+                        size_t workspace_bytes, void* stream) {
+  return nn_run("nn_match", h, cfg, in, nullptr, out, workspace, workspace_bytes, stream);
+}
+
+extern "C" int nn_match_guided(NnHandle* h, const NnConfig* cfg, const NnInputs* in, const NnGuide* guide,
+                               const NnOutputs* out, void* workspace, size_t workspace_bytes, void* stream) {
+  if (!guide) return nn_error("nn_match_guided", "null argument");
+  return nn_run("nn_match_guided", h, cfg, in, guide, out, workspace, workspace_bytes, stream);
 }

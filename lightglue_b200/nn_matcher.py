@@ -27,7 +27,15 @@ class NearestNeighborMatcher(nn.Module):
 
     Returns ``matches0`` [B, M] / ``matches1`` [B, N] int64 (-1 unmatched), ``matching_scores0`` / ``matching_scores1``
     float32 ((1 + d0_i . d1_j) / 2 for a match, else 0), and per pair ``matches`` [K_b, 2] (i, j) in ascending i with
-    ``scores`` [K_b].  D is a multiple of 64 in [64, 512]."""
+    ``scores`` [K_b].  D is a multiple of 64 in [64, 512].
+
+    Guided matching: ``forward(data, F=...)`` or ``forward(data, H=...)`` matches each pair again under its estimated
+    fundamental matrix (x1^T F x0 = 0) or homography (image 0 -> image 1), [B, 3, 3] of any float dtype, as
+    ``lightglue_b200.geometry`` returns them.  A candidate (i, j) counts only when its error under the model (the
+    estimators' inlier error: the transfer error for H, the larger point-to-epipolar-line distance for F, squared) is
+    below ``max_error``^2 pixels^2; the ratio, distance and mutual tests then run among those candidates only.  It needs
+    ``data["image0"]["keypoints"]`` [B, M, 2] and ``data["image1"]["keypoints"]`` [B, N, 2].  A pair whose ``valid``
+    [B] entry is zero (e.g. an estimator's ``success``) is matched ungated, exactly as without a model."""
 
     default_conf = {"ratio_thresh": None, "distance_thresh": None, "mutual_check": True}
 
@@ -45,6 +53,37 @@ class NearestNeighborMatcher(nn.Module):
         if t is not None and not (0.0 < float(t) < math.inf):
             raise ValueError(f"distance_thresh={t!r}: None or a positive number")
 
+    @staticmethod
+    def _guide(d0: dict, d1: dict, b: int, m: int, n: int, F, H, valid, max_error):
+        """Checks the guided keywords; returns (kind, model, kpts0, kpts1, valid or None) as given."""
+        if F is not None and H is not None:
+            raise ValueError("give at most one of F and H")
+        kind, model = (_cabi.NN_GUIDE_F, F) if F is not None else (_cabi.NN_GUIDE_H, H)
+        if not isinstance(model, torch.Tensor) or not model.is_floating_point() or tuple(model.shape) != (b, 3, 3):
+            shape = tuple(model.shape) if isinstance(model, torch.Tensor) else type(model).__name__
+            raise ValueError(f"model {shape}: expected a float tensor [{b}, 3, 3]")
+        try:
+            err = float(max_error)
+        except (TypeError, ValueError):
+            raise ValueError(f"max_error={max_error!r}: a positive number of pixels") from None
+        if not 0.0 < err < math.inf:
+            raise ValueError(f"max_error={max_error!r}: a positive number of pixels")
+        kps = []
+        for name, img, rows in (("image0", d0, m), ("image1", d1, n)):
+            k = img.get("keypoints")
+            if k is None:
+                raise ValueError(f"guided matching needs data[{name!r}]['keypoints']")
+            if not isinstance(k, torch.Tensor) or tuple(k.shape) != (b, rows, 2):
+                shape = tuple(k.shape) if isinstance(k, torch.Tensor) else type(k).__name__
+                raise ValueError(f"{name} keypoints {shape}: expected [{b}, {rows}, 2]")
+            kps.append(k.detach())
+        if valid is not None:
+            valid = torch.as_tensor(valid)
+            if valid.reshape(-1).numel() != b or valid.dim() > 1:
+                raise ValueError(f"valid {tuple(valid.shape)}: expected [{b}]")
+            valid = valid.reshape(b)
+        return kind, model.detach(), kps[0], kps[1], valid
+
     @classmethod
     def _handle(cls, device: torch.device):
         h = cls._handles.get(device.index)
@@ -55,7 +94,7 @@ class NearestNeighborMatcher(nn.Module):
             cls._handles[device.index] = h
         return h
 
-    def forward(self, data: dict) -> dict:
+    def forward(self, data: dict, *, F=None, H=None, valid=None, max_error: float = 4.0) -> dict:
         d0, d1 = data["image0"], data["image1"]
         x0, x1 = d0["descriptors"], d1["descriptors"]
         if not isinstance(x0, torch.Tensor) or not isinstance(x1, torch.Tensor):
@@ -68,6 +107,7 @@ class NearestNeighborMatcher(nn.Module):
             raise ValueError(f"descriptors {tuple(x0.shape)} and {tuple(x1.shape)}: batch and D must agree")
         if dim % 64 or not _cabi.NN_MIN_DIM <= dim <= _cabi.NN_MAX_DIM:
             raise ValueError(f"descriptor size {dim}: a multiple of 64 in [{_cabi.NN_MIN_DIM}, {_cabi.NN_MAX_DIM}]")
+        guide = None if F is None and H is None else self._guide(d0, d1, b, m, n, F, H, valid, max_error)
         if x0.device.type != "cuda" or x1.device.type != "cuda":
             raise RuntimeError("lightglue_b200.NearestNeighborMatcher runs on CUDA (sm_90a) tensors only; there is no "
                                "CPU path")
@@ -76,6 +116,12 @@ class NearestNeighborMatcher(nn.Module):
         device = x0.device
         x0 = x0.detach().to(torch.float32).contiguous()
         x1 = x1.detach().to(torch.float32).contiguous()
+        if guide is not None:
+            kind, model, kp0, kp1, ok = guide
+            model = model.to(device=device, dtype=torch.float64).reshape(b, 9).contiguous()
+            kp0 = kp0.to(device=device, dtype=torch.float32).contiguous()
+            kp1 = kp1.to(device=device, dtype=torch.float32).contiguous()
+            ok = None if ok is None else (ok.to(device) != 0).to(torch.uint8).contiguous()
 
         def lens(img, cap):
             t = img.get("num_keypoints")
@@ -108,10 +154,17 @@ class NearestNeighborMatcher(nn.Module):
             with torch.cuda.device(device):
                 lib = _cabi.load()
                 handle = self._handle(device)
-                ws = torch.empty(max(lib.nn_workspace_bytes(b, m, n, dim), 256), dtype=torch.uint8, device=device)
                 stream = torch.cuda.current_stream(device).cuda_stream
-                _cabi.check(lib.nn_match(handle, C.byref(cfg), C.byref(ins), C.byref(outs), ws.data_ptr(), ws.numel(),
-                                         stream), "nn_match")
+                if guide is None:
+                    ws = torch.empty(max(lib.nn_workspace_bytes(b, m, n, dim), 256), dtype=torch.uint8, device=device)
+                    _cabi.check(lib.nn_match(handle, C.byref(cfg), C.byref(ins), C.byref(outs), ws.data_ptr(),
+                                             ws.numel(), stream), "nn_match")
+                else:
+                    g = _cabi.NnGuide(kind, ptr(model), ptr(ok), ptr(kp0), ptr(kp1), float(max_error))
+                    ws = torch.empty(max(lib.nn_guided_workspace_bytes(b, m, n, dim), 256), dtype=torch.uint8,
+                                     device=device)
+                    _cabi.check(lib.nn_match_guided(handle, C.byref(cfg), C.byref(ins), C.byref(g), C.byref(outs),
+                                                    ws.data_ptr(), ws.numel(), stream), "nn_match_guided")
         counts = n_matches.tolist()  # the one read-back: the lengths of the per-pair lists
         out["matches"] = [pairs[i, : counts[i]] for i in range(b)]
         out["scores"] = [pscores[i, : counts[i]] for i in range(b)]
