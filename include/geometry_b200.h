@@ -375,6 +375,59 @@
  *      0.  Deviations from PoseLib and COLMAP: local optimisation runs at most once per chunk rather than at every new
  *      best, so the launch sequence is fixed and the result is deterministic; the score is quantised to integers;
  *      there is no non-minimal (EPnP) refit inside the LO and no PROSAC ordering.
+ *
+ * Affine and partial affine (geo_estimate_affine; oracle/affine_oracle.py restates it bit for bit): cv2.estimateAffine2D
+ * (GEO_AFFINE, x1 = A x0 with A = [[a00, a01, a02], [a10, a11, a12]], 6 degrees of freedom) and
+ * cv2.estimateAffinePartial2D (GEO_AFFINE_PARTIAL, A = [[a, -b, tx], [b, a, ty]]: rotation, uniform scale and
+ * translation, 4 degrees of freedom) with method=RANSAC and refineIters.  Expressions evaluate left to right as written;
+ * every multiply and add rounds on its own.
+ *
+ * AF1. Compaction and Hartley normalisation exactly as steps 1-2, with the same fixed-order sums.  The sample size is
+ *      s = 3 (GEO_AFFINE) or s = 2 (GEO_AFFINE_PARTIAL).
+ * AF2. Sampling as step 3 with that s.
+ * AF3. Minimal solvers, in double, on the normalised coordinates (x, y) of image 0 and (u, v) of image 1, points in
+ *      sample order.
+ *      Affine: Cramer's rule on the differences to point 0: dxj = x1 - x0, dyj = y1 - y0, dxk = x2 - x0,
+ *      dyk = y2 - y0, D = dxj*dyk - dxk*dyj, and likewise duj, dvj, duk, dvk of image 1.  The sample is rejected when
+ *      the triple is collinear in either image by step 4's rule (|D| <= GEO_FLT_EPS * (((|dxj| + |dyj|) + |dxk|) +
+ *      |dyk|), and the same with (duj, dvj, duk, dvk) and duj*dvk - duk*dvj: OpenCV's haveCollinearPoints).  Then
+ *      a = (duj*dyk - duk*dyj) / D, b = (dxj*duk - dxk*duj) / D, c = u0 - (a*x0 + b*y0),
+ *      d = (dvj*dyk - dvk*dyj) / D, e = (dxj*dvk - dxk*dvj) / D, f = v0 - (d*x0 + e*y0): An = [[a, b, c], [d, e, f],
+ *      [0, 0, 1]].  The pixel model is T1^-1 An T0 by step 4's T0, T1^-1 and 3x3 products, whose bottom row is
+ *      exactly (0, 0, 1); it is not rescaled.
+ *      Partial: dx = x1 - x0, dy = y1 - y0, du = u1 - u0, dv = v1 - v0, dd = dx*dx + dy*dy.  The sample is degenerate
+ *      when dd > 0 fails (coincident points in image 0) or du == 0 and dv == 0 (coincident points in image 1: a zero
+ *      scale).  Else a = (dx*du + dy*dv) / dd, b = (dx*dv - dy*du) / dd, tx = u0 - (a*x0 - b*y0),
+ *      ty = v0 - (b*x0 + a*y0).  T0 and T1 are isotropic, so the pixel model keeps the similarity form: with
+ *      r = 1.0 / s1, kx = s0*cx0 and ky = s0*cy0, a' = (a*s0)*r, b' = (b*s0)*r,
+ *      tx' = (tx - (a*kx - b*ky))*r + cx1, ty' = (ty - (b*kx + a*ky))*r + cy1, and A = [[a', -b', tx'], [b', a', ty']]
+ *      with A[0][1] the exact negation of A[1][0] and A[1][1] a copy of A[0][0].
+ *      Either kind: a sample whose normalised parameters or pixel model have a non-finite entry is degenerate.
+ * AF4. Scoring as step 5's H error in fp32 on the model rounded to float with h6 = h7 = 0 and h8 = 1: then
+ *      w = 1 / ((0*x0 + 0*y0) + 1) is exactly 1, so err = dx*dx + dy*dy with dx = x1 - ((a00*x0 + a01*y0) + a02),
+ *      dy = y1 - ((a10*x0 + a11*y0) + a12), bit for bit.  An inlier has err < (float)(threshold * threshold).  The
+ *      score is the inlier count; ties go to the lowest hypothesis.
+ * AF5. Stopping as step 6 with s = 3 or 2.
+ * AF6. Refinement.  With at least s inliers and refine_iters > 0, refine_iters Levenberg-Marquardt steps in double on
+ *      the untruncated squared transfer error of the best hypothesis's inliers (its AF4 inliers, a fixed set), from
+ *      its normalised parameters.  Per inlier, on the normalised coordinates of AF3: affine rx = ((a*x + b*y) + c) - u,
+ *      ry = ((d*x + e*y) + f) - v, Jacobian rows jx = (x, y, 1, 0, 0, 0), jy = (0, 0, 0, x, y, 1); partial
+ *      rx = ((a*x - b*y) + tx) - u, ry = ((b*x + a*y) + ty) - v, jx = (x, -y, 1, 0), jy = (y, x, 0, 1).  The terms
+ *      jx_i*jx_j + jy_i*jy_j (i <= j in row order), jx_i*rx + jy_i*ry and rx*rx + ry*ry are each summed over the
+ *      points in the order of step 2, other points adding 0: J^T J, J^T r and the cost.  A step solves A7's system
+ *      (damping, Cholesky, right-hand side -J^T r; 6x6 or 4x4), moves the parameters to p + delta, and is taken only
+ *      if the cost there is strictly lower; lambda starts at GEO_LO_LAMBDA0 and falls or rises tenfold: A7's
+ *      schedule.  An isotropic T1 scales every residual by s1, so the minimiser is the pixel one; the residual is
+ *      linear in the parameters, so the steps converge to the linear least-squares fit on those inliers.  The refined
+ *      parameters give the pixel model as AF3, which is re-scored as AF4 and replaces the hypothesis unless it has
+ *      fewer inliers.
+ * AF7. Outputs: model [B, 3, 3] the final A with the bottom row (0, 0, 1); inliers the points with err < thr2 under it
+ *      rounded to float, num_inliers their number; best_hypothesis the hypothesis the final model grew from;
+ *      num_hypotheses the samples drawn.  A pair fails (success 0, model all zero, no inliers, best_hypothesis -1)
+ *      when n < s, when its normalisation fails, or when every sample is degenerate.  Differences from OpenCV: inliers
+ *      are those of the final (refined) model, where OpenCV returns the minimal model's mask; stopping is checked per
+ *      chunk of GEO_CHUNK; the sampler is step 3's counter hash; there is no special case when n equals s; OpenCV's
+ *      refinement is its own Levenberg-Marquardt solver on the same inliers, converging to the same least-squares fit.
  */
 #ifndef GEOMETRY_B200_H
 #define GEOMETRY_B200_H
@@ -567,6 +620,26 @@ typedef struct GeoLoPnpOutputs {
 LG_API size_t geo_lo_pnp_workspace_bytes(int32_t B, int32_t M, int32_t max_iters);
 LG_API int geo_absolute_pose_lo(const GeoPnpConfig* cfg, const GeoPnpInputs* in, GeoLoPnpOutputs* out,
                                 void* workspace, size_t workspace_bytes, void* stream);
+
+#define GEO_AFFINE 3
+#define GEO_AFFINE_PARTIAL 4
+#define GEO_AFFINE_MAX_REFINE 100
+
+typedef struct GeoAffineConfig {
+  int32_t abi_version;  /* GEO_ABI_VERSION */
+  int32_t model;        /* GEO_AFFINE or GEO_AFFINE_PARTIAL */
+  int32_t max_iters;    /* hypotheses per pair, in [1, GEO_MAX_ITERS] */
+  uint32_t seed;
+  int32_t refine_iters; /* Levenberg-Marquardt steps, in [0, GEO_AFFINE_MAX_REFINE]; 0: none */
+  int32_t reserved;
+  double threshold;     /* pixels, > 0: transfer error */
+  double confidence;    /* in [0, 1] */
+} GeoAffineConfig;
+
+/* Affine and partial affine (steps AF1-AF7): out->model is [B, 3, 3] with the bottom row (0, 0, 1). */
+LG_API size_t geo_affine_workspace_bytes(int32_t B, int32_t M, int32_t max_iters);
+LG_API int geo_estimate_affine(const GeoAffineConfig* cfg, const GeoInputs* in, GeoOutputs* out, void* workspace,
+                               size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }

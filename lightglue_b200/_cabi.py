@@ -24,6 +24,7 @@ DHN_LAYOUT_BUFFERS = 16  # buffers of dhn_workspace_layout
 GEO_ABI_VERSION = 1  # include/geometry_b200.h
 GEO_HOMOGRAPHY, GEO_FUNDAMENTAL, GEO_ESSENTIAL = 0, 1, 2
 GEO_LO_QSCALE, GEO_LO_MAX_MATCHES = 65536, (1 << 20) - 1
+GEO_AFFINE, GEO_AFFINE_PARTIAL, GEO_AFFINE_MAX_REFINE = 3, 4, 100
 NN_ABI_VERSION = 1  # include/nn_b200.h
 NN_MIN_DIM, NN_MAX_DIM, NN_GROUP_ROWS = 64, 512, 32768
 NN_GUIDE_H, NN_GUIDE_F = 0, 1
@@ -175,6 +176,13 @@ class GeoLoPnpOutputs(C.Structure):
     _fields_ = [("pnp", GeoPnpOutputs), ("num_local_optimizations", C.c_void_p), ("cost", C.c_void_p)]
 
 
+class GeoAffineConfig(C.Structure):
+    _fields_ = [
+        ("abi_version", C.c_int32), ("model", C.c_int32), ("max_iters", C.c_int32), ("seed", C.c_uint32),
+        ("refine_iters", C.c_int32), ("reserved", C.c_int32), ("threshold", C.c_double), ("confidence", C.c_double),
+    ]
+
+
 class NnConfig(C.Structure):
     _fields_ = [
         ("abi_version", C.c_int32), ("dim", C.c_int32), ("mutual_check", C.c_int32), ("ratio_thresh", C.c_float),
@@ -291,6 +299,9 @@ GEO_PROTOTYPES = {  # include/geometry_b200.h
     "geo_lo_pnp_workspace_bytes": (_SZ, [_I32, _I32, _I32]),
     "geo_absolute_pose_lo": (C.c_int, [C.POINTER(GeoPnpConfig), C.POINTER(GeoPnpInputs), C.POINTER(GeoLoPnpOutputs),
                                        _VP, _SZ, _VP]),
+    "geo_affine_workspace_bytes": (_SZ, [_I32, _I32, _I32]),
+    "geo_estimate_affine": (C.c_int, [C.POINTER(GeoAffineConfig), C.POINTER(GeoInputs), C.POINTER(GeoOutputs), _VP,
+                                      _SZ, _VP]),
 }
 NN_PROTOTYPES = {  # include/nn_b200.h
     "nn_create": (C.c_int, [_VP, _HANDLE_OUT]),

@@ -1,16 +1,17 @@
-"""Geometric verification on the GPU: batched RANSAC homography and fundamental-matrix, relative-pose and
-absolute-pose estimation on the matcher's output, each plain and LO-RANSAC (C ABI ``include/geometry_b200.h``, CUDA
-``csrc/geo_api.cu``, ``csrc/lo_hf_api.cu``, ``csrc/pose_api.cu``, ``csrc/lo_pose_api.cu``, ``csrc/pnp_api.cu`` and
-``csrc/lo_pnp_api.cu``).
+"""Geometric verification on the GPU: batched RANSAC homography and fundamental-matrix, relative-pose,
+absolute-pose and affine estimation on the matcher's output, each of the first four plain and LO-RANSAC (C ABI
+``include/geometry_b200.h``, CUDA ``csrc/geo_api.cu``, ``csrc/lo_hf_api.cu``, ``csrc/pose_api.cu``,
+``csrc/lo_pose_api.cu``, ``csrc/pnp_api.cu``, ``csrc/lo_pnp_api.cu`` and ``csrc/affine_api.cu``).
 
-All eight functions take ``matches0`` [B, M] int64 exactly as ``LightGlue.forward``, ``PendingMatch.tensors`` and
+All ten functions take ``matches0`` [B, M] int64 exactly as ``LightGlue.forward``, ``PendingMatch.tensors`` and
 ``match_ragged`` give it (-1 or any index outside [0, N) is unmatched), run every pair of the batch in one call on the
 current stream, and return device tensors of fixed shapes without synchronising with the host, so a call can follow a
 matcher forward with no read-back in between, or be captured in a CUDA graph.  A match whose keypoint in either image,
 or whose 3D point, has a NaN or infinite coordinate is invalid like an unmatched row: it is never an inlier and does
 not count towards the pair's matches.  Parameter names and defaults are those of
 ``cv2.findHomography(RANSAC)``, ``cv2.findFundamentalMat(FM_RANSAC)``, ``cv2.findEssentialMat(RANSAC)`` with
-``cv2.recoverPose``, and ``cv2.solvePnPRansac``.
+``cv2.recoverPose``, ``cv2.solvePnPRansac``, and ``cv2.estimateAffine2D`` and ``cv2.estimateAffinePartial2D`` with
+``method=cv2.RANSAC``.
 
 ``find_homography`` and ``find_fundamental`` return a dict: ``H`` or ``F`` [B, 3, 3] float64 (H scaled to H[2, 2] = 1; F to unit Frobenius norm with its largest
 entry positive), ``inliers`` [B, M] bool, ``num_inliers`` [B] int32, ``success`` [B] bool, and the diagnostics
@@ -18,7 +19,8 @@ entry positive), ``inliers`` [B, M] bool, ``num_inliers`` [B] int32, ``success``
 the sample size, 4 or 8, or no non-degenerate hypothesis) has ``success`` False, a zero model and no inliers.
 ``find_homography_lo`` and ``find_fundamental_lo`` return the keys of ``find_homography`` and ``find_fundamental`` plus
 ``num_local_optimizations`` and ``cost``; so do ``estimate_relative_pose_lo`` and ``estimate_absolute_pose_lo`` with
-those of ``estimate_relative_pose`` and ``estimate_absolute_pose``.
+those of ``estimate_relative_pose`` and ``estimate_absolute_pose``.  ``estimate_affine_2d`` and
+``estimate_affine_partial_2d`` return those of ``find_homography`` with ``A`` [B, 2, 3] in place of ``H``.
 """
 from __future__ import annotations
 
@@ -317,3 +319,60 @@ def _absolute_pose(lo: bool, kpts0, points3d1, matches0, K0, ransac_reproj_thres
     if lo:
         return _run("geo_absolute_pose_lo", "geo_lo_pnp_workspace_bytes", shapes, device, b, m, max_iters, make_args)
     return _run("geo_absolute_pose", "geo_pnp_workspace_bytes", shapes, device, b, m, max_iters, make_args)
+
+
+def _affine(kind: int, kpts0, kpts1, matches0, threshold, max_iters, confidence, refine_iters, seed) -> dict:
+    _check_inputs(kpts0, kpts1, matches0)
+    _check_params(threshold, max_iters, confidence, seed)
+    if (not isinstance(refine_iters, int) or isinstance(refine_iters, bool)
+            or not 0 <= refine_iters <= _cabi.GEO_AFFINE_MAX_REFINE):
+        raise ValueError(f"refine_iters={refine_iters!r}: an int in [0, {_cabi.GEO_AFFINE_MAX_REFINE}]")
+    device = kpts0.device
+    b, m, n = kpts0.shape[0], kpts0.shape[1], kpts1.shape[1]
+    k0 = kpts0.detach().to(torch.float32).contiguous()
+    k1 = kpts1.detach().to(torch.float32).contiguous()
+    m0 = matches0.detach().contiguous()
+    i32, bl = torch.int32, torch.bool
+    shapes = {"model": ((b, 3, 3), torch.float64), "inliers": ((b, m), bl), "num_inliers": ((b,), i32),
+              "success": ((b,), bl), "best_hypothesis": ((b,), i32), "num_hypotheses": ((b,), i32)}
+
+    def make_args(out):
+        cfg = _cabi.GeoAffineConfig(_cabi.GEO_ABI_VERSION, kind, max_iters, seed, refine_iters, 0, float(threshold),
+                                    float(confidence))
+        ins = _cabi.GeoInputs(b, m, n, k0.data_ptr(), k1.data_ptr(), m0.data_ptr())
+        return cfg, ins, _cabi.GeoOutputs(*(out[k].data_ptr() for k in shapes))
+
+    out = _run("geo_estimate_affine", "geo_affine_workspace_bytes", shapes, device, b, m, max_iters, make_args)
+    return {"A": out.pop("model")[:, :2].contiguous(), **out}
+
+
+def estimate_affine_2d(kpts0: torch.Tensor, kpts1: torch.Tensor, matches0: torch.Tensor,
+                       ransac_reproj_threshold: float = 3.0, max_iters: int = 2000, confidence: float = 0.99,
+                       refine_iters: int = 10, seed: int = 0) -> dict:
+    """RANSAC affine transform per pair (6 degrees of freedom) from 3-point samples, mapping kpts0 to kpts1, then
+    ``refine_iters`` Levenberg-Marquardt steps on the best sample's inliers (0: none): an inlier has a squared transfer
+    error below ``ransac_reproj_threshold ** 2``.  Defaults of ``cv2.estimateAffine2D(method=cv2.RANSAC)``.
+
+    Returns ``A`` [B, 2, 3] float64 (OpenCV's layout: x1 = A [x0, y0, 1]^T); ``inliers`` [B, M] bool and
+    ``num_inliers`` [B] int32 of the final A (OpenCV returns the minimal sample's mask); ``success`` [B] bool; and the
+    diagnostics ``best_hypothesis`` [B] int32 (-1 without one) and ``num_hypotheses`` [B] int32.  A pair with fewer
+    than 3 valid matches, a failed normalisation or only degenerate (collinear) samples has ``success`` False, a zero
+    A and no inliers.  ``torch.cat([A, row], 1)`` with ``row = [[0, 0, 1]]`` is a homography whose transfer error, as
+    ``find_homography`` and ``NearestNeighborMatcher(...)(data, H=...)`` test it, equals this inlier test bit for
+    bit."""
+    return _affine(_cabi.GEO_AFFINE, kpts0, kpts1, matches0, ransac_reproj_threshold, max_iters, confidence,
+                   refine_iters, seed)
+
+
+def estimate_affine_partial_2d(kpts0: torch.Tensor, kpts1: torch.Tensor, matches0: torch.Tensor,
+                               ransac_reproj_threshold: float = 3.0, max_iters: int = 2000, confidence: float = 0.99,
+                               refine_iters: int = 10, seed: int = 0) -> dict:
+    """RANSAC similarity transform per pair (rotation, uniform scale and translation: 4 degrees of freedom) from
+    2-point samples, then ``refine_iters`` Levenberg-Marquardt steps on the best sample's inliers.  Defaults of
+    ``cv2.estimateAffinePartial2D(method=cv2.RANSAC)``.
+
+    Returns the keys of ``estimate_affine_2d``, with ``A`` exactly [[a, -b, tx], [b, a, ty]]: ``A[:, 0, 0]`` equals
+    ``A[:, 1, 1]`` and ``A[:, 0, 1]`` equals ``-A[:, 1, 0]`` bit for bit.  A pair with fewer than 2 valid matches or
+    only degenerate samples (coincident points in either image) fails as in ``estimate_affine_2d``."""
+    return _affine(_cabi.GEO_AFFINE_PARTIAL, kpts0, kpts1, matches0, ransac_reproj_threshold, max_iters, confidence,
+                   refine_iters, seed)
