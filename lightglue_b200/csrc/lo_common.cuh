@@ -1,12 +1,13 @@
-// The LO-RANSAC pieces shared by the relative pose (lo_pose_api.cu, header steps L3 and L7), the homography and the
-// fundamental matrix (lo_hf_api.cu, LH3 and LH7, LF3 and LF7) and the absolute pose (lo_pnp_api.cu, LA3 and LA7), all
-// compiled with -fmad=false: the packed MSAC score term, the fixed-order sums of the Levenberg-Marquardt terms, and one
-// LM loop and re-score over a model policy.
+// The LO-RANSAC pieces shared by the relative pose (lo_pose_api.cu, header steps L1-L8), the homography and the
+// fundamental matrix (lo_hf_api.cu, LH1-LH8 and LF1-LF8) and the absolute pose (lo_pnp_api.cu, LA1-LA8), all compiled
+// with -fmad=false: the packed MSAC score term, the fixed-order sums of the Levenberg-Marquardt terms, one LM loop and
+// re-score over a model policy, and the schedule of L4-L6 and L8 that every LO estimator runs on it.
 #pragma once
 #include <cuda_runtime.h>
 
 #include "geo_common.cuh"
 #include "geo_lm.cuh"
+#include "ws_bump.h"
 
 namespace {
 
@@ -106,6 +107,190 @@ __device__ void lo_rescore(LoShared<Model>& s, const Pair& P, Points pts, int n,
   for (int k = tid; k < n; k += RED) acc += lo_term(Model::err(s.fm, pts[k]), thr2, w);
   if (acc) atomicAdd(&s.score, acc);
   __syncthreads();
+}
+
+// ---- the LO schedule (header steps L4-L6 and L8; LH, LF and LA likewise) ----
+
+struct LoPair {
+  double model[12];          // the pair's model: R | t (relative and absolute pose), the scaled pixel model (H, F)
+  unsigned long long score;  // its score
+  int count;                 // its inliers
+  int hr;                    // h * 16 + r of the solution that seeded it; -1: none yet
+  int nlo;                   // local optimisations adopted
+};
+
+struct LoWs {
+  LoPair* pair;             // [B]
+  unsigned long long* acc;  // [B, GEO_CHUNK, SOLS] count << 40 | score of the current chunk's solutions
+};
+
+// The kernels' arguments: Base is the estimator's RANSAC arguments (GeoArgs, PoseArgs or PnpArgs)
+template <class Base>
+struct LoArgs {
+  Base p;
+  LoWs l;
+  int32_t* num_lo;
+  int64_t* cost;
+};
+
+// The estimator's workspace, then the LO one
+template <class Est>
+size_t lo_carve(char* base, int B, int M, LoArgs<typename Est::Base>* a) {
+  WsBump b{base, carve(base, B, M, &a->p.w)};
+  a->l.pair = b.take<LoPair>(B);
+  a->l.acc = b.take<unsigned long long>((size_t)B * GEO_CHUNK * Est::SOLS);
+  return b.bytes();
+}
+
+template <class Est>
+size_t lo_workspace_bytes(int B, int M) {
+  if (B < 0 || M < 0) return 0;
+  LoArgs<typename Est::Base> a;
+  return lo_carve<Est>(nullptr, B, M, &a) + 256;
+}
+
+// Pair b's LO state before its first chunk; every hyp kernel calls it
+__device__ __forceinline__ void lo_reset(const LoWs& l, int b, int c) {
+  if (c == 0 && threadIdx.x == 0) {
+    LoPair& L = l.pair[b];
+    L.score = 0;
+    L.count = 0;
+    L.hr = -1;
+    L.nlo = 0;
+  }
+}
+
+// The schedule runs over Est, the estimator's model policy (LoShared above) with:
+//   Base, its RANSAC arguments (a.p.w.pair[b] the pair, a.p.out the outputs); Score, its geo_score_kernel policy; S,
+//   the points per sample; SOLS, the solutions per sample;
+//   points(a, b), consts(a, b) and thr2(a, b), pair b's points, constants and squared threshold as the LM loop reads
+//   them;
+//   seed(s, a, b, hr, m, L, t), the LM start s.x of solution hr (index m of acc) and L.model of it (every thread; a
+//   barrier follows);
+//   store(s, L), the re-scored model of s into L.model (thread 0);
+//   load(s, a, b, L, t), the LM start of L.model (every thread; a barrier follows);
+//   restore(s, a, b, L, t), L's model, score and count as the re-scored model of s (every thread; ends on a barrier);
+//   fail(a, b, t), the model fields of a pair without a model, o.inliers already cleared (every thread);
+//   write(s, a, b, t), the masks and model fields of the re-scored model of s (every thread).
+
+// L4 and L5 after chunk c: the chunk's lowest (score, h, r); when it beats the pair's model, LM from it and a re-score,
+// adopted at a strictly lower score; then the adaptive stop.  A stopped pair's CTA returns at once.
+template <class Est>
+__global__ void __launch_bounds__(RED, 1) lo_chunk_kernel(LoArgs<typename Est::Base> a, int c) {
+  const int b = blockIdx.x, t = threadIdx.x;
+  auto& P = a.p.w.pair[b];
+  if (P.stop) return;
+  LoPair& L = a.l.pair[b];
+  __shared__ LoShared<Est> s;
+  if (t == 0) s.key = ~0ull;
+  __syncthreads();
+  if (t < GEO_CHUNK) {
+    const long slot = (long)b * GEO_CHUNK + t;
+    const int ns = geo_models(a.p.w, slot);
+    const unsigned h = c * GEO_CHUNK + t;
+    for (int r = 0; r < ns; ++r)
+      atomicMin(&s.key, (a.l.acc[slot * Est::SOLS + r] & LO_SCORE_MASK) << 28 | (h * 16u + (unsigned)r));
+  }
+  __syncthreads();
+  const unsigned long long key = s.key;
+  if (t == 0) s.take = key != ~0ull && (L.hr < 0 || (key >> 28) < L.score);
+  __syncthreads();
+  if (s.take) {
+    const unsigned hr = (unsigned)(key & 0xfffffffu);
+    const long m = ((long)b * GEO_CHUNK + (hr >> 4) - c * GEO_CHUNK) * Est::SOLS + (hr & 15);
+    Est::seed(s, a, b, hr, m, L, t);
+    if (t == 0) {
+      L.score = key >> 28;
+      L.count = (int)(a.l.acc[m] >> 40);
+      L.hr = (int)hr;
+    }
+    __syncthreads();
+    const auto pts = Est::points(a, b);
+    const float thr2 = Est::thr2(a, b);
+    lo_refine(s, Est::consts(a, b), pts, P.n, (double)thr2, GEO_LO_STEPS, t);
+    lo_rescore(s, Est::consts(a, b), pts, P.n, thr2, t);
+    if (t == 0 && (s.score & LO_SCORE_MASK) < L.score) {
+      Est::store(s, L);
+      L.score = s.score & LO_SCORE_MASK;
+      L.count = (int)(s.score >> 40);
+      L.nlo = L.nlo + 1;
+    }
+  }
+  if (t == 0) {
+    const int drawn = min((c + 1) * GEO_CHUNK, a.p.max_iters);
+    const int cnt = L.hr >= 0 ? L.count : 0;
+    P.drawn = drawn;
+    P.stop = drawn >= a.p.max_iters ||
+             drawn >= update_num_iters(a.p.confidence, 1.0 - (double)cnt / P.n, Est::S, a.p.max_iters);
+  }
+}
+
+// L6 and L8: the final refinement, kept unless its score rises, and the outputs
+template <class Est>
+__global__ void __launch_bounds__(RED, 1) lo_final_kernel(LoArgs<typename Est::Base> a) {
+  const int b = blockIdx.x, t = threadIdx.x;
+  const auto& P = a.p.w.pair[b];
+  const LoPair& L = a.l.pair[b];
+  const auto& o = a.p.out;
+  if (!P.ok || L.hr < 0) {
+    for (int i = t; i < a.p.M; i += RED) o.inliers[(long)b * a.p.M + i] = 0;
+    Est::fail(a, b, t);
+    if (t == 0) {
+      o.num_inliers[b] = 0;
+      o.success[b] = 0;
+      o.best_hypothesis[b] = -1;
+      if constexpr (Est::SOLS > 1) o.best_solution[b] = -1;  // only an estimator with several solutions reports one
+      o.num_hypotheses[b] = P.drawn;
+      a.num_lo[b] = 0;
+      a.cost[b] = 0;
+    }
+    return;
+  }
+  __shared__ LoShared<Est> s;
+  const auto pts = Est::points(a, b);
+  const float thr2 = Est::thr2(a, b);
+  Est::load(s, a, b, L, t);
+  __syncthreads();
+  lo_refine(s, Est::consts(a, b), pts, P.n, (double)thr2, GEO_LO_FINAL_STEPS, t);
+  lo_rescore(s, Est::consts(a, b), pts, P.n, thr2, t);
+  if (t == 0) s.take = (s.score & LO_SCORE_MASK) > L.score;
+  __syncthreads();
+  if (s.take) Est::restore(s, a, b, L, t);
+  Est::write(s, a, b, t);
+  if (t == 0) {
+    o.num_inliers[b] = (int)(s.score >> 40);
+    o.success[b] = 1;
+    o.best_hypothesis[b] = L.hr >> 4;
+    if constexpr (Est::SOLS > 1) o.best_solution[b] = L.hr & 15;
+    o.num_hypotheses[b] = P.drawn;
+    a.num_lo[b] = L.nlo;
+    a.cost[b] = (int64_t)(s.score & LO_SCORE_MASK);
+  }
+}
+
+// Every LO estimator's launches, all fixed by (B, M, max_iters): prepare, the estimator's compaction kernel; per chunk
+// of GEO_CHUNK samples, hyp (one CTA per pair, one thread per sample: the minimal solutions, fp32), geo_score_kernel
+// (count << 40 | MSAC score of every solution) and lo_chunk_kernel (one CTA per pair); then lo_final_kernel.
+template <class Est, class Base>
+int lo_launch(const Base& p, int32_t* num_lo, int64_t* cost, void* workspace, void (*prepare)(Base),
+              void (*hyp)(LoArgs<Base>, int), void* stream_) {
+  LoArgs<Base> a{p, {}, num_lo, cost};
+  lo_carve<Est>(geo_workspace_base(workspace), p.B, p.M, &a);
+  const int splits = geo_score_splits(p.B, p.M);
+  const cudaStream_t stream = (cudaStream_t)stream_;
+  prepare<<<p.B, 1024, 0, stream>>>(a.p);
+  LG_CHECK_LAUNCH();
+  for (int c = 0; c < p.chunks; ++c) {
+    hyp<<<p.B, GEO_CHUNK, 0, stream>>>(a, c);
+    LG_CHECK_LAUNCH();
+    geo_score_kernel<typename Est::Score><<<dim3(p.B, splits), GEO_CHUNK, 0, stream>>>(a);
+    LG_CHECK_LAUNCH();
+    lo_chunk_kernel<Est><<<p.B, RED, 0, stream>>>(a, c);
+    LG_CHECK_LAUNCH();
+  }
+  lo_final_kernel<Est><<<p.B, RED, 0, stream>>>(a);
+  LG_CHECK_LAUNCH();
+  return 0;
 }
 
 }  // namespace

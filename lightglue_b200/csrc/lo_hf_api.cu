@@ -1,19 +1,11 @@
 // Batched LO-RANSAC homography and fundamental matrix on the matcher's output: MSAC-scored four-point (H) or
 // eight-point (F) sampling with Levenberg-Marquardt local optimisation and a final refinement (include/geometry_b200.h,
 // steps LH1-LH8 and LF1-LF8).  H is refined at unit norm in the tangent space of the sphere, F at rank 2 in its
-// orthonormal representation (U, V, sigma).
-//
-// Launches, all fixed by (B, M, max_iters):
-//   prepare  geo_api.cu's compaction and Hartley normalisation kernel (geo_hf.cuh)
-//   per chunk of GEO_CHUNK samples:
-//     hyp    one CTA per pair, one thread per sample: the minimal solve of step 4, fp32
-//     score  (B, splits) CTAs: each streams a slice of the pair's points through shared memory against the chunk's
-//            models, one thread per sample, and adds count << 40 | MSAC score with one 64-bit atomic per sample
-//     lo     one CTA per pair: the chunk's lowest (score, h); when it beats the pair's model, LM on the truncated
-//            transfer (H) or Sampson (F) cost and a re-score; then the adaptive stop.  Otherwise it returns at once.
-//   final    one CTA per pair: the final LM refinement, the model and its inliers
-// A stopped pair's CTAs return at once.  Compiled with -fmad=false: oracle/lo_homography_oracle.py and
-// oracle/lo_fundamental_oracle.py take the same steps.
+// orthonormal representation (U, V, sigma).  Both run on lo_common.cuh's schedule: geo_api.cu's compaction and
+// Hartley normalisation kernel prepares the pair; hyp makes step 4's minimal solve, one model per sample (r = 0); a
+// local optimisation starts from the hypothesis solved again in double and runs LM on the truncated transfer (H) or
+// Sampson (F) cost.  Compiled with -fmad=false: oracle/lo_homography_oracle.py and oracle/lo_fundamental_oracle.py take
+// the same steps.
 #include <stdint.h>
 
 #include "geo_hf.cuh"
@@ -22,67 +14,34 @@
 
 namespace {
 
-struct LoHfPair {
-  double model[9];           // the pair's model in pixels, scaled as step 4
-  unsigned long long score;  // its LH3 / LF3 score
-  int count;                 // its inliers
-  int h;                     // the hypothesis that seeded it; -1: none yet
-  int nlo;                   // local optimisations adopted
-};
-
-struct LoHfWs {
-  LoHfPair* pair;           // [B]
-  unsigned long long* acc;  // [B, GEO_CHUNK] count << 40 | score of the current chunk's hypotheses
-};
-
-size_t lohf_carve(char* base, int B, int M, GeoWs* w, LoHfWs* l) {
-  WsBump b{base, carve(base, B, M, w)};
-  l->pair = b.take<LoHfPair>(B);
-  l->acc = b.take<unsigned long long>((size_t)B * GEO_CHUNK);
-  return b.bytes();
-}
-
-struct LoHfArgs {
-  GeoArgs g;
-  LoHfWs l;
-  int32_t* num_lo;
-  int64_t* cost;
-};
-
-// Step 4's hypotheses of chunk c (a.g.kind and a.g.s pick H or F), one thread per sample
-__global__ void __launch_bounds__(GEO_CHUNK, 1) lohf_hyp_kernel(LoHfArgs a, int c) {
+// Step 4's hypotheses of chunk c (a.p.kind and a.p.s pick H or F), one thread per sample
+__global__ void __launch_bounds__(GEO_CHUNK, 1) lohf_hyp_kernel(LoArgs<GeoArgs> a, int c) {
   const int b = blockIdx.x, t = threadIdx.x;
-  if (c == 0 && t == 0) {
-    LoHfPair& L = a.l.pair[b];
-    L.score = 0;
-    L.count = 0;
-    L.h = -1;
-    L.nlo = 0;
-  }
-  const GeoPair& P = a.g.w.pair[b];
+  lo_reset(a.l, b, c);
+  const GeoPair& P = a.p.w.pair[b];
   const int h = c * GEO_CHUNK + t;
   double m[9];
-  const bool ok = P.stop == 0 && h < a.g.max_iters && geo_hypothesis(a.g, P, a.g.w.pts + (long)b * a.g.M, h, m);
+  const bool ok = P.stop == 0 && h < a.p.max_iters && geo_hypothesis(a.p, P, a.p.w.pts + (long)b * a.p.M, h, m);
   if (ok) {
-    float* hm = a.g.w.hyp + ((long)b * GEO_CHUNK + t) * 9;
+    float* hm = a.p.w.hyp + ((long)b * GEO_CHUNK + t) * 9;
     for (int i = 0; i < 9; ++i) hm[i] = (float)m[i];
     a.l.acc[(long)b * GEO_CHUNK + t] = 0;
   }
-  a.g.w.count[(long)b * GEO_CHUNK + t] = ok ? 0 : -1;
+  a.p.w.count[(long)b * GEO_CHUNK + t] = ok ? 0 : -1;
 }
 
 // The chunk's LH3 / LF3 scores, count << 40 | MSAC score
 template <int KIND>
 struct LoHfScore {
-  using Args = LoHfArgs;
+  using Args = LoArgs<GeoArgs>;
   using Acc = unsigned long long;
   static constexpr int SOLS = 1, NF = 9, K = 1, TILE = ::TILE;
-  static __device__ const GeoWs& ws(const LoHfArgs& a) { return a.g.w; }
+  static __device__ const GeoWs& ws(const Args& a) { return a.p.w; }
   const float4* src[K];
   unsigned long long* sums;
   float thr2, w;
-  __device__ LoHfScore(const LoHfArgs& a, const GeoPair&, int b)
-      : src{a.g.w.pts + (long)b * a.g.M}, sums(a.l.acc), thr2(a.g.thr2), w((float)GEO_LO_QSCALE / a.g.thr2) {}
+  __device__ LoHfScore(const Args& a, const GeoPair&, int b)
+      : src{a.p.w.pts + (long)b * a.p.M}, sums(a.l.acc), thr2(a.p.thr2), w((float)GEO_LO_QSCALE / a.p.thr2) {}
   __device__ unsigned long long term(const float* h, const float4* p) const {
     return lo_term(geo_err(KIND, h, p[0]), thr2, w);
   }
@@ -123,9 +82,67 @@ __device__ void householder_basis(const double* Hn, double (*B)[9]) {
   }
 }
 
-// The homography for lo_common.cuh's LM loop and re-score: x = Hn, the unit-norm normalised model (header step LH7)
-struct HomographyLo {
-  static constexpr int KIND = GEO_HOMOGRAPHY, DOF = 8, TERMS = 45, GROUP = 15, NP = 9, NF = 9;
+// The schedule hooks of the homography and the fundamental matrix (lo_common.cuh), Model one of the two: L.model is the
+// scaled pixel model, the LM start Model::start of it
+template <class Model>
+struct HfLo {
+  using Base = GeoArgs;
+  using Args = LoArgs<GeoArgs>;
+  static constexpr int SOLS = 1;
+
+  static __device__ const float4* points(const Args& a, int b) { return a.p.w.pts + (long)b * a.p.M; }
+  static __device__ const GeoPair& consts(const Args& a, int b) { return a.p.w.pair[b]; }
+  static __device__ float thr2(const Args& a, int) { return a.p.thr2; }
+
+  // LH4 / LF4: hypothesis h solved again in double
+  static __device__ void seed(LoShared<Model>& s, const Args& a, int b, unsigned hr, long, LoPair& L, int t) {
+    if (t == 0) {
+      geo_hypothesis(a.p, a.p.w.pair[b], points(a, b), hr >> 4, L.model);
+      Model::start(s, a.p.w.pair[b], L.model);
+    }
+  }
+
+  static __device__ void store(LoShared<Model>& s, LoPair& L) {
+    for (int i = 0; i < 9; ++i) L.model[i] = s.px[i];
+  }
+
+  static __device__ void load(LoShared<Model>& s, const Args& a, int b, const LoPair& L, int t) {
+    if (t == 0) Model::start(s, a.p.w.pair[b], L.model);
+  }
+
+  static __device__ void restore(LoShared<Model>& s, const Args&, int, const LoPair& L, int t) {
+    if (t == 0) {
+      for (int i = 0; i < 9; ++i) {
+        s.px[i] = L.model[i];
+        s.fm[i] = (float)L.model[i];
+      }
+      s.score = (unsigned long long)L.count * LO_COUNT_ONE + L.score;
+    }
+    __syncthreads();
+  }
+
+  static __device__ void fail(const Args& a, int b, int t) {
+    if (t < 9) a.p.out.model[(long)b * 9 + t] = 0.0;
+  }
+
+  // LH8 / LF8: the model and its inliers
+  static __device__ void write(LoShared<Model>& s, const Args& a, int b, int t) {
+    const float4* pts = points(a, b);
+    const int* idx = a.p.w.idx + (long)b * a.p.M;
+    uint8_t* inl = a.p.out.inliers + (long)b * a.p.M;
+    for (int i = t; i < a.p.M; i += RED) inl[i] = 0;
+    __syncthreads();
+    for (int k = t; k < a.p.w.pair[b].n; k += RED)
+      if (Model::err(s.fm, pts[k]) < a.p.thr2) inl[idx[k]] = 1;
+    if (t < 9) a.p.out.model[(long)b * 9 + t] = s.px[t];
+  }
+};
+
+// The homography for lo_common.cuh's LM loop, re-score and schedule: x = Hn, the unit-norm normalised model (header
+// step LH7)
+struct HomographyLo : HfLo<HomographyLo> {
+  static constexpr int KIND = GEO_HOMOGRAPHY, S = 4, DOF = 8, TERMS = 45, GROUP = 15, NP = 9, NF = 9;
+  using Score = LoHfScore<KIND>;
   struct Scratch {
     double basis[DOF][9];     // tangent basis at the model being summed or updated
     double Hu[9], G[DOF][9];  // T1^-1 Hn T0 and its derivatives along the basis
@@ -222,10 +239,12 @@ __device__ void compose(const double* x, double* Fn) {
     for (int b = 0; b < 3; ++b) Fn[a * 3 + b] = U[a * 3] * V[b * 3] + x[18] * U[a * 3 + 1] * V[b * 3 + 1];
 }
 
-// The fundamental matrix for lo_common.cuh's LM loop and re-score: x = U (0-8), V (9-17) and sig (18), the orthonormal
-// representation Fn = u1 v1^T + sig u2 v2^T of the normalised model, u_k, v_k columns of U, V (header step LF7)
-struct FundamentalLo {
-  static constexpr int KIND = GEO_FUNDAMENTAL, DOF = 7, TERMS = 36, GROUP = 18, NP = 19, NF = 9;
+// The fundamental matrix for lo_common.cuh's LM loop, re-score and schedule: x = U (0-8), V (9-17) and sig (18), the
+// orthonormal representation Fn = u1 v1^T + sig u2 v2^T of the normalised model, u_k, v_k columns of U, V (header step
+// LF7)
+struct FundamentalLo : HfLo<FundamentalLo> {
+  static constexpr int KIND = GEO_FUNDAMENTAL, S = 8, DOF = 7, TERMS = 36, GROUP = 18, NP = 19, NF = 9;
+  using Score = LoHfScore<KIND>;
   struct Scratch {
     double Fu[9], G[DOF][9];  // T1^T Fn T0 and the directions at Fn in pixels
   };
@@ -353,110 +372,9 @@ struct FundamentalLo {
   static __device__ __forceinline__ float err(const float* h, float4 p) { return geo_err(KIND, h, p); }
 };
 
-// After chunk c: the chunk's best hypothesis, the local optimisation when it beats the pair's model, the stop
+// geo_homography_lo and geo_fundamental_lo: name for the error strings
 template <class Model>
-__global__ void __launch_bounds__(RED, 1) lohf_lo_kernel(LoHfArgs a, int c) {
-  const int b = blockIdx.x, t = threadIdx.x;
-  GeoPair& P = a.g.w.pair[b];
-  if (P.stop) return;
-  LoHfPair& L = a.l.pair[b];
-  __shared__ LoShared<Model> s;
-  if (t == 0) s.key = ~0ull;
-  __syncthreads();
-  if (t < GEO_CHUNK && a.g.w.count[(long)b * GEO_CHUNK + t] >= 0)
-    atomicMin(&s.key, (a.l.acc[(long)b * GEO_CHUNK + t] & LO_SCORE_MASK) << 28 | (unsigned)(c * GEO_CHUNK + t));
-  __syncthreads();
-  const unsigned long long key = s.key;
-  const float4* pts = a.g.w.pts + (long)b * a.g.M;
-  if (t == 0) s.take = key != ~0ull && (L.h < 0 || (key >> 28) < L.score);
-  __syncthreads();
-  if (s.take) {
-    if (t == 0) {
-      const unsigned h = (unsigned)(key & 0xfffffffu);
-      geo_hypothesis(a.g, P, pts, h, L.model);
-      L.score = key >> 28;
-      L.count = (int)(a.l.acc[(long)b * GEO_CHUNK + h - c * GEO_CHUNK] >> 40);
-      L.h = (int)h;
-      Model::start(s, P, L.model);
-    }
-    __syncthreads();
-    lo_refine(s, P, pts, P.n, (double)a.g.thr2, GEO_LO_STEPS, t);
-    lo_rescore(s, P, pts, P.n, a.g.thr2, t);
-    if (t == 0 && (s.score & LO_SCORE_MASK) < L.score) {
-      for (int i = 0; i < 9; ++i) L.model[i] = s.px[i];
-      L.score = s.score & LO_SCORE_MASK;
-      L.count = (int)(s.score >> 40);
-      L.nlo = L.nlo + 1;
-    }
-  }
-  if (t == 0) {
-    const int drawn = min((c + 1) * GEO_CHUNK, a.g.max_iters);
-    const int cnt = L.h >= 0 ? L.count : 0;
-    P.drawn = drawn;
-    P.stop = drawn >= a.g.max_iters ||
-             drawn >= update_num_iters(a.g.confidence, 1.0 - (double)cnt / P.n, a.g.s, a.g.max_iters);
-  }
-}
-
-// Final refinement and the outputs (header steps LH6 and LH8, LF6 and LF8)
-template <class Model>
-__global__ void __launch_bounds__(RED, 1) lohf_final_kernel(LoHfArgs a) {
-  const int b = blockIdx.x, t = threadIdx.x;
-  const GeoPair& P = a.g.w.pair[b];
-  const LoHfPair& L = a.l.pair[b];
-  const GeoOutputs& o = a.g.out;
-  uint8_t* inl = o.inliers + (long)b * a.g.M;
-  for (int i = t; i < a.g.M; i += RED) inl[i] = 0;
-  if (!P.ok || L.h < 0) {
-    if (t < 9) o.model[(long)b * 9 + t] = 0.0;
-    if (t == 0) {
-      o.num_inliers[b] = 0;
-      o.success[b] = 0;
-      o.best_hypothesis[b] = -1;
-      o.num_hypotheses[b] = P.drawn;
-      a.num_lo[b] = 0;
-      a.cost[b] = 0;
-    }
-    return;
-  }
-  __shared__ LoShared<Model> s;
-  const float4* pts = a.g.w.pts + (long)b * a.g.M;
-  const int* idx = a.g.w.idx + (long)b * a.g.M;
-  if (t == 0) Model::start(s, P, L.model);
-  __syncthreads();
-  lo_refine(s, P, pts, P.n, (double)a.g.thr2, GEO_LO_FINAL_STEPS, t);
-  lo_rescore(s, P, pts, P.n, a.g.thr2, t);
-  if (t == 0 && (s.score & LO_SCORE_MASK) > L.score) {  // the refinement is kept unless its score rises
-    for (int i = 0; i < 9; ++i) {
-      s.px[i] = L.model[i];
-      s.fm[i] = (float)L.model[i];
-    }
-    s.score = (unsigned long long)L.count * LO_COUNT_ONE + L.score;
-  }
-  __syncthreads();
-  for (int k = t; k < P.n; k += RED)
-    if (Model::err(s.fm, pts[k]) < a.g.thr2) inl[idx[k]] = 1;
-  if (t < 9) o.model[(long)b * 9 + t] = s.px[t];
-  if (t == 0) {
-    o.num_inliers[b] = (int)(s.score >> 40);
-    o.success[b] = 1;
-    o.best_hypothesis[b] = L.h;
-    o.num_hypotheses[b] = P.drawn;
-    a.num_lo[b] = L.nlo;
-    a.cost[b] = (int64_t)(s.score & LO_SCORE_MASK);
-  }
-}
-
-size_t lohf_workspace_bytes(int B, int M) {
-  if (B < 0 || M < 0) return 0;
-  GeoWs w;
-  LoHfWs l;
-  return lohf_carve(nullptr, B, M, &w, &l) + 256;
-}
-
-// geo_homography_lo and geo_fundamental_lo: name for the error strings, s the points per sample
-template <class Model>
-int lohf_estimate(const char* name, int s, const GeoConfig* cfg, const GeoInputs* in, GeoLoOutputs* out,
+int lohf_estimate(const char* name, const GeoConfig* cfg, const GeoInputs* in, GeoLoOutputs* out,
                   void* workspace, size_t workspace_bytes, void* stream_) {
   int rc = geo_check_config(name, cfg, in, out, GEO_LO_MAX_MATCHES, [&] {
     return cfg->model == Model::KIND          ? nullptr
@@ -467,15 +385,13 @@ int lohf_estimate(const char* name, int s, const GeoConfig* cfg, const GeoInputs
     const GeoOutputs& o = out->geo;
     rc = geo_check_buffers(name, in, {o.model, o.num_inliers, o.success, o.best_hypothesis, o.num_hypotheses,
                                       out->num_local_optimizations, out->cost}, {o.inliers}, {}, in->kpts1,
-                           workspace, workspace_bytes, lohf_workspace_bytes(in->B, in->M));
+                           workspace, workspace_bytes, lo_workspace_bytes<Model>(in->B, in->M));
   }
   if (rc != GEO_RUN) return rc;
-  LoHfArgs a{};
-  lohf_carve(geo_workspace_base(workspace), in->B, in->M, &a.g.w, &a.l);
-  GeoArgs& g = a.g;
+  GeoArgs g{};
   g.B = in->B; g.M = in->M; g.N = in->N;
   g.kind = Model::KIND;
-  g.s = s;
+  g.s = Model::S;
   g.max_iters = cfg->max_iters;
   g.chunks = geo_chunks(cfg->max_iters);
   g.seed = cfg->seed;
@@ -483,41 +399,26 @@ int lohf_estimate(const char* name, int s, const GeoConfig* cfg, const GeoInputs
   g.confidence = cfg->confidence;
   g.kpts0 = in->kpts0; g.kpts1 = in->kpts1; g.matches0 = in->matches0;
   g.out = out->geo;
-  a.num_lo = out->num_local_optimizations;
-  a.cost = out->cost;
-  const int splits = geo_score_splits(g.B, g.M);
-  const cudaStream_t stream = (cudaStream_t)stream_;
-  geo_prepare_kernel<<<g.B, 1024, 0, stream>>>(g);
-  LG_CHECK_LAUNCH();
-  for (int c = 0; c < g.chunks; ++c) {
-    lohf_hyp_kernel<<<g.B, GEO_CHUNK, 0, stream>>>(a, c);
-    LG_CHECK_LAUNCH();
-    geo_score_kernel<LoHfScore<Model::KIND>><<<dim3(g.B, splits), GEO_CHUNK, 0, stream>>>(a);
-    LG_CHECK_LAUNCH();
-    lohf_lo_kernel<Model><<<g.B, RED, 0, stream>>>(a, c);
-    LG_CHECK_LAUNCH();
-  }
-  lohf_final_kernel<Model><<<g.B, RED, 0, stream>>>(a);
-  LG_CHECK_LAUNCH();
-  return 0;
+  return lo_launch<Model>(g, out->num_local_optimizations, out->cost, workspace, geo_prepare_kernel, lohf_hyp_kernel,
+                          stream_);
 }
 
 }  // namespace
 
 extern "C" size_t geo_lo_homography_workspace_bytes(int32_t B, int32_t M, int32_t) {
-  return lohf_workspace_bytes(B, M);
+  return lo_workspace_bytes<HomographyLo>(B, M);
 }
 
 extern "C" size_t geo_lo_fundamental_workspace_bytes(int32_t B, int32_t M, int32_t) {
-  return lohf_workspace_bytes(B, M);
+  return lo_workspace_bytes<FundamentalLo>(B, M);
 }
 
 extern "C" int geo_homography_lo(const GeoConfig* cfg, const GeoInputs* in, GeoLoOutputs* out, void* workspace,
                                  size_t workspace_bytes, void* stream) {
-  return lohf_estimate<HomographyLo>("geo_homography_lo", 4, cfg, in, out, workspace, workspace_bytes, stream);
+  return lohf_estimate<HomographyLo>("geo_homography_lo", cfg, in, out, workspace, workspace_bytes, stream);
 }
 
 extern "C" int geo_fundamental_lo(const GeoConfig* cfg, const GeoInputs* in, GeoLoOutputs* out, void* workspace,
                                   size_t workspace_bytes, void* stream) {
-  return lohf_estimate<FundamentalLo>("geo_fundamental_lo", 8, cfg, in, out, workspace, workspace_bytes, stream);
+  return lohf_estimate<FundamentalLo>("geo_fundamental_lo", cfg, in, out, workspace, workspace_bytes, stream);
 }

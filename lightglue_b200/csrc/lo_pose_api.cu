@@ -1,16 +1,8 @@
 // Batched LO-RANSAC relative pose on the matcher's output: MSAC-scored five-point sampling with Levenberg-Marquardt
-// local optimisation and a final refinement (include/geometry_b200.h, steps L1-L8).
-//
-// Launches, all fixed by (B, M, max_iters):
-//   prepare  pose_api.cu's compaction kernel (pose_common.cuh)
-//   per chunk of GEO_CHUNK samples:
-//     hyp    one CTA per pair, one thread per sample: the five-point solutions, fp32
-//     score  (B, splits) CTAs: each streams a slice of the pair's points through shared memory against every solution
-//            of the chunk, one thread per sample, and adds count << 40 | MSAC score with one 64-bit atomic per solution
-//     lo     one CTA per pair: the chunk's lowest (score, h, r); when it beats the pair's model, P7's pose choice, LM
-//            on the truncated Sampson cost and a re-score; then the adaptive stop.  Otherwise it returns at once.
-//   final    one CTA per pair: the final LM refinement, E, the inliers and the cheirality test of the chosen (R, t)
-// A stopped pair's CTAs return at once.  Compiled with -fmad=false: oracle/lo_pose_oracle.py takes the same steps.
+// local optimisation and a final refinement (include/geometry_b200.h, steps L1-L8), on lo_common.cuh's schedule.
+// pose_api.cu's compaction kernel prepares the pair; hyp draws the five-point solutions; a local optimisation starts
+// from P7's pose choice of its E and runs LM on the truncated Sampson cost; the final kernel adds the cheirality test
+// of the chosen (R, t).  Compiled with -fmad=false: oracle/lo_pose_oracle.py takes the same steps.
 #include <stdint.h>
 
 #include "geo_lm.cuh"
@@ -47,33 +39,6 @@ __device__ __forceinline__ void projection34(const double* R, const double* tv, 
   }
 }
 
-struct LoPair {
-  double R[9], t[3];         // the pair's model
-  unsigned long long score;  // its L3 score
-  int count;                 // its inliers
-  int hr;                    // h * 16 + r of the solution that seeded it; -1: none yet
-  int nlo;                   // local optimisations adopted
-};
-
-struct LoWs {
-  LoPair* pair;             // [B]
-  unsigned long long* acc;  // [B, GEO_CHUNK, SOLS] count << 40 | score of the current chunk's solutions
-};
-
-size_t lo_carve(char* base, int B, int M, PoseWs* w, LoWs* l) {
-  WsBump b{base, carve(base, B, M, w)};
-  l->pair = b.take<LoPair>(B);
-  l->acc = b.take<unsigned long long>((size_t)B * GEO_CHUNK * SOLS);
-  return b.bytes();
-}
-
-struct LoArgs {
-  PoseArgs p;
-  LoWs l;
-  int32_t* num_lo;
-  int64_t* cost;
-};
-
 // Column-wise cross product: column j of out is a x M[:, j] ([a]x M), M and out row-major
 __device__ __forceinline__ void cross_columns(const double* a, const double* M, double* out) {
   for (int j = 0; j < 3; ++j) {
@@ -106,9 +71,47 @@ __device__ __forceinline__ void lo_epipolar(const double* E, double x, double y,
   *b1 = (E[1] * u + E[4] * v) + E[7];
 }
 
-// The relative pose for lo_common.cuh's LM loop and re-score: x = R, t (header step L7)
+__global__ void __launch_bounds__(GEO_CHUNK, 1) lo_hyp_kernel(LoArgs<PoseArgs> a, int c) {
+  const int b = blockIdx.x, t = threadIdx.x;
+  lo_reset(a.l, b, c);
+  const PosePair& P = a.p.w.pair[b];
+  const int h = c * GEO_CHUNK + t;
+  int ns = 0;
+  int id[S];
+  if (P.stop == 0 && h < a.p.max_iters && geo_sample(a.p.seed, h, P.n, S, id) == S) {
+    double sol[SOLS][9];
+    ns = five_point(a.p.w.pts + (long)b * a.p.M, id, sol);
+    float* hm = a.p.w.hyp + ((long)b * GEO_CHUNK + t) * SOLS * 9;
+    for (int r = 0; r < ns; ++r) {
+      for (int i = 0; i < 9; ++i) hm[r * 9 + i] = (float)sol[r][i];
+      a.l.acc[((long)b * GEO_CHUNK + t) * SOLS + r] = 0;
+    }
+  }
+  a.p.w.nsol[(long)b * GEO_CHUNK + t] = ns;
+}
+
+// The chunk's L3 scores of every solution, count << 40 | MSAC score
+struct LoPoseScore {
+  using Args = LoArgs<PoseArgs>;
+  using Acc = unsigned long long;
+  static constexpr int SOLS = ::SOLS, NF = 9, K = 1, TILE = ::TILE;
+  static __device__ const PoseWs& ws(const Args& a) { return a.p.w; }
+  const float4* src[K];
+  unsigned long long* sums;
+  float thr2, w;
+  __device__ LoPoseScore(const Args& a, const PosePair& P, int b)
+      : src{a.p.w.pts + (long)b * a.p.M}, sums(a.l.acc), thr2(P.thr2), w((float)GEO_LO_QSCALE / P.thr2) {}
+  __device__ unsigned long long term(const float* g, const float4* p) const {
+    return lo_term(sampson(g, p[0]), thr2, w);
+  }
+};
+
+// The relative pose for lo_common.cuh's LM loop, re-score and schedule: x = R, t (header step L7)
 struct PoseLo {
-  static constexpr int DOF = 5, TERMS = 21, GROUP = 21, NP = 12, NF = 9;
+  static constexpr int DOF = 5, TERMS = 21, GROUP = 21, NP = 12, NF = 9, S = ::S, SOLS = ::SOLS;
+  using Base = PoseArgs;
+  using Args = LoArgs<PoseArgs>;
+  using Score = LoPoseScore;
   struct Scratch {
     double E[9], dE[5][9];   // [t]x R and its derivatives at the pose being summed
     double Rs[2][9], ts[3];  // P7 candidates
@@ -188,46 +191,68 @@ struct PoseLo {
   }
 
   static __device__ __forceinline__ float err(const float* h, float4 p) { return sampson(h, p); }
-};
 
-__global__ void __launch_bounds__(GEO_CHUNK, 1) lo_hyp_kernel(LoArgs a, int c) {
-  const int b = blockIdx.x, t = threadIdx.x;
-  if (c == 0 && t == 0) {
-    LoPair& L = a.l.pair[b];
-    L.score = 0;
-    L.count = 0;
-    L.hr = -1;
-    L.nlo = 0;
+  static __device__ const float4* points(const Args& a, int b) { return a.p.w.pts + (long)b * a.p.M; }
+  static __device__ const PosePair& consts(const Args& a, int b) { return a.p.w.pair[b]; }
+  static __device__ float thr2(const Args& a, int b) { return a.p.w.pair[b].thr2; }
+
+  // L4's start: P7's pose choice of the solution's E (lo_choose_pose, below)
+  static __device__ void seed(LoShared<PoseLo>& s, const Args& a, int b, unsigned hr, long m, LoPair& L, int t);
+
+  static __device__ void store(LoShared<PoseLo>& s, LoPair& L) {
+    for (int i = 0; i < 12; ++i) L.model[i] = s.x[i];
   }
-  const PosePair& P = a.p.w.pair[b];
-  const int h = c * GEO_CHUNK + t;
-  int ns = 0;
-  int id[S];
-  if (P.stop == 0 && h < a.p.max_iters && geo_sample(a.p.seed, h, P.n, S, id) == S) {
-    double sol[SOLS][9];
-    ns = five_point(a.p.w.pts + (long)b * a.p.M, id, sol);
-    float* hm = a.p.w.hyp + ((long)b * GEO_CHUNK + t) * SOLS * 9;
-    for (int r = 0; r < ns; ++r) {
-      for (int i = 0; i < 9; ++i) hm[r * 9 + i] = (float)sol[r][i];
-      a.l.acc[((long)b * GEO_CHUNK + t) * SOLS + r] = 0;
+
+  static __device__ void load(LoShared<PoseLo>& s, const Args&, int, const LoPair& L, int t) {
+    if (t < 12) s.x[t] = L.model[t];
+  }
+
+  // The output E is [t]x R, not the sampled E: the stored (R, t) is scored again
+  static __device__ void restore(LoShared<PoseLo>& s, const Args& a, int b, const LoPair& L, int t) {
+    load(s, a, b, L, t);
+    __syncthreads();
+    lo_rescore(s, consts(a, b), points(a, b), a.p.w.pair[b].n, thr2(a, b), t);
+  }
+
+  static __device__ void fail(const Args& a, int b, int t) {
+    const GeoPoseOutputs& o = a.p.out;
+    for (int i = t; i < a.p.M; i += RED) o.pose_inliers[(long)b * a.p.M + i] = 0;
+    if (t < 9) o.E[(long)b * 9 + t] = o.R[(long)b * 9 + t] = 0.0;
+    if (t < 3) o.t[(long)b * 3 + t] = 0.0;
+    if (t == 0) o.num_pose_inliers[b] = 0;
+  }
+
+  // L8: the inliers of E and those that pass the cheirality test of (R, t)
+  static __device__ void write(LoShared<PoseLo>& s, const Args& a, int b, int t) {
+    const PosePair& P = a.p.w.pair[b];
+    const GeoPoseOutputs& o = a.p.out;
+    const float4* pts = points(a, b);
+    const int* idx = a.p.w.idx + (long)b * a.p.M;
+    uint8_t* inl = o.inliers + (long)b * a.p.M;
+    uint8_t* pinl = o.pose_inliers + (long)b * a.p.M;
+    for (int i = t; i < a.p.M; i += RED) inl[i] = pinl[i] = 0;
+    if (t == 0) s.m.count = 0;
+    __syncthreads();
+    int cnt = 0;
+    double P1[3][4];
+    projection34(s.x, s.x + 9, P1);
+    for (int k = t; k < P.n; k += RED) {
+      const float4 p = pts[k];
+      if (!(sampson(s.fm, p) < P.thr2)) continue;
+      inl[idx[k]] = 1;
+      if (cheirality_pass(P1, p.x, p.y, p.z, p.w, a.p.distance)) {
+        pinl[idx[k]] = 1;
+        ++cnt;
+      }
     }
-  }
-  a.p.w.nsol[(long)b * GEO_CHUNK + t] = ns;
-}
-
-// The chunk's L3 scores of every solution, count << 40 | MSAC score
-struct LoPoseScore {
-  using Args = LoArgs;
-  using Acc = unsigned long long;
-  static constexpr int SOLS = ::SOLS, NF = 9, K = 1, TILE = ::TILE;
-  static __device__ const PoseWs& ws(const LoArgs& a) { return a.p.w; }
-  const float4* src[K];
-  unsigned long long* sums;
-  float thr2, w;
-  __device__ LoPoseScore(const LoArgs& a, const PosePair& P, int b)
-      : src{a.p.w.pts + (long)b * a.p.M}, sums(a.l.acc), thr2(P.thr2), w((float)GEO_LO_QSCALE / P.thr2) {}
-  __device__ unsigned long long term(const float* g, const float4* p) const {
-    return lo_term(sampson(g, p[0]), thr2, w);
+    if (cnt) atomicAdd(&s.m.count, cnt);
+    __syncthreads();
+    if (t < 9) {
+      o.E[(long)b * 9 + t] = s.px[t];
+      o.R[(long)b * 9 + t] = s.x[t];
+    }
+    if (t < 3) o.t[(long)b * 3 + t] = s.x[9 + t];
+    if (t == 0) o.num_pose_inliers[b] = s.m.count;
   }
 };
 
@@ -263,136 +288,18 @@ __device__ void lo_choose_pose(LoShared<PoseLo>& s, const float4* pts, int n, fl
   __syncthreads();
 }
 
-// After chunk c: the chunk's best solution, the local optimisation when it beats the pair's model, the stop
-__global__ void __launch_bounds__(RED, 1) lo_kernel(LoArgs a, int c) {
-  const int b = blockIdx.x, t = threadIdx.x;
-  PosePair& P = a.p.w.pair[b];
-  if (P.stop) return;
-  LoPair& L = a.l.pair[b];
-  __shared__ LoShared<PoseLo> s;
-  if (t == 0) s.key = ~0ull;
-  __syncthreads();
-  if (t < GEO_CHUNK) {
-    const int ns = a.p.w.nsol[(long)b * GEO_CHUNK + t];
-    const unsigned h = c * GEO_CHUNK + t;
-    for (int r = 0; r < ns; ++r) {
-      const unsigned long long v = a.l.acc[((long)b * GEO_CHUNK + t) * SOLS + r];
-      atomicMin(&s.key, (v & LO_SCORE_MASK) << 28 | (h * 16u + (unsigned)r));
-    }
-  }
-  __syncthreads();
-  const unsigned long long key = s.key;
-  const float4* pts = a.p.w.pts + (long)b * a.p.M;
-  if (key != ~0ull && (L.hr < 0 || (key >> 28) < L.score)) {
-    const unsigned hr = (unsigned)(key & 0xfffffffu);
-    const long slot = (long)b * GEO_CHUNK + (hr >> 4) - c * GEO_CHUNK;
-    if (t < 9) s.fm[t] = a.p.w.hyp[(slot * SOLS + (hr & 15)) * 9 + t];
-    __syncthreads();
-    lo_choose_pose(s, pts, P.n, P.thr2, a.p.distance, t);
-    if (t == 0) {
-      for (int i = 0; i < 9; ++i) L.R[i] = s.x[i];
-      for (int i = 0; i < 3; ++i) L.t[i] = s.x[9 + i];
-      L.score = key >> 28;
-      L.count = (int)(a.l.acc[slot * SOLS + (hr & 15)] >> 40);
-      L.hr = (int)hr;
-    }
-    lo_refine(s, P, pts, P.n, (double)P.thr2, GEO_LO_STEPS, t);
-    lo_rescore(s, P, pts, P.n, P.thr2, t);
-    if (t == 0 && (s.score & LO_SCORE_MASK) < L.score) {
-      for (int i = 0; i < 9; ++i) L.R[i] = s.x[i];
-      for (int i = 0; i < 3; ++i) L.t[i] = s.x[9 + i];
-      L.score = s.score & LO_SCORE_MASK;
-      L.count = (int)(s.score >> 40);
-      L.nlo = L.nlo + 1;
-    }
-  }
-  if (t == 0) {
-    const int drawn = min((c + 1) * GEO_CHUNK, a.p.max_iters);
-    const int cnt = L.hr >= 0 ? L.count : 0;
-    P.drawn = drawn;
-    P.stop = drawn >= a.p.max_iters ||
-             drawn >= update_num_iters(a.p.confidence, 1.0 - (double)cnt / P.n, S, a.p.max_iters);
-  }
-}
-
-// Final refinement and the outputs (header steps L6, L8)
-__global__ void __launch_bounds__(RED, 1) lo_final_kernel(LoArgs a) {
-  const int b = blockIdx.x, t = threadIdx.x;
+__device__ void PoseLo::seed(LoShared<PoseLo>& s, const Args& a, int b, unsigned, long m, LoPair& L, int t) {
   const PosePair& P = a.p.w.pair[b];
-  const LoPair& L = a.l.pair[b];
-  const GeoPoseOutputs& o = a.p.out;
-  uint8_t* inl = o.inliers + (long)b * a.p.M;
-  uint8_t* pinl = o.pose_inliers + (long)b * a.p.M;
-  for (int i = t; i < a.p.M; i += RED) inl[i] = pinl[i] = 0;
-  if (!P.ok || L.hr < 0) {
-    if (t < 9) o.E[(long)b * 9 + t] = o.R[(long)b * 9 + t] = 0.0;
-    if (t < 3) o.t[(long)b * 3 + t] = 0.0;
-    if (t == 0) {
-      o.num_inliers[b] = o.num_pose_inliers[b] = 0;
-      o.success[b] = 0;
-      o.best_hypothesis[b] = o.best_solution[b] = -1;
-      o.num_hypotheses[b] = P.drawn;
-      a.num_lo[b] = 0;
-      a.cost[b] = 0;
-    }
-    return;
-  }
-  __shared__ LoShared<PoseLo> s;
-  const float4* pts = a.p.w.pts + (long)b * a.p.M;
-  const int* idx = a.p.w.idx + (long)b * a.p.M;
-  if (t < 9) s.x[t] = L.R[t];
-  if (t < 3) s.x[9 + t] = L.t[t];
+  if (t < 9) s.fm[t] = a.p.w.hyp[m * 9 + t];
   __syncthreads();
-  lo_refine(s, P, pts, P.n, (double)P.thr2, GEO_LO_FINAL_STEPS, t);
-  lo_rescore(s, P, pts, P.n, P.thr2, t);
-  const bool keep = (s.score & LO_SCORE_MASK) <= L.score;
-  __syncthreads();
-  if (!keep) {
-    if (t < 9) s.x[t] = L.R[t];
-    if (t < 3) s.x[9 + t] = L.t[t];
-    __syncthreads();
-    lo_rescore(s, P, pts, P.n, P.thr2, t);
-  }
-  if (t == 0) s.m.count = 0;
-  __syncthreads();
-  int cnt = 0;
-  double P1[3][4];
-  projection34(s.x, s.x + 9, P1);
-  for (int k = t; k < P.n; k += RED) {
-    const float4 p = pts[k];
-    if (!(sampson(s.fm, p) < P.thr2)) continue;
-    inl[idx[k]] = 1;
-    if (cheirality_pass(P1, p.x, p.y, p.z, p.w, a.p.distance)) {
-      pinl[idx[k]] = 1;
-      ++cnt;
-    }
-  }
-  if (cnt) atomicAdd(&s.m.count, cnt);
-  __syncthreads();
-  if (t < 9) {
-    o.E[(long)b * 9 + t] = s.px[t];
-    o.R[(long)b * 9 + t] = s.x[t];
-  }
-  if (t < 3) o.t[(long)b * 3 + t] = s.x[9 + t];
-  if (t == 0) {
-    o.num_inliers[b] = (int)(s.score >> 40);
-    o.num_pose_inliers[b] = s.m.count;
-    o.success[b] = 1;
-    o.best_hypothesis[b] = L.hr >> 4;
-    o.best_solution[b] = L.hr & 15;
-    o.num_hypotheses[b] = P.drawn;
-    a.num_lo[b] = L.nlo;
-    a.cost[b] = (int64_t)(s.score & LO_SCORE_MASK);
-  }
+  lo_choose_pose(s, points(a, b), P.n, P.thr2, a.p.distance, t);
+  if (t == 0) store(s, L);
 }
 
 }  // namespace
 
 extern "C" size_t geo_lo_pose_workspace_bytes(int32_t B, int32_t M, int32_t) {
-  if (B < 0 || M < 0) return 0;
-  PoseWs w;
-  LoWs l;
-  return lo_carve(nullptr, B, M, &w, &l) + 256;
+  return lo_workspace_bytes<PoseLo>(B, M);
 }
 
 extern "C" int geo_relative_pose_lo(const GeoLoPoseConfig* cfg, const GeoPoseInputs* in, GeoLoPoseOutputs* out,
@@ -410,9 +317,7 @@ extern "C" int geo_relative_pose_lo(const GeoLoPoseConfig* cfg, const GeoPoseInp
                            geo_lo_pose_workspace_bytes(in->B, in->M, cfg->max_iters));
   }
   if (rc != GEO_RUN) return rc;
-  LoArgs a{};
-  lo_carve(geo_workspace_base(workspace), in->B, in->M, &a.p.w, &a.l);
-  PoseArgs& p = a.p;
+  PoseArgs p{};
   p.B = in->B; p.M = in->M; p.N = in->N;
   p.max_iters = cfg->max_iters;
   p.chunks = geo_chunks(cfg->max_iters);
@@ -423,21 +328,6 @@ extern "C" int geo_relative_pose_lo(const GeoLoPoseConfig* cfg, const GeoPoseInp
   p.kpts0 = in->kpts0; p.kpts1 = in->kpts1; p.matches0 = in->matches0;
   p.K0 = in->K0; p.K1 = in->K1;
   p.out = out->pose;
-  a.num_lo = out->num_local_optimizations;
-  a.cost = out->cost;
-  const int splits = geo_score_splits(p.B, p.M);
-  const cudaStream_t stream = (cudaStream_t)stream_;
-  pose_prepare_kernel<<<p.B, 1024, 0, stream>>>(p);
-  LG_CHECK_LAUNCH();
-  for (int c = 0; c < p.chunks; ++c) {
-    lo_hyp_kernel<<<p.B, GEO_CHUNK, 0, stream>>>(a, c);
-    LG_CHECK_LAUNCH();
-    geo_score_kernel<LoPoseScore><<<dim3(p.B, splits), GEO_CHUNK, 0, stream>>>(a);
-    LG_CHECK_LAUNCH();
-    lo_kernel<<<p.B, RED, 0, stream>>>(a, c);
-    LG_CHECK_LAUNCH();
-  }
-  lo_final_kernel<<<p.B, RED, 0, stream>>>(a);
-  LG_CHECK_LAUNCH();
-  return 0;
+  return lo_launch<PoseLo>(p, out->num_local_optimizations, out->cost, workspace, pose_prepare_kernel, lo_hyp_kernel,
+                           stream_);
 }

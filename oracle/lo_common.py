@@ -1,6 +1,7 @@
 """numpy restatement of csrc/geo_lm.cuh and lo_common.cuh: the damped Cholesky step and A7's quaternion rotation that
-every Levenberg-Marquardt refinement takes, the LM loop of the LO-RANSAC estimators (header steps L7, LH7 and LF7),
-and the chunk driver that the LO-RANSAC homography and fundamental matrix share (steps LH1-LH8 and LF1-LF8).
+every Levenberg-Marquardt refinement takes, the LM loop of the LO-RANSAC estimators (header steps L7, LH7, LF7 and
+LA7), the schedule of L4-L6 that they all run (LH, LF and LA likewise), and the pair of the LO-RANSAC homography and
+fundamental matrix (steps LH1-LH8 and LF1-LF8).
 
 Python floats and elementwise numpy only, so the CUDA build compiled with -fmad=false agrees bit for bit.
 """
@@ -85,6 +86,38 @@ def refine(terms, update, x, dof, steps: int):
     return x
 
 
+def lo_pair(n, s, max_iters, confidence, candidates, refine, rescore, restore=None):
+    """L4-L6 of one pair of n points and s points per sample.  candidates(h) gives the valid solutions of the samples h
+    in (sample, solution) order as (scores, counts, samples, solution indices, seed), or None without one; seed(i) is
+    the model of solution i.  refine(model, steps) gives the LM result of steps steps from a model and rescore(x) the
+    (model, score, count) of an LM result.  After the final refinement, a score above the pair's gives restore(model,
+    score, count) of the pair's model (default: as it is).  Returns ((h, r, model, score, count) or None, local
+    optimisations adopted, samples drawn)."""
+    best, nlo, drawn = None, 0, 0  # best: (score, count, h, r, model)
+    for c in range(-(-max_iters // go.CHUNK)):
+        h = np.arange(c * go.CHUNK, min((c + 1) * go.CHUNK, max_iters), dtype=np.int64)
+        cands = candidates(h)
+        if cands is not None:
+            sc, cnt, hs, rs, seed = cands
+            i = int(np.argmin(sc))  # first minimum: the lowest (sample, solution)
+            if best is None or sc[i] < best[0]:
+                best = (int(sc[i]), int(cnt[i]), int(hs[i]), int(rs[i]), seed(i))
+                model, sl, cl = rescore(refine(best[4], lpo.STEPS))
+                if sl < best[0]:
+                    best = (sl, cl, best[2], best[3], model)
+                    nlo += 1
+        drawn = min((c + 1) * go.CHUNK, max_iters)
+        ep = 1.0 - (best[1] if best else 0) / n
+        if drawn >= max_iters or drawn >= go.update_num_iters(confidence, ep, s, max_iters):
+            break
+    if best is None:
+        return None, nlo, drawn
+    model, cost, count = rescore(refine(best[4], lpo.FINAL_STEPS))
+    if cost > best[0]:  # the refinement is kept unless its score rises
+        model, cost, count = (restore or (lambda *m: m))(best[4], best[0], best[1])
+    return (best[2], best[3], model, cost, count), nlo, drawn
+
+
 def lo_hf_pair(kind, s, key, start, refine_model, rescore, kpts0, kpts1, m0, threshold, max_iters, confidence,
                seed) -> dict:
     """One pair of the LO-RANSAC homography (LH1-LH8) or fundamental matrix (LF1-LF8), kind and s its step 4 model and
@@ -102,31 +135,21 @@ def lo_hf_pair(kind, s, key, start, refine_model, rescore, kpts0, kpts1, m0, thr
             "best_hypothesis": -1, "num_hypotheses": 0, "num_local_optimizations": 0, "cost": 0}
     if norm is None:
         return fail
-    best, nlo, drawn = None, 0, 0  # best: (score, count, h, model)
-    for c in range(-(-max_iters // go.CHUNK)):
-        h = np.arange(c * go.CHUNK, min((c + 1) * go.CHUNK, max_iters), dtype=np.int64)
+
+    def candidates(h):
         models, ok = go.hypotheses(kind, seed, h, pts, norm)
-        if ok.any():
-            sc, cnt = lpo.score(go.errors(kind, models[ok], pts), thr2)
-            i = int(np.argmin(sc))  # first minimum: the lowest hypothesis
-            if best is None or sc[i] < best[0]:
-                best = (int(sc[i]), int(cnt[i]), int(h[ok][i]), models[ok][i])
-                Ml, sl, cl = rescore(norm, refine_model(norm, start(norm, best[3]), pts, float(thr2), lpo.STEPS), pts,
-                                     thr2)
-                if sl < best[0]:
-                    best = (sl, cl, best[2], Ml)
-                    nlo += 1
-        drawn = min((c + 1) * go.CHUNK, max_iters)
-        ep = 1.0 - (best[1] if best else 0) / n
-        if drawn >= max_iters or drawn >= go.update_num_iters(confidence, ep, s, max_iters):
-            break
-    if best is None:
+        if not ok.any():
+            return None
+        sc, cnt = lpo.score(go.errors(kind, models[ok], pts), thr2)
+        return sc, cnt, h[ok], np.zeros(len(sc), dtype=np.int64), lambda i: models[ok][i]
+
+    found, nlo, drawn = lo_pair(n, s, max_iters, confidence, candidates,
+                                lambda model, steps: refine_model(norm, start(norm, model), pts, float(thr2), steps),
+                                lambda x: rescore(norm, x, pts, thr2))
+    if found is None:
         return dict(fail, num_hypotheses=drawn)
-    model, cost, count = rescore(norm, refine_model(norm, start(norm, best[3]), pts, float(thr2), lpo.FINAL_STEPS),
-                                 pts, thr2)
-    if cost > best[0]:
-        cost, count, model = best[0], best[1], best[3]
+    h, _, model, cost, count = found
     inliers = np.zeros(M, dtype=bool)
     inliers[idx[go.errors(kind, model[None], pts)[0] < thr2]] = True
     return {key: model.reshape(3, 3), "inliers": inliers, "num_inliers": count, "success": True,
-            "best_hypothesis": best[2], "num_hypotheses": drawn, "num_local_optimizations": nlo, "cost": cost}
+            "best_hypothesis": h, "num_hypotheses": drawn, "num_local_optimizations": nlo, "cost": cost}

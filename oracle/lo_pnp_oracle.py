@@ -2,10 +2,10 @@
 csrc/lo_pnp_api.cu).
 
 The compaction, calibration, samples, Lambda Twist solutions, projections and fp32 inlier test are pnp_oracle's; the
-MSAC score is lo_pose_oracle's; the Cholesky step, quaternion rotation and LM loop are lo_common's.  What is new here is
-the fp32 reprojection error that the score reads and the Levenberg-Marquardt refinement of (R, t) on the truncated
-squared reprojection error in pixels (double, elementwise operations only, so the CUDA build compiled with -fmad=false
-agrees bit for bit).
+MSAC score is lo_pose_oracle's; the Cholesky step, quaternion rotation, LM loop and schedule are lo_common's.  What is
+new here is the fp32 reprojection error that the score reads and the Levenberg-Marquardt refinement of (R, t) on the
+truncated squared reprojection error in pixels (double, elementwise operations only, so the CUDA build compiled with
+-fmad=false agrees bit for bit).
 """
 from __future__ import annotations
 
@@ -110,37 +110,26 @@ def lo_absolute_pose_pair(kpts0, points3d1, m0, K0, threshold=8.0, max_iters=100
         return _fail(M, 0)
     bear = pnp.calibrate(K0, pix)
     thr2 = np.float32(threshold * threshold)
-    best, nlo, drawn = None, 0, 0  # best: (score, count, h, r, x)
-    for c in range(-(-max_iters // go.CHUNK)):
-        h = np.arange(c * go.CHUNK, min((c + 1) * go.CHUNK, max_iters), dtype=np.int64)
+
+    def candidates(h):
         R, t, kept = pnp.solutions(seed, h, bear, wld)
-        if kept.any():
-            sc, cnt = lpo.score(errors(pnp.projection(R[kept], t[kept], K0), pix, wld), thr2)
-            i = int(np.argmin(sc))  # first minimum: the lowest (sample, solution)
-            if best is None or sc[i] < best[0]:
-                hh, rr = np.nonzero(kept)
-                x = [float(v) for v in R[hh[i], rr[i]]] + [float(v) for v in t[hh[i], rr[i]]]
-                best = (int(sc[i]), int(cnt[i]), int(h[hh[i]]), int(rr[i]), x)
-                xl = refine(x, K0, pix, wld, float(thr2), STEPS)
-                sl, cl = rescore(xl, K0, pix, wld, thr2)
-                if sl < best[0]:
-                    best = (sl, cl, best[2], best[3], xl)
-                    nlo += 1
-        drawn = min((c + 1) * go.CHUNK, max_iters)
-        ep = 1.0 - (best[1] if best else 0) / n
-        if drawn >= max_iters or drawn >= go.update_num_iters(confidence, ep, S, max_iters):
-            break
-    if best is None:
+        if not kept.any():
+            return None
+        sc, cnt = lpo.score(errors(pnp.projection(R[kept], t[kept], K0), pix, wld), thr2)
+        hh, rr = np.nonzero(kept)
+        return sc, cnt, h[hh], rr, lambda i: [float(v) for v in R[hh[i], rr[i]]] + [float(v) for v in t[hh[i], rr[i]]]
+
+    found, nlo, drawn = lc.lo_pair(n, S, max_iters, confidence, candidates,
+                                   lambda x, steps: refine(x, K0, pix, wld, float(thr2), steps),
+                                   lambda x: (x, *rescore(x, K0, pix, wld, thr2)))
+    if found is None:
         return _fail(M, drawn)
-    x = refine(best[4], K0, pix, wld, float(thr2), FINAL_STEPS)
-    cost, count = rescore(x, K0, pix, wld, thr2)
-    if cost > best[0]:  # the refinement is kept unless its score rises
-        x, cost, count = best[4], best[0], best[1]
+    h, r, x, cost, count = found
     P = pnp.projection(np.array(x[:9]), np.array(x[9:]), K0)
     inliers = np.zeros(M, dtype=bool)
     inliers[idx[pnp.reproj_inliers(P[None], pix, wld, thr2)[0]]] = True
     return {"R": np.array(x[:9]).reshape(3, 3), "t": np.array(x[9:]), "inliers": inliers, "num_inliers": count,
-            "success": True, "best_hypothesis": best[2], "best_solution": best[3], "num_hypotheses": drawn,
+            "success": True, "best_hypothesis": h, "best_solution": r, "num_hypotheses": drawn,
             "num_local_optimizations": nlo, "cost": cost}
 
 

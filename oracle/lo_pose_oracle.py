@@ -2,9 +2,9 @@
 csrc/pose_api.cu).
 
 The sampling, the five-point solutions, the fp32 Sampson error and the cheirality test are pose_oracle's; the sums are
-geometry_oracle's fixed order; the Cholesky step, quaternion and LM loop are lo_common's.  What is new here is the
-integer MSAC score, the 5-DOF pose update and terms on the truncated Sampson cost (double, elementwise operations only,
-so the CUDA build compiled with -fmad=false agrees bit for bit) and the once-per-chunk local optimisation schedule.
+geometry_oracle's fixed order; the Cholesky step, quaternion, LM loop and once-per-chunk local optimisation schedule
+are lo_common's.  What is new here is the integer MSAC score and the 5-DOF pose update and terms on the truncated
+Sampson cost (double, elementwise operations only, so the CUDA build compiled with -fmad=false agrees bit for bit).
 """
 from __future__ import annotations
 
@@ -165,48 +165,40 @@ def lo_relative_pose_pair(kpts0, kpts1, m0, K0, K1, threshold, max_iters, confid
         return _fail(M, 0)
     pts = np.concatenate([po.calibrate(K0, px[:, :2]), po.calibrate(K1, px[:, 2:])], 1)
     thr2 = po.threshold2(K0, K1, threshold)
-    best, nlo, drawn = None, 0, 0  # best: (score, count, h, r, R, t)
-    for c in range(-(-max_iters // po.CHUNK)):
-        h = np.arange(c * po.CHUNK, min((c + 1) * po.CHUNK, max_iters), dtype=np.int64)
+
+    def candidates(h):
         E, found = po.solutions(seed, h, pts)
-        if found.any():
-            err = po.sampson(E[found], pts)
-            sc, cnt = score(err, thr2)
-            i = int(np.argmin(sc))  # first minimum: the lowest (sample, solution)
-            if best is None or sc[i] < best[0]:
-                hh, rr = np.nonzero(found)
-                Es = E[found][i].astype(np.float32).astype(np.float64)
-                R, t = choose_pose(Es, pts, err[i] < thr2, distance)
-                best = (int(sc[i]), int(cnt[i]), int(h[hh[i]]), int(rr[i]), R, t)
-                Rl, tl = refine(R, t, pts, float(thr2), STEPS)
-                sl, cl = score(model_errors(Rl, tl, pts), thr2)
-                if int(sl) < best[0]:
-                    best = (int(sl), int(cl), best[2], best[3], Rl, tl)
-                    nlo += 1
-        drawn = min((c + 1) * po.CHUNK, max_iters)
-        ep = 1.0 - (best[1] if best else 0) / n
-        if drawn >= max_iters or drawn >= go.update_num_iters(confidence, ep, po.S, max_iters):
-            break
-    if best is None:
+        if not found.any():
+            return None
+        err = po.sampson(E[found], pts)
+        sc, cnt = score(err, thr2)
+        hh, rr = np.nonzero(found)
+        # L4's start: P7's pose choice of the solution's E, widened from fp32, on its inliers
+        return sc, cnt, h[hh], rr, lambda i: choose_pose(E[found][i].astype(np.float32).astype(np.float64), pts,
+                                                         err[i] < thr2, distance)
+
+    def rescore(x):
+        sc, cnt = score(model_errors(*x, pts), thr2)
+        return x, int(sc), int(cnt)
+
+    # the output E is [t]x R, not the sampled E: a restored (R, t) is scored again
+    found, nlo, drawn = lc.lo_pair(n, po.S, max_iters, confidence, candidates,
+                                   lambda x, steps: refine(*x, pts, float(thr2), steps), rescore,
+                                   lambda x, sc, cnt: rescore(x))
+    if found is None:
         return _fail(M, drawn)
-    R, t = best[4], best[5]
-    Rf, tf = refine(R, t, pts, float(thr2), FINAL_STEPS)
-    sf, _ = score(model_errors(Rf, tf, pts), thr2)
-    if int(sf) <= best[0]:
-        R, t = Rf, tf
+    h, r, (R, t), cost, count = found
     E = po.unit_scale(np.array(essential(R, t)))
-    err = po.sampson(E[None], pts)[0]
-    cost, count = score(err, thr2)
-    inl = err < thr2
+    inl = po.sampson(E[None], pts)[0] < thr2
     good = po.cheirality(R, t, pts[inl], distance)
     inliers = np.zeros(M, dtype=bool)
     inliers[idx[inl]] = True
     pose = np.zeros(M, dtype=bool)
     pose[idx[inl][good]] = True
     return {"E": E.reshape(3, 3), "R": np.array(R).reshape(3, 3), "t": np.array(t), "inliers": inliers,
-            "num_inliers": int(count), "pose_inliers": pose, "num_pose_inliers": int(good.sum()), "success": True,
-            "best_hypothesis": best[2], "best_solution": best[3], "num_hypotheses": drawn,
-            "num_local_optimizations": nlo, "cost": int(cost)}
+            "num_inliers": count, "pose_inliers": pose, "num_pose_inliers": int(good.sum()), "success": True,
+            "best_hypothesis": h, "best_solution": r, "num_hypotheses": drawn, "num_local_optimizations": nlo,
+            "cost": cost}
 
 
 def lo_relative_pose(kpts0, kpts1, matches0, K0, K1, threshold=1.0, max_iters=1000, confidence=0.999, distance=50.0,
