@@ -5,10 +5,11 @@
 // Launches, all fixed by (B, M, max_iters):
 //   prepare  geo_prepare_kernel of geo_hf.cuh: ordered compaction, Hartley normalisation
 //   per chunk of GEO_CHUNK hypotheses:
-//     hyp    one CTA per pair: folds the previous chunk's counts (geo_fold), decides the adaptive stop, then one thread
-//            per hypothesis draws and solves its sample in double
+//     hyp    geo_hyp_kernel, one CTA per pair: folds the previous chunk's counts (geo_fold), decides the adaptive
+//            stop, then one thread per hypothesis draws and solves its sample in double
 //     score  geo_score_kernel with AfScore: the inlier counts of the chunk's fp32 models
-//   final    one CTA per pair: folds the last chunk, LM refinement through lo_common.cuh's loop, re-score, outputs
+//   final    geo_final_kernel<AfRansac>, one CTA per pair: folds the last chunk, LM refinement through
+//            lo_common.cuh's loop, re-score, outputs
 // A stopped pair's CTAs return at once.  Compiled with -fmad=false, like geo_api.cu: oracle/affine_oracle.py takes the
 // same steps in numpy.
 #include "geo_hf.cuh"
@@ -96,20 +97,19 @@ __device__ bool af_hypothesis(const GeoArgs& a, const GeoPair& P, const float4* 
   return fin;
 }
 
+// geo_hyp_kernel's solver: X of af_hypothesis per sample, scored as its pixel model
 template <bool PARTIAL>
-__global__ void __launch_bounds__(GEO_CHUNK, 1) af_hyp_kernel(GeoArgs a, int c) {
-  const int b = blockIdx.x, t = threadIdx.x;
-  if (c > 0) geo_fold<1>(a, a.s, b, c - 1);
-  const GeoPair& P = a.w.pair[b];
-  const int h = c * GEO_CHUNK + t;
-  double X[6], A[6];
-  const bool ok = P.stop == 0 && h < a.max_iters && af_hypothesis<PARTIAL>(a, P, a.w.pts + (long)b * a.M, h, X, A);
-  if (ok) {
-    float* hm = a.w.hyp + ((long)b * GEO_CHUNK + t) * 6;
-    for (int i = 0; i < 6; ++i) hm[i] = (float)A[i];
+struct AfSolver {
+  static constexpr int SOLS = 1, NX = PARTIAL ? 4 : 6, NF = 6;
+  static __device__ int s(const GeoArgs& a) { return a.s; }
+  static __device__ int solve(const GeoArgs& a, int b, unsigned h, double (*x)[NX]) {
+    double A[6];
+    return af_hypothesis<PARTIAL>(a, a.w.pair[b], a.w.pts + (long)b * a.M, h, x[0], A);
   }
-  a.w.count[(long)b * GEO_CHUNK + t] = ok ? 0 : -1;
-}
+  static __device__ void pixels(const GeoArgs& a, int b, const double* x, double* px) {
+    af_pixels<PARTIAL>(a.w.pair[b], x, px);
+  }
+};
 
 // Affine inlier counts of the chunk's six-float models
 struct AfScore {
@@ -179,79 +179,42 @@ struct AffineLm {
   }
 };
 
+// The affine model for geo_final_kernel: refine_iters LM steps on the best hypothesis's inliers (header step AF6)
 template <bool PARTIAL>
-__global__ void __launch_bounds__(RED, 1) af_final_kernel(GeoArgs a, int refine_iters) {
-  const int b = blockIdx.x, t = threadIdx.x;
-  geo_fold<1>(a, a.s, b, a.chunks - 1);
-  const GeoPair& P = a.w.pair[b];
-  const float4* pts = a.w.pts + (long)b * a.M;
-  const int* idx = a.w.idx + (long)b * a.M;
-  uint8_t* inl = a.out.inliers + (long)b * a.M;
-  __shared__ LoShared<AffineLm<PARTIAL>> s;
-  __shared__ double model[2][6];  // the best hypothesis's pixel model and the refined one
-  __shared__ float fm[2][6];
-  __shared__ int count[2];
-  for (int i = t; i < a.M; i += RED) inl[i] = 0;
-  const unsigned long long key = P.best;
-  if (!P.ok || key == 0) {
-    if (t < 9) a.out.model[(long)b * 9 + t] = 0.0;
-    if (t == 0) {
-      a.out.num_inliers[b] = 0;
-      a.out.success[b] = 0;
-      a.out.best_hypothesis[b] = -1;
-      a.out.num_hypotheses[b] = P.drawn;
-    }
-    return;
-  }
-  const unsigned hb = ~(unsigned)(key & 0xffffffffu) >> 4;
-  const int hcount = (int)(key >> 32) - 1;
-  if (t == 0) {
-    af_hypothesis<PARTIAL>(a, P, pts, hb, s.x, model[0]);
-    for (int i = 0; i < 6; ++i) fm[0][i] = (float)model[0][i];
-    count[0] = hcount;
-    count[1] = -1;
-  }
-  __syncthreads();
-  if (hcount >= a.s && refine_iters > 0) {
-    lo_refine(s, P, AfPoints{pts, fm[0]}, P.n, (double)a.thr2, refine_iters, t);
-    if (t == 0) {
-      af_pixels<PARTIAL>(P, s.x, model[1]);
-      for (int i = 0; i < 6; ++i) fm[1][i] = (float)model[1][i];
-      count[1] = 0;
-    }
-    __syncthreads();
-    int k1 = 0;
-    for (int k = t; k < P.n; k += RED) k1 += af_err(fm[1], pts[k]) < a.thr2;
-    if (k1) atomicAdd(&count[1], k1);
-    __syncthreads();
-  }
-  const int u = count[1] >= count[0] ? 1 : 0;
-  for (int k = t; k < P.n; k += RED)
-    if (af_err(fm[u], pts[k]) < a.thr2) inl[idx[k]] = 1;
-  if (t < 9) a.out.model[(long)b * 9 + t] = t < 6 ? model[u][t] : t == 8 ? 1.0 : 0.0;
-  if (t == 0) {
-    a.out.num_inliers[b] = count[u];
-    a.out.success[b] = 1;
-    a.out.best_hypothesis[b] = (int)hb;
-    a.out.num_hypotheses[b] = P.drawn;
-  }
-}
+struct AfRansac : AfSolver<PARTIAL> {
+  using Base = GeoArgs;
+  using Score = AfScore;
+  using Scratch = LoShared<AffineLm<PARTIAL>>;
 
-template <bool PARTIAL>
-int af_launch(const GeoArgs& a, int refine_iters, cudaStream_t stream) {
-  const int splits = geo_score_splits(a.B, a.M);
-  geo_prepare_kernel<<<a.B, 1024, 0, stream>>>(a);
-  LG_CHECK_LAUNCH();
-  for (int c = 0; c < a.chunks; ++c) {
-    af_hyp_kernel<PARTIAL><<<a.B, GEO_CHUNK, 0, stream>>>(a, c);
-    LG_CHECK_LAUNCH();
-    geo_score_kernel<AfScore><<<dim3(a.B, splits), GEO_CHUNK, 0, stream>>>(a);
-    LG_CHECK_LAUNCH();
+  static __device__ bool inlier(const GeoArgs& a, int b, const float* g, int k) {
+    return af_err(g, a.w.pts[(long)b * a.M + k]) < a.thr2;
   }
-  af_final_kernel<PARTIAL><<<a.B, RED, 0, stream>>>(a, refine_iters);
-  LG_CHECK_LAUNCH();
-  return 0;
-}
+  static __device__ void clear(const GeoArgs& a, int b, int t) {
+    for (int i = t; i < a.M; i += RED) a.out.inliers[(long)b * a.M + i] = 0;
+  }
+  static __device__ void fail(const GeoArgs& a, int b, int t) {
+    if (t < 9) a.out.model[(long)b * 9 + t] = 0.0;
+  }
+  static __device__ bool refits(const GeoArgs& a, int hcount) { return hcount >= a.s && a.refine_iters > 0; }
+
+  static __device__ void refit(GeoFinal<AfRansac>& s, const GeoArgs& a, int b, int t) {
+    constexpr int NP = AfSolver<PARTIAL>::NX;
+    if (t == 0)
+      for (int i = 0; i < NP; ++i) s.m.x[i] = s.x[0][i];
+    __syncthreads();
+    const GeoPair& P = a.w.pair[b];
+    lo_refine(s.m, P, AfPoints{a.w.pts + (long)b * a.M, s.fm[0]}, P.n, (double)a.thr2, a.refine_iters,
+              GEO_LO_LAMBDA0, t);
+    if (t == 0)
+      for (int i = 0; i < NP; ++i) s.x[1][i] = s.m.x[i];
+  }
+
+  // [A; 0 0 1] and its inliers
+  static __device__ void write(GeoFinal<AfRansac>& s, const GeoArgs& a, int b, int u, int t) {
+    geo_write_mask<AfRansac>(a, b, s.fm[u], t);
+    if (t < 9) a.out.model[(long)b * 9 + t] = t < 6 ? s.px[u][t] : t == 8 ? 1.0 : 0.0;
+  }
+};
 
 }  // namespace
 
@@ -287,7 +250,8 @@ extern "C" int geo_estimate_affine(const GeoAffineConfig* cfg, const GeoInputs* 
   a.confidence = cfg->confidence;
   a.kpts0 = in->kpts0; a.kpts1 = in->kpts1; a.matches0 = in->matches0;
   a.out = *out;
+  a.refine_iters = cfg->refine_iters;
   const cudaStream_t stream = (cudaStream_t)stream_;
-  return cfg->model == GEO_AFFINE ? af_launch<false>(a, cfg->refine_iters, stream)
-                                  : af_launch<true>(a, cfg->refine_iters, stream);
+  return cfg->model == GEO_AFFINE ? geo_launch<AfRansac<false>>(a, geo_prepare_kernel, stream)
+                                  : geo_launch<AfRansac<true>>(a, geo_prepare_kernel, stream);
 }

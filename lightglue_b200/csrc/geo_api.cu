@@ -1,34 +1,21 @@
 // Batched RANSAC on the matcher's output (include/geometry_b200.h, which states the algorithm step by step).
 //
 // Launches, all fixed by (B, M, max_iters):
-//   prepare  one 1024-thread CTA per pair: ordered compaction of the valid matches, Hartley normalisation
+//   prepare  geo_prepare_kernel, one 1024-thread CTA per pair: ordered compaction of the valid matches, Hartley
+//            normalisation
 //   per chunk of GEO_CHUNK hypotheses:
-//     hyp    one CTA per pair: folds the previous chunk's counts into the pair's best (geo_fold), decides the
-//            adaptive stop, then one thread per hypothesis draws and solves its sample in double
-//     score  (B, splits) CTAs: each streams a slice of the pair's points through shared memory against the chunk's
-//            fp32 models, one thread per hypothesis, and adds its inlier counts
-//   refit    one CTA per pair: folds the last chunk, least-squares refit on the best hypothesis's inliers, recount,
-//            outputs
+//     hyp    geo_hyp_kernel, one CTA per pair: folds the previous chunk's counts into the pair's best (geo_fold),
+//            decides the adaptive stop, then one thread per hypothesis draws and solves its sample in double
+//     score  geo_score_kernel<HfScore>, (B, splits) CTAs: each streams a slice of the pair's points through shared
+//            memory against the chunk's fp32 models, one thread per hypothesis, and adds its inlier counts
+//   final    geo_final_kernel<HfRansac>, one CTA per pair: folds the last chunk, least-squares refit on the best
+//            hypothesis's inliers, recount, outputs
 // A stopped pair's CTAs return at once.  This file is compiled with -fmad=false: every multiply and add rounds on its
 // own, as numpy's do in oracle/geometry_oracle.py.
 #include "geo_hf.cuh"
 #include "lg_internal.h"
 
 namespace {
-
-__global__ void __launch_bounds__(GEO_CHUNK, 1) geo_hyp_kernel(GeoArgs a, int c) {
-  const int b = blockIdx.x, t = threadIdx.x;
-  if (c > 0) geo_fold<1>(a, a.s, b, c - 1);
-  const GeoPair& P = a.w.pair[b];
-  const int h = c * GEO_CHUNK + t;
-  double m[9];
-  const bool ok = P.stop == 0 && h < a.max_iters && geo_hypothesis(a, P, a.w.pts + (long)b * a.M, h, m);
-  if (ok) {
-    float* hm = a.w.hyp + ((long)b * GEO_CHUNK + t) * 9;
-    for (int i = 0; i < 9; ++i) hm[i] = (float)m[i];
-  }
-  a.w.count[(long)b * GEO_CHUNK + t] = ok ? 0 : -1;
-}
 
 // H or F inlier counts, the model kind read at run time
 struct HfScore {
@@ -60,88 +47,44 @@ __device__ __forceinline__ int geo_rows(int kind, const GeoPair& P, float4 p, do
   return 1;
 }
 
-__global__ void __launch_bounds__(RED, 1) geo_refit_kernel(GeoArgs a) {
-  const int b = blockIdx.x, t = threadIdx.x;
-  geo_fold<1>(a, a.s, b, a.chunks - 1);
-  const GeoPair& P = a.w.pair[b];
-  const float4* pts = a.w.pts + (long)b * a.M;
-  const int* idx = a.w.idx + (long)b * a.M;
-  uint8_t* inl = a.out.inliers + (long)b * a.M;
-  __shared__ double red[RED];
-  __shared__ double ata[45];
-  __shared__ double model[2][9];
-  __shared__ float fm[2][9];
-  __shared__ int count[2];
-  for (int i = t; i < a.M; i += RED) inl[i] = 0;
-  const unsigned long long key = P.best;
-  if (!P.ok || key == 0) {
+// H or F for geo_final_kernel: least-squares refit on the best hypothesis's inliers (header step 7)
+struct HfRansac : HfSolver {
+  using Base = GeoArgs;
+  using Score = HfScore;
+  struct Scratch {
+    double red[RED];
+    double ata[45];
+  };
+
+  static __device__ bool inlier(const GeoArgs& a, int b, const float* g, int k) {
+    return geo_err(a.kind, g, a.w.pts[(long)b * a.M + k]) < a.thr2;
+  }
+  static __device__ void clear(const GeoArgs& a, int b, int t) {
+    for (int i = t; i < a.M; i += RED) a.out.inliers[(long)b * a.M + i] = 0;
+  }
+  static __device__ void fail(const GeoArgs& a, int b, int t) {
     if (t < 9) a.out.model[(long)b * 9 + t] = 0.0;
-    if (t == 0) {
-      a.out.num_inliers[b] = 0;
-      a.out.success[b] = 0;
-      a.out.best_hypothesis[b] = -1;
-      a.out.num_hypotheses[b] = P.drawn;
-    }
-    return;
   }
-  const unsigned hb = ~(unsigned)(key & 0xffffffffu) >> 4;
-  const int hcount = (int)(key >> 32) - 1;
-  if (t == 0) {
-    geo_hypothesis(a, P, pts, hb, model[0]);
-    for (int i = 0; i < 9; ++i) fm[0][i] = (float)model[0][i];
-    count[0] = hcount;
-    count[1] = -1;
-  }
-  __syncthreads();
-  if (hcount >= a.s) {
-    // one pass over the points per row i of the upper triangle keeps 9 accumulators in registers
-    for (int i = 0, e0 = 0; i < 9; e0 += 9 - i, ++i) {
-      double acc[9];
-#pragma unroll
-      for (int j = 0; j < 9; ++j) acc[j] = 0.0;
-      for (int k = t; k < P.n; k += RED) {
-        const float4 p = pts[k];
-        if (!(geo_err(a.kind, fm[0], p) < a.thr2)) continue;
-        double ra[9], rb[9];
-        const int rows = geo_rows(a.kind, P, p, ra, rb);
-#pragma unroll
-        for (int j = 0; j < 9; ++j)
-          if (j >= i) acc[j] = acc[j] + (rows == 2 ? ra[i] * ra[j] + rb[i] * rb[j] : ra[i] * ra[j]);
-      }
-#pragma unroll
-      for (int j = 0; j < 9; ++j)
-        if (j >= i) {
-          const double s = tree_sum(acc[j], red, t);
-          if (t == 0) ata[e0 + j - i] = s;
-        }
-    }
+  static __device__ bool refits(const GeoArgs& a, int hcount) { return hcount >= a.s; }
+
+  static __device__ void refit(GeoFinal<HfRansac>& s, const GeoArgs& a, int b, int t) {
+    const GeoPair& P = a.w.pair[b];
+    const float4* pts = a.w.pts + (long)b * a.M;
+    geo_ata(P.n, [&](int k) { return inlier(a, b, s.fm[0], k); },
+            [&](int k, double* ra, double* rb) { return geo_rows(a.kind, P, pts[k], ra, rb); }, s.m.red, s.m.ata, t);
     if (t == 0) {
-      double A[9][9], v[9];
-      for (int i = 0, e = 0; i < 9; ++i)
-        for (int j = i; j < 9; ++j, ++e) A[i][j] = A[j][i] = ata[e];
-      smallest_eigvec<9>(A, v);
+      double v[9];
+      ata_null_vector(s.m.ata, v);
       if (a.kind == GEO_FUNDAMENTAL) rank2(v);
-      denormalise(a.kind, P, v, model[1]);
-      for (int i = 0; i < 9; ++i) fm[1][i] = (float)model[1][i];
-      count[1] = 0;
+      denormalise(a.kind, P, v, s.x[1]);
     }
-    __syncthreads();
-    int k1 = 0;
-    for (int k = t; k < P.n; k += RED) k1 += geo_err(a.kind, fm[1], pts[k]) < a.thr2;
-    if (k1) atomicAdd(&count[1], k1);
-    __syncthreads();
   }
-  const int u = count[1] >= count[0] ? 1 : 0;
-  for (int k = t; k < P.n; k += RED)
-    if (geo_err(a.kind, fm[u], pts[k]) < a.thr2) inl[idx[k]] = 1;
-  if (t < 9) a.out.model[(long)b * 9 + t] = model[u][t];
-  if (t == 0) {
-    a.out.num_inliers[b] = count[u];
-    a.out.success[b] = 1;
-    a.out.best_hypothesis[b] = (int)hb;
-    a.out.num_hypotheses[b] = P.drawn;
+
+  static __device__ void write(GeoFinal<HfRansac>& s, const GeoArgs& a, int b, int u, int t) {
+    geo_write_mask<HfRansac>(a, b, s.fm[u], t);
+    if (t < 9) a.out.model[(long)b * 9 + t] = s.px[u][t];
   }
-}
+};
 
 }  // namespace
 
@@ -174,17 +117,5 @@ extern "C" int geo_estimate(const GeoConfig* cfg, const GeoInputs* in, GeoOutput
   a.confidence = cfg->confidence;
   a.kpts0 = in->kpts0; a.kpts1 = in->kpts1; a.matches0 = in->matches0;
   a.out = *out;
-  const int splits = geo_score_splits(a.B, a.M);
-  const cudaStream_t stream = (cudaStream_t)stream_;
-  geo_prepare_kernel<<<a.B, 1024, 0, stream>>>(a);
-  LG_CHECK_LAUNCH();
-  for (int c = 0; c < a.chunks; ++c) {
-    geo_hyp_kernel<<<a.B, GEO_CHUNK, 0, stream>>>(a, c);
-    LG_CHECK_LAUNCH();
-    geo_score_kernel<HfScore><<<dim3(a.B, splits), GEO_CHUNK, 0, stream>>>(a);
-    LG_CHECK_LAUNCH();
-  }
-  geo_refit_kernel<<<a.B, RED, 0, stream>>>(a);
-  LG_CHECK_LAUNCH();
-  return 0;
+  return geo_launch<HfRansac>(a, geo_prepare_kernel, (cudaStream_t)stream_);
 }

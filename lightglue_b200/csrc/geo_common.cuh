@@ -154,6 +154,10 @@ __device__ void smallest_eigvec(double (*A)[N], double* out) {
 template <class Ws>
 __device__ __forceinline__ int geo_models(const Ws& w, long slot) { return w.nsol[slot]; }
 
+// Records that chunk slot `slot` holds ns models, as geo_models reads it back
+template <class Ws>
+__device__ __forceinline__ void geo_set_models(const Ws& w, long slot, int ns) { w.nsol[slot] = ns; }
+
 // Folds chunk c's counts (SOLS per sample) into the pair's best and decides whether the pair stops after s-point
 // samples.  The best is packed (count + 1) << 32 | ~(h * 16 + r) and kept by atomic max, so ties go to the smallest
 // hypothesis h, then solution r.  Called by every thread of a GEO_CHUNK-thread CTA; thread t owns sample
@@ -231,6 +235,184 @@ __global__ void __launch_bounds__(GEO_CHUNK) geo_score_kernel(typename Q::Args a
 #pragma unroll
   for (int r = 0; r < Q::SOLS; ++r)
     if (r < ns && k[r]) atomicAdd(q.sums + slot * Q::SOLS + r, k[r]);
+}
+
+// The hyp launch of a chunk runs on a Solver, the estimator's minimal solve:
+//   SOLS, NX and NF: up to SOLS solutions of NX doubles per sample, each scored as a pixel model of NF floats;
+//   s(a), the points per sample;
+//   solve(a, b, h, x), sample h of pair b solved into x[0..ns-1], returning ns (0 for a degenerate sample);
+//   pixels(a, b, x, px), a solution's pixel model.
+// The schedule is picked by the argument type: plain RANSAC (Base) folds the previous chunk on entry and zeroes the
+// inlier counts; LO-RANSAC (LoArgs<Base>, lo_common.cuh) resets the pair's LO state and zeroes the MSAC sums.
+template <class Solver, class Base>
+__device__ __forceinline__ const Base& geo_enter(const Base& a, int b, int c) {
+  if (c > 0) geo_fold<Solver::SOLS>(a, Solver::s(a), b, c - 1);
+  return a;
+}
+
+template <class Base>
+__device__ __forceinline__ int* geo_sums(const Base& a) { return a.w.count; }
+
+// Chunk c's hypotheses, one CTA per pair, one thread per sample: solved in double, rounded into w.hyp
+template <class Solver, class Args>
+__global__ void __launch_bounds__(GEO_CHUNK, 1) geo_hyp_kernel(Args a, int c) {
+  const int b = blockIdx.x, t = threadIdx.x;
+  const auto& p = geo_enter<Solver>(a, b, c);
+  const auto& P = p.w.pair[b];
+  const int h = c * GEO_CHUNK + t;
+  const long slot = (long)b * GEO_CHUNK + t;
+  int ns = 0;
+  if (P.stop == 0 && h < p.max_iters) {
+    double x[Solver::SOLS][Solver::NX];
+    ns = Solver::solve(p, b, h, x);
+    float* hm = p.w.hyp + slot * Solver::SOLS * Solver::NF;
+    for (int r = 0; r < ns; ++r) {
+      double px[Solver::NF];
+      Solver::pixels(p, b, x[r], px);
+      for (int i = 0; i < Solver::NF; ++i) hm[r * Solver::NF + i] = (float)px[i];
+      geo_sums(a)[slot * Solver::SOLS + r] = 0;
+    }
+  }
+  // On the plain H/F workspace the one count is also the slot's model record, so a valid slot gets the same 0 again
+  geo_set_models(p.w, slot, ns);
+}
+
+// The upper triangle of A^T A (45 sums, row-major) over the points k < n with inlier(k), each adding the rows that
+// rows(k, ra, rb) fills (it returns 1 or 2), in step 2's fixed order.  One pass over the points per row i keeps 9
+// accumulators in registers.  Every thread of a RED-thread CTA calls it; ata is valid on thread 0.
+template <class Inlier, class Rows>
+__device__ void geo_ata(int n, Inlier inlier, Rows rows, double* red, double* ata, int t) {
+  for (int i = 0, e0 = 0; i < 9; e0 += 9 - i, ++i) {
+    double acc[9];
+#pragma unroll
+    for (int j = 0; j < 9; ++j) acc[j] = 0.0;
+    for (int k = t; k < n; k += RED) {
+      if (!inlier(k)) continue;
+      double ra[9], rb[9];
+      const int nr = rows(k, ra, rb);
+#pragma unroll
+      for (int j = 0; j < 9; ++j)
+        if (j >= i) acc[j] = acc[j] + (nr == 2 ? ra[i] * ra[j] + rb[i] * rb[j] : ra[i] * ra[j]);
+    }
+#pragma unroll
+    for (int j = 0; j < 9; ++j)
+      if (j >= i) {
+        const double s = tree_sum(acc[j], red, t);
+        if (t == 0) ata[e0 + j - i] = s;
+      }
+  }
+}
+
+// The smallest-eigenvalue eigenvector of the symmetric 9x9 whose upper triangle is ata (geo_ata's layout)
+__device__ __forceinline__ void ata_null_vector(const double* ata, double* v) {
+  double A[9][9];
+  for (int i = 0, e = 0; i < 9; ++i)
+    for (int j = i; j < 9; ++j, ++e) A[i][j] = A[j][i] = ata[e];
+  smallest_eigvec<9>(A, v);
+}
+
+// The final kernel's shared state: the best hypothesis re-solved (0) and its refit (1)
+template <class Est>
+struct GeoFinal {
+  double x[2][Est::NX];   // the solutions
+  double px[2][Est::NF];  // their pixel models
+  float fm[2][Est::NF];   // rounded to float
+  int count[2];           // their inliers; count[1] == -1: no refit
+  typename Est::Scratch m;
+};
+
+// The final launch of plain RANSAC, one RED-thread CTA per pair: folds the last chunk, solves the best hypothesis again
+// in double, refits it on its inliers, keeps the refit unless it has fewer inliers, and writes the outputs.  Est is the
+// Solver with:
+//   Base, the kernel's arguments; Score, its geo_score_kernel policy; Scratch, its shared state in GeoFinal;
+//   clear(a, b, t), the masks set to 0 before anything else (every thread);
+//   fail(a, b, t), the model fields of a pair without a model (every thread);
+//   refits(a, hcount), whether a best hypothesis with hcount inliers is refitted;
+//   refit(s, a, b, t), s.x[1] from s.x[0] on the inliers of s.fm[0] (every thread, ends with s.x[1] on thread 0);
+//   inlier(a, b, g, k), the fp32 test of compacted point k against the float model g;
+//   write(s, a, b, u, t), the masks and model fields of solution u of s (every thread).
+template <class Est>
+__global__ void __launch_bounds__(RED, 1) geo_final_kernel(typename Est::Base a) {
+  const int b = blockIdx.x, t = threadIdx.x;
+  geo_fold<Est::SOLS>(a, Est::s(a), b, a.chunks - 1);
+  const auto& P = a.w.pair[b];
+  const auto& o = a.out;
+  __shared__ GeoFinal<Est> s;
+  Est::clear(a, b, t);
+  const unsigned long long key = P.best;
+  if (!P.ok || key == 0) {
+    Est::fail(a, b, t);
+    if (t == 0) {
+      o.num_inliers[b] = 0;
+      o.success[b] = 0;
+      o.best_hypothesis[b] = -1;
+      if constexpr (Est::SOLS > 1) o.best_solution[b] = -1;  // only an estimator with several solutions reports one
+      o.num_hypotheses[b] = P.drawn;
+    }
+    return;
+  }
+  const unsigned hr = ~(unsigned)(key & 0xffffffffu);
+  const int hcount = (int)(key >> 32) - 1;
+  if (t == 0) {
+    double x[Est::SOLS][Est::NX];
+    Est::solve(a, b, hr >> 4, x);
+    for (int i = 0; i < Est::NX; ++i) s.x[0][i] = x[hr & 15][i];
+    Est::pixels(a, b, s.x[0], s.px[0]);
+    for (int i = 0; i < Est::NF; ++i) s.fm[0][i] = (float)s.px[0][i];
+    s.count[0] = hcount;
+    s.count[1] = -1;
+  }
+  __syncthreads();
+  if (Est::refits(a, hcount)) {
+    Est::refit(s, a, b, t);
+    if (t == 0) {
+      Est::pixels(a, b, s.x[1], s.px[1]);
+      for (int i = 0; i < Est::NF; ++i) s.fm[1][i] = (float)s.px[1][i];
+      s.count[1] = 0;
+    }
+    __syncthreads();
+    int k1 = 0;
+    for (int k = t; k < P.n; k += RED) k1 += Est::inlier(a, b, s.fm[1], k);
+    if (k1) atomicAdd(&s.count[1], k1);
+    __syncthreads();
+  }
+  const int u = s.count[1] >= s.count[0] ? 1 : 0;
+  Est::write(s, a, b, u, t);
+  if (t == 0) {
+    o.num_inliers[b] = s.count[u];
+    o.success[b] = 1;
+    o.best_hypothesis[b] = (int)(hr >> 4);
+    if constexpr (Est::SOLS > 1) o.best_solution[b] = (int)(hr & 15);
+    o.num_hypotheses[b] = P.drawn;
+  }
+}
+
+// The mask of the inliers of float model g, by row of matches0 through w.idx (every thread; clear(a, b, t) zeroed it)
+template <class Est>
+__device__ void geo_write_mask(const typename Est::Base& a, int b, const float* g, int t) {
+  const int* idx = a.w.idx + (long)b * a.M;
+  uint8_t* inl = a.out.inliers + (long)b * a.M;
+  for (int k = t; k < a.w.pair[b].n; k += RED)
+    if (Est::inlier(a, b, g, k)) inl[idx[k]] = 1;
+}
+
+// Every plain estimator's launches, all fixed by (B, M, max_iters): prepare, the estimator's compaction kernel; per
+// chunk of GEO_CHUNK samples, geo_hyp_kernel and geo_score_kernel (the inlier counts of every solution); then
+// geo_final_kernel.  The caller launches the estimator's tail after it.  Returns 0 or the launch error.
+template <class Est, class Base>
+int geo_launch(const Base& a, void (*prepare)(Base), cudaStream_t stream) {
+  const int splits = geo_score_splits(a.B, a.M);
+  prepare<<<a.B, 1024, 0, stream>>>(a);
+  LG_CHECK_LAUNCH();
+  for (int c = 0; c < a.chunks; ++c) {
+    geo_hyp_kernel<Est, Base><<<a.B, GEO_CHUNK, 0, stream>>>(a, c);
+    LG_CHECK_LAUNCH();
+    geo_score_kernel<typename Est::Score><<<dim3(a.B, splits), GEO_CHUNK, 0, stream>>>(a);
+    LG_CHECK_LAUNCH();
+  }
+  geo_final_kernel<Est><<<a.B, RED, 0, stream>>>(a);
+  LG_CHECK_LAUNCH();
+  return 0;
 }
 
 // ---- host side of the entry points ----

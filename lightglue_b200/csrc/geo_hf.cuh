@@ -42,11 +42,13 @@ size_t carve(char* base, int B, int M, GeoWs* w) {
 
 // geo_fold's and geo_score_kernel's valid models of chunk slot `slot`: one, unless degenerate or not drawn
 __device__ __forceinline__ int geo_models(const GeoWs& w, long slot) { return w.count[slot] >= 0; }
+__device__ __forceinline__ void geo_set_models(const GeoWs& w, long slot, int ns) { w.count[slot] = ns ? 0 : -1; }
 
 struct GeoArgs {
   int B, M, N, kind, s, max_iters, chunks;
   unsigned seed;
   float thr2;
+  int refine_iters;  // the affine refinement's LM steps
   double confidence;
   const float* kpts0;
   const float* kpts1;
@@ -196,6 +198,18 @@ __device__ bool geo_hypothesis(const GeoArgs& a, const GeoPair& P, const float4*
   denormalise(a.kind, P, v, model);
   return true;
 }
+
+// geo_hyp_kernel's solver of H or F (a.kind and a.s pick it): one pixel model per sample
+struct HfSolver {
+  static constexpr int SOLS = 1, NX = 9, NF = 9;
+  static __device__ int s(const GeoArgs& a) { return a.s; }
+  static __device__ int solve(const GeoArgs& a, int b, unsigned h, double (*x)[NX]) {
+    return geo_hypothesis(a, a.w.pair[b], a.w.pts + (long)b * a.M, h, x[0]);
+  }
+  static __device__ void pixels(const GeoArgs&, int, const double* x, double* px) {
+    for (int i = 0; i < NF; ++i) px[i] = x[i];
+  }
+};
 
 // fp32 error of one correspondence (header step 5)
 __device__ __forceinline__ float geo_err(int kind, const float* h, float4 p) {

@@ -61,12 +61,14 @@ struct LoShared {
   int take, step_ok;
 };
 
-// steps LM steps from s.x, in place (header steps L7, LH7, LF7, LA7); every thread of the CTA calls it
+// steps LM steps from s.x at damping lam0, in place (header steps L7, LH7, LF7, LA7, A7 and AF6); every thread of the
+// CTA calls it
 template <class Model, class Pair, class Points>
-__device__ void lo_refine(LoShared<Model>& s, const Pair& P, Points pts, int n, double thr2, int steps, int tid) {
+__device__ void lo_refine(LoShared<Model>& s, const Pair& P, Points pts, int n, double thr2, int steps, double lam0,
+                          int tid) {
   constexpr int NH = Model::DOF * (Model::DOF + 1) / 2;
   Model::terms(s, P, s.x, pts, n, thr2, s.sums, tid);
-  double lam = GEO_LO_LAMBDA0;  // every thread keeps the same schedule
+  double lam = lam0;  // every thread keeps the same schedule
   for (int it = 0; it < steps; ++it) {
     if (tid == 0) {
       double d[Model::DOF];
@@ -149,7 +151,7 @@ size_t lo_workspace_bytes(int B, int M) {
   return lo_carve<Est>(nullptr, B, M, &a) + 256;
 }
 
-// Pair b's LO state before its first chunk; every hyp kernel calls it
+// Pair b's LO state before its first chunk
 __device__ __forceinline__ void lo_reset(const LoWs& l, int b, int c) {
   if (c == 0 && threadIdx.x == 0) {
     LoPair& L = l.pair[b];
@@ -160,9 +162,19 @@ __device__ __forceinline__ void lo_reset(const LoWs& l, int b, int c) {
   }
 }
 
+// geo_hyp_kernel's LO-RANSAC schedule (geo_common.cuh): lo_reset on entry, and the MSAC sums zeroed
+template <class Solver, class Base>
+__device__ __forceinline__ const Base& geo_enter(const LoArgs<Base>& a, int b, int c) {
+  lo_reset(a.l, b, c);
+  return a.p;
+}
+
+template <class Base>
+__device__ __forceinline__ unsigned long long* geo_sums(const LoArgs<Base>& a) { return a.l.acc; }
+
 // The schedule runs over Est, the estimator's model policy (LoShared above) with:
-//   Base, its RANSAC arguments (a.p.w.pair[b] the pair, a.p.out the outputs); Score, its geo_score_kernel policy; S,
-//   the points per sample; SOLS, the solutions per sample;
+//   Base, its RANSAC arguments (a.p.w.pair[b] the pair, a.p.out the outputs); Solver, its geo_hyp_kernel solver;
+//   Score, its geo_score_kernel policy; S, the points per sample; SOLS, the solutions per sample;
 //   points(a, b), consts(a, b) and thr2(a, b), pair b's points, constants and squared threshold as the LM loop reads
 //   them;
 //   seed(s, a, b, hr, m, L, t), the LM start s.x of solution hr (index m of acc) and L.model of it (every thread; a
@@ -207,7 +219,7 @@ __global__ void __launch_bounds__(RED, 1) lo_chunk_kernel(LoArgs<typename Est::B
     __syncthreads();
     const auto pts = Est::points(a, b);
     const float thr2 = Est::thr2(a, b);
-    lo_refine(s, Est::consts(a, b), pts, P.n, (double)thr2, GEO_LO_STEPS, t);
+    lo_refine(s, Est::consts(a, b), pts, P.n, (double)thr2, GEO_LO_STEPS, GEO_LO_LAMBDA0, t);
     lo_rescore(s, Est::consts(a, b), pts, P.n, thr2, t);
     if (t == 0 && (s.score & LO_SCORE_MASK) < L.score) {
       Est::store(s, L);
@@ -251,7 +263,7 @@ __global__ void __launch_bounds__(RED, 1) lo_final_kernel(LoArgs<typename Est::B
   const float thr2 = Est::thr2(a, b);
   Est::load(s, a, b, L, t);
   __syncthreads();
-  lo_refine(s, Est::consts(a, b), pts, P.n, (double)thr2, GEO_LO_FINAL_STEPS, t);
+  lo_refine(s, Est::consts(a, b), pts, P.n, (double)thr2, GEO_LO_FINAL_STEPS, GEO_LO_LAMBDA0, t);
   lo_rescore(s, Est::consts(a, b), pts, P.n, thr2, t);
   if (t == 0) s.take = (s.score & LO_SCORE_MASK) > L.score;
   __syncthreads();
@@ -269,11 +281,11 @@ __global__ void __launch_bounds__(RED, 1) lo_final_kernel(LoArgs<typename Est::B
 }
 
 // Every LO estimator's launches, all fixed by (B, M, max_iters): prepare, the estimator's compaction kernel; per chunk
-// of GEO_CHUNK samples, hyp (one CTA per pair, one thread per sample: the minimal solutions, fp32), geo_score_kernel
-// (count << 40 | MSAC score of every solution) and lo_chunk_kernel (one CTA per pair); then lo_final_kernel.
+// of GEO_CHUNK samples, geo_hyp_kernel (one CTA per pair, one thread per sample: the minimal solutions, fp32),
+// geo_score_kernel (count << 40 | MSAC score of every solution) and lo_chunk_kernel (one CTA per pair); then
+// lo_final_kernel.
 template <class Est, class Base>
-int lo_launch(const Base& p, int32_t* num_lo, int64_t* cost, void* workspace, void (*prepare)(Base),
-              void (*hyp)(LoArgs<Base>, int), void* stream_) {
+int lo_launch(const Base& p, int32_t* num_lo, int64_t* cost, void* workspace, void (*prepare)(Base), void* stream_) {
   LoArgs<Base> a{p, {}, num_lo, cost};
   lo_carve<Est>(geo_workspace_base(workspace), p.B, p.M, &a);
   const int splits = geo_score_splits(p.B, p.M);
@@ -281,7 +293,7 @@ int lo_launch(const Base& p, int32_t* num_lo, int64_t* cost, void* workspace, vo
   prepare<<<p.B, 1024, 0, stream>>>(a.p);
   LG_CHECK_LAUNCH();
   for (int c = 0; c < p.chunks; ++c) {
-    hyp<<<p.B, GEO_CHUNK, 0, stream>>>(a, c);
+    geo_hyp_kernel<typename Est::Solver, LoArgs<Base>><<<p.B, GEO_CHUNK, 0, stream>>>(a, c);
     LG_CHECK_LAUNCH();
     geo_score_kernel<typename Est::Score><<<dim3(p.B, splits), GEO_CHUNK, 0, stream>>>(a);
     LG_CHECK_LAUNCH();

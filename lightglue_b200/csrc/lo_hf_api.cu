@@ -2,10 +2,10 @@
 // eight-point (F) sampling with Levenberg-Marquardt local optimisation and a final refinement (include/geometry_b200.h,
 // steps LH1-LH8 and LF1-LF8).  H is refined at unit norm in the tangent space of the sphere, F at rank 2 in its
 // orthonormal representation (U, V, sigma).  Both run on lo_common.cuh's schedule: geo_api.cu's compaction and
-// Hartley normalisation kernel prepares the pair; hyp makes step 4's minimal solve, one model per sample (r = 0); a
-// local optimisation starts from the hypothesis solved again in double and runs LM on the truncated transfer (H) or
-// Sampson (F) cost.  Compiled with -fmad=false: oracle/lo_homography_oracle.py and oracle/lo_fundamental_oracle.py take
-// the same steps.
+// Hartley normalisation kernel prepares the pair; geo_hyp_kernel makes step 4's minimal solve, one model per sample
+// (r = 0); a local optimisation starts from the hypothesis solved again in double and runs LM on the truncated
+// transfer (H) or Sampson (F) cost.  Compiled with -fmad=false: oracle/lo_homography_oracle.py and
+// oracle/lo_fundamental_oracle.py take the same steps.
 #include <stdint.h>
 
 #include "geo_hf.cuh"
@@ -13,22 +13,6 @@
 #include "lo_common.cuh"
 
 namespace {
-
-// Step 4's hypotheses of chunk c (a.p.kind and a.p.s pick H or F), one thread per sample
-__global__ void __launch_bounds__(GEO_CHUNK, 1) lohf_hyp_kernel(LoArgs<GeoArgs> a, int c) {
-  const int b = blockIdx.x, t = threadIdx.x;
-  lo_reset(a.l, b, c);
-  const GeoPair& P = a.p.w.pair[b];
-  const int h = c * GEO_CHUNK + t;
-  double m[9];
-  const bool ok = P.stop == 0 && h < a.p.max_iters && geo_hypothesis(a.p, P, a.p.w.pts + (long)b * a.p.M, h, m);
-  if (ok) {
-    float* hm = a.p.w.hyp + ((long)b * GEO_CHUNK + t) * 9;
-    for (int i = 0; i < 9; ++i) hm[i] = (float)m[i];
-    a.l.acc[(long)b * GEO_CHUNK + t] = 0;
-  }
-  a.p.w.count[(long)b * GEO_CHUNK + t] = ok ? 0 : -1;
-}
 
 // The chunk's LH3 / LF3 scores, count << 40 | MSAC score
 template <int KIND>
@@ -88,6 +72,7 @@ template <class Model>
 struct HfLo {
   using Base = GeoArgs;
   using Args = LoArgs<GeoArgs>;
+  using Solver = HfSolver;
   static constexpr int SOLS = 1;
 
   static __device__ const float4* points(const Args& a, int b) { return a.p.w.pts + (long)b * a.p.M; }
@@ -97,7 +82,7 @@ struct HfLo {
   // LH4 / LF4: hypothesis h solved again in double
   static __device__ void seed(LoShared<Model>& s, const Args& a, int b, unsigned hr, long, LoPair& L, int t) {
     if (t == 0) {
-      geo_hypothesis(a.p, a.p.w.pair[b], points(a, b), hr >> 4, L.model);
+      HfSolver::solve(a.p, b, hr >> 4, (double(*)[9])L.model);
       Model::start(s, a.p.w.pair[b], L.model);
     }
   }
@@ -399,8 +384,7 @@ int lohf_estimate(const char* name, const GeoConfig* cfg, const GeoInputs* in, G
   g.confidence = cfg->confidence;
   g.kpts0 = in->kpts0; g.kpts1 = in->kpts1; g.matches0 = in->matches0;
   g.out = out->geo;
-  return lo_launch<Model>(g, out->num_local_optimizations, out->cost, workspace, geo_prepare_kernel, lohf_hyp_kernel,
-                          stream_);
+  return lo_launch<Model>(g, out->num_local_optimizations, out->cost, workspace, geo_prepare_kernel, stream_);
 }
 
 }  // namespace

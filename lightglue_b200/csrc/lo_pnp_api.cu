@@ -1,8 +1,8 @@
 // Batched LO-RANSAC absolute pose on the matcher's 2D-3D matches: MSAC-scored Lambda Twist P3P sampling with
 // Levenberg-Marquardt local optimisation of (R, t) and a final refinement (include/geometry_b200.h, steps LA1-LA8), on
-// lo_common.cuh's schedule.  pnp_api.cu's compaction and calibration kernel prepares the pair; hyp draws up to 4 P3P
-// solutions as fp32 projections; a local optimisation starts from its solution re-solved in double and runs LM on the
-// truncated reprojection cost; the final kernel writes the inlier mask of every row of matches0.  Compiled with
+// lo_common.cuh's schedule.  pnp_api.cu's compaction and calibration kernel prepares the pair; geo_hyp_kernel draws up
+// to 4 P3P solutions as fp32 projections; a local optimisation starts from its solution re-solved in double and runs LM
+// on the truncated reprojection cost; the final kernel writes the inlier mask of every row of matches0.  Compiled with
 // -fmad=false: oracle/lo_pnp_oracle.py takes the same steps.
 #include <stdint.h>
 
@@ -22,28 +22,6 @@ struct PnpPoints {
   const float4* wld;
   __device__ __forceinline__ PnpPoint operator[](int k) const { return {pix[k], wld[k]}; }
 };
-
-__global__ void __launch_bounds__(GEO_CHUNK, 1) lopnp_hyp_kernel(LoArgs<PnpArgs> a, int c) {
-  const int b = blockIdx.x, t = threadIdx.x;
-  lo_reset(a.l, b, c);
-  const PnpPair& P = a.p.w.pair[b];
-  const int h = c * GEO_CHUNK + t;
-  int ns = 0;
-  int id[S];
-  if (P.stop == 0 && h < a.p.max_iters && geo_sample(a.p.seed, h, P.n, S, id) == S) {
-    double Rs[SOLS][9], ts[SOLS][3];
-    ns = p3p(a.p.w.pts + (long)b * a.p.M, a.p.w.wld + (long)b * a.p.M, id, Rs, ts);
-    const double* K = a.p.K0 + (long)b * 9;
-    float* hm = a.p.w.hyp + ((long)b * GEO_CHUNK + t) * SOLS * 12;
-    for (int r = 0; r < ns; ++r) {
-      double Pm[12];
-      projection(K, Rs[r], ts[r], Pm);
-      for (int i = 0; i < 12; ++i) hm[r * 12 + i] = (float)Pm[i];
-      a.l.acc[((long)b * GEO_CHUNK + t) * SOLS + r] = 0;
-    }
-  }
-  a.p.w.nsol[(long)b * GEO_CHUNK + t] = ns;
-}
 
 // The chunk's LA3 scores of every projection, count << 40 | MSAC score, on a tile of pixels and world points
 struct LoPnpScore {
@@ -68,44 +46,22 @@ struct PnpLo {
   static constexpr int DOF = 6, TERMS = 28, GROUP = 14, NP = 12, NF = 12, S = ::S, SOLS = ::SOLS;
   using Base = PnpArgs;
   using Args = LoArgs<PnpArgs>;
+  using Solver = PnpSolver;
   using Score = LoPnpScore;
   struct Scratch {};
 
   // The TERMS sums at x: A7's Jacobian over the points in front of the camera with err < thr2, and the truncated cost
   static __device__ void terms(LoShared<PnpLo>& s, const double* K, const double* x, PnpPoints pts, int n, double thr2,
                                double* out, int tid) {
-    const double fx = K[0], sk = K[1], cx = K[2], fy = K[4], cy = K[5];
-    const double* R = x;
-    const double* t = x + 9;
     double acc[TERMS];
 #pragma unroll
     for (int i = 0; i < TERMS; ++i) acc[i] = 0.0;
     for (int k = tid; k < n; k += RED) {
-      const float4 p = pts.pix[k], q = pts.wld[k];
-      const double u = p.x, v = p.y, W[3] = {q.x, q.y, q.z};
-      double Xc[3];
-      for (int i = 0; i < 3; ++i) Xc[i] = R[3 * i] * W[0] + R[3 * i + 1] * W[1] + R[3 * i + 2] * W[2] + t[i];
-      const double iz = 1.0 / Xc[2];
-      const double ax = Xc[0] * iz, bx = Xc[1] * iz;
-      const double pu = fx * ax + sk * bx;
-      const double ru = pu + cx - u, rv = fy * bx + cy - v;
-      const double err = ru * ru + rv * rv;
-      const bool in = Xc[2] > 0.0 && err < thr2;
+      const PnpResidual e = pnp_residual(K, x, x + 9, pts.pix[k], pts.wld[k]);
+      const double err = e.ru * e.ru + e.rv * e.rv;
+      const bool in = e.Xc[2] > 0.0 && err < thr2;
       acc[TERMS - 1] = acc[TERMS - 1] + (in ? err : thr2);
-      if (!in) continue;
-      const double gu[3] = {fx * iz, sk * iz, -(pu * iz)};
-      const double gv[3] = {0.0, fy * iz, -(fy * bx * iz)};
-      const double ju[6] = {gu[2] * Xc[1] - gu[1] * Xc[2], gu[0] * Xc[2] - gu[2] * Xc[0], gu[1] * Xc[0] - gu[0] * Xc[1],
-                            gu[0], gu[1], gu[2]};
-      const double jv[6] = {gv[2] * Xc[1] - gv[1] * Xc[2], gv[0] * Xc[2] - gv[2] * Xc[0], gv[1] * Xc[0] - gv[0] * Xc[1],
-                            gv[0], gv[1], gv[2]};
-      int e = 0;
-#pragma unroll
-      for (int i = 0; i < DOF; ++i)
-#pragma unroll
-        for (int j = i; j < DOF; ++j, ++e) acc[e] = acc[e] + (ju[i] * ju[j] + jv[i] * jv[j]);
-#pragma unroll
-      for (int i = 0; i < DOF; ++i) acc[21 + i] = acc[21 + i] + (ju[i] * ru + jv[i] * rv);
+      if (in) pnp_add_normal(K, e, acc);
     }
     lo_tree_sums<TERMS, GROUP>(acc, s.red, out, tid);
   }
@@ -131,13 +87,9 @@ struct PnpLo {
   // LA4: sample h re-solved in double, as the score's projections were solved
   static __device__ void seed(LoShared<PnpLo>& s, const Args& a, int b, unsigned hr, long, LoPair& L, int t) {
     if (t == 0) {
-      const PnpPoints pts = points(a, b);
-      int id[S];
-      double Rs[SOLS][9], ts[SOLS][3];
-      geo_sample(a.p.seed, hr >> 4, a.p.w.pair[b].n, S, id);
-      p3p(pts.pix, pts.wld, id, Rs, ts);
-      for (int i = 0; i < 9; ++i) s.x[i] = L.model[i] = Rs[hr & 15][i];
-      for (int i = 0; i < 3; ++i) s.x[9 + i] = L.model[9 + i] = ts[hr & 15][i];
+      double x[SOLS][12];
+      PnpSolver::solve(a.p, b, hr >> 4, x);
+      for (int i = 0; i < 12; ++i) s.x[i] = L.model[i] = x[hr & 15][i];
     }
   }
 
@@ -206,6 +158,5 @@ extern "C" int geo_absolute_pose_lo(const GeoPnpConfig* cfg, const GeoPnpInputs*
   p.kpts0 = in->kpts0; p.points3d1 = in->points3d1; p.matches0 = in->matches0;
   p.K0 = in->K0;
   p.out = out->pnp;
-  return lo_launch<PnpLo>(p, out->num_local_optimizations, out->cost, workspace, pnp_prepare_kernel, lopnp_hyp_kernel,
-                          stream_);
+  return lo_launch<PnpLo>(p, out->num_local_optimizations, out->cost, workspace, pnp_prepare_kernel, stream_);
 }

@@ -1,8 +1,8 @@
 // Batched LO-RANSAC relative pose on the matcher's output: MSAC-scored five-point sampling with Levenberg-Marquardt
 // local optimisation and a final refinement (include/geometry_b200.h, steps L1-L8), on lo_common.cuh's schedule.
-// pose_api.cu's compaction kernel prepares the pair; hyp draws the five-point solutions; a local optimisation starts
-// from P7's pose choice of its E and runs LM on the truncated Sampson cost; the final kernel adds the cheirality test
-// of the chosen (R, t).  Compiled with -fmad=false: oracle/lo_pose_oracle.py takes the same steps.
+// pose_api.cu's compaction kernel prepares the pair; geo_hyp_kernel draws the five-point solutions; a local
+// optimisation starts from P7's pose choice of its E and runs LM on the truncated Sampson cost; the final kernel adds
+// the cheirality test of the chosen (R, t).  Compiled with -fmad=false: oracle/lo_pose_oracle.py takes the same steps.
 #include <stdint.h>
 
 #include "geo_lm.cuh"
@@ -71,25 +71,6 @@ __device__ __forceinline__ void lo_epipolar(const double* E, double x, double y,
   *b1 = (E[1] * u + E[4] * v) + E[7];
 }
 
-__global__ void __launch_bounds__(GEO_CHUNK, 1) lo_hyp_kernel(LoArgs<PoseArgs> a, int c) {
-  const int b = blockIdx.x, t = threadIdx.x;
-  lo_reset(a.l, b, c);
-  const PosePair& P = a.p.w.pair[b];
-  const int h = c * GEO_CHUNK + t;
-  int ns = 0;
-  int id[S];
-  if (P.stop == 0 && h < a.p.max_iters && geo_sample(a.p.seed, h, P.n, S, id) == S) {
-    double sol[SOLS][9];
-    ns = five_point(a.p.w.pts + (long)b * a.p.M, id, sol);
-    float* hm = a.p.w.hyp + ((long)b * GEO_CHUNK + t) * SOLS * 9;
-    for (int r = 0; r < ns; ++r) {
-      for (int i = 0; i < 9; ++i) hm[r * 9 + i] = (float)sol[r][i];
-      a.l.acc[((long)b * GEO_CHUNK + t) * SOLS + r] = 0;
-    }
-  }
-  a.p.w.nsol[(long)b * GEO_CHUNK + t] = ns;
-}
-
 // The chunk's L3 scores of every solution, count << 40 | MSAC score
 struct LoPoseScore {
   using Args = LoArgs<PoseArgs>;
@@ -111,6 +92,7 @@ struct PoseLo {
   static constexpr int DOF = 5, TERMS = 21, GROUP = 21, NP = 12, NF = 9, S = ::S, SOLS = ::SOLS;
   using Base = PoseArgs;
   using Args = LoArgs<PoseArgs>;
+  using Solver = PoseSolver;
   using Score = LoPoseScore;
   struct Scratch {
     double E[9], dE[5][9];   // [t]x R and its derivatives at the pose being summed
@@ -328,6 +310,5 @@ extern "C" int geo_relative_pose_lo(const GeoLoPoseConfig* cfg, const GeoPoseInp
   p.kpts0 = in->kpts0; p.kpts1 = in->kpts1; p.matches0 = in->matches0;
   p.K0 = in->K0; p.K1 = in->K1;
   p.out = out->pose;
-  return lo_launch<PoseLo>(p, out->num_local_optimizations, out->cost, workspace, pose_prepare_kernel, lo_hyp_kernel,
-                           stream_);
+  return lo_launch<PoseLo>(p, out->num_local_optimizations, out->cost, workspace, pose_prepare_kernel, stream_);
 }

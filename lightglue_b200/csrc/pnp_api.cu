@@ -2,45 +2,26 @@
 // inliers (include/geometry_b200.h, steps A1-A8).
 //
 // Launches, all fixed by (B, M, max_iters):
-//   prepare  one 1024-thread CTA per pair: ordered compaction of the valid matches, calibrated coordinates, K check
+//   prepare  pnp_prepare_kernel, one 1024-thread CTA per pair: ordered compaction of the valid matches, calibrated
+//            coordinates, K check
 //   per chunk of GEO_CHUNK samples:
-//     hyp    one CTA per pair: folds the previous chunk's counts into the pair's best (geo_fold), decides the
-//            adaptive stop, then one thread per sample solves it: up to 4 fp32 projections
-//     score  (B, splits) CTAs: each streams a slice of the pair's points through shared memory against every solution
-//            of the chunk, one thread per sample, and adds the inlier counts
-//   refit    one CTA per pair: folds the last chunk, Levenberg-Marquardt from the best solution, recount, R and t
-//   mask     one thread per row of matches0: the final inlier mask
+//     hyp    geo_hyp_kernel, one CTA per pair: folds the previous chunk's counts into the pair's best (geo_fold),
+//            decides the adaptive stop, then one thread per sample solves it: up to 4 fp32 projections
+//     score  geo_score_kernel<PnpScore>, (B, splits) CTAs: each streams a slice of the pair's points through shared
+//            memory against every solution of the chunk, one thread per sample, and adds the inlier counts
+//   final    geo_final_kernel<PnpRansac>, one CTA per pair: folds the last chunk, Levenberg-Marquardt from the best
+//            solution (lo_common.cuh's loop), recount, R and t
+//   mask     pnp_mask_kernel, one thread per row of matches0: the final inlier mask
 // A stopped pair's CTAs return at once.  Compiled with -fmad=false, like geo_api.cu: oracle/pnp_oracle.py takes the same
 // steps in numpy.
 #include <stdint.h>
 
+#include "lo_common.cuh"
 #include "pnp_common.cuh"
 
 namespace {
 
 constexpr int MASK_THREADS = 256;
-
-__global__ void __launch_bounds__(GEO_CHUNK, 1) pnp_hyp_kernel(PnpArgs a, int c) {
-  const int b = blockIdx.x, t = threadIdx.x;
-  if (c > 0) geo_fold<SOLS>(a, S, b, c - 1);
-  const PnpPair& P = a.w.pair[b];
-  const int h = c * GEO_CHUNK + t;
-  int ns = 0;
-  int id[S];
-  if (P.stop == 0 && h < a.max_iters && geo_sample(a.seed, h, P.n, S, id) == S) {
-    double Rs[SOLS][9], ts[SOLS][3];
-    ns = p3p(a.w.pts + (long)b * a.M, a.w.wld + (long)b * a.M, id, Rs, ts);
-    const double* K = a.K0 + (long)b * 9;
-    float* hm = a.w.hyp + ((long)b * GEO_CHUNK + t) * SOLS * 12;
-    for (int r = 0; r < ns; ++r) {
-      double Pm[12];
-      projection(K, Rs[r], ts[r], Pm);
-      for (int i = 0; i < 12; ++i) hm[r * 12 + i] = (float)Pm[i];
-      a.w.count[((long)b * GEO_CHUNK + t) * SOLS + r] = 0;
-    }
-  }
-  a.w.nsol[(long)b * GEO_CHUNK + t] = ns;
-}
 
 // Inlier counts of every projection, on a tile of pixels and world points
 struct PnpScore {
@@ -56,147 +37,77 @@ struct PnpScore {
   __device__ int term(const float* g, const float4* p) const { return reproj_inlier(g, p[0], p[1], thr2); }
 };
 
-constexpr int LM_TERMS = 28;  // J^T J upper triangle (21), J^T r (6), cost
+// The points of the refinement and its fixed inlier set: those of the float projection fm (header step A7)
+struct PnpFixed {
+  const float4* pix;
+  const float4* wld;
+  const float* fm;
+};
 
-// This thread's partial sums of the refit's terms at (R, t) over the inliers k = t, t + RED, ... (header step A7)
-__device__ void lm_partials(const double* K, const double* R, const double* t, const float4* pts, const float4* wld,
-                            const uint8_t* inl, int n, int tid, double* acc) {
-  const double fx = K[0], s = K[1], cx = K[2], fy = K[4], cy = K[5];
-  for (int i = 0; i < LM_TERMS; ++i) acc[i] = 0.0;
-  for (int k = tid; k < n; k += RED) {
-    if (!inl[k]) continue;
-    const float4 p = pts[k], q = wld[k];
-    const double u = p.x, v = p.y, W[3] = {q.x, q.y, q.z};
-    double Xc[3];
-    for (int i = 0; i < 3; ++i) Xc[i] = R[3 * i] * W[0] + R[3 * i + 1] * W[1] + R[3 * i + 2] * W[2] + t[i];
-    const double iz = 1.0 / Xc[2];
-    const double ax = Xc[0] * iz, bx = Xc[1] * iz;
-    const double pu = fx * ax + s * bx;
-    const double ru = pu + cx - u, rv = fy * bx + cy - v;
-    const double gu[3] = {fx * iz, s * iz, -(pu * iz)};
-    const double gv[3] = {0.0, fy * iz, -(fy * bx * iz)};
-    const double ju[6] = {gu[2] * Xc[1] - gu[1] * Xc[2], gu[0] * Xc[2] - gu[2] * Xc[0], gu[1] * Xc[0] - gu[0] * Xc[1],
-                          gu[0], gu[1], gu[2]};
-    const double jv[6] = {gv[2] * Xc[1] - gv[1] * Xc[2], gv[0] * Xc[2] - gv[2] * Xc[0], gv[1] * Xc[0] - gv[0] * Xc[1],
-                          gv[0], gv[1], gv[2]};
-    int e = 0;
+// (R, t) for lo_common.cuh's LM loop on A7's fixed inliers: x = R (0-8, row-major) and t (9-11); the pair's constants
+// are its K0
+struct PnpLm {
+  static constexpr int DOF = 6, TERMS = 28, GROUP = 14, NP = 12, NF = 12;
+  struct Scratch {};
+
+  static __device__ void terms(LoShared<PnpLm>& s, const double* K, const double* x, PnpFixed pts, int n, double thr2,
+                               double* out, int tid) {
+    double acc[TERMS];
 #pragma unroll
-    for (int i = 0; i < 6; ++i)
-#pragma unroll
-      for (int j = i; j < 6; ++j, ++e) acc[e] = acc[e] + (ju[i] * ju[j] + jv[i] * jv[j]);
-#pragma unroll
-    for (int i = 0; i < 6; ++i) acc[21 + i] = acc[21 + i] + (ju[i] * ru + jv[i] * rv);
-    acc[27] = acc[27] + (ru * ru + rv * rv);
+    for (int i = 0; i < TERMS; ++i) acc[i] = 0.0;
+    for (int k = tid; k < n; k += RED) {
+      const float4 p = pts.pix[k], q = pts.wld[k];
+      if (!reproj_inlier(pts.fm, p, q, (float)thr2)) continue;
+      const PnpResidual e = pnp_residual(K, x, x + 9, p, q);
+      pnp_add_normal(K, e, acc);
+      acc[TERMS - 1] = acc[TERMS - 1] + (e.ru * e.ru + e.rv * e.rv);
+    }
+    lo_tree_sums<TERMS, GROUP>(acc, s.red, out, tid);
   }
-}
 
-__global__ void __launch_bounds__(RED, 1) pnp_refit_kernel(PnpArgs a) {
-  const int b = blockIdx.x, t = threadIdx.x;
-  geo_fold<SOLS>(a, S, b, a.chunks - 1);
-  PnpPair& P = a.w.pair[b];
-  const float4* pts = a.w.pts + (long)b * a.M;
-  const float4* wld = a.w.wld + (long)b * a.M;
-  const double* K = a.K0 + (long)b * 9;
-  __shared__ double red[RED];
-  __shared__ double pose[2][12];  // R, t of the best solution and of the refit
-  __shared__ double cand[12];     // the LM step's candidate
-  __shared__ double sums[LM_TERMS], csum[LM_TERMS];
-  __shared__ float fm[2][12];
-  __shared__ int count[2];
-  __shared__ int step_ok;
-  const unsigned long long key = P.best;
-  if (!P.ok || key == 0) {
+  static __device__ void update(LoShared<PnpLm>&, const double* x, const double* d, double* out) {
+    lm_update(x, x + 9, d, out, out + 9);
+  }
+};
+
+// The absolute pose for geo_final_kernel: GEO_PNP_LM_STEPS Levenberg-Marquardt steps on the best solution's inliers
+// (header step A7)
+struct PnpRansac : PnpSolver {
+  using Base = PnpArgs;
+  using Score = PnpScore;
+  using Scratch = LoShared<PnpLm>;
+
+  static __device__ bool inlier(const PnpArgs& a, int b, const float* g, int k) {
+    const long i = (long)b * a.M + k;
+    return reproj_inlier(g, a.w.pts[i], a.w.wld[i], a.w.pair[b].thr2);
+  }
+  static __device__ void clear(const PnpArgs&, int, int) {}  // pnp_mask_kernel writes every row
+  static __device__ void fail(const PnpArgs& a, int b, int t) {
     if (t < 9) a.out.R[(long)b * 9 + t] = 0.0;
     if (t < 3) a.out.t[(long)b * 3 + t] = 0.0;
-    if (t == 0) {
-      a.out.num_inliers[b] = 0;
-      a.out.success[b] = 0;
-      a.out.best_hypothesis[b] = a.out.best_solution[b] = -1;
-      a.out.num_hypotheses[b] = P.drawn;
-    }
-    return;
   }
-  const unsigned hr = ~(unsigned)(key & 0xffffffffu);
-  const int hcount = (int)(key >> 32) - 1;
-  const float thr2 = P.thr2;
-  if (t == 0) {
-    int id[S];
-    double Rs[SOLS][9], ts[SOLS][3], Pm[12];
-    geo_sample(a.seed, hr >> 4, P.n, S, id);
-    p3p(pts, wld, id, Rs, ts);
-    for (int i = 0; i < 9; ++i) pose[0][i] = pose[1][i] = Rs[hr & 15][i];
-    for (int i = 0; i < 3; ++i) pose[0][9 + i] = pose[1][9 + i] = ts[hr & 15][i];
-    projection(K, pose[0], pose[0] + 9, Pm);
-    for (int i = 0; i < 12; ++i) fm[0][i] = (float)Pm[i];
-    count[0] = hcount;
-    count[1] = -1;
-  }
-  __syncthreads();
-  if (hcount >= GEO_PNP_REFIT_MIN) {
-    uint8_t* inl = a.w.inl + (long)b * a.M;
-    for (int k = t; k < P.n; k += RED) inl[k] = reproj_inlier(fm[0], pts[k], wld[k], thr2);
+  static __device__ bool refits(const PnpArgs&, int hcount) { return hcount >= GEO_PNP_REFIT_MIN; }
+
+  static __device__ void refit(GeoFinal<PnpRansac>& s, const PnpArgs& a, int b, int t) {
+    if (t == 0)
+      for (int i = 0; i < 12; ++i) s.m.x[i] = s.x[0][i];
     __syncthreads();
-    double acc[LM_TERMS];
-    lm_partials(K, pose[1], pose[1] + 9, pts, wld, inl, P.n, t, acc);
-    for (int i = 0; i < LM_TERMS; ++i) {
-      const double s = tree_sum(acc[i], red, t);
-      if (t == 0) sums[i] = s;
-    }
-    double lam = GEO_PNP_LM_LAMBDA0;  // every thread keeps the same schedule
-    for (int it = 0; it < GEO_PNP_LM_STEPS; ++it) {
-      if (t == 0) {
-        double d[6];
-        step_ok = lm_solve<6>(sums, sums + 21, lam, d);
-        if (step_ok) lm_update(pose[1], pose[1] + 9, d, cand, cand + 9);
-      }
-      __syncthreads();
-      if (!step_ok) {
-        lam = lam * 10.0;
-        __syncthreads();
-        continue;
-      }
-      lm_partials(K, cand, cand + 9, pts, wld, inl, P.n, t, acc);
-      for (int i = 0; i < LM_TERMS; ++i) {
-        const double s = tree_sum(acc[i], red, t);
-        if (t == 0) csum[i] = s;
-      }
-      __syncthreads();
-      const bool better = csum[27] < sums[27];
-      __syncthreads();
-      if (better) {
-        if (t < 12) pose[1][t] = cand[t];
-        if (t < LM_TERMS) sums[t] = csum[t];
-        lam = lam / 10.0;
-      } else {
-        lam = lam * 10.0;
-      }
-      __syncthreads();
-    }
-    if (t == 0) {
-      double Pm[12];
-      projection(K, pose[1], pose[1] + 9, Pm);
-      for (int i = 0; i < 12; ++i) fm[1][i] = (float)Pm[i];
-      count[1] = 0;
-    }
-    __syncthreads();
-    int k1 = 0;
-    for (int k = t; k < P.n; k += RED) k1 += reproj_inlier(fm[1], pts[k], wld[k], thr2);
-    if (k1) atomicAdd(&count[1], k1);
-    __syncthreads();
+    const PnpFixed pts{a.w.pts + (long)b * a.M, a.w.wld + (long)b * a.M, s.fm[0]};
+    const float thr2 = a.w.pair[b].thr2;
+    lo_refine(s.m, a.K0 + (long)b * 9, pts, a.w.pair[b].n, (double)thr2, GEO_PNP_LM_STEPS, GEO_PNP_LM_LAMBDA0, t);
+    if (t == 0)
+      for (int i = 0; i < 12; ++i) s.x[1][i] = s.m.x[i];
   }
-  const int u = count[1] >= count[0] ? 1 : 0;
-  if (t < 12) P.P[t] = fm[u][t];
-  if (t < 9) a.out.R[(long)b * 9 + t] = pose[u][t];
-  if (t < 3) a.out.t[(long)b * 3 + t] = pose[u][9 + t];
-  if (t == 0) {
-    a.out.num_inliers[b] = count[u];
-    a.out.success[b] = 1;
-    a.out.best_hypothesis[b] = (int)(hr >> 4);
-    a.out.best_solution[b] = (int)(hr & 15);
-    a.out.num_hypotheses[b] = P.drawn;
-    P.success = 1;
+
+  // R, t, and the projection for pnp_mask_kernel
+  static __device__ void write(GeoFinal<PnpRansac>& s, const PnpArgs& a, int b, int u, int t) {
+    PnpPair& P = a.w.pair[b];
+    if (t < 12) P.P[t] = s.fm[u][t];
+    if (t < 9) a.out.R[(long)b * 9 + t] = s.x[u][t];
+    if (t < 3) a.out.t[(long)b * 3 + t] = s.x[u][9 + t];
+    if (t == 0) P.success = 1;
   }
-}
+};
 
 __global__ void __launch_bounds__(MASK_THREADS) pnp_mask_kernel(PnpArgs a) {
   const int b = blockIdx.x, i = blockIdx.y * MASK_THREADS + threadIdx.x;
@@ -237,18 +148,8 @@ extern "C" int geo_absolute_pose(const GeoPnpConfig* cfg, const GeoPnpInputs* in
   a.kpts0 = in->kpts0; a.points3d1 = in->points3d1; a.matches0 = in->matches0;
   a.K0 = in->K0;
   a.out = *out;
-  const int splits = geo_score_splits(a.B, a.M);
   const cudaStream_t stream = (cudaStream_t)stream_;
-  pnp_prepare_kernel<<<a.B, 1024, 0, stream>>>(a);
-  LG_CHECK_LAUNCH();
-  for (int c = 0; c < a.chunks; ++c) {
-    pnp_hyp_kernel<<<a.B, GEO_CHUNK, 0, stream>>>(a, c);
-    LG_CHECK_LAUNCH();
-    geo_score_kernel<PnpScore><<<dim3(a.B, splits), GEO_CHUNK, 0, stream>>>(a);
-    LG_CHECK_LAUNCH();
-  }
-  pnp_refit_kernel<<<a.B, RED, 0, stream>>>(a);
-  LG_CHECK_LAUNCH();
+  if (int rc = geo_launch<PnpRansac>(a, pnp_prepare_kernel, stream)) return rc;
   if (a.M > 0) {
     pnp_mask_kernel<<<dim3(a.B, (a.M + MASK_THREADS - 1) / MASK_THREADS), MASK_THREADS, 0, stream>>>(a);
     LG_CHECK_LAUNCH();

@@ -17,14 +17,14 @@ constexpr int SOLS = GEO_PNP_MAX_SOLUTIONS;
 constexpr int TILE = 512;              // points per shared-memory tile of the score kernel
 
 struct PnpPair {
-  float P[12];               // the final K0 [R | t], fp32 (refit -> mask)
+  float P[12];               // the final K0 [R | t], fp32 (final -> mask)
   unsigned long long best;   // (count + 1) << 32 | ~(h * 16 + r) of the best solution so far; 0: none
   float thr2;                // threshold^2
   int n;                     // valid matches
   int ok;                    // n >= 3 and K0 valid
   int stop;                  // no further samples are drawn
   int drawn;                 // samples drawn so far
-  int success;               // set by the refit kernel
+  int success;               // set by the final kernel
 };
 
 struct PnpWs {
@@ -35,7 +35,6 @@ struct PnpWs {
   float* hyp;      // [B, GEO_CHUNK, SOLS, 12] the current chunk's projections, fp32
   int* nsol;       // [B, GEO_CHUNK] their number; 0: degenerate or not drawn
   int* count;      // [B, GEO_CHUNK, SOLS] their inlier counts
-  uint8_t* inl;    // [B, M] the best solution's inliers, per compacted point (refit)
 };
 
 size_t carve(char* base, int B, int M, PnpWs* w) {
@@ -47,7 +46,6 @@ size_t carve(char* base, int B, int M, PnpWs* w) {
   w->hyp = b.take<float>((size_t)B * GEO_CHUNK * SOLS * 12);
   w->nsol = b.take<int>((size_t)B * GEO_CHUNK);
   w->count = b.take<int>((size_t)B * GEO_CHUNK * SOLS);
-  w->inl = b.take<uint8_t>((size_t)B * M);
   return b.bytes();
 }
 
@@ -82,8 +80,8 @@ __device__ __forceinline__ void root2(double b, double c, double* r1, double* r2
 __device__ __forceinline__ double cubic(double g, double cb, double cc, double cd) { return ((g + cb) * g + cc) * g + cd; }
 
 // Lambda Twist P3P on the calibrated (x, y) in pts[id[k]].z/w and the world points wlds[id[k]] (header step A4).
-// Writes the kept solutions' R (row-major) and t in the solver's order; returns their number.
-__device__ __noinline__ int p3p(const float4* pts, const float4* wlds, const int* id, double (*Rs)[9], double (*ts)[3]) {
+// Writes the kept solutions' R (row-major, 0-8) and t (9-11) in the solver's order; returns their number.
+__device__ __noinline__ int p3p(const float4* pts, const float4* wlds, const int* id, double (*sol)[12]) {
   double y[3][3], X[3][3];
   for (int k = 0; k < 3; ++k) {
     const float4 p = pts[id[k]], q = wlds[id[k]];
@@ -213,8 +211,8 @@ __device__ __noinline__ int p3p(const float4* pts, const float4* wlds, const int
         yd2[i] = ry[0][i] - ry[2][i];
       }
       cross3(yd1, yd2, yc);
-      double* R = Rs[ns];
-      double* t = ts[ns];
+      double* R = sol[ns];
+      double* t = sol[ns] + 9;
       bool fin = true;
       for (int i = 0; i < 3; ++i)
         for (int j = 0; j < 3; ++j) {
@@ -257,6 +255,60 @@ __device__ __forceinline__ float reproj_err(const float* g, float4 p, float4 q) 
   const float du = p.x - (g[0] * q.x + g[1] * q.y + g[2] * q.z + g[3]) * iw;
   const float dv = p.y - (g[4] * q.x + g[5] * q.y + g[6] * q.z + g[7]) * iw;
   return w > 0.f ? du * du + dv * dv : INFINITY;
+}
+
+// geo_hyp_kernel's solver of the absolute pose: sample h's P3P solutions (R, t), scored as K0 [R | t]
+struct PnpSolver {
+  static constexpr int SOLS = ::SOLS, NX = 12, NF = 12;
+  static __device__ int s(const PnpArgs&) { return S; }
+  static __device__ int solve(const PnpArgs& a, int b, unsigned h, double (*x)[NX]) {
+    int id[S];
+    if (geo_sample(a.seed, h, a.w.pair[b].n, S, id) < S) return 0;
+    return p3p(a.w.pts + (long)b * a.M, a.w.wld + (long)b * a.M, id, x);
+  }
+  static __device__ void pixels(const PnpArgs& a, int b, const double* x, double* px) {
+    projection(a.K0 + (long)b * 9, x, x + 9, px);
+  }
+};
+
+// The reprojection residual (ru, rv) of world point q at pixel p (u, v) under K [R | t], and what its Jacobian needs
+struct PnpResidual {
+  double Xc[3];  // the camera-frame point; Xc[2] is its depth
+  double iz, pu, bx, ru, rv;
+};
+
+__device__ __forceinline__ PnpResidual pnp_residual(const double* K, const double* R, const double* t, float4 p,
+                                                    float4 q) {
+  const double fx = K[0], sk = K[1], cx = K[2], fy = K[4], cy = K[5];
+  const double u = p.x, v = p.y, W[3] = {q.x, q.y, q.z};
+  PnpResidual e;
+  for (int i = 0; i < 3; ++i) e.Xc[i] = R[3 * i] * W[0] + R[3 * i + 1] * W[1] + R[3 * i + 2] * W[2] + t[i];
+  e.iz = 1.0 / e.Xc[2];
+  const double ax = e.Xc[0] * e.iz;
+  e.bx = e.Xc[1] * e.iz;
+  e.pu = fx * ax + sk * e.bx;
+  e.ru = e.pu + cx - u;
+  e.rv = fy * e.bx + cy - v;
+  return e;
+}
+
+// Adds the point's J^T J upper triangle (acc[0..20]) and J^T r (acc[21..26]) in A7's parameters (header step A7)
+__device__ __forceinline__ void pnp_add_normal(const double* K, const PnpResidual& e, double* acc) {
+  const double fx = K[0], sk = K[1], fy = K[4];
+  const double* Xc = e.Xc;
+  const double gu[3] = {fx * e.iz, sk * e.iz, -(e.pu * e.iz)};
+  const double gv[3] = {0.0, fy * e.iz, -(fy * e.bx * e.iz)};
+  const double ju[6] = {gu[2] * Xc[1] - gu[1] * Xc[2], gu[0] * Xc[2] - gu[2] * Xc[0], gu[1] * Xc[0] - gu[0] * Xc[1],
+                        gu[0], gu[1], gu[2]};
+  const double jv[6] = {gv[2] * Xc[1] - gv[1] * Xc[2], gv[0] * Xc[2] - gv[2] * Xc[0], gv[1] * Xc[0] - gv[0] * Xc[1],
+                        gv[0], gv[1], gv[2]};
+  int k = 0;
+#pragma unroll
+  for (int i = 0; i < 6; ++i)
+#pragma unroll
+    for (int j = i; j < 6; ++j, ++k) acc[k] = acc[k] + (ju[i] * ju[j] + jv[i] * jv[j]);
+#pragma unroll
+  for (int i = 0; i < 6; ++i) acc[21 + i] = acc[21 + i] + (ju[i] * e.ru + jv[i] * e.rv);
 }
 
 __device__ bool k_valid(const double* K) {

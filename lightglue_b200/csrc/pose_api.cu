@@ -2,15 +2,17 @@
 // (include/geometry_b200.h, steps P1-P8).
 //
 // Launches, all fixed by (B, M, max_iters):
-//   prepare  one 1024-thread CTA per pair: ordered compaction of the valid matches, calibrated coordinates, K checks
+//   prepare  pose_prepare_kernel, one 1024-thread CTA per pair: ordered compaction of the valid matches, calibrated
+//            coordinates, K checks
 //   per chunk of GEO_CHUNK samples:
-//     hyp    one CTA per pair: folds the previous chunk's counts into the pair's best (geo_fold), decides the
-//            adaptive stop, then one thread per sample solves it: up to 10 fp32 models
-//     score  (B, splits) CTAs: each streams a slice of the pair's points through shared memory against every solution
-//            of the chunk, one thread per sample, and adds the inlier counts
-//   refit    one CTA per pair: folds the last chunk, least-squares refit projected on the essential manifold, recount,
-//            E and the inliers
-//   pose     one CTA per pair: the four (R, t) of E, linear triangulation of every inlier, the cheirality test
+//     hyp    geo_hyp_kernel, one CTA per pair: folds the previous chunk's counts into the pair's best (geo_fold),
+//            decides the adaptive stop, then one thread per sample solves it: up to 10 fp32 models
+//     score  geo_score_kernel<PoseScore>, (B, splits) CTAs: each streams a slice of the pair's points through shared
+//            memory against every solution of the chunk, one thread per sample, and adds the inlier counts
+//   final    geo_final_kernel<PoseRansac>, one CTA per pair: folds the last chunk, least-squares refit projected on the
+//            essential manifold, recount, E and the inliers
+//   pose     pose_kernel, one CTA per pair: the four (R, t) of E, linear triangulation of every inlier, the cheirality
+//            test
 // A stopped pair's CTAs return at once.  Compiled with -fmad=false, like geo_api.cu: oracle/pose_oracle.py takes the same
 // steps in numpy.
 #include <stdint.h>
@@ -19,25 +21,6 @@
 #include "pose_common.cuh"
 
 namespace {
-
-__global__ void __launch_bounds__(GEO_CHUNK, 1) pose_hyp_kernel(PoseArgs a, int c) {
-  const int b = blockIdx.x, t = threadIdx.x;
-  if (c > 0) geo_fold<SOLS>(a, S, b, c - 1);
-  const PosePair& P = a.w.pair[b];
-  const int h = c * GEO_CHUNK + t;
-  int ns = 0;
-  int id[S];
-  if (P.stop == 0 && h < a.max_iters && geo_sample(a.seed, h, P.n, S, id) == S) {
-    double sol[SOLS][9];
-    ns = five_point(a.w.pts + (long)b * a.M, id, sol);
-    float* hm = a.w.hyp + ((long)b * GEO_CHUNK + t) * SOLS * 9;
-    for (int r = 0; r < ns; ++r) {
-      for (int i = 0; i < 9; ++i) hm[r * 9 + i] = (float)sol[r][i];
-      a.w.count[((long)b * GEO_CHUNK + t) * SOLS + r] = 0;
-    }
-  }
-  a.w.nsol[(long)b * GEO_CHUNK + t] = ns;
-}
 
 // Inlier counts of every solution
 struct PoseScore {
@@ -53,100 +36,56 @@ struct PoseScore {
   __device__ int term(const float* g, const float4* p) const { return sampson(g, p[0]) < thr2; }
 };
 
-__global__ void __launch_bounds__(RED, 1) pose_refit_kernel(PoseArgs a) {
-  const int b = blockIdx.x, t = threadIdx.x;
-  geo_fold<SOLS>(a, S, b, a.chunks - 1);
-  PosePair& P = a.w.pair[b];
-  const float4* pts = a.w.pts + (long)b * a.M;
-  const int* idx = a.w.idx + (long)b * a.M;
-  uint8_t* inl = a.out.inliers + (long)b * a.M;
-  uint8_t* pinl = a.out.pose_inliers + (long)b * a.M;
-  __shared__ double red[RED];
-  __shared__ double ata[45];
-  __shared__ double model[2][9];
-  __shared__ float fm[2][9];
-  __shared__ int count[2];
-  for (int i = t; i < a.M; i += RED) inl[i] = pinl[i] = 0;
-  const unsigned long long key = P.best;
-  if (!P.ok || key == 0) {
+// The relative pose for geo_final_kernel: least-squares refit projected on the essential manifold (header step P5)
+struct PoseRansac : PoseSolver {
+  using Base = PoseArgs;
+  using Score = PoseScore;
+  struct Scratch {
+    double red[RED];
+    double ata[45];
+  };
+
+  static __device__ bool inlier(const PoseArgs& a, int b, const float* g, int k) {
+    return sampson(g, a.w.pts[(long)b * a.M + k]) < a.w.pair[b].thr2;
+  }
+  static __device__ void clear(const PoseArgs& a, int b, int t) {
+    for (int i = t; i < a.M; i += RED) a.out.inliers[(long)b * a.M + i] = a.out.pose_inliers[(long)b * a.M + i] = 0;
+  }
+  static __device__ void fail(const PoseArgs& a, int b, int t) {
     if (t < 9) a.out.E[(long)b * 9 + t] = a.out.R[(long)b * 9 + t] = 0.0;
     if (t < 3) a.out.t[(long)b * 3 + t] = 0.0;
-    if (t == 0) {
-      a.out.num_inliers[b] = a.out.num_pose_inliers[b] = 0;
-      a.out.success[b] = 0;
-      a.out.best_hypothesis[b] = a.out.best_solution[b] = -1;
-      a.out.num_hypotheses[b] = P.drawn;
-    }
-    return;
+    if (t == 0) a.out.num_pose_inliers[b] = 0;
   }
-  const unsigned hr = ~(unsigned)(key & 0xffffffffu);
-  const int hcount = (int)(key >> 32) - 1;
-  const float thr2 = P.thr2;
-  if (t == 0) {
-    int id[S];
-    double sol[SOLS][9];
-    geo_sample(a.seed, hr >> 4, P.n, S, id);
-    five_point(pts, id, sol);
-    for (int i = 0; i < 9; ++i) {
-      model[0][i] = sol[hr & 15][i];
-      fm[0][i] = (float)model[0][i];
-    }
-    count[0] = hcount;
-    count[1] = -1;
-  }
-  __syncthreads();
-  if (hcount >= GEO_REFIT_MIN) {
-    for (int i = 0, e0 = 0; i < 9; e0 += 9 - i, ++i) {
-      double acc[9];
-#pragma unroll
-      for (int j = 0; j < 9; ++j) acc[j] = 0.0;
-      for (int k = t; k < P.n; k += RED) {
-        const float4 p = pts[k];
-        if (!(sampson(fm[0], p) < thr2)) continue;
-        const double x = p.x, y = p.y, u = p.z, v = p.w;
-        const double ra[9] = {u * x, u * y, u, v * x, v * y, v, x, y, 1.0};
-#pragma unroll
-        for (int j = 0; j < 9; ++j)
-          if (j >= i) acc[j] = acc[j] + ra[i] * ra[j];
-      }
-#pragma unroll
-      for (int j = 0; j < 9; ++j)
-        if (j >= i) {
-          const double s = tree_sum(acc[j], red, t);
-          if (t == 0) ata[e0 + j - i] = s;
-        }
-    }
+  static __device__ bool refits(const PoseArgs&, int hcount) { return hcount >= GEO_REFIT_MIN; }
+
+  static __device__ void refit(GeoFinal<PoseRansac>& s, const PoseArgs& a, int b, int t) {
+    const float4* pts = a.w.pts + (long)b * a.M;
+    geo_ata(a.w.pair[b].n, [&](int k) { return inlier(a, b, s.fm[0], k); },
+            [&](int k, double* ra, double*) {
+              const float4 p = pts[k];
+              const double x = p.x, y = p.y, u = p.z, v = p.w;
+              const double r[9] = {u * x, u * y, u, v * x, v * y, v, x, y, 1.0};
+              for (int i = 0; i < 9; ++i) ra[i] = r[i];
+              return 1;
+            }, s.m.red, s.m.ata, t);
     if (t == 0) {
-      double A[9][9], v[9], u1[3], u2[3], v1[3], v2[3];
-      for (int i = 0, e = 0; i < 9; ++i)
-        for (int j = i; j < 9; ++j, ++e) A[i][j] = A[j][i] = ata[e];
-      smallest_eigvec<9>(A, v);
+      double v[9], u1[3], u2[3], v1[3], v2[3];
+      ata_null_vector(s.m.ata, v);
       svd2(v, u1, u2, v1, v2);
       for (int r = 0; r < 3; ++r)
-        for (int c = 0; c < 3; ++c) model[1][r * 3 + c] = u1[r] * v1[c] + u2[r] * v2[c];
-      unit_scale(model[1]);
-      for (int i = 0; i < 9; ++i) fm[1][i] = (float)model[1][i];
-      count[1] = 0;
+        for (int c = 0; c < 3; ++c) s.x[1][r * 3 + c] = u1[r] * v1[c] + u2[r] * v2[c];
+      unit_scale(s.x[1]);
     }
-    __syncthreads();
-    int k1 = 0;
-    for (int k = t; k < P.n; k += RED) k1 += sampson(fm[1], pts[k]) < thr2;
-    if (k1) atomicAdd(&count[1], k1);
-    __syncthreads();
   }
-  const int u = count[1] >= count[0] ? 1 : 0;
-  for (int k = t; k < P.n; k += RED)
-    if (sampson(fm[u], pts[k]) < thr2) inl[idx[k]] = 1;
-  if (t < 9) a.out.E[(long)b * 9 + t] = P.E[t] = model[u][t];
-  if (t == 0) {
-    a.out.num_inliers[b] = count[u];
-    a.out.success[b] = 1;
-    a.out.best_hypothesis[b] = (int)(hr >> 4);
-    a.out.best_solution[b] = (int)(hr & 15);
-    a.out.num_hypotheses[b] = P.drawn;
-    P.success = 1;
+
+  // E and its inliers, and E for pose_kernel
+  static __device__ void write(GeoFinal<PoseRansac>& s, const PoseArgs& a, int b, int u, int t) {
+    PosePair& P = a.w.pair[b];
+    geo_write_mask<PoseRansac>(a, b, s.fm[u], t);
+    if (t < 9) a.out.E[(long)b * 9 + t] = P.E[t] = s.px[u][t];
+    if (t == 0) P.success = 1;
   }
-}
+};
 
 __global__ void __launch_bounds__(POSE_THREADS, 1) pose_kernel(PoseArgs a) {
   const int b = blockIdx.x, t = threadIdx.x;
@@ -239,18 +178,8 @@ extern "C" int geo_relative_pose(const GeoPoseConfig* cfg, const GeoPoseInputs* 
   a.kpts0 = in->kpts0; a.kpts1 = in->kpts1; a.matches0 = in->matches0;
   a.K0 = in->K0; a.K1 = in->K1;
   a.out = *out;
-  const int splits = geo_score_splits(a.B, a.M);
   const cudaStream_t stream = (cudaStream_t)stream_;
-  pose_prepare_kernel<<<a.B, 1024, 0, stream>>>(a);
-  LG_CHECK_LAUNCH();
-  for (int c = 0; c < a.chunks; ++c) {
-    pose_hyp_kernel<<<a.B, GEO_CHUNK, 0, stream>>>(a, c);
-    LG_CHECK_LAUNCH();
-    geo_score_kernel<PoseScore><<<dim3(a.B, splits), GEO_CHUNK, 0, stream>>>(a);
-    LG_CHECK_LAUNCH();
-  }
-  pose_refit_kernel<<<a.B, RED, 0, stream>>>(a);
-  LG_CHECK_LAUNCH();
+  if (int rc = geo_launch<PoseRansac>(a, pose_prepare_kernel, stream)) return rc;
   pose_kernel<<<a.B, POSE_THREADS, 0, stream>>>(a);
   LG_CHECK_LAUNCH();
   return 0;

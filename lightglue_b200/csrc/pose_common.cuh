@@ -365,6 +365,20 @@ __device__ __noinline__ int five_point(const float4* pts, const int* id, double 
   return ns;
 }
 
+// geo_hyp_kernel's solver of the relative pose: sample h's five-point solutions E
+struct PoseSolver {
+  static constexpr int SOLS = ::SOLS, NX = 9, NF = 9;
+  static __device__ int s(const PoseArgs&) { return S; }
+  static __device__ int solve(const PoseArgs& a, int b, unsigned h, double (*x)[NX]) {
+    int id[S];
+    if (geo_sample(a.seed, h, a.w.pair[b].n, S, id) < S) return 0;
+    return five_point(a.w.pts + (long)b * a.M, id, x);
+  }
+  static __device__ void pixels(const PoseArgs&, int, const double* x, double* px) {
+    for (int i = 0; i < NF; ++i) px[i] = x[i];
+  }
+};
+
 // fp32 squared Sampson error of one correspondence (header step P4)
 __device__ __forceinline__ float sampson(const float* g, float4 p) {
   const float a0 = (g[0] * p.x + g[1] * p.y) + g[2], a1 = (g[3] * p.x + g[4] * p.y) + g[5];

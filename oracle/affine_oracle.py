@@ -12,6 +12,7 @@ import numpy as np
 
 from oracle import geometry_oracle as go
 from oracle import lo_common as lc
+from oracle import lo_pose_oracle as lpo
 
 AFFINE, PARTIAL = 3, 4
 MAX_REFINE = 100
@@ -121,7 +122,8 @@ def refine(kind: int, norm, pts: np.ndarray, inl: np.ndarray, X, steps: int) -> 
     """AF6: steps Levenberg-Marquardt steps from the normalised parameters X on the fixed inlier set inl."""
     def update(p, d):
         return [p[i] + d[i] for i in range(len(p))]
-    return np.array(lc.refine(lambda p: terms(kind, norm, pts, inl, p), update, [float(c) for c in X], dof(kind), steps))
+    return np.array(lc.refine(lambda p: terms(kind, norm, pts, inl, p), update, [float(c) for c in X], dof(kind), steps,
+                             lpo.LAMBDA0))
 
 
 def _fail(M: int, drawn: int) -> dict:
@@ -145,19 +147,14 @@ def estimate_pair(kind, kpts0, kpts1, m0, threshold=3.0, max_iters=2000, confide
     norm = go.normalisation(pts)
     if norm is None:
         return _fail(M, 0)
-    best_cnt, best_h, drawn = -1, -1, 0
-    for c in range(-(-max_iters // go.CHUNK)):
-        h = np.arange(c * go.CHUNK, min((c + 1) * go.CHUNK, max_iters), dtype=np.int64)
+
+    def candidates(h):
         _, A, ok = hypotheses(kind, seed, h, pts, norm)
-        if ok.any():
-            cnt = (errors(A[ok], pts) < thr2).sum(1)
-            i = int(np.argmax(cnt))  # first maximum: the lowest hypothesis index
-            if cnt[i] > best_cnt:
-                best_cnt, best_h = int(cnt[i]), int(h[ok][i])
-        drawn = min((c + 1) * go.CHUNK, max_iters)
-        ep = 1.0 - max(best_cnt, 0) / n
-        if drawn >= max_iters or drawn >= go.update_num_iters(confidence, ep, s, max_iters):
-            break
+        if not ok.any():
+            return None
+        return (errors(A[ok], pts) < thr2).sum(1), h[ok], np.zeros(int(ok.sum()), dtype=np.int64)
+
+    best_cnt, best_h, _, drawn = go.ransac_pair(n, s, max_iters, confidence, candidates)
     if best_h < 0:
         return _fail(M, drawn)
     X, A, _ = hypotheses(kind, seed, np.array([best_h]), pts, norm)

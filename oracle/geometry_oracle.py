@@ -278,8 +278,46 @@ def update_num_iters(p: float, ep: float, s: int, max_iters: int) -> int:
     return max_iters if (denom >= 0.0 or -num >= max_iters * (-denom)) else int(round(num / denom))
 
 
+def ransac_pair(n: int, s: int, max_iters: int, confidence: float, candidates):
+    """The chunk loop of one pair of n points and s points per sample (header steps 3 and 6).  candidates(h) gives the
+    valid solutions of the samples h in (sample, solution) order as (inlier counts, samples, solution indices), or None
+    without one.  The best is the first maximum count: ties go to the lowest (sample, solution).  Returns (best count,
+    h, r, samples drawn), with h = r = -1 and count -1 when no sample had a valid solution."""
+    best_cnt, best_h, best_r, drawn = -1, -1, -1, 0
+    for c in range(-(-max_iters // CHUNK)):
+        h = np.arange(c * CHUNK, min((c + 1) * CHUNK, max_iters), dtype=np.int64)
+        cands = candidates(h)
+        if cands is not None:
+            cnt, hs, rs = cands
+            i = int(np.argmax(cnt))
+            if cnt[i] > best_cnt:
+                best_cnt, best_h, best_r = int(cnt[i]), int(hs[i]), int(rs[i])
+        drawn = min((c + 1) * CHUNK, max_iters)
+        ep = 1.0 - max(best_cnt, 0) / n
+        if drawn >= max_iters or drawn >= update_num_iters(confidence, ep, s, max_iters):
+            break
+    return best_cnt, best_h, best_r, drawn
+
+
+def ata(ra: np.ndarray, rb, inl: np.ndarray) -> np.ndarray:
+    """The symmetric 9x9 A^T A of the refit (header step 7): over the points with inl, each point's row ra [n, 9] and,
+    when rb is not None, its second row rb, every upper-triangle entry summed in the fixed order."""
+    terms = []
+    for i in range(9):
+        for j in range(i, 9):
+            e = ra[:, i] * ra[:, j] + rb[:, i] * rb[:, j] if rb is not None else ra[:, i] * ra[:, j]
+            terms.append(np.where(inl, e, 0.0))
+    sums = fixed_sum(np.stack(terms))
+    A, e = np.zeros((9, 9)), 0
+    for i in range(9):
+        for j in range(i, 9):
+            A[i, j] = A[j, i] = sums[e]
+            e += 1
+    return A
+
+
 def _eigvec_smallest(A):
-    A = [list(r) for r in A]
+    A = [[float(x) for x in r] for r in A]
     V = [[1.0 if i == j else 0.0 for j in range(9)] for i in range(9)]
     for _ in range(EIG_SWEEPS):
         for p in range(8):
@@ -326,38 +364,21 @@ def estimate_pair(kind, kpts0, kpts1, m0, threshold, max_iters, confidence, seed
     norm = normalisation(pts)
     if norm is None:
         return _fail(M, 0)
-    best_cnt, best_h, drawn = -1, -1, 0
-    for c in range(-(-max_iters // CHUNK)):
-        h = np.arange(c * CHUNK, min((c + 1) * CHUNK, max_iters), dtype=np.int64)
+
+    def candidates(h):
         models, ok = hypotheses(kind, seed, h, pts, norm)
-        if ok.any():
-            cnt = (errors(kind, models[ok], pts) < thr2).sum(1)
-            i = int(np.argmax(cnt))  # first maximum: the lowest hypothesis index
-            if cnt[i] > best_cnt:
-                best_cnt, best_h = int(cnt[i]), int(h[ok][i])
-        drawn = min((c + 1) * CHUNK, max_iters)
-        ep = 1.0 - max(best_cnt, 0) / n
-        if drawn >= max_iters or drawn >= update_num_iters(confidence, ep, s, max_iters):
-            break
+        if not ok.any():
+            return None
+        return (errors(kind, models[ok], pts) < thr2).sum(1), h[ok], np.zeros(int(ok.sum()), dtype=np.int64)
+
+    best_cnt, best_h, _, drawn = ransac_pair(n, s, max_iters, confidence, candidates)
     if best_h < 0:
         return _fail(M, drawn)
     hyp, _ = hypotheses(kind, seed, np.array([best_h]), pts, norm)
     cands = [(hyp[0], best_cnt)]
     if best_cnt >= s:
         inl = errors(kind, hyp, pts)[0] < thr2
-        ra, rb = rows(kind, norm, pts)
-        ata = []
-        for i in range(9):
-            for j in range(i, 9):
-                e = ra[:, i] * ra[:, j] + rb[:, i] * rb[:, j] if rb is not None else ra[:, i] * ra[:, j]
-                ata.append(np.where(inl, e, 0.0))
-        ata = fixed_sum(np.stack(ata))
-        A, e = [[0.0] * 9 for _ in range(9)], 0
-        for i in range(9):
-            for j in range(i, 9):
-                A[i][j] = A[j][i] = float(ata[e])
-                e += 1
-        v = _eigvec_smallest(A)[None]
+        v = _eigvec_smallest(ata(*rows(kind, norm, pts), inl))[None]
         with np.errstate(all="ignore"):
             if kind == FUNDAMENTAL:
                 v = rank2(v)

@@ -64,13 +64,13 @@ def quat_rotation(d):
             2.0 * (qx * qz - qw * qy), 2.0 * (qy * qz + qw * qx), 1.0 - 2.0 * (qx * qx + qy * qy)]
 
 
-def refine(terms, update, x, dof, steps: int):
-    """steps Levenberg-Marquardt steps on a truncated cost from the model x.  terms(x) gives its fixed-order sums: the
-    J^T J upper triangle, J^T r (dof each) and the cost last; update(x, d) the candidate of the step d.  A candidate is
-    taken when its cost is lower; the damping starts at LAMBDA0 and falls or rises tenfold."""
+def refine(terms, update, x, dof, steps: int, lam0: float):
+    """steps Levenberg-Marquardt steps on a cost from the model x.  terms(x) gives its fixed-order sums: the J^T J upper
+    triangle, J^T r (dof each) and the cost last; update(x, d) the candidate of the step d.  A candidate is taken when
+    its cost is lower; the damping starts at lam0 and falls or rises tenfold."""
     nh = dof * (dof + 1) // 2
     sums = terms(x)
-    lam = lpo.LAMBDA0
+    lam = lam0
     for _ in range(steps):
         d = lm_solve(sums[:nh], sums[nh:nh + dof], lam, dof)
         if d is None:

@@ -155,7 +155,7 @@ def refine(norm, model, pts: np.ndarray, thr2: float, steps: int):
     """steps Levenberg-Marquardt steps on the truncated Sampson cost from model = (U, V, sig), inliers re-selected at
     every model."""
     x = [float(v) for v in model[0]], [float(v) for v in model[1]], float(model[2])
-    return lc.refine(lambda m: terms(norm, *m, pts, thr2), lambda m, d: update(*m, d), x, DOF, steps)
+    return lc.refine(lambda m: terms(norm, *m, pts, thr2), lambda m, d: update(*m, d), x, DOF, steps, LAMBDA0)
 
 
 def rescore(norm, model, pts: np.ndarray, thr2: np.float32):

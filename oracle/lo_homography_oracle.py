@@ -112,7 +112,7 @@ def terms(norm, Hn, pts: np.ndarray, thr2: float) -> np.ndarray:
 
 def refine(norm, Hn, pts: np.ndarray, thr2: float, steps: int):
     """steps Levenberg-Marquardt steps on the truncated transfer cost from Hn, inliers re-selected at every model."""
-    return lc.refine(lambda x: terms(norm, x, pts, thr2), update, [float(v) for v in Hn], DOF, steps)
+    return lc.refine(lambda x: terms(norm, x, pts, thr2), update, [float(v) for v in Hn], DOF, steps, LAMBDA0)
 
 
 def rescore(norm, Hn, pts: np.ndarray, thr2: np.float32):

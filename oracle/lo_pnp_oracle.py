@@ -2,10 +2,10 @@
 csrc/lo_pnp_api.cu).
 
 The compaction, calibration, samples, Lambda Twist solutions, projections and fp32 inlier test are pnp_oracle's; the
-MSAC score is lo_pose_oracle's; the Cholesky step, quaternion rotation, LM loop and schedule are lo_common's.  What is
-new here is the fp32 reprojection error that the score reads and the Levenberg-Marquardt refinement of (R, t) on the
-truncated squared reprojection error in pixels (double, elementwise operations only, so the CUDA build compiled with
--fmad=false agrees bit for bit).
+MSAC score is lo_pose_oracle's; the Cholesky step, quaternion rotation, LM loop and schedule are lo_common's; the
+double residuals, Jacobian and step of (R, t) are pnp_oracle's.  What is new here is the fp32 reprojection error that
+the score reads and the truncated squared reprojection cost that the Levenberg-Marquardt refinement minimises
+(elementwise operations only, so the CUDA build compiled with -fmad=false agrees bit for bit).
 """
 from __future__ import annotations
 
@@ -20,6 +20,7 @@ S = pnp.S
 DOF = 6              # parameters of an LM step: a rotation increment and a translation increment
 TERMS = 28           # J^T J upper triangle (21), J^T r (6), truncated cost
 QSCALE, STEPS, FINAL_STEPS, LAMBDA0 = lpo.QSCALE, lpo.STEPS, lpo.FINAL_STEPS, lpo.LAMBDA0
+residuals, update = pnp.residuals, pnp.update  # A7's residuals, Jacobian and step, as the plain refit's
 
 
 def errors(P: np.ndarray, pix: np.ndarray, wld: np.ndarray) -> np.ndarray:
@@ -36,55 +37,18 @@ def errors(P: np.ndarray, pix: np.ndarray, wld: np.ndarray) -> np.ndarray:
         return np.where(w > 0.0, du * du + dv * dv, np.float32(np.inf))
 
 
-def residuals(x, K, pix: np.ndarray, wld: np.ndarray):
-    """At x = R (9, row-major) + t (3): double residuals (ru, rv) in pixels, errors ru*ru + rv*rv, depths Xc2 and the
-    Jacobian rows ju, jv [6, n] of A7 (header step LA7)."""
-    R, t = x[:9], x[9:]
-    fx, s, cx, fy, cy = (float(K[i]) for i in (0, 1, 2, 4, 5))
-    u, v = pix[:, 0].astype(np.float64), pix[:, 1].astype(np.float64)
-    W = [wld[:, i].astype(np.float64) for i in range(3)]
-    with np.errstate(all="ignore"):
-        Xc = [R[3 * i] * W[0] + R[3 * i + 1] * W[1] + R[3 * i + 2] * W[2] + t[i] for i in range(3)]
-        iz = 1.0 / Xc[2]
-        a, b = Xc[0] * iz, Xc[1] * iz
-        pu = fx * a + s * b
-        ru, rv = pu + cx - u, fy * b + cy - v
-        gu = [fx * iz, s * iz, -(pu * iz)]
-        gv = [np.zeros_like(iz), fy * iz, -(fy * b * iz)]
-
-        def jrow(g):
-            return [g[2] * Xc[1] - g[1] * Xc[2], g[0] * Xc[2] - g[2] * Xc[0], g[1] * Xc[0] - g[0] * Xc[1], g[0], g[1], g[2]]
-        ju, jv = np.stack(jrow(gu)), np.stack(jrow(gv))
-        err = ru * ru + rv * rv
-    return ru, rv, err, Xc[2], ju, jv
-
-
 def terms(x, K, pix: np.ndarray, wld: np.ndarray, thr2: float) -> np.ndarray:
     """The TERMS fixed-order sums at x: the points in front of the camera with err < thr2 give J^T J and J^T r, every
     point its truncated cost (err for those, else thr2)."""
     ru, rv, err, z, ju, jv = residuals(x, K, pix, wld)
     with np.errstate(invalid="ignore"):
         inl = (z > 0.0) & (err < thr2)
-    rows = []
-    with np.errstate(all="ignore"):
-        for i in range(DOF):
-            for j in range(i, DOF):
-                rows.append(np.where(inl, ju[i] * ju[j] + jv[i] * jv[j], 0.0))
-        for i in range(DOF):
-            rows.append(np.where(inl, ju[i] * ru + jv[i] * rv, 0.0))
-    rows.append(np.where(inl, err, thr2))
-    return go.fixed_sum(np.stack(rows))
-
-
-def update(x, d):
-    """R' = Q R, t' = Q t + d[3:] (A7's step)."""
-    Rn, tn = pnp._update(x[:9], x[9:], d)
-    return Rn + tn
+    return go.fixed_sum(np.stack(pnp.normal_sums(ru, rv, ju, jv, inl) + [np.where(inl, err, thr2)]))
 
 
 def refine(x, K, pix: np.ndarray, wld: np.ndarray, thr2: float, steps: int):
     """steps Levenberg-Marquardt steps on the truncated reprojection cost from x, inliers re-selected at every pose."""
-    return lc.refine(lambda y: terms(y, K, pix, wld, thr2), update, [float(v) for v in x], DOF, steps)
+    return lc.refine(lambda y: terms(y, K, pix, wld, thr2), update, [float(v) for v in x], DOF, steps, LAMBDA0)
 
 
 def rescore(x, K, pix: np.ndarray, wld: np.ndarray, thr2: np.float32):

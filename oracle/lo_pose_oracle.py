@@ -127,7 +127,7 @@ def update(R, t, d):
 def refine(R, t, pts: np.ndarray, thr2: float, steps: int):
     """steps Levenberg-Marquardt steps on the truncated Sampson cost from (R, t), inliers re-selected at every pose."""
     x = [float(v) for v in R], [float(v) for v in t]
-    return lc.refine(lambda m: terms(*m, pts, thr2), lambda m, d: update(*m, d), x, 5, steps)
+    return lc.refine(lambda m: terms(*m, pts, thr2), lambda m, d: update(*m, d), x, 5, steps, LAMBDA0)
 
 
 def model_errors(R, t, pts: np.ndarray) -> np.ndarray:

@@ -212,8 +212,10 @@ def solutions(seed: int, h: np.ndarray, bear: np.ndarray, wld: np.ndarray):
             np.take_along_axis(kept, order, 1))
 
 
-def _terms(R, t, K, pix, wld, inl):
-    """The refit's 28 sums at (R, t): J^T J (upper triangle, row order), J^T r and the cost, over the inliers."""
+def residuals(x, K, pix: np.ndarray, wld: np.ndarray):
+    """At x = R (9, row-major) + t (3): double residuals (ru, rv) in pixels, errors ru*ru + rv*rv, depths Xc2 and the
+    Jacobian rows ju, jv [6, n] of A7 (header steps A7 and LA7)."""
+    R, t = x[:9], x[9:]
     fx, s, cx, fy, cy = (float(K[i]) for i in (0, 1, 2, 4, 5))
     u, v = pix[:, 0].astype(np.float64), pix[:, 1].astype(np.float64)
     W = [wld[:, i].astype(np.float64) for i in range(3)]
@@ -228,40 +230,35 @@ def _terms(R, t, K, pix, wld, inl):
 
         def jrow(g):
             return [g[2] * Xc[1] - g[1] * Xc[2], g[0] * Xc[2] - g[2] * Xc[0], g[1] * Xc[0] - g[0] * Xc[1], g[0], g[1], g[2]]
-        ju, jv = jrow(gu), jrow(gv)
-        vals = [ju[i] * ju[j] + jv[i] * jv[j] for i in range(6) for j in range(i, 6)]
-        vals += [ju[i] * ru + jv[i] * rv for i in range(6)]
-        vals.append(ru * ru + rv * rv)
-    sums = go.fixed_sum(np.stack([np.where(inl, x, 0.0) for x in vals]))
-    return [float(x) for x in sums[:21]], [float(x) for x in sums[21:27]], float(sums[27])
+        ju, jv = np.stack(jrow(gu)), np.stack(jrow(gv))
+        err = ru * ru + rv * rv
+    return ru, rv, err, Xc[2], ju, jv
 
 
-def _update(R, t, d):
-    """R' = Q R, t' = Q t + d[3:] with Q the rotation of the unit quaternion (1, d[:3] / 2) / norm."""
+def normal_sums(ru, rv, ju, jv, inl) -> list:
+    """J^T J (upper triangle, row order) and J^T r over the points with inl, unsummed: 27 [n] arrays."""
+    with np.errstate(all="ignore"):
+        rows = [np.where(inl, ju[i] * ju[j] + jv[i] * jv[j], 0.0) for i in range(6) for j in range(i, 6)]
+        return rows + [np.where(inl, ju[i] * ru + jv[i] * rv, 0.0) for i in range(6)]
+
+
+def update(x, d):
+    """R' = Q R, t' = Q t + d[3:] with Q the rotation of the unit quaternion (1, d[:3] / 2) / norm (A7's step)."""
+    R, t = x[:9], x[9:]
     Q = lc.quat_rotation(d)
     Rn = [Q[3 * i] * R[j] + Q[3 * i + 1] * R[3 + j] + Q[3 * i + 2] * R[6 + j] for i in range(3) for j in range(3)]
     tn = [Q[3 * i] * t[0] + Q[3 * i + 1] * t[1] + Q[3 * i + 2] * t[2] + d[3 + i] for i in range(3)]
-    return Rn, tn
+    return Rn + tn
 
 
 def refine_lm(R, t, K, pix, wld, inl):
     """GEO_PNP_LM_STEPS Levenberg-Marquardt steps on the squared reprojection error of the inliers, from (R, t)."""
-    R, t = [float(c) for c in R], [float(c) for c in t]
-    Hu, g, cost = _terms(R, t, K, pix, wld, inl)
-    lam = LM_LAMBDA0
-    for _ in range(LM_STEPS):
-        d = lc.lm_solve(Hu, g, lam, 6)
-        if d is None:
-            lam = lam * 10.0
-            continue
-        Rn, tn = _update(R, t, d)
-        Hn, gn, cn = _terms(Rn, tn, K, pix, wld, inl)
-        if cn < cost:
-            R, t, Hu, g, cost = Rn, tn, Hn, gn, cn
-            lam = lam / 10.0
-        else:
-            lam = lam * 10.0
-    return np.array(R), np.array(t)
+    def terms(x):
+        ru, rv, err, _, ju, jv = residuals(x, K, pix, wld)
+        return go.fixed_sum(np.stack(normal_sums(ru, rv, ju, jv, inl) + [np.where(inl, err, 0.0)]))
+
+    x = lc.refine(terms, update, [float(c) for c in R] + [float(c) for c in t], 6, LM_STEPS, LM_LAMBDA0)
+    return np.array(x[:9]), np.array(x[9:])
 
 
 def _fail(M: int, drawn: int) -> dict:
@@ -281,20 +278,15 @@ def absolute_pose_pair(kpts0, points3d1, m0, K0, threshold, max_iters, confidenc
         return _fail(M, 0)
     bear = calibrate(K0, pix)
     thr2 = np.float32(threshold * threshold)
-    best_cnt, best_h, best_r, drawn = -1, -1, -1, 0
-    for c in range(-(-max_iters // CHUNK)):
-        h = np.arange(c * CHUNK, min((c + 1) * CHUNK, max_iters), dtype=np.int64)
+
+    def candidates(h):
         R, t, kept = solutions(seed, h, bear, wld)
-        if kept.any():
-            cnt = reproj_inliers(projection(R[kept], t[kept], K0), pix, wld, thr2).sum(1)
-            i = int(np.argmax(cnt))  # first maximum: the lowest (sample, solution)
-            if cnt[i] > best_cnt:
-                hh, rr = np.nonzero(kept)
-                best_cnt, best_h, best_r = int(cnt[i]), int(h[hh[i]]), int(rr[i])
-        drawn = min((c + 1) * CHUNK, max_iters)
-        ep = 1.0 - max(best_cnt, 0) / n
-        if drawn >= max_iters or drawn >= go.update_num_iters(confidence, ep, S, max_iters):
-            break
+        if not kept.any():
+            return None
+        hh, rr = np.nonzero(kept)
+        return reproj_inliers(projection(R[kept], t[kept], K0), pix, wld, thr2).sum(1), h[hh], rr
+
+    best_cnt, best_h, best_r, drawn = go.ransac_pair(n, S, max_iters, confidence, candidates)
     if best_h < 0:
         return _fail(M, drawn)
     R, t, _ = solutions(seed, np.array([best_h]), bear, wld)

@@ -406,20 +406,15 @@ def relative_pose_pair(kpts0, kpts1, m0, K0, K1, threshold, max_iters, confidenc
         return _fail(M, 0)
     pts = np.concatenate([calibrate(K0, px[:, :2]), calibrate(K1, px[:, 2:])], 1)
     thr2 = threshold2(K0, K1, threshold)
-    best_cnt, best_h, best_r, drawn = -1, -1, -1, 0
-    for c in range(-(-max_iters // CHUNK)):
-        h = np.arange(c * CHUNK, min((c + 1) * CHUNK, max_iters), dtype=np.int64)
+
+    def candidates(h):
         E, found = solutions(seed, h, pts)
-        if found.any():
-            cnt = (sampson(E[found], pts) < thr2).sum(1)  # integer counts: exact in any order
-            i = int(np.argmax(cnt))  # first maximum: the lowest (hypothesis, solution)
-            if cnt[i] > best_cnt:
-                hh, rr = np.nonzero(found)
-                best_cnt, best_h, best_r = int(cnt[i]), int(h[hh[i]]), int(rr[i])
-        drawn = min((c + 1) * CHUNK, max_iters)
-        ep = 1.0 - max(best_cnt, 0) / n
-        if drawn >= max_iters or drawn >= go.update_num_iters(confidence, ep, S, max_iters):
-            break
+        if not found.any():
+            return None
+        hh, rr = np.nonzero(found)
+        return (sampson(E[found], pts) < thr2).sum(1), h[hh], rr
+
+    best_cnt, best_h, best_r, drawn = go.ransac_pair(n, S, max_iters, confidence, candidates)
     if best_h < 0:
         return _fail(M, drawn)
     E, _ = solutions(seed, np.array([best_h]), pts)
@@ -427,15 +422,9 @@ def relative_pose_pair(kpts0, kpts1, m0, K0, K1, threshold, max_iters, confidenc
     if best_cnt >= REFIT_MIN:
         inl = sampson(E[0, best_r][None], pts)[0] < thr2
         x, y, u, v = (pts[:, q].astype(np.float64) for q in range(4))
-        ra = [u * x, u * y, u, v * x, v * y, v, x, y, np.ones_like(x)]
-        ata = go.fixed_sum(np.stack([np.where(inl, ra[i] * ra[j], 0.0) for i in range(9) for j in range(i, 9)]))
-        A, e = np.zeros((9, 9)), 0
-        for i in range(9):
-            for j in range(i, 9):
-                A[i, j] = A[j, i] = ata[e]
-                e += 1
+        ra = np.stack([u * x, u * y, u, v * x, v * y, v, x, y, np.ones_like(x)], 1)
         with np.errstate(all="ignore"):
-            refit = essential_projection(eigvec_smallest(A))
+            refit = essential_projection(eigvec_smallest(go.ata(ra, None, inl)))
         cands.append((refit, int((sampson(refit[None], pts)[0] < thr2).sum())))
     Ef, count = cands[1] if len(cands) == 2 and cands[1][1] >= cands[0][1] else cands[0]
     inl = sampson(Ef[None], pts)[0] < thr2
