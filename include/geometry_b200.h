@@ -428,6 +428,54 @@
  *      are those of the final (refined) model, where OpenCV returns the minimal model's mask; stopping is checked per
  *      chunk of GEO_CHUNK; the sampler is step 3's counter hash; there is no special case when n equals s; OpenCV's
  *      refinement is its own Levenberg-Marquardt solver on the same inliers, converging to the same least-squares fit.
+ *
+ * Lens distortion (geo_undistort_points, geo_distort_points; oracle/camera_oracle.py restates it bit for bit):
+ * OpenCV's rational model with thin prism terms.  The coefficients are (k1, k2, p1, p2[, k3[, k4, k5, k6[, s1, s2, s3,
+ * s4]]]): 4, 5, 8 or 12 of them, missing trailing ones zero.  COLMAP's SIMPLE_RADIAL (k), RADIAL (k1, k2), OPENCV
+ * (k1, k2, p1, p2) and FULL_OPENCV (k1, k2, p1, p2, k3, k4, k5, k6) are special cases.  Expressions evaluate left to
+ * right as written; every multiply and add rounds on its own.
+ *
+ * D1. Distort a normalised point (x, y): r2 = x*x + y*y, r4 = r2*r2, r6 = r4*r2, a1 = 2*x*y, a2 = r2 + 2*x*x,
+ *     a3 = r2 + 2*y*y, cdist = 1 + k1*r2 + k2*r4 + k3*r6, icdist2 = 1 / (1 + k4*r2 + k5*r4 + k6*r6),
+ *     xd = x*cdist*icdist2 + p1*a1 + p2*a2 + s1*r2 + s2*r4, yd = y*cdist*icdist2 + p1*a3 + p2*a1 + s3*r2 + s4*r4
+ *     (cv2.projectPoints' formula).  geo_distort_points maps a pixel (u, v) to y = (v - cy) / fy,
+ *     x = ((u - cx) - s*y) / fx (A2's rule), D1, and the pixel (fx*xd + s*yd + cx, fy*yd + cy).
+ * D2. Undistort a pixel (u, v), OpenCV's fixed-point iteration as cv2.undistortPointsIter runs it:
+ *     y0 = (v - cy) / fy, x0 = ((u - cx) - s*y0) / fx, (x, y) = (x0, y0), e = DBL_MAX.  Up to max_iters times: stop
+ *     when e < eps; r2 = x*x + y*y, icdist = (1 + ((k6*r2 + k5)*r2 + k4)*r2) / (1 + ((k3*r2 + k2)*r2 + k1)*r2);
+ *     when icdist < 0, (x, y) = (x0, y0) and stop; dx = 2*p1*x*y + p2*(r2 + 2*x*x) + s1*r2 + s2*r2*r2,
+ *     dy = p1*(r2 + 2*y*y) + 2*p2*x*y + s3*r2 + s4*r2*r2, x = (x0 - dx)*icdist, y = (y0 - dy)*icdist; with eps > 0,
+ *     (xd, yd) of D1 at (x, y), du = fx*xd + s*yd + cx - u, dv = fy*yd + cy - v and e = sqrt(du*du + dv*dv).  (eps = 0
+ *     never stops early: e >= 0.)  The output pixel is (fx*x + s*y + cx, fy*y + cy), cv2.undistortPoints with P = K.
+ *     OpenCV ignores the skew K[0][1] on input; with s = 0 the two agree.
+ * D3. Validity.  K is valid as P1 states it; the coefficients when all are finite.  An invalid K or coefficients, or a
+ *     non-finite input pixel, give a NaN output row, which every estimator here treats as an invalid match.  Inputs
+ *     are float or double, read as double; outputs are computed in double and written in the input's type.
+ *
+ * Distortion-aware absolute pose (geo_absolute_pose_dist, geo_absolute_pose_lo_dist; oracle/pnp_dist_oracle.py
+ * restates them bit for bit): cv2.solvePnPRansac with distCoeffs.  The minimal
+ * solutions see undistorted bearings; the inlier test and Levenberg-Marquardt see distorted pixels.  Each step is A1-A8
+ * (LA1-LA8 for the LO estimator) with these changes:
+ *
+ * AD1. Compaction as A1.  The calibrated coordinates that P3P reads are D2's (x, y) of the pixel with 5 iterations and
+ *      eps = 0 (cv2.solvePnP inside cv2.solvePnPRansac), rounded to float.  Coefficients that fail D3 fail the pair as
+ *      an invalid K0 does (A8).
+ * AD2. The inlier test, in fp32 without fused multiply-adds, in distorted pixels: M = [R | t] rounded to float
+ *      (m0..m11 row-major), Xc0 = m0*X + m1*Y + m2*Z + m3, Xc1 likewise with m4..m7, w = m8*X + m9*Y + m10*Z + m11;
+ *      x = Xc0 / w, y = Xc1 / w; D1 in fp32 with K0 and the coefficients rounded to float; du = u - (fx*xd + s*yd + cx),
+ *      dv = v - (fy*yd + cy).  An inlier has w > 0 and du*du + dv*dv < (float)(threshold * threshold).  The LO
+ *      estimator's MSAC term reads this error as LA3 reads A5's (+inf behind the camera).
+ * AD3. Levenberg-Marquardt (the refit of A7 and the LM of LA7), in double: Xc_i = R_i0*X + R_i1*Y + R_i2*Z + t_i,
+ *      iz = 1.0 / Xc2, a = Xc0*iz, b = Xc1*iz, (xd, yd) of D1 at (a, b), ru = fx*xd + s*yd + cx - u,
+ *      rv = fy*yd + cy - v.  D1's Jacobian at (a, b): r2 = a*a + b*b, r4 = r2*r2, id = 1.0 / (1.0 + k4*r2 + k5*r4 +
+ *      k6*r2*r4), c = (1.0 + k1*r2 + k2*r4 + k3*r2*r4)*id, dc = (k1 + 2.0*k2*r2 + 3.0*k3*r4 - c*(k4 + 2.0*k5*r2 +
+ *      3.0*k6*r4))*id, gx = s1 + 2.0*s2*r2, gy = s3 + 2.0*s4*r2, J00 = c + 2.0*a*(a*dc + gx) + 2.0*p1*b + 6.0*p2*a,
+ *      J01 = 2.0*b*(a*dc + p2 + gx) + 2.0*p1*a, J10 = 2.0*a*(b*dc + p1 + gy) + 2.0*p2*b, J11 = c + 2.0*b*(b*dc + gy)
+ *      + 6.0*p1*b + 2.0*p2*a.  With ua = fx*J00 + s*J10, ub = fx*J01 + s*J11, va = fy*J10, vb = fy*J11:
+ *      gu = (ua*iz, ub*iz, -((ua*a + ub*b)*iz)), gv = (va*iz, vb*iz, -((va*a + vb*b)*iz)), and A7's Jacobian rows
+ *      from gu and gv.  The refit's fixed inliers are those of AD2; LA7's inlier at a pose has Xc2 > 0 and
+ *      ru*ru + rv*rv < (double)thr2.  The parametrisation, schedule and sums are A7's and LA7's.
+ * AD4. Outputs, failures and diagnostics as A8 and LA8, with AD2's test in place of A5's.
  */
 #ifndef GEOMETRY_B200_H
 #define GEOMETRY_B200_H
@@ -620,6 +668,48 @@ typedef struct GeoLoPnpOutputs {
 LG_API size_t geo_lo_pnp_workspace_bytes(int32_t B, int32_t M, int32_t max_iters);
 LG_API int geo_absolute_pose_lo(const GeoPnpConfig* cfg, const GeoPnpInputs* in, GeoLoPnpOutputs* out,
                                 void* workspace, size_t workspace_bytes, void* stream);
+
+#define GEO_CAMERA_FLOAT32 0
+#define GEO_CAMERA_FLOAT64 1
+#define GEO_UNDISTORT_MAX_ITERS 1000
+
+typedef struct GeoCameraConfig {
+  int32_t abi_version; /* GEO_ABI_VERSION */
+  int32_t num_dist;    /* coefficients per pair: 4, 5, 8 or 12 */
+  int32_t max_iters;   /* D2's iterations, in [0, GEO_UNDISTORT_MAX_ITERS]; geo_distort_points ignores it */
+  int32_t dtype;       /* GEO_CAMERA_FLOAT32 or GEO_CAMERA_FLOAT64: the type of in->pts and out->pts */
+  double eps;          /* D2's reprojection stop in pixels, finite and >= 0; 0: none */
+} GeoCameraConfig;
+
+typedef struct GeoCameraInputs {
+  int32_t B, N;
+  const void* pts;     /* [B, N, 2] pixels */
+  const double* K;     /* [B, 9] row-major intrinsics */
+  const double* dist;  /* [B, num_dist] */
+} GeoCameraInputs;
+
+typedef struct GeoCameraOutputs {
+  void* pts;           /* [B, N, 2] pixels, the input's type */
+} GeoCameraOutputs;
+
+/* Lens distortion (steps D1-D3): one launch, B <= 65535, no workspace. */
+LG_API int geo_undistort_points(const GeoCameraConfig* cfg, const GeoCameraInputs* in, GeoCameraOutputs* out,
+                                void* stream);
+LG_API int geo_distort_points(const GeoCameraConfig* cfg, const GeoCameraInputs* in, GeoCameraOutputs* out,
+                              void* stream);
+
+typedef struct GeoPnpDistInputs {
+  GeoPnpInputs pnp;        /* as geo_absolute_pose's */
+  int32_t num_dist;        /* 4, 5, 8 or 12 */
+  const double* dist0;     /* [B, num_dist] distortion coefficients of image 0 */
+} GeoPnpDistInputs;
+
+/* Distortion-aware absolute pose (steps AD1-AD4); the workspaces are geo_pnp_workspace_bytes' and
+ * geo_lo_pnp_workspace_bytes'. */
+LG_API int geo_absolute_pose_dist(const GeoPnpConfig* cfg, const GeoPnpDistInputs* in, GeoPnpOutputs* out,
+                                  void* workspace, size_t workspace_bytes, void* stream);
+LG_API int geo_absolute_pose_lo_dist(const GeoPnpConfig* cfg, const GeoPnpDistInputs* in, GeoLoPnpOutputs* out,
+                                     void* workspace, size_t workspace_bytes, void* stream);
 
 #define GEO_AFFINE 3
 #define GEO_AFFINE_PARTIAL 4

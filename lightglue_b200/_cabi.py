@@ -25,6 +25,7 @@ GEO_ABI_VERSION = 1  # include/geometry_b200.h
 GEO_HOMOGRAPHY, GEO_FUNDAMENTAL, GEO_ESSENTIAL = 0, 1, 2
 GEO_LO_QSCALE, GEO_LO_MAX_MATCHES = 65536, (1 << 20) - 1
 GEO_AFFINE, GEO_AFFINE_PARTIAL, GEO_AFFINE_MAX_REFINE = 3, 4, 100
+GEO_CAMERA_FLOAT32, GEO_CAMERA_FLOAT64, GEO_UNDISTORT_MAX_ITERS = 0, 1, 1000
 NN_ABI_VERSION = 1  # include/nn_b200.h
 NN_MIN_DIM, NN_MAX_DIM, NN_GROUP_ROWS = 64, 512, 32768
 NN_GUIDE_H, NN_GUIDE_F = 0, 1
@@ -183,6 +184,25 @@ class GeoAffineConfig(C.Structure):
     ]
 
 
+class GeoCameraConfig(C.Structure):
+    _fields_ = [
+        ("abi_version", C.c_int32), ("num_dist", C.c_int32), ("max_iters", C.c_int32), ("dtype", C.c_int32),
+        ("eps", C.c_double),
+    ]
+
+
+class GeoCameraInputs(C.Structure):
+    _fields_ = [("B", C.c_int32), ("N", C.c_int32), ("pts", C.c_void_p), ("K", C.c_void_p), ("dist", C.c_void_p)]
+
+
+class GeoCameraOutputs(C.Structure):
+    _fields_ = [("pts", C.c_void_p)]
+
+
+class GeoPnpDistInputs(C.Structure):
+    _fields_ = [("pnp", GeoPnpInputs), ("num_dist", C.c_int32), ("dist0", C.c_void_p)]
+
+
 class NnConfig(C.Structure):
     _fields_ = [
         ("abi_version", C.c_int32), ("dim", C.c_int32), ("mutual_check", C.c_int32), ("ratio_thresh", C.c_float),
@@ -299,6 +319,14 @@ GEO_PROTOTYPES = {  # include/geometry_b200.h
     "geo_lo_pnp_workspace_bytes": (_SZ, [_I32, _I32, _I32]),
     "geo_absolute_pose_lo": (C.c_int, [C.POINTER(GeoPnpConfig), C.POINTER(GeoPnpInputs), C.POINTER(GeoLoPnpOutputs),
                                        _VP, _SZ, _VP]),
+    "geo_undistort_points": (C.c_int, [C.POINTER(GeoCameraConfig), C.POINTER(GeoCameraInputs),
+                                       C.POINTER(GeoCameraOutputs), _VP]),
+    "geo_distort_points": (C.c_int, [C.POINTER(GeoCameraConfig), C.POINTER(GeoCameraInputs),
+                                     C.POINTER(GeoCameraOutputs), _VP]),
+    "geo_absolute_pose_dist": (C.c_int, [C.POINTER(GeoPnpConfig), C.POINTER(GeoPnpDistInputs),
+                                         C.POINTER(GeoPnpOutputs), _VP, _SZ, _VP]),
+    "geo_absolute_pose_lo_dist": (C.c_int, [C.POINTER(GeoPnpConfig), C.POINTER(GeoPnpDistInputs),
+                                            C.POINTER(GeoLoPnpOutputs), _VP, _SZ, _VP]),
     "geo_affine_workspace_bytes": (_SZ, [_I32, _I32, _I32]),
     "geo_estimate_affine": (C.c_int, [C.POINTER(GeoAffineConfig), C.POINTER(GeoInputs), C.POINTER(GeoOutputs), _VP,
                                       _SZ, _VP]),

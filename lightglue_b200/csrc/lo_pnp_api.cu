@@ -2,8 +2,9 @@
 // Levenberg-Marquardt local optimisation of (R, t) and a final refinement (include/geometry_b200.h, steps LA1-LA8), on
 // lo_common.cuh's schedule.  pnp_api.cu's compaction and calibration kernel prepares the pair; geo_hyp_kernel draws up
 // to 4 P3P solutions as fp32 projections; a local optimisation starts from its solution re-solved in double and runs LM
-// on the truncated reprojection cost; the final kernel writes the inlier mask of every row of matches0.  Compiled with
-// -fmad=false: oracle/lo_pnp_oracle.py takes the same steps.
+// on the truncated reprojection cost; the final kernel writes the inlier mask of every row of matches0.  With lens
+// distortion (geo_absolute_pose_lo_dist, steps AD1-AD4) PnpDistLo runs the same schedule in distorted pixels.  Compiled
+// with -fmad=false: oracle/lo_pnp_oracle.py takes the same steps.
 #include <stdint.h>
 
 #include "lo_common.cuh"
@@ -130,6 +131,127 @@ struct PnpLo {
   }
 };
 
+// ---- with lens distortion (header steps AD1-AD4 on LA1-LA8) ----
+
+// One compacted point and the pair's camera for AD2's test
+struct PnpDistPoint {
+  float4 p, q;
+  const Camera<float>* cam;
+};
+
+struct PnpDistPoints {
+  const float4* pix;
+  const float4* wld;
+  Camera<float> cam;
+  __device__ __forceinline__ PnpDistPoint operator[](int k) const { return {pix[k], wld[k], &cam}; }
+};
+
+// LoPnpScore with AD2's error of every [R | t]
+struct LoPnpDistScore {
+  using Args = LoArgs<PnpDistArgs>;
+  using Acc = unsigned long long;
+  static constexpr int SOLS = ::SOLS, NF = 12, K = 2, TILE = ::TILE;
+  static __device__ const PnpWs& ws(const Args& a) { return a.p.w; }
+  const float4* src[K];
+  unsigned long long* sums;
+  float thr2, w;
+  Camera<float> cam;
+  __device__ LoPnpDistScore(const Args& a, const PnpPair& P, int b)
+      : src{a.p.w.pts + (long)b * a.p.M, a.p.w.wld + (long)b * a.p.M}, sums(a.l.acc), thr2(P.thr2),
+        w((float)GEO_LO_QSCALE / P.thr2), cam(pair_camera<float>(a.p, b)) {}
+  __device__ unsigned long long term(const float* g, const float4* p) const {
+    return lo_term(dist_reproj_err(g, cam, p[0], p[1]), thr2, w);
+  }
+};
+
+// PnpLo with AD2's error and AD3's residuals: x = R (0-8, row-major) and t (9-11), scored as [R | t]; the pair's
+// constants are its camera in double
+struct PnpDistLo {
+  static constexpr int DOF = 6, TERMS = 28, GROUP = 14, NP = 12, NF = 12, S = ::S, SOLS = ::SOLS;
+  using Base = PnpDistArgs;
+  using Args = LoArgs<PnpDistArgs>;
+  using Solver = PnpDistSolver;
+  using Score = LoPnpDistScore;
+  struct Scratch {};
+
+  static __device__ void terms(LoShared<PnpDistLo>& s, const Camera<double>& c, const double* x,
+                               const PnpDistPoints& pts, int n, double thr2, double* out, int tid) {
+    double acc[TERMS];
+#pragma unroll
+    for (int i = 0; i < TERMS; ++i) acc[i] = 0.0;
+    for (int k = tid; k < n; k += RED) {
+      const PnpDistResidual e = pnp_dist_residual(c, x, x + 9, pts.pix[k], pts.wld[k]);
+      const double err = e.ru * e.ru + e.rv * e.rv;
+      const bool in = e.Xc[2] > 0.0 && err < thr2;
+      acc[TERMS - 1] = acc[TERMS - 1] + (in ? err : thr2);
+      if (in) pnp_dist_add_normal(c, e, acc);
+    }
+    lo_tree_sums<TERMS, GROUP>(acc, s.red, out, tid);
+  }
+
+  static __device__ void update(LoShared<PnpDistLo>&, const double* x, const double* d, double* out) {
+    lm_update(x, x + 9, d, out, out + 9);
+  }
+
+  static __device__ void pixels(LoShared<PnpDistLo>&, const Camera<double>&, const double* x, double* out) {
+    rt_matrix(x, out);
+  }
+
+  static __device__ __forceinline__ float err(const float* g, PnpDistPoint pt) {
+    return dist_reproj_err(g, *pt.cam, pt.p, pt.q);
+  }
+
+  static __device__ PnpDistPoints points(const Args& a, int b) {
+    return {a.p.w.pts + (long)b * a.p.M, a.p.w.wld + (long)b * a.p.M, pair_camera<float>(a.p, b)};
+  }
+  static __device__ Camera<double> consts(const Args& a, int b) { return pair_camera<double>(a.p, b); }
+  static __device__ float thr2(const Args& a, int b) { return a.p.w.pair[b].thr2; }
+
+  static __device__ void seed(LoShared<PnpDistLo>& s, const Args& a, int b, unsigned hr, long, LoPair& L, int t) {
+    if (t == 0) {
+      double x[SOLS][12];
+      PnpDistSolver::solve(a.p, b, hr >> 4, x);
+      for (int i = 0; i < 12; ++i) s.x[i] = L.model[i] = x[hr & 15][i];
+    }
+  }
+
+  static __device__ void store(LoShared<PnpDistLo>& s, LoPair& L) {
+    for (int i = 0; i < 12; ++i) L.model[i] = s.x[i];
+  }
+
+  static __device__ void load(LoShared<PnpDistLo>& s, const Args&, int, const LoPair& L, int t) {
+    if (t < 12) s.x[t] = L.model[t];
+  }
+
+  static __device__ void restore(LoShared<PnpDistLo>& s, const Args&, int, const LoPair& L, int t) {
+    if (t == 0) {
+      for (int i = 0; i < 12; ++i) s.x[i] = L.model[i];
+      rt_matrix(L.model, s.px);
+      for (int i = 0; i < 12; ++i) s.fm[i] = (float)s.px[i];
+      s.score = (unsigned long long)L.count * LO_COUNT_ONE + L.score;
+    }
+    __syncthreads();
+  }
+
+  static __device__ void fail(const Args& a, int b, int t) {
+    if (t < 9) a.p.out.R[(long)b * 9 + t] = 0.0;
+    if (t < 3) a.p.out.t[(long)b * 3 + t] = 0.0;
+  }
+
+  // AD4: AD2's test per row of matches0
+  static __device__ void write(LoShared<PnpDistLo>& s, const Args& a, int b, int t) {
+    const PnpDistPoints pts = points(a, b);
+    const int* slot = a.p.w.slot + (long)b * a.p.M;
+    uint8_t* inl = a.p.out.inliers + (long)b * a.p.M;
+    for (int i = t; i < a.p.M; i += RED) {
+      const int k = slot[i];
+      inl[i] = k >= 0 && err(s.fm, pts[k]) < a.p.w.pair[b].thr2;
+    }
+    if (t < 9) a.p.out.R[(long)b * 9 + t] = s.x[t];
+    if (t < 3) a.p.out.t[(long)b * 3 + t] = s.x[9 + t];
+  }
+};
+
 }  // namespace
 
 extern "C" size_t geo_lo_pnp_workspace_bytes(int32_t B, int32_t M, int32_t) {
@@ -148,15 +270,26 @@ extern "C" int geo_absolute_pose_lo(const GeoPnpConfig* cfg, const GeoPnpInputs*
                            geo_lo_pnp_workspace_bytes(in->B, in->M, cfg->max_iters));
   }
   if (rc != GEO_RUN) return rc;
-  PnpArgs p{};
-  p.B = in->B; p.M = in->M; p.N = in->N;
-  p.max_iters = cfg->max_iters;
-  p.chunks = geo_chunks(cfg->max_iters);
-  p.seed = cfg->seed;
-  p.threshold = cfg->threshold;
-  p.confidence = cfg->confidence;
-  p.kpts0 = in->kpts0; p.points3d1 = in->points3d1; p.matches0 = in->matches0;
-  p.K0 = in->K0;
+  PnpArgs p = pnp_args(cfg, in);
   p.out = out->pnp;
   return lo_launch<PnpLo>(p, out->num_local_optimizations, out->cost, workspace, pnp_prepare_kernel, stream_);
+}
+
+extern "C" int geo_absolute_pose_lo_dist(const GeoPnpConfig* cfg, const GeoPnpDistInputs* din, GeoLoPnpOutputs* out,
+                                         void* workspace, size_t workspace_bytes, void* stream_) {
+  const char* entry = "geo_absolute_pose_lo_dist";
+  const GeoPnpInputs* in = din ? &din->pnp : nullptr;
+  int rc = geo_check_config(entry, cfg, in, out, GEO_LO_MAX_MATCHES, geo_no_check,
+                            [&] { return dist_count_check(din->num_dist); });
+  if (rc == GEO_RUN) {
+    const GeoPnpOutputs& o = out->pnp;
+    rc = geo_check_buffers(entry, in, {o.R, o.t, o.num_inliers, o.success, o.best_hypothesis, o.best_solution,
+                                       o.num_hypotheses, out->num_local_optimizations, out->cost}, {o.inliers},
+                           {in->K0, din->dist0}, in->points3d1, workspace, workspace_bytes,
+                           geo_lo_pnp_workspace_bytes(in->B, in->M, cfg->max_iters));
+  }
+  if (rc != GEO_RUN) return rc;
+  PnpDistArgs p{pnp_args(cfg, in), din->dist0, din->num_dist};
+  p.out = out->pnp;
+  return lo_launch<PnpDistLo>(p, out->num_local_optimizations, out->cost, workspace, pnp_dist_prepare_kernel, stream_);
 }

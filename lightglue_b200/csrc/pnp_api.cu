@@ -12,8 +12,10 @@
 //   final    geo_final_kernel<PnpRansac>, one CTA per pair: folds the last chunk, Levenberg-Marquardt from the best
 //            solution (lo_common.cuh's loop), recount, R and t
 //   mask     pnp_mask_kernel, one thread per row of matches0: the final inlier mask
-// A stopped pair's CTAs return at once.  Compiled with -fmad=false, like geo_api.cu: oracle/pnp_oracle.py takes the same
-// steps in numpy.
+// A stopped pair's CTAs return at once.  With lens distortion (geo_absolute_pose_dist, steps AD1-AD4) the same launches
+// run pnp_dist_prepare_kernel (D2's calibrated coordinates), PnpDistScore and PnpDistRansac (the float model is [R | t]
+// and the test is in distorted pixels) and pnp_dist_mask_kernel.  Compiled with -fmad=false, like geo_api.cu:
+// oracle/pnp_oracle.py takes the same steps in numpy.
 #include <stdint.h>
 
 #include "lo_common.cuh"
@@ -119,6 +121,105 @@ __global__ void __launch_bounds__(MASK_THREADS) pnp_mask_kernel(PnpArgs a) {
   a.out.inliers[(long)b * a.M + i] = in;
 }
 
+// ---- with lens distortion (header steps AD1-AD4) ----
+
+// AD2's inlier counts of every [R | t], on a tile of pixels and world points
+struct PnpDistScore {
+  using Args = PnpDistArgs;
+  using Acc = int;
+  static constexpr int SOLS = ::SOLS, NF = 12, K = 2, TILE = ::TILE;
+  static __device__ const PnpWs& ws(const PnpDistArgs& a) { return a.w; }
+  const float4* src[K];
+  int* sums;
+  float thr2;
+  Camera<float> cam;
+  __device__ PnpDistScore(const PnpDistArgs& a, const PnpPair& P, int b)
+      : src{a.w.pts + (long)b * a.M, a.w.wld + (long)b * a.M}, sums(a.w.count), thr2(P.thr2),
+        cam(pair_camera<float>(a, b)) {}
+  __device__ int term(const float* g, const float4* p) const { return dist_reproj_err(g, cam, p[0], p[1]) < thr2; }
+};
+
+// The refinement's points and its fixed inlier set: those of the float [R | t] fm under AD2
+struct PnpDistFixed {
+  const float4* pix;
+  const float4* wld;
+  const float* fm;
+  Camera<float> cam;
+};
+
+// PnpLm with AD3's residuals; the pair's constants are its camera in double
+struct PnpDistLm {
+  static constexpr int DOF = 6, TERMS = 28, GROUP = 14, NP = 12, NF = 12;
+  struct Scratch {};
+
+  static __device__ void terms(LoShared<PnpDistLm>& s, const Camera<double>& c, const double* x,
+                               const PnpDistFixed& pts, int n, double thr2, double* out, int tid) {
+    double acc[TERMS];
+#pragma unroll
+    for (int i = 0; i < TERMS; ++i) acc[i] = 0.0;
+    for (int k = tid; k < n; k += RED) {
+      const float4 p = pts.pix[k], q = pts.wld[k];
+      if (!(dist_reproj_err(pts.fm, pts.cam, p, q) < (float)thr2)) continue;
+      const PnpDistResidual e = pnp_dist_residual(c, x, x + 9, p, q);
+      pnp_dist_add_normal(c, e, acc);
+      acc[TERMS - 1] = acc[TERMS - 1] + (e.ru * e.ru + e.rv * e.rv);
+    }
+    lo_tree_sums<TERMS, GROUP>(acc, s.red, out, tid);
+  }
+
+  static __device__ void update(LoShared<PnpDistLm>&, const double* x, const double* d, double* out) {
+    lm_update(x, x + 9, d, out, out + 9);
+  }
+};
+
+// PnpRansac with AD2's test and AD3's refit; the float model is [R | t]
+struct PnpDistRansac : PnpDistSolver {
+  using Base = PnpDistArgs;
+  using Score = PnpDistScore;
+  using Scratch = LoShared<PnpDistLm>;
+
+  static __device__ bool inlier(const PnpDistArgs& a, int b, const float* g, int k) {
+    const long i = (long)b * a.M + k;
+    return dist_reproj_err(g, pair_camera<float>(a, b), a.w.pts[i], a.w.wld[i]) < a.w.pair[b].thr2;
+  }
+  static __device__ void clear(const PnpDistArgs&, int, int) {}  // pnp_dist_mask_kernel writes every row
+  static __device__ void fail(const PnpDistArgs& a, int b, int t) { PnpRansac::fail(a, b, t); }
+  static __device__ bool refits(const PnpDistArgs&, int hcount) { return hcount >= GEO_PNP_REFIT_MIN; }
+
+  static __device__ void refit(GeoFinal<PnpDistRansac>& s, const PnpDistArgs& a, int b, int t) {
+    if (t == 0)
+      for (int i = 0; i < 12; ++i) s.m.x[i] = s.x[0][i];
+    __syncthreads();
+    const PnpDistFixed pts{a.w.pts + (long)b * a.M, a.w.wld + (long)b * a.M, s.fm[0], pair_camera<float>(a, b)};
+    const float thr2 = a.w.pair[b].thr2;
+    lo_refine(s.m, pair_camera<double>(a, b), pts, a.w.pair[b].n, (double)thr2, GEO_PNP_LM_STEPS, GEO_PNP_LM_LAMBDA0,
+              t);
+    if (t == 0)
+      for (int i = 0; i < 12; ++i) s.x[1][i] = s.m.x[i];
+  }
+
+  // R, t, and [R | t] for pnp_dist_mask_kernel
+  static __device__ void write(GeoFinal<PnpDistRansac>& s, const PnpDistArgs& a, int b, int u, int t) {
+    PnpPair& P = a.w.pair[b];
+    if (t < 12) P.P[t] = s.fm[u][t];
+    if (t < 9) a.out.R[(long)b * 9 + t] = s.x[u][t];
+    if (t < 3) a.out.t[(long)b * 3 + t] = s.x[u][9 + t];
+    if (t == 0) P.success = 1;
+  }
+};
+
+__global__ void __launch_bounds__(MASK_THREADS) pnp_dist_mask_kernel(PnpDistArgs a) {
+  const int b = blockIdx.x, i = blockIdx.y * MASK_THREADS + threadIdx.x;
+  if (i >= a.M) return;
+  const PnpPair& P = a.w.pair[b];
+  const int k = a.w.slot[(long)b * a.M + i];
+  bool in = false;
+  if (P.success && k >= 0)
+    in = dist_reproj_err(P.P, pair_camera<float>(a, b), a.w.pts[(long)b * a.M + k], a.w.wld[(long)b * a.M + k]) <
+         P.thr2;
+  a.out.inliers[(long)b * a.M + i] = in;
+}
+
 }  // namespace
 
 extern "C" size_t geo_pnp_workspace_bytes(int32_t B, int32_t M, int32_t) {
@@ -137,21 +238,37 @@ extern "C" int geo_absolute_pose(const GeoPnpConfig* cfg, const GeoPnpInputs* in
                            in->points3d1, workspace, workspace_bytes,
                            geo_pnp_workspace_bytes(in->B, in->M, cfg->max_iters));
   if (rc != GEO_RUN) return rc;
-  PnpArgs a{};
+  PnpArgs a = pnp_args(cfg, in);
   carve(geo_workspace_base(workspace), in->B, in->M, &a.w);
-  a.B = in->B; a.M = in->M; a.N = in->N;
-  a.max_iters = cfg->max_iters;
-  a.chunks = geo_chunks(cfg->max_iters);
-  a.seed = cfg->seed;
-  a.threshold = cfg->threshold;
-  a.confidence = cfg->confidence;
-  a.kpts0 = in->kpts0; a.points3d1 = in->points3d1; a.matches0 = in->matches0;
-  a.K0 = in->K0;
   a.out = *out;
   const cudaStream_t stream = (cudaStream_t)stream_;
   if (int rc = geo_launch<PnpRansac>(a, pnp_prepare_kernel, stream)) return rc;
   if (a.M > 0) {
     pnp_mask_kernel<<<dim3(a.B, (a.M + MASK_THREADS - 1) / MASK_THREADS), MASK_THREADS, 0, stream>>>(a);
+    LG_CHECK_LAUNCH();
+  }
+  return 0;
+}
+
+extern "C" int geo_absolute_pose_dist(const GeoPnpConfig* cfg, const GeoPnpDistInputs* din, GeoPnpOutputs* out,
+                                      void* workspace, size_t workspace_bytes, void* stream_) {
+  const char* entry = "geo_absolute_pose_dist";
+  const GeoPnpInputs* in = din ? &din->pnp : nullptr;
+  int rc = geo_check_config(entry, cfg, in, out, INT_MAX, geo_no_check,
+                            [&] { return dist_count_check(din->num_dist); });
+  if (rc == GEO_RUN)
+    rc = geo_check_buffers(entry, in, {out->R, out->t, out->num_inliers, out->success, out->best_hypothesis,
+                                       out->best_solution, out->num_hypotheses}, {out->inliers}, {in->K0, din->dist0},
+                           in->points3d1, workspace, workspace_bytes,
+                           geo_pnp_workspace_bytes(in->B, in->M, cfg->max_iters));
+  if (rc != GEO_RUN) return rc;
+  PnpDistArgs a{pnp_args(cfg, in), din->dist0, din->num_dist};
+  carve(geo_workspace_base(workspace), in->B, in->M, &a.w);
+  a.out = *out;
+  const cudaStream_t stream = (cudaStream_t)stream_;
+  if (int rc = geo_launch<PnpDistRansac>(a, pnp_dist_prepare_kernel, stream)) return rc;
+  if (a.M > 0) {
+    pnp_dist_mask_kernel<<<dim3(a.B, (a.M + MASK_THREADS - 1) / MASK_THREADS), MASK_THREADS, 0, stream>>>(a);
     LG_CHECK_LAUNCH();
   }
   return 0;

@@ -1,10 +1,12 @@
 // The absolute-pose pieces shared by the plain (pnp_api.cu, header steps A1-A8) and the LO-RANSAC estimator
 // (lo_pnp_api.cu, LA1-LA8), both compiled with -fmad=false: the workspace, the compaction kernel, the Lambda Twist
-// solver, the projection, the fp32 reprojection test and the pose update of the Levenberg-Marquardt steps.
+// solver, the projection, the fp32 reprojection test and the pose update of the Levenberg-Marquardt steps; and their
+// counterparts with lens distortion (AD1-AD4).
 #pragma once
 #include <stdint.h>
 
 #include "block_scan.cuh"
+#include "camera_common.cuh"
 #include "geo_common.cuh"
 #include "geo_lm.cuh"
 #include "lg_internal.h"
@@ -292,12 +294,10 @@ __device__ __forceinline__ PnpResidual pnp_residual(const double* K, const doubl
   return e;
 }
 
-// Adds the point's J^T J upper triangle (acc[0..20]) and J^T r (acc[21..26]) in A7's parameters (header step A7)
-__device__ __forceinline__ void pnp_add_normal(const double* K, const PnpResidual& e, double* acc) {
-  const double fx = K[0], sk = K[1], fy = K[4];
-  const double* Xc = e.Xc;
-  const double gu[3] = {fx * e.iz, sk * e.iz, -(e.pu * e.iz)};
-  const double gv[3] = {0.0, fy * e.iz, -(fy * e.bx * e.iz)};
+// Adds a point's J^T J upper triangle (acc[0..20]) and J^T r (acc[21..26]) in A7's parameters, from its camera-frame
+// point Xc, the gradients gu, gv of its residuals (ru, rv) with respect to Xc, and the residuals (header step A7)
+__device__ __forceinline__ void pnp_add_rows(const double* Xc, const double* gu, const double* gv, double ru, double rv,
+                                             double* acc) {
   const double ju[6] = {gu[2] * Xc[1] - gu[1] * Xc[2], gu[0] * Xc[2] - gu[2] * Xc[0], gu[1] * Xc[0] - gu[0] * Xc[1],
                         gu[0], gu[1], gu[2]};
   const double jv[6] = {gv[2] * Xc[1] - gv[1] * Xc[2], gv[0] * Xc[2] - gv[2] * Xc[0], gv[1] * Xc[0] - gv[0] * Xc[1],
@@ -308,13 +308,15 @@ __device__ __forceinline__ void pnp_add_normal(const double* K, const PnpResidua
 #pragma unroll
     for (int j = i; j < 6; ++j, ++k) acc[k] = acc[k] + (ju[i] * ju[j] + jv[i] * jv[j]);
 #pragma unroll
-  for (int i = 0; i < 6; ++i) acc[21 + i] = acc[21 + i] + (ju[i] * e.ru + jv[i] * e.rv);
+  for (int i = 0; i < 6; ++i) acc[21 + i] = acc[21 + i] + (ju[i] * ru + jv[i] * rv);
 }
 
-__device__ bool k_valid(const double* K) {
-  bool finite = true;
-  for (int i = 0; i < 9; ++i) finite = finite && isfinite(K[i]);
-  return finite && K[0] > 0.0 && K[4] > 0.0 && K[6] == 0.0 && K[7] == 0.0 && K[8] == 1.0;
+// The same sums of a pinhole residual (header step A7)
+__device__ __forceinline__ void pnp_add_normal(const double* K, const PnpResidual& e, double* acc) {
+  const double fx = K[0], sk = K[1], fy = K[4];
+  const double gu[3] = {fx * e.iz, sk * e.iz, -(e.pu * e.iz)};
+  const double gv[3] = {0.0, fy * e.iz, -(fy * e.bx * e.iz)};
+  pnp_add_rows(e.Xc, gu, gv, e.ru, e.rv, acc);
 }
 
 __global__ void __launch_bounds__(1024) pnp_prepare_kernel(PnpArgs a) {
@@ -370,6 +372,147 @@ __device__ void lm_update(const double* R, const double* t, const double* d, dou
     for (int j = 0; j < 3; ++j) Rn[3 * i + j] = Q[3 * i] * R[j] + Q[3 * i + 1] * R[3 + j] + Q[3 * i + 2] * R[6 + j];
     tn[i] = Q[3 * i] * t[0] + Q[3 * i + 1] * t[1] + Q[3 * i + 2] * t[2] + d[3 + i];
   }
+}
+
+// The kernel arguments of an entry point's configuration and inputs; the caller carves the workspace and sets out
+inline PnpArgs pnp_args(const GeoPnpConfig* cfg, const GeoPnpInputs* in) {
+  PnpArgs a{};
+  a.B = in->B; a.M = in->M; a.N = in->N;
+  a.max_iters = cfg->max_iters;
+  a.chunks = geo_chunks(cfg->max_iters);
+  a.seed = cfg->seed;
+  a.threshold = cfg->threshold;
+  a.confidence = cfg->confidence;
+  a.kpts0 = in->kpts0; a.points3d1 = in->points3d1; a.matches0 = in->matches0;
+  a.K0 = in->K0;
+  return a;
+}
+
+// ---- the distortion-aware absolute pose (header steps AD1-AD4) ----
+
+constexpr int PNP_UNDISTORT_ITERS = 5;  // AD1: cv2.solvePnP's undistortion
+
+struct PnpDistArgs : PnpArgs {
+  const double* dist0;  // [B, nd]
+  int nd;
+};
+
+__device__ __forceinline__ const double* pair_dist(const PnpDistArgs& a, int b) { return a.dist0 + (long)b * a.nd; }
+
+// Pair b's K0 and coefficients in T: double for the LM, float for AD2's test
+template <class T>
+__device__ __forceinline__ Camera<T> pair_camera(const PnpDistArgs& a, int b) {
+  return load_camera<T>(a.K0 + (long)b * 9, pair_dist(a, b), a.nd);
+}
+
+// AD1: pnp_prepare_kernel's compaction with D2's calibrated coordinates; invalid coefficients fail the pair as an
+// invalid K0.  A separate kernel, so that the pinhole one keeps its instructions.
+__global__ void __launch_bounds__(1024) pnp_dist_prepare_kernel(PnpDistArgs a) {
+  const int b = blockIdx.x, tid = threadIdx.x;
+  __shared__ int warp_sums[32];
+  __shared__ int carry;
+  if (tid == 0) carry = 0;
+  __syncthreads();
+  const double* K = a.K0 + (long)b * 9;
+  const double* dist = pair_dist(a, b);
+  const int64_t* m0 = a.matches0 + (long)b * a.M;
+  float4* pts = a.w.pts + (long)b * a.M;
+  float4* wld = a.w.wld + (long)b * a.M;
+  int* slot = a.w.slot + (long)b * a.M;
+  for (int base = 0; base < a.M; base += 1024) {
+    const int i = base + tid;
+    const int64_t j = i < a.M ? m0[i] : -1;
+    float X = 0.f, Y = 0.f, Z = 0.f;
+    float2 p = make_float2(0.f, 0.f);
+    if (j >= 0 && j < a.N) {
+      const float* q = a.points3d1 + ((long)b * a.N + j) * 3;
+      X = q[0];
+      Y = q[1];
+      Z = q[2];
+      p = reinterpret_cast<const float2*>(a.kpts0)[(long)b * a.M + i];
+    }
+    const bool valid = j >= 0 && j < a.N && isfinite(X) && isfinite(Y) && isfinite(Z) && finite2(p);
+    const int k = block_scan_step(valid, tid, warp_sums, &carry);
+    if (i < a.M) slot[i] = valid ? k : -1;
+    if (valid) {
+      double xx, yy;
+      undistort(load_camera<double>(K, dist, a.nd), p.x, p.y, PNP_UNDISTORT_ITERS, 0.0, &xx, &yy);
+      pts[k] = make_float4(p.x, p.y, (float)xx, (float)yy);
+      wld[k] = make_float4(X, Y, Z, 0.f);
+    }
+  }
+  __syncthreads();
+  if (tid == 0) {
+    PnpPair& P = a.w.pair[b];
+    P.thr2 = (float)(a.threshold * a.threshold);
+    P.best = 0;
+    P.n = carry;
+    P.ok = carry >= S && k_valid(K) && dist_valid(dist, a.nd);
+    P.stop = !P.ok;
+    P.drawn = 0;
+    P.success = 0;
+  }
+}
+
+// M = [R | t] as a row-major 3x4, the model AD2 rounds to float
+__device__ __forceinline__ void rt_matrix(const double* x, double* M) {
+  for (int i = 0; i < 3; ++i) {
+    for (int j = 0; j < 3; ++j) M[i * 4 + j] = x[i * 3 + j];
+    M[i * 4 + 3] = x[9 + i];
+  }
+}
+
+// geo_hyp_kernel's solver of the distortion-aware pose: PnpSolver's P3P solutions, scored as [R | t]
+struct PnpDistSolver : PnpSolver {
+  static __device__ void pixels(const PnpArgs&, int, const double* x, double* px) { rt_matrix(x, px); }
+};
+
+// AD2's fp32 error of one point under the float [R | t] g: du * du + dv * dv in distorted pixels in front of the
+// camera, +inf behind it (so that an inlier has err < thr2 and lo_term counts the others as outliers)
+__device__ __forceinline__ float dist_reproj_err(const float* g, const Camera<float>& c, float4 p, float4 q) {
+  const float X0 = g[0] * q.x + g[1] * q.y + g[2] * q.z + g[3];
+  const float X1 = g[4] * q.x + g[5] * q.y + g[6] * q.z + g[7];
+  const float w = g[8] * q.x + g[9] * q.y + g[10] * q.z + g[11];
+  float xd, yd;
+  distort(c.d, X0 / w, X1 / w, &xd, &yd);
+  const float du = p.x - (c.fx * xd + c.s * yd + c.cx), dv = p.y - (c.fy * yd + c.cy);
+  return w > 0.f ? du * du + dv * dv : INFINITY;
+}
+
+// AD3's residual (ru, rv) of world point q at pixel p, in distorted pixels, and what its Jacobian needs
+struct PnpDistResidual {
+  double Xc[3];  // the camera-frame point; Xc[2] is its depth
+  double iz, a, b, ru, rv;
+};
+
+__device__ __forceinline__ PnpDistResidual pnp_dist_residual(const Camera<double>& c, const double* R, const double* t,
+                                                             float4 p, float4 q) {
+  const double W[3] = {q.x, q.y, q.z};
+  PnpDistResidual e;
+  for (int i = 0; i < 3; ++i) e.Xc[i] = R[3 * i] * W[0] + R[3 * i + 1] * W[1] + R[3 * i + 2] * W[2] + t[i];
+  e.iz = 1.0 / e.Xc[2];
+  e.a = e.Xc[0] * e.iz;
+  e.b = e.Xc[1] * e.iz;
+  double xd, yd;
+  distort(c.d, e.a, e.b, &xd, &yd);
+  e.ru = c.fx * xd + c.s * yd + c.cx - (double)p.x;
+  e.rv = c.fy * yd + c.cy - (double)p.y;
+  return e;
+}
+
+// AD3's J^T J and J^T r terms of one point: A7's rows through D1's Jacobian
+__device__ __forceinline__ void pnp_dist_add_normal(const Camera<double>& c, const PnpDistResidual& e, double* acc) {
+  double J[4];
+  distort_jacobian(c.d, e.a, e.b, J);
+  const double ua = c.fx * J[0] + c.s * J[2], ub = c.fx * J[1] + c.s * J[3], va = c.fy * J[2], vb = c.fy * J[3];
+  const double gu[3] = {ua * e.iz, ub * e.iz, -((ua * e.a + ub * e.b) * e.iz)};
+  const double gv[3] = {va * e.iz, vb * e.iz, -((va * e.a + vb * e.b) * e.iz)};
+  pnp_add_rows(e.Xc, gu, gv, e.ru, e.rv, acc);
+}
+
+// The entry points' check of the coefficient count, at geo_check_config's distance() place
+inline const char* dist_count_check(int nd) {
+  return nd == 4 || nd == 5 || nd == 8 || nd == 12 ? nullptr : "num_dist must be 4, 5, 8 or 12";
 }
 
 }  // namespace

@@ -29,6 +29,7 @@ import ctypes as C
 import torch
 
 from . import _cabi
+from .camera import dist_coeffs
 
 
 def _check_params(threshold, max_iters, confidence, seed) -> None:
@@ -253,11 +254,11 @@ def _relative_pose(lo: bool, kpts0, kpts1, matches0, K0, K1, ransac_reproj_thres
 
 def estimate_absolute_pose(kpts0: torch.Tensor, points3d1: torch.Tensor, matches0: torch.Tensor, K0: torch.Tensor,
                            ransac_reproj_threshold: float = 8.0, max_iters: int = 100, confidence: float = 0.99,
-                           seed: int = 0) -> dict:
+                           seed: int = 0, dist_coeffs0: torch.Tensor | None = None) -> dict:
     """Absolute pose per pair from 2D-3D matches: Lambda Twist P3P RANSAC on the query pixels ``kpts0`` [B, M, 2] and
     the world points ``points3d1`` [B, N, 3] of image 1's keypoints (a row with a non-finite coordinate has no 3D point,
     so its matches are invalid), then Levenberg-Marquardt on the inliers.  An inlier lies in front of the camera with a
-    squared reprojection error through ``K0`` ([3, 3] or [B, 3, 3], no distortion) below
+    squared reprojection error through ``K0`` ([3, 3] or [B, 3, 3]; lens distortion: ``dist_coeffs0`` below) below
     ``ransac_reproj_threshold ** 2``.  Defaults of ``cv2.solvePnPRansac``.
 
     Returns ``R`` [B, 3, 3] and ``t`` [B, 3] float64 with x_cam = R X + t (OpenCV's rvec/tvec convention);
@@ -265,13 +266,19 @@ def estimate_absolute_pose(kpts0: torch.Tensor, points3d1: torch.Tensor, matches
     diagnostics ``best_hypothesis``, ``best_solution`` and ``num_hypotheses`` [B] int32.  A pair with fewer than 3
     valid matches, an invalid K0 (a non-finite entry, fx or fy <= 0, or a bottom row other than [0, 0, 1]) or no
     non-degenerate sample has ``success`` False, zero R and t, no inliers and -1 for ``best_hypothesis`` and
-    ``best_solution``."""
-    return _absolute_pose(False, kpts0, points3d1, matches0, K0, ransac_reproj_threshold, max_iters, confidence, seed)
+    ``best_solution``.
+
+    ``dist_coeffs0`` ([k] or [B, k], k = 4, 5, 8 or 12; see ``lightglue_b200.camera``) gives the query camera's lens
+    distortion, as ``cv2.solvePnPRansac(..., distCoeffs)`` takes it: the P3P samples see the pixels undistorted by
+    OpenCV's 5 fixed-point iterations, and the inlier test and the refit measure the reprojection error in distorted
+    pixels (header steps AD1-AD4).  A pair with a non-finite coefficient fails as one with an invalid K0."""
+    return _absolute_pose(False, kpts0, points3d1, matches0, K0, ransac_reproj_threshold, max_iters, confidence, seed,
+                          dist_coeffs0)
 
 
 def estimate_absolute_pose_lo(kpts0: torch.Tensor, points3d1: torch.Tensor, matches0: torch.Tensor, K0: torch.Tensor,
                               ransac_reproj_threshold: float = 8.0, max_iters: int = 100, confidence: float = 0.99,
-                              seed: int = 0) -> dict:
+                              seed: int = 0, dist_coeffs0: torch.Tensor | None = None) -> dict:
     """LO-RANSAC absolute pose per pair: the samples and P3P solutions of ``estimate_absolute_pose``, scored by a
     truncated (MSAC) squared reprojection error, with Levenberg-Marquardt local optimisation of (R, t) after each chunk
     of 256 samples that improves the best model, and a final Levenberg-Marquardt refinement.  The accuracy of PoseLib's
@@ -284,12 +291,14 @@ def estimate_absolute_pose_lo(kpts0: torch.Tensor, points3d1: torch.Tensor, matc
     within the threshold of it; ``best_hypothesis`` and ``best_solution`` the P3P solution the final model grew from)
     plus ``num_local_optimizations`` [B] int32, the local optimisations whose model was adopted, and ``cost`` [B]
     int64, the final model's integer MSAC score.  Failures are those of ``estimate_absolute_pose``, with
-    ``num_local_optimizations`` and ``cost`` 0."""
-    return _absolute_pose(True, kpts0, points3d1, matches0, K0, ransac_reproj_threshold, max_iters, confidence, seed)
+    ``num_local_optimizations`` and ``cost`` 0.  ``dist_coeffs0`` is ``estimate_absolute_pose``'s: the MSAC score
+    and the Levenberg-Marquardt steps then read the reprojection error in distorted pixels."""
+    return _absolute_pose(True, kpts0, points3d1, matches0, K0, ransac_reproj_threshold, max_iters, confidence, seed,
+                          dist_coeffs0)
 
 
 def _absolute_pose(lo: bool, kpts0, points3d1, matches0, K0, ransac_reproj_threshold, max_iters, confidence,
-                   seed) -> dict:
+                   seed, dist_coeffs0=None) -> dict:
     _check_inputs(kpts0, points3d1, matches0, "points3d1", 3)
     _check_params(ransac_reproj_threshold, max_iters, confidence, seed)
     if lo and kpts0.shape[1] > _cabi.GEO_LO_MAX_MATCHES:
@@ -297,6 +306,7 @@ def _absolute_pose(lo: bool, kpts0, points3d1, matches0, K0, ransac_reproj_thres
     device = kpts0.device
     b, m, n = kpts0.shape[0], kpts0.shape[1], points3d1.shape[1]
     k0 = _intrinsics("K0", K0, b, device)
+    d0 = None if dist_coeffs0 is None else dist_coeffs("dist_coeffs0", dist_coeffs0, b, device)
     p0 = kpts0.detach().to(torch.float32).contiguous()
     x1 = points3d1.detach().to(torch.float32).contiguous()
     m0 = matches0.detach().contiguous()
@@ -311,14 +321,16 @@ def _absolute_pose(lo: bool, kpts0, points3d1, matches0, K0, ransac_reproj_thres
         cfg = _cabi.GeoPnpConfig(_cabi.GEO_ABI_VERSION, max_iters, seed, 0, float(ransac_reproj_threshold),
                                  float(confidence))
         ins = _cabi.GeoPnpInputs(b, m, n, p0.data_ptr(), x1.data_ptr(), m0.data_ptr(), k0.data_ptr())
+        if d0 is not None:
+            ins = _cabi.GeoPnpDistInputs(ins, d0.shape[1], d0.data_ptr())
         outs = _cabi.GeoPnpOutputs(*(out[k].data_ptr() for k in list(shapes)[:8]))
         if lo:
             outs = _cabi.GeoLoPnpOutputs(outs, out["num_local_optimizations"].data_ptr(), out["cost"].data_ptr())
         return cfg, ins, outs
 
-    if lo:
-        return _run("geo_absolute_pose_lo", "geo_lo_pnp_workspace_bytes", shapes, device, b, m, max_iters, make_args)
-    return _run("geo_absolute_pose", "geo_pnp_workspace_bytes", shapes, device, b, m, max_iters, make_args)
+    entry = "geo_absolute_pose_lo" if lo else "geo_absolute_pose"
+    ws = "geo_lo_pnp_workspace_bytes" if lo else "geo_pnp_workspace_bytes"
+    return _run(entry if d0 is None else entry + "_dist", ws, shapes, device, b, m, max_iters, make_args)
 
 
 def _affine(kind: int, kpts0, kpts1, matches0, threshold, max_iters, confidence, refine_iters, seed) -> dict:
