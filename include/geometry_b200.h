@@ -476,6 +476,50 @@
  *      from gu and gv.  The refit's fixed inliers are those of AD2; LA7's inlier at a pose has Xc2 > 0 and
  *      ru*ru + rv*rv < (double)thr2.  The parametrisation, schedule and sums are A7's and LA7's.
  * AD4. Outputs, failures and diagnostics as A8 and LA8, with AD2's test in place of A5's.
+ *
+ * 3D rigid and similarity transforms (geo_estimate_rigid; oracle/rigid_oracle.py restates it bit for bit): x1 = scale
+ * R x0 + t between matched 3D points, with R a proper rotation and scale = 1 (GEO_RIGID_3D, SE(3)) or scale > 0
+ * (GEO_SIMILARITY_3D, Sim(3)).  kpts0 and kpts1 of GeoInputs hold [B, M, 3] and [B, N, 3] points.  Expressions
+ * evaluate left to right as written; every multiply and add rounds on its own.
+ *
+ * RG1. Compaction as step 1: match i is valid when 0 <= matches0[b, i] < N and all six coordinates of p =
+ *      kpts0[b, i] and q = kpts1[b, matches0[b, i]] (float) are finite.  There is no normalisation: the solver centres
+ *      its points.  The solver reads the floats widened to double.
+ * RG2. Sampling as step 3 with s = 3.
+ * RG3. Minimal solver, in double: Horn's closed-form quaternion method.  The sample is degenerate when either triangle
+ *      p0 p1 p2 or q0 q1 q2 is collinear or coincident: with d1 = x1 - x0, d2 = x2 - x0, c = d1 x d2 (a x b =
+ *      (a1*b2 - a2*b1, a2*b0 - a0*b2, a0*b1 - a1*b0)) and a.b = (a0*b0 + a1*b1) + a2*b2, unless
+ *      c.c > GEO_RIGID_COLLINEAR_EPS * (d1.d1 * d2.d2).  Centroids in sample order, pb = ((p0 + p1) + p2) / 3.0 and qb
+ *      likewise per coordinate; a_k = p_k - pb, b_k = q_k - qb; S_ij = sum_k a_k,i * b_k,j and saa = sum_k a_k.a_k,
+ *      each summed over k = 0, 1, 2 from 0.0.  Then the closed form, shared with RG6, from (pb, qb, S, saa):
+ *        N = [[(Sxx + Syy) + Szz, Syz - Szy, Szx - Sxz, Sxy - Syx],
+ *             [Syz - Szy, (Sxx - Syy) - Szz, Sxy + Syx, Szx + Sxz],
+ *             [Szx - Sxz, Sxy + Syx, (Syy - Sxx) - Szz, Syz + Szy],
+ *             [Sxy - Syx, Szx + Sxz, Syz + Szy, (Szz - Sxx) - Syy]]   (Sxy = S_01 and so on);
+ *      v = the least eigenvector of -N (each entry negated) by step 7's cyclic Jacobi on a 4x4, the eigenvector of N's
+ *      largest eigenvalue; nq = sqrt(((v0*v0 + v1*v1) + v2*v2) + v3*v3), (w, x, y, z) = v / nq; R = A7's rotation of
+ *      that quaternion ([1.0 - 2.0 * (y*y + z*z), 2.0 * (x*y - w*z), 2.0 * (x*z + w*y)], ...).  Similarity:
+ *      scale = num / saa with num = sum of R_ij * S_ji over i, then j, ascending from 0.0, which is
+ *      sum_k b_k.(R a_k) (Umeyama's least-squares scale); rigid: scale = 1.0.  t_i = qb_i - scale *
+ *      ((R_i0*pb0 + R_i1*pb1) + R_i2*pb2).  A scale that is not finite and positive, or a non-finite entry of R or t,
+ *      makes the sample degenerate.  A unit quaternion's R is a proper rotation, so no reflection can arise.
+ * RG4. Scoring in fp32 without fused multiply-adds: the model rounded to float as the 3x4 row-major [M | t] with
+ *      M_ij = scale * R_ij (g0..g11); e_i = (((g_4i*x + g_4i+1*y) + g_4i+2*z) + g_4i+3) - q_i for p = (x, y, z),
+ *      err = (e0*e0 + e1*e1) + e2*e2.  An inlier has err < (float)(threshold * threshold): the threshold is a distance
+ *      in the units of kpts1.  The score is the inlier count; ties go to the lowest hypothesis.
+ * RG5. Stopping as step 6 with s = 3.
+ * RG6. Refit.  With at least 3 inliers, RG3's closed form on the inliers of the best hypothesis (its RG4 inliers, k
+ *      of them), in two passes of step 2's fixed-order sums, other points adding 0: first pb_i = sum(p_i) / k and
+ *      qb_i = sum(q_i) / k; then S_ij = sum(a_i * b_j) and saa = sum(a.a) with a = p - pb, b = q - qb.  The refit is
+ *      scored as RG4 and replaces the hypothesis unless it has fewer inliers; a degenerate refit (RG3's rule) has none.
+ *      The closed form is the least-squares fit on those inliers, so no iterative refinement follows.
+ * RG7. Outputs: R [B, 3, 3], t [B, 3] and scale [B] of the final model (scale exactly 1.0 for GEO_RIGID_3D); inliers
+ *      the points with err < thr2 under it rounded to float, num_inliers their number; best_hypothesis the hypothesis
+ *      the final model grew from; num_hypotheses the samples drawn.  A pair fails (success 0, R, t and scale zero, no
+ *      inliers, best_hypothesis -1) when n < 3 or when every sample is degenerate.  Differences from the usual tools:
+ *      inliers are those of the final (refitted) model; stopping is checked per chunk of GEO_CHUNK; the sampler is
+ *      step 3's counter hash.  On a fixed inlier set the fit equals Umeyama's (and, for Sim(3),
+ *      cv2.estimateAffine3D(src, dst, force_rotation=True)).
  */
 #ifndef GEOMETRY_B200_H
 #define GEOMETRY_B200_H
@@ -710,6 +754,27 @@ LG_API int geo_absolute_pose_dist(const GeoPnpConfig* cfg, const GeoPnpDistInput
                                   void* workspace, size_t workspace_bytes, void* stream);
 LG_API int geo_absolute_pose_lo_dist(const GeoPnpConfig* cfg, const GeoPnpDistInputs* in, GeoLoPnpOutputs* out,
                                      void* workspace, size_t workspace_bytes, void* stream);
+
+#define GEO_RIGID_3D 5
+#define GEO_SIMILARITY_3D 6
+#define GEO_RIGID_COLLINEAR_EPS 1e-10
+
+typedef struct GeoRigidOutputs {
+  double* R;                /* [B, 3, 3] proper rotation: x1 = scale R x0 + t */
+  double* t;                /* [B, 3] */
+  double* scale;            /* [B]; exactly 1.0 for GEO_RIGID_3D */
+  uint8_t* inliers;         /* [B, M] */
+  int32_t* num_inliers;     /* [B] */
+  uint8_t* success;         /* [B] */
+  int32_t* best_hypothesis; /* [B], -1 without one */
+  int32_t* num_hypotheses;  /* [B] */
+} GeoRigidOutputs;
+
+/* 3D rigid and similarity transforms (steps RG1-RG7): cfg->model is GEO_RIGID_3D or GEO_SIMILARITY_3D and
+ * cfg->threshold a distance in the units of the points; in->kpts0 and in->kpts1 hold [B, M, 3] and [B, N, 3] points. */
+LG_API size_t geo_rigid_workspace_bytes(int32_t B, int32_t M, int32_t max_iters);
+LG_API int geo_estimate_rigid(const GeoConfig* cfg, const GeoInputs* in, GeoRigidOutputs* out, void* workspace,
+                              size_t workspace_bytes, void* stream);
 
 #define GEO_AFFINE 3
 #define GEO_AFFINE_PARTIAL 4

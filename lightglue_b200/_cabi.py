@@ -26,6 +26,7 @@ GEO_HOMOGRAPHY, GEO_FUNDAMENTAL, GEO_ESSENTIAL = 0, 1, 2
 GEO_LO_QSCALE, GEO_LO_MAX_MATCHES = 65536, (1 << 20) - 1
 GEO_AFFINE, GEO_AFFINE_PARTIAL, GEO_AFFINE_MAX_REFINE = 3, 4, 100
 GEO_CAMERA_FLOAT32, GEO_CAMERA_FLOAT64, GEO_UNDISTORT_MAX_ITERS = 0, 1, 1000
+GEO_RIGID_3D, GEO_SIMILARITY_3D = 5, 6
 NN_ABI_VERSION = 1  # include/nn_b200.h
 NN_MIN_DIM, NN_MAX_DIM, NN_GROUP_ROWS = 64, 512, 32768
 NN_GUIDE_H, NN_GUIDE_F = 0, 1
@@ -203,6 +204,14 @@ class GeoPnpDistInputs(C.Structure):
     _fields_ = [("pnp", GeoPnpInputs), ("num_dist", C.c_int32), ("dist0", C.c_void_p)]
 
 
+class GeoRigidOutputs(C.Structure):
+    _fields_ = [
+        ("R", C.c_void_p), ("t", C.c_void_p), ("scale", C.c_void_p), ("inliers", C.c_void_p),
+        ("num_inliers", C.c_void_p), ("success", C.c_void_p), ("best_hypothesis", C.c_void_p),
+        ("num_hypotheses", C.c_void_p),
+    ]
+
+
 class NnConfig(C.Structure):
     _fields_ = [
         ("abi_version", C.c_int32), ("dim", C.c_int32), ("mutual_check", C.c_int32), ("ratio_thresh", C.c_float),
@@ -327,6 +336,9 @@ GEO_PROTOTYPES = {  # include/geometry_b200.h
                                          C.POINTER(GeoPnpOutputs), _VP, _SZ, _VP]),
     "geo_absolute_pose_lo_dist": (C.c_int, [C.POINTER(GeoPnpConfig), C.POINTER(GeoPnpDistInputs),
                                             C.POINTER(GeoLoPnpOutputs), _VP, _SZ, _VP]),
+    "geo_rigid_workspace_bytes": (_SZ, [_I32, _I32, _I32]),
+    "geo_estimate_rigid": (C.c_int, [C.POINTER(GeoConfig), C.POINTER(GeoInputs), C.POINTER(GeoRigidOutputs), _VP,
+                                     _SZ, _VP]),
     "geo_affine_workspace_bytes": (_SZ, [_I32, _I32, _I32]),
     "geo_estimate_affine": (C.c_int, [C.POINTER(GeoAffineConfig), C.POINTER(GeoInputs), C.POINTER(GeoOutputs), _VP,
                                       _SZ, _VP]),

@@ -1,9 +1,10 @@
 """Geometric verification on the GPU: batched RANSAC homography and fundamental-matrix, relative-pose,
-absolute-pose and affine estimation on the matcher's output, each of the first four plain and LO-RANSAC (C ABI
-``include/geometry_b200.h``, CUDA ``csrc/geo_api.cu``, ``csrc/lo_hf_api.cu``, ``csrc/pose_api.cu``,
-``csrc/lo_pose_api.cu``, ``csrc/pnp_api.cu``, ``csrc/lo_pnp_api.cu`` and ``csrc/affine_api.cu``).
+absolute-pose, affine and 3D rigid and similarity estimation on the matcher's output, each of the first four plain and
+LO-RANSAC (C ABI ``include/geometry_b200.h``, CUDA ``csrc/geo_api.cu``, ``csrc/lo_hf_api.cu``, ``csrc/pose_api.cu``,
+``csrc/lo_pose_api.cu``, ``csrc/pnp_api.cu``, ``csrc/lo_pnp_api.cu``, ``csrc/affine_api.cu`` and
+``csrc/rigid_api.cu``).
 
-All ten functions take ``matches0`` [B, M] int64 exactly as ``LightGlue.forward``, ``PendingMatch.tensors`` and
+All twelve functions take ``matches0`` [B, M] int64 exactly as ``LightGlue.forward``, ``PendingMatch.tensors`` and
 ``match_ragged`` give it (-1 or any index outside [0, N) is unmatched), run every pair of the batch in one call on the
 current stream, and return device tensors of fixed shapes without synchronising with the host, so a call can follow a
 matcher forward with no read-back in between, or be captured in a CUDA graph.  A match whose keypoint in either image,
@@ -21,6 +22,8 @@ the sample size, 4 or 8, or no non-degenerate hypothesis) has ``success`` False,
 ``num_local_optimizations`` and ``cost``; so do ``estimate_relative_pose_lo`` and ``estimate_absolute_pose_lo`` with
 those of ``estimate_relative_pose`` and ``estimate_absolute_pose``.  ``estimate_affine_2d`` and
 ``estimate_affine_partial_2d`` return those of ``find_homography`` with ``A`` [B, 2, 3] in place of ``H``.
+``estimate_rigid_3d`` and ``estimate_similarity_3d`` register matched 3D points (``cv2.estimateAffine3D`` with
+``force_rotation=True`` fits the same model without RANSAC) and return ``R``, ``t`` and ``scale`` in place of ``H``.
 """
 from __future__ import annotations
 
@@ -32,35 +35,36 @@ from . import _cabi
 from .camera import dist_coeffs
 
 
-def _check_params(threshold, max_iters, confidence, seed) -> None:
+def _check_params(threshold, max_iters, confidence, seed, name="ransac_reproj_threshold",
+                  what="a positive number of pixels") -> None:
     if not isinstance(max_iters, int) or isinstance(max_iters, bool) or not 1 <= max_iters <= 1 << 24:
         raise ValueError(f"max_iters={max_iters!r}: an int in [1, 2**24]")
     if not float(threshold) > 0.0 or float(threshold) == float("inf"):
-        raise ValueError(f"ransac_reproj_threshold={threshold!r}: a positive number of pixels")
+        raise ValueError(f"{name}={threshold!r}: {what}")
     if not 0.0 <= float(confidence) <= 1.0:
         raise ValueError(f"confidence={confidence!r}: in [0, 1]")
     if not isinstance(seed, int) or isinstance(seed, bool) or not 0 <= seed < 1 << 32:
         raise ValueError(f"seed={seed!r}: an int in [0, 2**32)")
 
 
-def _check_inputs(kpts0, kpts1, matches0, name1="kpts1", dim1=2) -> None:
-    for name, t in (("kpts0", kpts0), (name1, kpts1), ("matches0", matches0)):
+def _check_inputs(kpts0, kpts1, matches0, name1="kpts1", dim1=2, name0="kpts0", dim0=2) -> None:
+    for name, t in ((name0, kpts0), (name1, kpts1), ("matches0", matches0)):
         if not isinstance(t, torch.Tensor):
             raise ValueError(f"{name} must be a torch.Tensor")
         if t.device.type != "cuda":
             raise RuntimeError("lightglue_b200.geometry runs on CUDA (sm_90a) tensors only; there is no CPU path")
-    if kpts0.dim() != 3 or kpts0.shape[-1] != 2 or kpts1.dim() != 3 or kpts1.shape[-1] != dim1:
-        raise ValueError(f"kpts0 {tuple(kpts0.shape)} and {name1} {tuple(kpts1.shape)}: expected [B, M, 2] and "
+    if kpts0.dim() != 3 or kpts0.shape[-1] != dim0 or kpts1.dim() != 3 or kpts1.shape[-1] != dim1:
+        raise ValueError(f"{name0} {tuple(kpts0.shape)} and {name1} {tuple(kpts1.shape)}: expected [B, M, {dim0}] and "
                          f"[B, N, {dim1}]")
     if matches0.dim() != 2 or matches0.shape != kpts0.shape[:2] or kpts1.shape[0] != kpts0.shape[0]:
-        raise ValueError(f"matches0 {tuple(matches0.shape)}: expected [B, M] of kpts0 {tuple(kpts0.shape)} with the "
+        raise ValueError(f"matches0 {tuple(matches0.shape)}: expected [B, M] of {name0} {tuple(kpts0.shape)} with the "
                          f"batch of {name1} {tuple(kpts1.shape)}")
     if not kpts0.is_floating_point() or not kpts1.is_floating_point():
-        raise ValueError(f"kpts0 and {name1} must be floating point" + (" pixels" if dim1 == 2 else ""))
+        raise ValueError(f"{name0} and {name1} must be floating point" + (" pixels" if dim1 == 2 else ""))
     if matches0.dtype != torch.int64:
         raise ValueError(f"matches0 must be int64, not {matches0.dtype}")
     if kpts1.device != kpts0.device or matches0.device != kpts0.device:
-        raise ValueError(f"kpts0, {name1} and matches0 must be on one device")
+        raise ValueError(f"{name0}, {name1} and matches0 must be on one device")
 
 
 def _run(entry: str, ws_entry: str, shapes: dict, device, b: int, m: int, max_iters: int, make_args) -> dict:
@@ -388,3 +392,52 @@ def estimate_affine_partial_2d(kpts0: torch.Tensor, kpts1: torch.Tensor, matches
     only degenerate samples (coincident points in either image) fails as in ``estimate_affine_2d``."""
     return _affine(_cabi.GEO_AFFINE_PARTIAL, kpts0, kpts1, matches0, ransac_reproj_threshold, max_iters, confidence,
                    refine_iters, seed)
+
+
+def _rigid(kind: int, points0, points1, matches0, threshold, max_iters, confidence, seed) -> dict:
+    _check_inputs(points0, points1, matches0, "points1", 3, "points0", 3)
+    _check_params(threshold, max_iters, confidence, seed, "ransac_threshold", "a positive distance in points1's units")
+    device = points0.device
+    b, m, n = points0.shape[0], points0.shape[1], points1.shape[1]
+    p0 = points0.detach().to(torch.float32).contiguous()
+    p1 = points1.detach().to(torch.float32).contiguous()
+    m0 = matches0.detach().contiguous()
+    f64, i32, bl = torch.float64, torch.int32, torch.bool
+    shapes = {"R": ((b, 3, 3), f64), "t": ((b, 3), f64), "scale": ((b,), f64), "inliers": ((b, m), bl),
+              "num_inliers": ((b,), i32), "success": ((b,), bl), "best_hypothesis": ((b,), i32),
+              "num_hypotheses": ((b,), i32)}
+
+    def make_args(out):
+        cfg = _cabi.GeoConfig(_cabi.GEO_ABI_VERSION, kind, max_iters, seed, float(threshold), float(confidence))
+        ins = _cabi.GeoInputs(b, m, n, p0.data_ptr(), p1.data_ptr(), m0.data_ptr())
+        return cfg, ins, _cabi.GeoRigidOutputs(*(out[k].data_ptr() for k in shapes))
+
+    return _run("geo_estimate_rigid", "geo_rigid_workspace_bytes", shapes, device, b, m, max_iters, make_args)
+
+
+def estimate_rigid_3d(points0: torch.Tensor, points1: torch.Tensor, matches0: torch.Tensor, ransac_threshold: float,
+                      max_iters: int = 1000, confidence: float = 0.99, seed: int = 0) -> dict:
+    """RANSAC rigid transform (SE(3)) per pair between matched 3D points: x1 = R x0 + t from 3-point samples by Horn's
+    closed-form quaternion method, then the same closed form (the least-squares Kabsch fit) on the best sample's
+    inliers.  ``points0`` [B, M, 3] and ``points1`` [B, N, 3] are floating point, read as float32; a point with a
+    non-finite coordinate (NaN for a missing depth) makes its matches invalid.  An inlier's squared distance
+    |R x0 + t - x1|^2 is below ``ransac_threshold ** 2``, in the units of ``points1``; there is no default, since no
+    single value fits both metres and millimetres.  ``max_iters`` and ``confidence`` default to those of
+    ``cv2.estimateAffine3D``.
+
+    Returns ``R`` [B, 3, 3] float64, a proper rotation; ``t`` [B, 3] float64; ``scale`` [B] float64, exactly 1.0 on
+    success; ``inliers`` [B, M] bool and ``num_inliers`` [B] int32 of the final transform; ``success`` [B] bool; and
+    the diagnostics ``best_hypothesis`` [B] int32 (-1 without one) and ``num_hypotheses`` [B] int32.  A pair with
+    fewer than 3 valid matches or only degenerate (collinear or coincident) samples has ``success`` False, zero R, t
+    and scale, and no inliers."""
+    return _rigid(_cabi.GEO_RIGID_3D, points0, points1, matches0, ransac_threshold, max_iters, confidence, seed)
+
+
+def estimate_similarity_3d(points0: torch.Tensor, points1: torch.Tensor, matches0: torch.Tensor,
+                           ransac_threshold: float, max_iters: int = 1000, confidence: float = 0.99,
+                           seed: int = 0) -> dict:
+    """RANSAC similarity transform (Sim(3)) per pair between matched 3D points: x1 = scale R x0 + t, with Umeyama's
+    least-squares scale, for maps or reconstructions that each have their own scale.  Arguments, outputs and failures
+    are those of ``estimate_rigid_3d``, with ``scale`` > 0 free; ``ransac_threshold`` is measured in the frame of
+    ``points1``.  On a fixed inlier set the fit equals ``cv2.estimateAffine3D(src, dst, force_rotation=True)``."""
+    return _rigid(_cabi.GEO_SIMILARITY_3D, points0, points1, matches0, ransac_threshold, max_iters, confidence, seed)
