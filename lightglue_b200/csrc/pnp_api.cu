@@ -2,19 +2,19 @@
 // inliers (include/geometry_b200.h, steps A1-A8).
 //
 // Launches, all fixed by (B, M, max_iters):
-//   prepare  pnp_prepare_kernel, one 1024-thread CTA per pair: ordered compaction of the valid matches, calibrated
-//            coordinates, K check
+//   prepare  pnp_prepare_kernel<Cam>, one 1024-thread CTA per pair: ordered compaction of the valid matches,
+//            calibrated coordinates, camera check
 //   per chunk of GEO_CHUNK samples:
 //     hyp    geo_hyp_kernel, one CTA per pair: folds the previous chunk's counts into the pair's best (geo_fold),
-//            decides the adaptive stop, then one thread per sample solves it: up to 4 fp32 projections
-//     score  geo_score_kernel<PnpScore>, (B, splits) CTAs: each streams a slice of the pair's points through shared
-//            memory against every solution of the chunk, one thread per sample, and adds the inlier counts
-//   final    geo_final_kernel<PnpRansac>, one CTA per pair: folds the last chunk, Levenberg-Marquardt from the best
-//            solution (lo_common.cuh's loop), recount, R and t
-//   mask     pnp_mask_kernel, one thread per row of matches0: the final inlier mask
-// A stopped pair's CTAs return at once.  With lens distortion (geo_absolute_pose_dist, steps AD1-AD4) the same launches
-// run pnp_dist_prepare_kernel (D2's calibrated coordinates), PnpDistScore and PnpDistRansac (the float model is [R | t]
-// and the test is in distorted pixels) and pnp_dist_mask_kernel.  Compiled with -fmad=false, like geo_api.cu:
+//            decides the adaptive stop, then one thread per sample solves it: up to 4 fp32 models
+//     score  geo_score_kernel<PnpScore<Cam>>, (B, splits) CTAs: each streams a slice of the pair's points through
+//            shared memory against every solution of the chunk, one thread per sample, and adds the inlier counts
+//   final    geo_final_kernel<PnpRansac<Cam>>, one CTA per pair: folds the last chunk, Levenberg-Marquardt from the
+//            best solution (lo_common.cuh's loop), recount, R and t
+//   mask     pnp_mask_kernel<Cam>, one thread per row of matches0: the final inlier mask
+// A stopped pair's CTAs return at once.  Cam is pnp_common.cuh's camera policy: Pinhole for geo_absolute_pose (the
+// float model is K0 [R | t]), Distorted for geo_absolute_pose_dist (steps AD1-AD4: D2's calibrated coordinates, the
+// float model [R | t] and the test in distorted pixels).  Compiled with -fmad=false, like geo_api.cu:
 // oracle/pnp_oracle.py takes the same steps in numpy.
 #include <stdint.h>
 
@@ -25,7 +25,8 @@ namespace {
 
 constexpr int MASK_THREADS = 256;
 
-// Inlier counts of every projection, on a tile of pixels and world points
+// Inlier counts of every model, on a tile of pixels and world points
+template <class Cam>
 struct PnpScore {
   using Args = PnpArgs;
   using Acc = int;
@@ -34,34 +35,38 @@ struct PnpScore {
   const float4* src[K];
   int* sums;
   float thr2;
+  typename Cam::Test cam;
   __device__ PnpScore(const PnpArgs& a, const PnpPair& P, int b)
-      : src{a.w.pts + (long)b * a.M, a.w.wld + (long)b * a.M}, sums(a.w.count), thr2(P.thr2) {}
-  __device__ int term(const float* g, const float4* p) const { return reproj_inlier(g, p[0], p[1], thr2); }
+      : src{a.w.pts + (long)b * a.M, a.w.wld + (long)b * a.M}, sums(a.w.count), thr2(P.thr2), cam(Cam::test(a, b)) {}
+  __device__ int term(const float* g, const float4* p) const { return Cam::inlier(cam, g, p[0], p[1], thr2); }
 };
 
-// The points of the refinement and its fixed inlier set: those of the float projection fm (header step A7)
+// The points of the refinement and its fixed inlier set: those of the float model fm (header step A7)
+template <class Cam>
 struct PnpFixed {
   const float4* pix;
   const float4* wld;
   const float* fm;
+  typename Cam::Test cam;
 };
 
 // (R, t) for lo_common.cuh's LM loop on A7's fixed inliers: x = R (0-8, row-major) and t (9-11); the pair's constants
-// are its K0
+// are Cam's
+template <class Cam>
 struct PnpLm {
   static constexpr int DOF = 6, TERMS = 28, GROUP = 14, NP = 12, NF = 12;
   struct Scratch {};
 
-  static __device__ void terms(LoShared<PnpLm>& s, const double* K, const double* x, PnpFixed pts, int n, double thr2,
-                               double* out, int tid) {
+  static __device__ void terms(LoShared<PnpLm>& s, const typename Cam::Consts& c, const double* x,
+                               const PnpFixed<Cam>& pts, int n, double thr2, double* out, int tid) {
     double acc[TERMS];
 #pragma unroll
     for (int i = 0; i < TERMS; ++i) acc[i] = 0.0;
     for (int k = tid; k < n; k += RED) {
       const float4 p = pts.pix[k], q = pts.wld[k];
-      if (!reproj_inlier(pts.fm, p, q, (float)thr2)) continue;
-      const PnpResidual e = pnp_residual(K, x, x + 9, p, q);
-      pnp_add_normal(K, e, acc);
+      if (!Cam::inlier(pts.cam, pts.fm, p, q, (float)thr2)) continue;
+      const auto e = Cam::residual(c, x, p, q);
+      Cam::add_normal(c, e, acc);
       acc[TERMS - 1] = acc[TERMS - 1] + (e.ru * e.ru + e.rv * e.rv);
     }
     lo_tree_sums<TERMS, GROUP>(acc, s.red, out, tid);
@@ -74,14 +79,15 @@ struct PnpLm {
 
 // The absolute pose for geo_final_kernel: GEO_PNP_LM_STEPS Levenberg-Marquardt steps on the best solution's inliers
 // (header step A7)
-struct PnpRansac : PnpSolver {
+template <class Cam>
+struct PnpRansac : PnpSolver<Cam> {
   using Base = PnpArgs;
-  using Score = PnpScore;
-  using Scratch = LoShared<PnpLm>;
+  using Score = PnpScore<Cam>;
+  using Scratch = LoShared<PnpLm<Cam>>;
 
   static __device__ bool inlier(const PnpArgs& a, int b, const float* g, int k) {
     const long i = (long)b * a.M + k;
-    return reproj_inlier(g, a.w.pts[i], a.w.wld[i], a.w.pair[b].thr2);
+    return Cam::inlier(Cam::test(a, b), g, a.w.pts[i], a.w.wld[i], a.w.pair[b].thr2);
   }
   static __device__ void clear(const PnpArgs&, int, int) {}  // pnp_mask_kernel writes every row
   static __device__ void fail(const PnpArgs& a, int b, int t) {
@@ -94,14 +100,14 @@ struct PnpRansac : PnpSolver {
     if (t == 0)
       for (int i = 0; i < 12; ++i) s.m.x[i] = s.x[0][i];
     __syncthreads();
-    const PnpFixed pts{a.w.pts + (long)b * a.M, a.w.wld + (long)b * a.M, s.fm[0]};
+    const PnpFixed<Cam> pts{a.w.pts + (long)b * a.M, a.w.wld + (long)b * a.M, s.fm[0], Cam::test(a, b)};
     const float thr2 = a.w.pair[b].thr2;
-    lo_refine(s.m, a.K0 + (long)b * 9, pts, a.w.pair[b].n, (double)thr2, GEO_PNP_LM_STEPS, GEO_PNP_LM_LAMBDA0, t);
+    lo_refine(s.m, Cam::consts(a, b), pts, a.w.pair[b].n, (double)thr2, GEO_PNP_LM_STEPS, GEO_PNP_LM_LAMBDA0, t);
     if (t == 0)
       for (int i = 0; i < 12; ++i) s.x[1][i] = s.m.x[i];
   }
 
-  // R, t, and the projection for pnp_mask_kernel
+  // R, t, and the float model for pnp_mask_kernel
   static __device__ void write(GeoFinal<PnpRansac>& s, const PnpArgs& a, int b, int u, int t) {
     PnpPair& P = a.w.pair[b];
     if (t < 12) P.P[t] = s.fm[u][t];
@@ -111,113 +117,44 @@ struct PnpRansac : PnpSolver {
   }
 };
 
+template <class Cam>
 __global__ void __launch_bounds__(MASK_THREADS) pnp_mask_kernel(PnpArgs a) {
   const int b = blockIdx.x, i = blockIdx.y * MASK_THREADS + threadIdx.x;
   if (i >= a.M) return;
   const PnpPair& P = a.w.pair[b];
   const int k = a.w.slot[(long)b * a.M + i];
   bool in = false;
-  if (P.success && k >= 0) in = reproj_inlier(P.P, a.w.pts[(long)b * a.M + k], a.w.wld[(long)b * a.M + k], P.thr2);
+  if (P.success && k >= 0)
+    in = Cam::inlier(Cam::test(a, b), P.P, a.w.pts[(long)b * a.M + k], a.w.wld[(long)b * a.M + k], P.thr2);
   a.out.inliers[(long)b * a.M + i] = in;
 }
 
-// ---- with lens distortion (header steps AD1-AD4) ----
-
-// AD2's inlier counts of every [R | t], on a tile of pixels and world points
-struct PnpDistScore {
-  using Args = PnpDistArgs;
-  using Acc = int;
-  static constexpr int SOLS = ::SOLS, NF = 12, K = 2, TILE = ::TILE;
-  static __device__ const PnpWs& ws(const PnpDistArgs& a) { return a.w; }
-  const float4* src[K];
-  int* sums;
-  float thr2;
-  Camera<float> cam;
-  __device__ PnpDistScore(const PnpDistArgs& a, const PnpPair& P, int b)
-      : src{a.w.pts + (long)b * a.M, a.w.wld + (long)b * a.M}, sums(a.w.count), thr2(P.thr2),
-        cam(pair_camera<float>(a, b)) {}
-  __device__ int term(const float* g, const float4* p) const { return dist_reproj_err(g, cam, p[0], p[1]) < thr2; }
-};
-
-// The refinement's points and its fixed inlier set: those of the float [R | t] fm under AD2
-struct PnpDistFixed {
-  const float4* pix;
-  const float4* wld;
-  const float* fm;
-  Camera<float> cam;
-};
-
-// PnpLm with AD3's residuals; the pair's constants are its camera in double
-struct PnpDistLm {
-  static constexpr int DOF = 6, TERMS = 28, GROUP = 14, NP = 12, NF = 12;
-  struct Scratch {};
-
-  static __device__ void terms(LoShared<PnpDistLm>& s, const Camera<double>& c, const double* x,
-                               const PnpDistFixed& pts, int n, double thr2, double* out, int tid) {
-    double acc[TERMS];
-#pragma unroll
-    for (int i = 0; i < TERMS; ++i) acc[i] = 0.0;
-    for (int k = tid; k < n; k += RED) {
-      const float4 p = pts.pix[k], q = pts.wld[k];
-      if (!(dist_reproj_err(pts.fm, pts.cam, p, q) < (float)thr2)) continue;
-      const PnpDistResidual e = pnp_dist_residual(c, x, x + 9, p, q);
-      pnp_dist_add_normal(c, e, acc);
-      acc[TERMS - 1] = acc[TERMS - 1] + (e.ru * e.ru + e.rv * e.rv);
-    }
-    lo_tree_sums<TERMS, GROUP>(acc, s.red, out, tid);
+// geo_absolute_pose and geo_absolute_pose_dist: the checks, then the launches
+template <class Cam>
+int absolute_pose(const char* entry, const GeoPnpConfig* cfg, const GeoPnpInputs* in, const double* dist0,
+                  int num_dist, GeoPnpOutputs* out, void* workspace, size_t workspace_bytes, void* stream_) {
+  int rc = geo_check_config(entry, cfg, in, out, INT_MAX, geo_no_check,
+                            [&] { return Cam::COEFFS ? dist_count_check(num_dist) : nullptr; });
+  if (rc == GEO_RUN) {
+    const auto buffers = [&](std::initializer_list<const void*> intrinsics) {
+      return geo_check_buffers(entry, in, {out->R, out->t, out->num_inliers, out->success, out->best_hypothesis,
+                                           out->best_solution, out->num_hypotheses}, {out->inliers}, intrinsics,
+                               in->points3d1, workspace, workspace_bytes,
+                               geo_pnp_workspace_bytes(in->B, in->M, cfg->max_iters));
+    };
+    rc = Cam::COEFFS ? buffers({in->K0, dist0}) : buffers({in->K0});
   }
-
-  static __device__ void update(LoShared<PnpDistLm>&, const double* x, const double* d, double* out) {
-    lm_update(x, x + 9, d, out, out + 9);
+  if (rc != GEO_RUN) return rc;
+  PnpArgs a = pnp_args(cfg, in, dist0, num_dist);
+  carve(geo_workspace_base(workspace), in->B, in->M, &a.w);
+  a.out = *out;
+  const cudaStream_t stream = (cudaStream_t)stream_;
+  if (int rc = geo_launch<PnpRansac<Cam>>(a, pnp_prepare_kernel<Cam>, stream)) return rc;
+  if (a.M > 0) {
+    pnp_mask_kernel<Cam><<<dim3(a.B, (a.M + MASK_THREADS - 1) / MASK_THREADS), MASK_THREADS, 0, stream>>>(a);
+    LG_CHECK_LAUNCH();
   }
-};
-
-// PnpRansac with AD2's test and AD3's refit; the float model is [R | t]
-struct PnpDistRansac : PnpDistSolver {
-  using Base = PnpDistArgs;
-  using Score = PnpDistScore;
-  using Scratch = LoShared<PnpDistLm>;
-
-  static __device__ bool inlier(const PnpDistArgs& a, int b, const float* g, int k) {
-    const long i = (long)b * a.M + k;
-    return dist_reproj_err(g, pair_camera<float>(a, b), a.w.pts[i], a.w.wld[i]) < a.w.pair[b].thr2;
-  }
-  static __device__ void clear(const PnpDistArgs&, int, int) {}  // pnp_dist_mask_kernel writes every row
-  static __device__ void fail(const PnpDistArgs& a, int b, int t) { PnpRansac::fail(a, b, t); }
-  static __device__ bool refits(const PnpDistArgs&, int hcount) { return hcount >= GEO_PNP_REFIT_MIN; }
-
-  static __device__ void refit(GeoFinal<PnpDistRansac>& s, const PnpDistArgs& a, int b, int t) {
-    if (t == 0)
-      for (int i = 0; i < 12; ++i) s.m.x[i] = s.x[0][i];
-    __syncthreads();
-    const PnpDistFixed pts{a.w.pts + (long)b * a.M, a.w.wld + (long)b * a.M, s.fm[0], pair_camera<float>(a, b)};
-    const float thr2 = a.w.pair[b].thr2;
-    lo_refine(s.m, pair_camera<double>(a, b), pts, a.w.pair[b].n, (double)thr2, GEO_PNP_LM_STEPS, GEO_PNP_LM_LAMBDA0,
-              t);
-    if (t == 0)
-      for (int i = 0; i < 12; ++i) s.x[1][i] = s.m.x[i];
-  }
-
-  // R, t, and [R | t] for pnp_dist_mask_kernel
-  static __device__ void write(GeoFinal<PnpDistRansac>& s, const PnpDistArgs& a, int b, int u, int t) {
-    PnpPair& P = a.w.pair[b];
-    if (t < 12) P.P[t] = s.fm[u][t];
-    if (t < 9) a.out.R[(long)b * 9 + t] = s.x[u][t];
-    if (t < 3) a.out.t[(long)b * 3 + t] = s.x[u][9 + t];
-    if (t == 0) P.success = 1;
-  }
-};
-
-__global__ void __launch_bounds__(MASK_THREADS) pnp_dist_mask_kernel(PnpDistArgs a) {
-  const int b = blockIdx.x, i = blockIdx.y * MASK_THREADS + threadIdx.x;
-  if (i >= a.M) return;
-  const PnpPair& P = a.w.pair[b];
-  const int k = a.w.slot[(long)b * a.M + i];
-  bool in = false;
-  if (P.success && k >= 0)
-    in = dist_reproj_err(P.P, pair_camera<float>(a, b), a.w.pts[(long)b * a.M + k], a.w.wld[(long)b * a.M + k]) <
-         P.thr2;
-  a.out.inliers[(long)b * a.M + i] = in;
+  return 0;
 }
 
 }  // namespace
@@ -229,47 +166,13 @@ extern "C" size_t geo_pnp_workspace_bytes(int32_t B, int32_t M, int32_t) {
 }
 
 extern "C" int geo_absolute_pose(const GeoPnpConfig* cfg, const GeoPnpInputs* in, GeoPnpOutputs* out, void* workspace,
-                                 size_t workspace_bytes, void* stream_) {
-  const char* entry = "geo_absolute_pose";
-  int rc = geo_check_config(entry, cfg, in, out, INT_MAX, geo_no_check, geo_no_check);
-  if (rc == GEO_RUN)
-    rc = geo_check_buffers(entry, in, {out->R, out->t, out->num_inliers, out->success, out->best_hypothesis,
-                                       out->best_solution, out->num_hypotheses}, {out->inliers}, {in->K0},
-                           in->points3d1, workspace, workspace_bytes,
-                           geo_pnp_workspace_bytes(in->B, in->M, cfg->max_iters));
-  if (rc != GEO_RUN) return rc;
-  PnpArgs a = pnp_args(cfg, in);
-  carve(geo_workspace_base(workspace), in->B, in->M, &a.w);
-  a.out = *out;
-  const cudaStream_t stream = (cudaStream_t)stream_;
-  if (int rc = geo_launch<PnpRansac>(a, pnp_prepare_kernel, stream)) return rc;
-  if (a.M > 0) {
-    pnp_mask_kernel<<<dim3(a.B, (a.M + MASK_THREADS - 1) / MASK_THREADS), MASK_THREADS, 0, stream>>>(a);
-    LG_CHECK_LAUNCH();
-  }
-  return 0;
+                                 size_t workspace_bytes, void* stream) {
+  return absolute_pose<Pinhole>("geo_absolute_pose", cfg, in, nullptr, 0, out, workspace, workspace_bytes, stream);
 }
 
 extern "C" int geo_absolute_pose_dist(const GeoPnpConfig* cfg, const GeoPnpDistInputs* din, GeoPnpOutputs* out,
-                                      void* workspace, size_t workspace_bytes, void* stream_) {
-  const char* entry = "geo_absolute_pose_dist";
-  const GeoPnpInputs* in = din ? &din->pnp : nullptr;
-  int rc = geo_check_config(entry, cfg, in, out, INT_MAX, geo_no_check,
-                            [&] { return dist_count_check(din->num_dist); });
-  if (rc == GEO_RUN)
-    rc = geo_check_buffers(entry, in, {out->R, out->t, out->num_inliers, out->success, out->best_hypothesis,
-                                       out->best_solution, out->num_hypotheses}, {out->inliers}, {in->K0, din->dist0},
-                           in->points3d1, workspace, workspace_bytes,
-                           geo_pnp_workspace_bytes(in->B, in->M, cfg->max_iters));
-  if (rc != GEO_RUN) return rc;
-  PnpDistArgs a{pnp_args(cfg, in), din->dist0, din->num_dist};
-  carve(geo_workspace_base(workspace), in->B, in->M, &a.w);
-  a.out = *out;
-  const cudaStream_t stream = (cudaStream_t)stream_;
-  if (int rc = geo_launch<PnpDistRansac>(a, pnp_dist_prepare_kernel, stream)) return rc;
-  if (a.M > 0) {
-    pnp_dist_mask_kernel<<<dim3(a.B, (a.M + MASK_THREADS - 1) / MASK_THREADS), MASK_THREADS, 0, stream>>>(a);
-    LG_CHECK_LAUNCH();
-  }
-  return 0;
+                                      void* workspace, size_t workspace_bytes, void* stream) {
+  // a null din goes on as a null in, which geo_check_config reports
+  return absolute_pose<Distorted>("geo_absolute_pose_dist", cfg, din ? &din->pnp : nullptr, din ? din->dist0 : nullptr,
+                                  din ? din->num_dist : 0, out, workspace, workspace_bytes, stream);
 }

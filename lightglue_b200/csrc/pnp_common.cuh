@@ -1,7 +1,8 @@
 // The absolute-pose pieces shared by the plain (pnp_api.cu, header steps A1-A8) and the LO-RANSAC estimator
-// (lo_pnp_api.cu, LA1-LA8), both compiled with -fmad=false: the workspace, the compaction kernel, the Lambda Twist
-// solver, the projection, the fp32 reprojection test and the pose update of the Levenberg-Marquardt steps; and their
-// counterparts with lens distortion (AD1-AD4).
+// (lo_pnp_api.cu, LA1-LA8), both compiled with -fmad=false: the workspace, the Lambda Twist solver, the projection,
+// the fp32 reprojection test, the residuals and pose update of the Levenberg-Marquardt steps, and their counterparts
+// with lens distortion (AD1-AD4); then the two camera policies, Pinhole and Distorted, that route to one or the other,
+// and the solver and compaction kernel templated on them.
 #pragma once
 #include <stdint.h>
 
@@ -61,6 +62,8 @@ struct PnpArgs {
   const double* K0;
   PnpWs w;
   GeoPnpOutputs out;
+  const double* dist0;  // [B, nd]: the coefficients, read by the Distorted camera only
+  int nd;
 };
 
 __device__ __forceinline__ double dot3(const double* a, const double* b) { return a[0] * b[0] + a[1] * b[1] + a[2] * b[2]; }
@@ -259,20 +262,6 @@ __device__ __forceinline__ float reproj_err(const float* g, float4 p, float4 q) 
   return w > 0.f ? du * du + dv * dv : INFINITY;
 }
 
-// geo_hyp_kernel's solver of the absolute pose: sample h's P3P solutions (R, t), scored as K0 [R | t]
-struct PnpSolver {
-  static constexpr int SOLS = ::SOLS, NX = 12, NF = 12;
-  static __device__ int s(const PnpArgs&) { return S; }
-  static __device__ int solve(const PnpArgs& a, int b, unsigned h, double (*x)[NX]) {
-    int id[S];
-    if (geo_sample(a.seed, h, a.w.pair[b].n, S, id) < S) return 0;
-    return p3p(a.w.pts + (long)b * a.M, a.w.wld + (long)b * a.M, id, x);
-  }
-  static __device__ void pixels(const PnpArgs& a, int b, const double* x, double* px) {
-    projection(a.K0 + (long)b * 9, x, x + 9, px);
-  }
-};
-
 // The reprojection residual (ru, rv) of world point q at pixel p (u, v) under K [R | t], and what its Jacobian needs
 struct PnpResidual {
   double Xc[3];  // the camera-frame point; Xc[2] is its depth
@@ -319,51 +308,6 @@ __device__ __forceinline__ void pnp_add_normal(const double* K, const PnpResidua
   pnp_add_rows(e.Xc, gu, gv, e.ru, e.rv, acc);
 }
 
-__global__ void __launch_bounds__(1024) pnp_prepare_kernel(PnpArgs a) {
-  const int b = blockIdx.x, tid = threadIdx.x;
-  __shared__ int warp_sums[32];
-  __shared__ int carry;
-  if (tid == 0) carry = 0;
-  __syncthreads();
-  const double* K = a.K0 + (long)b * 9;
-  const int64_t* m0 = a.matches0 + (long)b * a.M;
-  float4* pts = a.w.pts + (long)b * a.M;
-  float4* wld = a.w.wld + (long)b * a.M;
-  int* slot = a.w.slot + (long)b * a.M;
-  for (int base = 0; base < a.M; base += 1024) {
-    const int i = base + tid;
-    const int64_t j = i < a.M ? m0[i] : -1;
-    float X = 0.f, Y = 0.f, Z = 0.f;
-    float2 p = make_float2(0.f, 0.f);
-    if (j >= 0 && j < a.N) {
-      const float* q = a.points3d1 + ((long)b * a.N + j) * 3;
-      X = q[0];
-      Y = q[1];
-      Z = q[2];
-      p = reinterpret_cast<const float2*>(a.kpts0)[(long)b * a.M + i];
-    }
-    const bool valid = j >= 0 && j < a.N && isfinite(X) && isfinite(Y) && isfinite(Z) && finite2(p);
-    const int k = block_scan_step(valid, tid, warp_sums, &carry);
-    if (i < a.M) slot[i] = valid ? k : -1;
-    if (valid) {
-      const double yy = ((double)p.y - K[5]) / K[4], xx = (((double)p.x - K[2]) - K[1] * yy) / K[0];
-      pts[k] = make_float4(p.x, p.y, (float)xx, (float)yy);
-      wld[k] = make_float4(X, Y, Z, 0.f);
-    }
-  }
-  __syncthreads();
-  if (tid == 0) {
-    PnpPair& P = a.w.pair[b];
-    P.thr2 = (float)(a.threshold * a.threshold);
-    P.best = 0;
-    P.n = carry;
-    P.ok = carry >= S && k_valid(K);
-    P.stop = !P.ok;
-    P.drawn = 0;
-    P.success = 0;
-  }
-}
-
 // R' = Q R, t' = Q t + d[3..5], Q of the unit quaternion (1, d[0..2] / 2) / norm
 __device__ void lm_update(const double* R, const double* t, const double* d, double* Rn, double* tn) {
   double Q[9];
@@ -374,8 +318,9 @@ __device__ void lm_update(const double* R, const double* t, const double* d, dou
   }
 }
 
-// The kernel arguments of an entry point's configuration and inputs; the caller carves the workspace and sets out
-inline PnpArgs pnp_args(const GeoPnpConfig* cfg, const GeoPnpInputs* in) {
+// The kernel arguments of an entry point's configuration, inputs and coefficients (none for the pinhole camera); the
+// caller carves the workspace and sets out
+inline PnpArgs pnp_args(const GeoPnpConfig* cfg, const GeoPnpInputs* in, const double* dist0, int nd) {
   PnpArgs a{};
   a.B = in->B; a.M = in->M; a.N = in->N;
   a.max_iters = cfg->max_iters;
@@ -385,73 +330,21 @@ inline PnpArgs pnp_args(const GeoPnpConfig* cfg, const GeoPnpInputs* in) {
   a.confidence = cfg->confidence;
   a.kpts0 = in->kpts0; a.points3d1 = in->points3d1; a.matches0 = in->matches0;
   a.K0 = in->K0;
+  a.dist0 = dist0;
+  a.nd = nd;
   return a;
 }
 
-// ---- the distortion-aware absolute pose (header steps AD1-AD4) ----
+// ---- the lens distortion primitives (header steps AD1-AD4) ----
 
 constexpr int PNP_UNDISTORT_ITERS = 5;  // AD1: cv2.solvePnP's undistortion
 
-struct PnpDistArgs : PnpArgs {
-  const double* dist0;  // [B, nd]
-  int nd;
-};
-
-__device__ __forceinline__ const double* pair_dist(const PnpDistArgs& a, int b) { return a.dist0 + (long)b * a.nd; }
+__device__ __forceinline__ const double* pair_dist(const PnpArgs& a, int b) { return a.dist0 + (long)b * a.nd; }
 
 // Pair b's K0 and coefficients in T: double for the LM, float for AD2's test
 template <class T>
-__device__ __forceinline__ Camera<T> pair_camera(const PnpDistArgs& a, int b) {
+__device__ __forceinline__ Camera<T> pair_camera(const PnpArgs& a, int b) {
   return load_camera<T>(a.K0 + (long)b * 9, pair_dist(a, b), a.nd);
-}
-
-// AD1: pnp_prepare_kernel's compaction with D2's calibrated coordinates; invalid coefficients fail the pair as an
-// invalid K0.  A separate kernel, so that the pinhole one keeps its instructions.
-__global__ void __launch_bounds__(1024) pnp_dist_prepare_kernel(PnpDistArgs a) {
-  const int b = blockIdx.x, tid = threadIdx.x;
-  __shared__ int warp_sums[32];
-  __shared__ int carry;
-  if (tid == 0) carry = 0;
-  __syncthreads();
-  const double* K = a.K0 + (long)b * 9;
-  const double* dist = pair_dist(a, b);
-  const int64_t* m0 = a.matches0 + (long)b * a.M;
-  float4* pts = a.w.pts + (long)b * a.M;
-  float4* wld = a.w.wld + (long)b * a.M;
-  int* slot = a.w.slot + (long)b * a.M;
-  for (int base = 0; base < a.M; base += 1024) {
-    const int i = base + tid;
-    const int64_t j = i < a.M ? m0[i] : -1;
-    float X = 0.f, Y = 0.f, Z = 0.f;
-    float2 p = make_float2(0.f, 0.f);
-    if (j >= 0 && j < a.N) {
-      const float* q = a.points3d1 + ((long)b * a.N + j) * 3;
-      X = q[0];
-      Y = q[1];
-      Z = q[2];
-      p = reinterpret_cast<const float2*>(a.kpts0)[(long)b * a.M + i];
-    }
-    const bool valid = j >= 0 && j < a.N && isfinite(X) && isfinite(Y) && isfinite(Z) && finite2(p);
-    const int k = block_scan_step(valid, tid, warp_sums, &carry);
-    if (i < a.M) slot[i] = valid ? k : -1;
-    if (valid) {
-      double xx, yy;
-      undistort(load_camera<double>(K, dist, a.nd), p.x, p.y, PNP_UNDISTORT_ITERS, 0.0, &xx, &yy);
-      pts[k] = make_float4(p.x, p.y, (float)xx, (float)yy);
-      wld[k] = make_float4(X, Y, Z, 0.f);
-    }
-  }
-  __syncthreads();
-  if (tid == 0) {
-    PnpPair& P = a.w.pair[b];
-    P.thr2 = (float)(a.threshold * a.threshold);
-    P.best = 0;
-    P.n = carry;
-    P.ok = carry >= S && k_valid(K) && dist_valid(dist, a.nd);
-    P.stop = !P.ok;
-    P.drawn = 0;
-    P.success = 0;
-  }
 }
 
 // M = [R | t] as a row-major 3x4, the model AD2 rounds to float
@@ -461,11 +354,6 @@ __device__ __forceinline__ void rt_matrix(const double* x, double* M) {
     M[i * 4 + 3] = x[9 + i];
   }
 }
-
-// geo_hyp_kernel's solver of the distortion-aware pose: PnpSolver's P3P solutions, scored as [R | t]
-struct PnpDistSolver : PnpSolver {
-  static __device__ void pixels(const PnpArgs&, int, const double* x, double* px) { rt_matrix(x, px); }
-};
 
 // AD2's fp32 error of one point under the float [R | t] g: du * du + dv * dv in distorted pixels in front of the
 // camera, +inf behind it (so that an inlier has err < thr2 and lo_term counts the others as outliers)
@@ -513,6 +401,143 @@ __device__ __forceinline__ void pnp_dist_add_normal(const Camera<double>& c, con
 // The entry points' check of the coefficient count, at geo_check_config's distance() place
 inline const char* dist_count_check(int nd) {
   return nd == 4 || nd == 5 || nd == 8 || nd == 12 ? nullptr : "num_dist must be 4, 5, 8 or 12";
+}
+
+// ---- the camera policies ----
+//
+// Everything that differs between the pinhole absolute pose (A1-A8, LA1-LA8) and the one with lens distortion
+// (AD1-AD4) is one of these two policies, on which every kernel and entry point below is a template:
+//   COEFFS, whether the entry point takes coefficients (host);
+//   Consts and consts(a, b), pair b's constants of the LM and the scored model; Test and test(a, b), those of the fp32
+//   test;
+//   valid(K, dist, nd), whether K (and the coefficients) let the pair run;
+//   bearing(K, dist, nd, p, x, y), the calibrated (x, y) of pixel p that P3P reads;
+//   model(c, x, px), the 12-float model of x = (R, t) that is rounded to float and scored;
+//   inlier(c, g, p, q, thr2) and err(c, g, p, q), the fp32 test and error of a point against the float model g;
+//   residual(c, x, p, q) and add_normal(c, e, acc), a point's double residual and its J^T J and J^T r terms.
+
+// The pinhole camera: K0^-1 (A2), K0 [R | t] (A5), the fp32 test in pixels (A5, LA3) and A7's residual
+struct Pinhole {
+  static constexpr bool COEFFS = false;
+  using Consts = const double*;  // K0
+  struct Test {};
+
+  static __device__ __forceinline__ Consts consts(const PnpArgs& a, int b) { return a.K0 + (long)b * 9; }
+  static __device__ __forceinline__ Test test(const PnpArgs&, int) { return {}; }
+  static __device__ __forceinline__ bool valid(const double* K, const double*, int) { return k_valid(K); }
+  static __device__ __forceinline__ void bearing(const double* K, const double*, int, float2 p, double* x, double* y) {
+    const double yy = ((double)p.y - K[5]) / K[4], xx = (((double)p.x - K[2]) - K[1] * yy) / K[0];
+    *x = xx;
+    *y = yy;
+  }
+  static __device__ __forceinline__ void model(const double* K, const double* x, double* px) {
+    projection(K, x, x + 9, px);
+  }
+  static __device__ __forceinline__ bool inlier(Test, const float* g, float4 p, float4 q, float thr2) {
+    return reproj_inlier(g, p, q, thr2);
+  }
+  static __device__ __forceinline__ float err(Test, const float* g, float4 p, float4 q) { return reproj_err(g, p, q); }
+  static __device__ __forceinline__ PnpResidual residual(const double* K, const double* x, float4 p, float4 q) {
+    return pnp_residual(K, x, x + 9, p, q);
+  }
+  static __device__ __forceinline__ void add_normal(const double* K, const PnpResidual& e, double* acc) {
+    pnp_add_normal(K, e, acc);
+  }
+};
+
+// The camera with lens distortion: D2's undistortion (AD1), [R | t] and the fp32 test in distorted pixels (AD2) and
+// AD3's residual; invalid coefficients fail the pair as an invalid K0
+struct Distorted {
+  static constexpr bool COEFFS = true;
+  using Consts = Camera<double>;
+  using Test = Camera<float>;
+
+  static __device__ __forceinline__ Consts consts(const PnpArgs& a, int b) { return pair_camera<double>(a, b); }
+  static __device__ __forceinline__ Test test(const PnpArgs& a, int b) { return pair_camera<float>(a, b); }
+  static __device__ __forceinline__ bool valid(const double* K, const double* dist, int nd) {
+    return k_valid(K) && dist_valid(dist, nd);
+  }
+  static __device__ __forceinline__ void bearing(const double* K, const double* dist, int nd, float2 p, double* x,
+                                                 double* y) {
+    undistort(load_camera<double>(K, dist, nd), p.x, p.y, PNP_UNDISTORT_ITERS, 0.0, x, y);
+  }
+  static __device__ __forceinline__ void model(const Consts&, const double* x, double* px) { rt_matrix(x, px); }
+  static __device__ __forceinline__ bool inlier(const Test& c, const float* g, float4 p, float4 q, float thr2) {
+    return dist_reproj_err(g, c, p, q) < thr2;
+  }
+  static __device__ __forceinline__ float err(const Test& c, const float* g, float4 p, float4 q) {
+    return dist_reproj_err(g, c, p, q);
+  }
+  static __device__ __forceinline__ PnpDistResidual residual(const Consts& c, const double* x, float4 p, float4 q) {
+    return pnp_dist_residual(c, x, x + 9, p, q);
+  }
+  static __device__ __forceinline__ void add_normal(const Consts& c, const PnpDistResidual& e, double* acc) {
+    pnp_dist_add_normal(c, e, acc);
+  }
+};
+
+// geo_hyp_kernel's solver of the absolute pose: sample h's P3P solutions (R, t), scored as Cam's model
+template <class Cam>
+struct PnpSolver {
+  static constexpr int SOLS = ::SOLS, NX = 12, NF = 12;
+  static __device__ int s(const PnpArgs&) { return S; }
+  static __device__ int solve(const PnpArgs& a, int b, unsigned h, double (*x)[NX]) {
+    int id[S];
+    if (geo_sample(a.seed, h, a.w.pair[b].n, S, id) < S) return 0;
+    return p3p(a.w.pts + (long)b * a.M, a.w.wld + (long)b * a.M, id, x);
+  }
+  static __device__ void pixels(const PnpArgs& a, int b, const double* x, double* px) {
+    Cam::model(Cam::consts(a, b), x, px);
+  }
+};
+
+// A1 (and AD1): ordered compaction of the valid matches with Cam's calibrated coordinates, and the camera check
+template <class Cam>
+__global__ void __launch_bounds__(1024) pnp_prepare_kernel(PnpArgs a) {
+  const int b = blockIdx.x, tid = threadIdx.x;
+  __shared__ int warp_sums[32];
+  __shared__ int carry;
+  if (tid == 0) carry = 0;
+  __syncthreads();
+  const double* K = a.K0 + (long)b * 9;
+  const double* dist = pair_dist(a, b);
+  const int64_t* m0 = a.matches0 + (long)b * a.M;
+  float4* pts = a.w.pts + (long)b * a.M;
+  float4* wld = a.w.wld + (long)b * a.M;
+  int* slot = a.w.slot + (long)b * a.M;
+  for (int base = 0; base < a.M; base += 1024) {
+    const int i = base + tid;
+    const int64_t j = i < a.M ? m0[i] : -1;
+    float X = 0.f, Y = 0.f, Z = 0.f;
+    float2 p = make_float2(0.f, 0.f);
+    if (j >= 0 && j < a.N) {
+      const float* q = a.points3d1 + ((long)b * a.N + j) * 3;
+      X = q[0];
+      Y = q[1];
+      Z = q[2];
+      p = reinterpret_cast<const float2*>(a.kpts0)[(long)b * a.M + i];
+    }
+    const bool valid = j >= 0 && j < a.N && isfinite(X) && isfinite(Y) && isfinite(Z) && finite2(p);
+    const int k = block_scan_step(valid, tid, warp_sums, &carry);
+    if (i < a.M) slot[i] = valid ? k : -1;
+    if (valid) {
+      double xx, yy;
+      Cam::bearing(K, dist, a.nd, p, &xx, &yy);
+      pts[k] = make_float4(p.x, p.y, (float)xx, (float)yy);
+      wld[k] = make_float4(X, Y, Z, 0.f);
+    }
+  }
+  __syncthreads();
+  if (tid == 0) {
+    PnpPair& P = a.w.pair[b];
+    P.thr2 = (float)(a.threshold * a.threshold);
+    P.best = 0;
+    P.n = carry;
+    P.ok = carry >= S && Cam::valid(K, dist, a.nd);
+    P.stop = !P.ok;
+    P.drawn = 0;
+    P.success = 0;
+  }
 }
 
 }  // namespace

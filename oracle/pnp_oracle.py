@@ -6,9 +6,14 @@ inliers, R and t.  Only elementwise operations sit on those paths (no BLAS, no n
 reduction may reorder or fuse.  The P3P solver is vectorised over a chunk's samples; the refit's per-point terms over a
 pair's points, its 6x6 solve on Python floats.
 
+The camera enters only through a ``Camera``: ``pinhole(K0)``, or pnp_dist_oracle.camera(K0, dist) with lens
+distortion (steps AD1-AD4).  The pair loops here and in lo_pnp_oracle take either.
+
 ``localization_scene`` draws seeded query images of a known 3D point cloud with a known K, R and t.
 """
 from __future__ import annotations
+
+from typing import Callable, NamedTuple
 
 import numpy as np
 
@@ -186,9 +191,10 @@ def projection(R: np.ndarray, t: np.ndarray, K) -> np.ndarray:
                      for i in range(3) for j in range(4)], -1)
 
 
-def reproj_inliers(P: np.ndarray, pix: np.ndarray, wld: np.ndarray, thr2: np.float32) -> np.ndarray:
-    """fp32 inlier masks [H, n] of projections P [H, 12] (cast to fp32) on pixels [n, 2] and world points [n, 3]: depth
-    w > 0 and squared reprojection error below thr2."""
+def errors(P: np.ndarray, pix: np.ndarray, wld: np.ndarray) -> np.ndarray:
+    """fp32 errors [H, n] of projections P [H, 12] (cast to fp32) on pixels [n, 2] and world points [n, 3] (header
+    steps A5 and LA3): du*du + dv*dv in front of the camera (w > 0), +inf behind it, so that the inlier test err < thr2
+    and the LA3 score both count such a point as an outlier."""
     g = [P.astype(np.float32)[:, i:i + 1] for i in range(12)]
     u, v = pix[None, :, 0], pix[None, :, 1]
     X, Y, Z = wld[None, :, 0], wld[None, :, 1], wld[None, :, 2]
@@ -197,7 +203,20 @@ def reproj_inliers(P: np.ndarray, pix: np.ndarray, wld: np.ndarray, thr2: np.flo
         iw = np.float32(1.0) / w
         du = u - (g[0] * X + g[1] * Y + g[2] * Z + g[3]) * iw
         dv = v - (g[4] * X + g[5] * Y + g[6] * Z + g[7]) * iw
-        return (w > 0.0) & (du * du + dv * dv < thr2)
+        return np.where(w > 0.0, du * du + dv * dv, np.float32(np.inf))
+
+
+def inliers(camera, M: np.ndarray, pix: np.ndarray, wld: np.ndarray, thr2: np.float32) -> np.ndarray:
+    """The fp32 inlier masks [H, n] of the camera's models M [H, 12]: err < thr2 (A5, AD2)."""
+    with np.errstate(invalid="ignore"):
+        return camera.errors(M, pix, wld) < thr2
+
+
+def reproj_inliers(P: np.ndarray, pix: np.ndarray, wld: np.ndarray, thr2: np.float32) -> np.ndarray:
+    """fp32 inlier masks [H, n] of projections P [H, 12] (cast to fp32) on pixels [n, 2] and world points [n, 3]: depth
+    w > 0 and squared reprojection error below thr2."""
+    with np.errstate(invalid="ignore"):
+        return errors(P, pix, wld) < thr2
 
 
 def solutions(seed: int, h: np.ndarray, bear: np.ndarray, wld: np.ndarray):
@@ -251,10 +270,29 @@ def update(x, d):
     return Rn + tn
 
 
-def refine_lm(R, t, K, pix, wld, inl):
-    """GEO_PNP_LM_STEPS Levenberg-Marquardt steps on the squared reprojection error of the inliers, from (R, t)."""
+class Camera(NamedTuple):
+    """What the pair loops of both estimators read of a pair's camera."""
+    valid: bool          # K0 (and the coefficients) let the pair run
+    bearings: Callable   # fp32 pixels [n, 2] -> the fp32 calibrated (x, y) [n, 2] that P3P reads
+    model: Callable      # (R [..., 9], t [..., 3]) -> the model [..., 12] that is rounded to fp32 and scored
+    errors: Callable     # (models [H, 12], pixels, world points) -> fp32 errors [H, n], +inf behind the camera
+    residuals: Callable  # (x, pixels, world points) -> (ru, rv, err, depth, ju, jv) in double, as residuals below
+
+
+def pinhole(K) -> Camera:
+    """The pinhole camera K (header steps A1-A8): K^-1, P = K [R | t], the fp32 error in pixels and A7's residuals."""
+    K = np.asarray(K, dtype=np.float64).reshape(9)
+    return Camera(k_valid(K), lambda pix: calibrate(K, pix), lambda R, t: projection(R, t, K), errors,
+                  lambda x, pix, wld: residuals(x, K, pix, wld))
+
+
+def refine_lm(R, t, K, pix, wld, inl, camera=None):
+    """GEO_PNP_LM_STEPS Levenberg-Marquardt steps on the squared reprojection error of the inliers, from (R, t), through
+    the camera (None: pinhole(K))."""
+    cam = pinhole(K) if camera is None else camera
+
     def terms(x):
-        ru, rv, err, _, ju, jv = residuals(x, K, pix, wld)
+        ru, rv, err, _, ju, jv = cam.residuals(x, pix, wld)
         return go.fixed_sum(np.stack(normal_sums(ru, rv, ju, jv, inl) + [np.where(inl, err, 0.0)]))
 
     x = lc.refine(terms, update, [float(c) for c in R] + [float(c) for c in t], 6, LM_STEPS, LM_LAMBDA0)
@@ -266,39 +304,44 @@ def _fail(M: int, drawn: int) -> dict:
             "success": False, "best_hypothesis": -1, "best_solution": -1, "num_hypotheses": drawn}
 
 
-def absolute_pose_pair(kpts0, points3d1, m0, K0, threshold, max_iters, confidence, seed) -> dict:
+def absolute_pose_pair(kpts0, points3d1, m0, K0, threshold, max_iters, confidence, seed, camera=None) -> dict:
+    """One pair of geo_absolute_pose, or of geo_absolute_pose_dist with camera=pnp_dist_oracle.camera(K0, dist).
+    camera=None is pinhole(K0)."""
     kpts0 = np.asarray(kpts0, dtype=np.float32)
     points3d1 = np.asarray(points3d1, dtype=np.float32)
     m0 = np.asarray(m0, dtype=np.int64)
-    K0 = np.asarray(K0, dtype=np.float64).reshape(9)
+    cam = pinhole(K0) if camera is None else camera
     M = m0.shape[0]
     idx, pix, wld = compact(kpts0, points3d1, m0)
     n = pix.shape[0]
-    if n < S or not k_valid(K0):
+    if n < S or not cam.valid:
         return _fail(M, 0)
-    bear = calibrate(K0, pix)
+    bear = cam.bearings(pix)
     thr2 = np.float32(threshold * threshold)
+
+    def inl(R, t):
+        return inliers(cam, cam.model(R, t), pix, wld, thr2)
 
     def candidates(h):
         R, t, kept = solutions(seed, h, bear, wld)
         if not kept.any():
             return None
         hh, rr = np.nonzero(kept)
-        return reproj_inliers(projection(R[kept], t[kept], K0), pix, wld, thr2).sum(1), h[hh], rr
+        return inl(R[kept], t[kept]).sum(1), h[hh], rr
 
     best_cnt, best_h, best_r, drawn = go.ransac_pair(n, S, max_iters, confidence, candidates)
     if best_h < 0:
         return _fail(M, drawn)
     R, t, _ = solutions(seed, np.array([best_h]), bear, wld)
-    cands = [(R[0, best_r], t[0, best_r], best_cnt)]
+    R0, t0 = R[0, best_r], t[0, best_r]
+    cands = [(R0, t0, best_cnt)]
     if best_cnt >= REFIT_MIN:
-        inl = reproj_inliers(projection(R[0, best_r], t[0, best_r], K0)[None], pix, wld, thr2)[0]
-        Rr, tr = refine_lm(R[0, best_r], t[0, best_r], K0, pix, wld, inl)
-        cands.append((Rr, tr, int(reproj_inliers(projection(Rr, tr, K0)[None], pix, wld, thr2)[0].sum())))
+        Rr, tr = refine_lm(R0, t0, K0, pix, wld, inl(R0[None], t0[None])[0], cam)
+        cands.append((Rr, tr, int(inl(Rr[None], tr[None])[0].sum())))
     Rf, tf, count = cands[1] if len(cands) == 2 and cands[1][2] >= cands[0][2] else cands[0]
-    inliers = np.zeros(M, dtype=bool)
-    inliers[idx[reproj_inliers(projection(Rf, tf, K0)[None], pix, wld, thr2)[0]]] = True
-    return {"R": np.asarray(Rf).reshape(3, 3), "t": np.asarray(tf), "inliers": inliers, "num_inliers": count,
+    mask = np.zeros(M, dtype=bool)
+    mask[idx[inl(np.asarray(Rf)[None], np.asarray(tf)[None])[0]]] = True
+    return {"R": np.asarray(Rf).reshape(3, 3), "t": np.asarray(tf), "inliers": mask, "num_inliers": count,
             "success": True, "best_hypothesis": best_h, "best_solution": best_r, "num_hypotheses": drawn}
 
 
