@@ -17,6 +17,7 @@ SP_TC_BUFFERS = 9  # buffers of the tensor-core backbone's workspace plan (sp_tc
 AL_ABI_VERSION = 1
 AL_LAYOUT_BUFFERS = 30  # buffers of al_workspace_layout
 SIFT_ABI_VERSION = 1
+SIFT_LAYOUT_BUFFERS, SIFT_LAYOUT_MAX_OCTAVES = 10, 16  # sift_workspace_layout
 DISK_ABI_VERSION = 1
 DISK_LAYOUT_BUFFERS = 13  # buffers of disk_workspace_layout
 DHN_ABI_VERSION = 1
@@ -61,6 +62,13 @@ class SiftConfig(C.Structure):
         ("max_num_keypoints", C.c_int32), ("rootsift", C.c_int32), ("reserved", C.c_int32),
         ("detection_threshold", C.c_double), ("edge_threshold", C.c_double),
     ]
+
+
+# numpy dtypes of the SIFT list records in the workspace (SiftCand, SiftKpt in csrc/sift_pipeline.h, 32 bytes each)
+SIFT_CAND_DTYPE = [("x", "<f4"), ("y", "<f4"), ("size", "<f4"), ("response", "<f4"), ("r", "<i4"), ("c", "<i4"),
+                   ("layer", "<i4"), ("octave_packed", "<i4")]
+SIFT_KPT_DTYPE = [("x", "<f4"), ("y", "<f4"), ("size", "<f4"), ("angle", "<f4"), ("response", "<f4"),
+                  ("octave_packed", "<i4"), ("o", "<i4"), ("layer", "<i4")]
 
 
 class DiskConfig(C.Structure):
@@ -286,6 +294,9 @@ SIFT_PROTOTYPES = {  # include/sift_b200.h
     "sift_max_keypoints": (_I64, [_VP, _I32, _I32]),
     "sift_workspace_bytes": (_SZ, [_VP, _I32, _I32, _I32]),
     "sift_forward": (C.c_int, [_VP, _VP, _I32, _VP, _I32, _I32, _I32, _I64] + [_VP] * 7 + [_SZ, _VP]),
+    "sift_workspace_layout": (_I64, [C.POINTER(SiftConfig), _I32, _I32, _I32, _I32, C.POINTER(C.c_int64),
+                                     C.POINTER(C.c_int64), C.POINTER(C.c_int32), C.POINTER(C.c_int32),
+                                     C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
 }
 DISK_PROTOTYPES = {  # include/disk_b200.h
     "disk_weight_blob_floats": (_SZ, []),

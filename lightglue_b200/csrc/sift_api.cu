@@ -78,6 +78,39 @@ extern "C" size_t sift_workspace_bytes(const SiftHandle* h, int32_t, int32_t H, 
   return w.bytes + 256;
 }
 
+extern "C" int64_t sift_workspace_layout(const SiftConfig* cfg, int32_t H, int32_t W, int32_t h, int32_t w, int64_t* offsets,
+                                         int64_t* bytes, int32_t* n_octaves, int32_t* dims, int64_t* gauss, int64_t* dog) {
+  if (!cfg || cfg->abi_version != SIFT_ABI_VERSION || cfg->num_octave_layers < 1 ||
+      cfg->num_octave_layers > SIFT_MAX_LAYERS || cfg->max_num_keypoints <= 0 || cfg->nms_radius < -1)
+    return 0;
+  if (H <= 0 || W <= 0 || h < 1 || h > H || w < 1 || w > W) return 0;
+  static_assert(SIFT_LAYOUT_MAX_OCTAVES == SIFT_MAX_OCTAVES, "pyramid plan size");
+  const int L = cfg->num_octave_layers;
+  char* const base = reinterpret_cast<char*>(kLayoutBase);
+  SiftWs ws;
+  sift_carve(base, H, W, L, cfg->max_num_keypoints, &ws);
+  const size_t raw = (size_t)ws.raw_cap, n_out = (size_t)cfg->max_num_keypoints;
+  const void* p[SIFT_LAYOUT_BUFFERS] = {ws.counters, ws.q, ws.tmp, ws.pyr, ws.cand, ws.kpt, ws.order, ws.flags, ws.pix,
+                                        ws.out_src};
+  const size_t n[SIFT_LAYOUT_BUFFERS] = {8 * sizeof(int), (size_t)H * W * sizeof(float), (size_t)4 * H * W * sizeof(float),
+                                         sift_pyr_floats(H, W, L) * sizeof(float), raw * sizeof(SiftCand),
+                                         raw * sizeof(SiftKpt), raw * sizeof(int), raw * sizeof(int), raw * sizeof(int),
+                                         n_out * sizeof(int)};
+  for (int i = 0; i < SIFT_LAYOUT_BUFFERS; ++i) {
+    if (offsets) offsets[i] = (int64_t)((const char*)p[i] - base);
+    if (bytes) bytes[i] = (int64_t)n[i];
+  }
+  SiftPyr P;
+  sift_layout(ws, h, w, L, &P);
+  if (n_octaves) *n_octaves = P.n_oct;
+  for (int o = 0; o < P.n_oct; ++o) {
+    if (dims) { dims[2 * o] = P.h[o]; dims[2 * o + 1] = P.w[o]; }
+    for (int i = 0; gauss && i < L + 3; ++i) gauss[o * (L + 3) + i] = (int64_t)((const char*)P.gauss[o][i] - base);
+    for (int i = 0; dog && i < L + 2; ++i) dog[o * (L + 2) + i] = (int64_t)((const char*)P.dog[o][i] - base);
+  }
+  return (int64_t)(ws.bytes + 256);
+}
+
 extern "C" int sift_forward(SiftHandle* h, const float* image, int32_t channels, const int32_t* image_size, int32_t B,
                             int32_t H, int32_t W, int64_t cap, float* keypoints, float* scales, float* oris, float* scores,
                             float* descriptors, int32_t* counts, void* workspace, size_t workspace_bytes, void* stream_) {

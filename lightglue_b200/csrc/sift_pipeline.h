@@ -17,6 +17,10 @@
 // DoG layers 1..L are refined and tested (candidates), each candidate gets an orientation histogram and one keypoint
 // per peak (raw keypoints), the raw list is sorted and filtered (OpenCV's dedupe and retainBest, the reference's
 // filter_dog_point and top-k), and the survivors get descriptors.
+//
+// After sift_forward the workspace still holds the last image's state; sift_workspace_layout (include/sift_b200.h)
+// locates each buffer, so that tests check every stage against float64 from its captured input
+// (tests/test_gpu_sift_layers.py, oracle/sift_oracle.py).
 #pragma once
 #include <float.h>
 #include <math.h>
@@ -205,6 +209,12 @@ struct SiftKpt {  // a raw keypoint in final (halved) coordinates
   int octave_packed;  // after the first-octave adjustment
   int o, layer;       // pyramid octave (0 = upsampled) and layer of the descriptor
 };
+
+// The record layouts include/sift_b200.h states (sift_workspace_layout) and the tests read back.
+static_assert(sizeof(SiftCand) == 32 && offsetof(SiftCand, response) == 12 && offsetof(SiftCand, r) == 16 &&
+                  offsetof(SiftCand, octave_packed) == 28, "SiftCand layout");
+static_assert(sizeof(SiftKpt) == 32 && offsetof(SiftKpt, angle) == 12 && offsetof(SiftKpt, octave_packed) == 20 &&
+                  offsetof(SiftKpt, layer) == 28, "SiftKpt layout");
 
 struct SiftParams {
   int L;                    // nOctaveLayers (the reference's num_octaves)

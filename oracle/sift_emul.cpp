@@ -50,16 +50,24 @@ struct HostExec {
 
 extern "C" {
 // Outputs as sift_forward (include/sift_b200.h); image_size: int32 [B, 2] (w, h) or NULL.  counts[b] = -1 when image b
-// overflowed the raw keypoint list.  Returns 0 on success.
-int sift_emul_forward(int L, double contrast, double edge, int nms_radius, int max_kpts, int rootsift, const float* image,
-                      int C, const int* image_size, int B, int H, int W, long cap, float* kpts, float* scales, float* oris,
-                      float* scores, float* desc, int* counts) {
-  if (L < 1 || L > SIFT_MAX_LAYERS || max_kpts <= 0 || cap < max_kpts) return 1;
+// overflowed the raw keypoint list.  workspace: a caller-owned host buffer of at least sift_emul_workspace_bytes, carved
+// as sift_forward carves its device workspace, so that sift_workspace_layout locates the last image's intermediates in
+// it.  Returns 0 on success.
+size_t sift_emul_workspace_bytes(int L, int max_kpts, int H, int W) {
+  if (L < 1 || L > SIFT_MAX_LAYERS || max_kpts <= 0 || H <= 0 || W <= 0) return 0;
   SiftWs w;
   sift_carve(nullptr, H, W, L, max_kpts, &w);
-  char* base = (char*)malloc(w.bytes + 256);
-  if (!base) return 2;
-  char* aligned = (char*)(((uintptr_t)base + 255) & ~(uintptr_t)255);
+  return w.bytes + 256;
+}
+
+int sift_emul_forward_ws(int L, double contrast, double edge, int nms_radius, int max_kpts, int rootsift,
+                         const float* image, int C, const int* image_size, int B, int H, int W, long cap, float* kpts,
+                         float* scales, float* oris, float* scores, float* desc, int* counts, void* workspace,
+                         size_t workspace_bytes) {
+  if (L < 1 || L > SIFT_MAX_LAYERS || max_kpts <= 0 || cap < max_kpts) return 1;
+  if (!workspace || workspace_bytes < sift_emul_workspace_bytes(L, max_kpts, H, W)) return 2;
+  char* aligned = (char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  SiftWs w;
   sift_carve(aligned, H, W, L, max_kpts, &w);
   const SiftParams p = sift_params(L, contrast, edge, nms_radius, max_kpts, rootsift);
   HostExec ex;
@@ -70,6 +78,38 @@ int sift_emul_forward(int L, double contrast, double edge, int nms_radius, int m
                   oris + b * cap, scores + b * cap, desc + b * cap * SIFT_DESC);
     counts[b] = w.counters[3] ? -1 : w.counters[2];
   }
+  return rc;
+}
+
+// The ordering and filtering functors of sift_run on n caller-made raw keypoints (SiftKpt records, cap >= n): order,
+// flags and pix [cap], out_src [max_kpts], counters [8] as sift_workspace_layout describes them.  Reaches states an
+// image does not give, such as equal-score pixel duplicates with equal angles.
+int sift_emul_filter(const SiftKpt* kpt, int n, int cap, int w, int nms_radius, int max_kpts, int* order, int* flags,
+                     int* pix, int* out_src, int* counters) {
+  if (n < 0 || n > cap || max_kpts <= 0) return 1;
+  const SiftParams p = sift_params(1, 0.0, 10.0, nms_radius, max_kpts, 0);
+  HostExec ex;
+  ex.zero(counters, 8);
+  counters[4] = counters[5] = n;
+  const SiftPost s{kpt, counters + 5, cap, order, flags, pix, counters, w};
+  ex.run(SiftSortLex{s});
+  ex.run(SiftRetain{s, p});
+  ex.run(SiftDogFilter{s, p});
+  ex.run(SiftNms{s, p});
+  ex.run(SiftSelect{s, p, out_src});
+  return 0;
+}
+
+// sift_emul_forward_ws on a workspace of its own.
+int sift_emul_forward(int L, double contrast, double edge, int nms_radius, int max_kpts, int rootsift, const float* image,
+                      int C, const int* image_size, int B, int H, int W, long cap, float* kpts, float* scales, float* oris,
+                      float* scores, float* desc, int* counts) {
+  const size_t bytes = sift_emul_workspace_bytes(L, max_kpts, H, W);
+  if (!bytes) return 1;
+  void* base = malloc(bytes);
+  if (!base) return 2;
+  const int rc = sift_emul_forward_ws(L, contrast, edge, nms_radius, max_kpts, rootsift, image, C, image_size, B, H, W,
+                                      cap, kpts, scales, oris, scores, desc, counts, base, bytes);
   free(base);
   return rc;
 }
