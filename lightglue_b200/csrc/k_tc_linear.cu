@@ -66,10 +66,9 @@ struct TcLinParams {
   int conv_pstride;
   long conv_arows;
   int mma_n;  // N of the MMAs when fewer than 256 output columns exist (64 / 128; 0 = 256): the weight rows beyond are zero
-  // TMA stores of the staged epilogues, 64-row boxes (one MMA warpgroup's rows): TEPI_QKV: q, k ([S H Lp, 64], box 64 x 64)
-  // and vt ([S H 64, Lp], box 64 rows x 64 d); TEPI_RESID / F32 / CONV / LN_GELU: out_f32 (box 16 x 64, also the
-  // residual's load map), out_h, out_l (box 16 x 64)
-  CUtensorMap out_map[3];
+  // TEPI_QKV: the TMA store map of vt ([S H 64, Lp], box 64 rows x 64 d); TEPI_RESID: out_f32 (box 16 x 64), the map the
+  // producer prefetches the residual x to L2 with
+  CUtensorMap out_map;
   // TEPI_TOP2_H / F (appended, so the parameter offsets of the other epilogues stay put): gate records, field f of row
   // r at gate_rec[f * S Lp + r] (H: 2 fields, F: 6), gate_on[pair] != 0 for a guided pair, and the squared threshold
   const float* gate_rec; const int* gate_on; float gate_t2;
@@ -85,11 +84,12 @@ struct LinCfg {
   static constexpr int STAGE_BYTES = A_TILE_BYTES + W_TILE_BYTES;
   static constexpr int THREADS = 384;
   static constexpr int MMA_WARPS = 8;
-  // one staged output box: 64 rows x 128 bytes, or 16 fp32 + 2 x 16 bf16 columns of 64 rows; LayerNorm: 2 x 16 bf16
-  // columns (hi / lo), which leaves room for a 4-stage ring
-  static constexpr int STG_BOX = LN ? 4096 : 8192;
-  static constexpr int H16 = LN ? 0 : 4096;  // offset of the bf16 hi image in a box (lo: + 2048)
-  static constexpr int STG_BYTES = 2 * 2 * STG_BOX;  // two output boxes per MMA warpgroup
+  // QKV: one staged vt box of 64 rows x 64 d (8 KB), two per MMA warpgroup; the guided top-2 sweeps: the tile's column
+  // gate records (6 fields x 256 floats); every other epilogue stores from registers
+  static constexpr int STG_BOX = 8192;
+  static constexpr int STG_BYTES = EPI == TEPI_QKV ? 2 * 2 * STG_BOX
+                                   : (EPI == TEPI_TOP2_H || EPI == TEPI_TOP2_F) ? 6 * BN * 4
+                                                                                : 0;
   static constexpr int PAR_BYTES = (LN ? 3 : 1) * BN * 4;  // the tile's bias / LayerNorm bias, gamma, beta
   static constexpr int RED_BYTES = LN ? 2 * TBM * 4 : 0;  // LayerNorm: [pass][row] the peer CTA's row partial sums
   static constexpr int FIXED_BYTES = STG_BYTES + PAR_BYTES + RED_BYTES + 1024 + 256;  // + alignment slack + barriers
@@ -120,6 +120,43 @@ __device__ __forceinline__ float gelu_erf(float y) {
   const float erf_abs = fmaf(-pl * tt, ez, 1.f);
   const float hy = 0.5f * y;
   return fmaf(copysignf(erf_abs, y), hy, hy);
+}
+// Transpose of a 32-column chunk of one accumulator row inside the quad of lanes that holds it.  On entry lane q (=
+// lane % 4) holds in v[i] the W words of its column pair 8 i + 2 q, +1 (i = 0 .. 3: the chunk's four 8-column groups);
+// on return it holds in v[i] the words of the column pair 8 q + 2 i, +1, so 8 consecutive columns, which it writes with
+// 16-byte stores.  Two butterfly exchanges (lanes q ^ 2, then q ^ 1) of two pairs each, then a reorder by source lane;
+// words are only moved, never changed.
+template <int W>
+__device__ __forceinline__ void quad_transpose(uint32_t (&v)[4][W], int q) {
+  const bool b1 = (q & 2) != 0, b0 = (q & 1) != 0;
+  uint32_t s[2][2][W];  // [source: this lane, lane q ^ 2][e]: the column pair of group 2 b1 + e
+#pragma unroll
+  for (int e = 0; e < 2; ++e)
+#pragma unroll
+    for (int w = 0; w < W; ++w) {
+      const uint32_t give = b1 ? v[e][w] : v[2 + e][w];
+      s[0][e][w] = b1 ? v[2 + e][w] : v[e][w];
+      s[1][e][w] = __shfl_xor_sync(0xffffffffu, give, 2);
+    }
+  uint32_t t[4][W];  // the column pair of group q from lane q ^ d
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int w = 0; w < W; ++w) {
+      const uint32_t give = b0 ? s[h][0][w] : s[h][1][w];
+      t[2 * h][w] = b0 ? s[h][1][w] : s[h][0][w];
+      t[2 * h + 1][w] = __shfl_xor_sync(0xffffffffu, give, 1);
+    }
+#pragma unroll
+  for (int i = 0; i < 4; ++i)  // v[i] = t[i ^ q]
+#pragma unroll
+    for (int w = 0; w < W; ++w) {
+      const uint32_t a = b0 ? t[i ^ 1][w] : t[i][w], b = b0 ? t[i ^ 3][w] : t[i ^ 2][w];
+      v[i][w] = b1 ? b : a;
+    }
+}
+__device__ __forceinline__ void st_v4(void* p, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
+  *reinterpret_cast<uint4*>(p) = make_uint4(a, b, c, d);
 }
 __device__ __forceinline__ void mma_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }  // the two MMA warpgroups
 __device__ __forceinline__ void wg_bar(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory"); }  // one of them
@@ -171,21 +208,19 @@ __global__ void __launch_bounds__(LinCfg<EPI>::THREADS, 1) tc_linear_kernel(cons
   using C = LinCfg<EPI>;
   constexpr int STAGES = C::STAGES, STAGE_BYTES = C::STAGE_BYTES, STG_BOX = C::STG_BOX;
   constexpr bool LN = C::LN;
-  // element-wise epilogues: results are staged in shared memory and written by TMA stores that drain while the next
-  // tile's MMAs run
-  constexpr bool STAGED = EPI == TEPI_QKV || EPI == TEPI_RESID || EPI == TEPI_F32 || EPI == TEPI_CONV || LN;
+  // element-wise epilogues: each lane stores its results from registers (vt: through staged TMA stores)
+  constexpr bool ELEMWISE = EPI == TEPI_QKV || EPI == TEPI_RESID || EPI == TEPI_F32 || EPI == TEPI_CONV || LN;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // align by OFFSETTING the shared array (not by rebuilding a pointer from an integer): the compiler keeps the
   // shared address space and emits LDS / STS instead of generic LD / ST for everything derived from it.  The offset is
   // the same in both CTAs of a cluster, so a shared address maps to the same variable in the peer (mapa).
   uint8_t* smem = smem_raw + ((1024u - (static_cast<uint32_t>(reinterpret_cast<uintptr_t>(smem_raw)) & 1023u)) & 1023u);
-  uint8_t* s_stg = smem + STAGES * STAGE_BYTES;                        // [MMA warpgroup][2 boxes of STG_BOX bytes]
+  uint8_t* s_stg = smem + STAGES * STAGE_BYTES;                        // QKV: [MMA warpgroup][2 vt boxes of STG_BOX bytes]
   float* s_par = reinterpret_cast<float*>(s_stg + C::STG_BYTES);      // tile bias [256] / LayerNorm b, gamma, beta [3][256]
   float* s_red = reinterpret_cast<float*>(s_stg + C::STG_BYTES + C::PAR_BYTES);  // LayerNorm: [pass][128 rows]
   uint64_t* full = reinterpret_cast<uint64_t*>(s_stg + C::STG_BYTES + C::PAR_BYTES + C::RED_BYTES);
   uint64_t* empty = full + STAGES;
-  uint64_t* xfull = empty + STAGES;  // TEPI_RESID: [MMA warpgroup][box] the residual x has landed in the box
-  uint64_t* lnbar = xfull + 4;       // LayerNorm: [MMA warpgroup][pass] the peer's partial sums have landed in s_red
+  uint64_t* lnbar = empty + STAGES;  // LayerNorm: [MMA warpgroup][pass] the peer's partial sums have landed in s_red
 
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
   const int n_tiles = p.n_tiles;
@@ -197,10 +232,8 @@ __global__ void __launch_bounds__(LinCfg<EPI>::THREADS, 1) tc_linear_kernel(cons
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&p.a_hi[0]);
     tma_prefetch_desc(&p.w_hi);
-    if (STAGED)
-      for (int i = 0; i < 3; ++i) tma_prefetch_desc(&p.out_map[i]);
+    if (EPI == TEPI_QKV || EPI == TEPI_RESID) tma_prefetch_desc(&p.out_map);
     for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], C::MMA_WARPS); }
-    for (int i = 0; i < 4; ++i) mbar_init(&xfull[i], 1);
     if (LN)  // one arrival per row-owning lane (lane % 4 == 0) of the peer's warpgroup
       for (int i = 0; i < 4; ++i) mbar_init(&lnbar[i], 32);
     fence_barrier_init();
@@ -223,7 +256,7 @@ __global__ void __launch_bounds__(LinCfg<EPI>::THREADS, 1) tc_linear_kernel(cons
       while (walk.next(p, ti)) {
         if (EPI == TEPI_RESID)  // the epilogue's residual (x does not fit in L2) comes from HBM while the MMAs run
           for (int c = 0; c < 2 * BN / 16; ++c)
-            tma_prefetch_l2_2d(&p.out_map[0], ti.n_tile * BN + (c % 16) * 16, (int)ti.grow0 + (c / 16) * 64);
+            tma_prefetch_l2_2d(&p.out_map, ti.n_tile * BN + (c % 16) * 16, (int)ti.grow0 + (c / 16) * 64);
         for (int it = 0; it < iters; ++it, ++g) {
           const int stage = g % STAGES, round = g / STAGES;
           mbar_wait(&empty[stage], (round & 1) ^ 1, p.dbg, 17, it);
@@ -273,12 +306,11 @@ __global__ void __launch_bounds__(LinCfg<EPI>::THREADS, 1) tc_linear_kernel(cons
     if (lane == 0) mbar_arrive(&empty[stage]);
   };
   const int mt = threadIdx.x - 128;                // 0 .. 255 over the MMA warpgroups
-  const bool issuer = (threadIdx.x & 127) == 0;   // issues this warpgroup's TMA stores (and residual loads)
-  const int rw = wq * 16 + tr;                      // box row of registers 4 j, 4 j + 1 (+8: 4 j + 2, 4 j + 3)
+  const bool issuer = (threadIdx.x & 127) == 0;   // issues this warpgroup's vt TMA stores
+  const int rw = wq * 16 + tr;                      // warpgroup row of registers 4 j, 4 j + 1 (+8: 4 j + 2, 4 j + 3)
   uint8_t* stg = s_stg + wg * 2 * STG_BOX;
-  uint64_t* xf = xfull + 2 * wg;
-  uint32_t u = 0;  // boxes this warpgroup has staged: box u uses buffer u & 1
-  // output columns the staged epilogues write
+  uint32_t u = 0;  // vt boxes this warpgroup has staged: box u uses buffer u & 1
+  // output columns the element-wise epilogues write
   const int ocols = EPI == TEPI_QKV ? n_tiles * BN
                     : EPI == TEPI_CONV ? p.ldb
                                        : max(p.ldo, p.out_h != nullptr ? p.ldb : 0);
@@ -293,20 +325,10 @@ __global__ void __launch_bounds__(LinCfg<EPI>::THREADS, 1) tc_linear_kernel(cons
   TileWalk<C::CLUSTER> walk(total_tiles, n_tiles, rank);
   TileInfo ti;
   while (walk.next(p, ti)) {
-    // TEPI_RESID: TMA load of the residual x (16 columns of this warpgroup's 64 rows) into buffer v & 1
-    auto load_x = [&](uint32_t v, int box) {
-      mbar_arrive_expect_tx(&xf[v & 1], 64 * 16 * 4);
-      tma_load_2d(stg + (v & 1) * STG_BOX, &p.out_map[0], ti.n_tile * BN + box * 16, (int)ti.grow0 + wg * 64, &xf[v & 1]);
-    };
     float bias_r = 0.f;  // bias of column mt of this tile, moved to shared memory after the main loop
-    if (STAGED && !LN) {
+    if (ELEMWISE && !LN) {
       const int col = ti.n_tile * BN + mt;
       if (col < ocols) bias_r = __ldg(p.bias + (p.w_select == 1 ? (long)ti.sel * p.bias_sel_stride : 0) + col);
-    }
-    if (EPI == TEPI_RESID && issuer) {  // the first two boxes of x land while the MMAs run
-      bulk_wait_read<0>();
-      load_x(u, 0);
-      load_x(u + 1, 1);
     }
 #pragma unroll
     for (int i = 0; i < 128; ++i) acc[i] = 0.f;
@@ -337,7 +359,7 @@ __global__ void __launch_bounds__(LinCfg<EPI>::THREADS, 1) tc_linear_kernel(cons
     wgmma_wait<0>();
     fence_regs(acc);
     if (prev >= 0) release(prev);
-    if (STAGED && !LN) {  // both warpgroups are done with the previous tile's bias
+    if (ELEMWISE && !LN) {  // both warpgroups are done with the previous tile's bias
       mma_bar();
       s_par[mt] = bias_r;
       mma_bar();
@@ -417,7 +439,7 @@ __global__ void __launch_bounds__(LinCfg<EPI>::THREADS, 1) tc_linear_kernel(cons
       // columns: the first maximum wins) and the best over the slot's other columns s2 (equal to s1 on a tie)
       const int lens = p.st.len[ti.sel];
       // Guided sweeps: only the columns whose gate passes enter the top-2.  The gate records of the tile's 256 partner
-      // columns are staged in shared memory, one array per field (the staging boxes are free in this epilogue); the
+      // columns are staged in shared memory, one array per field (s_stg is sized for them in this epilogue); the
       // tile's own rows read theirs from global memory.  A pair that is not guided takes the ungated path: the flag is
       // uniform per tile, so both MMA warpgroups meet the same barriers.
       float* s_rec = reinterpret_cast<float*>(s_stg);  // [GATE_FIELDS][BN]
@@ -570,30 +592,56 @@ __global__ void __launch_bounds__(LinCfg<EPI>::THREADS, 1) tc_linear_kernel(cons
       continue;
     }
 
-    // ------------------------------------------------------------------ element-wise epilogues, staged
-    // Each warpgroup writes its 64 rows into shared-memory boxes laid out as their TMA store maps declare them (128 / 64
-    // / 32-byte swizzle: the fragment writes are free of bank conflicts); its issuer thread stores a box once every
-    // writer has fenced it, and a box is rewritten only after the store that read it two boxes earlier has finished
-    // reading.  Box loops are unrolled so that the accumulators stay in registers.
-    auto claim = [&]() {  // the next box: the store that last read its buffer is done with it
-      if (issuer) bulk_wait_read<1>();
-      wg_bar(wg);
-      return stg + (u & 1) * STG_BOX;
-    };
-    auto publish = [&]() {  // the box is complete: hand it to the TMA engine
-      fence_proxy_async();
-      wg_bar(wg);
-    };
-    const int row0 = (int)ti.grow0 + wg * 64;  // first row of this warpgroup's boxes
+    // ------------------------------------------------------------------ element-wise epilogues, direct stores
+    // Each lane applies the epilogue arithmetic to its accumulator pairs, element by element, the quad of lanes that
+    // holds a row transposes each 32-column chunk (quad_transpose), and every lane then writes 8 consecutive columns of
+    // its row with 16-byte stores: one warp store instruction covers 8 rows x 64 contiguous bytes, whole 32-byte sectors.
+    // Rows need no bound: Lp is a multiple of the 128-row tile, so every tile lies inside the S Lp rows.  Chunk loops are
+    // unrolled so that the accumulators stay in registers.
+    const int row0 = (int)ti.grow0 + wg * 64;  // first row of this warpgroup
     if (EPI == TEPI_QKV) {
       // which output a QKV tile feeds: packed channel order [q | k | v] (self) or [qk | v] (cross)
       const int which = ti.n_tile;
       const bool qkv_v = p.rope ? which == 2 : which == 1;
-      const bool use_rope = p.rope && !qkv_v;
-      // RoPE cos / sin of the two rows, loaded before the stores; frequency index d / 2 = 4 (j % 8) + tq, the same for
-      // every head
+      if (qkv_v) {
+        // V is stored transposed [S, H, 64, Lp] (K-major B operand of P*V): each warpgroup writes a head at a time into a
+        // shared-memory box [64 d][64 rows] (128-byte swizzle, as the store map declares) that its issuer thread stores
+        // with TMA once every writer has fenced it; a box is rewritten only after the store that read it two boxes
+        // earlier has finished reading.  Padding rows are written as zeros: attention multiplies them by P = 0, which
+        // stays 0 whatever x held there.
+#pragma unroll
+        for (int hh = 0; hh < BN / LG_HDIM; ++hh) {
+          if (issuer) bulk_wait_read<1>();
+          wg_bar(wg);
+          uint8_t* box = stg + (u & 1) * STG_BOX;
+#pragma unroll
+          for (int hr = 0; hr < 2; ++hr) {
+            const int row = rw + 8 * hr;
+            const bool live = ti.r0 + wg * 64 + row < ti.len;
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+              const int j = 8 * hh + jj, d = 8 * jj + 2 * tq;
+              const float2 bb = *reinterpret_cast<const float2*>(s_par + 8 * j + 2 * tq);
+              float v0 = acc[4 * j + 2 * hr] + bb.x, v1 = acc[4 * j + 2 * hr + 1] + bb.y;
+              if (!live) v0 = v1 = 0.f;
+              *reinterpret_cast<__half*>(box + swz(d * 128 + row * 2, 0x70)) = __float2half_rn(v0);
+              *reinterpret_cast<__half*>(box + swz((d + 1) * 128 + row * 2, 0x70)) = __float2half_rn(v1);
+            }
+          }
+          fence_proxy_async();
+          wg_bar(wg);
+          if (issuer) {
+            tma_store_2d(&p.out_map, box, ti.r0 + wg * 64, (ti.s * LG_HEADS + hh) * LG_HDIM);
+            bulk_commit();
+          }
+          ++u;
+        }
+        continue;
+      }
+      // q / k: [S, H, Lp, 64] fp16, a row's 64 d of a head are 128 contiguous bytes.  RoPE cos / sin of the two rows,
+      // loaded before the stores; frequency index d / 2 = 4 (j % 8) + tq, the same for every head
       float rc[2][8], rs[2][8];
-      if (use_rope) {
+      if (p.rope) {
 #pragma unroll
         for (int hr = 0; hr < 2; ++hr)
 #pragma unroll
@@ -603,54 +651,44 @@ __global__ void __launch_bounds__(LinCfg<EPI>::THREADS, 1) tc_linear_kernel(cons
             rs[hr][jj] = __ldg(p.cs + grow * 64 + 32 + 4 * jj + tq);
           }
       }
+      __half* out = which == 0 ? p.q : p.k;
 #pragma unroll
-      for (int hh = 0; hh < BN / LG_HDIM; ++hh) {  // one box per head
-        uint8_t* box = claim();
+      for (int hh = 0; hh < BN / LG_HDIM; ++hh)
 #pragma unroll
         for (int hr = 0; hr < 2; ++hr) {
-          const int row = rw + 8 * hr;
-          const bool live = ti.r0 + wg * 64 + row < ti.len;
+          __half* orow = out + ((long)(ti.s * LG_HEADS + hh) * p.st.Lp + ti.r0 + wg * 64 + rw + 8 * hr) * LG_HDIM;
 #pragma unroll
-          for (int jj = 0; jj < 8; ++jj) {
-            const int j = 8 * hh + jj, d = 8 * jj + 2 * tq;
-            const float2 bb = *reinterpret_cast<const float2*>(s_par + 8 * j + 2 * tq);
-            float v0 = acc[4 * j + 2 * hr] + bb.x, v1 = acc[4 * j + 2 * hr + 1] + bb.y;
-            if (qkv_v) {
-              // V is stored transposed [S, H, 64, Lp] (K-major B operand of P*V); box [64 d][64 rows].  Padding rows
-              // are written as zeros: attention multiplies them by P = 0, which stays 0 whatever x held there.
-              if (!live) v0 = v1 = 0.f;
-              *reinterpret_cast<__half*>(box + swz(d * 128 + row * 2, 0x70)) = __float2half_rn(v0);
-              *reinterpret_cast<__half*>(box + swz((d + 1) * 128 + row * 2, 0x70)) = __float2half_rn(v1);
-              continue;
+          for (int ch = 0; ch < 2; ++ch) {  // 32 d of the head
+            uint32_t w[4][1];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+              const int jj = 4 * ch + i, j = 8 * hh + jj;
+              const float2 bb = *reinterpret_cast<const float2*>(s_par + 8 * j + 2 * tq);
+              float v0 = acc[4 * j + 2 * hr] + bb.x, v1 = acc[4 * j + 2 * hr + 1] + bb.y;
+              if (p.rope) {  // rotary embedding on q / k (lightglue.py:58-65, 168-169); freq index = d / 2
+                const float c = rc[hr][jj], s = rs[hr][jj];
+                const float a = v0, b = v1;
+                v0 = a * c - b * s;
+                v1 = b * c + a * s;
+              }
+              const __half2 h2 = __floats2half2_rn(v0, v1);
+              w[i][0] = *reinterpret_cast<const uint32_t*>(&h2);
             }
-            if (use_rope) {  // rotary embedding on q / k (lightglue.py:58-65, 168-169); freq index = d / 2
-              const float c = rc[hr][jj], s = rs[hr][jj];
-              const float a = v0, b = v1;
-              v0 = a * c - b * s;
-              v1 = b * c + a * s;
-            }
-            *reinterpret_cast<__half2*>(box + swz(row * 128 + d * 2, 0x70)) = __floats2half2_rn(v0, v1);  // [64 rows][64 d]
+            quad_transpose(w, tq);
+            st_v4(orow + 32 * ch + 8 * tq, w[0][0], w[1][0], w[2][0], w[3][0]);
           }
         }
-        publish();
-        if (issuer) {
-          const int bh = ti.s * LG_HEADS + hh;
-          if (qkv_v) tma_store_2d(&p.out_map[2], box, ti.r0 + wg * 64, bh * LG_HDIM);
-          else tma_store_2d(&p.out_map[which], box, 0, bh * p.st.Lp + ti.r0 + wg * 64);
-          bulk_commit();
-        }
-        ++u;
-      }
       continue;
     }
 
-    // bias (* scale) (+ ReLU) (+ residual) -> fp32 and / or bf16 hi (/ lo), or LayerNorm + GELU -> bf16 hi (/ lo); boxes
-    // of 16 columns: fp32 [64][16] (64-byte swizzle) at 0, hi / lo [64][16] (32-byte swizzle) at H16 / H16 + 2048 (4096 /
-    // 6144; LayerNorm: 0 / 2048).  Map bounds clip the columns >= ldo / ldb and the rows >= S Lp.
+    // bias (* scale) (+ ReLU) (+ residual) -> fp32 and / or bf16 hi (/ lo), or LayerNorm + GELU -> bf16 hi (/ lo).
+    // Column bounds: fp32 columns < ldo (a multiple of 4), bf16 columns < ldb (a multiple of 8), both checked by tc_gemm,
+    // so each 16-byte store is wholly inside or outside.
     const bool f32out = EPI == TEPI_RESID || EPI == TEPI_F32;
     const bool has16 = EPI == TEPI_CONV || EPI == TEPI_RESID || LN || (EPI == TEPI_F32 && p.out_h != nullptr);
     const bool haslo = has16 && p.out_l != nullptr;
-    const int nbox = (min(BN, ocols - ti.n_tile * BN) + 15) / 16;
+    const int cbase = ti.n_tile * BN;
+    const int nch = (min(BN, ocols - cbase) + 31) / 32;  // 32-column chunks with columns to write
     bool inside[2] = {true, true};
     if (EPI == TEPI_CONV) {  // the padding pixels of the NHWC image stay zero for the next layer's taps
 #pragma unroll
@@ -662,22 +700,30 @@ __global__ void __launch_bounds__(LinCfg<EPI>::THREADS, 1) tc_linear_kernel(cons
                      xx < p.conv_w + p.conv_pad;
       }
     }
+    // TEPI_RESID: the residual x of this lane's 8 columns of both rows (L2-resident: the producer prefetched the tile's
+    // x), loaded one chunk ahead of the chunk being stored
+    float4 xc[2][2], xn[2][2];
+    auto load_x = [&](int ch, float4 (&xv)[2][2]) {
 #pragma unroll
-    for (int bx = 0; bx < BN / 16; ++bx) {
-      if (bx >= nbox) break;
-      uint8_t* box;
-      if (EPI == TEPI_RESID) {  // x of this box, loaded two boxes ahead
-        box = stg + (u & 1) * STG_BOX;
-        mbar_wait(&xf[u & 1], (u >> 1) & 1, p.dbg, 19, bx);
-      } else {
-        box = claim();
-      }
+      for (int hr = 0; hr < 2; ++hr)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int col = cbase + 32 * ch + 8 * tq + 4 * h;
+          xv[hr][h] = col < p.ldo ? *reinterpret_cast<const float4*>(p.out_f32 + (long)(row0 + rw + 8 * hr) * p.ldo + col)
+                                  : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+    };
+    if (EPI == TEPI_RESID) load_x(0, xc);
+#pragma unroll
+    for (int ch = 0; ch < BN / 32; ++ch) {
+      if (ch >= nch) break;
+      if (EPI == TEPI_RESID && ch + 1 < nch) load_x(ch + 1, xn);
 #pragma unroll
       for (int hr = 0; hr < 2; ++hr) {
-        const int row = rw + 8 * hr;
+        uint32_t w[4][2];
 #pragma unroll
-        for (int jl = 0; jl < 2; ++jl) {
-          const int j = 2 * bx + jl, c = 8 * jl + 2 * tq;  // accumulator column pair, column inside the box
+        for (int i = 0; i < 4; ++i) {
+          const int j = 4 * ch + i;  // accumulator column group
           float v0, v1;
           if (LN) {  // the bias is in acc already (statistics above)
             const float2 gg = *reinterpret_cast<const float2*>(s_par + BN + 8 * j + 2 * tq);
@@ -693,37 +739,54 @@ __global__ void __launch_bounds__(LinCfg<EPI>::THREADS, 1) tc_linear_kernel(cons
             v0 = inside[hr] ? ((p.relu && v0 < 0.f) ? 0.f : v0) : 0.f;
             v1 = inside[hr] ? ((p.relu && v1 < 0.f) ? 0.f : v1) : 0.f;
           }
-          float2* px = reinterpret_cast<float2*>(box + swz(row * 64 + c * 4, 0x30));
-          if (EPI == TEPI_RESID) {  // x + ffn(...) (lightglue.py:172 / 228-229)
-            const float2 xr = *px;
-            v0 += xr.x; v1 += xr.y;
+          w[i][0] = __float_as_uint(v0); w[i][1] = __float_as_uint(v1);
+        }
+        quad_transpose(w, tq);  // lane tq: columns 32 ch + 8 tq .. +7 of the tile
+        float v[8];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) { v[2 * i] = __uint_as_float(w[i][0]); v[2 * i + 1] = __uint_as_float(w[i][1]); }
+        if (EPI == TEPI_RESID) {  // x + ffn(...) (lightglue.py:172 / 228-229)
+          const float4 a = xc[hr][0], b = xc[hr][1];
+          v[0] += a.x; v[1] += a.y; v[2] += a.z; v[3] += a.w; v[4] += b.x; v[5] += b.y; v[6] += b.z; v[7] += b.w;
+        }
+        const long grow = row0 + rw + 8 * hr;
+        const int col = cbase + 32 * ch + 8 * tq;
+        if (f32out) {
+          // 8 fp32 columns are one 32-byte sector, two 16-byte stores: lanes tq and tq ^ 1 swap halves so that each
+          // store instruction writes whole sectors.  Lane tq then holds columns 4 (tq & 1) .. +3 of the groups tq & ~1
+          // (a) and tq | 1 (b).
+          const bool odd = tq & 1;
+          uint32_t a[4], b[4];
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            const uint32_t got = __shfl_xor_sync(0xffffffffu, __float_as_uint(odd ? v[k] : v[4 + k]), 1);
+            a[k] = odd ? got : __float_as_uint(v[k]);
+            b[k] = odd ? __float_as_uint(v[4 + k]) : got;
           }
-          if (f32out) *px = make_float2(v0, v1);
-          if (has16) {
-            const uint32_t o = swz(row * 32 + c * 2, 0x10);
-            const uint32_t hi = pack_bf16x2(v0, v1);
-            *reinterpret_cast<uint32_t*>(box + C::H16 + o) = hi;
-            if (haslo) *reinterpret_cast<uint32_t*>(box + C::H16 + 2048 + o) = pack_bf16x2_lo(v0, v1, hi);
-          }
+          const int ca = cbase + 32 * ch + 8 * (tq & ~1) + 4 * odd, cb = ca + 8;
+          float* o = p.out_f32 + grow * p.ldo;
+          if (ca < p.ldo) st_v4(o + ca, a[0], a[1], a[2], a[3]);
+          if (cb < p.ldo) st_v4(o + cb, b[0], b[1], b[2], b[3]);
+        }
+        if (has16 && col < p.ldb) {
+          uint32_t hi[4];
+#pragma unroll
+          for (int i = 0; i < 4; ++i) hi[i] = pack_bf16x2(v[2 * i], v[2 * i + 1]);
+          st_v4(p.out_h + grow * p.ldb + col, hi[0], hi[1], hi[2], hi[3]);
+          if (haslo)
+            st_v4(p.out_l + grow * p.ldb + col, pack_bf16x2_lo(v[0], v[1], hi[0]), pack_bf16x2_lo(v[2], v[3], hi[1]),
+                  pack_bf16x2_lo(v[4], v[5], hi[2]), pack_bf16x2_lo(v[6], v[7], hi[3]));
         }
       }
-      publish();
-      if (issuer) {
-        const int col = ti.n_tile * BN + bx * 16;
-        if (f32out) tma_store_2d(&p.out_map[0], box, col, row0);
-        if (has16) tma_store_2d(&p.out_map[1], box + C::H16, col, row0);
-        if (haslo) tma_store_2d(&p.out_map[2], box + C::H16 + 2048, col, row0);
-        bulk_commit();
-        if (EPI == TEPI_RESID && bx + 2 < nbox) {  // the buffer's next box: once this store has read it
-          bulk_wait_read<0>();
-          load_x(u, bx + 2);
-        }
+      if (EPI == TEPI_RESID) {
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) { xc[hr][0] = xn[hr][0]; xc[hr][1] = xn[hr][1]; }
       }
-      ++u;
     }
   }
-  // the stores must be complete (not only read) when the grid ends: the next kernel's griddepcontrol.wait relies on it
-  if (STAGED && issuer) bulk_wait_all();
+  // the vt stores must be complete (not only read) when the grid ends: the next kernel's griddepcontrol.wait relies on
+  // it.  The direct stores are plain global stores, which the grid's completion covers.
+  if (EPI == TEPI_QKV && issuer) bulk_wait_all();
   if (C::CLUSTER > 1) {  // neither CTA of a cluster exits while the other may still write into its shared memory
     __syncwarp();
     cluster_sync_all();
@@ -839,22 +902,23 @@ int tc_gemm(TcEngine& e, const SeqState& st, const TcOperands& d, int n_tiles, T
   if ((r = wmap(&p.w_hi, d.wh))) return r;
   p.w_lo = p.w_hi;
   if (e.x3 && (r = wmap(&p.w_lo, d.wl))) return r;
-  // output maps of the staged epilogues (64-row boxes)
-  if (p.epi == TEPI_QKV) {
+  if (p.epi == TEPI_QKV) {  // the vt store map (64-row boxes)
     const uint64_t sh = (uint64_t)st.S * LG_HEADS;
-    if ((r = tc_tmap(e, {p.q, 2, {LG_HDIM, sh * st.Lp}, {LG_HDIM * 2}, {LG_HDIM, 64}}, &p.out_map[0]))) return r;
-    if ((r = tc_tmap(e, {p.k, 2, {LG_HDIM, sh * st.Lp}, {LG_HDIM * 2}, {LG_HDIM, 64}}, &p.out_map[1]))) return r;
-    if ((r = tc_tmap(e, {p.vt, 2, {(uint64_t)st.Lp, sh * LG_HDIM}, {(uint64_t)st.Lp * 2}, {64, LG_HDIM}}, &p.out_map[2])))
+    if ((r = tc_tmap(e, {p.vt, 2, {(uint64_t)st.Lp, sh * LG_HDIM}, {(uint64_t)st.Lp * 2}, {64, LG_HDIM}}, &p.out_map)))
       return r;
   } else if (p.epi == TEPI_RESID || p.epi == TEPI_F32 || p.epi == TEPI_CONV || p.epi == TEPI_LN_GELU) {
-    const uint64_t ldo = p.ldo, ldb = p.ldb;
-    if (p.out_f32 && (r = tc_tmap(e, {p.out_f32, 2, {ldo, rows}, {ldo * 4}, {16, 64}, CU_TENSOR_MAP_SWIZZLE_64B,
-                                      CU_TENSOR_MAP_DATA_TYPE_FLOAT32}, &p.out_map[0])))
-      return r;
-    const __nv_bfloat16* o16[2] = {p.out_h, p.out_l};
-    for (int i = 0; i < 2; ++i)
-      if (o16[i] && (r = tc_tmap(e, {o16[i], 2, {ldb, rows}, {ldb * 2}, {16, 64}, CU_TENSOR_MAP_SWIZZLE_32B}, &p.out_map[1 + i])))
+    // the epilogue writes 16-byte vectors: 4 fp32 or 8 bf16 columns, at row starts on 16-byte boundaries
+    auto aligned = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+    if (p.out_f32 && (p.ldo % 4 != 0 || !aligned(p.out_f32)))
+      return lg_set_error("tc_gemm: an fp32 output needs ldo % 4 == 0 and a 16-byte aligned base");
+    if ((p.out_h || p.out_l) && (p.ldb % 8 != 0 || !aligned(p.out_h) || !aligned(p.out_l)))
+      return lg_set_error("tc_gemm: a bf16 output needs ldb % 8 == 0 and 16-byte aligned bases");
+    if (p.epi == TEPI_RESID) {  // the producer prefetches each tile's residual x to L2 through this map
+      const uint64_t ldo = p.ldo;
+      if ((r = tc_tmap(e, {p.out_f32, 2, {ldo, rows}, {ldo * 4}, {16, 64}, CU_TENSOR_MAP_SWIZZLE_64B,
+                           CU_TENSOR_MAP_DATA_TYPE_FLOAT32}, &p.out_map)))
         return r;
+    }
   }
   p.kb_total = (int)(K / BK);
   p.kb0 = d.k1 ? d.k0 / BK : p.kb_total;
