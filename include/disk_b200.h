@@ -60,6 +60,14 @@ LG_API int disk_forward(DiskHandle* h, const float* image, int32_t C, int32_t B,
 LG_API int disk_heads(DiskHandle* h, const float* image, int32_t C, int32_t B, int32_t H, int32_t W, const int32_t* pos,
                       int32_t P, float* heatmap, float* descriptors, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Test entry: the detection alone, as disk_forward runs it on the network's heatmap: NMS (a pixel is kept iff it is the
+ * first maximum, in row-major order, of its nms_window_size window), detection_threshold (strict) and kornia's top-k of
+ * max_num_keypoints, on a caller-given heatmap [B, H, W] fp32.  positions [B, cap] int32 (pixel y W + x) and scores
+ * [B, cap] fp32: the first counts[b] rows of image b are the keypoints disk_forward would return, in row-major pixel
+ * order; the rest is zero.  Same H, W, cap and workspace as disk_forward. */
+LG_API int disk_detect(DiskHandle* h, const float* heatmap, int32_t B, int32_t H, int32_t W, int64_t cap, int32_t* positions,
+                       float* scores, int32_t* counts, void* workspace, size_t workspace_bytes, void* stream);
+
 /* Host-only introspection (no device work): the workspace plan of disk_forward / disk_heads for this handle and a
  * [B, C, H, W] batch.  Writes, when non-null, the byte offset from the workspace's start and the size of each of its
  * DISK_LAYOUT_BUFFERS buffers, in this order:

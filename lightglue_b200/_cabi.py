@@ -14,6 +14,7 @@ ABI_VERSION = 3
 # include/doghardnet_b200.h, include/geometry_b200.h and include/nn_b200.h: same library
 SP_ABI_VERSION = 2
 SP_TC_BUFFERS = 9  # buffers of the tensor-core backbone's workspace plan (sp_tc_layout)
+SP_LAYOUT_BUFFERS = 13  # buffers of sp_workspace_layout
 AL_ABI_VERSION = 1
 AL_LAYOUT_BUFFERS = 30  # buffers of al_workspace_layout
 SIFT_ABI_VERSION = 1
@@ -277,6 +278,8 @@ SP_PROTOTYPES = {  # include/superpoint_b200.h
     "sp_workspace_bytes": (_SZ, [_VP, _I32, _I32, _I32]),
     "sp_forward": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _I64] + [_VP] * 5 + [_SZ, _VP]),
     "sp_backbone": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _VP, _VP, _VP, _SZ, _VP]),
+    "sp_post": (C.c_int, [_VP, _VP, _VP, _I32, _I32, _I32, _I64] + [_VP] * 5 + [_SZ, _VP]),
+    "sp_workspace_layout": (_I64, [C.POINTER(SpConfig), _I32, _I32, _I32, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "sp_tc_layout": (_I64, [_I32, _I32, _I32, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
 }
 AL_PROTOTYPES = {  # include/aliked_b200.h
@@ -307,6 +310,7 @@ DISK_PROTOTYPES = {  # include/disk_b200.h
     "disk_forward": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _I32, _I64] + [_VP] * 5 + [_SZ, _VP]),
     "disk_heads": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _I32, _VP, _I32, _VP, _VP, _VP, _SZ, _VP]),
     "disk_workspace_layout": (_I64, [_VP, _I32, _I32, _I32, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "disk_detect": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _I64] + [_VP] * 4 + [_SZ, _VP]),
 }
 DHN_PROTOTYPES = {  # include/doghardnet_b200.h
     "dhn_weight_blob_floats": (_SZ, []),

@@ -460,6 +460,19 @@ int run_desc(DiskHandle* h, const Geo& g, const DiskWs& w, const int* n_sel, con
   return 0;
 }
 
+// NMS, threshold and kornia's top-k of heat [B, H, W]: the selected pixels (y W + x) and scores of image b at
+// sel_pos / sel_score + b out_cap (out_cap >= g.ocap; slots past the count untouched), the counts in n_sel [B]
+int detect(const DiskHandle* h, const Geo& g, const DiskWs& w, const float* heat, int* sel_pos, float* sel_score, int* n_sel,
+           long out_cap, cudaStream_t s) {
+  const long n = (long)g.B * g.H * g.W;
+  disk_nms_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(heat, w.kept, g.B, g.H, g.W, h->cfg.nms_window_size / 2);
+  LG_CHECK_LAUNCH();
+  LG_RC(kp_compact(w.kept, g.B, g.H, g.W, h->cfg.detection_threshold, g.ccap, w.row_count, w.row_start, w.n_cand, w.cand_pos,
+                   w.cand_score, s));
+  return kp_select_above_kth(w.n_cand, w.cand_pos, w.cand_score, sel_pos, sel_score, n_sel, g.B, h->cfg.max_num_keypoints,
+                             g.ccap, out_cap, s);
+}
+
 int check_size(const DiskConfig& c, int B, int H, int W, int Cimg) {
   if (B <= 0 || H <= 0 || W <= 0) return lg_set_error("disk: B, H and W must be positive");
   if (Cimg != 1 && Cimg != 3) return lg_set_error("disk: the image must have 1 or 3 channels");
@@ -553,14 +566,7 @@ extern "C" int disk_forward(DiskHandle* h, const float* image, int32_t C, int32_
   carve((char*)workspace, g, &w);
   cudaStream_t s = (cudaStream_t)stream_;
   LG_RC(run_unet(h, image, C, g, g.ld, w, w.heat, s));
-  const long n = (long)B * H * W;
-  const int r = h->cfg.nms_window_size / 2;
-  disk_nms_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(w.heat, w.kept, B, H, W, r);
-  LG_CHECK_LAUNCH();
-  LG_RC(kp_compact(w.kept, B, H, W, h->cfg.detection_threshold, g.ccap, w.row_count, w.row_start, w.n_cand, w.cand_pos,
-                   w.cand_score, s));
-  LG_RC(kp_select_above_kth(w.n_cand, w.cand_pos, w.cand_score, w.sel_pos, w.sel_score, w.n_sel, B, h->cfg.max_num_keypoints,
-                            g.ccap, g.ocap, s));
+  LG_RC(detect(h, g, w, w.heat, w.sel_pos, w.sel_score, w.n_sel, g.ocap, s));
   LG_RC(run_desc(h, g, w, w.n_sel, w.sel_pos, w.sel_score, g.ocap, cap, 1, keypoints, scores, descriptors, s));
   LG_CU(cudaMemcpyAsync(counts, w.n_sel, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
   return 0;
@@ -581,4 +587,19 @@ extern "C" int disk_heads(DiskHandle* h, const float* image, int32_t C, int32_t 
   disk_fill_kernel<<<1, 1024, 0, s>>>(w.n_sel, B, P);
   LG_CHECK_LAUNCH();
   return run_desc(h, g, w, w.n_sel, pos, nullptr, P, P, 0, nullptr, nullptr, descriptors, s);
+}
+
+extern "C" int disk_detect(DiskHandle* h, const float* heatmap, int32_t B, int32_t H, int32_t W, int64_t cap, int32_t* positions,
+                           float* scores, int32_t* counts, void* workspace, size_t workspace_bytes, void* stream_) {
+  if (!h || !heatmap || !positions || !scores || !counts) return lg_set_error("disk_detect: null argument");
+  LG_RC(check_size(h->cfg, B, H, W, 1));
+  if (cap < disk_max_keypoints(h, H, W)) return lg_set_error("disk_detect: output capacity below disk_max_keypoints()");
+  const Geo g = geometry(h->cfg, B, H, W);
+  DiskWs w;
+  if (!workspace || workspace_bytes < carve(nullptr, g, &w)) return lg_set_error("disk_detect: workspace too small");
+  carve((char*)workspace, g, &w);
+  cudaStream_t s = (cudaStream_t)stream_;
+  LG_CU(cudaMemsetAsync(positions, 0, (size_t)B * cap * sizeof(int32_t), s));
+  LG_CU(cudaMemsetAsync(scores, 0, (size_t)B * cap * sizeof(float), s));
+  return detect(h, g, w, heatmap, positions, scores, counts, cap, s);
 }

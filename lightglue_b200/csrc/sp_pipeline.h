@@ -207,6 +207,14 @@ struct SpSelect {
   }
 };
 
+// simple_nms keeps every pixel of a plateau, so without top-k an image can have more candidates than the NMS packing
+// bound (sp_keypoint_cap) that sizes the outputs.  Its count becomes -1 and its rows stay zero: no silent cut.
+struct SpOverflow {
+  const int* n_cand; int* n_sel; int B; long out_cap;
+  SP_HD long count() const { return B; }
+  SP_HD void operator()(long b) const { if (n_cand[b] > out_cap) n_sel[b] = -1; }
+};
+
 struct SpNormalizeDense {  // F.normalize(descriptors, p=2, dim=1) on the coarse map (222), in place
   float* d; int B, Hc, Wc;
   SP_HD long count() const { return (long)B * Hc * Wc; }
@@ -428,6 +436,7 @@ int sp_run_post(Exec& exec, const SpParams& prm, int B, int H, int W, long out_c
   const long cap = (long)H * W;
   if ((rc = stages.compact(exec, ws, B, H, W, prm.detection_threshold, cap))) return rc;
   if ((rc = stages.select(exec, ws, B, prm.max_num_keypoints, cap, out_cap))) return rc;
+  if (prm.max_num_keypoints <= 0) { SpOverflow s{ws.n_cand, ws.n_sel, B, out_cap}; if ((rc = exec.run(s))) return rc; }
   // descriptors (222-226)
   { SpNormalizeDense s{ws.dense, B, Hc, Wc}; if ((rc = exec.run(s))) return rc; }
   if ((rc = stages.sample(exec, ws, kpts, kscores, desc, B, Hc, Wc, out_cap))) return rc;

@@ -63,4 +63,25 @@ int sp_emul_forward(const float* weights, int nms_radius, int max_num_keypoints,
   free(base);
   return rc;
 }
+
+// sp_post (include/superpoint_b200.h) on the host: the post-processing functors on caller-given logits [B,65,H/8,W/8] and
+// dense [B,256,H/8,W/8], in the caller's workspace, carved as sp_workspace_layout lays out a precision-0 workspace
+// (cap = sp_max_keypoints), so each stage's output can be read where the GPU leaves it.  Returns 0 on success.
+int sp_emul_post(int nms_radius, int max_num_keypoints, int remove_borders, float detection_threshold, const float* logits,
+                 const float* dense, int B, int H, int W, long cap, float* kpts, float* scores, float* desc, int* counts,
+                 void* workspace, size_t workspace_bytes) {
+  if (B <= 0 || H < SP_CELL || W < SP_CELL || cap < sp_keypoint_cap(nms_radius, max_num_keypoints, H, W)) return 1;
+  SpWorkspace w;
+  sp_carve(nullptr, B, H, W, cap, &w);
+  if (!workspace || workspace_bytes < w.bytes) return 2;
+  sp_carve((char*)workspace, B, H, W, cap, &w);
+  const size_t cells = (size_t)B * (H / SP_CELL) * (W / SP_CELL);
+  memcpy(w.logits, logits, 65 * cells * sizeof(float));
+  memcpy(w.dense, dense, SP_DESC * cells * sizeof(float));
+  HostExec ex;
+  const SpParams prm{nms_radius, max_num_keypoints, remove_borders, detection_threshold};
+  const int rc = sp_run_post(ex, prm, B, H / SP_CELL * SP_CELL, W / SP_CELL * SP_CELL, cap, w, kpts, scores, desc);
+  if (!rc) memcpy(counts, w.n_sel, (size_t)B * sizeof(int));
+  return rc;
+}
 }

@@ -101,15 +101,16 @@ def dense_scores(logits: torch.Tensor) -> torch.Tensor:
     return prob.permute(0, 1, 3, 2, 4).reshape(b, hc * CELL, wc * CELL)
 
 
-def simple_nms(scores: torch.Tensor, radius: int) -> torch.Tensor:
-    """52-68: keep local maxima of a (2r+1)^2 window, then twice re-admit maxima of what is left outside the
-    suppression zones of the maxima found so far."""
+def simple_nms(scores: torch.Tensor, radius: int, rounds: int = 2) -> torch.Tensor:
+    """52-68: keep local maxima of a (2r+1)^2 window, then twice (`rounds`) re-admit maxima of what is left outside the
+    suppression zones of the maxima found so far.  Only max and == touch the values, so any dtype that holds them is
+    exact."""
     def window_max(x):
         return F.max_pool2d(x, kernel_size=2 * radius + 1, stride=1, padding=radius)
 
     zero = torch.zeros_like(scores)
     keep = scores == window_max(scores)
-    for _ in range(2):
+    for _ in range(rounds):
         suppressed = window_max(keep.float()) > 0
         rest = torch.where(suppressed, zero, scores)
         keep = keep | ((rest == window_max(rest)) & ~suppressed)
@@ -127,6 +128,73 @@ def sample_descriptors(kpts_xy: torch.Tensor, dense: torch.Tensor, cell: int = C
     return F.normalize(out.reshape(c, -1), p=2, dim=0).t().contiguous()
 
 
+def borders(scores: torch.Tensor, pad: int) -> torch.Tensor:
+    """193-198: scores [B, H, W] within `pad` pixels of an edge := -1, in place; returns `scores`."""
+    if pad:
+        scores[:, :pad] = -1
+        scores[:, :, :pad] = -1
+        scores[:, -pad:] = -1
+        scores[:, :, -pad:] = -1
+    return scores
+
+
+def candidates(nms: torch.Tensor, threshold: float) -> Tuple[torch.Tensor, torch.Tensor]:
+    """201-208 for one image: the pixels of nms [H, W] strictly above the threshold (as the fp32 value the kernels
+    compare with), row-major -> (flat index y W + x, value)."""
+    flat = nms.reshape(-1)
+    pos = torch.nonzero(flat > torch.tensor(threshold, dtype=torch.float32).item()).reshape(-1)
+    return pos, flat[pos]
+
+
+def top_k(pos: torch.Tensor, score: torch.Tensor, k: Optional[int]) -> Tuple[torch.Tensor, torch.Tensor]:
+    """71-76: with k < n candidates, the k best by descending score; torch.topk leaves the order of equal scores open, and
+    the rule here (csrc/sp_pipeline.h) takes the lower candidate index first.  Otherwise the row-major order stays."""
+    if not k or k >= score.numel():
+        return pos, score
+    order = torch.sort(score, descending=True, stable=True).indices[:k]
+    return pos[order], score[order]
+
+
+def post(
+    logits: torch.Tensor,
+    dense: torch.Tensor,
+    *,
+    nms_radius: int = 4,
+    max_num_keypoints: Optional[int] = None,
+    detection_threshold: float = 0.0005,
+    remove_borders: int = 4,
+    given: Optional[dict] = None,
+) -> dict:
+    """SuperPoint's post-processing (186-226) from logits [B,65,Hc,Wc] and the un-normalised dense map [B,256,Hc,Wc],
+    stage by stage.  Each stage reads `given[<previous stage>]` when present (a kernel's captured output), else the
+    previous stage of this function:
+      scores        float64 soft-max scores [B, 8 Hc, 8 Wc] (from logits in float64);
+      nms           simple_nms of the fp32 scores, then the borders, [B, 8 Hc, 8 Wc] (float64 holding fp32 values);
+      cand          per image (flat pixel index, value) above the threshold, row-major;
+      sel           per image the kept candidates in output order (top_k);
+      dense         the L2-normalised map in float64;
+      keypoints     per image (x, y) of the selection;
+      descriptors   per image sample_descriptors of the (given) normalised map at those keypoints, float64."""
+    given = given or {}
+    out = {"scores": dense_scores(logits.double())}
+    s = given.get("scores", out["scores"].float())
+    nms = simple_nms(s.double(), nms_radius)
+    out["nms"] = borders(nms, remove_borders)
+    nms = given.get("nms", out["nms"])
+    out["cand"] = [candidates(nms[b], detection_threshold) for b in range(nms.shape[0])]
+    out["sel"] = [top_k(p, v, max_num_keypoints) for p, v in given.get("cand", out["cand"])]
+    out["dense"] = F.normalize(dense.double(), p=2, dim=1)
+    dn = given.get("dense", out["dense"]).double()
+    ws = nms.shape[-1]
+    out["keypoints"], out["descriptors"] = [], []
+    for b, (p, _) in enumerate(given.get("sel", out["sel"])):
+        xy = torch.stack([p % ws, p // ws], dim=-1).double()
+        out["keypoints"].append(xy)
+        out["descriptors"].append(sample_descriptors(xy, dn[b]))
+    return out
+
+
+
 def forward(
     w: Dict[str, torch.Tensor],
     image: torch.Tensor,
@@ -140,13 +208,7 @@ def forward(
     lists (the reference stacks them, which needs equal counts): keypoints [K,2] (x, y), keypoint_scores [K],
     descriptors [K,256]."""
     logits, dense = heads(w, image)
-    scores = simple_nms(dense_scores(logits), nms_radius)
-    if remove_borders:  # 193-198
-        p = remove_borders
-        scores[:, :p] = -1
-        scores[:, :, :p] = -1
-        scores[:, -p:] = -1
-        scores[:, :, -p:] = -1
+    scores = borders(simple_nms(dense_scores(logits), nms_radius), remove_borders)
     dense = F.normalize(dense, p=2, dim=1)  # 222
     kpts, kscores, descs = [], [], []
     for b in range(image.shape[0]):

@@ -311,16 +311,28 @@ MODES = [
     ("mean fallback", "aliked-n16", 64, 96, dict(detection_threshold=0.9999999)),
     ("nms_radius 1", "aliked-n16", 67, 45, dict(nms_radius=1)),
     ("nms_radius 3", "aliked-t16", 96, 128, dict(nms_radius=3)),
+    ("top-k, flat image", "aliked-n16", 64, 64, dict(detection_threshold=-1, max_num_keypoints=100)),
+    ("top-k, nms_radius 0, k = 4096", "aliked-n16", 96, 96, dict(detection_threshold=-1, max_num_keypoints=4096, nms_radius=0)),
+    ("top-k, nms_radius 0, k = 4097", "aliked-n16", 96, 96, dict(detection_threshold=-1, max_num_keypoints=4097, nms_radius=0)),
 ]
+
+
+def mode_image(mode, h, w):
+    if "flat" in mode:  # one grey level: a plateau of equal scores, and filler rows after its few maxima
+        return torch.full((1, 3, h, w), 0.5)
+    return als.make_image(h, w, 1, 700 + h)
 
 
 @pytest.mark.parametrize("mode,model_name,h,w,conf", MODES, ids=[m[0] for m in MODES])
 def test_dkd_modes(mode, model_name, h, w, conf):
     bad = []
-    res = check_forward(bad, model_name, state_dict(model_name), als.make_image(h, w, 1, 700 + h).cuda(),
-                        {**DEFAULT, **conf})
+    res = check_forward(bad, model_name, state_dict(model_name), mode_image(mode, h, w).cuda(), {**DEFAULT, **conf})
     assert not bad, bad
     assert res["counts"][0] > 0
+    if "flat" in mode:
+        assert 0 < res["maxima"][0] < res["counts"][0] == conf["max_num_keypoints"]
+    if "4096" in mode or "4097" in mode:  # the block kernel and, above 4096, the functor, on 9216 NMS survivors
+        assert res["counts"][0] == conf["max_num_keypoints"]
     if "n_limit" in mode:
         assert res["counts"][0] == 20 < res["passed"][0]
     if "fewer" in mode:  # filler rows follow the maxima
