@@ -94,6 +94,35 @@ LG_API size_t nn_workspace_bytes(int32_t B, int32_t M, int32_t N, int32_t D);
 LG_API int nn_match(NnHandle* h, const NnConfig* cfg, const NnInputs* in, const NnOutputs* out, void* workspace,
                     size_t workspace_bytes, void* stream);
 
+/* Host-only introspection (no handle, no device): where nn_match (guided = 0) or nn_match_guided (guided != 0,
+ * below) leaves each stage's output in its workspace for a (B, M, N, D) problem.  The pairs run in groups of G (the
+ * last group holds g = B - (groups - 1) G <= G of them); a group of g pairs has 2g sequences of Lp rows each, sequence
+ * s < g holding image 0 of the group's pair s and sequence g + s image 1 of it, so row r of sequence s is row s Lp + r
+ * of the buffers below, which are sized for R = 2 G Lp rows.  Every buffer is reused by each group: after a call it
+ * holds the LAST group's values (pairs (groups - 1) G .. B - 1).  Writes, when non-null, plan = {G, Lp, pstride,
+ * groups} and the byte offset from the workspace start and the size of each of the NN_LAYOUT_BUFFERS buffers, in
+ * order:
+ *   0 hi      bf16 [R, D]: bf16_rn(d) of each live row, zero past the row's pair length;
+ *   1 lo      bf16 [R, D]: bf16_rn(d - hi), zero past the pair length;
+ *   2 part    fp32 [R, pstride, 2]: per row and 128-column slot t of the partner sequence (its columns
+ *             128 t .. 128 t + 127), (s1, s2) of the live (guided: live and gated) columns: the slot's best
+ *             similarity and the best over its other columns (s1 on a tie; -inf with one such column; s1 = s2 = -inf
+ *             with none);
+ *   3 parg    int32 [R, pstride]: the slot's j1, the lowest column among its maxima (INT32_MAX with no such column);
+ *             part and parg are written for the live rows, in the slot pairs of every 256-column tile with a live
+ *             column; the tail reads slots t < ceil(n / 128), n the partner's length;
+ *   4 jbest   int32 [R]: the row's j1 when it passes the ratio and distance tests, else -1 (live rows only);
+ *   5 sbest   fp32 [R]: the row's s1 (live rows only);
+ *   6 len     int32 [2G]: the clamped length of each sequence (the first 2g);
+ *   7 stop    int32 [G]: zero (the first g);
+ *   8 rec     fp32 [6, R]: guided only (offset -1 and size 0 otherwise): field f of row r at f 2g Lp + r, the gate
+ *             records of nn_match_guided (H: fields 0 and 1, F: all six), zero for rows past M or N;
+ *   9 gate_on int32 [G]: guided only: non-zero for a pair matched under its model (the first g).
+ * Returns the workspace size (nn_workspace_bytes or nn_guided_workspace_bytes), 0 for B < 1 or an invalid size. */
+#define NN_LAYOUT_BUFFERS 10
+LG_API int64_t nn_workspace_layout(int32_t B, int32_t M, int32_t N, int32_t D, int32_t guided, int64_t* offsets,
+                                   int64_t* bytes, int32_t* plan);
+
 /* Guided matching: each pair is matched again under its estimated homography H (image 0 -> image 1) or fundamental
  * matrix F (x1^T F x0 = 0), with the conventions of geo_estimate (include/geometry_b200.h), and a candidate (i, j)
  * counts only when it is consistent with that model (oracle/nn_guided_oracle.py restates the rules in float64).

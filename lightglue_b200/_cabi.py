@@ -32,6 +32,7 @@ GEO_RIGID_3D, GEO_SIMILARITY_3D = 5, 6
 NN_ABI_VERSION = 1  # include/nn_b200.h
 NN_MIN_DIM, NN_MAX_DIM, NN_GROUP_ROWS = 64, 512, 32768
 NN_GUIDE_H, NN_GUIDE_F = 0, 1
+NN_LAYOUT_BUFFERS = 10  # buffers of nn_workspace_layout
 
 
 class LgConfig(C.Structure):
@@ -363,6 +364,8 @@ NN_PROTOTYPES = {  # include/nn_b200.h
     "nn_destroy": (C.c_int, [_VP]),
     "nn_workspace_bytes": (_SZ, [_I32, _I32, _I32, _I32]),
     "nn_match": (C.c_int, [_VP, C.POINTER(NnConfig), C.POINTER(NnInputs), C.POINTER(NnOutputs), _VP, _SZ, _VP]),
+    "nn_workspace_layout": (_I64, [_I32, _I32, _I32, _I32, _I32, C.POINTER(C.c_int64), C.POINTER(C.c_int64),
+                                   C.POINTER(C.c_int32)]),
     "nn_guided_workspace_bytes": (_SZ, [_I32, _I32, _I32, _I32]),
     "nn_match_guided": (C.c_int, [_VP, C.POINTER(NnConfig), C.POINTER(NnInputs), C.POINTER(NnGuide),
                                   C.POINTER(NnOutputs), _VP, _SZ, _VP]),

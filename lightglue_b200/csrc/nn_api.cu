@@ -256,6 +256,30 @@ extern "C" size_t nn_guided_workspace_bytes(int32_t B, int32_t M, int32_t N, int
   return carve(nullptr, B, M, N, D, &w, true);
 }
 
+extern "C" int64_t nn_workspace_layout(int32_t B, int32_t M, int32_t N, int32_t D, int32_t guided, int64_t* offsets,
+                                       int64_t* bytes, int32_t* plan) {
+  if (B < 1 || M < 0 || N < 0 || !dim_ok(D)) return 0;
+  NnWs w;
+  char* const base = reinterpret_cast<char*>(kLayoutBase);
+  const size_t total = carve(base, B, M, N, D, &w, guided != 0);
+  const size_t R = 2 * (size_t)w.G * w.Lp, G = (size_t)w.G, f = sizeof(float), i = sizeof(int), h = sizeof(__nv_bfloat16);
+  const struct { const void* p; size_t n; } buf[NN_LAYOUT_BUFFERS] = {
+      {w.hi, R * D * h}, {w.lo, R * D * h},       {w.part, R * w.pstride * 2 * f}, {w.parg, R * w.pstride * i},
+      {w.jbest, R * i},  {w.sbest, R * f},        {w.len, 2 * G * i},              {w.stop, G * i},
+      {w.rec, R * GATE_FIELDS * f}, {w.gate_on, G * i}};
+  for (int k = 0; k < NN_LAYOUT_BUFFERS; ++k) {
+    if (offsets) offsets[k] = buf[k].p ? (int64_t)((const char*)buf[k].p - base) : -1;
+    if (bytes) bytes[k] = buf[k].p ? (int64_t)buf[k].n : 0;
+  }
+  if (plan) {
+    plan[0] = w.G;
+    plan[1] = w.Lp;
+    plan[2] = w.pstride;
+    plan[3] = (B + w.G - 1) / w.G;
+  }
+  return (int64_t)total;
+}
+
 static int nn_error(const char* entry, const char* what) {
   char msg[128];
   snprintf(msg, sizeof(msg), "%s: %s", entry, what);

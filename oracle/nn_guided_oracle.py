@@ -6,11 +6,13 @@ that bool mask [B, M, N] and restates nn_oracle.match's rules over the gated col
 neighbour is the lowest gated index among the maxima, the second best the largest similarity over the other gated
 columns (-inf when there are none), and a row with no gated column matches nothing.  Its result has nn_oracle.match's
 keys and ``sides``, so ``nn_oracle.decided`` applies to it unchanged; the margins are over gated columns only.  With
-``gate=None`` it is nn_oracle.match.
+``gate=None`` it is nn_oracle.match.  ``chunk_gate`` builds the same gate a block of rows at a time in torch, for
+nn_oracle.match_chunked.
 """
 from __future__ import annotations
 
 import numpy as np
+import torch
 
 from . import geometry_oracle as geo
 from . import nn_oracle
@@ -59,12 +61,53 @@ def one_way(S: np.ndarray, r2, t2, G: np.ndarray | None = None) -> dict:
     return out
 
 
+def block_errors(kind, model9, x0, x1):
+    """geometry_oracle.errors of one model ([9] float64 torch) on every (x0[i], x1[j]), x0 [m, 2] and x1 [n, 2] fp32
+    torch on one device -> [m, n] fp32: the same fp32 operations in the same order, each a separate eager op, so each
+    is rounded on its own as numpy rounds it."""
+    g = model9.float()
+    one = torch.ones((), dtype=torch.float32, device=g.device)
+    a0, b0 = x0[:, 0:1], x0[:, 1:2]  # [m, 1]
+    a1, b1 = x1[None, :, 0], x1[None, :, 1]  # [1, n]
+    if kind == geo.HOMOGRAPHY:
+        w = one / ((g[6] * a0 + g[7] * b0) + g[8])
+        dx = a1 - ((g[0] * a0 + g[1] * b0) + g[2]) * w
+        dy = b1 - ((g[3] * a0 + g[4] * b0) + g[5]) * w
+        return dx * dx + dy * dy
+    la, lb, lc = (g[0] * a0 + g[1] * b0) + g[2], (g[3] * a0 + g[4] * b0) + g[5], (g[6] * a0 + g[7] * b0) + g[8]
+    d2, s2 = (a1 * la + b1 * lb) + lc, one / (la * la + lb * lb)
+    la, lb, lc = (g[0] * a1 + g[3] * b1) + g[6], (g[1] * a1 + g[4] * b1) + g[7], (g[2] * a1 + g[5] * b1) + g[8]
+    d1, s1 = (a0 * la + b0 * lb) + lc, one / (la * la + lb * lb)
+    return torch.fmax(d1 * d1 * s1, d2 * d2 * s2)
+
+
+def chunk_gate(kind, model, kpts0, kpts1, max_error, valid=None, lens0=None, lens1=None, device="cpu"):
+    """``gate`` for nn_oracle.match_chunked: a function (b, side, r0, r1) -> the bool gate [r1 - r0, partner length] of
+    rows r0 .. r1 - 1 of pair b's image `side`, built on `device` with fp32 torch ops (block_errors), bit for bit
+    ``gate``'s; None (every column) for a pair with valid[b] == 0."""
+    model = torch.as_tensor(np.asarray(model, dtype=np.float64)).reshape(-1, 9).to(device)
+    k0 = torch.as_tensor(np.asarray(kpts0, dtype=np.float32)).to(device)
+    k1 = torch.as_tensor(np.asarray(kpts1, dtype=np.float32)).to(device)
+    M, N = k0.shape[1], k1.shape[1]
+    t2 = torch.tensor(float(np.float32(float(max_error) * float(max_error))), dtype=torch.float32, device=device)
+
+    def fn(b, side, r0, r1):
+        if valid is not None and not valid[b]:
+            return None
+        m = nn_oracle._pair_len(lens0, b, M)
+        n = nn_oracle._pair_len(lens1, b, N)
+        if side == 0:
+            return block_errors(kind, model[b], k0[b, r0:r1], k1[b, :n]) < t2  # NaN fails
+        return (block_errors(kind, model[b], k0[b, :m], k1[b, r0:r1]) < t2).T
+    return fn
+
+
 def match(desc0, desc1, lens0=None, lens1=None, ratio_thresh=None, distance_thresh=None, mutual_check=True,
-          gate=None) -> dict:
+          gate=None, split=False) -> dict:
     """nn_oracle.match with the gate [B, M, N] bool (see ``gate``) restricting both sides to the gated pairs (i, j);
-    gate None: nn_oracle.match itself."""
+    gate None: nn_oracle.match itself.  split: s from the device's split-bf16 products, as nn_oracle.match."""
     if gate is None:
-        return nn_oracle.match(desc0, desc1, lens0, lens1, ratio_thresh, distance_thresh, mutual_check)
+        return nn_oracle.match(desc0, desc1, lens0, lens1, ratio_thresh, distance_thresh, mutual_check, split)
     d0 = np.asarray(desc0, dtype=np.float64)
     d1 = np.asarray(desc1, dtype=np.float64)
     B, M, _ = d0.shape
@@ -78,7 +121,7 @@ def match(desc0, desc1, lens0=None, lens1=None, ratio_thresh=None, distance_thre
     for b in range(B):
         m = M if lens0 is None else int(min(max(int(lens0[b]), 0), M))
         n = N if lens1 is None else int(min(max(int(lens1[b]), 0), N))
-        S = d0[b, :m] @ d1[b, :n].T if m and n else np.zeros((m, n))
+        S = nn_oracle.similarity(d0[b, :m], d1[b, :n], split) if m and n else np.zeros((m, n))
         G = np.asarray(gate[b], dtype=bool)[:m, :n]
         a, c = one_way(S, r2, t2, G), one_way(S.T, r2, t2, G.T)  # an empty side keeps nothing
         for i in range(m):

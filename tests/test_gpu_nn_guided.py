@@ -15,11 +15,11 @@ from oracle import geometry_oracle as geo
 from oracle import geometry_synth as gs
 from oracle import nn_guided_oracle as ngo
 from oracle import sift_synth
+from tests.test_nn_emulation import TOL_D, TOL_S  # the split-bf16 gates, calibrated by emulation
 
 pytestmark = pytest.mark.gpu
 
 KEYS = ("matches0", "matches1", "matching_scores0", "matching_scores1")
-TOL_S, TOL_D = 2e-4, 4e-4  # the split-bf16 bound of test_gpu_nn_matcher.py
 KIND = {"H": geo.HOMOGRAPHY, "F": geo.FUNDAMENTAL}
 GATE_PX = {"H": 60.0, "F": 24.0}  # a disc of 60 px, a band of 2 x 24 px around the epipolar line
 

@@ -12,14 +12,11 @@ from lightglue_b200.geometry import find_homography
 from lightglue_b200.ragged import match_ragged
 from oracle import nn_oracle as nno
 from oracle import sift_synth
+from tests.test_nn_emulation import TOL_D, TOL_S  # the split-bf16 gates, calibrated by emulation
 
 pytestmark = pytest.mark.gpu
 
 KEYS = ("matches0", "matches1", "matching_scores0", "matching_scores1")
-# split-bf16 rounding of s for unit descriptors, D <= 512: the hi / lo split leaves 2^-17 relative per operand, the
-# dropped lo * lo term is below 2^-18, and fp32 accumulation over D terms adds D 2^-24: about 5e-5 in all.  The
-# tolerances leave a factor of four (2e-4 in s, 4e-4 in D = 2 (1 - s)).
-TOL_S, TOL_D = 2e-4, 4e-4
 
 
 def _run(d0, d1, lens0=None, lens1=None, **conf):
