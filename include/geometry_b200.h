@@ -265,6 +265,40 @@
  *      and the result is deterministic; the score is quantised to integers; samples have 8 points rather than 7, so
  *      they are find_fundamental's; there is no non-minimal refit inside the LO, and no DEGENSAC or PROSAC.
  *
+ * MAGSAC++ homography and fundamental matrix (geo_homography_magsac, geo_fundamental_magsac;
+ * oracle/magsac_oracle.py restates them bit for bit): LH1-LH8 and LF1-LF8 with the truncated squared error replaced
+ * by MAGSAC++'s loss marginalised over the noise scale sigma in [0, sigma_max] (Barath, Noskova, Ivashechkin and Matas,
+ * CVPR 2020), nu = 4 degrees of freedom, and its local optimisation by iteratively reweighted least squares with the
+ * weights of the same marginalisation.  threshold (thr2 = (float)(threshold * threshold)) keeps its meaning: it sets
+ * the inliers, num_inliers and the count that drives stopping.  max_threshold = T = GEO_MAGSAC_K * sigma_max sets the
+ * loss: mt2 = (float)(max_threshold * max_threshold), z = err / mt2.  With c = GEO_MAGSAC_K^2 / 2 and gamma_l, Gamma_u
+ * the unnormalised lower and upper incomplete gamma functions, for z < 1
+ *   rho(z) = [gamma_l(5/2, c z) + c z (Gamma_u(3/2, c z) - Gamma_u(3/2, c))] / gamma_l(5/2, c),
+ *   w(z) = (Gamma_u(3/2, c z) - Gamma_u(3/2, c)) / (Gamma_u(3/2, 0) - Gamma_u(3/2, c)),
+ * and rho = 1, w = 0 for z >= 1 or a non-finite err: rho rises from 0 to 1, w falls from 1 to 0, and w is
+ * proportional to d rho / dz.  Neither is evaluated: both are the tables R and W of GEO_MAGSAC_KNOTS + 1 knots at
+ * z = i / GEO_MAGSAC_KNOTS, the double literals of lightglue_b200/csrc/magsac_table.h (linear interpolation is within
+ * 1.8e-6 of rho and 5.8e-5 of w), read by linear interpolation as below.
+ *
+ * MH1, MF1. As LH1 and LF1; mt2 as above.  M <= GEO_LO_MAX_MATCHES.
+ * MH2, MF2. As LH2 and LF2: with the same seed, sample h and its hypothesis are LO's sample h.
+ * MH3, MF3. Score, per hypothesis, from step 5's fp32 err (the model rounded to float): u = err * ks in fp32 with
+ *      ks = (float)GEO_MAGSAC_KNOTS / mt2 (fp32 quotient); for u < GEO_MAGSAC_KNOTS, i = (int)u, f = u - (float)i,
+ *      r = R'_i + f * (R'_(i+1) - R'_i) with R' = R rounded to float, and q = (uint32)fminf(r * GEO_LO_QSCALE,
+ *      GEO_LO_QSCALE); otherwise (a NaN included) q = GEO_LO_QSCALE.  score = sum of q over the points in uint64,
+ *      count = the number of err < thr2, packed as L3's count << 40 | score.  Since q <= GEO_LO_QSCALE, the bound
+ *      GEO_LO_MAX_MATCHES holds.  Lower is better; ties go to the lowest h.
+ * MH4, MF4. As LH4 and LF4 with MH3's score and MH7's LM.
+ * MH5, MF5. As LH5 and LF5: stopping from the model's count at thr2.
+ * MH6, MF6. As LH6 and LF6 with MH3's score and MH7's LM.
+ * MH7, MF7. LM as LH7 and LF7 (parametrisation, residuals, Jacobians, damping, steps), on the MAGSAC++ cost: per point
+ *      u = err * ((double)GEO_MAGSAC_KNOTS / (double)mt2); a point with u < GEO_MAGSAC_KNOTS has i = (int)u,
+ *      f = u - (double)i, cost R_i + f * (R_(i+1) - R_i) and weight wt = W_i + f * (W_(i+1) - W_i) (double), and adds
+ *      wt * (jx_i*jx_j + jy_i*jy_j) and wt * (jx_i*dx + jy_i*dy) (H) or wt * (J_i*J_j) and wt * (J_i*r) (F); any other
+ *      point costs 1.0 and adds no terms.  So every point within T contributes, not only those within thr2.  The sums
+ *      run in step 2's order and the step is taken only if the summed cost is strictly lower.
+ * MH8, MF8. Outputs as LH8 and LF8 (inliers and num_inliers at thr2), cost the final model's MH3 / MF3 score.
+ *
  * Absolute pose (geo_absolute_pose; oracle/pnp_oracle.py restates it bit for bit): the (R, t) of x_cam = R X + t that
  * maps the world points of image 1's keypoints into the query camera 0, OpenCV's rvec/tvec convention.  Expressions
  * below evaluate left to right as written (a + b + c is (a + b) + c); no step whose result must match bit for bit calls
@@ -660,6 +694,24 @@ LG_API int geo_homography_lo(const GeoConfig* cfg, const GeoInputs* in, GeoLoOut
 LG_API size_t geo_lo_fundamental_workspace_bytes(int32_t B, int32_t M, int32_t max_iters);
 LG_API int geo_fundamental_lo(const GeoConfig* cfg, const GeoInputs* in, GeoLoOutputs* out, void* workspace,
                               size_t workspace_bytes, void* stream);
+
+#define GEO_MAGSAC_KNOTS 1024             /* intervals of the loss and weight tables (lightglue_b200/csrc/magsac_table.h) */
+#define GEO_MAGSAC_K 3.6437211935036444   /* k = sqrt(chi2_0.99(4)): max_threshold = k * sigma_max */
+
+typedef struct GeoMagsacConfig {
+  GeoConfig geo;         /* as geo_homography_lo's and geo_fundamental_lo's; threshold sets the inliers and the count */
+  double max_threshold;  /* T, pixels, finite and > 0: the scale of the MAGSAC++ loss and weights */
+} GeoMagsacConfig;
+
+/* MAGSAC++ homography (steps MH1-MH8): cfg->geo.model must be GEO_HOMOGRAPHY, in->M <= GEO_LO_MAX_MATCHES.  The
+ * workspace is geo_lo_homography_workspace_bytes'. */
+LG_API int geo_homography_magsac(const GeoMagsacConfig* cfg, const GeoInputs* in, GeoLoOutputs* out, void* workspace,
+                                 size_t workspace_bytes, void* stream);
+
+/* MAGSAC++ fundamental matrix (steps MF1-MF8): cfg->geo.model must be GEO_FUNDAMENTAL, in->M <= GEO_LO_MAX_MATCHES.
+ * The workspace is geo_lo_fundamental_workspace_bytes'. */
+LG_API int geo_fundamental_magsac(const GeoMagsacConfig* cfg, const GeoInputs* in, GeoLoOutputs* out, void* workspace,
+                                  size_t workspace_bytes, void* stream);
 
 #define GEO_PNP_MAX_SOLUTIONS 4
 #define GEO_PNP_COLLINEAR_EPS 1e-10

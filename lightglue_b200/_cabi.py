@@ -26,6 +26,7 @@ DHN_LAYOUT_BUFFERS = 16  # buffers of dhn_workspace_layout
 GEO_ABI_VERSION = 1  # include/geometry_b200.h
 GEO_HOMOGRAPHY, GEO_FUNDAMENTAL, GEO_ESSENTIAL = 0, 1, 2
 GEO_LO_QSCALE, GEO_LO_MAX_MATCHES = 65536, (1 << 20) - 1
+GEO_MAGSAC_KNOTS, GEO_MAGSAC_K = 1024, 3.6437211935036444
 GEO_AFFINE, GEO_AFFINE_PARTIAL, GEO_AFFINE_MAX_REFINE = 3, 4, 100
 GEO_CAMERA_FLOAT32, GEO_CAMERA_FLOAT64, GEO_UNDISTORT_MAX_ITERS = 0, 1, 1000
 GEO_RIGID_3D, GEO_SIMILARITY_3D = 5, 6
@@ -160,6 +161,10 @@ class GeoLoPoseOutputs(C.Structure):
 
 class GeoLoOutputs(C.Structure):
     _fields_ = [("geo", GeoOutputs), ("num_local_optimizations", C.c_void_p), ("cost", C.c_void_p)]
+
+
+class GeoMagsacConfig(C.Structure):
+    _fields_ = [("geo", GeoConfig), ("max_threshold", C.c_double)]
 
 
 class GeoPnpConfig(C.Structure):
@@ -338,6 +343,10 @@ GEO_PROTOTYPES = {  # include/geometry_b200.h
     "geo_lo_fundamental_workspace_bytes": (_SZ, [_I32, _I32, _I32]),
     "geo_fundamental_lo": (C.c_int, [C.POINTER(GeoConfig), C.POINTER(GeoInputs), C.POINTER(GeoLoOutputs), _VP, _SZ,
                                      _VP]),
+    "geo_homography_magsac": (C.c_int, [C.POINTER(GeoMagsacConfig), C.POINTER(GeoInputs), C.POINTER(GeoLoOutputs),
+                                        _VP, _SZ, _VP]),
+    "geo_fundamental_magsac": (C.c_int, [C.POINTER(GeoMagsacConfig), C.POINTER(GeoInputs), C.POINTER(GeoLoOutputs),
+                                         _VP, _SZ, _VP]),
     "geo_pnp_workspace_bytes": (_SZ, [_I32, _I32, _I32]),
     "geo_absolute_pose": (C.c_int, [C.POINTER(GeoPnpConfig), C.POINTER(GeoPnpInputs), C.POINTER(GeoPnpOutputs), _VP,
                                     _SZ, _VP]),

@@ -228,7 +228,8 @@ __device__ __forceinline__ float geo_err(int kind, const float* h, float4 p) {
   return fmaxf(d1 * d1 * s1, d2 * d2 * s2);
 }
 
-__global__ void __launch_bounds__(1024) geo_prepare_kernel(GeoArgs a) {
+// Step 1's compaction and step 2's normalisation of pair blockIdx.x, by a CTA of 1024 threads
+__device__ __forceinline__ void geo_prepare(GeoArgs a) {
   const int b = blockIdx.x, tid = threadIdx.x;
   __shared__ int warp_sums[32];
   __shared__ int carry;
@@ -283,5 +284,7 @@ __global__ void __launch_bounds__(1024) geo_prepare_kernel(GeoArgs a) {
     P.drawn = 0;
   }
 }
+
+__global__ void __launch_bounds__(1024) geo_prepare_kernel(GeoArgs a) { geo_prepare(a); }
 
 }  // namespace

@@ -1,12 +1,14 @@
 // The LO-RANSAC pieces shared by the relative pose (lo_pose_api.cu, header steps L1-L8), the homography and the
 // fundamental matrix (lo_hf_api.cu, LH1-LH8 and LF1-LF8) and the absolute pose (lo_pnp_api.cu, LA1-LA8), all compiled
-// with -fmad=false: the packed MSAC score term, the fixed-order sums of the Levenberg-Marquardt terms, one LM loop and
-// re-score over a model policy, and the schedule of L4-L6 and L8 that every LO estimator runs on it.
+// with -fmad=false: the packed score term of the MSAC and MAGSAC++ losses, the fixed-order sums of the
+// Levenberg-Marquardt terms, one LM loop and re-score over a model policy, and the schedule of L4-L6 and L8 that every
+// LO estimator runs on it (the MAGSAC++ homography and fundamental matrix, MH1-MH8 and MF1-MF8, included).
 #pragma once
 #include <cuda_runtime.h>
 
 #include "geo_common.cuh"
 #include "geo_lm.cuh"
+#include "magsac_table.h"
 #include "ws_bump.h"
 
 namespace {
@@ -20,6 +22,63 @@ __device__ __forceinline__ unsigned long long lo_term(float e, float thr2, float
   if (!(e < thr2)) return GEO_LO_QSCALE;
   return LO_COUNT_ONE + (e == 0.f ? 0u : (unsigned)fminf(e * w, (float)GEO_LO_QSCALE));
 }
+
+// The loss of an LO estimator: the score term of its fp32 errors (L3) and the per-point cost and weight of its LM
+// (L7).  A loss object carries the call's thresholds; term() gives the score term's functor, lm() the scale the LM
+// loop passes to the model's terms(), whose per-point sums read point(scale, err, cost, wt) and weigh(wt, x):
+//   Msac, the truncated squared error of L3 and L7 at the user's thr2 (every estimator but MH / MF);
+//   Magsac, MAGSAC++'s sigma-marginalised loss at the scale T^2 = mt2 (header steps MH3 and MH7), with the count bit
+//   still at the user's thr2.
+struct Msac {
+  float thr2;
+  struct Term {
+    float thr2, w;
+    __device__ __forceinline__ unsigned long long operator()(float e) const { return lo_term(e, thr2, w); }
+  };
+  __device__ __forceinline__ Term term() const { return {thr2, (float)GEO_LO_QSCALE / thr2}; }
+  __device__ __forceinline__ double lm() const { return (double)thr2; }
+  // An inlier (err < thr2) adds err and its unweighted terms; any other point adds thr2
+  static __device__ __forceinline__ bool point(double thr2, double err, double& cost, double&) {
+    const bool in = err < thr2;
+    cost = in ? err : thr2;
+    return in;
+  }
+  static __device__ __forceinline__ double weigh(double, double x) { return x; }
+};
+
+struct Magsac {
+  float thr2, mt2;  // the user's squared threshold (the count) and T^2 (the loss)
+  // MH3: u = e * (KNOTS / mt2) in fp32; for u < KNOTS, i = (int)u, f = u - i and rho = R_i + f * (R_(i+1) - R_i)
+  // with R the table rounded to float, q = (uint32)fminf(rho * QSCALE, QSCALE); else (NaN included) q = QSCALE
+  struct Term {
+    float thr2, ks;
+    __device__ __forceinline__ unsigned long long operator()(float e) const {
+      const unsigned long long c = e < thr2 ? LO_COUNT_ONE : 0ull;
+      const float u = e * ks;
+      if (!(u < (float)GEO_MAGSAC_KNOTS)) return c + GEO_LO_QSCALE;
+      const int i = (int)u;
+      const float f = u - (float)i, r0 = (float)MAGSAC_RHO[i], r1 = (float)MAGSAC_RHO[i + 1];
+      return c + (unsigned)fminf((r0 + f * (r1 - r0)) * (float)GEO_LO_QSCALE, (float)GEO_LO_QSCALE);
+    }
+  };
+  __device__ __forceinline__ Term term() const { return {thr2, (float)GEO_MAGSAC_KNOTS / mt2}; }
+  __device__ __forceinline__ double lm() const { return (double)mt2; }
+  // MH7: u = err * ((double)KNOTS / T^2); for u < KNOTS, i = (int)u, f = u - i, cost = R_i + f * (R_(i+1) - R_i) and
+  // wt = W_i + f * (W_(i+1) - W_i) in double; else the point costs 1 and adds no terms
+  static __device__ __forceinline__ bool point(double mt2, double err, double& cost, double& wt) {
+    const double u = err * ((double)GEO_MAGSAC_KNOTS / mt2);
+    if (!(u < (double)GEO_MAGSAC_KNOTS)) {
+      cost = 1.0;
+      return false;
+    }
+    const int i = (int)u;
+    const double f = u - (double)i;
+    cost = MAGSAC_RHO[i] + f * (MAGSAC_RHO[i + 1] - MAGSAC_RHO[i]);
+    wt = MAGSAC_W[i] + f * (MAGSAC_W[i + 1] - MAGSAC_W[i]);
+    return true;
+  }
+  static __device__ __forceinline__ double weigh(double wt, double x) { return wt * x; }
+};
 
 // The fixed-order sums (header step 2) of T terms, G at a time through red [G][RED]; every thread of the CTA calls it
 template <int T, int G>
@@ -43,7 +102,7 @@ __device__ void lo_tree_sums(const double* acc, double (*red)[RED], double* out,
 //   lo_tree_sums, which keeps red within static shared memory), NP (the length of the parameter vector x) and NF (the
 //   length of the pixel model that is scored);
 //   Scratch, the model's own shared state;
-//   terms(s, P, x, pts, n, thr2, out, tid), the TERMS sums at x (every thread);
+//   terms(s, P, x, pts, n, scale, out, tid), the TERMS sums at x (every thread), scale the loss's lm();
 //   update(s, x, d, out), x moved by the LM step d (thread 0);
 //   pixels(s, P, x, out), x as the scaled pixel model that is rounded to float and scored (thread 0);
 //   err(h, pts[k]), the fp32 error of point k against a float model.
@@ -95,18 +154,18 @@ __device__ void lo_refine(LoShared<Model>& s, const Pair& P, Points pts, int n, 
   }
 }
 
-// L3 / LH3 / LF3 / LA3 score and count of s.x in pixels (s.px), rounded to float (s.fm)
-template <class Model, class Pair, class Points>
-__device__ void lo_rescore(LoShared<Model>& s, const Pair& P, Points pts, int n, float thr2, int tid) {
+// L3 / LH3 / LF3 / LA3 / MH3 / MF3 score and count of s.x in pixels (s.px), rounded to float (s.fm)
+template <class Model, class Pair, class Points, class Loss>
+__device__ void lo_rescore(LoShared<Model>& s, const Pair& P, Points pts, int n, Loss loss, int tid) {
   if (tid == 0) {
     Model::pixels(s, P, s.x, s.px);
     for (int i = 0; i < Model::NF; ++i) s.fm[i] = (float)s.px[i];
     s.score = 0;
   }
   __syncthreads();
-  const float w = (float)GEO_LO_QSCALE / thr2;
+  const auto term = loss.term();
   unsigned long long acc = 0;
-  for (int k = tid; k < n; k += RED) acc += lo_term(Model::err(s.fm, pts[k]), thr2, w);
+  for (int k = tid; k < n; k += RED) acc += term(Model::err(s.fm, pts[k]));
   if (acc) atomicAdd(&s.score, acc);
   __syncthreads();
 }
@@ -175,8 +234,8 @@ __device__ __forceinline__ unsigned long long* geo_sums(const LoArgs<Base>& a) {
 // The schedule runs over Est, the estimator's model policy (LoShared above) with:
 //   Base, its RANSAC arguments (a.p.w.pair[b] the pair, a.p.out the outputs); Solver, its geo_hyp_kernel solver;
 //   Score, its geo_score_kernel policy; S, the points per sample; SOLS, the solutions per sample;
-//   points(a, b), consts(a, b) and thr2(a, b), pair b's points, constants and squared threshold as the LM loop reads
-//   them;
+//   points(a, b), consts(a, b) and loss(a, b), pair b's points, constants and loss (Msac or Magsac above) as the LM
+//   loop and the re-score read them;
 //   seed(s, a, b, hr, m, L, t), the LM start s.x of solution hr (index m of acc) and L.model of it (every thread; a
 //   barrier follows);
 //   store(s, L), the re-scored model of s into L.model (thread 0);
@@ -218,9 +277,9 @@ __global__ void __launch_bounds__(RED, 1) lo_chunk_kernel(LoArgs<typename Est::B
     }
     __syncthreads();
     const auto pts = Est::points(a, b);
-    const float thr2 = Est::thr2(a, b);
-    lo_refine(s, Est::consts(a, b), pts, P.n, (double)thr2, GEO_LO_STEPS, GEO_LO_LAMBDA0, t);
-    lo_rescore(s, Est::consts(a, b), pts, P.n, thr2, t);
+    const auto loss = Est::loss(a, b);
+    lo_refine(s, Est::consts(a, b), pts, P.n, loss.lm(), GEO_LO_STEPS, GEO_LO_LAMBDA0, t);
+    lo_rescore(s, Est::consts(a, b), pts, P.n, loss, t);
     if (t == 0 && (s.score & LO_SCORE_MASK) < L.score) {
       Est::store(s, L);
       L.score = s.score & LO_SCORE_MASK;
@@ -260,11 +319,11 @@ __global__ void __launch_bounds__(RED, 1) lo_final_kernel(LoArgs<typename Est::B
   }
   __shared__ LoShared<Est> s;
   const auto pts = Est::points(a, b);
-  const float thr2 = Est::thr2(a, b);
+  const auto loss = Est::loss(a, b);
   Est::load(s, a, b, L, t);
   __syncthreads();
-  lo_refine(s, Est::consts(a, b), pts, P.n, (double)thr2, GEO_LO_FINAL_STEPS, GEO_LO_LAMBDA0, t);
-  lo_rescore(s, Est::consts(a, b), pts, P.n, thr2, t);
+  lo_refine(s, Est::consts(a, b), pts, P.n, loss.lm(), GEO_LO_FINAL_STEPS, GEO_LO_LAMBDA0, t);
+  lo_rescore(s, Est::consts(a, b), pts, P.n, loss, t);
   if (t == 0) s.take = (s.score & LO_SCORE_MASK) > L.score;
   __syncthreads();
   if (s.take) Est::restore(s, a, b, L, t);
@@ -282,7 +341,7 @@ __global__ void __launch_bounds__(RED, 1) lo_final_kernel(LoArgs<typename Est::B
 
 // Every LO estimator's launches, all fixed by (B, M, max_iters): prepare, the estimator's compaction kernel; per chunk
 // of GEO_CHUNK samples, geo_hyp_kernel (one CTA per pair, one thread per sample: the minimal solutions, fp32),
-// geo_score_kernel (count << 40 | MSAC score of every solution) and lo_chunk_kernel (one CTA per pair); then
+// geo_score_kernel (count << 40 | score of every solution) and lo_chunk_kernel (one CTA per pair); then
 // lo_final_kernel.
 template <class Est, class Base>
 int lo_launch(const Base& p, int32_t* num_lo, int64_t* cost, void* workspace, void (*prepare)(Base), void* stream_) {

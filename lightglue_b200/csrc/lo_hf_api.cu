@@ -4,8 +4,10 @@
 // orthonormal representation (U, V, sigma).  Both run on lo_common.cuh's schedule: geo_api.cu's compaction and
 // Hartley normalisation kernel prepares the pair; geo_hyp_kernel makes step 4's minimal solve, one model per sample
 // (r = 0); a local optimisation starts from the hypothesis solved again in double and runs LM on the truncated
-// transfer (H) or Sampson (F) cost.  Compiled with -fmad=false: oracle/lo_homography_oracle.py and
-// oracle/lo_fundamental_oracle.py take the same steps.
+// transfer (H) or Sampson (F) cost.  The MAGSAC++ estimators (MH1-MH8, MF1-MF8) are the same models and schedule
+// over lo_common.cuh's Magsac loss: the sigma-marginalised score, and LM weighted by its IRLS weights.  Compiled with
+// -fmad=false: oracle/lo_homography_oracle.py, oracle/lo_fundamental_oracle.py and oracle/magsac_oracle.py take the
+// same steps.
 #include <stdint.h>
 
 #include "geo_hf.cuh"
@@ -30,6 +32,32 @@ struct LoHfScore {
     return lo_term(geo_err(KIND, h, p[0]), thr2, w);
   }
 };
+
+// The MAGSAC++ estimators' arguments: GeoArgs and T^2
+struct MagsacArgs : GeoArgs {
+  float mt2;
+};
+
+__global__ void __launch_bounds__(1024) magsac_prepare_kernel(MagsacArgs a) { geo_prepare(a); }
+
+// The chunk's MH3 / MF3 scores, count << 40 | MAGSAC++ score
+template <int KIND>
+struct MagsacHfScore {
+  using Args = LoArgs<MagsacArgs>;
+  using Acc = unsigned long long;
+  static constexpr int SOLS = 1, NF = 9, K = 1, TILE = ::TILE;
+  static __device__ const GeoWs& ws(const Args& a) { return a.p.w; }
+  const float4* src[K];
+  unsigned long long* sums;
+  Magsac::Term q;
+  __device__ MagsacHfScore(const Args& a, const GeoPair&, int b)
+      : src{a.p.w.pts + (long)b * a.p.M}, sums(a.l.acc), q(Magsac{a.p.thr2, a.p.mt2}.term()) {}
+  __device__ unsigned long long term(const float* h, const float4* p) const { return q(geo_err(KIND, h, p[0])); }
+};
+
+// The loss of each argument type: MSAC at thr2 for LO-RANSAC, MAGSAC++ at mt2 (counting at thr2) for MAGSAC++
+__device__ __forceinline__ Msac hf_loss(const GeoArgs& p) { return {p.thr2}; }
+__device__ __forceinline__ Magsac hf_loss(const MagsacArgs& p) { return {p.thr2, p.mt2}; }
 
 // T1^-1 X T0 (H) or (T1^T X) T0 (F), unscaled: the first half of denormalise
 template <int KIND>
@@ -66,18 +94,18 @@ __device__ void householder_basis(const double* Hn, double (*B)[9]) {
   }
 }
 
-// The schedule hooks of the homography and the fundamental matrix (lo_common.cuh), Model one of the two: L.model is the
-// scaled pixel model, the LM start Model::start of it
-template <class Model>
+// The schedule hooks of the homography and the fundamental matrix (lo_common.cuh), Model one of the two and Base its
+// arguments (GeoArgs or MagsacArgs): L.model is the scaled pixel model, the LM start Model::start of it
+template <class Model, class B>
 struct HfLo {
-  using Base = GeoArgs;
-  using Args = LoArgs<GeoArgs>;
+  using Base = B;
+  using Args = LoArgs<B>;
   using Solver = HfSolver;
   static constexpr int SOLS = 1;
 
   static __device__ const float4* points(const Args& a, int b) { return a.p.w.pts + (long)b * a.p.M; }
   static __device__ const GeoPair& consts(const Args& a, int b) { return a.p.w.pair[b]; }
-  static __device__ float thr2(const Args& a, int) { return a.p.thr2; }
+  static __device__ auto loss(const Args& a, int) { return hf_loss(a.p); }
 
   // LH4 / LF4: hypothesis h solved again in double
   static __device__ void seed(LoShared<Model>& s, const Args& a, int b, unsigned hr, long, LoPair& L, int t) {
@@ -123,18 +151,35 @@ struct HfLo {
   }
 };
 
-// The homography for lo_common.cuh's LM loop, re-score and schedule: x = Hn, the unit-norm normalised model (header
-// step LH7)
-struct HomographyLo : HfLo<HomographyLo> {
-  static constexpr int KIND = GEO_HOMOGRAPHY, S = 4, DOF = 8, TERMS = 45, GROUP = 15, NP = 9, NF = 9;
+// The policies of a loss: MSAC on GeoArgs with LoHfScore, MAGSAC++ on MagsacArgs with MagsacHfScore
+template <class Loss>
+struct HfLoss;
+template <>
+struct HfLoss<Msac> {
+  using Base = GeoArgs;
+  template <int KIND>
   using Score = LoHfScore<KIND>;
+};
+template <>
+struct HfLoss<Magsac> {
+  using Base = MagsacArgs;
+  template <int KIND>
+  using Score = MagsacHfScore<KIND>;
+};
+
+// The homography for lo_common.cuh's LM loop, re-score and schedule over Loss, Self the estimator: x = Hn, the
+// unit-norm normalised model (header steps LH7 and MH7)
+template <class Self, class Loss>
+struct HomographyModel : HfLo<Self, typename HfLoss<Loss>::Base> {
+  static constexpr int KIND = GEO_HOMOGRAPHY, S = 4, DOF = 8, TERMS = 45, GROUP = 15, NP = 9, NF = 9;
+  using Score = typename HfLoss<Loss>::template Score<KIND>;
   struct Scratch {
     double basis[DOF][9];     // tangent basis at the model being summed or updated
     double Hu[9], G[DOF][9];  // T1^-1 Hn T0 and its derivatives along the basis
   };
 
   // Hn = T1 H T0^-1 at unit Frobenius norm of a pixel H; thread 0 only
-  static __device__ void start(LoShared<HomographyLo>& s, const GeoPair& P, const double* H) {
+  static __device__ void start(LoShared<Self>& s, const GeoPair& P, const double* H) {
     const double T1[9] = {P.s1, 0.0, -(P.s1 * P.cx1), 0.0, P.s1, -(P.s1 * P.cy1), 0.0, 0.0, 1.0};
     const double r = 1.0 / P.s0;
     const double T0i[9] = {r, 0.0, P.cx0, 0.0, r, P.cy0, 0.0, 0.0, 1.0};
@@ -147,8 +192,8 @@ struct HomographyLo : HfLo<HomographyLo> {
     for (int i = 0; i < 9; ++i) s.x[i] = s.x[i] / f;
   }
 
-  static __device__ void terms(LoShared<HomographyLo>& s, const GeoPair& P, const double* X, const float4* pts, int n,
-                               double thr2, double* out, int tid) {
+  static __device__ void terms(LoShared<Self>& s, const GeoPair& P, const double* X, const float4* pts, int n,
+                               double scale, double* out, int tid) {
     if (tid == 0) {
       householder_basis(X, s.m.basis);
       to_pixels<KIND>(P, X, s.m.Hu);
@@ -166,8 +211,9 @@ struct HomographyLo : HfLo<HomographyLo> {
       const double px = ((h[0] * x + h[1] * y) + h[2]) * w, py = ((h[3] * x + h[4] * y) + h[5]) * w;
       const double dx = u - px, dy = v - py;
       const double err = dx * dx + dy * dy;
-      const bool in = err < thr2;
-      acc[TERMS - 1] = acc[TERMS - 1] + (in ? err : thr2);
+      double cost, wt;
+      const bool in = Loss::point(scale, err, cost, wt);
+      acc[TERMS - 1] = acc[TERMS - 1] + cost;
       if (!in) continue;
       double jx[DOF], jy[DOF];
 #pragma unroll
@@ -182,15 +228,15 @@ struct HomographyLo : HfLo<HomographyLo> {
 #pragma unroll
       for (int i = 0; i < DOF; ++i)
 #pragma unroll
-        for (int j = i; j < DOF; ++j, ++e) acc[e] = acc[e] + (jx[i] * jx[j] + jy[i] * jy[j]);
+        for (int j = i; j < DOF; ++j, ++e) acc[e] = acc[e] + Loss::weigh(wt, jx[i] * jx[j] + jy[i] * jy[j]);
 #pragma unroll
-      for (int i = 0; i < DOF; ++i) acc[36 + i] = acc[36 + i] + (jx[i] * dx + jy[i] * dy);
+      for (int i = 0; i < DOF; ++i) acc[36 + i] = acc[36 + i] + Loss::weigh(wt, jx[i] * dx + jy[i] * dy);
     }
     lo_tree_sums<TERMS, GROUP>(acc, s.red, out, tid);
   }
 
   // X' = normalize(X + sum_k d_k basis_k), the basis taken at X
-  static __device__ void update(LoShared<HomographyLo>& s, const double* X, const double* d, double* out) {
+  static __device__ void update(LoShared<Self>& s, const double* X, const double* d, double* out) {
     householder_basis(X, s.m.basis);
     double f = 0.0;
     for (int i = 0; i < 9; ++i) {
@@ -203,12 +249,15 @@ struct HomographyLo : HfLo<HomographyLo> {
     for (int i = 0; i < 9; ++i) out[i] = out[i] / f;
   }
 
-  static __device__ void pixels(LoShared<HomographyLo>&, const GeoPair& P, const double* X, double* out) {
+  static __device__ void pixels(LoShared<Self>&, const GeoPair& P, const double* X, double* out) {
     denormalise(KIND, P, X, out);
   }
 
   static __device__ __forceinline__ float err(const float* h, float4 p) { return geo_err(KIND, h, p); }
 };
+
+struct HomographyLo : HomographyModel<HomographyLo, Msac> {};
+struct HomographyMagsac : HomographyModel<HomographyMagsac, Magsac> {};
 
 __device__ __forceinline__ void cross3(const double* a, const double* b, double* c) {
   c[0] = a[1] * b[2] - a[2] * b[1];
@@ -224,18 +273,19 @@ __device__ void compose(const double* x, double* Fn) {
     for (int b = 0; b < 3; ++b) Fn[a * 3 + b] = U[a * 3] * V[b * 3] + x[18] * U[a * 3 + 1] * V[b * 3 + 1];
 }
 
-// The fundamental matrix for lo_common.cuh's LM loop, re-score and schedule: x = U (0-8), V (9-17) and sig (18), the
-// orthonormal representation Fn = u1 v1^T + sig u2 v2^T of the normalised model, u_k, v_k columns of U, V (header step
-// LF7)
-struct FundamentalLo : HfLo<FundamentalLo> {
+// The fundamental matrix for lo_common.cuh's LM loop, re-score and schedule over Loss, Self the estimator: x = U (0-8),
+// V (9-17) and sig (18), the orthonormal representation Fn = u1 v1^T + sig u2 v2^T of the normalised model, u_k, v_k
+// columns of U, V (header steps LF7 and MF7)
+template <class Self, class Loss>
+struct FundamentalModel : HfLo<Self, typename HfLoss<Loss>::Base> {
   static constexpr int KIND = GEO_FUNDAMENTAL, S = 8, DOF = 7, TERMS = 36, GROUP = 18, NP = 19, NF = 9;
-  using Score = LoHfScore<KIND>;
+  using Score = typename HfLoss<Loss>::template Score<KIND>;
   struct Scratch {
     double Fu[9], G[DOF][9];  // T1^T Fn T0 and the directions at Fn in pixels
   };
 
   // x of a pixel F: Fn = (T1^-T F) T0^-1, then U, V and sig by step 4's one-sided Jacobi; thread 0 only
-  static __device__ void start(LoShared<FundamentalLo>& s, const GeoPair& P, const double* F) {
+  static __device__ void start(LoShared<Self>& s, const GeoPair& P, const double* F) {
     const double r1 = 1.0 / P.s1, r0 = 1.0 / P.s0;
     const double T1it[9] = {r1, 0.0, 0.0, 0.0, r1, 0.0, P.cx1, P.cy1, 1.0};
     const double T0i[9] = {r0, 0.0, P.cx0, 0.0, r0, P.cy0, 0.0, 0.0, 1.0};
@@ -276,8 +326,8 @@ struct FundamentalLo : HfLo<FundamentalLo> {
     s.x[18] = s2 / s1;
   }
 
-  static __device__ void terms(LoShared<FundamentalLo>& s, const GeoPair& P, const double* X, const float4* pts, int n,
-                               double thr2, double* out, int tid) {
+  static __device__ void terms(LoShared<Self>& s, const GeoPair& P, const double* X, const float4* pts, int n,
+                               double scale, double* out, int tid) {
     if (tid == 0) {
       double Fn[9], D[9];
       compose(X, Fn);
@@ -312,8 +362,9 @@ struct FundamentalLo : HfLo<FundamentalLo> {
       const double b0 = (f[0] * u + f[3] * v) + f[6], b1 = (f[1] * u + f[4] * v) + f[7];
       const double den = ((a0 * a0 + a1 * a1) + b0 * b0) + b1 * b1;
       const double err = (d * d) / den;
-      const bool in = err < thr2;
-      acc[TERMS - 1] = acc[TERMS - 1] + (in ? err : thr2);
+      double cost, wt;
+      const bool in = Loss::point(scale, err, cost, wt);
+      acc[TERMS - 1] = acc[TERMS - 1] + cost;
       if (!in) continue;
       const double sq = sqrt(den), r = d / sq;
       double J[DOF];
@@ -331,15 +382,15 @@ struct FundamentalLo : HfLo<FundamentalLo> {
 #pragma unroll
       for (int i = 0; i < DOF; ++i)
 #pragma unroll
-        for (int j = i; j < DOF; ++j, ++e) acc[e] = acc[e] + J[i] * J[j];
+        for (int j = i; j < DOF; ++j, ++e) acc[e] = acc[e] + Loss::weigh(wt, J[i] * J[j]);
 #pragma unroll
-      for (int i = 0; i < DOF; ++i) acc[28 + i] = acc[28 + i] + J[i] * r;
+      for (int i = 0; i < DOF; ++i) acc[28 + i] = acc[28 + i] + Loss::weigh(wt, J[i] * r);
     }
     lo_tree_sums<TERMS, GROUP>(acc, s.red, out, tid);
   }
 
   // U' = Q(d0..2) U, V' = Q(d3..5) V, sig' = sig + d6
-  static __device__ void update(LoShared<FundamentalLo>&, const double* X, const double* d, double* out) {
+  static __device__ void update(LoShared<Self>&, const double* X, const double* d, double* out) {
     double Q[9];
     quat_rotation(d, Q);
     mm3(Q, X, out);
@@ -348,7 +399,7 @@ struct FundamentalLo : HfLo<FundamentalLo> {
     out[18] = X[18] + d[6];
   }
 
-  static __device__ void pixels(LoShared<FundamentalLo>&, const GeoPair& P, const double* X, double* out) {
+  static __device__ void pixels(LoShared<Self>&, const GeoPair& P, const double* X, double* out) {
     double Fn[9];
     compose(X, Fn);
     denormalise(KIND, P, Fn, out);
@@ -357,15 +408,20 @@ struct FundamentalLo : HfLo<FundamentalLo> {
   static __device__ __forceinline__ float err(const float* h, float4 p) { return geo_err(KIND, h, p); }
 };
 
-// geo_homography_lo and geo_fundamental_lo: name for the error strings
-template <class Model>
-int lohf_estimate(const char* name, const GeoConfig* cfg, const GeoInputs* in, GeoLoOutputs* out,
-                  void* workspace, size_t workspace_bytes, void* stream_) {
+struct FundamentalLo : FundamentalModel<FundamentalLo, Msac> {};
+struct FundamentalMagsac : FundamentalModel<FundamentalMagsac, Magsac> {};
+
+// geo_homography_lo and geo_fundamental_lo (GeoArgs from a GeoConfig), geo_homography_magsac and
+// geo_fundamental_magsac (MagsacArgs from a GeoMagsacConfig): name for the error strings
+template <class Model, class Extra>
+int lohf_estimate(const char* name, const GeoConfig* cfg, const GeoInputs* in, GeoLoOutputs* out, void* workspace,
+                  size_t workspace_bytes, void* stream_, typename Model::Base g, void (*prepare)(typename Model::Base),
+                  Extra extra) {
   int rc = geo_check_config(name, cfg, in, out, GEO_LO_MAX_MATCHES, [&] {
     return cfg->model == Model::KIND          ? nullptr
            : Model::KIND == GEO_HOMOGRAPHY ? "model must be GEO_HOMOGRAPHY"
                                            : "model must be GEO_FUNDAMENTAL";
-  }, geo_no_check);
+  }, extra);
   if (rc == GEO_RUN) {
     const GeoOutputs& o = out->geo;
     rc = geo_check_buffers(name, in, {o.model, o.num_inliers, o.success, o.best_hypothesis, o.num_hypotheses,
@@ -373,7 +429,6 @@ int lohf_estimate(const char* name, const GeoConfig* cfg, const GeoInputs* in, G
                            workspace, workspace_bytes, lo_workspace_bytes<Model>(in->B, in->M));
   }
   if (rc != GEO_RUN) return rc;
-  GeoArgs g{};
   g.B = in->B; g.M = in->M; g.N = in->N;
   g.kind = Model::KIND;
   g.s = Model::S;
@@ -384,7 +439,30 @@ int lohf_estimate(const char* name, const GeoConfig* cfg, const GeoInputs* in, G
   g.confidence = cfg->confidence;
   g.kpts0 = in->kpts0; g.kpts1 = in->kpts1; g.matches0 = in->matches0;
   g.out = out->geo;
-  return lo_launch<Model>(g, out->num_local_optimizations, out->cost, workspace, geo_prepare_kernel, stream_);
+  return lo_launch<Model>(g, out->num_local_optimizations, out->cost, workspace, prepare, stream_);
+}
+
+template <class Model>
+int lohf_lo(const char* name, const GeoConfig* cfg, const GeoInputs* in, GeoLoOutputs* out, void* workspace,
+            size_t workspace_bytes, void* stream) {
+  return lohf_estimate<Model>(name, cfg, in, out, workspace, workspace_bytes, stream, GeoArgs{}, geo_prepare_kernel,
+                              geo_no_check);
+}
+
+// The MAGSAC++ entry points: the checks of the LO ones, with max_threshold's at the place of distance() in
+// geo_check_config.  The carve is LO-RANSAC's (MagsacArgs holds the same GeoWs), so the workspace sizes are
+// geo_lo_homography_workspace_bytes' and geo_lo_fundamental_workspace_bytes'.
+template <class Model>
+int lohf_magsac(const char* name, const GeoMagsacConfig* cfg, const GeoInputs* in, GeoLoOutputs* out, void* workspace,
+                size_t workspace_bytes, void* stream) {
+  if (!cfg) return geo_error(name, "null argument");
+  const double T = cfg->max_threshold;
+  MagsacArgs g{};
+  g.mt2 = (float)(T * T);
+  return lohf_estimate<Model>(name, &cfg->geo, in, out, workspace, workspace_bytes, stream, g, magsac_prepare_kernel,
+                              [T]() -> const char* {
+                                return T > 0.0 && isfinite(T) ? nullptr : "max_threshold must be positive";
+                              });
 }
 
 }  // namespace
@@ -399,10 +477,20 @@ extern "C" size_t geo_lo_fundamental_workspace_bytes(int32_t B, int32_t M, int32
 
 extern "C" int geo_homography_lo(const GeoConfig* cfg, const GeoInputs* in, GeoLoOutputs* out, void* workspace,
                                  size_t workspace_bytes, void* stream) {
-  return lohf_estimate<HomographyLo>("geo_homography_lo", cfg, in, out, workspace, workspace_bytes, stream);
+  return lohf_lo<HomographyLo>("geo_homography_lo", cfg, in, out, workspace, workspace_bytes, stream);
 }
 
 extern "C" int geo_fundamental_lo(const GeoConfig* cfg, const GeoInputs* in, GeoLoOutputs* out, void* workspace,
                                   size_t workspace_bytes, void* stream) {
-  return lohf_estimate<FundamentalLo>("geo_fundamental_lo", cfg, in, out, workspace, workspace_bytes, stream);
+  return lohf_lo<FundamentalLo>("geo_fundamental_lo", cfg, in, out, workspace, workspace_bytes, stream);
+}
+
+extern "C" int geo_homography_magsac(const GeoMagsacConfig* cfg, const GeoInputs* in, GeoLoOutputs* out,
+                                     void* workspace, size_t workspace_bytes, void* stream) {
+  return lohf_magsac<HomographyMagsac>("geo_homography_magsac", cfg, in, out, workspace, workspace_bytes, stream);
+}
+
+extern "C" int geo_fundamental_magsac(const GeoMagsacConfig* cfg, const GeoInputs* in, GeoLoOutputs* out,
+                                      void* workspace, size_t workspace_bytes, void* stream) {
+  return lohf_magsac<FundamentalMagsac>("geo_fundamental_magsac", cfg, in, out, workspace, workspace_bytes, stream);
 }

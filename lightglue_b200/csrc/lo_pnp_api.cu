@@ -93,7 +93,7 @@ struct PnpLo {
     return {a.p.w.pts + (long)b * a.p.M, a.p.w.wld + (long)b * a.p.M, Cam::test(a.p, b)};
   }
   static __device__ typename Cam::Consts consts(const Args& a, int b) { return Cam::consts(a.p, b); }
-  static __device__ float thr2(const Args& a, int b) { return a.p.w.pair[b].thr2; }
+  static __device__ Msac loss(const Args& a, int b) { return {a.p.w.pair[b].thr2}; }
 
   // LA4: sample h re-solved in double, as the score's models were solved
   static __device__ void seed(LoShared<PnpLo>& s, const Args& a, int b, unsigned hr, long, LoPair& L, int t) {

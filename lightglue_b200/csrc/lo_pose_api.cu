@@ -176,7 +176,7 @@ struct PoseLo {
 
   static __device__ const float4* points(const Args& a, int b) { return a.p.w.pts + (long)b * a.p.M; }
   static __device__ const PosePair& consts(const Args& a, int b) { return a.p.w.pair[b]; }
-  static __device__ float thr2(const Args& a, int b) { return a.p.w.pair[b].thr2; }
+  static __device__ Msac loss(const Args& a, int b) { return {a.p.w.pair[b].thr2}; }
 
   // L4's start: P7's pose choice of the solution's E (lo_choose_pose, below)
   static __device__ void seed(LoShared<PoseLo>& s, const Args& a, int b, unsigned hr, long m, LoPair& L, int t);
@@ -193,7 +193,7 @@ struct PoseLo {
   static __device__ void restore(LoShared<PoseLo>& s, const Args& a, int b, const LoPair& L, int t) {
     load(s, a, b, L, t);
     __syncthreads();
-    lo_rescore(s, consts(a, b), points(a, b), a.p.w.pair[b].n, thr2(a, b), t);
+    lo_rescore(s, consts(a, b), points(a, b), a.p.w.pair[b].n, loss(a, b), t);
   }
 
   static __device__ void fail(const Args& a, int b, int t) {

@@ -1,10 +1,10 @@
 """Geometric verification on the GPU: batched RANSAC homography and fundamental-matrix, relative-pose,
 absolute-pose, affine and 3D rigid and similarity estimation on the matcher's output, each of the first four plain and
-LO-RANSAC (C ABI ``include/geometry_b200.h``, CUDA ``csrc/geo_api.cu``, ``csrc/lo_hf_api.cu``, ``csrc/pose_api.cu``,
+LO-RANSAC, and the first two MAGSAC++ as well (C ABI ``include/geometry_b200.h``, CUDA ``csrc/geo_api.cu``, ``csrc/lo_hf_api.cu``, ``csrc/pose_api.cu``,
 ``csrc/lo_pose_api.cu``, ``csrc/pnp_api.cu``, ``csrc/lo_pnp_api.cu``, ``csrc/affine_api.cu`` and
 ``csrc/rigid_api.cu``).
 
-All twelve functions take ``matches0`` [B, M] int64 exactly as ``LightGlue.forward``, ``PendingMatch.tensors`` and
+All fourteen functions take ``matches0`` [B, M] int64 exactly as ``LightGlue.forward``, ``PendingMatch.tensors`` and
 ``match_ragged`` give it (-1 or any index outside [0, N) is unmatched), run every pair of the batch in one call on the
 current stream, and return device tensors of fixed shapes without synchronising with the host, so a call can follow a
 matcher forward with no read-back in between, or be captured in a CUDA graph.  A match whose keypoint in either image,
@@ -19,7 +19,8 @@ entry positive), ``inliers`` [B, M] bool, ``num_inliers`` [B] int32, ``success``
 ``best_hypothesis`` [B] int32 (-1 without one) and ``num_hypotheses`` [B] int32.  A failed pair (fewer valid matches than
 the sample size, 4 or 8, or no non-degenerate hypothesis) has ``success`` False, a zero model and no inliers.
 ``find_homography_lo`` and ``find_fundamental_lo`` return the keys of ``find_homography`` and ``find_fundamental`` plus
-``num_local_optimizations`` and ``cost``; so do ``estimate_relative_pose_lo`` and ``estimate_absolute_pose_lo`` with
+``num_local_optimizations`` and ``cost``; so do ``find_homography_magsac`` and ``find_fundamental_magsac`` (MAGSAC++,
+``cv2.USAC_MAGSAC``), and ``estimate_relative_pose_lo`` and ``estimate_absolute_pose_lo`` with
 those of ``estimate_relative_pose`` and ``estimate_absolute_pose``.  ``estimate_affine_2d`` and
 ``estimate_affine_partial_2d`` return those of ``find_homography`` with ``A`` [B, 2, 3] in place of ``H``.
 ``estimate_rigid_3d`` and ``estimate_similarity_3d`` register matched 3D points (``cv2.estimateAffine3D`` with
@@ -83,9 +84,12 @@ def _run(entry: str, ws_entry: str, shapes: dict, device, b: int, m: int, max_it
 
 
 def _estimate(kind: int, key: str, kpts0, kpts1, matches0, threshold, max_iters, confidence, seed,
-              lo: bool = False) -> dict:
+              lo: bool = False, max_threshold=None) -> dict:
+    """Plain RANSAC, LO-RANSAC (lo) or MAGSAC++ (lo and a max_threshold)."""
     _check_inputs(kpts0, kpts1, matches0)
     _check_params(threshold, max_iters, confidence, seed)
+    if max_threshold is not None:
+        _check_params(max_threshold, max_iters, confidence, seed, "max_threshold", "a positive finite number of pixels")
     if lo and kpts0.shape[1] > _cabi.GEO_LO_MAX_MATCHES:
         raise ValueError(f"kpts0 {tuple(kpts0.shape)}: at most {_cabi.GEO_LO_MAX_MATCHES} rows per pair")
     device = kpts0.device
@@ -101,6 +105,8 @@ def _estimate(kind: int, key: str, kpts0, kpts1, matches0, threshold, max_iters,
 
     def make_args(out):
         cfg = _cabi.GeoConfig(_cabi.GEO_ABI_VERSION, kind, max_iters, seed, float(threshold), float(confidence))
+        if max_threshold is not None:
+            cfg = _cabi.GeoMagsacConfig(cfg, float(max_threshold))
         ins = _cabi.GeoInputs(b, m, n, k0.data_ptr(), k1.data_ptr(), m0.data_ptr())
         outs = _cabi.GeoOutputs(*(out[k].data_ptr() for k in list(shapes)[:6]))
         if lo:
@@ -110,7 +116,8 @@ def _estimate(kind: int, key: str, kpts0, kpts1, matches0, threshold, max_iters,
     if not lo:
         return _run("geo_estimate", "geo_workspace_bytes", shapes, device, b, m, max_iters, make_args)
     name = "homography" if kind == _cabi.GEO_HOMOGRAPHY else "fundamental"
-    return _run(f"geo_{name}_lo", f"geo_lo_{name}_workspace_bytes", shapes, device, b, m, max_iters, make_args)
+    entry = f"geo_{name}_lo" if max_threshold is None else f"geo_{name}_magsac"
+    return _run(entry, f"geo_lo_{name}_workspace_bytes", shapes, device, b, m, max_iters, make_args)
 
 
 def find_homography(kpts0: torch.Tensor, kpts1: torch.Tensor, matches0: torch.Tensor, ransac_reproj_threshold: float = 3.0,
@@ -164,6 +171,48 @@ def find_fundamental_lo(kpts0: torch.Tensor, kpts1: torch.Tensor, matches0: torc
     Failures are those of ``find_fundamental``, with ``num_local_optimizations`` and ``cost`` 0."""
     return _estimate(_cabi.GEO_FUNDAMENTAL, "F", kpts0, kpts1, matches0, ransac_reproj_threshold, max_iters, confidence,
                      seed, lo=True)
+
+
+def find_homography_magsac(kpts0: torch.Tensor, kpts1: torch.Tensor, matches0: torch.Tensor,
+                           ransac_reproj_threshold: float = 3.0, max_threshold: float = 7.5, max_iters: int = 2000,
+                           confidence: float = 0.995, seed: int = 0) -> dict:
+    """MAGSAC++ homography per pair (Barath et al., CVPR 2020; ``cv2.USAC_MAGSAC``): the samples and four-point
+    hypotheses of ``find_homography_lo``, scored by the MAGSAC++ loss marginalised over the noise scale, with local
+    optimisation by Levenberg-Marquardt reweighted by the same marginalisation, on the schedule of
+    ``find_homography_lo``.  Returns the keys of ``find_homography_lo``, ``cost`` being the final model's integer
+    MAGSAC++ score; failures are those of ``find_homography_lo``.
+
+    ``ransac_reproj_threshold`` keeps its meaning from every other estimator here: it sets ``inliers``,
+    ``num_inliers`` and the inlier count that drives the adaptive stop.  ``max_threshold`` is new: T = k * sigma_max
+    (k = 3.64, the square root of the 0.99 quantile of chi-square with 4 degrees of freedom) is the scale of the loss
+    and the weights, so a point whose error is T or more costs as an outlier and has weight 0.  The default of 7.5 px
+    follows OpenCV's USAC_MAGSAC, whose accuracy does not move with the user's threshold.  Neither does this one's: on
+    the synthetic scenes of tests/test_magsac_oracle.py the model is the same at every user threshold from 1 to 6 px,
+    and the median homography error moves by 1.5x over T from 5 to 15 px (lower at larger T under 1.5 px of noise).
+    At most 2**20 - 1 rows of ``matches0`` per pair."""
+    return _estimate(_cabi.GEO_HOMOGRAPHY, "H", kpts0, kpts1, matches0, ransac_reproj_threshold, max_iters, confidence,
+                     seed, lo=True, max_threshold=max_threshold)
+
+
+def find_fundamental_magsac(kpts0: torch.Tensor, kpts1: torch.Tensor, matches0: torch.Tensor,
+                            ransac_reproj_threshold: float = 3.0, max_threshold: float = 7.5, max_iters: int = 1000,
+                            confidence: float = 0.99, seed: int = 0) -> dict:
+    """MAGSAC++ fundamental matrix per pair (``cv2.USAC_MAGSAC``): the samples and eight-point hypotheses of
+    ``find_fundamental_lo``, scored by the MAGSAC++ loss of the epipolar distance, with local optimisation of a rank-2
+    F by Levenberg-Marquardt on the Sampson error reweighted by the same marginalisation, on the schedule of
+    ``find_fundamental_lo``.  Returns the keys of ``find_fundamental_lo``, ``cost`` being the final model's integer
+    MAGSAC++ score; failures are those of ``find_fundamental_lo``.
+
+    ``ransac_reproj_threshold`` keeps its meaning from every other estimator here: it sets ``inliers``,
+    ``num_inliers`` and the inlier count that drives the adaptive stop.  ``max_threshold`` is new: T = k * sigma_max
+    (k = 3.64, the square root of the 0.99 quantile of chi-square with 4 degrees of freedom) is the scale of the loss
+    and the weights, so a point whose error is T or more costs as an outlier and has weight 0.  The default of 7.5 px
+    follows OpenCV's USAC_MAGSAC, whose accuracy does not move with the user's threshold.  Neither does this one's: on
+    the synthetic scenes of tests/test_magsac_oracle.py the model is the same at every user threshold from 1 to 6 px,
+    and the median homography error moves by 1.5x over T from 5 to 15 px (lower at larger T under 1.5 px of noise).
+    At most 2**20 - 1 rows of ``matches0`` per pair."""
+    return _estimate(_cabi.GEO_FUNDAMENTAL, "F", kpts0, kpts1, matches0, ransac_reproj_threshold, max_iters, confidence,
+                     seed, lo=True, max_threshold=max_threshold)
 
 
 def _intrinsics(name: str, K, b: int, device) -> torch.Tensor:

@@ -3,12 +3,13 @@
 Prints one JSON line:
   * the card's name and power limit, read in this run;
   * GPU ms per batch (CUDA events) for find_homography and find_fundamental, and for their LO-RANSAC variants
-    find_homography_lo and find_fundamental_lo ("lo_adaptive", "lo_full"), at B pairs of M putative matches, inlier
+    find_homography_lo and find_fundamental_lo ("lo_adaptive", "lo_full") and their MAGSAC++ variants
+    find_homography_magsac and find_fundamental_magsac ("magsac_adaptive", "magsac_full"), at B pairs of M putative matches, inlier
     ratios 0.8 / 0.5 / 0.3, with OpenCV's adaptive stopping ("adaptive") and with confidence 1 ("full", every
     hypothesis);
   * OpenCV on the host for the same pairs, one after another and in a thread pool (null without cv2), and
     cv2.findHomography / cv2.findFundamentalMat(USAC_ACCURATE), the LO-RANSAC the LO variants are compared with
-    ("opencv_usac_accurate");
+    ("opencv_usac_accurate"), and USAC_MAGSAC, which the MAGSAC++ variants follow ("opencv_usac_magsac");
   * pairs/s of LightGlue (bf16x3, N = 2048, synthetic weights) alone and followed by find_fundamental,
     find_homography_lo or find_fundamental_lo on one stream, the runs alternated.
 The scenes come from oracle/geometry_synth.py (0.5 px noise, 640x480); nothing is written to disk.
@@ -29,12 +30,14 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 from lightglue_b200 import LightGlue, synth  # noqa: E402
-from lightglue_b200.geometry import (find_fundamental, find_fundamental_lo, find_homography,  # noqa: E402
-                                     find_homography_lo)
+from lightglue_b200.geometry import (find_fundamental, find_fundamental_lo,  # noqa: E402
+                                     find_fundamental_magsac, find_homography, find_homography_lo,
+                                     find_homography_magsac)
 from oracle import geometry_synth as gs  # noqa: E402
 
 DEFAULTS = {"H": (find_homography, 2000, 0.995), "F": (find_fundamental, 1000, 0.99)}
 LO = {"H": find_homography_lo, "F": find_fundamental_lo}
+MAGSAC = {"H": find_homography_magsac, "F": find_fundamental_magsac}
 
 
 def gpu_info() -> dict:
@@ -60,21 +63,23 @@ def time_gpu(fn, reps: int) -> float:
     return start.elapsed_time(stop) / reps
 
 
-def opencv_times(key, k0, k1, m0, threads, usac=False):
+def opencv_times(key, k0, k1, m0, threads, usac=None):
     try:
         import cv2
     except ImportError:
         return None
     cv2.setNumThreads(1)
     iters, conf = DEFAULTS[key][1:]
+    method = {None: cv2.RANSAC if key == "H" else cv2.FM_RANSAC, "accurate": cv2.USAC_ACCURATE,
+              "magsac": cv2.USAC_MAGSAC}[usac]
 
     def one(b):
         v = m0[b] >= 0
         a, c = k0[b][v], k1[b][m0[b][v]]
         if key == "H":
-            cv2.findHomography(a, c, cv2.USAC_ACCURATE if usac else cv2.RANSAC, 3.0, maxIters=iters, confidence=conf)
+            cv2.findHomography(a, c, method, 3.0, maxIters=iters, confidence=conf)
         else:
-            cv2.findFundamentalMat(a, c, cv2.USAC_ACCURATE if usac else cv2.FM_RANSAC, 3.0, conf, iters)
+            cv2.findFundamentalMat(a, c, method, 3.0, conf, iters)
 
     t = time.perf_counter()
     for b in range(len(m0)):
@@ -109,15 +114,16 @@ def main() -> None:
                 row[mode] = {"gpu_ms": round(time_gpu(lambda: fn(t0, t1, tm, confidence=c), args.reps), 3),
                              "mean_hypotheses": float(out["num_hypotheses"].float().mean()),
                              "mean_inliers": float(out["num_inliers"].float().mean())}
-                lo = LO[key]
-                out = lo(t0, t1, tm, confidence=c)
-                row["lo_" + mode] = {
-                    "gpu_ms": round(time_gpu(lambda: lo(t0, t1, tm, confidence=c), args.reps), 3),
-                    "mean_hypotheses": float(out["num_hypotheses"].float().mean()),
-                    "mean_inliers": float(out["num_inliers"].float().mean()),
-                    "mean_local_optimizations": float(out["num_local_optimizations"].float().mean())}
+                for name, lo in (("lo_", LO[key]), ("magsac_", MAGSAC[key])):
+                    out = lo(t0, t1, tm, confidence=c)
+                    row[name + mode] = {
+                        "gpu_ms": round(time_gpu(lambda: lo(t0, t1, tm, confidence=c), args.reps), 3),
+                        "mean_hypotheses": float(out["num_hypotheses"].float().mean()),
+                        "mean_inliers": float(out["num_inliers"].float().mean()),
+                        "mean_local_optimizations": float(out["num_local_optimizations"].float().mean())}
             row["opencv"] = opencv_times(key, k0, k1, m0, threads)
-            row["opencv_usac_accurate"] = opencv_times(key, k0, k1, m0, threads, usac=True)
+            row["opencv_usac_accurate"] = opencv_times(key, k0, k1, m0, threads, usac="accurate")
+            row["opencv_usac_magsac"] = opencv_times(key, k0, k1, m0, threads, usac="magsac")
             res["ransac"][f"{key}_inliers{inl}"] = row
     # the matcher alone, and followed by find_fundamental on its device output (no host read-back in between)
     data, _ = synth.make_pair(2048, b=args.batch, seed=7)
