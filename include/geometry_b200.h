@@ -511,6 +511,57 @@
  *      ru*ru + rv*rv < (double)thr2.  The parametrisation, schedule and sums are A7's and LA7's.
  * AD4. Outputs, failures and diagnostics as A8 and LA8, with AD2's test in place of A5's.
  *
+ * Fisheye camera (geo_fisheye_undistort_points, geo_fisheye_distort_points; oracle/fisheye_oracle.py restates it bit
+ * for bit): cv2.fisheye's equidistant (Kannala-Brandt) model, COLMAP's OPENCV_FISHEYE.  The coefficients are D = (k1, k2,
+ * k3, k4), exactly 4; the skew s = K[0][1] is OpenCV's alpha = s / fx.  Expressions evaluate left to right as written;
+ * every multiply and add rounds on its own.  No step calls a library transcendental: atan and tan are FE1's.
+ *
+ * FE1. atan and tan, a range reduction and an odd polynomial p = t + t*(z*Q), z = t*t, Q = q0 + q1*z + ... by Horner
+ *      from the last coefficient (acc = q_last, then acc = acc*z + q_i).  The constants and coefficients are the
+ *      hexadecimal literals of lightglue_b200/csrc/fisheye_poly.h (generated by oracle/make_fisheye_poly.py).
+ *      atan in double, a = |r|: when a > FE_TAN_3PI_8, FE_PI_2_HI + (FE_PI_2_LO + p(-1.0 / a)); else when
+ *      a > FE_TAN_PI_8, FE_PI_4_HI + (FE_PI_4_LO + p((a - 1.0) / (a + 1.0))); else p(a); Q = FE_ATAN_D; negated for
+ *      r < 0.  atan in float: when a > 1, FE_PI_2_HI_F + (FE_PI_2_LO_F + p(-1 / a)), else p(a); Q = FE_ATAN_F; negated
+ *      for r < 0.  tan in double: n = rint(x * FE_2_PI) (ties to even), y = ((x - n*FE_PIO2_1) - n*FE_PIO2_2) -
+ *      n*FE_PIO2_3, p(y) with Q = FE_TAN_D, and -1.0 / p when n is odd (floor(n * 0.5) != n * 0.5).  On [0, 1e6]
+ *      the double atan is within 2 ulp of the correctly rounded value and the float one within 1 ulp; the double tan
+ *      within 2 ulp on [0, pi/2).
+ * FE2. Distort a normalised point (x, y), cv2.fisheye.distortPoints' model: r = sqrt(x*x + y*y), th = atan(r),
+ *      t2 = th*th, t4 = t2*t2, t6 = t4*t2, t8 = t4*t4, thd = th*(1 + k1*t2 + k2*t4 + k3*t6 + k4*t8), cdist = thd / r
+ *      when r > 1e-8, else 1; (xd, yd) = (cdist*x, cdist*y).  geo_fisheye_distort_points maps a pixel to (x, y) by
+ *      D1's rule (skew included), FE2, and the pixel (fx*xd + s*yd + cx, fy*yd + cy).
+ * FE3. Undistort a pixel (u, v), as cv2.fisheye.undistortPoints(pts, K, D, P=K, criteria) runs it: (x0, y0) by D2's
+ *      rule (OpenCV ignores the skew on input; with s = 0 the two agree); thd = sqrt(x0*x0 + y0*y0), clamped to
+ *      [-FE_PI_2_HI, FE_PI_2_HI]; th = thd.  With eps > 0 and |thd| <= eps the point converges with scale 0.  Otherwise
+ *      up to max_iters times: t2 = th*th, t4 = t2*t2, t6 = t4*t2, t8 = t6*t2, a2 = k1*t2, a4 = k2*t4, a6 = k3*t6,
+ *      a8 = k4*t8, fix = (th*(1 + a2 + a4 + a6 + a8) - thd) / (1 + 3*a2 + 5*a4 + 7*a6 + 9*a8), th = th - fix, and with
+ *      eps > 0 the point converges and stops once |fix| < eps; then scale = tan(th) / thd.  The output is
+ *      (scale*x0, scale*y0) through K as D2's.  A point fails when th and thd have opposite signs, or when eps > 0
+ *      and it did not converge; its output row is NaN where OpenCV writes (-1e6, -1e6).  With eps = 0 the principal
+ *      point is 0 / 0, NaN as in OpenCV.  eps is in radians of theta, not pixels.  The clamp is OpenCV's: a point
+ *      whose thd exceeds pi/2 (beyond the model's 180 degree field) comes back at a plausible but wrong angle.
+ * FE4. Validity.  K is valid as P1; the coefficients are exactly 4, all finite.  An invalid K or coefficients, a
+ *      non-finite input pixel or a failing FE3 give a NaN output row.  Inputs and outputs as D3.
+ *
+ * Fisheye absolute pose (geo_absolute_pose_fisheye, geo_absolute_pose_lo_fisheye; oracle/fisheye_oracle.py restates
+ * them bit for bit): cv2.solvePnPRansac with the fisheye camera, with the test and the refinement in fisheye pixels.
+ * The minimal solutions see undistorted bearings; everything that scores or refines sees the fisheye image.  Each step
+ * is A1-A8 (LA1-LA8 for the LO estimator) with these changes:
+ *
+ * AE1. Compaction as A1, with FE3's (x, y) at GEO_FISHEYE_ITERS and GEO_FISHEYE_EPS (cv2.fisheye.solvePnPRansac's
+ *      default criteria), rounded to float, as the P3P input.  A match whose FE3 fails is invalid at compaction, as a
+ *      NaN keypoint is: it is not counted in n, never sampled and never an inlier.  Coefficients that fail FE4 fail the
+ *      pair as an invalid K0 does (A8).
+ * AE2. The inlier test as AD2 with FE2 in fp32 in place of D1: the float atan of FE1, K0 and D rounded to float.  An
+ *      inlier has w > 0 and du*du + dv*dv < (float)(threshold * threshold); the LO estimator's MSAC term reads this
+ *      error, +inf behind the camera.
+ * AE3. Levenberg-Marquardt as AD3 with FE2 in double in place of D1, and FE2's Jacobian at (a, b): r2 = a*a + b*b,
+ *      r = sqrt(r2), th, t2..t8 and thd as FE2; when r > 1e-8, c = thd / r, dd = 1.0 + 3.0*k1*t2 + 5.0*k2*t4 +
+ *      7.0*k3*t6 + 9.0*k4*t8 (d thd / d th), g = ((dd / (1.0 + r2) - c) / r) / r ((dc/dr) / r, with d th / d r =
+ *      1 / (1 + r2)); else c = 1.0, g = 0.0.  ga = g*a, gb = g*b, J00 = c + ga*a, J01 = ga*b, J10 = gb*a,
+ *      J11 = c + gb*b, chained onto A7's rows as AD3 chains D1's.
+ * AE4. Outputs, failures and diagnostics as A8 and LA8, with AE2's test in place of A5's.
+ *
  * 3D rigid and similarity transforms (geo_estimate_rigid; oracle/rigid_oracle.py restates it bit for bit): x1 = scale
  * R x0 + t between matched 3D points, with R a proper rotation and scale = 1 (GEO_RIGID_3D, SE(3)) or scale > 0
  * (GEO_SIMILARITY_3D, Sim(3)).  kpts0 and kpts1 of GeoInputs hold [B, M, 3] and [B, N, 3] points.  Expressions
@@ -796,7 +847,7 @@ LG_API int geo_distort_points(const GeoCameraConfig* cfg, const GeoCameraInputs*
 
 typedef struct GeoPnpDistInputs {
   GeoPnpInputs pnp;        /* as geo_absolute_pose's */
-  int32_t num_dist;        /* 4, 5, 8 or 12 */
+  int32_t num_dist;        /* 4, 5, 8 or 12; 4 for the fisheye entry points */
   const double* dist0;     /* [B, num_dist] distortion coefficients of image 0 */
 } GeoPnpDistInputs;
 
@@ -806,6 +857,25 @@ LG_API int geo_absolute_pose_dist(const GeoPnpConfig* cfg, const GeoPnpDistInput
                                   void* workspace, size_t workspace_bytes, void* stream);
 LG_API int geo_absolute_pose_lo_dist(const GeoPnpConfig* cfg, const GeoPnpDistInputs* in, GeoLoPnpOutputs* out,
                                      void* workspace, size_t workspace_bytes, void* stream);
+
+#define GEO_FISHEYE_ITERS 10 /* FE3's iterations in cv2.fisheye's default criteria */
+#define GEO_FISHEYE_EPS 1e-8 /* FE3's stop in those criteria, radians of theta */
+
+/* Fisheye camera (steps FE1-FE4), on the structs of the lens distortion: cfg->num_dist must be 4, cfg->max_iters is
+ * FE3's in [0, GEO_UNDISTORT_MAX_ITERS] and cfg->eps FE3's stop in radians of theta (not pixels), finite and >= 0
+ * (0: none, OpenCV's COUNT-only criterion); geo_fisheye_distort_points ignores both.  One launch, B <= 65535, no
+ * workspace. */
+LG_API int geo_fisheye_undistort_points(const GeoCameraConfig* cfg, const GeoCameraInputs* in, GeoCameraOutputs* out,
+                                        void* stream);
+LG_API int geo_fisheye_distort_points(const GeoCameraConfig* cfg, const GeoCameraInputs* in, GeoCameraOutputs* out,
+                                      void* stream);
+
+/* Fisheye absolute pose (steps AE1-AE4): in->num_dist must be 4; the workspaces are geo_pnp_workspace_bytes' and
+ * geo_lo_pnp_workspace_bytes'. */
+LG_API int geo_absolute_pose_fisheye(const GeoPnpConfig* cfg, const GeoPnpDistInputs* in, GeoPnpOutputs* out,
+                                     void* workspace, size_t workspace_bytes, void* stream);
+LG_API int geo_absolute_pose_lo_fisheye(const GeoPnpConfig* cfg, const GeoPnpDistInputs* in, GeoLoPnpOutputs* out,
+                                        void* workspace, size_t workspace_bytes, void* stream);
 
 #define GEO_RIGID_3D 5
 #define GEO_SIMILARITY_3D 6

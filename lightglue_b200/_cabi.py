@@ -29,6 +29,7 @@ GEO_LO_QSCALE, GEO_LO_MAX_MATCHES = 65536, (1 << 20) - 1
 GEO_MAGSAC_KNOTS, GEO_MAGSAC_K = 1024, 3.6437211935036444
 GEO_AFFINE, GEO_AFFINE_PARTIAL, GEO_AFFINE_MAX_REFINE = 3, 4, 100
 GEO_CAMERA_FLOAT32, GEO_CAMERA_FLOAT64, GEO_UNDISTORT_MAX_ITERS = 0, 1, 1000
+GEO_FISHEYE_ITERS, GEO_FISHEYE_EPS = 10, 1e-8
 GEO_RIGID_3D, GEO_SIMILARITY_3D = 5, 6
 NN_ABI_VERSION = 1  # include/nn_b200.h
 NN_MIN_DIM, NN_MAX_DIM, NN_GROUP_ROWS = 64, 512, 32768
@@ -361,6 +362,14 @@ GEO_PROTOTYPES = {  # include/geometry_b200.h
                                          C.POINTER(GeoPnpOutputs), _VP, _SZ, _VP]),
     "geo_absolute_pose_lo_dist": (C.c_int, [C.POINTER(GeoPnpConfig), C.POINTER(GeoPnpDistInputs),
                                             C.POINTER(GeoLoPnpOutputs), _VP, _SZ, _VP]),
+    "geo_fisheye_undistort_points": (C.c_int, [C.POINTER(GeoCameraConfig), C.POINTER(GeoCameraInputs),
+                                               C.POINTER(GeoCameraOutputs), _VP]),
+    "geo_fisheye_distort_points": (C.c_int, [C.POINTER(GeoCameraConfig), C.POINTER(GeoCameraInputs),
+                                             C.POINTER(GeoCameraOutputs), _VP]),
+    "geo_absolute_pose_fisheye": (C.c_int, [C.POINTER(GeoPnpConfig), C.POINTER(GeoPnpDistInputs),
+                                            C.POINTER(GeoPnpOutputs), _VP, _SZ, _VP]),
+    "geo_absolute_pose_lo_fisheye": (C.c_int, [C.POINTER(GeoPnpConfig), C.POINTER(GeoPnpDistInputs),
+                                               C.POINTER(GeoLoPnpOutputs), _VP, _SZ, _VP]),
     "geo_rigid_workspace_bytes": (_SZ, [_I32, _I32, _I32]),
     "geo_estimate_rigid": (C.c_int, [C.POINTER(GeoConfig), C.POINTER(GeoInputs), C.POINTER(GeoRigidOutputs), _VP,
                                      _SZ, _VP]),

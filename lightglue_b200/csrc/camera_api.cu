@@ -1,7 +1,10 @@
-// Batched undistortion and distortion of keypoints under OpenCV's lens model (include/geometry_b200.h, steps D1-D3):
-// one thread per point, computed in double from float or double pixels.  One launch per call, fixed by (B, N), with no
-// host synchronisation.  Compiled with -fmad=false: oracle/camera_oracle.py takes the same steps.
+// Batched undistortion and distortion of keypoints under OpenCV's lens model (include/geometry_b200.h, steps D1-D3)
+// and its fisheye model (FE1-FE4): one thread per point, computed in double from float or double pixels.  One launch
+// per call, fixed by (B, N), with no host synchronisation.  Compiled with -fmad=false: oracle/camera_oracle.py and
+// oracle/fisheye_oracle.py take the same steps.
 #include <stdint.h>
+
+#include <type_traits>
 
 #include "camera_common.cuh"
 #include "geo_common.cuh"
@@ -19,9 +22,9 @@ struct CamArgs {
   void* out;
 };
 
-// D2 (undistort) or D1 through K (distort) of point i of pair b; NaN for an invalid K or coefficients, or a non-finite
-// input pixel
-template <class T, bool UNDISTORT>
+// D2 or FE3 (undistort) or D1 or FE2 through K (distort) of point i of pair b, as Lens is BrownLens or FisheyeLens;
+// NaN for an invalid K or coefficients, a non-finite input pixel or a point FE3 fails on
+template <class T, class Lens, bool UNDISTORT>
 __global__ void __launch_bounds__(CAM_THREADS) camera_kernel(CamArgs a) {
   const int b = blockIdx.y, i = blockIdx.x * CAM_THREADS + threadIdx.x;
   if (i >= a.N) return;
@@ -30,29 +33,35 @@ __global__ void __launch_bounds__(CAM_THREADS) camera_kernel(CamArgs a) {
   const long o = ((long)b * a.N + i) * 2;
   const double u = (double)((const T*)a.in)[o], v = (double)((const T*)a.in)[o + 1];
   double pu = NAN, pv = NAN;
-  if (k_valid(K) && dist_valid(dist, a.nd) && isfinite(u) && isfinite(v)) {
+  if (k_valid(K) && Lens::valid(dist, a.nd) && isfinite(u) && isfinite(v)) {
     const Camera<double> c = load_camera<double>(K, dist, a.nd);
     double x, y;
+    bool ok = true;
     if (UNDISTORT) {
-      undistort(c, u, v, a.max_iters, a.eps, &x, &y);
+      ok = Lens::undistort(c, u, v, a.max_iters, a.eps, &x, &y);
     } else {
       const double y0 = (v - c.cy) / c.fy, x0 = ((u - c.cx) - c.s * y0) / c.fx;
-      distort(c.d, x0, y0, &x, &y);
+      Lens::distort(c.d, x0, y0, &x, &y);
     }
-    pu = c.fx * x + c.s * y + c.cx;
-    pv = c.fy * y + c.cy;
+    if (ok) {
+      pu = c.fx * x + c.s * y + c.cx;
+      pv = c.fy * y + c.cy;
+    }
   }
   ((T*)a.out)[o] = (T)pu;
   ((T*)a.out)[o + 1] = (T)pv;
 }
 
+template <class Lens>
 int camera_run(const char* entry, bool undist, const GeoCameraConfig* cfg, const GeoCameraInputs* in,
                GeoCameraOutputs* out, void* stream) {
+  constexpr bool FISHEYE = std::is_same<Lens, FisheyeLens>::value;
   if (!cfg || !in || !out) return geo_error(entry, "null argument");
   if (cfg->abi_version != GEO_ABI_VERSION) return geo_error(entry, "ABI version mismatch");
   if (cfg->dtype != GEO_CAMERA_FLOAT32 && cfg->dtype != GEO_CAMERA_FLOAT64) return geo_error(entry, "unknown dtype");
   const int nd = cfg->num_dist;
-  if (nd != 4 && nd != 5 && nd != 8 && nd != 12) return geo_error(entry, "num_dist must be 4, 5, 8 or 12");
+  if (FISHEYE && nd != 4) return geo_error(entry, "num_dist must be 4");
+  if (!FISHEYE && nd != 4 && nd != 5 && nd != 8 && nd != 12) return geo_error(entry, "num_dist must be 4, 5, 8 or 12");
   if (undist && (cfg->max_iters < 0 || cfg->max_iters > GEO_UNDISTORT_MAX_ITERS))
     return geo_error(entry, "max_iters outside [0, GEO_UNDISTORT_MAX_ITERS]");
   if (undist && !(cfg->eps >= 0.0 && isfinite(cfg->eps))) return geo_error(entry, "eps must be finite and >= 0");
@@ -66,11 +75,11 @@ int camera_run(const char* entry, bool undist, const GeoCameraConfig* cfg, const
   const cudaStream_t s = (cudaStream_t)stream;
   const bool f64 = cfg->dtype == GEO_CAMERA_FLOAT64;
   if (undist) {
-    if (f64) camera_kernel<double, true><<<grid, CAM_THREADS, 0, s>>>(a);
-    else camera_kernel<float, true><<<grid, CAM_THREADS, 0, s>>>(a);
+    if (f64) camera_kernel<double, Lens, true><<<grid, CAM_THREADS, 0, s>>>(a);
+    else camera_kernel<float, Lens, true><<<grid, CAM_THREADS, 0, s>>>(a);
   } else {
-    if (f64) camera_kernel<double, false><<<grid, CAM_THREADS, 0, s>>>(a);
-    else camera_kernel<float, false><<<grid, CAM_THREADS, 0, s>>>(a);
+    if (f64) camera_kernel<double, Lens, false><<<grid, CAM_THREADS, 0, s>>>(a);
+    else camera_kernel<float, Lens, false><<<grid, CAM_THREADS, 0, s>>>(a);
   }
   LG_CHECK_LAUNCH();
   return 0;
@@ -80,10 +89,20 @@ int camera_run(const char* entry, bool undist, const GeoCameraConfig* cfg, const
 
 extern "C" int geo_undistort_points(const GeoCameraConfig* cfg, const GeoCameraInputs* in, GeoCameraOutputs* out,
                                     void* stream) {
-  return camera_run("geo_undistort_points", true, cfg, in, out, stream);
+  return camera_run<BrownLens>("geo_undistort_points", true, cfg, in, out, stream);
 }
 
 extern "C" int geo_distort_points(const GeoCameraConfig* cfg, const GeoCameraInputs* in, GeoCameraOutputs* out,
                                   void* stream) {
-  return camera_run("geo_distort_points", false, cfg, in, out, stream);
+  return camera_run<BrownLens>("geo_distort_points", false, cfg, in, out, stream);
+}
+
+extern "C" int geo_fisheye_undistort_points(const GeoCameraConfig* cfg, const GeoCameraInputs* in,
+                                            GeoCameraOutputs* out, void* stream) {
+  return camera_run<FisheyeLens>("geo_fisheye_undistort_points", true, cfg, in, out, stream);
+}
+
+extern "C" int geo_fisheye_distort_points(const GeoCameraConfig* cfg, const GeoCameraInputs* in, GeoCameraOutputs* out,
+                                          void* stream) {
+  return camera_run<FisheyeLens>("geo_fisheye_distort_points", false, cfg, in, out, stream);
 }

@@ -4,7 +4,8 @@
 // up to 4 P3P solutions as fp32 models; a local optimisation starts from its solution re-solved in double and runs LM
 // on the truncated reprojection cost; the final kernel writes the inlier mask of every row of matches0.  Every piece is
 // a template on pnp_common.cuh's camera policy: PnpLo<Pinhole> for geo_absolute_pose_lo, PnpLo<Distorted> for
-// geo_absolute_pose_lo_dist (steps AD1-AD4, in distorted pixels).  Compiled with -fmad=false:
+// geo_absolute_pose_lo_dist (steps AD1-AD4, in distorted pixels), PnpLo<Fisheye> for geo_absolute_pose_lo_fisheye
+// (AE1-AE4, in fisheye pixels).  Compiled with -fmad=false:
 // oracle/lo_pnp_oracle.py takes the same steps.
 #include <stdint.h>
 
@@ -141,12 +142,12 @@ struct PnpLo {
   }
 };
 
-// geo_absolute_pose_lo and geo_absolute_pose_lo_dist: the checks, then the launches
+// geo_absolute_pose_lo, geo_absolute_pose_lo_dist and geo_absolute_pose_lo_fisheye: the checks, then the launches
 template <class Cam>
 int absolute_pose(const char* entry, const GeoPnpConfig* cfg, const GeoPnpInputs* in, const double* dist0,
                   int num_dist, GeoLoPnpOutputs* out, void* workspace, size_t workspace_bytes, void* stream_) {
   int rc = geo_check_config(entry, cfg, in, out, GEO_LO_MAX_MATCHES, geo_no_check,
-                            [&] { return Cam::COEFFS ? dist_count_check(num_dist) : nullptr; });
+                            [&] { return Cam::count_check(num_dist); });
   if (rc == GEO_RUN) {
     const GeoPnpOutputs& o = out->pnp;
     const auto buffers = [&](std::initializer_list<const void*> intrinsics) {
@@ -180,4 +181,12 @@ extern "C" int geo_absolute_pose_lo_dist(const GeoPnpConfig* cfg, const GeoPnpDi
   return absolute_pose<Distorted>("geo_absolute_pose_lo_dist", cfg, din ? &din->pnp : nullptr,
                                   din ? din->dist0 : nullptr, din ? din->num_dist : 0, out, workspace, workspace_bytes,
                                   stream);
+}
+
+extern "C" int geo_absolute_pose_lo_fisheye(const GeoPnpConfig* cfg, const GeoPnpDistInputs* din,
+                                            GeoLoPnpOutputs* out, void* workspace, size_t workspace_bytes,
+                                            void* stream) {
+  return absolute_pose<Fisheye>("geo_absolute_pose_lo_fisheye", cfg, din ? &din->pnp : nullptr,
+                                din ? din->dist0 : nullptr, din ? din->num_dist : 0, out, workspace, workspace_bytes,
+                                stream);
 }

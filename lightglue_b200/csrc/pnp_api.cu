@@ -14,7 +14,8 @@
 //   mask     pnp_mask_kernel<Cam>, one thread per row of matches0: the final inlier mask
 // A stopped pair's CTAs return at once.  Cam is pnp_common.cuh's camera policy: Pinhole for geo_absolute_pose (the
 // float model is K0 [R | t]), Distorted for geo_absolute_pose_dist (steps AD1-AD4: D2's calibrated coordinates, the
-// float model [R | t] and the test in distorted pixels).  Compiled with -fmad=false, like geo_api.cu:
+// float model [R | t] and the test in distorted pixels), Fisheye for geo_absolute_pose_fisheye (AE1-AE4: FE3's
+// calibrated coordinates, which may drop a match, and the test in fisheye pixels).  Compiled with -fmad=false, like geo_api.cu:
 // oracle/pnp_oracle.py takes the same steps in numpy.
 #include <stdint.h>
 
@@ -129,12 +130,12 @@ __global__ void __launch_bounds__(MASK_THREADS) pnp_mask_kernel(PnpArgs a) {
   a.out.inliers[(long)b * a.M + i] = in;
 }
 
-// geo_absolute_pose and geo_absolute_pose_dist: the checks, then the launches
+// geo_absolute_pose, geo_absolute_pose_dist and geo_absolute_pose_fisheye: the checks, then the launches
 template <class Cam>
 int absolute_pose(const char* entry, const GeoPnpConfig* cfg, const GeoPnpInputs* in, const double* dist0,
                   int num_dist, GeoPnpOutputs* out, void* workspace, size_t workspace_bytes, void* stream_) {
   int rc = geo_check_config(entry, cfg, in, out, INT_MAX, geo_no_check,
-                            [&] { return Cam::COEFFS ? dist_count_check(num_dist) : nullptr; });
+                            [&] { return Cam::count_check(num_dist); });
   if (rc == GEO_RUN) {
     const auto buffers = [&](std::initializer_list<const void*> intrinsics) {
       return geo_check_buffers(entry, in, {out->R, out->t, out->num_inliers, out->success, out->best_hypothesis,
@@ -175,4 +176,11 @@ extern "C" int geo_absolute_pose_dist(const GeoPnpConfig* cfg, const GeoPnpDistI
   // a null din goes on as a null in, which geo_check_config reports
   return absolute_pose<Distorted>("geo_absolute_pose_dist", cfg, din ? &din->pnp : nullptr, din ? din->dist0 : nullptr,
                                   din ? din->num_dist : 0, out, workspace, workspace_bytes, stream);
+}
+
+extern "C" int geo_absolute_pose_fisheye(const GeoPnpConfig* cfg, const GeoPnpDistInputs* din, GeoPnpOutputs* out,
+                                         void* workspace, size_t workspace_bytes, void* stream) {
+  return absolute_pose<Fisheye>("geo_absolute_pose_fisheye", cfg, din ? &din->pnp : nullptr,
+                                din ? din->dist0 : nullptr, din ? din->num_dist : 0, out, workspace, workspace_bytes,
+                                stream);
 }

@@ -1,8 +1,8 @@
 // The absolute-pose pieces shared by the plain (pnp_api.cu, header steps A1-A8) and the LO-RANSAC estimator
 // (lo_pnp_api.cu, LA1-LA8), both compiled with -fmad=false: the workspace, the Lambda Twist solver, the projection,
 // the fp32 reprojection test, the residuals and pose update of the Levenberg-Marquardt steps, and their counterparts
-// with lens distortion (AD1-AD4); then the two camera policies, Pinhole and Distorted, that route to one or the other,
-// and the solver and compaction kernel templated on them.
+// with lens distortion (AD1-AD4) or the fisheye lens (AE1-AE4); then the three camera policies, Pinhole, Distorted and
+// Fisheye, that route to one or the other, and the solver and compaction kernel templated on them.
 #pragma once
 #include <stdint.h>
 
@@ -355,24 +355,26 @@ __device__ __forceinline__ void rt_matrix(const double* x, double* M) {
   }
 }
 
-// AD2's fp32 error of one point under the float [R | t] g: du * du + dv * dv in distorted pixels in front of the
-// camera, +inf behind it (so that an inlier has err < thr2 and lo_term counts the others as outliers)
+// AD2's (AE2's) fp32 error of one point under the float [R | t] g: du * du + dv * dv in distorted pixels of Lens in
+// front of the camera, +inf behind it (so that an inlier has err < thr2 and lo_term counts the others as outliers)
+template <class Lens>
 __device__ __forceinline__ float dist_reproj_err(const float* g, const Camera<float>& c, float4 p, float4 q) {
   const float X0 = g[0] * q.x + g[1] * q.y + g[2] * q.z + g[3];
   const float X1 = g[4] * q.x + g[5] * q.y + g[6] * q.z + g[7];
   const float w = g[8] * q.x + g[9] * q.y + g[10] * q.z + g[11];
   float xd, yd;
-  distort(c.d, X0 / w, X1 / w, &xd, &yd);
+  Lens::distort(c.d, X0 / w, X1 / w, &xd, &yd);
   const float du = p.x - (c.fx * xd + c.s * yd + c.cx), dv = p.y - (c.fy * yd + c.cy);
   return w > 0.f ? du * du + dv * dv : INFINITY;
 }
 
-// AD3's residual (ru, rv) of world point q at pixel p, in distorted pixels, and what its Jacobian needs
+// AD3's (AE3's) residual (ru, rv) of world point q at pixel p, in distorted pixels of Lens, and what its Jacobian needs
 struct PnpDistResidual {
   double Xc[3];  // the camera-frame point; Xc[2] is its depth
   double iz, a, b, ru, rv;
 };
 
+template <class Lens>
 __device__ __forceinline__ PnpDistResidual pnp_dist_residual(const Camera<double>& c, const double* R, const double* t,
                                                              float4 p, float4 q) {
   const double W[3] = {q.x, q.y, q.z};
@@ -382,16 +384,17 @@ __device__ __forceinline__ PnpDistResidual pnp_dist_residual(const Camera<double
   e.a = e.Xc[0] * e.iz;
   e.b = e.Xc[1] * e.iz;
   double xd, yd;
-  distort(c.d, e.a, e.b, &xd, &yd);
+  Lens::distort(c.d, e.a, e.b, &xd, &yd);
   e.ru = c.fx * xd + c.s * yd + c.cx - (double)p.x;
   e.rv = c.fy * yd + c.cy - (double)p.y;
   return e;
 }
 
-// AD3's J^T J and J^T r terms of one point: A7's rows through D1's Jacobian
+// AD3's (AE3's) J^T J and J^T r terms of one point: A7's rows through D1's (FE2's) Jacobian
+template <class Lens>
 __device__ __forceinline__ void pnp_dist_add_normal(const Camera<double>& c, const PnpDistResidual& e, double* acc) {
   double J[4];
-  distort_jacobian(c.d, e.a, e.b, J);
+  Lens::jacobian(c.d, e.a, e.b, J);
   const double ua = c.fx * J[0] + c.s * J[2], ub = c.fx * J[1] + c.s * J[3], va = c.fy * J[2], vb = c.fy * J[3];
   const double gu[3] = {ua * e.iz, ub * e.iz, -((ua * e.a + ub * e.b) * e.iz)};
   const double gv[3] = {va * e.iz, vb * e.iz, -((va * e.a + vb * e.b) * e.iz)};
@@ -405,9 +408,11 @@ inline const char* dist_count_check(int nd) {
 
 // ---- the camera policies ----
 //
-// Everything that differs between the pinhole absolute pose (A1-A8, LA1-LA8) and the one with lens distortion
-// (AD1-AD4) is one of these two policies, on which every kernel and entry point below is a template:
-//   COEFFS, whether the entry point takes coefficients (host);
+// Everything that differs between the pinhole absolute pose (A1-A8, LA1-LA8) and the ones with lens distortion
+// (AD1-AD4) or a fisheye lens (AE1-AE4) is one of these three policies, on which every kernel and entry point below is
+// a template:
+//   COEFFS, whether the entry point takes coefficients, and count_check(nd), its check of their number (host);
+//   BEARING_FAILS, whether bearing can fail a match (AE1): then it runs before the compaction and returns false;
 //   Consts and consts(a, b), pair b's constants of the LM and the scored model; Test and test(a, b), those of the fp32
 //   test;
 //   valid(K, dist, nd), whether K (and the coefficients) let the pair run;
@@ -418,7 +423,8 @@ inline const char* dist_count_check(int nd) {
 
 // The pinhole camera: K0^-1 (A2), K0 [R | t] (A5), the fp32 test in pixels (A5, LA3) and A7's residual
 struct Pinhole {
-  static constexpr bool COEFFS = false;
+  static constexpr bool COEFFS = false, BEARING_FAILS = false;
+  static const char* count_check(int) { return nullptr; }
   using Consts = const double*;  // K0
   struct Test {};
 
@@ -448,7 +454,8 @@ struct Pinhole {
 // The camera with lens distortion: D2's undistortion (AD1), [R | t] and the fp32 test in distorted pixels (AD2) and
 // AD3's residual; invalid coefficients fail the pair as an invalid K0
 struct Distorted {
-  static constexpr bool COEFFS = true;
+  static constexpr bool COEFFS = true, BEARING_FAILS = false;
+  static const char* count_check(int nd) { return dist_count_check(nd); }
   using Consts = Camera<double>;
   using Test = Camera<float>;
 
@@ -463,16 +470,49 @@ struct Distorted {
   }
   static __device__ __forceinline__ void model(const Consts&, const double* x, double* px) { rt_matrix(x, px); }
   static __device__ __forceinline__ bool inlier(const Test& c, const float* g, float4 p, float4 q, float thr2) {
-    return dist_reproj_err(g, c, p, q) < thr2;
+    return dist_reproj_err<BrownLens>(g, c, p, q) < thr2;
   }
   static __device__ __forceinline__ float err(const Test& c, const float* g, float4 p, float4 q) {
-    return dist_reproj_err(g, c, p, q);
+    return dist_reproj_err<BrownLens>(g, c, p, q);
   }
   static __device__ __forceinline__ PnpDistResidual residual(const Consts& c, const double* x, float4 p, float4 q) {
-    return pnp_dist_residual(c, x, x + 9, p, q);
+    return pnp_dist_residual<BrownLens>(c, x, x + 9, p, q);
   }
   static __device__ __forceinline__ void add_normal(const Consts& c, const PnpDistResidual& e, double* acc) {
-    pnp_dist_add_normal(c, e, acc);
+    pnp_dist_add_normal<BrownLens>(c, e, acc);
+  }
+};
+
+// The fisheye camera: FE3's bearing at cv2.fisheye's default criteria, which drops its match when it fails (AE1),
+// [R | t] and the fp32 test in fisheye pixels (AE2) and AE3's residual; coefficients that fail FE4 fail the pair as an
+// invalid K0
+struct Fisheye {
+  static constexpr bool COEFFS = true, BEARING_FAILS = true;
+  static const char* count_check(int nd) { return nd == 4 ? nullptr : "num_dist must be 4"; }
+  using Consts = Camera<double>;
+  using Test = Camera<float>;
+
+  static __device__ __forceinline__ Consts consts(const PnpArgs& a, int b) { return pair_camera<double>(a, b); }
+  static __device__ __forceinline__ Test test(const PnpArgs& a, int b) { return pair_camera<float>(a, b); }
+  static __device__ __forceinline__ bool valid(const double* K, const double* dist, int) {
+    return k_valid(K) && fisheye_valid(dist);
+  }
+  static __device__ __forceinline__ bool bearing(const double* K, const double* dist, int nd, float2 p, double* x,
+                                                 double* y) {
+    return fisheye_undistort(load_camera<double>(K, dist, nd), p.x, p.y, GEO_FISHEYE_ITERS, GEO_FISHEYE_EPS, x, y);
+  }
+  static __device__ __forceinline__ void model(const Consts&, const double* x, double* px) { rt_matrix(x, px); }
+  static __device__ __forceinline__ bool inlier(const Test& c, const float* g, float4 p, float4 q, float thr2) {
+    return dist_reproj_err<FisheyeLens>(g, c, p, q) < thr2;
+  }
+  static __device__ __forceinline__ float err(const Test& c, const float* g, float4 p, float4 q) {
+    return dist_reproj_err<FisheyeLens>(g, c, p, q);
+  }
+  static __device__ __forceinline__ PnpDistResidual residual(const Consts& c, const double* x, float4 p, float4 q) {
+    return pnp_dist_residual<FisheyeLens>(c, x, x + 9, p, q);
+  }
+  static __device__ __forceinline__ void add_normal(const Consts& c, const PnpDistResidual& e, double* acc) {
+    pnp_dist_add_normal<FisheyeLens>(c, e, acc);
   }
 };
 
@@ -491,7 +531,7 @@ struct PnpSolver {
   }
 };
 
-// A1 (and AD1): ordered compaction of the valid matches with Cam's calibrated coordinates, and the camera check
+// A1 (and AD1, AE1): ordered compaction of the valid matches with Cam's calibrated coordinates, and the camera check
 template <class Cam>
 __global__ void __launch_bounds__(1024) pnp_prepare_kernel(PnpArgs a) {
   const int b = blockIdx.x, tid = threadIdx.x;
@@ -517,12 +557,13 @@ __global__ void __launch_bounds__(1024) pnp_prepare_kernel(PnpArgs a) {
       Z = q[2];
       p = reinterpret_cast<const float2*>(a.kpts0)[(long)b * a.M + i];
     }
-    const bool valid = j >= 0 && j < a.N && isfinite(X) && isfinite(Y) && isfinite(Z) && finite2(p);
+    bool valid = j >= 0 && j < a.N && isfinite(X) && isfinite(Y) && isfinite(Z) && finite2(p);
+    double xx, yy;
+    if constexpr (Cam::BEARING_FAILS) valid = valid && Cam::bearing(K, dist, a.nd, p, &xx, &yy);
     const int k = block_scan_step(valid, tid, warp_sums, &carry);
     if (i < a.M) slot[i] = valid ? k : -1;
     if (valid) {
-      double xx, yy;
-      Cam::bearing(K, dist, a.nd, p, &xx, &yy);
+      if constexpr (!Cam::BEARING_FAILS) Cam::bearing(K, dist, a.nd, p, &xx, &yy);
       pts[k] = make_float4(p.x, p.y, (float)xx, (float)yy);
       wld[k] = make_float4(X, Y, Z, 0.f);
     }

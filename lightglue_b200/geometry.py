@@ -33,7 +33,7 @@ import ctypes as C
 import torch
 
 from . import _cabi
-from .camera import dist_coeffs
+from .camera import check_fisheye_count, dist_coeffs
 
 
 def _check_params(threshold, max_iters, confidence, seed, name="ransac_reproj_threshold",
@@ -324,7 +324,8 @@ def estimate_absolute_pose(kpts0: torch.Tensor, points3d1: torch.Tensor, matches
     ``dist_coeffs0`` ([k] or [B, k], k = 4, 5, 8 or 12; see ``lightglue_b200.camera``) gives the query camera's lens
     distortion, as ``cv2.solvePnPRansac(..., distCoeffs)`` takes it: the P3P samples see the pixels undistorted by
     OpenCV's 5 fixed-point iterations, and the inlier test and the refit measure the reprojection error in distorted
-    pixels (header steps AD1-AD4).  A pair with a non-finite coefficient fails as one with an invalid K0."""
+    pixels (header steps AD1-AD4).  A pair with a non-finite coefficient fails as one with an invalid K0.  A fisheye
+    lens is ``estimate_absolute_pose_fisheye``'s."""
     return _absolute_pose(False, kpts0, points3d1, matches0, K0, ransac_reproj_threshold, max_iters, confidence, seed,
                           dist_coeffs0)
 
@@ -350,8 +351,38 @@ def estimate_absolute_pose_lo(kpts0: torch.Tensor, points3d1: torch.Tensor, matc
                           dist_coeffs0)
 
 
+def estimate_absolute_pose_fisheye(kpts0: torch.Tensor, points3d1: torch.Tensor, matches0: torch.Tensor,
+                                   K0: torch.Tensor, D0: torch.Tensor, ransac_reproj_threshold: float = 8.0,
+                                   max_iters: int = 100, confidence: float = 0.99, seed: int = 0) -> dict:
+    """``estimate_absolute_pose`` for a query camera with a fisheye lens: ``K0`` and ``D0`` ([4] or [B, 4]: k1, k2,
+    k3, k4, see ``lightglue_b200.camera``) as ``cv2.fisheye`` takes them (header steps AE1-AE4).  The P3P samples see
+    the pixels undistorted as ``cv2.fisheye.undistortPoints`` does with its default criteria, and a match whose pixel
+    does not undistort is invalid; the inlier test and the refit measure the reprojection error in fisheye pixels.
+    ``cv2.fisheye.solvePnPRansac`` instead tests undistorted pinhole pixels, where a fixed threshold grows as
+    1 / cos^2 of the field angle and drops true inliers toward the edge of a wide lens;
+    ``camera.fisheye_undistort_points`` followed by ``estimate_absolute_pose`` reproduces that.  Arguments, outputs and
+    failures are ``estimate_absolute_pose``'s; non-finite coefficients fail the pair as an invalid K0 does, and a
+    ``D0`` that is None or does not hold exactly 4 coefficients per pair is a ``ValueError``.
+
+    This is a function of its own, not a keyword of ``estimate_absolute_pose``, so that the signatures of
+    ``estimate_absolute_pose`` and ``estimate_absolute_pose_lo`` stay as they were, ending at ``dist_coeffs0``."""
+    return _absolute_pose(False, kpts0, points3d1, matches0, K0, ransac_reproj_threshold, max_iters, confidence, seed,
+                          D0, fisheye=True)
+
+
+def estimate_absolute_pose_lo_fisheye(kpts0: torch.Tensor, points3d1: torch.Tensor, matches0: torch.Tensor,
+                                      K0: torch.Tensor, D0: torch.Tensor, ransac_reproj_threshold: float = 8.0,
+                                      max_iters: int = 100, confidence: float = 0.99, seed: int = 0) -> dict:
+    """``estimate_absolute_pose_lo`` for a query camera with a fisheye lens, as ``estimate_absolute_pose_fisheye``:
+    the MSAC score and the Levenberg-Marquardt steps read the reprojection error in fisheye pixels."""
+    return _absolute_pose(True, kpts0, points3d1, matches0, K0, ransac_reproj_threshold, max_iters, confidence, seed,
+                          D0, fisheye=True)
+
+
 def _absolute_pose(lo: bool, kpts0, points3d1, matches0, K0, ransac_reproj_threshold, max_iters, confidence,
-                   seed, dist_coeffs0=None) -> dict:
+                   seed, dist_coeffs0=None, fisheye: bool = False) -> dict:
+    if fisheye:  # a fisheye pose never falls back to the pinhole or the rational lens
+        check_fisheye_count("D0", dist_coeffs0)
     _check_inputs(kpts0, points3d1, matches0, "points3d1", 3)
     _check_params(ransac_reproj_threshold, max_iters, confidence, seed)
     if lo and kpts0.shape[1] > _cabi.GEO_LO_MAX_MATCHES:
@@ -359,7 +390,8 @@ def _absolute_pose(lo: bool, kpts0, points3d1, matches0, K0, ransac_reproj_thres
     device = kpts0.device
     b, m, n = kpts0.shape[0], kpts0.shape[1], points3d1.shape[1]
     k0 = _intrinsics("K0", K0, b, device)
-    d0 = None if dist_coeffs0 is None else dist_coeffs("dist_coeffs0", dist_coeffs0, b, device)
+    d0 = None if dist_coeffs0 is None else dist_coeffs("D0" if fisheye else "dist_coeffs0", dist_coeffs0, b, device,
+                                                       fisheye)
     p0 = kpts0.detach().to(torch.float32).contiguous()
     x1 = points3d1.detach().to(torch.float32).contiguous()
     m0 = matches0.detach().contiguous()
@@ -383,7 +415,8 @@ def _absolute_pose(lo: bool, kpts0, points3d1, matches0, K0, ransac_reproj_thres
 
     entry = "geo_absolute_pose_lo" if lo else "geo_absolute_pose"
     ws = "geo_lo_pnp_workspace_bytes" if lo else "geo_pnp_workspace_bytes"
-    return _run(entry if d0 is None else entry + "_dist", ws, shapes, device, b, m, max_iters, make_args)
+    suffix = "" if d0 is None else "_fisheye" if fisheye else "_dist"
+    return _run(entry + suffix, ws, shapes, device, b, m, max_iters, make_args)
 
 
 def _affine(kind: int, kpts0, kpts1, matches0, threshold, max_iters, confidence, refine_iters, seed) -> dict:
